@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py — headline benchmark of the COVINS hot path on B200 (contract: see DESIGN.md §Measurement).
+"""bench.py — headline benchmark of the COVINS hot path on H100 (contract: see DESIGN.md §Measurement).
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--gba-config C3]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--gba-config C3] [--dump-outputs DIR]
 
 Metric (BASELINE.json): global-BA iterations/s & descriptor-match Gpairs/s on the 5-agent EuRoC-sized synthetic map
 (config C3: 2000 KF / 100k LM / ~800k obs; 1000 ORB features per KF).  One "step" is one pass of the hot path: one outer
@@ -9,7 +9,11 @@ trust-region iteration of the visual-inertial global BA (linearise → Schur →
 query keyframe matched against every keyframe of the rank's map shard (2 Gpairs, fused k-NN + ratio filter).  The legs
 are timed separately; the JSON line carries the GBA rate as `value` and the matching rate under `match` (each with its
 own e2e / roofline / cpu_baseline); `pgo` carries the pose-graph optimisation rate on the same map, `match.sift_l2` /
-`match.landmark_descriptor` the SIFT and ComputeDescriptor kernels.  Scalars of the nested legs are repeated at the top
+`match.landmark_descriptor` the SIFT and ComputeDescriptor kernels.  `--steps` is the number of timed steps of every leg.
+
+`--dump-outputs DIR`: after the timed steps, the results of the last timed step (GBA state; accepted matches of the
+request) are written as DIR/<name>.npy (float32 / float64).  Inputs are seeded, so two builds can be compared output for
+output.  Scalars of the nested legs are repeated at the top
 level (`match_gpairs_per_sec`, `pgo_iterations_per_sec`, …) so that per-N scaling records carry them.
 
 `--impl reference`: the CPU arm — the compiled CPU port of the optimisation path (oracle/ba_port.cpp: analytic Jacobians,
@@ -34,7 +38,7 @@ if ROOT not in sys.path:
 
 N_KF, N_FEAT = 2000, 1000          # C3: 5 agents x 400 KF, 1000 ORB features per KF
 THR, RATIO = 40.0, 0.8             # config/config_backend.yaml:38-39
-N_COPIES = 4                       # 4 x 64 MB map copies rotated per step → inputs (256 MB) > L2 (126 MB)
+N_COPIES = 4                       # 4 x 64 MB map copies rotated per step → inputs (256 MB) > L2 (50 MB)
 
 WORKLOAD = ("C3 5-agent EuRoC-sized synthetic map (2000 KF / 100k LM / ~800k obs, 1000 ORB features per KF): "
             "visual-inertial global-BA trust-region iterations + ORB k-NN(k=2)+ratio-filter of one query KF vs every KF")
@@ -47,17 +51,7 @@ def _measured():
 
 def _peaks():
     d = _measured()
-    return (d["hbm_gbs"], "MEASURED_PEAKS.json") if "hbm_gbs" in d else (6650.0, "fallback (B200_PROFILING.md)")
-
-
-def _traffic(key):
-    """dram bytes per launch of a dominant kernel, from the committed ncu --set full captures (profiles/r02_traffic.json,
-    written by tools/r02_traffic.py out of the .ncu-rep files); None when no capture is committed for `key`."""
-    p = os.path.join(ROOT, "profiles", "r02_traffic.json")
-    if not os.path.exists(p):
-        return None, None
-    d = json.load(open(p)).get(key)
-    return (d["dram_bytes"], d.get("source")) if d else (None, None)
+    return (d["hbm_gbs"], "MEASURED_PEAKS.json") if "hbm_gbs" in d else (3350.0, "H100 SXM data sheet (not measured)")
 
 
 class ClockSampler:
@@ -312,6 +306,17 @@ def int8_gemm_peak(dev):
         return 2.0 * bf, f"2 x bf16_tflops of MEASURED_PEAKS.json (torch._int_mm unavailable: {type(ex).__name__})"
 
 
+def dump_outputs(d, gba, match):
+    """What the timed path computed in its last step: the GBA state after the timed trust-region iterations and the
+    accepted matches of the last matching request (match_train / match_dist [n_kf, nq], n_matches [n_kf]); 27 MB at C3."""
+    os.makedirs(d, exist_ok=True)
+    arrays = {"gba_pose": gba["pose"], "gba_speedbias": gba["speedbias"], "gba_landmarks": gba["lm"], "gba_cost": gba["cost"],
+              "match_train": match[0].cpu().numpy(), "match_dist": match[1].cpu().numpy(), "match_n_matches": match[2].cpu().numpy()}
+    for name, a in arrays.items():
+        a = np.asarray(a)
+        np.save(os.path.join(d, name + ".npy"), a.astype(np.float32 if a.dtype == np.float32 else np.float64))
+
+
 def run_ours(args):
     import torch
     import torch.distributed as dist
@@ -419,7 +424,7 @@ def run_ours(args):
                 if done_ < n:
                     ps.restart()
             return done_
-        pgo_steps = max(args.steps, 10)
+        pgo_steps = args.steps
         pgo_iters(args.warmup); ps.restart()
         ctx.sync(); lp = ctx.launch_count(); t0 = time.perf_counter()
         pgo_iters(pgo_steps)
@@ -473,7 +478,7 @@ def run_ours(args):
     def step_match_raw(i):      # raw-pointer API: packed rows only, the operand tiles are expanded inside every call
         return M.match_candidates_hamming(ctx, q, maps[i % N_COPIES], (d_seg, h_seg), THR, RATIO)
 
-    m_steps = max(args.steps, 10)
+    m_steps = args.steps
     for i in range(args.warmup):
         step_match(i)
     barrier()
@@ -487,6 +492,8 @@ def run_ours(args):
     ms_match = max_over_ranks(e0.elapsed_time(e1))
     match_launches = ctx.launch_count() - l0
     n_accepted = int(out_m[2].sum().item())
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, res, out_m)
     gp = pairs * world * m_steps / (ms_match * 1e-3) / 1e9
 
     for i in range(3):
@@ -512,7 +519,7 @@ def run_ours(args):
     # e2e through the resident-map API (cvb_db_*): keyframes uploaded once when they join the map (outside the timed
     # region, as in the server's life cycle), per request the query keyframe goes up and the accepted matches come down.
     h_queries = [np.ascontiguousarray(h_maps_np[0][k * N_FEAT:(k + 1) * N_FEAT]) for k in (123, 777, 1500, 42)]
-    db_steps = max(args.steps, 30)
+    db_steps = args.steps
     d2h_db = 0
     for i in range(3):
         dbs[i % N_COPIES].match_hamming(h_queries[i % 4], THR, RATIO)
@@ -533,7 +540,7 @@ def run_ours(args):
     alg_bytes = 32 * N_KF * N_FEAT + 32 * N_FEAT + 8 * N_KF * N_FEAT + 4 * N_KF   # SURVEY §8d: 32 Nt + 32 Nq + outputs
     ms_step = ms_match / m_steps
     hbm_gbs = alg_bytes / (ms_step * 1e-3) / 1e9
-    # dominant kernel: cvb_tc::xt::tc_xt_kernel<2> — u8 x s8 -> s32 tcgen05 GEMM over the resident operand tiles (K = 256 bit
+    # dominant kernel: cvb_tc::xt::tc_xt_kernel<2> — u8 x s8 -> s32 wgmma GEMM over the resident operand tiles (K = 256 bit
     # bytes + a 32-byte key slice that makes the accumulator the sort key) + fused top-2 / ratio filter.  Algorithmic ops:
     # 2 x 256 per pair (SURVEY 8d); the key slice's 12.5 % extra MMA work is not counted.
     tops = 2.0 * 256 * pairs / (ms_step * 1e-3) / 1e12
@@ -592,7 +599,6 @@ def run_ours(args):
                                "frac": b7 / (ms7 * 1e-3) / 1e9 / hbm_peak, "traffic": None, "algorithmic_bytes_per_launch": b7,
                                "note": "32 B per observation read once + 36 B per landmark written; includes the clone of the old descriptors"}}
         del c7
-    tr_match, tr_match_src = _traffic("tc_xt_kernel")
     match = {
         "metric": "match_gpairs_per_sec", "value": gp, "unit": "Gpairs/s", "ms_per_step": ms_step, "steps": m_steps,
         "scaling": "weak", "dtype": "u8",
@@ -602,7 +608,7 @@ def run_ours(args):
                    "data": "synth.orb_keyframes: keyframes share landmarks (matched Hamming ~16, unmatched ~128)",
                    "accepted_matches_per_step": n_accepted,
                    "pairs_per_step_per_gpu": pairs,
-                   "l2_policy": f"{N_COPIES} map copies (256 MB > 126 MB L2) rotated per step",
+                   "l2_policy": f"{N_COPIES} map copies (256 MB > 50 MB L2) rotated per step",
                    "parallelism": f"map sharded by keyframe x{world}, no data-path collective"},
         "e2e": {"value": e2e_db_gp, "unit": "Gpairs/s", "h2d_bytes_per_step": int(h_queries[0].nbytes),
                 "d2h_bytes_per_step": int(d2h_db // db_steps), "steps": db_steps, "ms_per_step": dt_db * 1e3,
@@ -616,12 +622,12 @@ def run_ours(args):
                                       "api": "cvb_match_hamming_batch: the whole 64 MB map re-uploaded from host memory on "
                                              "every call and the dense [n_kf][nq] result matrices downloaded (PCIe-bound)"}},
         "gpu_launches": int(match_launches),
-        "roofline": {"bound": "tensor", "achieved": tops, "peak": i8_peak, "unit": "TOP/s", "frac": tops / i8_peak, "traffic": tr_match,
-                     "traffic_source": tr_match_src, "peak_source": i8_src,
-                     "kernel": "cvb_tc::xt::tc_xt_kernel<2> (tcgen05.mma kind::i8 u8 x s8, query block in TMEM, operand tiles by cp.async.bulk, "
-                               "accumulator = packed sort key, fused top-2 + ratio filter)",
-                     "hw_peak": {"tops": 2 * 8192 * 148 * 1.965e9 / 1e12, "frac": tops / (2 * 8192 * 148 * 1.965e9 / 1e12),
-                                 "source": "8192 MAC/clk/SM measured with tools/micro/umma_rate.cu (profiles/r02_umma_rate.txt) x 148 SMs x 1965 MHz"},
+        "roofline": {"bound": "tensor", "achieved": tops, "peak": i8_peak, "unit": "TOP/s", "frac": tops / i8_peak, "traffic": None,
+                     "peak_source": i8_src,
+                     "kernel": "cvb_tc::xt::tc_xt_kernel<2> (wgmma m64n128k32 u8 x s8, query block and operand tiles in shared memory, "
+                               "tiles by cp.async.bulk, accumulator = packed sort key, fused top-2 + ratio filter)",
+                     "hw_peak": {"tops": 1979.0, "frac": tops / 1979.0,
+                                 "source": "NVIDIA H100 SXM data sheet, dense INT8 at up to 700 W (not measured)"},
                      "operand_tile_bytes_per_launch": tile_bytes_per_launch,
                      "raw_pointer_api": {"ms_per_step": ms_raw, "gpairs_per_s": pairs / (ms_raw * 1e-3) / 1e9,
                                          "note": "cvb_match_hamming_batch_dev on packed rows only: the 590 MB of operand tiles are expanded inside "
@@ -635,14 +641,13 @@ def run_ours(args):
         "landmark_descriptor": lmdesc,
     }
 
-    tr_gba, tr_gba_src = _traffic("syrk_kernel")
     line = {
         "metric": "gba_iterations_per_sec", "value": gba_rate, "unit": "iterations/s", "n_gpus": world, "steps": args.steps,
         "warmup": args.warmup, "ms_per_step": dt_gba / args.steps * 1e3, "higher_is_better": True, "scaling": "strong",
         "vs_baseline": None, "dtype": "f64", "data": "synthetic",
         "config": {"workload": WORKLOAD, "gba_config": args.gba_config, "K": int(prob["K"]), "L": int(prob["L"]), "n_obs": int(n_obs),
                    "n_imu": int(len(prob["imu_i"])), "n_loop": int(len(prob["loop_i"])), "reduced_system_dim": int(15 * prob["K"]),
-                   "l2_policy": "working set (0.8 GB of packed tiles of the reduced camera system + 0.5 GB of observation records at C3) >> 126 MB L2",
+                   "l2_policy": "working set (0.8 GB of packed tiles of the reduced camera system + 0.5 GB of observation records at C3) >> 50 MB L2",
                    "parallelism": (f"landmark blocks sharded x{world}; reduced camera system reduce-scattered by peer pull (CUDA IPC over NVLink) onto "
                                    f"tile-column owners; Cholesky distributed by tile columns, panels handed over through peer memory; small vectors all-reduced (NCCL)"
                                    if p2p else f"landmark blocks sharded x{world}; all-reduce of the reduced normal equations; solve replicated") if world > 1 else "single GPU",
@@ -660,7 +665,7 @@ def run_ours(args):
         "device_ms_per_step": dev_ms / args.steps,
         "final_cost": res["final_cost"], "initial_cost": res["initial_cost"],
         "roofline": {"bound": "tensor", "achieved": chol_tflops, "peak": dgemm_peak, "unit": "TFLOP/s",
-                     "frac": chol_tflops / dgemm_peak if dgemm_peak else None, "traffic": tr_gba, "traffic_source": tr_gba_src,
+                     "frac": chol_tflops / dgemm_peak if dgemm_peak else None, "traffic": None,
                      "peak_source": "cuBLAS DGEMM 6144^3 measured in this run (FP64; MEASURED_PEAKS.json holds no FP64 figure)",
                      "kernel": "cvb_chol::syrk_kernel (FP64 DMMA m8n8k4, 64x64x128 per CTA, 3 CTAs/SM) inside the tile-sparse Cholesky of the reduced camera system; "
                                "achieved = tile-GEMM flops executed by rank 0 / factorisation time (includes the latency-bound diagonal-tile chain)",
@@ -691,6 +696,8 @@ def main():
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--gba-config", default=os.environ.get("COVINS_GBA_CONFIG", "C3"))
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the outputs of the last timed step as DIR/<name>.npy")
     args = ap.parse_args()
     if args.impl == "ours":
         args.warmup = max(args.warmup, 3)

@@ -25,7 +25,7 @@ class CvbError(RuntimeError):
 
 
 def build(force: bool = False) -> str:
-    """Compile every CUDA source for sm_100a with nvcc (in-tree; the .so travels with the repo snapshot)."""
+    """Compile every CUDA source for sm_90a with nvcc (in-tree: covins_b200/libcovins_b200.so)."""
     args = ["make", "-C", os.path.join(_HERE, "csrc"), "-j8", "-s"]
     if force:
         args.append("-B")

@@ -1405,7 +1405,7 @@ int engine_setup(Engine& E, const cvb_ba_problem* p, const cvb_ba_options* o) {
     for (int t = sb_ranges[g].first / TT; t <= (sb_ranges[g].second - 1) / TT; t++) col_group[t] = (int)g;
   // ownership of the tile columns (world > 1): an IMU chain's speed-bias columns — a pure latency chain — stay on one
   // rank, the remaining (pose) columns go round the ranks in blocks of COVINS_B200_DIST_BLOCK columns (default 6: every
-  // change of owner puts a flag + a 128 KB NVLink copy on the critical chain, measured ~40 us; profiles/r02_block_sweep_4gpu.txt)
+  // change of owner puts a flag + a 128 KB NVLink copy on the critical chain; tools/mgpu_block_sweep.py)
   std::vector<int> h_owner;
   if (E.world > 1) {
     int blk = 6;

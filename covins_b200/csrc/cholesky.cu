@@ -8,7 +8,7 @@
 // At EuRoC scale every keyframe is covisible with hundreds of others (all agents fly the same hall), so the pose part
 // of S is ~10 % block-dense before fill and fills in almost completely: a tiled dense-tile factorisation is the right
 // shape for the GPU; this is the one BA stage that is a true GEMM and runs on the FP64 tensor cores (DMMA,
-// mma.sync.m8n8k4.f64 — tcgen05 has no FP64 kind).
+// mma.sync.m8n8k4.f64 — wgmma has no FP64 kind).
 //
 // Right-looking, panel width 128:
 //   potrf_inv_kernel   1 CTA: factor the 128x128 diagonal tile in shared memory, write L, write L^-1
@@ -200,7 +200,7 @@ __global__ void __launch_bounds__(SYRK_THREADS, 3) syrk_kernel(double* __restric
 
 // Factor the diagonal tile k in shared memory and invert the factor, one CTA of 512 threads.  This kernel is the serial
 // chain of the whole factorisation (one launch per tile column, nothing else can run before its panel is solved), so it
-// is organised around dependent-operation latency (measured on B200: DFMA 8.7, SHFL 30, STS→LDS 35, rsqrt 65 cycles):
+// is organised around dependent-operation latency (DFMA, SHFL, STS→LDS and rsqrt latencies on the critical chain):
 //   Cholesky: blocked right-looking, 16-wide block columns.  Per block column
 //     (a) warp 0 factors the 16x16 diagonal block register-resident (lane = 2*row + half).  Per pivot the *unscaled*
 //         column goes through 128 B of shared memory and the update uses a_rj * a_cj / pivot, so the chain per pivot is

@@ -19,7 +19,7 @@ struct cvb_buf {
 struct cvb_ctx {
   int device = 0;
   cudaStream_t stream = nullptr;
-  int sm_count = 148;
+  int sm_count = 132;
   int64_t launches = 0;
   std::string err;
   // grow-only device workspaces (named slots so independent stages never alias)

@@ -1,4 +1,4 @@
-// match_kernels.cu — descriptor matching kernels for sm_100a and their C-ABI entry points.
+// match_kernels.cu — descriptor matching kernels for sm_90a and their C-ABI entry points.
 //
 //   scan_kernel<HammingMetric,…>   K1  brute-force Hamming k-NN          (cv::BFMatcher(NORM_HAMMING)::knnMatch,
 //                                      placerec_gen_be.cpp:82-100, RelNonCentralPosSolver.cpp:303-324)

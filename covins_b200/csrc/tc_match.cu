@@ -1,22 +1,22 @@
-// tc_match.cu — descriptor k-NN on the 5th-generation tensor cores (tcgen05, kind::i8, accumulators in TMEM).
+// tc_match.cu — descriptor k-NN on the Hopper tensor cores (wgmma.mma_async, integer kinds, accumulators in registers).
 //
 // Same contract as scan_kernel in match_kernels.cu (K1 Hamming / K2 L2 / K3 DenseMatcher lists), different bound.
-// The POPC formulation tops out at 16 POPC/clk/SM (measured: 94 % of that roofline).  Here the pairwise term is a
-// u8 x u8 -> s32 GEMM:
+// The POPC formulation is bound by the integer pipe.  Here the pairwise term is a u8 x u8 -> s32 GEMM:
 //     Hamming(a,b) = popc(a) + popc(b) - 2 <bits(a), bits(b)>      (bits expanded to 0/1 bytes in shared memory)
 //     |a-b|^2      = |a|^2 + |b|^2 - 2 <a, b>                      (u8 SIFT, exact in s32)
-// issued as tcgen05.mma.cta_group::1.kind::i8 (M = 128 queries, N = 128 train rows, K = 32 bytes per instruction) with
-// the 128x128 s32 accumulator in tensor memory.  One TMEM lane = one query row = one epilogue thread, which receives
-// the train rows of a tile in ascending order — so the per-query selection is the same sequential OpenCV /
-// DenseMatcher rule as in the scalar kernel and the result is bit-identical.
+// issued as wgmma.mma_async.m64n128k32.s32.u8.u8 by a warpgroup (64 queries x 128 train rows, K = 32 bytes per
+// instruction) with both operands in shared memory.  A thread of the warpgroup holds two query rows x 32 columns of the
+// accumulator (rows 16 w + lane / 4 and + 8, columns 8 i + 2 (lane % 4) + {0, 1}); it sees its columns in ascending order,
+// keeps per-row k-lists with the sequential OpenCV / DenseMatcher rule, and the four threads of a quad merge their lists
+// by (key, index) at the end of a segment — so the result is bit-identical to the scalar kernel.
 //
 // Warp-specialised, persistent CTA (one per SM), 4-stage ring:
-//   warps 0-3  epilogue   wait tmem_full[s] → tcgen05.ld 32x32b.x32 → d = pt[j] - 2 acc (+ pq) → k-list → tmem_empty[s]
-//   warps 4-7  producers  wait empty[s] → read packed rows from HBM (coalesced 16-B loads) → expand / copy into the
-//                         canonical K-major no-swizzle UMMA layout → fence.proxy.async → full[s]
-//   warp 8     MMA        wait full[s], tmem_empty[s] → K/32 x tcgen05.mma → tcgen05.commit → empty[s], tmem_full[s]
-// A CTA owns one block of 128 queries (expanded once, 32 KB of shared memory) and streams a contiguous range of
-// candidate segments.
+//   warps 0-7   consumers  (two warpgroups, query rows [0, 64) and [64, 128)): wait full[s] → K/32 x wgmma → wait →
+//                          empty[s] → epilogue d = pt[j] - 2 acc (+ pq) → k-lists
+//   warps 8-15  producers  wait empty[s] → read packed rows from HBM (coalesced 16-B loads) → expand / copy into the
+//                          canonical K-major no-swizzle layout → fence.proxy.async → full[s]
+// A CTA owns one block of 128 queries (expanded once into shared memory) and streams a contiguous range of candidate
+// segments.
 #include <float.h>
 #include <limits.h>
 #include <stdio.h>
@@ -30,123 +30,79 @@
 
 namespace cvb_tc {
 
-constexpr int TM = 128;       // queries per CTA (UMMA M)
-constexpr int TN = 128;       // train rows per tile (UMMA N)
+constexpr int TM = 128;       // queries per CTA (two warpgroups of 64)
+constexpr int TN = 128;       // train rows per tile (wgmma N)
 constexpr int STAGES = 4;        // shared-memory ring of expanded train tiles
-constexpr int ACC_STAGES = 3;    // TMEM ring of 128-column accumulators: columns [0, 384); the query operand sits at column 384
-constexpr uint32_t A_COL = ACC_STAGES * 128;
 constexpr int NORM_RING = 8;
 constexpr int kInf = 0x3FFFFFFF;   // list sentinel; rows that must never enter carry this as their norm term
 
-// ---- mbarrier / tcgen05 wrappers -------------------------------------------------------------------------------
+// ---- mbarrier / wgmma wrappers ---------------------------------------------------------------------------------
 __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(cvb_smem_addr(bar)) : "memory");
 }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ bool elect_one() {
-  uint32_t pred;
-  asm volatile(
-      "{\n"
-      ".reg .pred P;\n"
-      "elect.sync _|P, 0xffffffff;\n"
-      "selp.b32 %0, 1, 0, P;\n"
-      "}\n"
-      : "=r"(pred));
-  return pred != 0;
+
+#define CVB_D8(b) "+r"(d[b]), "+r"(d[b + 1]), "+r"(d[b + 2]), "+r"(d[b + 3]), "+r"(d[b + 4]), "+r"(d[b + 5]), "+r"(d[b + 6]), "+r"(d[b + 7])
+#define CVB_D64 CVB_D8(0), CVB_D8(8), CVB_D8(16), CVB_D8(24), CVB_D8(32), CVB_D8(40), CVB_D8(48), CVB_D8(56)
+#define CVB_R64                                                                                                         \
+  "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31," \
+  "%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}"
+// D[64 x 128] (+)= A[64 x 32] B[128 x 32]^T, both operands K-major in shared memory; B_SIGNED selects B = s8 (else u8)
+template <bool B_SIGNED>
+__device__ __forceinline__ void wg_mma_i8(uint32_t (&d)[64], uint64_t adesc, uint64_t bdesc, uint32_t acc) {
+  if constexpr (B_SIGNED) {
+    asm volatile(
+        "{\n.reg .pred p;\nsetp.ne.b32 p, %66, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n128k32.s32.u8.s8 " CVB_R64 ", %64, %65, p;\n}\n"
+        : CVB_D64 : "l"(adesc), "l"(bdesc), "r"(acc));
+  } else {
+    asm volatile(
+        "{\n.reg .pred p;\nsetp.ne.b32 p, %66, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n128k32.s32.u8.u8 " CVB_R64 ", %64, %65, p;\n}\n"
+        : CVB_D64 : "l"(adesc), "l"(bdesc), "r"(acc));
+  }
 }
-__device__ __forceinline__ void tc_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(cvb_smem_addr(bar))
-               : "memory");
+// the accumulator registers are written asynchronously: keep the compiler from moving their uses across the fence / wait
+__device__ __forceinline__ void wg_fence_operands(uint32_t (&d)[64]) {
+#pragma unroll
+  for (int i = 0; i < 64; i++) asm volatile("" : "+r"(d[i])::"memory");
 }
-__device__ __forceinline__ void tc_mma_i8(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t acc) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::i8 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(acc)
-      : "memory");
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_commit_wait() {
+  asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory");
+  asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory");
 }
-// A operand from tensor memory (row i of the 128 x K block in lane i, four K bytes per 32-bit column): the query block
-// is constant for the CTA's lifetime, and with both operands in shared memory the operand fetch alone (8 KB per 64-cycle
-// instruction) saturates the 128 B/clk shared-memory port that the producers' stores also need.
-__device__ __forceinline__ void tc_mma_i8_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t bdesc, uint32_t idesc, uint32_t acc) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::i8 [%0], [%1], %2, %3, p;\n"
-      "}\n" ::"r"(tmem_d),
-      "r"(tmem_a), "l"(bdesc), "r"(idesc), "r"(acc)
-      : "memory");
-}
-// 32 lanes x 8 columns per call: thread t of the warp writes registers r[0..7] to lane (warp % 4) * 32 + t
-__device__ __forceinline__ void tc_st8(uint32_t taddr, const uint32_t* r) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]),
-               "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7])
-               : "memory");
-}
-__device__ __forceinline__ void tc_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-        "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]),
-        "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-        "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+// NSLICE instructions of K = 32 over operands whose K chunks of 16 B lie 128 B apart (+256 B = +16 in the address field
+// per instruction); the accumulator is overwritten by the first
+template <bool B_SIGNED, int NSLICE>
+__device__ __forceinline__ void wg_gemm(uint32_t (&d)[64], uint64_t adesc0, uint64_t bdesc0) {
+  wg_fence_operands(d);
+  wg_fence();
+#pragma unroll
+  for (int k = 0; k < NSLICE; k++) wg_mma_i8<B_SIGNED>(d, adesc0 + (uint64_t)(k * 16), bdesc0 + (uint64_t)(k * 16), k > 0 ? 1u : 0u);
+  wg_commit_wait();
+  wg_fence_operands(d);
 }
 
-// 32 lanes x 32 columns, the low 16 bits of two adjacent columns packed into one register (even column low, odd column high)
-__device__ __forceinline__ void tc_ld32_pack16(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.pack::16b.x16.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-        "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-
-// 32 lanes x 128 columns as 64 packed registers
-__device__ __forceinline__ void tc_ld64_pack16(uint32_t taddr, uint32_t (&r)[64]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.pack::16b.x64.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,"
-      "%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, [%64];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-        "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]),
-        "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-        "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31]), "=r"(r[32]), "=r"(r[33]), "=r"(r[34]), "=r"(r[35]), "=r"(r[36]),
-        "=r"(r[37]), "=r"(r[38]), "=r"(r[39]), "=r"(r[40]), "=r"(r[41]), "=r"(r[42]), "=r"(r[43]), "=r"(r[44]), "=r"(r[45]),
-        "=r"(r[46]), "=r"(r[47]), "=r"(r[48]), "=r"(r[49]), "=r"(r[50]), "=r"(r[51]), "=r"(r[52]), "=r"(r[53]), "=r"(r[54]),
-        "=r"(r[55]), "=r"(r[56]), "=r"(r[57]), "=r"(r[58]), "=r"(r[59]), "=r"(r[60]), "=r"(r[61]), "=r"(r[62]), "=r"(r[63])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-
-// shared-memory matrix descriptor: K-major, no swizzle (canonical layout ((8,n),2):((16 B, SBO), LBO)); version 1
+// shared-memory matrix descriptor: K-major, no swizzle (core matrices of 8 rows x 16 B; LBO = stride between the two
+// core matrices of one K = 32 instruction, SBO = stride between 8-row groups); layout type 0 (interleave)
 __device__ __forceinline__ uint64_t make_desc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
   uint64_t d = 0;
   d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);
   d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
   d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= (uint64_t)1 << 46;   // descriptor version (Blackwell)
-  return d;                 // base_offset 0, lbo_mode 0, layout_type 0 (SWIZZLE_NONE)
-}
-// instruction descriptor, kind::i8: D = s32 (2), A = B = u8 (0), both K-major, N >> 3 at [17,23), M >> 4 at [24,29)
-__device__ __forceinline__ uint32_t make_idesc() {
-  return (2u << 4) | (0u << 7) | (0u << 10) | ((uint32_t)(TN >> 3) << 17) | ((uint32_t)(TM >> 4) << 24);
+  return d;
 }
 
 __device__ __forceinline__ uint4 ldg_nc(const void* p) {
   uint4 r;
   asm volatile("ld.global.nc.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(r.x), "=r"(r.y), "=r"(r.z), "=r"(r.w) : "l"(p));
   return r;
+}
+
+template <int S>
+__device__ __forceinline__ uint32_t shl(uint32_t w) {
+  if constexpr (S >= 0) return w << S; else return w >> (-S);
 }
 
 // ---- metrics: how a packed row becomes a K-major operand row, and its additive norm term ----------------------
@@ -161,28 +117,29 @@ struct TcHamming {
   static __device__ __forceinline__ void load_half(const uint8_t* __restrict__ row, int half, uint4 (&v)[kLoads]) {
     v[0] = ldg_nc(row + 16 * half);
   }
-  // writes operand chunks 8 half .. 8 half + 7 of the row and returns the partial popcount
+  // writes operand chunks 8 half .. 8 half + 7 of the row and returns the partial popcount.  A set bit becomes the byte
+  // 1 << BIT: 0x40 (u8 64) in the train operand of tc_scan_kernel, 0x80 (s8 -128) in the resident tiles.
+  template <int BIT = 6>
   static __device__ __forceinline__ int store_half(const uint4 (&v)[kLoads], int half, uint8_t* dst_row0) {
     const uint32_t w[4] = {v[0].x, v[0].y, v[0].z, v[0].w};
+    constexpr uint32_t M = 0x01010101u << BIT;
     int pc = 0;
 #pragma unroll
     for (int i = 0; i < 4; i++) {
       pc += __popc(w[i]);
-      // byte j of output word k is 0x80 if bit (k + 8 j) of w[i] is set, else 0 (the same permutation and the same
-      // 0/128 encoding on both operands → accumulator = 16384 * popc(a & b)).  The left shift is a multiply so that it
-      // issues on the FMA pipe; only the mask uses the (narrower) ALU pipe.
+      // byte j of output word k is 1 << BIT if bit (k + 8 j) of w[i] is set, else 0 (the same permutation on both operands)
       uint4 lo, hi;
-      lo.x = (w[i] * 128u) & 0x80808080u; lo.y = (w[i] * 64u) & 0x80808080u; lo.z = (w[i] * 32u) & 0x80808080u; lo.w = (w[i] * 16u) & 0x80808080u;
-      hi.x = (w[i] * 8u) & 0x80808080u; hi.y = (w[i] * 4u) & 0x80808080u; hi.z = (w[i] * 2u) & 0x80808080u; hi.w = w[i] & 0x80808080u;
+      lo.x = shl<BIT>(w[i]) & M; lo.y = shl<BIT - 1>(w[i]) & M; lo.z = shl<BIT - 2>(w[i]) & M; lo.w = shl<BIT - 3>(w[i]) & M;
+      hi.x = shl<BIT - 4>(w[i]) & M; hi.y = shl<BIT - 5>(w[i]) & M; hi.z = shl<BIT - 6>(w[i]) & M; hi.w = shl<BIT - 7>(w[i]) & M;
       *reinterpret_cast<uint4*>(dst_row0 + (8 * half + 2 * i) * 128) = lo;
       *reinterpret_cast<uint4*>(dst_row0 + (8 * half + 2 * i + 1) * 128) = hi;
     }
     return pc;
   }
-  // query side (tensor memory, one thread per row): the same K permutation with 0/1 bytes, so that accumulator =
-  // 128 * popc(a & b) = (2 popc(a & b)) << 6, which is what the packed 16-bit keys of the epilogue subtract.  Packed word i
-  // of the row becomes operand bytes [32 i, 32 i + 32) = one K = 32 instruction = 8 TMEM columns.
-  static constexpr int kQWords = 8;   // 32-byte operand groups per row
+  // query side (one thread per row): the same K permutation with 0/1 bytes, so that accumulator = 64 popc(a & b) =
+  // (2 popc(a & b)) << 5, which is what the packed 16-bit keys of the epilogue subtract.  Packed word i of the row becomes
+  // operand bytes [32 i, 32 i + 32) = one K = 32 instruction.
+  static constexpr int kQWords = 8;
   static __device__ __forceinline__ int load_q(const uint8_t* __restrict__ row, uint32_t (&w)[8]) {
     const uint4 a = ldg_nc(row), b = ldg_nc(row + 16);
     w[0] = a.x; w[1] = a.y; w[2] = a.z; w[3] = a.w; w[4] = b.x; w[5] = b.y; w[6] = b.z; w[7] = b.w;
@@ -262,18 +219,90 @@ __device__ __forceinline__ void insert_lex(int (&wk)[K], int (&wi)[K], int key, 
   }
   if (!placed) { wk[0] = key; wi[0] = idx; }
 }
+// sorted-list insertion of a packed int key (min/max network)
+template <int K>
+__device__ __forceinline__ void insert_packed(int (&wk)[K], int x) {
+#pragma unroll
+  for (int c = 0; c < K; c++) {
+    const int lo = min(wk[c], x);
+    x = max(wk[c], x);
+    wk[c] = lo;
+  }
+}
+template <int K>
+__device__ __forceinline__ void insert_packed16(unsigned (&pk)[K], unsigned x) {
+#pragma unroll
+  for (int c = 0; c < K; c++) {
+    const unsigned lo = __vminu2(pk[c], x);
+    x = __vmaxu2(pk[c], x);
+    pk[c] = lo;
+  }
+}
+// the four threads of a quad hold the lists of the same two rows over disjoint columns: after this all four hold the merge
+template <int K>
+__device__ __forceinline__ void quad_merge_packed(int (&wk)[K]) {
+#pragma unroll
+  for (int m = 1; m <= 2; m <<= 1) {
+    int o[K];
+#pragma unroll
+    for (int c = 0; c < K; c++) o[c] = __shfl_xor_sync(0xffffffffu, wk[c], m);
+#pragma unroll
+    for (int c = 0; c < K; c++) insert_packed<K>(wk, o[c]);
+  }
+}
+template <int K>
+__device__ __forceinline__ void quad_merge_lex(int (&wk)[K], int (&wi)[K]) {
+#pragma unroll
+  for (int m = 1; m <= 2; m <<= 1) {
+    int ok[K], oi[K];
+#pragma unroll
+    for (int c = 0; c < K; c++) { ok[c] = __shfl_xor_sync(0xffffffffu, wk[c], m); oi[c] = __shfl_xor_sync(0xffffffffu, wi[c], m); }
+#pragma unroll
+    for (int c = 0; c < K; c++)
+      if (oi[c] >= 0) insert_lex<K>(wk, wi, ok[c], oi[c]);
+  }
+}
 
-constexpr int GROUPS = 4;                       // epilogue column groups: group g owns columns [32 g, 32 g + 32) of every tile
-constexpr int EPI_THREADS = 128 * GROUPS;       // 16 epilogue warps
-constexpr int PROD_WARP0 = EPI_THREADS / 32;    // producer warps 16..23 (two threads per train row)
+// keys: Hamming → the distance; L2 → the bit pattern of sqrtf(d2) (non-negative floats order like their bits), which
+// is what OpenCV compares.  kInfKey is larger than any real key of either kind.
+constexpr int kInfKey = 0x7F000000;
+
+// one query's final list → outputs (filter: best match if it passes the threshold and the ratio test; else the k-list).
+// `writer` threads own one query row each; every lane of the warp must call this (ballot).
+template <int K, bool IS_L2>
+__device__ __forceinline__ void write_list(const TcParams& p, int seg, int q, bool writer, const int (&wk)[K], const int (&wi)[K],
+                                           const float (&fd)[K], int lane) {
+  const bool valid = writer && q < p.nq;
+  if (p.filter) {
+    bool ok = false;
+    if (K >= 2 && valid) {
+      const float dm = fd[0], dn = fd[K >= 2 ? 1 : 0];
+      ok = wi[0] >= 0 && wi[K >= 2 ? 1 : 0] >= 0 && dm <= p.thr && dm < __fmul_rn(p.ratio, dn);
+      const size_t o = (size_t)seg * p.nq + q;
+      p.match_train[o] = ok ? wi[0] : -1;
+      p.match_dist[o] = ok ? dm : FLT_MAX;
+    }
+    const unsigned b = __ballot_sync(0xffffffffu, ok);
+    if (lane == 0 && b) atomicAdd(&p.n_matches[seg], __popc(b));
+  } else if (valid) {
+    const size_t o = ((size_t)seg * p.nq + q) * K;
+#pragma unroll
+    for (int c = 0; c < K; c++) {
+      p.out_idx[o + c] = wi[c];
+      if (IS_L2) reinterpret_cast<float*>(p.out_dist)[o + c] = wi[c] >= 0 ? fd[c] : FLT_MAX;
+      else reinterpret_cast<int32_t*>(p.out_dist)[o + c] = wi[c] >= 0 ? wk[c] : INT_MAX;
+    }
+  }
+}
+
+constexpr int CONS_THREADS = 2 * 128;           // two consumer warpgroups
+constexpr int PROD_WARP0 = CONS_THREADS / 32;   // producer warps 8..15 (two threads per train row)
 constexpr int PROD_THREADS = 256;
-constexpr int MMA_WARP = PROD_WARP0 + PROD_THREADS / 32;   // warp 24
-constexpr int NUM_THREADS = (MMA_WARP + 1) * 32;
+constexpr int NUM_THREADS = CONS_THREADS + PROD_THREADS;
 
-template <class M, int K>
+template <class M>
 constexpr size_t smem_bytes() {
-  return (size_t)STAGES * TN * M::kKBytes + (size_t)NORM_RING * TN * sizeof(int) +
-         (size_t)2 * TM * GROUPS * K * 2 * sizeof(int) + 64 * sizeof(uint64_t);
+  return (size_t)(STAGES + 1) * TN * M::kKBytes + (size_t)NORM_RING * TN * sizeof(int) + 64 * sizeof(uint64_t);
 }
 
 // operand row r of a tile with KB operand bytes per row: byte offset of its chunk 0
@@ -282,58 +311,31 @@ __device__ __forceinline__ uint32_t row_offset(int r) {
   return (uint32_t)(r >> 3) * (KB * 8) + (uint32_t)(r & 7) * 16;
 }
 
-// keys: Hamming → the distance; L2 → the bit pattern of sqrtf(d2) (non-negative floats order like their bits), which
-// is what OpenCV compares.  kInfKey is larger than any real key of either kind.
-constexpr int kInfKey = 0x7F000000;
-
-// development trace (COVINS_B200_TC_DEBUG bit 16): clock64 stamps of CTA 0's first tiles, per role
-constexpr int TRACE_TILES = 48;
-__device__ long long g_tc_trace[3][TRACE_TILES][4];
-#define TC_STAMP(role, n, slot)                                                                                 \
-  do {                                                                                                          \
-    if ((p.dbg & 16) && blockIdx.x == 0 && (n) < TRACE_TILES) g_tc_trace[role][n][slot] = clock64();            \
-  } while (0)
-
 template <class M, int K>
 __global__ void __launch_bounds__(NUM_THREADS, 1) tc_scan_kernel(const TcParams p) {
   extern __shared__ __align__(1024) uint8_t smem[];
   constexpr int KB = M::kKBytes;
-  uint8_t* sB = smem;
+  uint8_t* sA = smem;                                        // the query block [TM][KB]
+  uint8_t* sB = sA + (size_t)TM * KB;                        // [STAGES][TN][KB]
   int* sNorm = reinterpret_cast<int*>(sB + (size_t)STAGES * TN * KB);
-  int* sList = sNorm + NORM_RING * TN;                       // [2][TM][GROUPS][K][2]
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sList + 2 * TM * GROUPS * K * 2);
-  uint64_t* full = bars;                 // [STAGES] producers → MMA (one arrival per producer warp)
-  uint64_t* empty = bars + STAGES;       // [STAGES] MMA completion → producers (tcgen05.commit)
-  uint64_t* tfull = bars + 2 * STAGES;   // [ACC_STAGES] MMA completion → epilogue (tcgen05.commit)
-  uint64_t* tempty = bars + 3 * STAGES;  // [ACC_STAGES] epilogue → MMA (one arrival per epilogue warp)
-  __shared__ uint32_t tmem_base_s;
+  uint64_t* bars = reinterpret_cast<uint64_t*>(sNorm + NORM_RING * TN);
+  uint64_t* full = bars;                 // [STAGES] producers → consumers (one arrival per producer warp)
+  uint64_t* empty = bars + STAGES;       // [STAGES] consumers' MMAs done → producers (one arrival per consumer warp)
   __shared__ int sQNorm[TM];
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int qb = blockIdx.x % p.nqb, part = blockIdx.x / p.nqb;
   const int seg0 = (int)((long)part * p.n_seg / p.parts), seg1 = (int)((long)(part + 1) * p.n_seg / p.parts);
 
-  // ---- one-time setup: barriers, TMEM, the query operand ----
+  // ---- one-time setup: barriers, the query operand ----
   if (tid == 0) {
     for (int s = 0; s < STAGES; s++) {
-      cvb_mbar_init(&full[s], PROD_THREADS / 32);     // one arrival per producer warp
-      cvb_mbar_init(&empty[s], 1);
-      cvb_mbar_init(&tfull[s], 1);
-      cvb_mbar_init(&tempty[s], EPI_THREADS / 32);    // one arrival per epilogue warp
+      cvb_mbar_init(&full[s], PROD_THREADS / 32);
+      cvb_mbar_init(&empty[s], CONS_THREADS / 32);
     }
     cvb_fence_mbar_init();
   }
-  if (warp == MMA_WARP) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], 512;" ::"r"(cvb_smem_addr(&tmem_base_s)));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = tmem_base_s;
   if (tid < TM) {
-    // the query block → tensor memory: thread = row = TMEM lane (warps 0-3 own lanes 32 w .. 32 w + 31), 8 columns
-    // (= one K = 32 instruction's worth) per tcgen05.st
     const int q = qb * TM + tid;
     uint32_t w[M::kIsL2 ? 32 : 8];
     int nrm = 0;
@@ -344,20 +346,19 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tc_scan_kernel(const TcParams 
       for (int i = 0; i < (M::kIsL2 ? 32 : 8); i++) w[i] = 0;
     }
     sQNorm[tid] = nrm;
-    const uint32_t a_taddr = tmem_base + ((uint32_t)(warp * 32) << 16) + A_COL;
+    uint8_t* dst = sA + row_offset<KB>(tid);
 #pragma unroll
     for (int i = 0; i < KB / 32; i++) {
       uint32_t r[8];
       M::expand_q(w, i, r);
-      tc_st8(a_taddr + 8 * i, r);
+      *reinterpret_cast<uint4*>(dst + (2 * i) * 128) = make_uint4(r[0], r[1], r[2], r[3]);
+      *reinterpret_cast<uint4*>(dst + (2 * i + 1) * 128) = make_uint4(r[4], r[5], r[6], r[7]);
     }
-    asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
+    fence_proxy_async();
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
 
-  if (warp >= PROD_WARP0 && warp < MMA_WARP) {
+  if (warp >= PROD_WARP0) {
     // =================================== producers ===================================
     // Two threads per train row; the packed rows of the next kPrefetch tiles are held in registers so that the HBM
     // latency (~1 us) of a tile overlaps the expansion of the previous ones.
@@ -402,9 +403,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tc_scan_kernel(const TcParams 
         for (int c = 0; c < M::kLoads; c++) cur[c] = pf[u][c];
         issue_load(pf[u]);   // refill this register slot with the tile PF steps ahead
         const int s = n % STAGES;
-        if (pt == 0) TC_STAMP(0, n, 0);
         if (n >= STAGES) cvb_mbar_wait(&empty[s], ((n / STAGES) - 1) & 1);
-        if (pt == 0) TC_STAMP(0, n, 1);
         uint8_t* dst = sB + (size_t)s * TN * KB + row_offset<KB>(prow);
         const bool rv = it.r0 + prow < it.len;
         int part = 0;
@@ -414,237 +413,135 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tc_scan_kernel(const TcParams 
           for (int c = 0; c < KB / 32; c++) *reinterpret_cast<uint4*>(dst + (half * (KB / 32) + c) * 128) = make_uint4(0, 0, 0, 0);
         }
         part += __shfl_xor_sync(0xffffffffu, part, 8);   // the two halves of a row sit 8 lanes apart
-        // Hamming: packed column term (popc(row) << 22 | segment-local index), L2: |row|^2; tail rows never enter a list
         if (M::kIsL2) {
           if (half == 0) sNorm[(n % NORM_RING) * TN + prow] = rv ? part : kInf;
         } else if (half == 0) {
-          // Hamming: 16-bit column term ((popc(row) + 256) << 6 | column within its 32-column group); 0xFFFF = no row
+          // Hamming: 16-bit column term ((popc(row) + 256) << 5 | slot), slot = 2 (column / 8) + column % 2 — the position
+          // of the column among the 32 columns one consumer thread holds; 0xFFFF = no row
           reinterpret_cast<uint16_t*>(sNorm)[(n % NORM_RING) * TN + prow] =
-              rv ? (uint16_t)(((part + 256) << 6) | (prow & 31)) : (uint16_t)0xFFFFu;
+              rv ? (uint16_t)(((part + 256) << 5) | ((prow >> 3) << 1) | (prow & 1)) : (uint16_t)0xFFFFu;
         }
-        // every lane makes its own stores visible to the async proxy; ONE arrival per warp (hundreds of same-address
-        // mbarrier arrivals per tile serialise in shared memory and cost more than the tile's MMAs)
-        if (pt == 0) TC_STAMP(0, n, 2);
+        // every lane makes its own stores visible to the async proxy; ONE arrival per warp
         fence_proxy_async();
         __syncwarp();
         if (lane == 0) mbar_arrive(&full[s]);
-        if (pt == 0) TC_STAMP(0, n, 3);
         it.advance();
         n++;
       }
     }
-  } else if (warp == MMA_WARP) {
-    // =================================== MMA issuer ===================================
-    // The WHOLE warp walks the tile sequence with warp-uniform values and one elected lane issues: under a divergent
-    // `if (lane == 0)` the compiler cannot keep the descriptors in uniform registers and wraps every tcgen05.mma in an
-    // ELECT / R2UR.BROADCAST waterfall loop (~150 cycles per instruction against the 64-cycle tensor floor).
-    const uint32_t idesc = make_idesc();
-    const uint32_t a_tmem = tmem_base + A_COL;
+  } else {
+    // =================================== consumers: warpgroup h = query rows [64 h, 64 h + 64) ===================================
+    const int h = warp >> 2;
+    const int quad = lane & 3;
+    const int row0 = 64 * h + 16 * (warp & 3) + (lane >> 2);   // this thread's rows: row0 and row0 + 8
+    const bool valid0 = qb * TM + row0 < p.nq, valid1 = qb * TM + row0 + 8 < p.nq;
+    const int qn0 = sQNorm[row0], qn1 = sQNorm[row0 + 8];
+    const uint64_t a_desc = make_desc(cvb_smem_addr(sA + (size_t)h * 64 * KB), 128, KB * 8);
     const uint32_t b_addr0 = cvb_smem_addr(sB);
+    int wk0[K], wi0[K], wd0[K], wk1[K], wi1[K], wd1[K];   // key, index, raw integer distance (pre-test only) per row
     int n = 0;
     for (int seg = seg0; seg < seg1; seg++) {
-      const int len = __shfl_sync(0xffffffffu, p.seg_ptr[seg + 1] - p.seg_ptr[seg], 0);
-      for (int r0 = 0; r0 < len; r0 += TN, n++) {
-        const int s = n % STAGES, ts = n % ACC_STAGES;
-        if (lane == 0) TC_STAMP(1, n, 0);
-        cvb_mbar_wait(&full[s], (n / STAGES) & 1);
-        if (lane == 0) TC_STAMP(1, n, 1);
-        if (n >= ACC_STAGES) cvb_mbar_wait(&tempty[ts], ((n / ACC_STAGES) - 1) & 1);
-        if (lane == 0) TC_STAMP(1, n, 2);
-        tc_fence_after();
-        const uint64_t b_desc0 = make_desc(b_addr0 + (uint32_t)s * (TN * KB), 128, KB * 8);
-        const uint32_t d_tmem = tmem_base + (uint32_t)ts * TN;
-        if (elect_one()) {
-#pragma unroll
-          for (int k = 0; k < KB / 32; k++)   // K chunk k: 256 B further in shared memory (+16 in the address field), 8 columns in TMEM
-            tc_mma_i8_ts(d_tmem, a_tmem + 8 * k, b_desc0 + (uint64_t)(k * 16), idesc, k > 0 ? 1u : 0u);
-          tc_commit(&empty[s]);    // shared-memory slot reusable once these MMAs have read it
-          tc_commit(&tfull[ts]);   // accumulator ready
-        }
-        if (lane == 0) TC_STAMP(1, n, 3);
-        __syncwarp();
-      }
-    }
-  } else {
-    // =================================== epilogue (warps 0..15) ===================================
-    const int grp = warp >> 2;                  // column group
-    const int row = (warp & 3) * 32 + lane;     // TMEM lane = query row inside the block
-    const int q = qb * TM + row;
-    const bool valid = q < p.nq;
-    const int qn = sQNorm[row];
-    int wk[K], wi[K], wd2[K];                   // key, index, raw integer distance (pre-test only)
-    int n = 0, segc = 0;
-    for (int seg = seg0; seg < seg1; seg++, segc++) {
       const int len = p.seg_ptr[seg + 1] - p.seg_ptr[seg];
 #pragma unroll
-      for (int c = 0; c < K; c++) { wk[c] = M::kIsL2 ? kInfKey : INT_MAX; wi[c] = -1; wd2[c] = kInf; }
+      for (int c = 0; c < K; c++) {
+        wk0[c] = wk1[c] = M::kIsL2 ? kInfKey : INT_MAX;
+        wi0[c] = wi1[c] = -1;
+        wd0[c] = wd1[c] = kInf;
+      }
       for (int r0 = 0; r0 < len; r0 += TN, n++) {
-        const int s = n % ACC_STAGES;
-        if (tid == 0) TC_STAMP(2, n, 0);
-        cvb_mbar_wait(&tfull[s], (n / ACC_STAGES) & 1);
-        if (tid == 0) TC_STAMP(2, n, 1);
-        tc_fence_after();
-        const uint32_t taddr = tmem_base + ((uint32_t)((warp & 3) * 32) << 16) + (uint32_t)s * TN + grp * 32;
-        uint32_t acc[32];
-        // Hamming: the accumulator 128 * popc(q & t) <= 32768 fits 16 bits, so two adjacent columns are read as ONE packed
-        // register (LDTM.x16.PACK16BIT: even column low, odd column high) — exactly the layout of the packed 16-bit keys
-        const bool pack16 = !M::kIsL2 && !(p.dbg & 8);   // dbg 8: the unpacked read (development comparison)
-        if (p.dbg & 4) {
-#pragma unroll
-          for (int i = 0; i < 32; i++) acc[i] = 0;      // experiment: no TMEM read at all (results invalid)
-        } else if (pack16) {
-          tc_ld32_pack16(taddr, acc);
-        } else {
-          tc_ld32(taddr, acc);
-        }
-        if (valid && !(p.dbg & 1)) {
+        const int s = n % STAGES;
+        cvb_mbar_wait(&full[s], (n / STAGES) & 1);
+        uint32_t acc[64];
+        wg_gemm<false, KB / 32>(acc, a_desc, make_desc(b_addr0 + (uint32_t)s * (TN * KB), 128, KB * 8));
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&empty[s]);   // operands consumed: the producers may refill this stage
+        if (!(p.dbg & 1)) {
           if (!M::kIsL2) {
-            // Two columns per instruction: 16-bit keys ((popc(t) - 2 popc(q & t) + 256) << 6 | column) packed pairwise
-            // (even column low, odd column high), k-lists kept per half with packed 16-bit min/max (VIMNMX.U16x2 issues
-            // at the 32-bit rate), merged into the 32-bit (distance, index) lists once per tile — and only if the tile
-            // holds a candidate that beats the current k-th entry (later tiles have larger indices, so "beats" is a
-            // strict distance comparison).
-            const uint4* nrm4 = reinterpret_cast<const uint4*>(reinterpret_cast<const uint16_t*>(sNorm) + (n % NORM_RING) * TN + grp * 32);
-            unsigned pk[K];
+            // Two columns per instruction: 16-bit keys ((popc(t) - 2 popc(q & t) + 256) << 5 | slot) packed pairwise
+            // (even column low, odd column high), k-lists kept per half with packed 16-bit min/max, merged into the 32-bit
+            // (distance, index) lists once per tile — and only if the tile holds a candidate that beats the current k-th
+            // entry (later tiles have larger indices, so "beats" is a strict distance comparison).
+            const uint32_t* nrm2 = reinterpret_cast<const uint32_t*>(reinterpret_cast<const uint16_t*>(sNorm) + (n % NORM_RING) * TN);
+            unsigned pk0[K], pk1[K];
 #pragma unroll
-            for (int c = 0; c < K; c++) pk[c] = 0xFFFFFFFFu;
+            for (int c = 0; c < K; c++) pk0[c] = pk1[c] = 0xFFFFFFFFu;
 #pragma unroll
-            for (int i4 = 0; i4 < 4; i4++) {
-              const uint4 nn = nrm4[i4];
-              const unsigned nv[4] = {nn.x, nn.y, nn.z, nn.w};
-#pragma unroll
-              for (int j = 0; j < 4; j++) {
-                const int i = 8 * i4 + 2 * j;   // columns i (low half) and i + 1 (high half)
-                unsigned x = pack16 ? nv[j] - acc[4 * i4 + j] : nv[j] + acc[i] * 0xFFFFFFFFu + acc[i + 1] * 0xFFFF0000u;
-#pragma unroll
-                for (int c = 0; c < K; c++) {
-                  const unsigned lo = __vminu2(pk[c], x);
-                  x = __vmaxu2(pk[c], x);
-                  pk[c] = lo;
-                }
-              }
+            for (int i = 0; i < 16; i++) {
+              const unsigned nv = nrm2[4 * i + quad];   // columns 8 i + 2 quad (low half) and + 1 (high half)
+              insert_packed16<K>(pk0, nv - __byte_perm(acc[4 * i], acc[4 * i + 1], 0x5410));
+              insert_packed16<K>(pk1, nv - __byte_perm(acc[4 * i + 2], acc[4 * i + 3], 0x5410));
             }
-            const unsigned best16 = min(pk[0] & 0xFFFFu, pk[0] >> 16);
-            const int worst_v = wk[K - 1] == INT_MAX ? 1024 : (wk[K - 1] >> kIdxBits) + 256;   // arithmetic shift: t-domain value
-            if ((int)(best16 >> 6) < worst_v) {
 #pragma unroll
-              for (int c = 0; c < K; c++)
+            for (int rr = 0; rr < 2; rr++) {
+              unsigned (&pk)[K] = rr ? pk1 : pk0;
+              int (&wk)[K] = rr ? wk1 : wk0;
+              const unsigned best16 = min(pk[0] & 0xFFFFu, pk[0] >> 16);
+              const int worst_v = wk[K - 1] == INT_MAX ? 1024 : (wk[K - 1] >> kIdxBits) + 256;   // arithmetic shift: t-domain value
+              if ((int)(best16 >> 5) < worst_v) {
 #pragma unroll
-                for (int h = 0; h < 2; h++) {
-                  const unsigned k16 = h ? (pk[c] >> 16) : (pk[c] & 0xFFFFu);
-                  int x = k16 == 0xFFFFu ? INT_MAX
-                                         : (int)((((unsigned)(k16 >> 6) - 256u) << kIdxBits) + (unsigned)(r0 + grp * 32 + (int)(k16 & 63u)));
+                for (int c = 0; c < K; c++)
 #pragma unroll
-                  for (int cc = 0; cc < K; cc++) {
-                    const int lo = min(wk[cc], x);
-                    x = max(wk[cc], x);
-                    wk[cc] = lo;
+                  for (int hh = 0; hh < 2; hh++) {
+                    const unsigned k16 = hh ? (pk[c] >> 16) : (pk[c] & 0xFFFFu);
+                    const int col = 8 * (int)((k16 & 31u) >> 1) + 2 * quad + (int)(k16 & 1u);
+                    insert_packed<K>(wk, k16 == 0xFFFFu ? INT_MAX
+                                                        : (int)((((unsigned)(k16 >> 5) - 256u) << kIdxBits) + (unsigned)(r0 + col)));
                   }
-                }
+              }
             }
           } else {
-            const int4* nrm4 = reinterpret_cast<const int4*>(sNorm + (n % NORM_RING) * TN + grp * 32);
+            const int* nrm = sNorm + (n % NORM_RING) * TN;
 #pragma unroll
-            for (int i4 = 0; i4 < 8; i4++) {
-              const int4 nn = nrm4[i4];
-              const int nv[4] = {nn.x, nn.y, nn.z, nn.w};
+            for (int i = 0; i < 16; i++) {
+              const int2 nn = *reinterpret_cast<const int2*>(nrm + 8 * i + 2 * quad);
 #pragma unroll
-              for (int j = 0; j < 4; j++) {
-                const int i = 4 * i4 + j;
-                const int d = qn + nv[j] - 2 * (int)acc[i];
-                if (d < wd2[K - 1]) {
+              for (int e = 0; e < 4; e++) {
+                const int j = 8 * i + 2 * quad + (e & 1);
+                const int tn = (e & 1) ? nn.y : nn.x;
+                int (&wk)[K] = e < 2 ? wk0 : wk1;
+                int (&wi)[K] = e < 2 ? wi0 : wi1;
+                int (&wd)[K] = e < 2 ? wd0 : wd1;
+                const int d = (e < 2 ? qn0 : qn1) + tn - 2 * (int)acc[4 * i + e];
+                if (d < wd[K - 1]) {
                   const int key = __float_as_int(__fsqrt_rn((float)d));
                   if (key < wk[K - 1]) {
-                    insert_key<K>(wk, wi, key, r0 + grp * 32 + i);
+                    insert_key<K>(wk, wi, key, r0 + j);
                     const float f = __int_as_float(wk[K - 1]);   // raw-distance bound of the worst entry (pre-test)
-                    wd2[K - 1] = wk[K - 1] == kInfKey ? kInf : (int)ceilf(f * f * 1.000001f) + 1;
+                    wd[K - 1] = wk[K - 1] == kInfKey ? kInf : (int)ceilf(f * f * 1.000001f) + 1;
                   }
                 }
               }
             }
           }
         }
-        if (tid == 0) TC_STAMP(2, n, 2);
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&tempty[s]);
-        if (tid == 0) TC_STAMP(2, n, 3);   // accumulator and norms consumed: the MMA warp may overwrite this TMEM stage
       }
-      // ---- segment finished: combine the 4 column-group lists of each query (k smallest by (key, idx)) ----
-      int* lst = sList + (size_t)(segc & 1) * TM * GROUPS * K * 2;
+      // ---- segment finished: merge the quad's lists; lane quad 0 writes row0, quad 1 writes row0 + 8 ----
+      const bool second = quad == 1;
+      int wk[K], wi[K];
+      float fd[K];
       if (!M::kIsL2) {
-        const int qq = qn << kIdxBits;
-#pragma unroll
-        for (int c = 0; c < K; c++) lst[(row * GROUPS + grp) * K + c] = wk[c] == INT_MAX ? INT_MAX : wk[c] + qq;
-      } else {
+        quad_merge_packed<K>(wk0);
+        quad_merge_packed<K>(wk1);
+        const int qq = (second ? qn1 : qn0) << kIdxBits;
 #pragma unroll
         for (int c = 0; c < K; c++) {
-          lst[((row * GROUPS + grp) * K + c) * 2 + 0] = wk[c];
-          lst[((row * GROUPS + grp) * K + c) * 2 + 1] = wi[c];
+          const int x = second ? wk1[c] : wk0[c];
+          wi[c] = x == INT_MAX ? -1 : (x & ((1 << kIdxBits) - 1));
+          wk[c] = x == INT_MAX ? INT_MAX : ((x + qq) >> kIdxBits);
+          fd[c] = (float)wk[c];
+        }
+      } else {
+        quad_merge_lex<K>(wk0, wi0);
+        quad_merge_lex<K>(wk1, wi1);
+#pragma unroll
+        for (int c = 0; c < K; c++) {
+          wk[c] = second ? wk1[c] : wk0[c];
+          wi[c] = second ? wi1[c] : wi0[c];
+          fd[c] = __int_as_float(wk[c]);
         }
       }
-      asm volatile("bar.sync 1, %0;" ::"n"(EPI_THREADS) : "memory");
-      if (grp == 0) {
-        float fd[K];   // final distances as float (DMatch::distance)
-        if (!M::kIsL2) {
-#pragma unroll
-          for (int c = 0; c < K; c++) wk[c] = INT_MAX;
-          for (int e = 0; e < GROUPS * K; e++) {
-            int x = lst[row * GROUPS * K + e];
-#pragma unroll
-            for (int c = 0; c < K; c++) {
-              const int lo = min(wk[c], x);
-              x = max(wk[c], x);
-              wk[c] = lo;
-            }
-          }
-#pragma unroll
-          for (int c = 0; c < K; c++) {
-            wi[c] = wk[c] == INT_MAX ? -1 : (wk[c] & ((1 << kIdxBits) - 1));
-            wk[c] = wk[c] == INT_MAX ? INT_MAX : (wk[c] >> kIdxBits);
-            fd[c] = (float)wk[c];
-          }
-        } else {
-#pragma unroll
-          for (int c = 0; c < K; c++) { wk[c] = kInfKey; wi[c] = -1; }
-          for (int g2 = 0; g2 < GROUPS; g2++)
-#pragma unroll
-            for (int c = 0; c < K; c++) {
-              const int kk = lst[((row * GROUPS + g2) * K + c) * 2], ii = lst[((row * GROUPS + g2) * K + c) * 2 + 1];
-              if (ii >= 0) insert_lex<K>(wk, wi, kk, ii);
-            }
-#pragma unroll
-          for (int c = 0; c < K; c++) fd[c] = __int_as_float(wk[c]);
-        }
-        if (p.filter) {
-          bool ok = false;
-          if (K >= 2 && valid) {
-            const float dm = fd[0], dn = fd[K >= 2 ? 1 : 0];
-            ok = wi[0] >= 0 && wi[K >= 2 ? 1 : 0] >= 0 && dm <= p.thr && dm < __fmul_rn(p.ratio, dn);
-            const size_t o = (size_t)seg * p.nq + q;
-            p.match_train[o] = ok ? wi[0] : -1;
-            p.match_dist[o] = ok ? dm : FLT_MAX;
-          }
-          const unsigned b = __ballot_sync(0xffffffffu, ok);
-          if (lane == 0 && b) atomicAdd(&p.n_matches[seg], __popc(b));
-        } else if (valid) {
-          const size_t o = ((size_t)seg * p.nq + q) * K;
-#pragma unroll
-          for (int c = 0; c < K; c++) {
-            p.out_idx[o + c] = wi[c];
-            if (M::kIsL2) reinterpret_cast<float*>(p.out_dist)[o + c] = wi[c] >= 0 ? fd[c] : FLT_MAX;
-            else reinterpret_cast<int32_t*>(p.out_dist)[o + c] = wi[c] >= 0 ? wk[c] : INT_MAX;
-          }
-        }
-      }
+      write_list<K, M::kIsL2>(p, seg, qb * TM + row0 + (second ? 8 : 0), quad < 2 && (second ? valid1 : valid0), wk, wi, fd, lane);
     }
-  }
-  // ---- teardown ----
-  tc_fence_before();
-  __syncthreads();
-  if (warp == MMA_WARP) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, 512;" ::"r"(tmem_base));
   }
 }
 
@@ -657,37 +554,34 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tc_scan_kernel(const TcParams 
 // from shared memory.  Both disappear when the operand the tensor core reads is stored once and reused by every query:
 //
 //   * cvb_tc::expand_tiles writes, per keyframe, ceil(rows / 128) tiles of 128 rows x 288 operand bytes in exactly the
-//     shared-memory image tcgen05.mma wants (K-major, no swizzle, 8-row groups of 2304 B): 256 data bytes (0x80 = -128
+//     shared-memory image wgmma wants (K-major, no swizzle, 8-row groups of 2304 B): 256 data bytes (0x80 = -128
 //     as s8 for a set bit) + a 32-byte KEY slice.  A tile is 36 KB and contiguous, so the producer is ONE thread issuing
 //     cp.async.bulk copies (TMA engine) — no register path, no expansion in the matching kernel.  The map database
-//     (map_db.cu) keeps these tiles resident next to the packed rows; 9 bytes of HBM per descriptor byte, read at
-//     ~2 TB/s by a kernel that is bound by the tensor pipe, not by HBM.
+//     (map_db.cu) keeps these tiles resident next to the packed rows; 9 bytes of HBM per descriptor byte.
 //   * the key slice folds the whole distance into the GEMM: with query bytes 0/2 (u8) and
 //         A key bytes = [1, 128, 128, 128, c4, c5, c6, 0...]   c4 + c5 + c6 = 2 popc(q)      (per query row)
 //         B key bytes = [col, p1, p2, p3, 64, 64, 64, 0...]    p1 + p2 + p3 = popc(t)        (per train row)
 //     the s32 accumulator is  (popc(q) + popc(t) - 2 popc(q & t)) << 7 | col  =  Hamming << 7 | row-in-tile: the sort key
-//     itself, <= 32895, so the epilogue reads it as packed 16-bit pairs (LDTM.PACK16BIT) and runs nothing but the
-//     packed min/max network.  Rows past a keyframe's end carry B key bytes [127,127,127,127,0...] → key 48895, which
-//     never enters a list.
-//   * three segment STREAMS: epilogue group g (4 warps = the 128 TMEM lanes) owns accumulator g and every third
-//     keyframe of the CTA's range; the MMA warp and the producer interleave the three streams' tiles.  A (query,
-//     keyframe) list therefore lives in ONE thread's registers from the first tile to the output — no cross-group
-//     merge, no shared-memory lists, no CTA barrier per keyframe — and three tiles are in different phases at any time.
+//     itself, <= 32895, so the epilogue packs two adjacent columns into one register and runs nothing but the packed
+//     min/max network.  Rows past a keyframe's end carry B key bytes [127,127,127,127,0...] → key 48895, which never
+//     enters a list.
+//   * NGRP segment STREAMS: consumer warpgroups (h, g) own query rows [64 h, 64 h + 64) and every NGRP-th keyframe of the
+//     CTA's range starting at g; the producer interleaves the streams' tiles, so while one stream's warpgroups run
+//     their epilogue the other's keep the tensor cores busy.  A (query, keyframe) list lives in one quad's registers
+//     from the first tile to the output — no shared-memory lists, no CTA barrier per keyframe.
 namespace xt {
 constexpr int KX = 288;                       // operand bytes per row
 constexpr int NSLICE = KX / 32;               // 9 instructions of K = 32 per tile
 constexpr int TILE_BYTES = TN * KX;           // 36864
-constexpr int XSTAGES = 5;                    // shared-memory ring (180 KB)
-constexpr int NGRP = 3;                       // streams = epilogue groups = accumulators
-constexpr int EPI_WARPS = 4 * NGRP;
-constexpr int TMA_WARP = EPI_WARPS;
-constexpr int MMA_WARP_X = EPI_WARPS + 1;
-constexpr int XTHREADS = (MMA_WARP_X + 1) * 32;
-constexpr uint32_t XA_COL = NGRP * 128;       // query operand: TMEM columns [384, 456)
+constexpr int XSTAGES = 5;                    // shared-memory ring (180 KB) — more than NGRP (phase parity of full[])
+constexpr int NGRP = 2;                       // streams
+constexpr int CONS_WARPS = 4 * 2 * NGRP;      // warpgroups (h, g), h = query half
+constexpr int TMA_WARP = CONS_WARPS;
+constexpr int XTHREADS = (TMA_WARP + 1) * 32;
 constexpr int kKeyInvalid = 32896;            // keys >= this are "no row"
 constexpr int kPaceWindow = 96;               // tiles a CTA may run ahead of the slowest CTA of its keyframe range (3.4 MB)
 constexpr long kPaceMinTiles = 1536;          // pacing only when a CTA walks more tiles than this
-constexpr size_t kSmemBytes = (size_t)XSTAGES * TILE_BYTES + 1024;
+constexpr size_t kSmemBytes = (size_t)(XSTAGES + 1) * TILE_BYTES + 1024;   // query block + ring + barriers
 
 __device__ __forceinline__ uint32_t xrow_off(int r) { return (uint32_t)(r >> 3) * (KX * 8) + (uint32_t)(r & 7) * 16; }
 
@@ -709,7 +603,7 @@ __global__ void __launch_bounds__(256) expand_tiles_kernel(const uint8_t* __rest
   if (rv) {
     uint4 v[1];
     TcHamming::load_half(t + (size_t)(s_begin + r0 + prow) * 32, half, v);
-    part = TcHamming::store_half(v, half, dst);
+    part = TcHamming::store_half<7>(v, half, dst);
   } else {
 #pragma unroll
     for (int c = 0; c < 8; c++) *reinterpret_cast<uint4*>(dst + (8 * half + c) * 128) = make_uint4(0, 0, 0, 0);
@@ -729,7 +623,7 @@ __global__ void __launch_bounds__(256) expand_tiles_kernel(const uint8_t* __rest
 }
 
 // the interleaved tile sequence of a CTA: stream g walks keyframes seg0 + g, seg0 + g + NGRP, ... ; round-robin over the
-// streams that still have tiles.  Producer, MMA warp and (per stream) the epilogue groups generate the same sequence.
+// streams that still have tiles.  Producer and consumers generate the same sequence.
 struct Streams {
   int seg[NGRP], t[NGRP], nt[NGRP], tile0[NGRP];
   int seg1;
@@ -749,7 +643,12 @@ struct Streams {
     for (int g = 0; g < NGRP; g++) { seg[g] = seg0 + g; nt[g] = 0; tile0[g] = 0; load(g); }
   }
   __device__ bool active(int g) const { return seg[g] < seg1; }
-  __device__ bool any() const { return seg[0] < seg1 || seg[1] < seg1 || seg[2] < seg1; }
+  __device__ bool any() const {
+    bool a = false;
+#pragma unroll
+    for (int g = 0; g < NGRP; g++) a |= seg[g] < seg1;
+    return a;
+  }
   __device__ void advance(int g) {
     if (++t[g] >= nt[g]) { seg[g] += NGRP; load(g); }
   }
@@ -758,33 +657,22 @@ struct Streams {
 template <int K>
 __global__ void __launch_bounds__(XTHREADS, 1) tc_xt_kernel(const TcParams p) {
   extern __shared__ __align__(1024) uint8_t smem[];
-  uint8_t* sB = smem;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + (size_t)XSTAGES * TILE_BYTES);
+  uint8_t* sA = smem;                                  // the query block, one tile image [TM][KX]
+  uint8_t* sB = smem + TILE_BYTES;                     // [XSTAGES] tiles
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + (size_t)(XSTAGES + 1) * TILE_BYTES);
   uint64_t* full = bars;                  // [XSTAGES] TMA bytes landed (expect_tx)
-  uint64_t* empty = bars + XSTAGES;       // [XSTAGES] MMAs that read the stage completed (tcgen05.commit)
-  uint64_t* tfull = bars + 2 * XSTAGES;   // [NGRP] accumulator g complete (tcgen05.commit)
-  uint64_t* tempty = tfull + NGRP;        // [NGRP] accumulator g read back by its 4 warps
-  __shared__ uint32_t tmem_base_s;
+  uint64_t* empty = bars + XSTAGES;       // [XSTAGES] the stage's two warpgroups finished their MMAs (one arrival per warp)
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int qb = blockIdx.x % p.nqb, part = blockIdx.x / p.nqb;
   const int seg0 = (int)((long)part * p.n_seg / p.parts), seg1 = (int)((long)(part + 1) * p.n_seg / p.parts);
 
   if (tid == 0) {
-    for (int s = 0; s < XSTAGES; s++) { cvb_mbar_init(&full[s], 1); cvb_mbar_init(&empty[s], 1); }
-    for (int g = 0; g < NGRP; g++) { cvb_mbar_init(&tfull[g], 1); cvb_mbar_init(&tempty[g], 4); }
+    for (int s = 0; s < XSTAGES; s++) { cvb_mbar_init(&full[s], 1); cvb_mbar_init(&empty[s], 8); }
     cvb_fence_mbar_init();
   }
-  if (warp == MMA_WARP_X) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], 512;" ::"r"(cvb_smem_addr(&tmem_base_s)));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = tmem_base_s;
   if (tid < TM) {
-    // query block → tensor memory (thread = row = lane): data bytes 0/2, then the key slice
+    // query block → shared memory (thread = row): data bytes 0/2, then the key slice
     const int q = qb * TM + tid;
     uint32_t w[8];
     int pq = 0;
@@ -794,25 +682,25 @@ __global__ void __launch_bounds__(XTHREADS, 1) tc_xt_kernel(const TcParams p) {
 #pragma unroll
       for (int i = 0; i < 8; i++) w[i] = 0;
     }
-    const uint32_t a_taddr = tmem_base + ((uint32_t)(warp * 32) << 16) + XA_COL;
+    uint8_t* dst = sA + xrow_off(tid);
 #pragma unroll
     for (int i = 0; i < 8; i++) {
       uint32_t r[8];
 #pragma unroll
       for (int b = 0; b < 8; b++) r[b] = ((w[i] >> b) & 0x01010101u) * 2u;
-      tc_st8(a_taddr + 8 * i, r);
+      *reinterpret_cast<uint4*>(dst + (2 * i) * 128) = make_uint4(r[0], r[1], r[2], r[3]);
+      *reinterpret_cast<uint4*>(dst + (2 * i + 1) * 128) = make_uint4(r[4], r[5], r[6], r[7]);
     }
     {
       const int c4 = min(2 * pq, 255), c5 = min(2 * pq - c4, 255), c6 = 2 * pq - c4 - c5;
-      uint32_t r[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-      if (q < p.nq) { r[0] = 0x80808001u; r[1] = (uint32_t)c4 | ((uint32_t)c5 << 8) | ((uint32_t)c6 << 16); }
-      tc_st8(a_taddr + 64, r);
+      uint4 key = make_uint4(0, 0, 0, 0);
+      if (q < p.nq) { key.x = 0x80808001u; key.y = (uint32_t)c4 | ((uint32_t)c5 << 8) | ((uint32_t)c6 << 16); }
+      *reinterpret_cast<uint4*>(dst + 16 * 128) = key;
+      *reinterpret_cast<uint4*>(dst + 17 * 128) = make_uint4(0, 0, 0, 0);
     }
-    asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
+    fence_proxy_async();
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
 
   if (warp == TMA_WARP) {
     // =================================== producer: one thread, bulk copies ===================================
@@ -828,8 +716,8 @@ __global__ void __launch_bounds__(XTHREADS, 1) tc_xt_kernel(const TcParams p) {
           if (p.progress != nullptr && (n & 15) == 0 && n > 0) {
             // Pacing (large maps only): the nqb CTAs that walk the same keyframe range read every tile once from HBM and
             // nqb - 1 times from L2 — as long as they stay within an L2's worth of each other.  Over thousands of tiles they
-            // drift apart (C5: 4448 tiles per CTA → 8x the HBM traffic, 4.8x the time); the producer therefore publishes its
-            // position every 16 tiles and waits while it is more than kPaceWindow tiles ahead of the slowest CTA of its group.
+            // can drift apart; the producer therefore publishes its position every 16 tiles and waits while it is more than
+            // kPaceWindow tiles ahead of the slowest CTA of its group.
             // (All CTAs are resident — grid <= SM count, one CTA per SM — so the wait cannot deadlock.)
             volatile int* grp_prog = p.progress + (size_t)part * p.nqb;
             grp_prog[qb] = n;
@@ -857,137 +745,98 @@ __global__ void __launch_bounds__(XTHREADS, 1) tc_xt_kernel(const TcParams p) {
       }
     }
     __syncwarp();
-  } else if (warp == MMA_WARP_X) {
-    // =================================== MMA issuer (warp-uniform, one elected lane) ===================================
-    // instruction descriptor: D = s32, A = u8, B = s8, both K-major, N = 128, M = 128
-    const uint32_t idesc = (2u << 4) | (0u << 7) | (1u << 10) | ((uint32_t)(TN >> 3) << 17) | ((uint32_t)(TM >> 4) << 24);
-    const uint32_t a_tmem = tmem_base + XA_COL;
+  } else {
+    // =================================== consumer warpgroup (h, g): every NGRP-th keyframe, start to finish ===================================
+    const int h = (warp >> 2) & 1, g = warp >> 3;
+    const int quad = lane & 3;
+    const int row0 = 64 * h + 16 * (warp & 3) + (lane >> 2);   // this thread's rows: row0 and row0 + 8
+    const uint64_t a_desc = make_desc(cvb_smem_addr(sA + (size_t)h * 8 * (KX * 8)), 128, KX * 8);
     const uint32_t b_addr0 = cvb_smem_addr(sB);
+    // empty keyframes of this stream have no tiles: their (empty) lists are written here
+    for (int seg = seg0 + g; seg < seg1; seg += NGRP) {
+      if (p.seg_tile[seg + 1] != p.seg_tile[seg]) continue;
+      int wk[K], wi[K];
+      float fd[K];
+#pragma unroll
+      for (int c = 0; c < K; c++) { wk[c] = INT_MAX; wi[c] = -1; fd[c] = (float)INT_MAX; }
+      write_list<K, false>(p, seg, qb * TM + row0 + (quad == 1 ? 8 : 0), quad < 2, wk, wi, fd, lane);
+    }
     Streams S;
     S.init(seg0, seg1, p.seg_tile);
-    int n = 0, j[NGRP] = {0, 0, 0};
+    int wk0[K], wk1[K];   // (distance << kIdxBits) + row within the keyframe, ascending — rows row0 and row0 + 8
+    int n = 0;
     while (S.any()) {
 #pragma unroll
-      for (int g = 0; g < NGRP; g++) {
-        if (!S.active(g)) continue;
-        const int s = n % XSTAGES;
-        cvb_mbar_wait(&full[s], (n / XSTAGES) & 1);
-        if (j[g] >= 1) cvb_mbar_wait(&tempty[g], (j[g] - 1) & 1);
-        tc_fence_after();
-        const uint64_t b_desc0 = make_desc(b_addr0 + (uint32_t)s * TILE_BYTES, 128, KX * 8);
-        const uint32_t d_tmem = tmem_base + (uint32_t)g * TN;
-        if (elect_one()) {
+      for (int g2 = 0; g2 < NGRP; g2++) {
+        if (!S.active(g2)) continue;
+        if (g2 == g) {
+          const int t = S.t[g2];
+          if (t == 0) {
 #pragma unroll
-          for (int k = 0; k < NSLICE; k++)
-            tc_mma_i8_ts(d_tmem, a_tmem + 8 * k, b_desc0 + (uint64_t)(k * 16), idesc, k > 0 ? 1u : 0u);
-          tc_commit(&empty[s]);
-          tc_commit(&tfull[g]);
+            for (int c = 0; c < K; c++) wk0[c] = wk1[c] = INT_MAX;
+          }
+          const int s = n % XSTAGES;
+          cvb_mbar_wait(&full[s], (n / XSTAGES) & 1);
+          uint32_t acc[64];
+          wg_gemm<true, NSLICE>(acc, a_desc, make_desc(b_addr0 + (uint32_t)s * TILE_BYTES, 128, KX * 8));
+          __syncwarp();
+          if (lane == 0) mbar_arrive(&empty[s]);   // operands consumed: the producer may refill this stage
+          if (!(p.dbg & 1)) {
+            unsigned pk0[K], pk1[K];
+#pragma unroll
+            for (int c = 0; c < K; c++) pk0[c] = pk1[c] = 0xFFFFFFFFu;
+#pragma unroll
+            for (int i = 0; i < 16; i++) {   // columns 8 i + 2 quad (low half) and + 1 (high half)
+              insert_packed16<K>(pk0, __byte_perm(acc[4 * i], acc[4 * i + 1], 0x5410));
+              insert_packed16<K>(pk1, __byte_perm(acc[4 * i + 2], acc[4 * i + 3], 0x5410));
+            }
+            // later tiles hold larger row indices: a candidate enters only with a strictly smaller distance than the k-th entry
+#pragma unroll
+            for (int rr = 0; rr < 2; rr++) {
+              unsigned (&pk)[K] = rr ? pk1 : pk0;
+              int (&wk)[K] = rr ? wk1 : wk0;
+              const unsigned best16 = min(pk[0] & 0xFFFFu, pk[0] >> 16);
+              const int worst_d = wk[K - 1] == INT_MAX ? 1024 : (wk[K - 1] >> kIdxBits);
+              if ((int)(best16 >> 7) < worst_d) {
+#pragma unroll
+                for (int c = 0; c < K; c++)
+#pragma unroll
+                  for (int hh = 0; hh < 2; hh++) {
+                    const unsigned k16 = hh ? (pk[c] >> 16) : (pk[c] & 0xFFFFu);
+                    insert_packed<K>(wk, k16 >= (unsigned)kKeyInvalid ? INT_MAX
+                                                                     : (int)(((k16 >> 7) << kIdxBits) + (unsigned)(t * TN) + (k16 & 127u)));
+                  }
+              }
+            }
+          }
+          if (t == S.nt[g2] - 1) {
+            // ---- keyframe finished: merge the quad's lists; lane quad 0 writes row0, quad 1 writes row0 + 8 ----
+            quad_merge_packed<K>(wk0);
+            quad_merge_packed<K>(wk1);
+            const bool second = quad == 1;
+            int wk[K], wi[K];
+            float fd[K];
+#pragma unroll
+            for (int c = 0; c < K; c++) {
+              const int x = second ? wk1[c] : wk0[c];
+              wi[c] = x == INT_MAX ? -1 : (x & ((1 << kIdxBits) - 1));
+              wk[c] = x == INT_MAX ? INT_MAX : (x >> kIdxBits);
+              fd[c] = (float)wk[c];
+            }
+            write_list<K, false>(p, S.seg[g2], qb * TM + row0 + (second ? 8 : 0), quad < 2, wk, wi, fd, lane);
+          }
         }
-        __syncwarp();
-        S.advance(g);
-        j[g]++;
+        S.advance(g2);
         n++;
       }
     }
-  } else {
-    // =================================== epilogue group g: every NGRP-th keyframe, start to finish ===================================
-    const int g = warp >> 2;
-    const int row = (warp & 3) * 32 + lane;
-    const int q = qb * TM + row;
-    const bool valid = q < p.nq;
-    const uint32_t taddr = tmem_base + ((uint32_t)((warp & 3) * 32) << 16) + (uint32_t)g * TN;
-    int jt = 0;
-    for (int seg = seg0 + g; seg < seg1; seg += NGRP) {
-      const int nt = p.seg_tile[seg + 1] - p.seg_tile[seg];
-      int wk[K];   // (distance << kIdxBits) + row within the keyframe, ascending
-#pragma unroll
-      for (int c = 0; c < K; c++) wk[c] = INT_MAX;
-      for (int t = 0; t < nt; t++, jt++) {
-        cvb_mbar_wait(&tfull[g], jt & 1);
-        tc_fence_after();
-        uint32_t acc[64];
-        tc_ld64_pack16(taddr, acc);            // 128 columns: register i = columns 2 i (low half) and 2 i + 1 (high half)
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&tempty[g]);   // accumulator in registers: the MMA warp may start this stream's next tile
-        if (valid && !(p.dbg & 1)) {
-          unsigned pk[K];
-#pragma unroll
-          for (int c = 0; c < K; c++) pk[c] = 0xFFFFFFFFu;
-#pragma unroll
-          for (int i = 0; i < 64; i++) {
-            unsigned x = acc[i];
-#pragma unroll
-            for (int c = 0; c < K; c++) {
-              const unsigned lo = __vminu2(pk[c], x);
-              x = __vmaxu2(pk[c], x);
-              pk[c] = lo;
-            }
-          }
-          // later tiles hold larger row indices: a candidate enters only with a strictly smaller distance than the k-th entry
-          const unsigned best16 = min(pk[0] & 0xFFFFu, pk[0] >> 16);
-          const int worst_d = wk[K - 1] == INT_MAX ? 1024 : (wk[K - 1] >> kIdxBits);
-          if ((int)(best16 >> 7) < worst_d) {
-#pragma unroll
-            for (int c = 0; c < K; c++)
-#pragma unroll
-              for (int h = 0; h < 2; h++) {
-                const unsigned k16 = h ? (pk[c] >> 16) : (pk[c] & 0xFFFFu);
-                int x = k16 >= (unsigned)kKeyInvalid ? INT_MAX : (int)(((k16 >> 7) << kIdxBits) + (unsigned)(t * TN) + (k16 & 127u));
-#pragma unroll
-                for (int cc = 0; cc < K; cc++) {
-                  const int lo = min(wk[cc], x);
-                  x = max(wk[cc], x);
-                  wk[cc] = lo;
-                }
-              }
-          }
-        }
-      }
-      // ---- keyframe finished: this thread holds the complete list of (query row, keyframe) ----
-      int wi[K];
-      float fd[K];
-#pragma unroll
-      for (int c = 0; c < K; c++) {
-        wi[c] = wk[c] == INT_MAX ? -1 : (wk[c] & ((1 << kIdxBits) - 1));
-        wk[c] = wk[c] == INT_MAX ? INT_MAX : (wk[c] >> kIdxBits);
-        fd[c] = (float)wk[c];
-      }
-      if (p.filter) {
-        bool ok = false;
-        if (K >= 2 && valid) {
-          const float dm = fd[0], dn = fd[K >= 2 ? 1 : 0];
-          ok = wi[0] >= 0 && wi[K >= 2 ? 1 : 0] >= 0 && dm <= p.thr && dm < __fmul_rn(p.ratio, dn);
-          const size_t o = (size_t)seg * p.nq + q;
-          p.match_train[o] = ok ? wi[0] : -1;
-          p.match_dist[o] = ok ? dm : FLT_MAX;
-        }
-        const unsigned b = __ballot_sync(0xffffffffu, ok);
-        if (lane == 0 && b) atomicAdd(&p.n_matches[seg], __popc(b));
-      } else if (valid) {
-        const size_t o = ((size_t)seg * p.nq + q) * K;
-#pragma unroll
-        for (int c = 0; c < K; c++) {
-          p.out_idx[o + c] = wi[c];
-          reinterpret_cast<int32_t*>(p.out_dist)[o + c] = wi[c] >= 0 ? wk[c] : INT_MAX;
-        }
-      }
-    }
-  }
-  // ---- teardown ----
-  tc_fence_before();
-  __syncthreads();
-  if (warp == MMA_WARP_X) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, 512;" ::"r"(tmem_base));
   }
 }
 
 template <int K>
 int launch_xt(cvb_ctx* ctx, TcParams p, long total_tiles, cudaStream_t st) {
   p.progress = nullptr;
-  // opt-in (COVINS_B200_TC_PACING=1): at C5 size the standalone request runs at full speed without it (1.77 ms, 5.6 Tpairs/s) and 6 %
-  // slower with it; it is kept for the case the CTAs of a keyframe range do drift out of each other's L2 window
+  // opt-in (COVINS_B200_TC_PACING=1): kept for the case the CTAs of a keyframe range drift out of each other's L2 window
   const char* pace = getenv("COVINS_B200_TC_PACING");
   if (p.nqb > 1 && total_tiles / p.parts > kPaceMinTiles && pace && atoi(pace)) {
     p.progress = (int*)cvb_ws(ctx, WS_XT_PROGRESS, sizeof(int) * (size_t)p.nqb * p.parts);
@@ -1026,27 +875,12 @@ int expand_tiles(cvb_ctx* ctx, const uint8_t* d_rows, const int32_t* d_seg_ptr, 
 template <class M, int K>
 int launch_tc(cvb_ctx* ctx, const TcParams& p, cudaStream_t st) {
   static cvb_once_per_device once;
-  const size_t smem = smem_bytes<M, K>();
+  const size_t smem = smem_bytes<M>();
   if (once.first(ctx->device)) {
     CVB_CUDA(ctx, cudaFuncSetAttribute(tc_scan_kernel<M, K>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   }
   tc_scan_kernel<M, K><<<p.nqb * p.parts, NUM_THREADS, smem, st>>>(p);
   CVB_CHECK_LAUNCH(ctx);
-  if (p.dbg & 16) {
-    static long long h[3][TRACE_TILES][4];
-    CVB_CUDA(ctx, cudaStreamSynchronize(st));
-    CVB_CUDA(ctx, cudaMemcpyFromSymbol(h, g_tc_trace, sizeof(h)));
-    const long long t0 = h[0][0][0];
-    fprintf(stderr, "tile | producer: wait_begin got_slot stored arrived | mma: begin full_ok tempty_ok issued | epilogue: begin tfull_ok done arrived\n");
-    for (int n = 0; n < TRACE_TILES; n++) {
-      fprintf(stderr, "%3d |", n);
-      for (int r = 0; r < 3; r++) {
-        for (int c = 0; c < 4; c++) fprintf(stderr, " %7lld", h[r][n][c] - t0);
-        fprintf(stderr, " |");
-      }
-      fprintf(stderr, "\n");
-    }
-  }
   return CVB_OK;
 }
 

@@ -1,4 +1,4 @@
-// tc_match.cuh — interface of the tcgen05 (tensor-core) matching kernel, see tc_match.cu
+// tc_match.cuh — interface of the wgmma (tensor-core) matching kernel, see tc_match.cu
 #pragma once
 #include <vector>
 

@@ -1,5 +1,5 @@
 /*
- * covins_b200.h — C-ABI of libcovins_b200.so: the B200-native (sm_100a) implementation of the COVINS
+ * covins_b200.h — C-ABI of libcovins_b200.so: the H100-native (sm_90a) implementation of the COVINS
  * server hot path (place-recognition descriptor matching + PGO / global BA).
  *
  * This is the drop-in boundary (SURVEY.md §8b).  The reference has no FFI layer — its seams are C++

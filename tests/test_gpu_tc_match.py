@@ -1,4 +1,4 @@
-"""GPU: the tcgen05 (tensor-core) matching kernel (tc_match.cu) forced on via COVINS_B200_MATCH_KERNEL=tc must be
+"""GPU: the wgmma (tensor-core) matching kernel (tc_match.cu) forced on via COVINS_B200_MATCH_KERNEL=tc must be
 bit-identical to the oracle / golden vectors / the scalar POPC kernel for every mode it serves."""
 import os
 
@@ -67,6 +67,13 @@ def test_tc_ties_and_filter_vs_oracle(ctx, tc):
     mt, md, nm = M.match_candidates_hamming(ctx, q, t, seg, 40.0, 0.8)
     rmt, rmd, rc = ora.ratio_filter(ri, rd.astype(np.float32), 40.0, 0.8)
     assert np.array_equal(mt, rmt) and np.array_equal(nm, rc)
+
+
+def test_tc_expanding_hamming_kernel_ties_and_filter_vs_oracle(ctx, tc, monkeypatch):
+    """the same cases on the Hamming kernel that expands the packed rows itself (tc_scan_kernel) instead of reading
+    resident operand tiles"""
+    monkeypatch.setenv("COVINS_B200_TC_XT", "0")
+    test_tc_ties_and_filter_vs_oracle(ctx, None)
 
 
 def test_tc_l2_vs_oracle(ctx, tc):

@@ -49,7 +49,7 @@ def test_accumulator_is_the_packed_sort_key():
     assert np.array_equal(acc[:, :n_valid], (ham[:, :n_valid] << 7) | col[:, :n_valid])
     assert acc[:, :n_valid].max() <= 32895 < 32896               # kKeyInvalid: every real key is below it
     assert np.all(acc[:, n_valid:] == 127 + 3 * 127 * 128)       # 48895: rows past the end never enter a list
-    assert acc.min() >= 0 and acc.max() < 65536                  # the packed 16-bit TMEM read loses nothing
+    assert acc.min() >= 0 and acc.max() < 65536                  # packing two columns into one 32-bit register loses nothing
     assert ham[5, 2] == 0 and acc[5, 2] == 2                     # a perfect match: key = column only
 
 

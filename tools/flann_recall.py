@@ -1,4 +1,4 @@
-"""SURVEY §8a M2: the reference's SIFT branch calls cv::FlannBasedMatcher (approximate, randomised kd-forest); the B200 path
+"""SURVEY §8a M2: the reference's SIFT branch calls cv::FlannBasedMatcher (approximate, randomised kd-forest); the CUDA path
 computes the EXACT brute-force 2-NN (== cv::BFMatcher(NORM_L2)).  This script reports how much of FLANN's output the exact
 matcher reproduces on SIFT-like synthetic keyframes — as recall of FLANN against the exact result (CPU only, cv2)."""
 import os, sys
