@@ -172,7 +172,6 @@ struct Engine {
   // 3 triangular solves + back-substitution, 4 dogleg / J*step / plus / candidate cost
   cudaEvent_t ev[8] = {};
   cvb_chol::FactorStreams fs;            // lookahead / chain streams of the factorisation
-  std::vector<cudaEvent_t> la_ev;
   cudaGraphExec_t g_factor = nullptr, g_solve = nullptr;   // the ~700 / ~480 launches of one factorisation / solve, captured once
   int n_factor_calls = 0, n_solve_calls = 0;
   double phase_ms[5] = {0, 0, 0, 0, 0};
@@ -217,13 +216,7 @@ struct Engine {
     if (h_scalars) cudaFreeHost(h_scalars);
     lap("pinned scalars");
     for (auto& e : ev) if (e) cudaEventDestroy(e);
-    for (auto& e : la_ev) if (e) cudaEventDestroy(e);
-    if (fs.bulk) cudaStreamDestroy(fs.bulk);
-    if (fs.fast) cudaStreamDestroy(fs.fast);
-    for (int g = 0; g < 8; g++) { if (fs.group_aux[g]) cudaStreamDestroy(fs.group_aux[g]); if (fs.join_aux[g]) cudaEventDestroy(fs.join_aux[g]); }
-    if (fs.fork_fast) cudaEventDestroy(fs.fork_fast);
-    for (int g = 0; g < fs.n_group; g++) { if (fs.group[g]) cudaStreamDestroy(fs.group[g]); if (fs.join[g]) cudaEventDestroy(fs.join[g]); }
-    if (fs.fork) cudaEventDestroy(fs.fork);
+    fs.destroy();
     lap("events, streams");
     if (g_factor) cudaGraphExecDestroy(g_factor);
     if (g_solve) cudaGraphExecDestroy(g_solve);
@@ -1311,7 +1304,7 @@ int engine_setup(Engine& E, const cvb_ba_problem* p, const cvb_ba_options* o) {
     for (int k = 0; k < K; k++)
       if (comp_size[find(k)] < 2) { E.h_off_pose[k] = cursor; cursor += 6; }
     n_total = cursor;
-  } else if (E.L_in == 0 && p->n_edge > 0 && !getenv("COVINS_B200_PGO_PLAIN_ORDER")) {
+  } else if (E.L_in == 0 && p->n_edge > 0) {
     // Pose graph (PoseGraphOptimization: no landmarks, only between-factors): the keyframes of one agent form a banded chain
     // (successor + 5 predecessor edges, optimization_be.cpp:947-1021) and the few loop edges couple distant keyframes.  In
     // plain keyframe order the tile columns are one long dependent chain (94 columns x ~100 us at C3).  Nested dissection
@@ -1627,31 +1620,7 @@ int engine_setup(Engine& E, const cvb_ba_problem* p, const cvb_ba_options* o) {
     return rc;
   ENG_CUDA(cudaMallocHost(&E.h_scalars, RED_SLOTS * sizeof(double)));
   for (auto& e : E.ev) ENG_CUDA(cudaEventCreate(&e));
-  {
-    int lo = 0, hi = 0;   // lo = numerically greatest = lowest priority
-    cudaDeviceGetStreamPriorityRange(&lo, &hi);
-    ENG_CUDA(cudaStreamCreateWithPriority(&E.fs.bulk, cudaStreamNonBlocking, lo));
-    E.la_ev.assign((size_t)5 * E.plan.nt, nullptr);
-    for (auto& e : E.la_ev) ENG_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-    E.fs.ev = E.la_ev.data();
-    // the critical-chain streams (cholesky.cu: "chain column"); COVINS_B200_CHAIN_STREAM=0 → the plain depth-1 lookahead
-    const char* cs = getenv("COVINS_B200_CHAIN_STREAM");
-    if (!getenv("COVINS_B200_NO_CHAIN_STREAM") && !(cs && !atoi(cs))) {
-      ENG_CUDA(cudaStreamCreateWithPriority(&E.fs.fast, cudaStreamNonBlocking, hi));
-      ENG_CUDA(cudaEventCreateWithFlags(&E.fs.fork_fast, cudaEventDisableTiming));
-      if (!getenv("COVINS_B200_NO_GROUP_CHAIN"))
-        for (int g = 0; g < 8; g++) {
-          ENG_CUDA(cudaStreamCreateWithPriority(&E.fs.group_aux[g], cudaStreamNonBlocking, hi));
-          ENG_CUDA(cudaEventCreateWithFlags(&E.fs.join_aux[g], cudaEventDisableTiming));
-        }
-    }
-    E.fs.n_group = 8;
-    for (int g = 0; g < 8; g++) {
-      ENG_CUDA(cudaStreamCreateWithPriority(&E.fs.group[g], cudaStreamNonBlocking, hi));
-      ENG_CUDA(cudaEventCreateWithFlags(&E.fs.join[g], cudaEventDisableTiming));
-    }
-    ENG_CUDA(cudaEventCreateWithFlags(&E.fs.fork, cudaEventDisableTiming));
-  }
+  if ((rc = E.fs.create(E.ctx, E.plan.nt))) return rc;
   ENG_CUDA(cudaStreamSynchronize(E.st));
   lap("vectors, S, streams (sync)");
   return CVB_OK;
@@ -1776,7 +1745,7 @@ int factor_rcs(Engine& E, double mu, bool* ok) {
   } else if (E.n_factor_calls == 1) {
     cudaGraph_t g = nullptr;
     ENG_CUDA(cudaStreamBeginCapture(E.st, cudaStreamCaptureModeThreadLocal));
-    rc = cvb_chol::factor(E.ctx, E.S.p, E.linv.p, E.flag.p, E.plan, E.st, &E.fs, dist ? &E.dv : nullptr);
+    rc = cvb_chol::factor(E.ctx, E.S.p, E.linv.p, E.flag.p, E.plan, E.st, E.fs, dist ? &E.dv : nullptr);
     cudaError_t ce = cudaStreamEndCapture(E.st, &g);
     if (rc) return rc;
     if (ce != cudaSuccess) return cvb_fail(E.ctx, CVB_ERR_CUDA, "graph capture of the factorisation failed: %s", cudaGetErrorString(ce));
@@ -1784,7 +1753,7 @@ int factor_rcs(Engine& E, double mu, bool* ok) {
     cudaGraphDestroy(g);
     ENG_CUDA(cudaGraphLaunch(E.g_factor, E.st));
   } else {
-    rc = cvb_chol::factor(E.ctx, E.S.p, E.linv.p, E.flag.p, E.plan, E.st, &E.fs, dist ? &E.dv : nullptr);
+    rc = cvb_chol::factor(E.ctx, E.S.p, E.linv.p, E.flag.p, E.plan, E.st, E.fs, dist ? &E.dv : nullptr);
     if (rc) return rc;
   }
   E.n_factor_calls++;
@@ -1899,7 +1868,7 @@ int prepare_step(Engine& E, bool* solver_ok, bool* grad_converged) {
     } else if (E.n_solve_calls == 1) {
       cudaGraph_t g = nullptr;
       ENG_CUDA(cudaStreamBeginCapture(E.st, cudaStreamCaptureModeThreadLocal));
-      rc = cvb_chol::solve(E.ctx, E.S.p, E.linv.p, E.gs.p, E.tmp.p, E.xsol.p, E.plan, E.st, &E.fs);
+      rc = cvb_chol::solve(E.ctx, E.S.p, E.linv.p, E.gs.p, E.tmp.p, E.xsol.p, E.plan, E.st, E.fs);
       cudaError_t ce = cudaStreamEndCapture(E.st, &g);
       if (rc) return rc;
       if (ce != cudaSuccess) return cvb_fail(E.ctx, CVB_ERR_CUDA, "graph capture of the solve failed: %s", cudaGetErrorString(ce));
@@ -1907,7 +1876,7 @@ int prepare_step(Engine& E, bool* solver_ok, bool* grad_converged) {
       cudaGraphDestroy(g);
       ENG_CUDA(cudaGraphLaunch(E.g_solve, E.st));
     } else {
-      if ((rc = cvb_chol::solve(E.ctx, E.S.p, E.linv.p, E.gs.p, E.tmp.p, E.xsol.p, E.plan, E.st, &E.fs))) return rc;
+      if ((rc = cvb_chol::solve(E.ctx, E.S.p, E.linv.p, E.gs.p, E.tmp.p, E.xsol.p, E.plan, E.st, E.fs))) return rc;
     }
     E.n_solve_calls++;
     if (E.L_in > 0) {

@@ -626,6 +626,45 @@ void TilePlan::release() {
   d_row_idx = d_pair_i = d_pair_j = d_rowc_idx = d_tile_of = nullptr;
 }
 
+int FactorStreams::create(cvb_ctx* ctx, int nt) {
+  int lo = 0, hi = 0;   // lo = numerically greatest = lowest priority
+  cudaDeviceGetStreamPriorityRange(&lo, &hi);
+  CVB_CUDA(ctx, cudaStreamCreateWithPriority(&bulk, cudaStreamNonBlocking, lo));
+  ev.assign((size_t)5 * nt, nullptr);
+  for (auto& e : ev) CVB_CUDA(ctx, cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+  CVB_CUDA(ctx, cudaStreamCreateWithPriority(&fast, cudaStreamNonBlocking, hi));
+  CVB_CUDA(ctx, cudaEventCreateWithFlags(&fork_fast, cudaEventDisableTiming));
+  for (int g = 0; g < n_group; g++) {
+    CVB_CUDA(ctx, cudaStreamCreateWithPriority(&group_aux[g], cudaStreamNonBlocking, hi));
+    CVB_CUDA(ctx, cudaEventCreateWithFlags(&join_aux[g], cudaEventDisableTiming));
+  }
+  for (int g = 0; g < n_group; g++) {
+    CVB_CUDA(ctx, cudaStreamCreateWithPriority(&group[g], cudaStreamNonBlocking, hi));
+    CVB_CUDA(ctx, cudaEventCreateWithFlags(&join[g], cudaEventDisableTiming));
+  }
+  CVB_CUDA(ctx, cudaEventCreateWithFlags(&fork, cudaEventDisableTiming));
+  return CVB_OK;
+}
+
+void FactorStreams::destroy() {
+  for (auto& e : ev) if (e) cudaEventDestroy(e);
+  ev.clear();
+  if (bulk) cudaStreamDestroy(bulk);
+  if (fast) cudaStreamDestroy(fast);
+  if (fork_fast) cudaEventDestroy(fork_fast);
+  for (int g = 0; g < n_group; g++) {
+    if (group_aux[g]) cudaStreamDestroy(group_aux[g]);
+    if (join_aux[g]) cudaEventDestroy(join_aux[g]);
+    if (group[g]) cudaStreamDestroy(group[g]);
+    if (join[g]) cudaEventDestroy(join[g]);
+    group_aux[g] = group[g] = nullptr;
+    join_aux[g] = join[g] = nullptr;
+  }
+  if (fork) cudaEventDestroy(fork);
+  bulk = fast = nullptr;
+  fork_fast = fork = nullptr;
+}
+
 // ---- cross-GPU hand-over of a finished panel (distributed factorisation) -------------------------------------------
 __device__ __forceinline__ int ld_acquire_sys(const int* p) {
   int v;
@@ -660,7 +699,7 @@ __global__ void wait_panel_kernel(const int* __restrict__ flag, const int* __res
 }
 
 int factor(cvb_ctx* ctx, double* S, double* linv, int* d_flag, const TilePlan& plan, cudaStream_t st,
-           const FactorStreams* fs, const DistView* dv) {
+           const FactorStreams& fs, const DistView* dv) {
   static cvb_once_per_device once;
   if (once.first(ctx->device)) {
     CVB_CUDA(ctx, cudaFuncSetAttribute(trsm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kTrsmSmem));
@@ -672,21 +711,21 @@ int factor(cvb_ctx* ctx, double* S, double* linv, int* d_flag, const TilePlan& p
   const int nt = plan.nt;
   const bool dist = dv != nullptr && dv->world > 1 && !plan.h_owner.empty();
   CVB_REQUIRE(ctx, plan.d_tile_of != nullptr && (int)plan.h_col_base.size() == nt, "tile plan not built / uploaded");
+  CVB_REQUIRE(ctx, fs.ev.size() >= (size_t)5 * nt, "factor streams not created for this plan");
   CVB_CUDA(ctx, cudaMemsetAsync(d_flag, 0, sizeof(int), st));
   if (dist) {
     bump_epoch_kernel<<<1, 1, 0, st>>>(dv->d_epoch);
     CVB_CHECK_LAUNCH(ctx);
   }
-  cudaStream_t st2 = fs ? fs->bulk : nullptr;
-  cudaEvent_t* ev = fs ? fs->ev : nullptr;
-  const int n_gs = (fs && !plan.h_col_group.empty()) ? fs->n_group : 0;
-  // Lookahead (depth 1) when a second stream is given: the diagonal-tile kernel and the panel solve of step k+1 only
-  // need the "panel" part of step k's trailing update (pairs in tile column k+1); the bulk of the update runs on the
-  // second (low-priority) stream concurrently.  ev[2k] = panel of step k available, ev[2k+1] = bulk update done.
+  cudaStream_t st2 = fs.bulk;
+  const std::vector<cudaEvent_t>& ev = fs.ev;
+  const int n_gs = plan.h_col_group.empty() ? 0 : fs.n_group;
+  // Lookahead (depth 1): the diagonal-tile kernel and the panel solve of step k+1 only need the "panel" part of step k's
+  // trailing update (pairs in tile column k+1); the bulk of the update runs on the second (low-priority) stream
+  // concurrently.  ev[5k] = panel of step k available, ev[5k+1] = bulk update done.
   // Independent column groups (the IMU chains of different agents, see TilePlan::h_col_group) run on their own
   // streams: their tile columns are pure latency chains (diagonal tile → panel → tiny update) that do not share tiles.
   // Distributed: "panel available" = factored here (owner) or pulled from the owner's memory (everyone else).
-  const bool la = st2 != nullptr && ev != nullptr;
   // Development trace (COVINS_B200_FACTOR_TRACE=<csv path>): per-column timeline of the first non-captured call.
   static bool traced = false;
   const char* trace_path = getenv("COVINS_B200_FACTOR_TRACE");
@@ -703,29 +742,26 @@ int factor(cvb_ctx* ctx, double* S, double* linv, int* d_flag, const TilePlan& p
   int last_bulk = -1;
   bool forked = false;
   std::vector<char> used(n_gs > 0 ? n_gs : 1, 0);
-  // Critical-chain stream (fs->fast, highest priority).  Step k+1's diagonal tile needs from step k only ONE tile of the
+  // Critical-chain stream (fs.fast, highest priority).  Step k+1's diagonal tile needs from step k only ONE tile of the
   // panel, L(k+1,k), and ONE update, S(k+1,k+1) -= L(k+1,k) L(k+1,k)^T.  So the chain
   //     potrf(k) -> solve tile (k+1,k) -> update tile (k+1,k+1) -> potrf(k+1) -> ...
   // runs on its own stream while the rest of panel k (main stream) and the rest of its updates (main: tile column k+1,
   // bulk stream: everything else) proceed beside it.  Distributed, the hand-over to the next column's owner moves one
   // 128 KB tile (flag A) instead of waiting for the whole panel (flag B).
-  cudaStream_t sf = (la && fs->fast) ? fs->fast : nullptr;
+  cudaStream_t sf = fs.fast;
   bool sf_live = false;          // sf has been forked off the main stream
   int prev_chain = -1;           // previous column handled by the chain (its evA is what step C waits for)
   // The column groups (IMU chains) are pure chains: the same split with the group's stream as the chain stream and a second
   // stream per group for the rest of the panel and all of its (small) updates.
-  const bool grp_chain = sf != nullptr && n_gs > 0 && fs->group_aux[0] != nullptr;
-  int prev_chain_g[8] = {-1, -1, -1, -1, -1, -1, -1, -1};
+  int prev_chain_g[FactorStreams::n_group] = {-1, -1, -1, -1, -1, -1, -1, -1};
   int rc_join = 0;
   auto join_groups = [&]() -> int {
     for (int g = 0; g < n_gs; g++)
       if (used[g]) {
-        if (grp_chain) {
-          CVB_CUDA(ctx, cudaEventRecord(fs->join_aux[g], fs->group_aux[g]));
-          CVB_CUDA(ctx, cudaStreamWaitEvent(fs->group[g], fs->join_aux[g], 0));
-        }
-        CVB_CUDA(ctx, cudaEventRecord(fs->join[g], fs->group[g]));
-        CVB_CUDA(ctx, cudaStreamWaitEvent(st, fs->join[g], 0));
+        CVB_CUDA(ctx, cudaEventRecord(fs.join_aux[g], fs.group_aux[g]));
+        CVB_CUDA(ctx, cudaStreamWaitEvent(fs.group[g], fs.join_aux[g], 0));
+        CVB_CUDA(ctx, cudaEventRecord(fs.join[g], fs.group[g]));
+        CVB_CUDA(ctx, cudaStreamWaitEvent(st, fs.join[g], 0));
         used[g] = 0;
       }
     return CVB_OK;
@@ -735,13 +771,13 @@ int factor(cvb_ctx* ctx, double* S, double* linv, int* d_flag, const TilePlan& p
     cudaStream_t s = st;
     if (grp >= 0) {
       if (!forked) {
-        CVB_CUDA(ctx, cudaEventRecord(fs->fork, st));
+        CVB_CUDA(ctx, cudaEventRecord(fs.fork, st));
         forked = true;
       }
-      s = fs->group[grp % n_gs];
+      s = fs.group[grp % n_gs];
       if (!used[grp % n_gs]) {
-        CVB_CUDA(ctx, cudaStreamWaitEvent(s, fs->fork, 0));
-        if (grp_chain) CVB_CUDA(ctx, cudaStreamWaitEvent(fs->group_aux[grp % n_gs], fs->fork, 0));
+        CVB_CUDA(ctx, cudaStreamWaitEvent(s, fs.fork, 0));
+        CVB_CUDA(ctx, cudaStreamWaitEvent(fs.group_aux[grp % n_gs], fs.fork, 0));
         used[grp % n_gs] = 1;
       }
     } else if (forked) {   // first column after the grouped ones: join
@@ -754,162 +790,114 @@ int factor(cvb_ctx* ctx, double* S, double* linv, int* d_flag, const TilePlan& p
     double* linv_k = linv + (size_t)k * TT;
     const bool mine = !dist || plan.h_owner[k] == dv->rank;
     const int p0 = plan.h_pair_ptr[k], np = plan.h_pair_ptr[k + 1] - p0;
-    if (sf && (grp < 0 || grp_chain)) {
-      // ------------------------------------ chain column ------------------------------------
-      cudaEvent_t evPanel = ev[5 * k], evBulk = ev[5 * k + 1], evP = ev[5 * k + 2], evD = ev[5 * k + 3], evA = ev[5 * k + 4];
-      const bool is_grp = grp >= 0;
-      const int gi = is_grp ? grp % n_gs : 0;
-      if (!is_grp && !sf_live) {   // everything before this column (column groups, plain columns) is on the main stream
-        CVB_CUDA(ctx, cudaEventRecord(fs->fork_fast, st));
-        CVB_CUDA(ctx, cudaStreamWaitEvent(sf, fs->fork_fast, 0));
-        sf_live = true;
-      }
-      cudaStream_t cs = is_grp ? fs->group[gi] : sf;        // chain stream of this column
-      cudaStream_t ws = is_grp ? fs->group_aux[gi] : st;    // its work stream (rest of the panel, tile column k+1)
-      int& pc = is_grp ? prev_chain_g[gi] : prev_chain;     // previous chain column of this sequence
-      const int lb = is_grp ? -1 : last_bulk;               // column groups have no bulk stream: all their updates are small
-      const bool has_next = m > 0 && plan.h_row_idx[plan.h_col_ptr[k]] == k + 1;
-      const bool mine_n = has_next && (!dist || plan.h_owner[k + 1] == dv->rank);
-      // does the pair list start with the diagonal pair (k+1, k+1)?  (owner-filtered lists hold it only when column k+1 is ours)
-      const int na = is_grp ? np : plan.h_pair_split[k];
-      const bool diag_pair = has_next && np > 0 && plan.h_pair_i[p0] == k + 1 && plan.h_pair_j[p0] == k + 1;
-      // A. tile (k,k) is final: column k-1's contribution came with the chain, the bulk updates of the columns <= k-2 were
-      //    waited for by the previous chain step (below) — nothing to wait for here
-      if (mine) {
-        potrf_inv_kernel<<<1, POTRF_THREADS, kPotrfSmem, cs>>>(diag, (size_t)T, 0, linv_k, d_flag, nullptr, 0);
-        CVB_CHECK_LAUNCH(ctx);
-      }
-      CVB_CUDA(ctx, cudaEventRecord(evP, cs));
-      if (tr) cudaEventRecord(tev[(size_t)k * 5 + 1], cs);
-      // C. tile (k+1,k): final once column k-1's updates of tile column k are done (evA of the previous chain column)
-      if (has_next) {
-        if (pc >= 0) CVB_CUDA(ctx, cudaStreamWaitEvent(cs, ev[5 * pc + 4], 0));
-        if (mine) {
-          chain_gemm_kernel<0><<<T / CHAIN_ROWS, T, kChainSmem, cs>>>(diag + TT, diag + TT, linv_k);
-          CVB_CHECK_LAUNCH(ctx);
-          if (dist && !is_grp) {     // (a column group stays on one rank: nobody waits for its flag A)
-            signal_panel_kernel<<<1, 32, 0, cs>>>(dv->d_peer_flag, k, dv->d_epoch, dv->world, dv->rank);          // flag A
-            CVB_CHECK_LAUNCH(ctx);
-          }
-        } else if (mine_n) {
-          wait_panel_kernel<<<1, 1, 0, cs>>>(dv->peer_flag[dv->rank] + k, dv->d_epoch, d_flag);
-          CVB_CHECK_LAUNCH(ctx);
-          CVB_CUDA(ctx, cudaMemcpyAsync(diag + TT, dv->peer_S[plan.h_owner[k]] + ((size_t)plan.h_col_base[k] + 1) * TT, TT * sizeof(double),
-                                        cudaMemcpyDeviceToDevice, cs));
-        }
-      }
-      // the bulk update of the previous column also writes tile (k+1,k+1) (and everything the next chain step reads): it has
-      // to be complete before the diagonal pair is applied / before potrf(k+1) — the depth-1 lookahead rule
-      if (lb >= 0) CVB_CUDA(ctx, cudaStreamWaitEvent(cs, ev[5 * lb + 1], 0));
-      if (diag_pair) {
-        chain_gemm_kernel<1><<<T / CHAIN_ROWS, T, kChainSmem, cs>>>(S + (size_t)plan.h_col_base[k + 1] * TT, diag + TT, diag + TT);
-        CVB_CHECK_LAUNCH(ctx);
-      }
-      CVB_CUDA(ctx, cudaEventRecord(evD, cs));
-      if (tr) cudaEventRecord(tev[(size_t)k * 5 + 2], cs);
-      // D. the rest of the panel on the work stream
-      const bool early_tile = has_next && (mine || mine_n);     // tile (k+1,k) was produced / fetched by the chain
-      if (mine) {
-        CVB_CUDA(ctx, cudaStreamWaitEvent(ws, evP, 0));
-        const int first = has_next ? 1 : 0;
-        if (m - first > 0) {
-          trsm_kernel<<<2 * (m - first), TRSM_THREADS, kTrsmSmem, ws>>>(diag + (size_t)(1 + first) * TT, linv_k);
-          CVB_CHECK_LAUNCH(ctx);
-        }
-        CVB_CUDA(ctx, cudaStreamWaitEvent(ws, evD, 0));
-        if (dist) {
-          signal_panel_kernel<<<1, 32, 0, ws>>>(dv->d_peer_flag, nt + k, dv->d_epoch, dv->world, dv->rank);       // flag B
-          CVB_CHECK_LAUNCH(ctx);
-        }
-      } else {
-        const int o = plan.h_owner[k];
-        wait_panel_kernel<<<1, 1, 0, ws>>>(dv->peer_flag[dv->rank] + nt + k, dv->d_epoch, d_flag);
-        CVB_CHECK_LAUNCH(ctx);
-        const double* src = dv->peer_S[o] + (size_t)plan.h_col_base[k] * TT;
-        if (early_tile) {   // the chain owns tile (k+1,k): copy around it
-          CVB_CUDA(ctx, cudaMemcpyAsync(diag, src, TT * sizeof(double), cudaMemcpyDeviceToDevice, ws));
-          if (m > 1) CVB_CUDA(ctx, cudaMemcpyAsync(diag + 2 * (size_t)TT, src + 2 * (size_t)TT, (size_t)(m - 1) * TT * sizeof(double), cudaMemcpyDeviceToDevice, ws));
-        } else {
-          CVB_CUDA(ctx, cudaMemcpyAsync(diag, src, (size_t)(1 + m) * TT * sizeof(double), cudaMemcpyDeviceToDevice, ws));
-        }
-        CVB_CUDA(ctx, cudaMemcpyAsync(linv_k, dv->peer_linv[o] + (size_t)k * TT, TT * sizeof(double), cudaMemcpyDeviceToDevice, ws));
-        CVB_CUDA(ctx, cudaStreamWaitEvent(ws, evD, 0));
-      }
-      // E. tile column k+1 (minus the diagonal pair), then "panel k available" for the bulk stream
-      if (m > 0) {
-        CVB_CUDA(ctx, cudaEventRecord(evPanel, ws));
-        if (lb >= 0) CVB_CUDA(ctx, cudaStreamWaitEvent(ws, ev[5 * lb + 1], 0));
-        const int a0 = diag_pair ? 1 : 0;
-        if (na - a0 > 0) {
-          syrk_kernel<<<4 * (na - a0), SYRK_THREADS, kSyrkSmem, ws>>>(S, plan.d_tile_of, nt, k, plan.d_pair_i + p0 + a0, plan.d_pair_j + p0 + a0);
-          CVB_CHECK_LAUNCH(ctx);
-        }
-        if (tr) cudaEventRecord(tev[(size_t)k * 5 + 3], ws);
-        if (np - na > 0) {
-          CVB_CUDA(ctx, cudaStreamWaitEvent(st2, evPanel, 0));
-          syrk_kernel<<<4 * (np - na), SYRK_THREADS, kSyrkSmem, st2>>>(S, plan.d_tile_of, nt, k, plan.d_pair_i + p0 + na, plan.d_pair_j + p0 + na);
-          CVB_CHECK_LAUNCH(ctx);
-          CVB_CUDA(ctx, cudaEventRecord(evBulk, st2));
-          if (tr) cudaEventRecord(tev[(size_t)k * 5 + 4], st2);
-          last_bulk = k;
-        }
-      }
-      CVB_CUDA(ctx, cudaEventRecord(evA, ws));
-      pc = k;
-      continue;
+    // ------------------------------------ chain column ------------------------------------
+    cudaEvent_t evPanel = ev[5 * k], evBulk = ev[5 * k + 1], evP = ev[5 * k + 2], evD = ev[5 * k + 3], evA = ev[5 * k + 4];
+    const bool is_grp = grp >= 0;
+    const int gi = is_grp ? grp % n_gs : 0;
+    if (!is_grp && !sf_live) {   // everything before this column (the column groups) is on the main stream
+      CVB_CUDA(ctx, cudaEventRecord(fs.fork_fast, st));
+      CVB_CUDA(ctx, cudaStreamWaitEvent(sf, fs.fork_fast, 0));
+      sf_live = true;
     }
+    cudaStream_t cs = is_grp ? fs.group[gi] : sf;        // chain stream of this column
+    cudaStream_t ws = is_grp ? fs.group_aux[gi] : st;    // its work stream (rest of the panel, tile column k+1)
+    int& pc = is_grp ? prev_chain_g[gi] : prev_chain;     // previous chain column of this sequence
+    const int lb = is_grp ? -1 : last_bulk;               // column groups have no bulk stream: all their updates are small
+    const bool has_next = m > 0 && plan.h_row_idx[plan.h_col_ptr[k]] == k + 1;
+    const bool mine_n = has_next && (!dist || plan.h_owner[k + 1] == dv->rank);
+    // does the pair list start with the diagonal pair (k+1, k+1)?  (owner-filtered lists hold it only when column k+1 is ours)
+    const int na = is_grp ? np : plan.h_pair_split[k];
+    const bool diag_pair = has_next && np > 0 && plan.h_pair_i[p0] == k + 1 && plan.h_pair_j[p0] == k + 1;
+    // A. tile (k,k) is final: column k-1's contribution came with the chain, the bulk updates of the columns <= k-2 were
+    //    waited for by the previous chain step (below) — nothing to wait for here
     if (mine) {
-      potrf_inv_kernel<<<1, POTRF_THREADS, kPotrfSmem, s>>>(diag, (size_t)T, 0, linv_k, d_flag, nullptr, 0);
+      potrf_inv_kernel<<<1, POTRF_THREADS, kPotrfSmem, cs>>>(diag, (size_t)T, 0, linv_k, d_flag, nullptr, 0);
       CVB_CHECK_LAUNCH(ctx);
-      if (tr) cudaEventRecord(tev[(size_t)k * 5 + 1], s);
-      if (m > 0) {
-        trsm_kernel<<<2 * m, TRSM_THREADS, kTrsmSmem, s>>>(diag + TT, linv_k);
+    }
+    CVB_CUDA(ctx, cudaEventRecord(evP, cs));
+    if (tr) cudaEventRecord(tev[(size_t)k * 5 + 1], cs);
+    // C. tile (k+1,k): final once column k-1's updates of tile column k are done (evA of the previous chain column)
+    if (has_next) {
+      if (pc >= 0) CVB_CUDA(ctx, cudaStreamWaitEvent(cs, ev[5 * pc + 4], 0));
+      if (mine) {
+        chain_gemm_kernel<0><<<T / CHAIN_ROWS, T, kChainSmem, cs>>>(diag + TT, diag + TT, linv_k);
+        CVB_CHECK_LAUNCH(ctx);
+        if (dist && !is_grp) {     // (a column group stays on one rank: nobody waits for its flag A)
+          signal_panel_kernel<<<1, 32, 0, cs>>>(dv->d_peer_flag, k, dv->d_epoch, dv->world, dv->rank);          // flag A
+          CVB_CHECK_LAUNCH(ctx);
+        }
+      } else if (mine_n) {
+        wait_panel_kernel<<<1, 1, 0, cs>>>(dv->peer_flag[dv->rank] + k, dv->d_epoch, d_flag);
+        CVB_CHECK_LAUNCH(ctx);
+        CVB_CUDA(ctx, cudaMemcpyAsync(diag + TT, dv->peer_S[plan.h_owner[k]] + ((size_t)plan.h_col_base[k] + 1) * TT, TT * sizeof(double),
+                                      cudaMemcpyDeviceToDevice, cs));
+      }
+    }
+    // the bulk update of the previous column also writes tile (k+1,k+1) (and everything the next chain step reads): it has
+    // to be complete before the diagonal pair is applied / before potrf(k+1) — the depth-1 lookahead rule
+    if (lb >= 0) CVB_CUDA(ctx, cudaStreamWaitEvent(cs, ev[5 * lb + 1], 0));
+    if (diag_pair) {
+      chain_gemm_kernel<1><<<T / CHAIN_ROWS, T, kChainSmem, cs>>>(S + (size_t)plan.h_col_base[k + 1] * TT, diag + TT, diag + TT);
+      CVB_CHECK_LAUNCH(ctx);
+    }
+    CVB_CUDA(ctx, cudaEventRecord(evD, cs));
+    if (tr) cudaEventRecord(tev[(size_t)k * 5 + 2], cs);
+    // D. the rest of the panel on the work stream
+    const bool early_tile = has_next && (mine || mine_n);     // tile (k+1,k) was produced / fetched by the chain
+    if (mine) {
+      CVB_CUDA(ctx, cudaStreamWaitEvent(ws, evP, 0));
+      const int first = has_next ? 1 : 0;
+      if (m - first > 0) {
+        trsm_kernel<<<2 * (m - first), TRSM_THREADS, kTrsmSmem, ws>>>(diag + (size_t)(1 + first) * TT, linv_k);
         CVB_CHECK_LAUNCH(ctx);
       }
+      CVB_CUDA(ctx, cudaStreamWaitEvent(ws, evD, 0));
       if (dist) {
-        signal_panel_kernel<<<1, 32, 0, s>>>(dv->d_peer_flag, nt + k, dv->d_epoch, dv->world, dv->rank);
+        signal_panel_kernel<<<1, 32, 0, ws>>>(dv->d_peer_flag, nt + k, dv->d_epoch, dv->world, dv->rank);       // flag B
         CVB_CHECK_LAUNCH(ctx);
       }
     } else {
       const int o = plan.h_owner[k];
-      wait_panel_kernel<<<1, 1, 0, s>>>(dv->peer_flag[dv->rank] + nt + k, dv->d_epoch, d_flag);
+      wait_panel_kernel<<<1, 1, 0, ws>>>(dv->peer_flag[dv->rank] + nt + k, dv->d_epoch, d_flag);
       CVB_CHECK_LAUNCH(ctx);
-      // the column's tiles are contiguous and sit at the same packed offset on every rank: one NVLink copy each
-      CVB_CUDA(ctx, cudaMemcpyAsync(diag, dv->peer_S[o] + (size_t)plan.h_col_base[k] * TT, (size_t)(1 + m) * TT * sizeof(double),
-                                    cudaMemcpyDeviceToDevice, s));
-      CVB_CUDA(ctx, cudaMemcpyAsync(linv_k, dv->peer_linv[o] + (size_t)k * TT, TT * sizeof(double), cudaMemcpyDeviceToDevice, s));
-      if (tr) cudaEventRecord(tev[(size_t)k * 5 + 1], s);
+      const double* src = dv->peer_S[o] + (size_t)plan.h_col_base[k] * TT;
+      if (early_tile) {   // the chain owns tile (k+1,k): copy around it
+        CVB_CUDA(ctx, cudaMemcpyAsync(diag, src, TT * sizeof(double), cudaMemcpyDeviceToDevice, ws));
+        if (m > 1) CVB_CUDA(ctx, cudaMemcpyAsync(diag + 2 * (size_t)TT, src + 2 * (size_t)TT, (size_t)(m - 1) * TT * sizeof(double), cudaMemcpyDeviceToDevice, ws));
+      } else {
+        CVB_CUDA(ctx, cudaMemcpyAsync(diag, src, (size_t)(1 + m) * TT * sizeof(double), cudaMemcpyDeviceToDevice, ws));
+      }
+      CVB_CUDA(ctx, cudaMemcpyAsync(linv_k, dv->peer_linv[o] + (size_t)k * TT, TT * sizeof(double), cudaMemcpyDeviceToDevice, ws));
+      CVB_CUDA(ctx, cudaStreamWaitEvent(ws, evD, 0));
     }
+    // E. tile column k+1 (minus the diagonal pair), then "panel k available" for the bulk stream
     if (m > 0) {
-      if (tr) cudaEventRecord(tev[(size_t)k * 5 + 2], s);
-      const bool la_k = la && grp < 0;
-      const int na = la_k ? plan.h_pair_split[k] : np;
-      if (la_k) {
-        CVB_CUDA(ctx, cudaEventRecord(ev[5 * k], s));
-        if (last_bulk >= 0) CVB_CUDA(ctx, cudaStreamWaitEvent(s, ev[5 * last_bulk + 1], 0));
-      }
-      if (na > 0) {
-        syrk_kernel<<<4 * na, SYRK_THREADS, kSyrkSmem, s>>>(S, plan.d_tile_of, nt, k, plan.d_pair_i + p0, plan.d_pair_j + p0);
+      CVB_CUDA(ctx, cudaEventRecord(evPanel, ws));
+      if (lb >= 0) CVB_CUDA(ctx, cudaStreamWaitEvent(ws, ev[5 * lb + 1], 0));
+      const int a0 = diag_pair ? 1 : 0;
+      if (na - a0 > 0) {
+        syrk_kernel<<<4 * (na - a0), SYRK_THREADS, kSyrkSmem, ws>>>(S, plan.d_tile_of, nt, k, plan.d_pair_i + p0 + a0, plan.d_pair_j + p0 + a0);
         CVB_CHECK_LAUNCH(ctx);
       }
-      if (tr) cudaEventRecord(tev[(size_t)k * 5 + 3], s);
-      if (la_k && np - na > 0) {
-        CVB_CUDA(ctx, cudaStreamWaitEvent(st2, ev[5 * k], 0));
-        syrk_kernel<<<4 * (np - na), SYRK_THREADS, kSyrkSmem, st2>>>(S, plan.d_tile_of, nt, k, plan.d_pair_i + p0 + na,
-                                                                     plan.d_pair_j + p0 + na);
+      if (tr) cudaEventRecord(tev[(size_t)k * 5 + 3], ws);
+      if (np - na > 0) {
+        CVB_CUDA(ctx, cudaStreamWaitEvent(st2, evPanel, 0));
+        syrk_kernel<<<4 * (np - na), SYRK_THREADS, kSyrkSmem, st2>>>(S, plan.d_tile_of, nt, k, plan.d_pair_i + p0 + na, plan.d_pair_j + p0 + na);
         CVB_CHECK_LAUNCH(ctx);
-        CVB_CUDA(ctx, cudaEventRecord(ev[5 * k + 1], st2));
+        CVB_CUDA(ctx, cudaEventRecord(evBulk, st2));
         if (tr) cudaEventRecord(tev[(size_t)k * 5 + 4], st2);
         last_bulk = k;
       }
     }
+    CVB_CUDA(ctx, cudaEventRecord(evA, ws));
+    pc = k;
   }
   if (sf_live) {   // join the chain stream
-    CVB_CUDA(ctx, cudaEventRecord(fs->fork_fast, sf));
-    CVB_CUDA(ctx, cudaStreamWaitEvent(st, fs->fork_fast, 0));
+    CVB_CUDA(ctx, cudaEventRecord(fs.fork_fast, sf));
+    CVB_CUDA(ctx, cudaStreamWaitEvent(st, fs.fork_fast, 0));
   }
   if (forked && (rc_join = join_groups())) return rc_join;
-  if (la && last_bulk >= 0) CVB_CUDA(ctx, cudaStreamWaitEvent(st, ev[5 * last_bulk + 1], 0));   // join
+  if (last_bulk >= 0) CVB_CUDA(ctx, cudaStreamWaitEvent(st, ev[5 * last_bulk + 1], 0));   // join
   if (tr) {
     cudaStreamSynchronize(st);
     FILE* f = fopen(trace_path, "w");
@@ -938,36 +926,36 @@ int factor(cvb_ctx* ctx, double* S, double* linv, int* d_flag, const TilePlan& p
 
 // solves L L^T x = b; b is destroyed, tmp is scratch (n_pad), result in x
 int solve(cvb_ctx* ctx, const double* L, const double* linv, double* b, double* tmp, double* x,
-          const TilePlan& plan, cudaStream_t st, const FactorStreams* fs) {
+          const TilePlan& plan, cudaStream_t st, const FactorStreams& fs) {
   const int nt = plan.nt;
   // The leading tile columns that belong to independent column groups (IMU chains, TilePlan::h_col_group) touch only
   // their own chain's rows of b / y, so the chains' substitution steps — pure launch-latency chains — run concurrently
   // on the group streams, forward before and backward after the sequential part.
-  const int n_gs = (fs && !plan.h_col_group.empty()) ? fs->n_group : 0;
+  const int n_gs = plan.h_col_group.empty() ? 0 : fs.n_group;
   int n_grouped = 0;
   while (n_gs > 0 && n_grouped < nt && plan.h_col_group[n_grouped] >= 0) n_grouped++;
   for (int k = n_grouped; k < nt; k++)
     if (n_gs > 0 && plan.h_col_group[k] >= 0) { n_grouped = 0; break; }   // groups must be a prefix; else run sequentially
   std::vector<char> used(n_gs > 0 ? n_gs : 1, 0);
   auto fork = [&]() -> int {
-    CVB_CUDA(ctx, cudaEventRecord(fs->fork, st));
+    CVB_CUDA(ctx, cudaEventRecord(fs.fork, st));
     std::fill(used.begin(), used.end(), 0);
     return CVB_OK;
   };
   auto stream_of = [&](int k, cudaStream_t* s) -> int {
     const int g = plan.h_col_group[k] % n_gs;
     if (!used[g]) {
-      CVB_CUDA(ctx, cudaStreamWaitEvent(fs->group[g], fs->fork, 0));
+      CVB_CUDA(ctx, cudaStreamWaitEvent(fs.group[g], fs.fork, 0));
       used[g] = 1;
     }
-    *s = fs->group[g];
+    *s = fs.group[g];
     return CVB_OK;
   };
   auto join = [&]() -> int {
     for (int g = 0; g < n_gs; g++)
       if (used[g]) {
-        CVB_CUDA(ctx, cudaEventRecord(fs->join[g], fs->group[g]));
-        CVB_CUDA(ctx, cudaStreamWaitEvent(st, fs->join[g], 0));
+        CVB_CUDA(ctx, cudaEventRecord(fs.join[g], fs.group[g]));
+        CVB_CUDA(ctx, cudaStreamWaitEvent(st, fs.join[g], 0));
       }
     return CVB_OK;
   };
@@ -1101,11 +1089,13 @@ extern "C" int cvb_dense_cholesky_solve(cvb_ctx* ctx, const double* A, int n, co
   cudaEventCreate(&e1);
   int rc = plan.upload(ctx, st);
   if (rc) return rc;
+  FactorStreams fs;
+  if ((rc = fs.create(ctx, nt))) return rc;
   cudaEventRecord(e0, st);
-  rc = factor(ctx, dS, dl, dflag, plan, st, nullptr);
+  rc = factor(ctx, dS, dl, dflag, plan, st, fs);
   cudaEventRecord(e1, st);
   if (rc) return rc;
-  rc = solve(ctx, dS, dl, dv, dv + np, dv + 2 * np, plan, st);
+  rc = solve(ctx, dS, dl, dv, dv + np, dv + 2 * np, plan, st, fs);
   if (rc) return rc;
   int flag = 0;
   CVB_CUDA(ctx, cudaMemcpyAsync(&flag, dflag, sizeof(int), cudaMemcpyDeviceToHost, st));

@@ -35,17 +35,24 @@ struct TilePlan {
   void release();
 };
 
-// Extra streams/events of a factorisation (all events with timing disabled); nullptr → everything on one stream.
+// Extra streams/events of a factorisation (all events with timing disabled), made by create() for a plan of nt tile
+// columns and released by destroy() or the destructor.
 struct FactorStreams {
+  FactorStreams() = default;
+  FactorStreams(const FactorStreams&) = delete;
+  FactorStreams& operator=(const FactorStreams&) = delete;
+  ~FactorStreams() { destroy(); }
+  static constexpr int n_group = 8;
   cudaStream_t bulk = nullptr;       // low-priority stream of the bulk trailing updates (depth-1 lookahead)
   cudaStream_t fast = nullptr;       // highest-priority stream of the critical chain (diagonal tile -> first panel tile -> next diagonal tile)
   cudaEvent_t fork_fast = nullptr;
-  cudaEvent_t* ev = nullptr;         // 5 * nt events: panel available, bulk done, diagonal tile done, chain step done, tile column k+1 updated
-  cudaStream_t group[8] = {};        // streams of the independent column groups (their chain streams)
-  cudaStream_t group_aux[8] = {};    // second stream per group: rest of the panel + updates, beside the group's chain
-  cudaEvent_t join_aux[8] = {};
-  int n_group = 0;
-  cudaEvent_t fork = nullptr, join[8] = {};
+  std::vector<cudaEvent_t> ev;       // 5 * nt events: panel available, bulk done, diagonal tile done, chain step done, tile column k+1 updated
+  cudaStream_t group[n_group] = {};  // streams of the independent column groups (their chain streams)
+  cudaStream_t group_aux[n_group] = {};   // second stream per group: rest of the panel + updates, beside the group's chain
+  cudaEvent_t join_aux[n_group] = {};
+  cudaEvent_t fork = nullptr, join[n_group] = {};
+  int create(cvb_ctx* ctx, int nt);
+  void destroy();
 };
 // Peer view of a distributed factorisation (one process per GPU, buffers mapped with CUDA IPC over NVLink):
 // every rank owns the tile columns h_owner says; after trsm of column k the owner raises flag[k] = epoch in every
@@ -61,8 +68,8 @@ struct DistView {
 };
 // S: packed tiles (plan.h_col_base / h_tile_of), linv: nt tile inverses
 int factor(cvb_ctx* ctx, double* S, double* linv, int* d_flag, const TilePlan& plan, cudaStream_t st,
-           const FactorStreams* fs, const DistView* dv = nullptr);
+           const FactorStreams& fs, const DistView* dv = nullptr);
 int solve(cvb_ctx* ctx, const double* L, const double* linv, double* b, double* tmp, double* x,
-          const TilePlan& plan, cudaStream_t st, const FactorStreams* fs = nullptr);
+          const TilePlan& plan, cudaStream_t st, const FactorStreams& fs);
 
 }  // namespace cvb_chol

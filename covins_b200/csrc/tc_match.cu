@@ -407,7 +407,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tc_scan_kernel(const TcParams 
         uint8_t* dst = sB + (size_t)s * TN * KB + row_offset<KB>(prow);
         const bool rv = it.r0 + prow < it.len;
         int part = 0;
-        if (rv && !(p.dbg & 2)) {
+        if (rv) {
           part = M::store_half(cur, half, dst);
         } else {
           for (int c = 0; c < KB / 32; c++) *reinterpret_cast<uint4*>(dst + (half * (KB / 32) + c) * 128) = make_uint4(0, 0, 0, 0);
@@ -455,60 +455,58 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tc_scan_kernel(const TcParams 
         wg_gemm<false, KB / 32>(acc, a_desc, make_desc(b_addr0 + (uint32_t)s * (TN * KB), 128, KB * 8));
         __syncwarp();
         if (lane == 0) mbar_arrive(&empty[s]);   // operands consumed: the producers may refill this stage
-        if (!(p.dbg & 1)) {
-          if (!M::kIsL2) {
-            // Two columns per instruction: 16-bit keys ((popc(t) - 2 popc(q & t) + 256) << 5 | slot) packed pairwise
-            // (even column low, odd column high), k-lists kept per half with packed 16-bit min/max, merged into the 32-bit
-            // (distance, index) lists once per tile — and only if the tile holds a candidate that beats the current k-th
-            // entry (later tiles have larger indices, so "beats" is a strict distance comparison).
-            const uint32_t* nrm2 = reinterpret_cast<const uint32_t*>(reinterpret_cast<const uint16_t*>(sNorm) + (n % NORM_RING) * TN);
-            unsigned pk0[K], pk1[K];
+        if (!M::kIsL2) {
+          // Two columns per instruction: 16-bit keys ((popc(t) - 2 popc(q & t) + 256) << 5 | slot) packed pairwise
+          // (even column low, odd column high), k-lists kept per half with packed 16-bit min/max, merged into the 32-bit
+          // (distance, index) lists once per tile — and only if the tile holds a candidate that beats the current k-th
+          // entry (later tiles have larger indices, so "beats" is a strict distance comparison).
+          const uint32_t* nrm2 = reinterpret_cast<const uint32_t*>(reinterpret_cast<const uint16_t*>(sNorm) + (n % NORM_RING) * TN);
+          unsigned pk0[K], pk1[K];
 #pragma unroll
-            for (int c = 0; c < K; c++) pk0[c] = pk1[c] = 0xFFFFFFFFu;
+          for (int c = 0; c < K; c++) pk0[c] = pk1[c] = 0xFFFFFFFFu;
 #pragma unroll
-            for (int i = 0; i < 16; i++) {
-              const unsigned nv = nrm2[4 * i + quad];   // columns 8 i + 2 quad (low half) and + 1 (high half)
-              insert_packed16<K>(pk0, nv - __byte_perm(acc[4 * i], acc[4 * i + 1], 0x5410));
-              insert_packed16<K>(pk1, nv - __byte_perm(acc[4 * i + 2], acc[4 * i + 3], 0x5410));
+          for (int i = 0; i < 16; i++) {
+            const unsigned nv = nrm2[4 * i + quad];   // columns 8 i + 2 quad (low half) and + 1 (high half)
+            insert_packed16<K>(pk0, nv - __byte_perm(acc[4 * i], acc[4 * i + 1], 0x5410));
+            insert_packed16<K>(pk1, nv - __byte_perm(acc[4 * i + 2], acc[4 * i + 3], 0x5410));
+          }
+#pragma unroll
+          for (int rr = 0; rr < 2; rr++) {
+            unsigned (&pk)[K] = rr ? pk1 : pk0;
+            int (&wk)[K] = rr ? wk1 : wk0;
+            const unsigned best16 = min(pk[0] & 0xFFFFu, pk[0] >> 16);
+            const int worst_v = wk[K - 1] == INT_MAX ? 1024 : (wk[K - 1] >> kIdxBits) + 256;   // arithmetic shift: t-domain value
+            if ((int)(best16 >> 5) < worst_v) {
+#pragma unroll
+              for (int c = 0; c < K; c++)
+#pragma unroll
+                for (int hh = 0; hh < 2; hh++) {
+                  const unsigned k16 = hh ? (pk[c] >> 16) : (pk[c] & 0xFFFFu);
+                  const int col = 8 * (int)((k16 & 31u) >> 1) + 2 * quad + (int)(k16 & 1u);
+                  insert_packed<K>(wk, k16 == 0xFFFFu ? INT_MAX
+                                                      : (int)((((unsigned)(k16 >> 5) - 256u) << kIdxBits) + (unsigned)(r0 + col)));
+                }
             }
+          }
+        } else {
+          const int* nrm = sNorm + (n % NORM_RING) * TN;
 #pragma unroll
-            for (int rr = 0; rr < 2; rr++) {
-              unsigned (&pk)[K] = rr ? pk1 : pk0;
-              int (&wk)[K] = rr ? wk1 : wk0;
-              const unsigned best16 = min(pk[0] & 0xFFFFu, pk[0] >> 16);
-              const int worst_v = wk[K - 1] == INT_MAX ? 1024 : (wk[K - 1] >> kIdxBits) + 256;   // arithmetic shift: t-domain value
-              if ((int)(best16 >> 5) < worst_v) {
+          for (int i = 0; i < 16; i++) {
+            const int2 nn = *reinterpret_cast<const int2*>(nrm + 8 * i + 2 * quad);
 #pragma unroll
-                for (int c = 0; c < K; c++)
-#pragma unroll
-                  for (int hh = 0; hh < 2; hh++) {
-                    const unsigned k16 = hh ? (pk[c] >> 16) : (pk[c] & 0xFFFFu);
-                    const int col = 8 * (int)((k16 & 31u) >> 1) + 2 * quad + (int)(k16 & 1u);
-                    insert_packed<K>(wk, k16 == 0xFFFFu ? INT_MAX
-                                                        : (int)((((unsigned)(k16 >> 5) - 256u) << kIdxBits) + (unsigned)(r0 + col)));
-                  }
-              }
-            }
-          } else {
-            const int* nrm = sNorm + (n % NORM_RING) * TN;
-#pragma unroll
-            for (int i = 0; i < 16; i++) {
-              const int2 nn = *reinterpret_cast<const int2*>(nrm + 8 * i + 2 * quad);
-#pragma unroll
-              for (int e = 0; e < 4; e++) {
-                const int j = 8 * i + 2 * quad + (e & 1);
-                const int tn = (e & 1) ? nn.y : nn.x;
-                int (&wk)[K] = e < 2 ? wk0 : wk1;
-                int (&wi)[K] = e < 2 ? wi0 : wi1;
-                int (&wd)[K] = e < 2 ? wd0 : wd1;
-                const int d = (e < 2 ? qn0 : qn1) + tn - 2 * (int)acc[4 * i + e];
-                if (d < wd[K - 1]) {
-                  const int key = __float_as_int(__fsqrt_rn((float)d));
-                  if (key < wk[K - 1]) {
-                    insert_key<K>(wk, wi, key, r0 + j);
-                    const float f = __int_as_float(wk[K - 1]);   // raw-distance bound of the worst entry (pre-test)
-                    wd[K - 1] = wk[K - 1] == kInfKey ? kInf : (int)ceilf(f * f * 1.000001f) + 1;
-                  }
+            for (int e = 0; e < 4; e++) {
+              const int j = 8 * i + 2 * quad + (e & 1);
+              const int tn = (e & 1) ? nn.y : nn.x;
+              int (&wk)[K] = e < 2 ? wk0 : wk1;
+              int (&wi)[K] = e < 2 ? wi0 : wi1;
+              int (&wd)[K] = e < 2 ? wd0 : wd1;
+              const int d = (e < 2 ? qn0 : qn1) + tn - 2 * (int)acc[4 * i + e];
+              if (d < wd[K - 1]) {
+                const int key = __float_as_int(__fsqrt_rn((float)d));
+                if (key < wk[K - 1]) {
+                  insert_key<K>(wk, wi, key, r0 + j);
+                  const float f = __int_as_float(wk[K - 1]);   // raw-distance bound of the worst entry (pre-test)
+                  wd[K - 1] = wk[K - 1] == kInfKey ? kInf : (int)ceilf(f * f * 1.000001f) + 1;
                 }
               }
             }
@@ -579,8 +577,6 @@ constexpr int CONS_WARPS = 4 * 2 * NGRP;      // warpgroups (h, g), h = query ha
 constexpr int TMA_WARP = CONS_WARPS;
 constexpr int XTHREADS = (TMA_WARP + 1) * 32;
 constexpr int kKeyInvalid = 32896;            // keys >= this are "no row"
-constexpr int kPaceWindow = 96;               // tiles a CTA may run ahead of the slowest CTA of its keyframe range (3.4 MB)
-constexpr long kPaceMinTiles = 1536;          // pacing only when a CTA walks more tiles than this
 constexpr size_t kSmemBytes = (size_t)(XSTAGES + 1) * TILE_BYTES + 1024;   // query block + ring + barriers
 
 __device__ __forceinline__ uint32_t xrow_off(int r) { return (uint32_t)(r >> 3) * (KX * 8) + (uint32_t)(r & 7) * 16; }
@@ -713,22 +709,6 @@ __global__ void __launch_bounds__(XTHREADS, 1) tc_xt_kernel(const TcParams p) {
         for (int g = 0; g < NGRP; g++) {
           if (!S.active(g)) continue;
           const int s = n % XSTAGES;
-          if (p.progress != nullptr && (n & 15) == 0 && n > 0) {
-            // Pacing (large maps only): the nqb CTAs that walk the same keyframe range read every tile once from HBM and
-            // nqb - 1 times from L2 — as long as they stay within an L2's worth of each other.  Over thousands of tiles they
-            // can drift apart; the producer therefore publishes its position every 16 tiles and waits while it is more than
-            // kPaceWindow tiles ahead of the slowest CTA of its group.
-            // (All CTAs are resident — grid <= SM count, one CTA per SM — so the wait cannot deadlock.)
-            volatile int* grp_prog = p.progress + (size_t)part * p.nqb;
-            grp_prog[qb] = n;
-            __threadfence();
-            for (;;) {
-              int mn = INT_MAX;
-              for (int i = 0; i < p.nqb; i++) mn = min(mn, grp_prog[i]);
-              if (mn + kPaceWindow >= n) break;
-              __nanosleep(500);
-            }
-          }
           if (n >= XSTAGES) cvb_mbar_wait(&empty[s], ((n / XSTAGES) - 1) & 1);
           cvb_mbar_expect_tx(&full[s], TILE_BYTES);
           const uint8_t* src = p.xt + (size_t)(S.tile0[g] + S.t[g]) * TILE_BYTES;
@@ -738,10 +718,6 @@ __global__ void __launch_bounds__(XTHREADS, 1) tc_xt_kernel(const TcParams p) {
           S.advance(g);
           n++;
         }
-      }
-      if (p.progress != nullptr) {   // done: never hold the others back
-        reinterpret_cast<volatile int*>(p.progress)[(size_t)part * p.nqb + qb] = INT_MAX;
-        __threadfence();
       }
     }
     __syncwarp();
@@ -781,32 +757,30 @@ __global__ void __launch_bounds__(XTHREADS, 1) tc_xt_kernel(const TcParams p) {
           wg_gemm<true, NSLICE>(acc, a_desc, make_desc(b_addr0 + (uint32_t)s * TILE_BYTES, 128, KX * 8));
           __syncwarp();
           if (lane == 0) mbar_arrive(&empty[s]);   // operands consumed: the producer may refill this stage
-          if (!(p.dbg & 1)) {
-            unsigned pk0[K], pk1[K];
+          unsigned pk0[K], pk1[K];
 #pragma unroll
-            for (int c = 0; c < K; c++) pk0[c] = pk1[c] = 0xFFFFFFFFu;
+          for (int c = 0; c < K; c++) pk0[c] = pk1[c] = 0xFFFFFFFFu;
 #pragma unroll
-            for (int i = 0; i < 16; i++) {   // columns 8 i + 2 quad (low half) and + 1 (high half)
-              insert_packed16<K>(pk0, __byte_perm(acc[4 * i], acc[4 * i + 1], 0x5410));
-              insert_packed16<K>(pk1, __byte_perm(acc[4 * i + 2], acc[4 * i + 3], 0x5410));
-            }
-            // later tiles hold larger row indices: a candidate enters only with a strictly smaller distance than the k-th entry
+          for (int i = 0; i < 16; i++) {   // columns 8 i + 2 quad (low half) and + 1 (high half)
+            insert_packed16<K>(pk0, __byte_perm(acc[4 * i], acc[4 * i + 1], 0x5410));
+            insert_packed16<K>(pk1, __byte_perm(acc[4 * i + 2], acc[4 * i + 3], 0x5410));
+          }
+          // later tiles hold larger row indices: a candidate enters only with a strictly smaller distance than the k-th entry
 #pragma unroll
-            for (int rr = 0; rr < 2; rr++) {
-              unsigned (&pk)[K] = rr ? pk1 : pk0;
-              int (&wk)[K] = rr ? wk1 : wk0;
-              const unsigned best16 = min(pk[0] & 0xFFFFu, pk[0] >> 16);
-              const int worst_d = wk[K - 1] == INT_MAX ? 1024 : (wk[K - 1] >> kIdxBits);
-              if ((int)(best16 >> 7) < worst_d) {
+          for (int rr = 0; rr < 2; rr++) {
+            unsigned (&pk)[K] = rr ? pk1 : pk0;
+            int (&wk)[K] = rr ? wk1 : wk0;
+            const unsigned best16 = min(pk[0] & 0xFFFFu, pk[0] >> 16);
+            const int worst_d = wk[K - 1] == INT_MAX ? 1024 : (wk[K - 1] >> kIdxBits);
+            if ((int)(best16 >> 7) < worst_d) {
 #pragma unroll
-                for (int c = 0; c < K; c++)
+              for (int c = 0; c < K; c++)
 #pragma unroll
-                  for (int hh = 0; hh < 2; hh++) {
-                    const unsigned k16 = hh ? (pk[c] >> 16) : (pk[c] & 0xFFFFu);
-                    insert_packed<K>(wk, k16 >= (unsigned)kKeyInvalid ? INT_MAX
-                                                                     : (int)(((k16 >> 7) << kIdxBits) + (unsigned)(t * TN) + (k16 & 127u)));
-                  }
-              }
+                for (int hh = 0; hh < 2; hh++) {
+                  const unsigned k16 = hh ? (pk[c] >> 16) : (pk[c] & 0xFFFFu);
+                  insert_packed<K>(wk, k16 >= (unsigned)kKeyInvalid ? INT_MAX
+                                                                   : (int)(((k16 >> 7) << kIdxBits) + (unsigned)(t * TN) + (k16 & 127u)));
+                }
             }
           }
           if (t == S.nt[g2] - 1) {
@@ -834,15 +808,7 @@ __global__ void __launch_bounds__(XTHREADS, 1) tc_xt_kernel(const TcParams p) {
 }
 
 template <int K>
-int launch_xt(cvb_ctx* ctx, TcParams p, long total_tiles, cudaStream_t st) {
-  p.progress = nullptr;
-  // opt-in (COVINS_B200_TC_PACING=1): kept for the case the CTAs of a keyframe range drift out of each other's L2 window
-  const char* pace = getenv("COVINS_B200_TC_PACING");
-  if (p.nqb > 1 && total_tiles / p.parts > kPaceMinTiles && pace && atoi(pace)) {
-    p.progress = (int*)cvb_ws(ctx, WS_XT_PROGRESS, sizeof(int) * (size_t)p.nqb * p.parts);
-    if (!p.progress) return CVB_ERR_CUDA;
-    CVB_CUDA(ctx, cudaMemsetAsync(p.progress, 0, sizeof(int) * (size_t)p.nqb * p.parts, st));
-  }
+int launch_xt(cvb_ctx* ctx, const TcParams& p, cudaStream_t st) {
   static cvb_once_per_device once;
   if (once.first(ctx->device)) {
     CVB_CUDA(ctx, cudaFuncSetAttribute(tc_xt_kernel<K>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes));
@@ -900,10 +866,6 @@ int launch(cvb_ctx* ctx, TcParams p, int metric, int k, cudaStream_t st) {
   if (parts < 1) parts = 1;
   if (parts > p.n_seg) parts = p.n_seg;
   p.parts = parts;
-  {
-    const char* d = getenv("COVINS_B200_TC_DEBUG");
-    p.dbg = d ? atoi(d) : 0;
-  }
   if (metric == 0 && !(getenv("COVINS_B200_TC_XT") && !strcmp(getenv("COVINS_B200_TC_XT"), "0"))) {
     if (!p.xt) {
       // no resident tile store for this train set (raw-pointer API): expand it into the workspace first (HBM-bound pre-pass)
@@ -920,12 +882,11 @@ int launch(cvb_ctx* ctx, TcParams p, int metric, int k, cudaStream_t st) {
       p.xt = d_xt;
       p.seg_tile = d_tile;
     }
-    const long total_tiles = (long)tiles_of(p.h_seg, p.n_seg, nullptr);
     switch (k) {
-      case 1: return xt::launch_xt<1>(ctx, p, total_tiles, st);
-      case 2: return xt::launch_xt<2>(ctx, p, total_tiles, st);
-      case 3: return xt::launch_xt<3>(ctx, p, total_tiles, st);
-      default: return xt::launch_xt<4>(ctx, p, total_tiles, st);
+      case 1: return xt::launch_xt<1>(ctx, p, st);
+      case 2: return xt::launch_xt<2>(ctx, p, st);
+      case 3: return xt::launch_xt<3>(ctx, p, st);
+      default: return xt::launch_xt<4>(ctx, p, st);
     }
   }
 #define TC_CASE(MM, KK) return launch_tc<MM, KK>(ctx, p, st)

@@ -17,9 +17,6 @@ struct TcParams {
   int nqb, parts;           // filled by launch()
   int32_t* out_idx;
   void* out_dist;
-  const uint8_t* skipA;
-  const uint8_t* skipB;
-  int ithr;
   int filter;
   float thr, ratio;
   int32_t* match_train;
@@ -30,8 +27,6 @@ struct TcParams {
   const uint8_t* xt;
   const int32_t* seg_tile;
   const int32_t* h_seg;
-  int* progress;            // filled by launch(): per (part, query block) tile counter of the pacing scheme, or nullptr
-  int dbg;   // development switches (COVINS_B200_TC_DEBUG): 1 = epilogue skips the selection, 2 = producers skip the expansion
 };
 
 // metric 0 = Hamming (32-byte rows), 1 = L2 on u8 (128-byte rows); OpenCV k-NN rule (the DenseMatcher list rule is

@@ -15,12 +15,7 @@ ctx = covins_b200.Context(local)
 cfg = sys.argv[1] if len(sys.argv) > 1 else "C3"
 p = synth_map.make_config(cfg)
 for spec in (sys.argv[2].split(",") if len(sys.argv) > 2 else "1,2,3,4,6,8".split(",")):
-    nochain = spec.endswith("nc")            # "6nc" = block 6 without the critical-chain stream
-    blk = int(spec[:-2] if nochain else spec)
-    os.environ["COVINS_B200_DIST_BLOCK"] = str(blk)
-    os.environ.pop("COVINS_B200_NO_CHAIN_STREAM", None)
-    if nochain:
-        os.environ["COVINS_B200_NO_CHAIN_STREAM"] = "1"
+    os.environ["COVINS_B200_DIST_BLOCK"] = str(int(spec))
     s = O.BaSolver(ctx, p, rank=rank, world=world, allreduce=O.torch_allreduce(), p2p=True)
     s.iterate(2); ctx.sync(); dist.barrier()
     s.restart(); s.timing(reset=True); ctx.sync(); dist.barrier()
