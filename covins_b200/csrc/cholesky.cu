@@ -8,7 +8,7 @@
 // At EuRoC scale every keyframe is covisible with hundreds of others (all agents fly the same hall), so the pose part
 // of S is ~10 % block-dense before fill and fills in almost completely: a tiled dense-tile factorisation is the right
 // shape for the GPU; this is the one BA stage that is a true GEMM and runs on the FP64 tensor cores (DMMA,
-// mma.sync.m8n8k4.f64 — wgmma has no FP64 kind).
+// mma.sync.m16n8k16.f64, Hopper's full-rate shape — wgmma has no FP64 kind).
 //
 // Right-looking, panel width 128:
 //   potrf_inv_kernel   1 CTA: factor the 128x128 diagonal tile in shared memory, write L, write L^-1
@@ -32,51 +32,62 @@ template <int N>
 __device__ __forceinline__ void cp_async_wait() {
   asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory");
 }
-__device__ __forceinline__ void dmma(double& c0, double& c1, double a, double b) {
-  asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};"
-               : "+d"(c0), "+d"(c1)
-               : "d"(a), "d"(b));
+// D = C + A B^T on one 16 x 8 x 16 block (SASS DMMA.16x8x16).  Fragments, g = lane / 4, t = lane % 4:
+//   a[i] = A(g + 8 (i % 2), t + 4 (i / 2)),  b[i] = B(g, t + 4 i),  c[i] = C(g + 8 (i / 2), 2 t + i % 2).
+__device__ __forceinline__ void dmma16816(double (&c)[4], const double (&a)[8], const double (&b)[4]) {
+  asm volatile("mma.sync.aligned.m16n8k16.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5,%6,%7,%8,%9,%10,%11}, "
+               "{%12,%13,%14,%15}, {%0,%1,%2,%3};"
+               : "+d"(c[0]), "+d"(c[1]), "+d"(c[2]), "+d"(c[3])
+               : "d"(a[0]), "d"(a[1]), "d"(a[2]), "d"(a[3]), "d"(a[4]), "d"(a[5]), "d"(a[6]), "d"(a[7]),
+                 "d"(b[0]), "d"(b[1]), "d"(b[2]), "d"(b[3]));
 }
 
 // acc(64 x BN) = A(64 x T) * B(BN x T)^T, both operands row-major with K contiguous (leading dims lda, ldb).
-// 2 x BN/32 warps, 32x32 per warp = 4x4 m8n8k4 tiles.  K is staged in chunks of 16 through a STAGES-deep cp.async ring
-// (one barrier per chunk).  Row stride 20 doubles (≡ 8 words mod 32): the fragment loads of a half-warp are
-// conflict-free.  The CTA is deliberately small (64 x 64 x 128 for the trailing update: 128 threads, 60 KB): three to
-// four CTAs share an SM, so one CTA's fixed costs — index fetch, pipeline fill, the C round trip of the epilogue, barrier
-// bubbles — overlap the others' main loops.  (One 128x128 tile per SM left the FP64 tensor pipe idle a third of the time.)
+// 2 x BN/32 warps, 32x32 per warp = 2 (m16) x 4 (n8) m16n8k16 blocks, acc[i][j] = rows 16 i.., columns 8 j.. of the warp
+// tile in the C-fragment order of dmma16816.  m16n8k16 is Hopper's full-rate FP64 MMA shape: on an H100 SXM (400 W limit)
+// a register-only probe sustained 64 TFLOP/s with it (~128 FMA/clk/SM) and 34 TFLOP/s with the Ampere m8n8k4 shape, and
+// its results were bit-identical to four chained m8n8k4 over the same 16-wide K chunk.  K is staged in chunks of 16 (one
+// MMA per block and chunk) through a STAGES-deep cp.async ring (one barrier per chunk).  Row stride 20 doubles (≡ 8 words
+// mod 32): the fragment loads of a half-warp (rows g = 0..3, columns t = 0..3) hit words 8g + 2t, conflict-free.  The CTA
+// is deliberately small (64 x 64 x 128 for the trailing update: 128 threads, 60 KB): three to four CTAs share an SM, so
+// one CTA's fixed costs — index fetch, pipeline fill, the C round trip of the epilogue, barrier bubbles — overlap the
+// others' main loops.  (One 128x128 tile per SM left the FP64 tensor pipe idle a third of the time.)
 constexpr int KC = 16;
 constexpr int LDS = KC + 4;
 constexpr int GEMM_STAGES = 3;
 
 template <int BN>
 __device__ __forceinline__ void gemm_abt_64(const double* __restrict__ A, size_t lda, const double* __restrict__ B,
-                                            size_t ldb, double (&acc)[4][4][2], double* smem) {
+                                            size_t ldb, double (&acc)[2][4][4], double* smem) {
   constexpr int WN = BN / 32, THREADS = 2 * WN * 32, STAGE = (64 + BN) * LDS, NCH = T / KC, UPR = KC / 2;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int wm = warp / WN, wn = warp % WN;
 #pragma unroll
-  for (int i = 0; i < 4; i++)
+  for (int i = 0; i < 2; i++)
 #pragma unroll
-    for (int j = 0; j < 4; j++) acc[i][j][0] = acc[i][j][1] = 0.0;
+    for (int j = 0; j < 4; j++)
+#pragma unroll
+      for (int e = 0; e < 4; e++) acc[i][j][e] = 0.0;
+  // a thread copies the same 16-byte segment of rows r0, r0 + RSTEP, ...: one base address per operand
+  constexpr int RSTEP = THREADS / UPR;
+  const int r0 = tid / UPR, seg = tid % UPR;
+  const double* ga = A + (size_t)r0 * lda + seg * 2;
+  const double* gb = B + (size_t)r0 * ldb + seg * 2;
+  const int so = r0 * LDS + seg * 2;
   auto load_chunk = [&](int kc) {
     if (kc < NCH) {
-      double* As = smem + (kc % GEMM_STAGES) * STAGE;
+      double* As = smem + (kc % GEMM_STAGES) * STAGE + so;
       double* Bs = As + 64 * LDS;
 #pragma unroll
-      for (int it = 0; it < 64 * UPR / THREADS; it++) {
-        const int u = tid + it * THREADS, r = u / UPR, seg = u % UPR;
-        cp_async16(As + r * LDS + seg * 2, A + (size_t)r * lda + kc * KC + seg * 2);
-      }
+      for (int it = 0; it < 64 / RSTEP; it++) cp_async16(As + it * RSTEP * LDS, ga + (size_t)it * RSTEP * lda + kc * KC);
 #pragma unroll
-      for (int it = 0; it < BN * UPR / THREADS; it++) {
-        const int u = tid + it * THREADS, r = u / UPR, seg = u % UPR;
-        cp_async16(Bs + r * LDS + seg * 2, B + (size_t)r * ldb + kc * KC + seg * 2);
-      }
+      for (int it = 0; it < BN / RSTEP; it++) cp_async16(Bs + it * RSTEP * LDS, gb + (size_t)it * RSTEP * ldb + kc * KC);
     }
     cp_async_commit();   // always commit (possibly empty) so the wait count below is uniform
   };
 #pragma unroll
   for (int c = 0; c < GEMM_STAGES - 1; c++) load_chunk(c);
+#pragma unroll 1   // unrolled, both instantiations exceed their register budgets and spill
   for (int kc = 0; kc < NCH; kc++) {
     cp_async_wait<GEMM_STAGES - 2>();   // chunk kc has landed
     __syncthreads();                    // ... for every thread, and chunk kc-1's stage is free again
@@ -84,17 +95,18 @@ __device__ __forceinline__ void gemm_abt_64(const double* __restrict__ A, size_t
     const double* As = smem + (kc % GEMM_STAGES) * STAGE;
     const double* a_base = As + (wm * 32 + (lane >> 2)) * LDS + (lane & 3);
     const double* b_base = As + 64 * LDS + (wn * 32 + (lane >> 2)) * LDS + (lane & 3);
+    double a[2][8];
 #pragma unroll
-    for (int ks = 0; ks < KC / 4; ks++) {
-      double a[4], b[4];
+    for (int i = 0; i < 2; i++)
 #pragma unroll
-      for (int i = 0; i < 4; i++) a[i] = a_base[i * 8 * LDS + ks * 4];
+      for (int e = 0; e < 8; e++) a[i][e] = a_base[(i * 16 + 8 * (e & 1)) * LDS + 4 * (e >> 1)];
 #pragma unroll
-      for (int j = 0; j < 4; j++) b[j] = b_base[j * 8 * LDS + ks * 4];
+    for (int j = 0; j < 4; j++) {
+      double b[4];
 #pragma unroll
-      for (int i = 0; i < 4; i++)
+      for (int e = 0; e < 4; e++) b[e] = b_base[j * 8 * LDS + 4 * e];
 #pragma unroll
-        for (int j = 0; j < 4; j++) dmma(acc[i][j][0], acc[i][j][1], a[i], b[j]);
+      for (int i = 0; i < 2; i++) dmma16816(acc[i][j], a[i], b);
     }
   }
 }
@@ -113,17 +125,19 @@ __global__ void __launch_bounds__(TRSM_THREADS, 2) trsm_kernel(double* __restric
   constexpr size_t ld = T;
   const int half = blockIdx.x & 1;
   double* At = panel + (size_t)(blockIdx.x >> 1) * TT + (size_t)half * 64 * T;
-  double acc[4][4][2];
+  double acc[2][4][4];
   gemm_abt_64<128>(At, ld, linv_k, T, acc, smem_d);
   __syncthreads();   // every warp is done reading this CTA's rows (they were all staged through shared memory)
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, wm = warp >> 2, wn = warp & 3;
 #pragma unroll
-  for (int a = 0; a < 4; a++)
+  for (int a = 0; a < 2; a++)
 #pragma unroll
-    for (int b = 0; b < 4; b++) {
-      const int r = wm * 32 + a * 8 + (lane >> 2), c = wn * 32 + b * 8 + (lane & 3) * 2;
-      *reinterpret_cast<double2*>(At + (size_t)r * ld + c) = make_double2(acc[a][b][0], acc[a][b][1]);
-    }
+    for (int b = 0; b < 4; b++)
+#pragma unroll
+      for (int h = 0; h < 2; h++) {
+        const int r = wm * 32 + a * 16 + h * 8 + (lane >> 2), c = wn * 32 + b * 8 + (lane & 3) * 2;
+        *reinterpret_cast<double2*>(At + (size_t)r * ld + c) = make_double2(acc[a][b][2 * h], acc[a][b][2 * h + 1]);
+      }
 }
 
 // The two small products of the critical chain (see factor(): "chain column"), one 128x128 tile each:
@@ -182,20 +196,22 @@ __global__ void __launch_bounds__(SYRK_THREADS, 3) syrk_kernel(double* __restric
   const double* Ai = S + (size_t)tile_of[(size_t)i * nt + k] * TT + (size_t)qr * 64 * T;
   const double* Aj = S + (size_t)tile_of[(size_t)j * nt + k] * TT + (size_t)qc * 64 * T;
   double* C = S + (size_t)tile_of[(size_t)i * nt + j] * TT + (size_t)qr * 64 * T + qc * 64;
-  double acc[4][4][2];
+  double acc[2][4][4];
   gemm_abt_64<64>(Ai, ld, Aj, ld, acc, smem_d);
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, wm = warp >> 1, wn = warp & 1;
 #pragma unroll
-  for (int a = 0; a < 4; a++)
+  for (int a = 0; a < 2; a++)
 #pragma unroll
-    for (int b = 0; b < 4; b++) {
-      const int r = wm * 32 + a * 8 + (lane >> 2), c = wn * 32 + b * 8 + (lane & 3) * 2;
-      double2* q = reinterpret_cast<double2*>(C + (size_t)r * ld + c);
-      double2 v = *q;
-      v.x -= acc[a][b][0];
-      v.y -= acc[a][b][1];
-      *q = v;
-    }
+    for (int b = 0; b < 4; b++)
+#pragma unroll
+      for (int h = 0; h < 2; h++) {
+        const int r = wm * 32 + a * 16 + h * 8 + (lane >> 2), c = wn * 32 + b * 8 + (lane & 3) * 2;
+        double2* q = reinterpret_cast<double2*>(C + (size_t)r * ld + c);
+        double2 v = *q;
+        v.x -= acc[a][b][2 * h];
+        v.y -= acc[a][b][2 * h + 1];
+        *q = v;
+      }
 }
 
 // Factor the diagonal tile k in shared memory and invert the factor, one CTA of 512 threads.  This kernel is the serial
