@@ -19,6 +19,7 @@
 
 #include "ba_math.cuh"
 #include "cvb_internal.cuh"
+#include "geom_common.cuh"
 
 namespace {
 
@@ -37,12 +38,6 @@ struct DevPair {
   int* match1; int* match2; int* match12; int* n_found;
 };
 
-__device__ __forceinline__ double mul(double a, double b) { return __dmul_rn(a, b); }
-__device__ __forceinline__ double add(double a, double b) { return __dadd_rn(a, b); }
-__device__ __forceinline__ double sub(double a, double b) { return __dsub_rn(a, b); }
-__device__ __forceinline__ double dot3(double a0, double a1, double a2, const double* p) {
-  return add(add(mul(a0, p[0]), mul(a1, p[1])), mul(a2, p[2]));
-}
 __device__ __forceinline__ void rt_apply(const double* T, const double* p, double* o) {
 #pragma unroll
   for (int r = 0; r < 3; r++) o[r] = add(dot3(T[4 * r], T[4 * r + 1], T[4 * r + 2], p), T[4 * r + 3]);
@@ -264,30 +259,9 @@ __global__ void __launch_bounds__(256) score_abs_kernel(const double* __restrict
   const double* M = model + 12 * (size_t)h;
   int in = 0;
   if (i < n) {
-    // inverseSolution = [R^T | -R^T t]
     double Ri[9], ti[3];
-#pragma unroll
-    for (int r = 0; r < 3; r++)
-#pragma unroll
-      for (int c = 0; c < 3; c++) Ri[3 * r + c] = M[4 * c + r];
-    const double t[3] = {M[3], M[7], M[11]};
-#pragma unroll
-    for (int r = 0; r < 3; r++) ti[r] = -dot3(Ri[3 * r], Ri[3 * r + 1], Ri[3 * r + 2], t);
-    const double p[3] = {pts[3 * (size_t)i], pts[3 * (size_t)i + 1], pts[3 * (size_t)i + 2]};
-    double b[3], q[3];
-#pragma unroll
-    for (int r = 0; r < 3; r++) b[r] = sub(add(dot3(Ri[3 * r], Ri[3 * r + 1], Ri[3 * r + 2], p), ti[r]), cam[r]);
-    const double* Rc = cam + 3;
-#pragma unroll
-    for (int r = 0; r < 3; r++) q[r] = dot3(Rc[r], Rc[3 + r], Rc[6 + r], b);
-    const double nrm = __dsqrt_rn(add(add(mul(q[0], q[0]), mul(q[1], q[1])), mul(q[2], q[2])));
-    double e2 = 0.0;
-#pragma unroll
-    for (int r = 0; r < 3; r++) {
-      const double e = sub(__ddiv_rn(q[r], nrm), f[3 * (size_t)i + r]);
-      e2 = r == 0 ? mul(e, e) : add(e2, mul(e, e));
-    }
-    const double s = __ddiv_rn(e2, sigma[i]);
+    abs_inverse(M, Ri, ti);
+    const double s = abs_score(Ri, ti, pts + 3 * (size_t)i, f + 3 * (size_t)i, sigma[i], cam);
     in = s < threshold;
     if (scores) scores[(size_t)h * n + i] = s;
     if (inlier) inlier[(size_t)h * n + i] = (uint8_t)in;
@@ -344,18 +318,6 @@ __global__ void __launch_bounds__(256) score_rel_kernel(const double* __restrict
   for (int o = 16; o > 0; o >>= 1) in += __shfl_xor_sync(0xffffffffu, in, o);
   if ((threadIdx.x & 31) == 0 && in) atomicAdd(n_inliers + h, in);
 }
-
-// ---- host staging: everything of a call goes through ONE pinned block and ONE device block --------------------------
-struct Stager {
-  std::vector<unsigned char> h;
-  size_t put(const void* p, size_t bytes) {
-    const size_t off = (h.size() + 15) & ~size_t(15);
-    h.resize(off + bytes);
-    if (p && bytes) memcpy(h.data() + off, p, bytes);
-    return off;
-  }
-  size_t reserve(size_t bytes) { return put(nullptr, bytes); }
-};
 
 size_t stage_kf(Stager& S, const cvb_kf_view* v, size_t off[9]) {
   const size_t n = (size_t)v->n;

@@ -965,6 +965,56 @@ inline std::vector<int> ScoreRelativePoseHypotheses(Context& ctx, const std::vec
   return std::vector<int>(cnt.begin(), cnt.begin() + n_hyp);
 }
 
+// The whole GP3P RANSAC of Se3Solver::projectiveAlignment (Se3Solver.cpp:59-110) for a batch of candidate keyframes in one
+// call (cvb_ransac_absolute_pose_batch): P3P hypothesis per sample, scoring and opengv's sequential model selection on the GPU.
+// Per problem: its correspondences (as ScoreAbsolutePoseHypotheses), its camera in the body frame and its samples (4 local
+// indices each; every problem of a call has the same number of samples, e.g. max_iterations plus headroom for skipped ones).
+struct AbsolutePoseRansacProblem {
+  std::vector<double> points, bearings, sigma_angles;   // 3n, 3n, n
+  double cam_offset[3] = {0, 0, 0};
+  double cam_rotation[9] = {1, 0, 0, 0, 1, 0, 0, 0, 1};   // row-major
+  std::vector<int32_t> samples;                          // 4 * n_samples
+};
+struct AbsolutePoseRansacResult {
+  int best_sample = -1;             // -1: no model
+  std::array<double, 12> model{};   // 3x4 [R|t] row-major, body in world
+  int n_inliers = 0, iterations = 0, samples_used = 0;
+  std::vector<uint8_t> inliers;     // n flags of the selected model
+};
+inline std::vector<AbsolutePoseRansacResult> RansacAbsolutePose(Context& ctx, const std::vector<AbsolutePoseRansacProblem>& problems, double threshold,
+                                                                 int max_iterations, double probability = 0.99) {
+  const int n_prob = (int)problems.size();
+  const size_t n_samples = n_prob ? problems[0].samples.size() / 4 : 0;
+  std::vector<int32_t> ptr(n_prob + 1, 0), samples;
+  std::vector<double> pts, f, sigma, cam_off, cam_rot;
+  for (int i = 0; i < n_prob; i++) {
+    const AbsolutePoseRansacProblem& p = problems[i];
+    if (p.samples.size() != 4 * n_samples || p.points.size() != 3 * p.sigma_angles.size() || p.bearings.size() != 3 * p.sigma_angles.size())
+      throw std::invalid_argument("covins_b200::RansacAbsolutePose: inconsistent problem sizes");
+    ptr[i + 1] = ptr[i] + (int32_t)p.sigma_angles.size();
+    pts.insert(pts.end(), p.points.begin(), p.points.end());
+    f.insert(f.end(), p.bearings.begin(), p.bearings.end());
+    sigma.insert(sigma.end(), p.sigma_angles.begin(), p.sigma_angles.end());
+    cam_off.insert(cam_off.end(), p.cam_offset, p.cam_offset + 3);
+    cam_rot.insert(cam_rot.end(), p.cam_rotation, p.cam_rotation + 9);
+    samples.insert(samples.end(), p.samples.begin(), p.samples.end());
+  }
+  const size_t m = n_prob > 0 ? n_prob : 1;
+  std::vector<int32_t> best(m), cnt(m), iters(m), used(m);
+  std::vector<double> models(12 * m);
+  std::vector<uint8_t> mask(ptr[n_prob] > 0 ? ptr[n_prob] : 1);
+  cvb_abs_ransac_problems P{n_prob, ptr.data(), pts.data(), f.data(), sigma.data(), cam_off.data(), cam_rot.data(), samples.data(), (int32_t)n_samples};
+  cvb_abs_ransac_result R{best.data(), models.data(), cnt.data(), iters.data(), used.data(), mask.data(), nullptr, nullptr, nullptr};
+  ctx.check(cvb_ransac_absolute_pose_batch(ctx.get(), &P, threshold, max_iterations, probability, &R), "cvb_ransac_absolute_pose_batch");
+  std::vector<AbsolutePoseRansacResult> out(n_prob);
+  for (int i = 0; i < n_prob; i++) {
+    out[i].best_sample = best[i]; out[i].n_inliers = cnt[i]; out[i].iterations = iters[i]; out[i].samples_used = used[i];
+    std::copy(models.begin() + 12 * i, models.begin() + 12 * (i + 1), out[i].model.begin());
+    out[i].inliers.assign(mask.begin() + ptr[i], mask.begin() + ptr[i + 1]);
+  }
+  return out;
+}
+
 // Resident-map descriptor database (cvb_db_*): the ORB descriptors of the map's keyframes live in HBM; the candidate
 // loop of PlaceRecognitionG::ComputeSE3 (placerec_gen_be.cpp:60-135) becomes one call per query keyframe.  The database
 // index of a keyframe is its insertion order; keep it next to the keyframe (e.g. std::map<idpair, int>).

@@ -5,6 +5,7 @@ the C-ABI:
   score_absolute_pose(...)      ↔ FrameAbsolutePoseSacProblem scoring   (FrameAbsolutePoseSacProblem.h:95-126; Se3Solver GP3P RANSAC)
   score_relative_pose(...)      ↔ FrameRelativePoseSacProblem scoring   (frame-relative-pose-sac-problem.hpp:69-104)
   ransac_select(...)            ↔ the model-selection rule of opengv::sac::Ransac::computeModel replayed over batched scores
+  ransac_absolute_pose(...)     ↔ the whole GP3P RANSAC of Se3Solver::projectiveAlignment from caller-supplied samples
 
 `KfView` flattens what the reference reads of a Keyframe (the C++ shim does the same from the containers)."""
 from __future__ import annotations
@@ -161,3 +162,36 @@ def ransac_select(n_inliers, n_points, sample_size, max_iterations, probability=
             k = log_p / np.log(pno)
         it += 1
     return best, it
+
+
+class CAbsRansacProblems(C.Structure):
+    _fields_ = [("n_prob", C.c_int32)] + [(k, c_vp) for k in ("prob_ptr", "pts", "f", "sigma", "cam_off", "cam_rot", "samples")] + \
+               [("n_samples", C.c_int32)]
+
+
+class CAbsRansacResult(C.Structure):
+    _fields_ = [(k, c_vp) for k in ("best_sample", "best_model", "best_count", "iterations", "consumed", "inlier_mask", "sample_model",
+                                    "sample_valid", "sample_count")]
+
+
+def ransac_absolute_pose(ctx: Context, prob_ptr, pts, bearings, sigma, cam_off, cam_rot, samples, threshold, max_iterations, probability=0.99,
+                         per_sample=False):
+    """Se3Solver::projectiveAlignment's GP3P RANSAC for a batch of problems (cvb_ransac_absolute_pose_batch): P3P hypothesis per sample,
+    scoring and ransac_select-style selection on the GPU.  prob_ptr [n_prob+1] correspondence ranges; pts / bearings [N,3], sigma [N];
+    cam_off [n_prob,3], cam_rot [n_prob,3,3] (camera in the body frame); samples [n_prob, n_samples, 4] problem-local indices.
+    → dict(best_sample, best_model [n_prob,3,4], best_count, iterations, consumed, inlier_mask [N]) and, with per_sample,
+    sample_model [n_prob,n_samples,3,4], sample_valid, sample_count."""
+    ptr = np.ascontiguousarray(prob_ptr, np.int32); n_prob = len(ptr) - 1
+    p = np.ascontiguousarray(pts, np.float64).reshape(-1, 3); f = np.ascontiguousarray(bearings, np.float64).reshape(-1, 3)
+    s = np.ascontiguousarray(sigma, np.float64).reshape(-1)
+    co = np.ascontiguousarray(cam_off, np.float64).reshape(n_prob, 3); cr = np.ascontiguousarray(cam_rot, np.float64).reshape(n_prob, 9)
+    smp = np.ascontiguousarray(samples, np.int32).reshape(n_prob, -1, 4); ns = smp.shape[1]
+    r = dict(best_sample=np.zeros(n_prob, np.int32), best_model=np.zeros((n_prob, 3, 4)), best_count=np.zeros(n_prob, np.int32),
+             iterations=np.zeros(n_prob, np.int32), consumed=np.zeros(n_prob, np.int32), inlier_mask=np.zeros(len(p), np.uint8))
+    if per_sample:
+        r.update(sample_model=np.zeros((n_prob, ns, 3, 4)), sample_valid=np.zeros((n_prob, ns), np.uint8),
+                 sample_count=np.zeros((n_prob, ns), np.int32))
+    P = CAbsRansacProblems(n_prob, ptr.ctypes.data, p.ctypes.data, f.ctypes.data, s.ctypes.data, co.ctypes.data, cr.ctypes.data, smp.ctypes.data, ns)
+    R = CAbsRansacResult(*[r[k].ctypes.data if k in r else None for k, _ in CAbsRansacResult._fields_])
+    ctx.check(lib().cvb_ransac_absolute_pose_batch(ctx.handle, C.byref(P), float(threshold), int(max_iterations), float(probability), C.byref(R)))
+    return r

@@ -298,6 +298,61 @@ CVB_API int cvb_score_relative_pose_batch(cvb_ctx* ctx, const double* model, int
                                           double* scores, uint8_t* inlier, int32_t* n_inliers);
 
 /*
+ * The whole absolute-pose RANSAC of Se3Solver::projectiveAlignment (GP3P, Se3Solver.cpp:59-110) for a batch of problems
+ * (candidate keyframes) in one launch, from the caller's samples: minimal solve, hypothesis choice, scoring, the sequential
+ * model selection of opengv's Ransac::computeModel and the inlier mask of the selected model.  Samples stay an input
+ * (opengv's random number generator cannot be reproduced, SURVEY §8c).
+ *   Hypothesis of a sample: P3P (Lambda Twist) on its first three correspondences; the solutions with positive depth for all
+ *   three points, as body-in-world models [R|t] (the scoring's convention); the one whose predicted direction of the fourth
+ *   point has the smallest 1 - cos angle to its bearing (strict <: the first of equal values wins).  A sample is invalid (no
+ *   hypothesis) if no solution survives, a value is non-finite, an index repeats within the sample or the problem has fewer
+ *   than 4 correspondences.  With one camera per problem the three rays share a centre, so GP3P's solution set is P3P's.
+ *   ASSUMPTION (opengv is not in the tree): sample size 4 and the fourth-point choice follow opengv's AbsolutePoseSacProblem.
+ *   Score: exactly cvb_score_absolute_pose_batch's per-correspondence score (the same device function), inlier iff
+ *   score < threshold.
+ *   Selection: samples are consumed in order; an invalid sample does not consume an iteration (ASSUMPTION: opengv's
+ *   skipped_count, at most 10 * max_iterations skips); valid hypotheses go through covins_b200.placerec.ransac_select with
+ *   sample_size 4 — the result equals ransac_select over the inlier counts of the valid samples in order, mapped back to
+ *   sample indices.  w^4 is computed as plain products and log on the device: the adaptive bound can differ from a host
+ *   evaluation (pow / glibc log) by an ulp, which only matters when it lands within an ulp of an integer.
+ * Inputs: correspondences concatenated over problems (prob_ptr[n_prob+1], prob_ptr[0] = 0): world point pts[i], unit bearing
+ * f[i], sigma[i] as in cvb_score_absolute_pose_batch; one camera per problem, cam_off [n_prob][3], cam_rot [n_prob][9]
+ * (row-major, in the body frame); samples [n_prob][n_samples][4], indices local to their problem (checked against the
+ * problem's size; the samples of a problem with fewer than 4 correspondences are not read).
+ * Outputs per problem: best_sample (-1 = none), best_model [12] (zeros if none), best_count, iterations (valid samples
+ * scored by the selection), consumed (samples read by the selection).  inlier_mask [N] (nullable): the selected model's
+ * inlier flags, 0 where there is none.  sample_model [n_prob][n_samples][12] / sample_valid / sample_count (nullable
+ * together, for tests): every sample's hypothesis (zeros if invalid) and inlier count — when requested, every sample is
+ * solved and scored, not only the consumed ones.
+ * Errors: CVB_ERR_INVALID for negative sizes, null required pointers or an out-of-range index, before any launch;
+ * n_prob = 0 succeeds.
+ */
+typedef struct cvb_abs_ransac_problems {
+  int32_t n_prob;
+  const int32_t* prob_ptr;   /* [n_prob+1] */
+  const double* pts;         /* [N][3] world points */
+  const double* f;           /* [N][3] unit bearings, camera frame */
+  const double* sigma;       /* [N] getSigmaAngle(i) */
+  const double* cam_off;     /* [n_prob][3] camera offset c in the body frame */
+  const double* cam_rot;     /* [n_prob][9] camera rotation Rc in the body frame, row-major */
+  const int32_t* samples;    /* [n_prob][n_samples][4] */
+  int32_t n_samples;
+} cvb_abs_ransac_problems;
+typedef struct cvb_abs_ransac_result {
+  int32_t* best_sample;      /* [n_prob] */
+  double* best_model;        /* [n_prob][12] 3x4 [R|t] row-major, body in world */
+  int32_t* best_count;       /* [n_prob] */
+  int32_t* iterations;       /* [n_prob] */
+  int32_t* consumed;         /* [n_prob] */
+  uint8_t* inlier_mask;      /* [N] nullable */
+  double* sample_model;      /* [n_prob][n_samples][12] nullable */
+  uint8_t* sample_valid;     /* [n_prob][n_samples]     nullable */
+  int32_t* sample_count;     /* [n_prob][n_samples]     nullable */
+} cvb_abs_ransac_result;
+CVB_API int cvb_ransac_absolute_pose_batch(cvb_ctx* ctx, const cvb_abs_ransac_problems* p, double threshold, int max_iterations,
+                                           double probability, cvb_abs_ransac_result* r);
+
+/*
  * Optimization::OptimizeRelativePose(kf1, kf2, matches1, T12, th2) (optimization_be.cpp:620-831): the 6-dof refinement of
  * the relative pose T12 from the matched landmark pairs, both ceres::Solve calls (5 + 5 iterations, DOGLEG, CauchyLoss(1))
  * and the outlier purge between them, in one call.  The caller (shim) flattens, per residual pair r (the reference's
