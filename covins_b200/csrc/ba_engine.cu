@@ -1413,7 +1413,7 @@ int engine_setup(Engine& E, const cvb_ba_problem* p, const cvb_ba_options* o) {
   std::vector<uint8_t> pre_fill(tmask);
   // the replicated plan (every rank applies every update); cvb_ba_enable_p2p swaps in the owner-filtered one — same tile
   // structure, same packed layout — once peer access is known to work on every rank
-  E.plan.build(nt, tmask);
+  E.plan.build(nt, tmask, col_group);
   E.h_prefill = pre_fill;
   E.h_owner = h_owner;
   E.n_tiles = (size_t)E.plan.n_tiles_L;
@@ -1427,7 +1427,6 @@ int engine_setup(Engine& E, const cvb_ba_problem* p, const cvb_ba_options* o) {
       }
   E.n_xt_all = (int)h_xt_all.size();
   E.n_xt_own = (int)h_xt_own.size();
-  E.plan.h_col_group = col_group;
   lap("tile structure + plan");
   // ---- by-keyframe CSR ----
   std::vector<int> h_kf_ptr(K + 1, 0), h_kf_obs(E.n_obs);
@@ -2202,12 +2201,8 @@ int cvb_ba_enable_p2p(cvb_ba* h) {
   ENG_CUDA(cudaMemcpyAsync(E.d_peer_S, dv.peer_S, sizeof(double*) * 16, cudaMemcpyHostToDevice, E.st));
   ENG_CUDA(cudaStreamSynchronize(E.st));
   // distributed plan: same structure, pair lists restricted to the tile columns this rank owns
-  {
-    const std::vector<int> groups = E.plan.h_col_group;
-    E.plan.build(E.plan.nt, E.h_prefill, &E.h_owner, E.rank);
-    E.plan.h_col_group = groups;
-    if ((rc = E.plan.upload(E.ctx, E.st))) return rc;
-  }
+  E.plan.build(E.plan.nt, E.h_prefill, E.plan.h_col_group, &E.h_owner, E.rank);
+  if ((rc = E.plan.upload(E.ctx, E.st))) return rc;
   E.dv = dv;
   E.p2p = true;
   return CVB_OK;

@@ -13,7 +13,8 @@
 // Right-looking, panel width 128:
 //   potrf_inv_kernel   1 CTA: factor the 128x128 diagonal tile in shared memory, write L, write L^-1
 //   trsm_kernel        row tiles below: A(i,k) <- A(i,k) * Linv^T            (128^3 DMMA GEMM per CTA)
-//   syrk_kernel        trailing tiles (i >= j > k): A(i,j) -= A(i,k) A(j,k)^T (128^3 DMMA GEMM per CTA)
+//   syrk_kernel        trailing tiles (i >= j > k): A(i,j) -= A(i,k) A(j,k)^T (128^3 DMMA GEMM per CTA and panel; in
+//                      blocks of kPanelBlock columns, all of a block's panels per visit to a tile — see factor())
 // Solves use the stored tile inverses: forward L y = b, backward L^T x = y, one launch per tile column.
 // All reductions have a fixed order → bit-reproducible run to run.
 #include "cholesky.cuh"
@@ -183,35 +184,47 @@ __global__ void __launch_bounds__(T, 1) chain_gemm_kernel(double* __restrict__ C
   }
 }
 
-// A(i,j) -= A(i,k) A(j,k)^T for the tile pairs (i >= j) of column k's non-zero rows: pi[]/pj[] enumerate them.
-// Four CTAs per pair, one 64x64 quadrant each (consecutive CTAs share the pair's operands in L2); the quadrant above
-// the diagonal of a diagonal tile is skipped.
+// A(i,j) -= A(i,k) A(j,k)^T for the tile pairs (i >= j) pi[]/pj[] and the panels k = k0 + q of the bits q of pmask[]
+// (TilePlan::h_pair_mask), in increasing k, each panel's product subtracted on its own.  Four CTAs per pair, one 64x64
+// quadrant each (consecutive CTAs share the pair's operands in L2); the quadrant above the diagonal of a diagonal tile is
+// skipped.  The quadrant (32 KB) is fetched into L2 at the start, so the first epilogue does not wait on HBM, and stays
+// there for the read-modify-write of the later panels: several panels per visit make one HBM round trip of C.
 __global__ void __launch_bounds__(SYRK_THREADS, 3) syrk_kernel(double* __restrict__ S, const int* __restrict__ tile_of, int nt,
-                                                                int k, const int* __restrict__ pi, const int* __restrict__ pj) {
+                                                                int k0, const int* __restrict__ pi, const int* __restrict__ pj,
+                                                                const int* __restrict__ pmask) {
   extern __shared__ __align__(16) double smem_d[];
   constexpr size_t ld = T;
   const int p = blockIdx.x >> 2, qr = (blockIdx.x >> 1) & 1, qc = blockIdx.x & 1;
   const int i = pi[p], j = pj[p];
   if (i == j && qc > qr) return;
-  const double* Ai = S + (size_t)tile_of[(size_t)i * nt + k] * TT + (size_t)qr * 64 * T;
-  const double* Aj = S + (size_t)tile_of[(size_t)j * nt + k] * TT + (size_t)qc * 64 * T;
   double* C = S + (size_t)tile_of[(size_t)i * nt + j] * TT + (size_t)qr * 64 * T + qc * 64;
-  double acc[2][4][4];
-  gemm_abt_64<64>(Ai, ld, Aj, ld, acc, smem_d);
+#pragma unroll
+  for (int u = threadIdx.x; u < 64 * 4; u += SYRK_THREADS)   // 64 rows x 4 lines of 128 B
+    asm volatile("prefetch.global.L2 [%0];" ::"l"(C + (size_t)(u >> 2) * ld + (u & 3) * 16));
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, wm = warp >> 1, wn = warp & 1;
+  unsigned mask = (unsigned)pmask[p];
+#pragma unroll 1
+  for (int k = k0; mask != 0; k++, mask >>= 1) {
+    if (!(mask & 1u)) continue;
+    const double* Ai = S + (size_t)tile_of[(size_t)i * nt + k] * TT + (size_t)qr * 64 * T;
+    const double* Aj = S + (size_t)tile_of[(size_t)j * nt + k] * TT + (size_t)qc * 64 * T;
+    double acc[2][4][4];
+    __syncthreads();   // every warp is done with the previous panel's last stages before the prologue refills them
+    gemm_abt_64<64>(Ai, ld, Aj, ld, acc, smem_d);
 #pragma unroll
-  for (int a = 0; a < 2; a++)
+    for (int a = 0; a < 2; a++)
 #pragma unroll
-    for (int b = 0; b < 4; b++)
+      for (int b = 0; b < 4; b++)
 #pragma unroll
-      for (int h = 0; h < 2; h++) {
-        const int r = wm * 32 + a * 16 + h * 8 + (lane >> 2), c = wn * 32 + b * 8 + (lane & 3) * 2;
-        double2* q = reinterpret_cast<double2*>(C + (size_t)r * ld + c);
-        double2 v = *q;
-        v.x -= acc[a][b][2 * h];
-        v.y -= acc[a][b][2 * h + 1];
-        *q = v;
-      }
+        for (int h = 0; h < 2; h++) {
+          const int r = wm * 32 + a * 16 + h * 8 + (lane >> 2), c = wn * 32 + b * 8 + (lane & 3) * 2;
+          double2* q = reinterpret_cast<double2*>(C + (size_t)r * ld + c);
+          double2 v = *q;
+          v.x -= acc[a][b][2 * h];
+          v.y -= acc[a][b][2 * h + 1];
+          *q = v;
+        }
+  }
 }
 
 // Factor the diagonal tile k in shared memory and invert the factor, one CTA of 512 threads.  This kernel is the serial
@@ -564,37 +577,79 @@ __global__ void __launch_bounds__(SOLVE_THREADS) bwd_kernel(const double* __rest
 
 // Symbolic phase (host): tile-level structure of L from the tile-level structure of S (lower, nt x nt, row-major
 // bools, diagonal forced).  Right-looking elimination: the non-zero rows of column k become a clique.
-void TilePlan::build(int nt_, std::vector<uint8_t> mask, const std::vector<int>* owner, int rank) {
+void TilePlan::build(int nt_, std::vector<uint8_t> mask, std::vector<int> col_group, const std::vector<int>* owner, int rank) {
   nt = nt_;
   my_rank = rank;
+  h_col_group = std::move(col_group);
   h_owner.clear();
   if (owner) h_owner = *owner;
   const bool dist = !h_owner.empty();
-  h_col_ptr.assign(1, 0); h_row_idx.clear(); h_pair_ptr.assign(1, 0); h_pair_i.clear(); h_pair_j.clear(); h_pair_split.clear();
+  h_col_ptr.assign(1, 0); h_row_idx.clear();
   for (int k = 0; k < nt; k++) mask[(size_t)k * nt + k] = 1;
-  double n_trsm = 0.0;
+  // Distributed: the structure (fill) is the global one, but a rank executes only the updates of the columns it owns.
+  double n_trsm = 0.0, n_upd = 0.0;
   for (int k = 0; k < nt; k++) {
     std::vector<int> rows;
     for (int i = k + 1; i < nt; i++)
       if (mask[(size_t)i * nt + k]) rows.push_back(i);
     if (!dist || h_owner[k] == rank) n_trsm += (double)rows.size();
-    // pairs whose column tile is k+1 first ("panel" part: all the next step's potrf/trsm depend on), then the rest.
-    // Distributed: the structure (fill) is the global one, but a rank lists only the pairs of the columns it owns.
-    int n_a = 0;
-    for (int pass = 0; pass < 2; pass++)
-      for (size_t a = 0; a < rows.size(); a++)
-        for (size_t b = 0; b <= a; b++) {
-          const bool is_a = rows[b] == k + 1;
-          if ((pass == 0) != is_a) continue;
-          mask[(size_t)rows[a] * nt + rows[b]] = 1;
-          if (dist && h_owner[rows[b]] != rank) continue;
-          h_pair_i.push_back(rows[a]);
-          h_pair_j.push_back(rows[b]);
-          if (is_a) n_a++;
-        }
-    h_pair_split.push_back(n_a);
+    for (size_t a = 0; a < rows.size(); a++)
+      for (size_t b = 0; b <= a; b++) {
+        mask[(size_t)rows[a] * nt + rows[b]] = 1;
+        if (!dist || h_owner[rows[b]] == rank) n_upd += 1.0;
+      }
     h_row_idx.insert(h_row_idx.end(), rows.begin(), rows.end());
     h_col_ptr.push_back((int)h_row_idx.size());
+  }
+  // Blocks: runs of up to kPanelBlock consecutive main-sequence columns.  Width 1 for the column groups (pure latency
+  // chains with tiny updates: nothing to amortise, and their updates stay off the bulk stream) and for the distributed
+  // factorisation (its owner map, flags and peer copies hand over one column at a time).
+  const auto in_group = [&](int k) { return !h_col_group.empty() && h_col_group[k] >= 0; };
+  h_blk_end.assign(nt, 0);
+  for (int k0 = 0; k0 < nt;) {
+    int k1 = k0 + 1;
+    if (!dist && !in_group(k0))
+      while (k1 < nt && k1 - k0 < kPanelBlock && !in_group(k1)) k1++;
+    for (int k = k0; k < k1; k++) h_blk_end[k] = k1;
+    k0 = k1;
+  }
+  // Launch lists.  Per target column: the next block's columns go on the work stream (the first of them first: the next
+  // panel solve needs it), the rest on the bulk stream; the column groups put all their updates on the work stream.
+  h_pair_ptr.assign(1, 0); h_pair_i.clear(); h_pair_j.clear(); h_pair_mask.clear(); h_pair_k0.clear(); h_pair_split.clear();
+  const auto tile = [&](int i, int j) { return mask[(size_t)i * nt + j] != 0; };
+  for (int k = 0; k < nt; k++) {
+    // panels [p_lo, k] onto the target columns [j_lo, nt) at a block's last column, panel k onto (k, k1) inside a block
+    const int k1 = h_blk_end[k];
+    const bool last = k1 == k + 1;
+    int p_lo = k;
+    if (last)
+      while (p_lo > 0 && h_blk_end[p_lo - 1] == k1) p_lo--;
+    const int j_lo = last ? k1 : k + 1, j_end = last ? nt : k1;
+    const int j_work = in_group(k) ? nt : (last && k1 < nt ? h_blk_end[k1] : k1);   // target columns < j_work: work stream
+    std::vector<int> rows;   // rows >= j_lo of the panels: the targets' rows and columns
+    for (int p = p_lo; p <= k; p++)
+      for (int q = h_col_ptr[p]; q < h_col_ptr[p + 1]; q++)
+        if (h_row_idx[q] >= j_lo && h_row_idx[q] < nt) rows.push_back(h_row_idx[q]);
+    std::sort(rows.begin(), rows.end());
+    rows.erase(std::unique(rows.begin(), rows.end()), rows.end());
+    int n_work = 0;
+    for (size_t b = 0; b < rows.size(); b++) {   // target column j = rows[b] (ascending: the first work column first)
+      const int j = rows[b];
+      if (j >= j_end || (dist && h_owner[j] != rank)) continue;
+      for (size_t a = b; a < rows.size(); a++) {
+        const int i = rows[a];
+        int m = 0;
+        for (int p = p_lo; p <= k; p++)   // (p+1, p+1) with panel p is the chain's product
+          if (tile(i, p) && tile(j, p) && !(i == p + 1 && j == p + 1)) m |= 1 << (p - p_lo);
+        if (!m) continue;
+        h_pair_i.push_back(i);
+        h_pair_j.push_back(j);
+        h_pair_mask.push_back(m);
+        if (j < j_work) n_work++;
+      }
+    }
+    h_pair_k0.push_back(p_lo);
+    h_pair_split.push_back(n_work);
     h_pair_ptr.push_back((int)h_pair_i.size());
   }
   h_rowc_ptr.assign(1, 0); h_rowc_idx.clear();
@@ -613,8 +668,8 @@ void TilePlan::build(int nt_, std::vector<uint8_t> mask, const std::vector<int>*
     h_tile_of[(size_t)k * nt + k] = next++;
     for (int q = h_col_ptr[k]; q < h_col_ptr[k + 1]; q++) h_tile_of[(size_t)h_row_idx[q] * nt + k] = next++;
   }
-  // flops this rank executes: one 128^3 GEMM (2 flop per MAC) per trsm tile and per syrk pair
-  flops = 2.0 * T * T * T * (n_trsm + (double)h_pair_i.size());
+  // flops this rank executes: one 128^3 GEMM (2 flop per MAC) per trsm tile and per (target tile, panel) update
+  flops = 2.0 * T * T * T * (n_trsm + n_upd);
 }
 
 int TilePlan::upload(cvb_ctx* ctx, cudaStream_t st) {
@@ -627,7 +682,7 @@ int TilePlan::upload(cvb_ctx* ctx, cudaStream_t st) {
   };
   int rc;
   if ((rc = up(&d_row_idx, h_row_idx)) || (rc = up(&d_pair_i, h_pair_i)) || (rc = up(&d_pair_j, h_pair_j)) ||
-      (rc = up(&d_rowc_idx, h_rowc_idx)) || (rc = up(&d_tile_of, h_tile_of)))
+      (rc = up(&d_pair_mask, h_pair_mask)) || (rc = up(&d_rowc_idx, h_rowc_idx)) || (rc = up(&d_tile_of, h_tile_of)))
     return rc;
   CVB_CUDA(ctx, cudaStreamSynchronize(st));
   return CVB_OK;
@@ -637,9 +692,10 @@ void TilePlan::release() {
   if (d_row_idx) cudaFree(d_row_idx);
   if (d_pair_i) cudaFree(d_pair_i);
   if (d_pair_j) cudaFree(d_pair_j);
+  if (d_pair_mask) cudaFree(d_pair_mask);
   if (d_rowc_idx) cudaFree(d_rowc_idx);
   if (d_tile_of) cudaFree(d_tile_of);
-  d_row_idx = d_pair_i = d_pair_j = d_rowc_idx = d_tile_of = nullptr;
+  d_row_idx = d_pair_i = d_pair_j = d_pair_mask = d_rowc_idx = d_tile_of = nullptr;
 }
 
 int FactorStreams::create(cvb_ctx* ctx, int nt) {
@@ -736,9 +792,13 @@ int factor(cvb_ctx* ctx, double* S, double* linv, int* d_flag, const TilePlan& p
   cudaStream_t st2 = fs.bulk;
   const std::vector<cudaEvent_t>& ev = fs.ev;
   const int n_gs = plan.h_col_group.empty() ? 0 : fs.n_group;
-  // Lookahead (depth 1): the diagonal-tile kernel and the panel solve of step k+1 only need the "panel" part of step k's
-  // trailing update (pairs in tile column k+1); the bulk of the update runs on the second (low-priority) stream
-  // concurrently.  ev[5k] = panel of step k available, ev[5k+1] = bulk update done.
+  // Blocked trailing update (TilePlan::h_blk_end): inside a block of kPanelBlock main-sequence columns each panel updates
+  // only the block's own columns; after the block's last panel one pass applies all of its panels to every tile past the
+  // block.  Lookahead (depth 1 block): the next block's steps only need the part of that pass on the next block's columns
+  // (the work stream; the first of them first); the bulk of the pass runs on the second (low-priority) stream
+  // concurrently.  The bulk writes the tiles past the next block only, so the one thing that waits for it is the first
+  // use of those tiles: the next block's own pass and its last chain step.  ev[5k] = panel of step k available,
+  // ev[5k+1] = bulk update of step k done.
   // Independent column groups (the IMU chains of different agents, see TilePlan::h_col_group) run on their own
   // streams: their tile columns are pure latency chains (diagonal tile → panel → tiny update) that do not share tiles.
   // Distributed: "panel available" = factored here (owner) or pulled from the owner's memory (everyone else).
@@ -818,23 +878,30 @@ int factor(cvb_ctx* ctx, double* S, double* linv, int* d_flag, const TilePlan& p
     cudaStream_t cs = is_grp ? fs.group[gi] : sf;        // chain stream of this column
     cudaStream_t ws = is_grp ? fs.group_aux[gi] : st;    // its work stream (rest of the panel, tile column k+1)
     int& pc = is_grp ? prev_chain_g[gi] : prev_chain;     // previous chain column of this sequence
-    const int lb = is_grp ? -1 : last_bulk;               // column groups have no bulk stream: all their updates are small
+    // the bulk is waited for at a block's last column only (column groups have no bulk stream: all their updates are small)
+    const bool blk_last = plan.h_blk_end[k] == k + 1;
+    const int lb = is_grp || !blk_last ? -1 : last_bulk;
     const bool has_next = m > 0 && plan.h_row_idx[plan.h_col_ptr[k]] == k + 1;
+    // tile (k+1,k+1) gets panel k from the chain when this rank applies the updates of column k+1
     const bool mine_n = has_next && (!dist || plan.h_owner[k + 1] == dv->rank);
-    // does the pair list start with the diagonal pair (k+1, k+1)?  (owner-filtered lists hold it only when column k+1 is ours)
-    const int na = is_grp ? np : plan.h_pair_split[k];
-    const bool diag_pair = has_next && np > 0 && plan.h_pair_i[p0] == k + 1 && plan.h_pair_j[p0] == k + 1;
-    // A. tile (k,k) is final: column k-1's contribution came with the chain, the bulk updates of the columns <= k-2 were
-    //    waited for by the previous chain step (below) — nothing to wait for here
+    const int na = plan.h_pair_split[k];
+    const int k0 = plan.h_pair_k0[k];
+    // a list that starts with (k+1,k+1) (at a block's last column) holds the block's earlier panels for it: they go on the
+    // chain stream, before the chain's own product and potrf(k+1)
+    const bool diag_pair = np > 0 && plan.h_pair_i[p0] == k + 1 && plan.h_pair_j[p0] == k + 1;
+    // A. tile (k,k) is final: column k-1's contribution came with the chain, the others were waited for by the previous
+    //    chain step (below) — nothing to wait for here
     if (mine) {
       potrf_inv_kernel<<<1, POTRF_THREADS, kPotrfSmem, cs>>>(diag, (size_t)T, 0, linv_k, d_flag, nullptr, 0);
       CVB_CHECK_LAUNCH(ctx);
     }
     CVB_CUDA(ctx, cudaEventRecord(evP, cs));
     if (tr) cudaEventRecord(tev[(size_t)k * 5 + 1], cs);
-    // C. tile (k+1,k): final once column k-1's updates of tile column k are done (evA of the previous chain column)
+    // C. tile (k+1,k): final once column k-1's updates of tile column k are done (evA of the previous chain column).
+    //    Inside a block the work stream also updates tile (k+1,k+1) (panels before k): the same wait orders potrf(k+1)
+    //    after those.
+    if (pc >= 0) CVB_CUDA(ctx, cudaStreamWaitEvent(cs, ev[5 * pc + 4], 0));
     if (has_next) {
-      if (pc >= 0) CVB_CUDA(ctx, cudaStreamWaitEvent(cs, ev[5 * pc + 4], 0));
       if (mine) {
         chain_gemm_kernel<0><<<T / CHAIN_ROWS, T, kChainSmem, cs>>>(diag + TT, diag + TT, linv_k);
         CVB_CHECK_LAUNCH(ctx);
@@ -849,10 +916,16 @@ int factor(cvb_ctx* ctx, double* S, double* linv, int* d_flag, const TilePlan& p
                                       cudaMemcpyDeviceToDevice, cs));
       }
     }
-    // the bulk update of the previous column also writes tile (k+1,k+1) (and everything the next chain step reads): it has
-    // to be complete before the diagonal pair is applied / before potrf(k+1) — the depth-1 lookahead rule
+    // at a block's last column, the previous block's bulk update also writes tile (k+1,k+1) (and everything the next
+    // chain step reads): it has to be complete before the diagonal pair is applied / before potrf(k+1) — the depth-1
+    // lookahead rule
     if (lb >= 0) CVB_CUDA(ctx, cudaStreamWaitEvent(cs, ev[5 * lb + 1], 0));
     if (diag_pair) {
+      syrk_kernel<<<4, SYRK_THREADS, kSyrkSmem, cs>>>(S, plan.d_tile_of, nt, k0, plan.d_pair_i + p0, plan.d_pair_j + p0,
+                                                       plan.d_pair_mask + p0);
+      CVB_CHECK_LAUNCH(ctx);
+    }
+    if (mine_n) {
       chain_gemm_kernel<1><<<T / CHAIN_ROWS, T, kChainSmem, cs>>>(S + (size_t)plan.h_col_base[k + 1] * TT, diag + TT, diag + TT);
       CVB_CHECK_LAUNCH(ctx);
     }
@@ -886,19 +959,23 @@ int factor(cvb_ctx* ctx, double* S, double* linv, int* d_flag, const TilePlan& p
       CVB_CUDA(ctx, cudaMemcpyAsync(linv_k, dv->peer_linv[o] + (size_t)k * TT, TT * sizeof(double), cudaMemcpyDeviceToDevice, ws));
       CVB_CUDA(ctx, cudaStreamWaitEvent(ws, evD, 0));
     }
-    // E. tile column k+1 (minus the diagonal pair), then "panel k available" for the bulk stream
-    if (m > 0) {
+    // E. the work stream's part of the update list (the next block's columns, minus the diagonal pair), then "panel k
+    //    available" for the bulk stream.  (At a block's last column the list holds all of the block's panels, so it can
+    //    be non-empty for a column without rows.)
+    if (np > 0) {
       CVB_CUDA(ctx, cudaEventRecord(evPanel, ws));
       if (lb >= 0) CVB_CUDA(ctx, cudaStreamWaitEvent(ws, ev[5 * lb + 1], 0));
       const int a0 = diag_pair ? 1 : 0;
       if (na - a0 > 0) {
-        syrk_kernel<<<4 * (na - a0), SYRK_THREADS, kSyrkSmem, ws>>>(S, plan.d_tile_of, nt, k, plan.d_pair_i + p0 + a0, plan.d_pair_j + p0 + a0);
+        syrk_kernel<<<4 * (na - a0), SYRK_THREADS, kSyrkSmem, ws>>>(S, plan.d_tile_of, nt, k0, plan.d_pair_i + p0 + a0,
+                                                                     plan.d_pair_j + p0 + a0, plan.d_pair_mask + p0 + a0);
         CVB_CHECK_LAUNCH(ctx);
       }
       if (tr) cudaEventRecord(tev[(size_t)k * 5 + 3], ws);
       if (np - na > 0) {
         CVB_CUDA(ctx, cudaStreamWaitEvent(st2, evPanel, 0));
-        syrk_kernel<<<4 * (np - na), SYRK_THREADS, kSyrkSmem, st2>>>(S, plan.d_tile_of, nt, k, plan.d_pair_i + p0 + na, plan.d_pair_j + p0 + na);
+        syrk_kernel<<<4 * (np - na), SYRK_THREADS, kSyrkSmem, st2>>>(S, plan.d_tile_of, nt, k0, plan.d_pair_i + p0 + na,
+                                                                       plan.d_pair_j + p0 + na, plan.d_pair_mask + p0 + na);
         CVB_CHECK_LAUNCH(ctx);
         CVB_CUDA(ctx, cudaEventRecord(evBulk, st2));
         if (tr) cudaEventRecord(tev[(size_t)k * 5 + 4], st2);
@@ -918,7 +995,9 @@ int factor(cvb_ctx* ctx, double* S, double* linv, int* d_flag, const TilePlan& p
     cudaStreamSynchronize(st);
     FILE* f = fopen(trace_path, "w");
     if (f) {
-      fprintf(f, "k,group,owner,n_rows,n_pairs,n_panel_pairs,t_start_us,t_panel_ready_us,t_trsm_us,t_syrk_a_us,t_bulk_us\n");
+      // n_pairs / n_work_pairs: pairs of column k's update list / of its work-stream part; t_bulk_us: end of the bulk
+      // update launched at column k (a block's last column), -1 if none
+      fprintf(f, "k,group,owner,n_rows,n_pairs,n_work_pairs,t_start_us,t_panel_ready_us,t_trsm_us,t_syrk_a_us,t_bulk_us\n");
       for (int k = 0; k < nt; k++) {
         float t[5];
         for (int e = 0; e < 5; e++) {

@@ -7,13 +7,25 @@
 namespace cvb_chol {
 
 constexpr int T = 128;  // tile edge
+// Width of the outer block of the main sequence: the trailing update of the tiles past a block applies all of the block's
+// panels in one visit to each tile (one C round trip to HBM per block instead of per panel).
+constexpr int kPanelBlock = 2;
 
 // Tile-level structure of the factor: which 128x128 tiles of L are structurally non-zero, as launch lists.
 struct TilePlan {
   int nt = 0;
   std::vector<int> h_col_ptr, h_row_idx;           // per tile column k: non-zero row tiles i > k
-  std::vector<int> h_pair_ptr, h_pair_i, h_pair_j; // per tile column k: (i >= j) pairs of those rows (trailing updates)
-  std::vector<int> h_pair_split;                   // per tile column k: how many of its pairs (listed first) lie in tile column k+1
+  // Trailing-update launch lists, issued after the panel of tile column k is solved: pairs (i >= j) of target tiles with
+  // the panels each one receives, bit q of h_pair_mask = panel h_pair_k0[k] + q (the panel tiles (i,k') and (j,k') both
+  // exist).  Width 1 (h_blk_end[k] == k + 1 and h_pair_k0[k] == k): the pairs of panel k.  Inside a block of
+  // kPanelBlock columns: panel k alone, on the targets inside the block.  At a block's last column: all of the block's
+  // panels on every target past the block.  The product S(k+1,k+1) -= L(k+1,k) L(k+1,k)^T is never listed: the chain
+  // (factor()) computes it.
+  std::vector<int> h_pair_ptr, h_pair_i, h_pair_j, h_pair_mask;
+  std::vector<int> h_pair_k0;                      // per tile column k: panel of mask bit 0
+  std::vector<int> h_pair_split;                   // per tile column k: how many of its pairs (listed first) go on the work
+                                                   // stream (the next block's columns); the rest go on the bulk stream
+  std::vector<int> h_blk_end;                      // per tile column k: one past the last column of its block
   std::vector<int> h_rowc_ptr, h_rowc_idx;         // per tile row k: non-zero column tiles i < k (backward solve)
   std::vector<int> h_col_group;                    // optional, per tile column: id (>= 0) of an independent column group
                                                    // (its columns share no tile with other groups), -1 = main sequence
@@ -25,11 +37,14 @@ struct TilePlan {
   // single GPU).  With an owner map the pair lists hold only the pairs whose TARGET column this rank owns.
   std::vector<int> h_owner;
   int my_rank = 0;
-  int *d_row_idx = nullptr, *d_pair_i = nullptr, *d_pair_j = nullptr, *d_rowc_idx = nullptr, *d_tile_of = nullptr;
+  int *d_row_idx = nullptr, *d_pair_i = nullptr, *d_pair_j = nullptr, *d_pair_mask = nullptr, *d_rowc_idx = nullptr,
+      *d_tile_of = nullptr;
   long n_tiles_L = 0;
   double flops = 0.0;   // flops of one numeric factorisation with this plan
-  // owner (optional, nt entries) + rank: distributed plan.  flops = the tile GEMMs this rank executes.
-  void build(int nt, std::vector<uint8_t> lower_mask, const std::vector<int>* owner = nullptr, int rank = 0);
+  // col_group (optional, nt entries): h_col_group.  owner (optional, nt entries) + rank: distributed plan.  flops = the
+  // tile GEMMs this rank executes.
+  void build(int nt, std::vector<uint8_t> lower_mask, std::vector<int> col_group = {}, const std::vector<int>* owner = nullptr,
+             int rank = 0);
   size_t tile_index(int i, int j) const { return (size_t)h_tile_of[(size_t)i * nt + j]; }
   int upload(cvb_ctx* ctx, cudaStream_t st);
   void release();
