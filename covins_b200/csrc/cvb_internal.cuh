@@ -23,7 +23,7 @@ struct cvb_ctx {
   int64_t launches = 0;
   std::string err;
   // grow-only device workspaces (named slots so independent stages never alias)
-  cvb_buf ws[26];
+  cvb_buf ws[27];   // one per WS_* slot below
   // pinned host staging
   void* h_pin = nullptr;
   size_t h_pin_cap = 0;
@@ -39,7 +39,8 @@ struct cvb_ctx {
 };
 
 enum { WS_Q = 0, WS_T, WS_SEG, WS_OUT0, WS_OUT1, WS_OUT2, WS_PART_I, WS_PART_D, WS_LIST_I, WS_LIST_D, WS_SKIPA,
-       WS_SKIPB, WS_TMP0, WS_TMP1, WS_FLAG, WS_MISC, WS_CHUNK_PS, WS_CHUNK_OFF, WS_GS0, WS_GS1, WS_GS2, WS_GS3, WS_GS4, WS_GS5, WS_XT, WS_XT_TILE };
+       WS_SKIPB, WS_TMP0, WS_TMP1, WS_FLAG, WS_MISC, WS_CHUNK_PS, WS_CHUNK_OFF, WS_GS0, WS_GS1, WS_GS2, WS_GS3, WS_GS4, WS_GS5, WS_GS6, WS_XT, WS_XT_TILE };
+static_assert(WS_XT_TILE < (int)(sizeof(cvb_ctx::ws) / sizeof(cvb_buf)), "cvb_ctx::ws has a buffer per workspace slot");
 
 // cudaFuncSetAttribute applies to the CURRENT device: one flag per (call site, device), so that a process that opens contexts
 // on several GPUs raises the dynamic shared-memory limit on each of them

@@ -278,39 +278,7 @@ __global__ void __launch_bounds__(256) score_rel_kernel(const double* __restrict
   const double* M = model + 12 * (size_t)h;
   int in = 0;
   if (i < n) {
-    const double t[3] = {M[3], M[7], M[11]};
-    double Ri[9], ti[3];
-#pragma unroll
-    for (int r = 0; r < 3; r++)
-#pragma unroll
-      for (int c = 0; c < 3; c++) Ri[3 * r + c] = M[4 * c + r];
-#pragma unroll
-    for (int r = 0; r < 3; r++) ti[r] = -dot3(Ri[3 * r], Ri[3 * r + 1], Ri[3 * r + 2], t);
-    const double a[3] = {f1[3 * (size_t)i], f1[3 * (size_t)i + 1], f1[3 * (size_t)i + 2]};
-    const double bb[3] = {f2[3 * (size_t)i], f2[3 * (size_t)i + 1], f2[3 * (size_t)i + 2]};
-    double u[3];
-#pragma unroll
-    for (int r = 0; r < 3; r++) u[r] = dot3(M[4 * r], M[4 * r + 1], M[4 * r + 2], bb);
-    // opengv::triangulation::triangulate2 [A]: lambda = A^-1 b, X = (lambda0 f1 + t12 + lambda1 R12 f2) / 2
-    const double b0 = dot3(t[0], t[1], t[2], a), b1 = dot3(t[0], t[1], t[2], u);
-    const double A00 = dot3(a[0], a[1], a[2], a), A10 = dot3(a[0], a[1], a[2], u), A01 = -A10, A11 = -dot3(u[0], u[1], u[2], u);
-    const double det = sub(mul(A00, A11), mul(A01, A10));
-    const double l0 = __ddiv_rn(sub(mul(A11, b0), mul(A01, b1)), det), l1 = __ddiv_rn(sub(mul(A00, b1), mul(A10, b0)), det);
-    double X[3], r2[3];
-#pragma unroll
-    for (int r = 0; r < 3; r++) X[r] = __ddiv_rn(add(mul(l0, a[r]), add(t[r], mul(l1, u[r]))), 2.0);
-#pragma unroll
-    for (int r = 0; r < 3; r++) r2[r] = add(dot3(Ri[3 * r], Ri[3 * r + 1], Ri[3 * r + 2], X), ti[r]);
-    const double n1 = __dsqrt_rn(add(add(mul(X[0], X[0]), mul(X[1], X[1])), mul(X[2], X[2])));
-    const double n2 = __dsqrt_rn(add(add(mul(r2[0], r2[0]), mul(r2[1], r2[1])), mul(r2[2], r2[2])));
-    double e1 = 0.0, e2 = 0.0;
-#pragma unroll
-    for (int r = 0; r < 3; r++) {
-      const double d1 = sub(__ddiv_rn(X[r], n1), a[r]), d2 = sub(__ddiv_rn(r2[r], n2), bb[r]);
-      e1 = r == 0 ? mul(d1, d1) : add(e1, mul(d1, d1));
-      e2 = r == 0 ? mul(d2, d2) : add(e2, mul(d2, d2));
-    }
-    const double s = add(__ddiv_rn(mul(e1, 0.5), s1[i]), __ddiv_rn(mul(e2, 0.5), s2[i]));
+    const double s = rel_score(M, f1, f2, s1, s2, i);
     in = s < threshold;
     if (scores) scores[(size_t)h * n + i] = s;
     if (inlier) inlier[(size_t)h * n + i] = (uint8_t)in;

@@ -1015,6 +1015,66 @@ inline std::vector<AbsolutePoseRansacResult> RansacAbsolutePose(Context& ctx, co
   return out;
 }
 
+// The 17-point non-central relative-pose RANSAC of RelNonCentralPosSolver::computeNonCentralRelPose (RelNonCentralPosSolver.cpp:
+// 146-173) for a batch of candidates in one call (cvb_ransac_noncentral_relative_pose_batch): 17-point hypothesis per sample,
+// scoring per camera pair and opengv's sequential model selection on the GPU.  Per problem: its correspondences (bearings in
+// their cameras' frames, sigmas, the camera of each side), its two rigs (at most CVB_REL_MAX_CAMS cameras each, in the rig
+// frame) and its samples (17 local indices each; every problem of a call has the same number of samples).
+struct NonCentralRelativePoseRansacProblem {
+  std::vector<double> bearings1, bearings2, sigma1, sigma2;   // 3n, 3n, n, n
+  std::vector<int32_t> cam1, cam2;                            // n camera indices into rig 1 / rig 2
+  std::vector<double> rig1_offsets, rig1_rotations;           // 3 / 9 (row-major) per camera of rig 1
+  std::vector<double> rig2_offsets, rig2_rotations;
+  std::vector<int32_t> samples;                               // 17 * n_samples
+};
+struct NonCentralRelativePoseRansacResult {
+  int best_sample = -1;             // -1: no model
+  std::array<double, 12> model{};   // 3x4 [R|t] row-major, X1 = R X2 + t (rig frames)
+  int n_inliers = 0, iterations = 0, samples_used = 0;
+  std::vector<uint8_t> inliers;     // n flags of the selected model
+};
+inline std::vector<NonCentralRelativePoseRansacResult> RansacNonCentralRelativePose(Context& ctx,
+                                                                                   const std::vector<NonCentralRelativePoseRansacProblem>& problems,
+                                                                                   double threshold, int max_iterations, double probability = 0.99) {
+  const int n_prob = (int)problems.size();
+  const size_t n_samples = n_prob ? problems[0].samples.size() / 17 : 0;
+  std::vector<int32_t> ptr(n_prob + 1, 0), cp1(n_prob + 1, 0), cp2(n_prob + 1, 0), cam1, cam2, samples;
+  std::vector<double> f1, f2, s1, s2, co1, cr1, co2, cr2;
+  for (int i = 0; i < n_prob; i++) {
+    const NonCentralRelativePoseRansacProblem& p = problems[i];
+    const size_t n = p.sigma1.size();
+    if (p.samples.size() != 17 * n_samples || p.bearings1.size() != 3 * n || p.bearings2.size() != 3 * n || p.sigma2.size() != n ||
+        p.cam1.size() != n || p.cam2.size() != n || p.rig1_rotations.size() != 3 * p.rig1_offsets.size() ||
+        p.rig2_rotations.size() != 3 * p.rig2_offsets.size() || p.rig1_offsets.size() % 3 || p.rig2_offsets.size() % 3)
+      throw std::invalid_argument("covins_b200::RansacNonCentralRelativePose: inconsistent problem sizes");
+    ptr[i + 1] = ptr[i] + (int32_t)n;
+    cp1[i + 1] = cp1[i] + (int32_t)(p.rig1_offsets.size() / 3);
+    cp2[i + 1] = cp2[i] + (int32_t)(p.rig2_offsets.size() / 3);
+    f1.insert(f1.end(), p.bearings1.begin(), p.bearings1.end()); f2.insert(f2.end(), p.bearings2.begin(), p.bearings2.end());
+    s1.insert(s1.end(), p.sigma1.begin(), p.sigma1.end()); s2.insert(s2.end(), p.sigma2.begin(), p.sigma2.end());
+    cam1.insert(cam1.end(), p.cam1.begin(), p.cam1.end()); cam2.insert(cam2.end(), p.cam2.begin(), p.cam2.end());
+    co1.insert(co1.end(), p.rig1_offsets.begin(), p.rig1_offsets.end()); cr1.insert(cr1.end(), p.rig1_rotations.begin(), p.rig1_rotations.end());
+    co2.insert(co2.end(), p.rig2_offsets.begin(), p.rig2_offsets.end()); cr2.insert(cr2.end(), p.rig2_rotations.begin(), p.rig2_rotations.end());
+    samples.insert(samples.end(), p.samples.begin(), p.samples.end());
+  }
+  const size_t m = n_prob > 0 ? n_prob : 1;
+  std::vector<int32_t> best(m), cnt(m), iters(m), used(m);
+  std::vector<double> models(12 * m);
+  std::vector<uint8_t> mask(ptr[n_prob] > 0 ? ptr[n_prob] : 1);
+  cvb_rel_ransac_problems P{n_prob,     ptr.data(), f1.data(), f2.data(), s1.data(),  s2.data(),  cam1.data(),    cam2.data(),
+                            cp1.data(), co1.data(), cr1.data(), cp2.data(), co2.data(), cr2.data(), samples.data(), (int32_t)n_samples};
+  cvb_rel_ransac_result R{best.data(), models.data(), cnt.data(), iters.data(), used.data(), mask.data(), nullptr, nullptr, nullptr};
+  ctx.check(cvb_ransac_noncentral_relative_pose_batch(ctx.get(), &P, threshold, max_iterations, probability, &R),
+            "cvb_ransac_noncentral_relative_pose_batch");
+  std::vector<NonCentralRelativePoseRansacResult> out(n_prob);
+  for (int i = 0; i < n_prob; i++) {
+    out[i].best_sample = best[i]; out[i].n_inliers = cnt[i]; out[i].iterations = iters[i]; out[i].samples_used = used[i];
+    std::copy(models.begin() + 12 * i, models.begin() + 12 * (i + 1), out[i].model.begin());
+    out[i].inliers.assign(mask.begin() + ptr[i], mask.begin() + ptr[i + 1]);
+  }
+  return out;
+}
+
 // Resident-map descriptor database (cvb_db_*): the ORB descriptors of the map's keyframes live in HBM; the candidate
 // loop of PlaceRecognitionG::ComputeSE3 (placerec_gen_be.cpp:60-135) becomes one call per query keyframe.  The database
 // index of a keyframe is its insertion order; keep it next to the keyframe (e.g. std::map<idpair, int>).

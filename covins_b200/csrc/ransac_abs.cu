@@ -112,14 +112,6 @@ __device__ void refine_depths(double* L, const double* a, const double* b) {
   }
 }
 
-__device__ void inv3(const double* m, double* o) {
-  const double c00 = sub(mul(m[4], m[8]), mul(m[5], m[7])), c01 = sub(mul(m[5], m[6]), mul(m[3], m[8])), c02 = sub(mul(m[3], m[7]), mul(m[4], m[6]));
-  const double det = add(add(mul(m[0], c00), mul(m[1], c01)), mul(m[2], c02));
-  o[0] = dv(c00, det); o[1] = dv(sub(mul(m[2], m[7]), mul(m[1], m[8])), det); o[2] = dv(sub(mul(m[1], m[5]), mul(m[2], m[4])), det);
-  o[3] = dv(c01, det); o[4] = dv(sub(mul(m[0], m[8]), mul(m[2], m[6])), det); o[5] = dv(sub(mul(m[2], m[3]), mul(m[0], m[5])), det);
-  o[6] = dv(c02, det); o[7] = dv(sub(mul(m[1], m[6]), mul(m[0], m[7])), det); o[8] = dv(sub(mul(m[0], m[4]), mul(m[1], m[3])), det);
-}
-
 // P3P: bearings f[3][3] (camera frame), world points x[3][3] → up to 4 poses Rt[k][12], lambda_i f_i = R x_i + t, lambda_i > 0
 __device__ int p3p(const double* f, const double* x, double* Rt) {
   double y[3][3];

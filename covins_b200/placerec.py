@@ -6,6 +6,8 @@ the C-ABI:
   score_relative_pose(...)      ↔ FrameRelativePoseSacProblem scoring   (frame-relative-pose-sac-problem.hpp:69-104)
   ransac_select(...)            ↔ the model-selection rule of opengv::sac::Ransac::computeModel replayed over batched scores
   ransac_absolute_pose(...)     ↔ the whole GP3P RANSAC of Se3Solver::projectiveAlignment from caller-supplied samples
+  ransac_noncentral_relative_pose(...) ↔ the 17-point RANSAC of RelNonCentralPosSolver::computeNonCentralRelPose from
+                                  caller-supplied samples
 
 `KfView` flattens what the reference reads of a Keyframe (the C++ shim does the same from the containers)."""
 from __future__ import annotations
@@ -194,4 +196,42 @@ def ransac_absolute_pose(ctx: Context, prob_ptr, pts, bearings, sigma, cam_off, 
     P = CAbsRansacProblems(n_prob, ptr.ctypes.data, p.ctypes.data, f.ctypes.data, s.ctypes.data, co.ctypes.data, cr.ctypes.data, smp.ctypes.data, ns)
     R = CAbsRansacResult(*[r[k].ctypes.data if k in r else None for k, _ in CAbsRansacResult._fields_])
     ctx.check(lib().cvb_ransac_absolute_pose_batch(ctx.handle, C.byref(P), float(threshold), int(max_iterations), float(probability), C.byref(R)))
+    return r
+
+
+class CRelRansacProblems(C.Structure):
+    _fields_ = [("n_prob", C.c_int32)] + [(k, c_vp) for k in ("prob_ptr", "f1", "f2", "sigma1", "sigma2", "cam1", "cam2", "cam_ptr1", "cam_off1",
+                                                               "cam_rot1", "cam_ptr2", "cam_off2", "cam_rot2", "samples")] + [("n_samples", C.c_int32)]
+
+
+class CRelRansacResult(CAbsRansacResult):
+    pass
+
+
+def ransac_noncentral_relative_pose(ctx: Context, prob_ptr, f1, f2, sigma1, sigma2, cam1, cam2, cam_ptr1, cam_off1, cam_rot1, cam_ptr2, cam_off2,
+                                    cam_rot2, samples, threshold, max_iterations, probability=0.99, per_sample=False):
+    """RelNonCentralPosSolver::computeNonCentralRelPose's 17-point RANSAC for a batch of problems
+    (cvb_ransac_noncentral_relative_pose_batch): 17-point hypothesis per sample, scoring per camera pair and ransac_select-style
+    selection on the GPU.  prob_ptr [n_prob+1] correspondence ranges; f1 / f2 [N,3] bearings in their cameras' frames, sigma1 /
+    sigma2 [N], cam1 / cam2 [N] problem-local camera indices; cam_ptr1 [n_prob+1] rig-1 camera ranges, cam_off1 [C1,3],
+    cam_rot1 [C1,3,3] (cameras in the rig frame), rig 2 likewise; samples [n_prob, n_samples, 17] problem-local indices.
+    → dict(best_sample, best_model [n_prob,3,4] (X1 = R X2 + t), best_count, iterations, consumed, inlier_mask [N]) and, with
+    per_sample, sample_model [n_prob,n_samples,3,4], sample_valid, sample_count."""
+    ptr = np.ascontiguousarray(prob_ptr, np.int32); n_prob = len(ptr) - 1
+    a = np.ascontiguousarray(f1, np.float64).reshape(-1, 3); b = np.ascontiguousarray(f2, np.float64).reshape(-1, 3)
+    s1 = np.ascontiguousarray(sigma1, np.float64).reshape(-1); s2 = np.ascontiguousarray(sigma2, np.float64).reshape(-1)
+    c1 = np.ascontiguousarray(cam1, np.int32).reshape(-1); c2 = np.ascontiguousarray(cam2, np.int32).reshape(-1)
+    cp1 = np.ascontiguousarray(cam_ptr1, np.int32); cp2 = np.ascontiguousarray(cam_ptr2, np.int32)
+    co1 = np.ascontiguousarray(cam_off1, np.float64).reshape(-1, 3); cr1 = np.ascontiguousarray(cam_rot1, np.float64).reshape(-1, 9)
+    co2 = np.ascontiguousarray(cam_off2, np.float64).reshape(-1, 3); cr2 = np.ascontiguousarray(cam_rot2, np.float64).reshape(-1, 9)
+    smp = np.ascontiguousarray(samples, np.int32).reshape(n_prob, -1, 17); ns = smp.shape[1]
+    r = dict(best_sample=np.zeros(n_prob, np.int32), best_model=np.zeros((n_prob, 3, 4)), best_count=np.zeros(n_prob, np.int32),
+             iterations=np.zeros(n_prob, np.int32), consumed=np.zeros(n_prob, np.int32), inlier_mask=np.zeros(len(a), np.uint8))
+    if per_sample:
+        r.update(sample_model=np.zeros((n_prob, ns, 3, 4)), sample_valid=np.zeros((n_prob, ns), np.uint8),
+                 sample_count=np.zeros((n_prob, ns), np.int32))
+    P = CRelRansacProblems(n_prob, *[x.ctypes.data for x in (ptr, a, b, s1, s2, c1, c2, cp1, co1, cr1, cp2, co2, cr2, smp)], ns)
+    R = CRelRansacResult(*[r[k].ctypes.data if k in r else None for k, _ in CRelRansacResult._fields_])
+    ctx.check(lib().cvb_ransac_noncentral_relative_pose_batch(ctx.handle, C.byref(P), float(threshold), int(max_iterations), float(probability),
+                                                              C.byref(R)))
     return r

@@ -353,6 +353,80 @@ CVB_API int cvb_ransac_absolute_pose_batch(cvb_ctx* ctx, const cvb_abs_ransac_pr
                                            double probability, cvb_abs_ransac_result* r);
 
 /*
+ * The non-central relative-pose RANSAC of RelNonCentralPosSolver::computeNonCentralRelPose (17-point,
+ * RelNonCentralPosSolver.cpp:146-173: the COVINS_G verification of a candidate, each side a rig of a keyframe and its
+ * neighbours) for a batch of problems in one launch, from the caller's samples: 17-point solve, scoring per camera pair,
+ * the sequential model selection of opengv's Ransac::computeModel and the inlier mask of the selected model.  Samples stay
+ * an input, as in cvb_ransac_absolute_pose_batch.
+ *   Rigs: a point x_c in camera frame j of a rig maps to Rc_j x_c + c_j in the rig frame.  At most CVB_REL_MAX_CAMS cameras
+ *   per rig.  A caller with one rig for both views (opengv's own adapter) passes it twice.
+ *   Model: [R|t] row-major 3x4 with X1 = R X2 + t (rig frames; cvb_score_relative_pose_batch's [R12|t12] convention).
+ *   Hypothesis of a sample (17 problem-local indices):
+ *     1. Plücker lines d = Rc f, m = c x d per side; row i of A (17x18), in sample order, is
+ *        [vec(d1 d2^T), vec(d1 m2^T + m1 d2^T)] (vec = row-major), from the generalised epipolar constraint
+ *        d1^T E d2 + d1^T R m2 + m1^T R d2 = 0, E = [t]x R.
+ *     2. Null vector x of A: Householder QR of A^T (18x17), x = Q e18.  The sample is invalid if
+ *        min_k |r_kk| < 1e-10 max_k |r_kk| (rank below 17: a rig whose cameras share one centre, repeated points).
+ *     3. R' = x[9:18] (row-major); if det R' < 0 it is negated, if det R' = 0 the sample is invalid.  R is the orthonormal
+ *        polar factor of R', from R' scaled to |R'|_F = sqrt(3) by 12 Newton steps X <- (X + X^-T) / 2.
+ *     4. t: least squares over the sample's 17 rows with R fixed, (R d2 x d1) . t = -(d1^T R m2 + m1^T R d2), by the 3x3
+ *        normal equations summed in sample order.
+ *     ASSUMPTION (opengv is not in the tree): opengv's seventeenpt may recover t from E instead; on noise-free data both give
+ *     the same model.
+ *     The sample is also invalid if the problem has fewer than 17 correspondences, an index repeats within the sample, a
+ *     bearing of the sample or a camera of either rig is not finite, or the model is not finite.
+ *   Score of correspondence i: with the camera-pair model R_p = Rc1^T R Rc2, t_p = Rc1^T (R c2 + t - c1) of its cameras
+ *   (cam1[i], cam2[i]), exactly cvb_score_relative_pose_batch's per-correspondence score (the same device function), inlier
+ *   iff score < threshold.  ASSUMPTION: the 17-point RANSAC scores with the same FrameRelativePoseSacProblem score as the
+ *   5-point one, applied per camera pair.
+ *   Selection: as cvb_ransac_absolute_pose_batch with sample size 17 (invalid samples do not consume an iteration, at most
+ *   10 * max_iterations are skipped; ransac_select's rule).  w^17 is a left-to-right product chain and log runs on the device:
+ *   the adaptive bound can differ from a host evaluation (pow / glibc log) by an ulp, which only matters when it lands within
+ *   an ulp of an integer.
+ * Inputs: correspondences concatenated over problems (prob_ptr[n_prob+1], prob_ptr[0] = 0): unit bearings f1[i], f2[i], each
+ * in its own camera's frame, sigma1[i], sigma2[i] as in cvb_score_relative_pose_batch, camera indices cam1[i], cam2[i] local to
+ * the problem's rigs.  Rig 1 of problem p is cameras cam_ptr1[p] .. cam_ptr1[p+1]-1 of cam_off1 [.][3] / cam_rot1 [.][9]
+ * (row-major), rig 2 likewise.  samples [n_prob][n_samples][17], indices local to their problem (the samples of a problem with
+ * fewer than 17 correspondences are not read).
+ * Outputs: as cvb_ransac_absolute_pose_batch (best_model = [R|t] above).
+ * Errors: CVB_ERR_INVALID before any launch for negative sizes, null required pointers, a decreasing prob_ptr / cam_ptr1 /
+ * cam_ptr2, an out-of-range sample index, a camera index outside its rig, a rig of more than CVB_REL_MAX_CAMS cameras, or
+ * per-sample outputs not requested together; n_prob = 0 succeeds.
+ */
+#define CVB_REL_MAX_CAMS 8
+typedef struct cvb_rel_ransac_problems {
+  int32_t n_prob;
+  const int32_t* prob_ptr;   /* [n_prob+1] */
+  const double* f1;          /* [N][3] unit bearings, frame of camera cam1[i] of rig 1 */
+  const double* f2;          /* [N][3] unit bearings, frame of camera cam2[i] of rig 2 */
+  const double* sigma1;      /* [N] */
+  const double* sigma2;      /* [N] */
+  const int32_t* cam1;       /* [N] camera of rig 1, local to the problem */
+  const int32_t* cam2;       /* [N] camera of rig 2, local to the problem */
+  const int32_t* cam_ptr1;   /* [n_prob+1] cameras of rig 1 per problem */
+  const double* cam_off1;    /* [cam_ptr1[n_prob]][3] camera centre c in the rig frame */
+  const double* cam_rot1;    /* [cam_ptr1[n_prob]][9] camera rotation Rc in the rig frame, row-major */
+  const int32_t* cam_ptr2;   /* [n_prob+1] */
+  const double* cam_off2;    /* [cam_ptr2[n_prob]][3] */
+  const double* cam_rot2;    /* [cam_ptr2[n_prob]][9] */
+  const int32_t* samples;    /* [n_prob][n_samples][17] */
+  int32_t n_samples;
+} cvb_rel_ransac_problems;
+typedef struct cvb_rel_ransac_result {
+  int32_t* best_sample;      /* [n_prob] */
+  double* best_model;        /* [n_prob][12] 3x4 [R|t] row-major, X1 = R X2 + t */
+  int32_t* best_count;       /* [n_prob] */
+  int32_t* iterations;       /* [n_prob] */
+  int32_t* consumed;         /* [n_prob] */
+  uint8_t* inlier_mask;      /* [N] nullable */
+  double* sample_model;      /* [n_prob][n_samples][12] nullable */
+  uint8_t* sample_valid;     /* [n_prob][n_samples]     nullable */
+  int32_t* sample_count;     /* [n_prob][n_samples]     nullable */
+} cvb_rel_ransac_result;
+CVB_API int cvb_ransac_noncentral_relative_pose_batch(cvb_ctx* ctx, const cvb_rel_ransac_problems* p, double threshold, int max_iterations,
+                                                      double probability, cvb_rel_ransac_result* r);
+
+/*
  * Optimization::OptimizeRelativePose(kf1, kf2, matches1, T12, th2) (optimization_be.cpp:620-831): the 6-dof refinement of
  * the relative pose T12 from the matched landmark pairs, both ceres::Solve calls (5 + 5 iterations, DOGLEG, CauchyLoss(1))
  * and the outlier purge between them, in one call.  The caller (shim) flattens, per residual pair r (the reference's
