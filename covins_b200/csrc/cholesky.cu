@@ -13,8 +13,9 @@
 // Right-looking, panel width 128:
 //   potrf_inv_kernel   1 CTA: factor the 128x128 diagonal tile in shared memory, write L, write L^-1
 //   trsm_kernel        row tiles below: A(i,k) <- A(i,k) * Linv^T            (128^3 DMMA GEMM per CTA)
-//   syrk_kernel        trailing tiles (i >= j > k): A(i,j) -= A(i,k) A(j,k)^T (128^3 DMMA GEMM per CTA and panel; in
-//                      blocks of kPanelBlock columns, all of a block's panels per visit to a tile — see factor())
+//   tile_update_kernel trailing tiles (i >= j > k): A(i,j) -= A(i,k) A(j,k)^T (one 128x128 tile per CTA, 128^3 DMMA GEMM
+//                      per panel; in blocks of kPanelBlock columns, all of a block's panels per visit to a tile — see
+//                      factor()); syrk_kernel does the same for the chain's diagonal pair, spread over 4 CTAs for latency
 // Solves use the stored tile inverses: forward L y = b, backward L^T x = y, one launch per tile column.
 // All reductions have a fixed order → bit-reproducible run to run.
 #include "cholesky.cuh"
@@ -50,9 +51,10 @@ __device__ __forceinline__ void dmma16816(double (&c)[4], const double (&a)[8], 
 // its results were bit-identical to four chained m8n8k4 over the same 16-wide K chunk.  K is staged in chunks of 16 (one
 // MMA per block and chunk) through a STAGES-deep cp.async ring (one barrier per chunk).  Row stride 20 doubles (≡ 8 words
 // mod 32): the fragment loads of a half-warp (rows g = 0..3, columns t = 0..3) hit words 8g + 2t, conflict-free.  The CTA
-// is deliberately small (64 x 64 x 128 for the trailing update: 128 threads, 60 KB): three to four CTAs share an SM, so
-// one CTA's fixed costs — index fetch, pipeline fill, the C round trip of the epilogue, barrier bubbles — overlap the
-// others' main loops.  (One 128x128 tile per SM left the FP64 tensor pipe idle a third of the time.)
+// is deliberately small (64 x 64 x 128 for syrk_kernel: 128 threads, 60 KB): three to four CTAs share an SM, so one CTA's
+// fixed costs — index fetch, pipeline fill, the C round trip of the epilogue, barrier bubbles — overlap the others' main
+// loops.  The throughput path of the trailing update (tile_update_kernel) takes the whole 128x128 tile per CTA instead:
+// it halves the operand bytes per FMA and keeps C in shared memory, so it has no per-panel C round trip to hide.
 constexpr int KC = 16;
 constexpr int LDS = KC + 4;
 constexpr int GEMM_STAGES = 3;
@@ -185,7 +187,8 @@ __global__ void __launch_bounds__(T, 1) chain_gemm_kernel(double* __restrict__ C
 }
 
 // A(i,j) -= A(i,k) A(j,k)^T for the tile pairs (i >= j) pi[]/pj[] and the panels k = k0 + q of the bits q of pmask[]
-// (TilePlan::h_pair_mask), in increasing k, each panel's product subtracted on its own.  Four CTAs per pair, one 64x64
+// (TilePlan::h_pair_mask), in increasing k, each panel's product subtracted on its own.  Used for the chain's diagonal pair
+// (factor()), where one tile is updated alone and latency counts: four CTAs per pair, one 64x64
 // quadrant each (consecutive CTAs share the pair's operands in L2); the quadrant above the diagonal of a diagonal tile is
 // skipped.  The quadrant (32 KB) is fetched into L2 at the start, so the first epilogue does not wait on HBM, and stays
 // there for the read-modify-write of the later panels: several panels per visit make one HBM round trip of C.
@@ -224,6 +227,135 @@ __global__ void __launch_bounds__(SYRK_THREADS, 3) syrk_kernel(double* __restric
           v.y -= acc[a][b][2 * h + 1];
           *q = v;
         }
+  }
+}
+
+// The same update, one CTA per pair and the whole 128x128 tile per CTA: the throughput path (every update list except the
+// chain's diagonal pair, see factor()).  Per 16-wide K chunk a CTA stages 128 rows of each operand for 128x128x16 FMA —
+// half the operand bytes per FMA of the 64x64 quadrants above, whose L2→SM traffic bounded them.  8 warps of 64x32
+// (4 m16 x 4 n8 blocks; a thread holds 128 accumulator doubles, the four B fragments of a chunk and one m16 row of A
+// fragments at a time): 221 registers, 1 CTA/SM.  The operands come through a 3-stage cp.async ring that runs on across
+// the panels of the pair's mask (a chunk's stage is refilled with the next panel's chunks while the epilogue runs).
+// C lives in shared memory for the whole visit: it is copied in during the first chunks, each panel's product
+// (accumulated from zero over the K chunks in order) is subtracted from it on its own, in increasing panel order, and it
+// is written back once.  So the results are bit-identical to syrk_kernel's, with one C read and one C write per visit
+// instead of an L2 read-modify-write per panel.  Ring rows are 128 B, unpadded: segment s of a row r sits at
+// s ^ 2 (r & 3), which makes the fragment loads conflict-free; C rows are 1 KB, 16-byte segment s of row r at s ^ 4 (r & 1),
+// which makes the epilogue's double2 accesses conflict-free.  Shared memory: 128 KB of C + 3 x 32 KB ring (+ 512 B).
+constexpr int TILE_THREADS = 256;
+constexpr int TILE_STAGES = 3;
+constexpr int TILE_STAGE = 2 * T * KC;   // doubles per ring stage: 128 rows of A(i,k), then 128 rows of A(j,k)
+constexpr size_t kTileSmem = (TT + (size_t)TILE_STAGES * TILE_STAGE) * sizeof(double);   // 229376 B → 1 CTA / SM
+
+__global__ void __launch_bounds__(TILE_THREADS, 1) tile_update_kernel(double* __restrict__ S, const int* __restrict__ tile_of,
+                                                                      int nt, int k0, const int* __restrict__ pi,
+                                                                      const int* __restrict__ pj,
+                                                                      const int* __restrict__ pmask) {
+  extern __shared__ __align__(128) double smem_d[];
+  __shared__ const double* s_ai[32];   // operand tiles A(i,k), A(j,k) of the pair's panels, in increasing k
+  __shared__ const double* s_aj[32];
+  constexpr int NCH = T / KC;
+  double* Cs = smem_d;            // [T][T], swizzled
+  double* ring = smem_d + TT;     // [TILE_STAGES][2 T][KC], swizzled
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int i = pi[blockIdx.x], j = pj[blockIdx.x];
+  const bool diag = i == j;
+  const unsigned mask = (unsigned)pmask[blockIdx.x];
+  double* C = S + (size_t)tile_of[(size_t)i * nt + j] * TT;
+  if (tid < 32 && ((mask >> tid) & 1u)) {
+    const int q = __popc(mask & ((1u << tid) - 1u));
+    s_ai[q] = S + (size_t)tile_of[(size_t)i * nt + k0 + tid] * TT;
+    s_aj[q] = S + (size_t)tile_of[(size_t)j * nt + k0 + tid] * TT;
+  }
+  __syncthreads();
+  const int nch = __popc(mask) * NCH;   // chunk c = K chunk c % NCH of the pair's panel c / NCH
+  // a thread copies 16-byte segment `seg` of rows r0, r0 + 32, ... of both operands (r0 & 3 fixes the swizzle)
+  const int r0 = tid >> 3, seg = tid & 7;
+  const int so = r0 * KC + ((seg ^ ((r0 & 3) << 1)) << 1);
+  auto load_chunk = [&](int c) {
+    if (c < nch) {
+      const size_t go = (size_t)r0 * T + (c % NCH) * KC + seg * 2;
+      const double* ga = s_ai[c / NCH] + go;
+      const double* gb = s_aj[c / NCH] + go;
+      double* As = ring + (c % TILE_STAGES) * TILE_STAGE + so;
+#pragma unroll
+      for (int it = 0; it < T / 32; it++) cp_async16(As + it * 32 * KC, ga + (size_t)it * 32 * T);
+#pragma unroll
+      for (int it = 0; it < T / 32; it++) cp_async16(As + T * KC + it * 32 * KC, gb + (size_t)it * 32 * T);
+    }
+    cp_async_commit();   // always commit (possibly empty) so the wait count below is uniform
+  };
+  // rows 32 part .. 32 part + 31 of C join the group of chunk part + 2 (part < 4): all of C has landed at chunk 5, before
+  // the first epilogue, and the copy overlaps the first chunks.  The quadrant above the diagonal of a diagonal tile is
+  // neither read nor written.
+  auto load_c = [&](int part) {
+#pragma unroll
+    for (int it = 0; it < 8; it++) {
+      const int u = tid + it * TILE_THREADS, r = part * 32 + (u >> 6), s = u & 63;
+      if (!(diag && r < 64 && s >= 32)) cp_async16(Cs + r * T + ((s ^ ((r & 1) << 2)) << 1), C + (size_t)r * T + s * 2);
+    }
+  };
+  const int g = lane >> 2, t = lane & 3, wm = warp >> 2, wn = warp & 3;   // warp tile: rows 64 wm.., columns 32 wn..
+  const bool idle = diag && wm == 0 && wn >= 2;                             // above the diagonal of a diagonal tile
+  int cq[4];   // ring column of fragment K index t + 4 q (rows g + 8 n: the swizzle depends on g & 3 only)
+#pragma unroll
+  for (int q = 0; q < 4; q++) cq[q] = t + 4 * (q ^ (g & 3));
+  double acc[4][4][4];
+#pragma unroll
+  for (int a = 0; a < 4; a++)
+#pragma unroll
+    for (int b = 0; b < 4; b++)
+#pragma unroll
+      for (int e = 0; e < 4; e++) acc[a][b][e] = 0.0;
+#pragma unroll
+  for (int c = 0; c < TILE_STAGES - 1; c++) load_chunk(c);
+#pragma unroll 1
+  for (int c = 0; c < nch; c++) {
+    cp_async_wait<TILE_STAGES - 2>();   // chunk c has landed
+    __syncthreads();                    // ... for every thread, and chunk c-1's stage is free again
+    if (c < 4) load_c(c);
+    load_chunk(c + TILE_STAGES - 1);
+    if (idle) continue;
+    const double* As = ring + (c % TILE_STAGES) * TILE_STAGE + (wm * 64 + g) * KC;
+    const double* Bs = ring + (c % TILE_STAGES) * TILE_STAGE + T * KC + (wn * 32 + g) * KC;
+    double b[4][4];
+#pragma unroll
+    for (int bj = 0; bj < 4; bj++)
+#pragma unroll
+      for (int e = 0; e < 4; e++) b[bj][e] = Bs[bj * 8 * KC + cq[e]];
+#pragma unroll
+    for (int ai = 0; ai < 4; ai++) {
+      double a[8];
+#pragma unroll
+      for (int e = 0; e < 8; e++) a[e] = As[(ai * 16 + 8 * (e & 1)) * KC + cq[e >> 1]];
+#pragma unroll
+      for (int bj = 0; bj < 4; bj++) dmma16816(acc[ai][bj], a, b[bj]);
+    }
+    if (c % NCH == NCH - 1) {   // the panel is complete: subtract it, start the next one from zero
+#pragma unroll
+      for (int ai = 0; ai < 4; ai++)
+#pragma unroll
+        for (int bj = 0; bj < 4; bj++)
+#pragma unroll
+          for (int h = 0; h < 2; h++) {
+            const int r = wm * 64 + ai * 16 + h * 8 + g, s = wn * 16 + bj * 4 + t;
+            double2* q = reinterpret_cast<double2*>(Cs + r * T + ((s ^ ((r & 1) << 2)) << 1));
+            double2 v = *q;
+            v.x -= acc[ai][bj][2 * h];
+            v.y -= acc[ai][bj][2 * h + 1];
+            *q = v;
+            acc[ai][bj][2 * h] = 0.0;
+            acc[ai][bj][2 * h + 1] = 0.0;
+          }
+    }
+  }
+  __syncthreads();   // every warp's last epilogue is in Cs
+#pragma unroll 8
+  for (int it = 0; it < (int)(TT / 2 / TILE_THREADS); it++) {
+    const int u = tid + it * TILE_THREADS, r = u >> 6, s = u & 63;
+    if (!(diag && r < 64 && s >= 32))
+      *reinterpret_cast<double2*>(C + (size_t)r * T + s * 2) =
+          *reinterpret_cast<const double2*>(Cs + r * T + ((s ^ ((r & 1) << 2)) << 1));
   }
 }
 
@@ -776,6 +908,7 @@ int factor(cvb_ctx* ctx, double* S, double* linv, int* d_flag, const TilePlan& p
   if (once.first(ctx->device)) {
     CVB_CUDA(ctx, cudaFuncSetAttribute(trsm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kTrsmSmem));
     CVB_CUDA(ctx, cudaFuncSetAttribute(syrk_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSyrkSmem));
+    CVB_CUDA(ctx, cudaFuncSetAttribute(tile_update_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kTileSmem));
     CVB_CUDA(ctx, cudaFuncSetAttribute(potrf_inv_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kPotrfSmem));
     CVB_CUDA(ctx, cudaFuncSetAttribute(chain_gemm_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kChainSmem));
     CVB_CUDA(ctx, cudaFuncSetAttribute(chain_gemm_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kChainSmem));
@@ -967,14 +1100,14 @@ int factor(cvb_ctx* ctx, double* S, double* linv, int* d_flag, const TilePlan& p
       if (lb >= 0) CVB_CUDA(ctx, cudaStreamWaitEvent(ws, ev[5 * lb + 1], 0));
       const int a0 = diag_pair ? 1 : 0;
       if (na - a0 > 0) {
-        syrk_kernel<<<4 * (na - a0), SYRK_THREADS, kSyrkSmem, ws>>>(S, plan.d_tile_of, nt, k0, plan.d_pair_i + p0 + a0,
+        tile_update_kernel<<<na - a0, TILE_THREADS, kTileSmem, ws>>>(S, plan.d_tile_of, nt, k0, plan.d_pair_i + p0 + a0,
                                                                      plan.d_pair_j + p0 + a0, plan.d_pair_mask + p0 + a0);
         CVB_CHECK_LAUNCH(ctx);
       }
       if (tr) cudaEventRecord(tev[(size_t)k * 5 + 3], ws);
       if (np - na > 0) {
         CVB_CUDA(ctx, cudaStreamWaitEvent(st2, evPanel, 0));
-        syrk_kernel<<<4 * (np - na), SYRK_THREADS, kSyrkSmem, st2>>>(S, plan.d_tile_of, nt, k0, plan.d_pair_i + p0 + na,
+        tile_update_kernel<<<np - na, TILE_THREADS, kTileSmem, st2>>>(S, plan.d_tile_of, nt, k0, plan.d_pair_i + p0 + na,
                                                                        plan.d_pair_j + p0 + na, plan.d_pair_mask + p0 + na);
         CVB_CHECK_LAUNCH(ctx);
         CVB_CUDA(ctx, cudaEventRecord(evBulk, st2));
