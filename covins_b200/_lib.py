@@ -82,6 +82,7 @@ SIGNATURES = {
     "cvb_score_relative_pose_batch": (C.c_int, [c_vp, c_vp, C.c_int, c_vp, c_vp, c_vp, c_vp, C.c_int, C.c_double, c_vp, c_vp, c_vp]),
     "cvb_ransac_absolute_pose_batch": (C.c_int, [c_vp, c_vp, C.c_double, C.c_int, C.c_double, c_vp]),
     "cvb_ransac_noncentral_relative_pose_batch": (C.c_int, [c_vp, c_vp, C.c_double, C.c_int, C.c_double, c_vp]),
+    "cvb_ransac_central_relative_pose_batch": (C.c_int, [c_vp, c_vp, C.c_double, C.c_int, C.c_double, c_vp]),
     "cvb_ba_iterate": (C.c_int, [c_vp, C.c_int, C.POINTER(C.c_int)]),
     "cvb_ba_result_get": (C.c_int, [c_vp, c_vp, c_vp]),
     "cvb_ba_reproj_norms": (C.c_int, [c_vp, c_vp, C.c_int]),

@@ -66,11 +66,9 @@ __device__ __forceinline__ double abs_score(const double* Ri, const double* ti, 
   return __ddiv_rn(e2, sigma);
 }
 
-// score of correspondence i (bearings f1 / f2 [.][3], sigma1 / sigma2) of FrameRelativePoseSacProblem
-// (frame-relative-pose-sac-problem.hpp:69-104) under the model M = [R12|t12] (X1 = R12 X2 + t12): opengv::triangulation::triangulate2 [A] (lambda = A^-1 b,
-// X = (lambda0 f1 + t12 + lambda1 R12 f2) / 2), then 0.5 |normalize(X) - f|^2 / sigma per view; inlier iff score < threshold
-__device__ __forceinline__ double rel_score(const double* __restrict__ M, const double* __restrict__ f1, const double* __restrict__ f2,
-                                            const double* __restrict__ s1, const double* __restrict__ s2, int i) {
+// opengv::triangulation::triangulate2 [A] of bearings a (view 1), bb (view 2) under the model M = [R12|t12] (X1 = R12 X2 + t12):
+// lambda = A^-1 b, X = (lambda0 a + t12 + lambda1 R12 bb) / 2 in view 1, r2 = R12^T X - R12^T t12 in view 2
+__device__ __forceinline__ void rel_triangulate(const double* __restrict__ M, const double* a, const double* bb, double X[3], double r2[3]) {
   const double t[3] = {M[3], M[7], M[11]};
   double Ri[9], ti[3];
 #pragma unroll
@@ -79,8 +77,6 @@ __device__ __forceinline__ double rel_score(const double* __restrict__ M, const 
     for (int c = 0; c < 3; c++) Ri[3 * r + c] = M[4 * c + r];
 #pragma unroll
   for (int r = 0; r < 3; r++) ti[r] = -dot3(Ri[3 * r], Ri[3 * r + 1], Ri[3 * r + 2], t);
-  const double a[3] = {f1[3 * (size_t)i], f1[3 * (size_t)i + 1], f1[3 * (size_t)i + 2]};
-  const double bb[3] = {f2[3 * (size_t)i], f2[3 * (size_t)i + 1], f2[3 * (size_t)i + 2]};
   double u[3];
 #pragma unroll
   for (int r = 0; r < 3; r++) u[r] = dot3(M[4 * r], M[4 * r + 1], M[4 * r + 2], bb);
@@ -88,11 +84,21 @@ __device__ __forceinline__ double rel_score(const double* __restrict__ M, const 
   const double A00 = dot3(a[0], a[1], a[2], a), A10 = dot3(a[0], a[1], a[2], u), A01 = -A10, A11 = -dot3(u[0], u[1], u[2], u);
   const double det = sub(mul(A00, A11), mul(A01, A10));
   const double l0 = __ddiv_rn(sub(mul(A11, b0), mul(A01, b1)), det), l1 = __ddiv_rn(sub(mul(A00, b1), mul(A10, b0)), det);
-  double X[3], r2[3];
 #pragma unroll
   for (int r = 0; r < 3; r++) X[r] = __ddiv_rn(add(mul(l0, a[r]), add(t[r], mul(l1, u[r]))), 2.0);
 #pragma unroll
   for (int r = 0; r < 3; r++) r2[r] = add(dot3(Ri[3 * r], Ri[3 * r + 1], Ri[3 * r + 2], X), ti[r]);
+}
+
+// score of correspondence i (bearings f1 / f2 [.][3], sigma1 / sigma2) of FrameRelativePoseSacProblem
+// (frame-relative-pose-sac-problem.hpp:69-104) under the model M = [R12|t12] (X1 = R12 X2 + t12): the triangulation above, then
+// 0.5 |normalize(X) - f|^2 / sigma per view; inlier iff score < threshold
+__device__ __forceinline__ double rel_score(const double* __restrict__ M, const double* __restrict__ f1, const double* __restrict__ f2,
+                                            const double* __restrict__ s1, const double* __restrict__ s2, int i) {
+  const double a[3] = {f1[3 * (size_t)i], f1[3 * (size_t)i + 1], f1[3 * (size_t)i + 2]};
+  const double bb[3] = {f2[3 * (size_t)i], f2[3 * (size_t)i + 1], f2[3 * (size_t)i + 2]};
+  double X[3], r2[3];
+  rel_triangulate(M, a, bb, X, r2);
   const double n1 = __dsqrt_rn(add(add(mul(X[0], X[0]), mul(X[1], X[1])), mul(X[2], X[2])));
   const double n2 = __dsqrt_rn(add(add(mul(r2[0], r2[0]), mul(r2[1], r2[1])), mul(r2[2], r2[2])));
   double e1 = 0.0, e2 = 0.0;

@@ -1075,6 +1075,47 @@ inline std::vector<NonCentralRelativePoseRansacResult> RansacNonCentralRelativeP
   return out;
 }
 
+// The 5-point central relative-pose RANSAC of RelNonCentralPosSolver::computePose (RelNonCentralPosSolver.cpp:343-377) for a
+// batch of pairings in one call (cvb_ransac_central_relative_pose_batch): 5-point hypothesis per sample, scoring and opengv's
+// sequential model selection on the GPU.  Per problem: its correspondences (unit bearings, sigmas) and its samples (5 local
+// indices each; every problem of a call has the same number of samples).  The six pairings of a place-recognition candidate
+// are six problems of one call.  Result as RansacNonCentralRelativePose (model [R|t], X1 = R X2 + t, |t| = 1).
+struct CentralRelativePoseRansacProblem {
+  std::vector<double> bearings1, bearings2, sigma1, sigma2;   // 3n, 3n, n, n
+  std::vector<int32_t> samples;                               // 5 * n_samples
+};
+inline std::vector<NonCentralRelativePoseRansacResult> RansacCentralRelativePose(Context& ctx, const std::vector<CentralRelativePoseRansacProblem>& problems,
+                                                                                double threshold, int max_iterations, double probability = 0.99) {
+  const int n_prob = (int)problems.size();
+  const size_t n_samples = n_prob ? problems[0].samples.size() / 5 : 0;
+  std::vector<int32_t> ptr(n_prob + 1, 0), samples;
+  std::vector<double> f1, f2, s1, s2;
+  for (int i = 0; i < n_prob; i++) {
+    const CentralRelativePoseRansacProblem& p = problems[i];
+    const size_t n = p.sigma1.size();
+    if (p.samples.size() != 5 * n_samples || p.bearings1.size() != 3 * n || p.bearings2.size() != 3 * n || p.sigma2.size() != n)
+      throw std::invalid_argument("covins_b200::RansacCentralRelativePose: inconsistent problem sizes");
+    ptr[i + 1] = ptr[i] + (int32_t)n;
+    f1.insert(f1.end(), p.bearings1.begin(), p.bearings1.end()); f2.insert(f2.end(), p.bearings2.begin(), p.bearings2.end());
+    s1.insert(s1.end(), p.sigma1.begin(), p.sigma1.end()); s2.insert(s2.end(), p.sigma2.begin(), p.sigma2.end());
+    samples.insert(samples.end(), p.samples.begin(), p.samples.end());
+  }
+  const size_t m = n_prob > 0 ? n_prob : 1;
+  std::vector<int32_t> best(m), cnt(m), iters(m), used(m);
+  std::vector<double> models(12 * m);
+  std::vector<uint8_t> mask(ptr[n_prob] > 0 ? ptr[n_prob] : 1);
+  cvb_central_rel_ransac_problems P{n_prob, ptr.data(), f1.data(), f2.data(), s1.data(), s2.data(), samples.data(), (int32_t)n_samples};
+  cvb_rel_ransac_result R{best.data(), models.data(), cnt.data(), iters.data(), used.data(), mask.data(), nullptr, nullptr, nullptr};
+  ctx.check(cvb_ransac_central_relative_pose_batch(ctx.get(), &P, threshold, max_iterations, probability, &R), "cvb_ransac_central_relative_pose_batch");
+  std::vector<NonCentralRelativePoseRansacResult> out(n_prob);
+  for (int i = 0; i < n_prob; i++) {
+    out[i].best_sample = best[i]; out[i].n_inliers = cnt[i]; out[i].iterations = iters[i]; out[i].samples_used = used[i];
+    std::copy(models.begin() + 12 * i, models.begin() + 12 * (i + 1), out[i].model.begin());
+    out[i].inliers.assign(mask.begin() + ptr[i], mask.begin() + ptr[i + 1]);
+  }
+  return out;
+}
+
 // Resident-map descriptor database (cvb_db_*): the ORB descriptors of the map's keyframes live in HBM; the candidate
 // loop of PlaceRecognitionG::ComputeSE3 (placerec_gen_be.cpp:60-135) becomes one call per query keyframe.  The database
 // index of a keyframe is its insertion order; keep it next to the keyframe (e.g. std::map<idpair, int>).

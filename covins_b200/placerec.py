@@ -8,6 +8,7 @@ the C-ABI:
   ransac_absolute_pose(...)     ↔ the whole GP3P RANSAC of Se3Solver::projectiveAlignment from caller-supplied samples
   ransac_noncentral_relative_pose(...) ↔ the 17-point RANSAC of RelNonCentralPosSolver::computeNonCentralRelPose from
                                   caller-supplied samples
+  ransac_central_relative_pose(...) ↔ the 5-point RANSAC of RelNonCentralPosSolver::computePose from caller-supplied samples
 
 `KfView` flattens what the reference reads of a Keyframe (the C++ shim does the same from the containers)."""
 from __future__ import annotations
@@ -234,4 +235,31 @@ def ransac_noncentral_relative_pose(ctx: Context, prob_ptr, f1, f2, sigma1, sigm
     R = CRelRansacResult(*[r[k].ctypes.data if k in r else None for k, _ in CRelRansacResult._fields_])
     ctx.check(lib().cvb_ransac_noncentral_relative_pose_batch(ctx.handle, C.byref(P), float(threshold), int(max_iterations), float(probability),
                                                               C.byref(R)))
+    return r
+
+
+class CCentralRelRansacProblems(C.Structure):
+    _fields_ = [("n_prob", C.c_int32)] + [(k, c_vp) for k in ("prob_ptr", "f1", "f2", "sigma1", "sigma2", "samples")] + [("n_samples", C.c_int32)]
+
+
+def ransac_central_relative_pose(ctx: Context, prob_ptr, f1, f2, sigma1, sigma2, samples, threshold, max_iterations, probability=0.99,
+                                 per_sample=False):
+    """RelNonCentralPosSolver::computePose's 5-point RANSAC for a batch of problems (cvb_ransac_central_relative_pose_batch):
+    5-point hypothesis per sample, scoring and ransac_select-style selection on the GPU.  prob_ptr [n_prob+1] correspondence
+    ranges; f1 / f2 [N,3] unit bearings, sigma1 / sigma2 [N]; samples [n_prob, n_samples, 5] problem-local indices.
+    → dict(best_sample, best_model [n_prob,3,4] (X1 = R X2 + t, |t| = 1), best_count, iterations, consumed, inlier_mask [N]) and,
+    with per_sample, sample_model [n_prob,n_samples,3,4], sample_valid, sample_count."""
+    ptr = np.ascontiguousarray(prob_ptr, np.int32); n_prob = len(ptr) - 1
+    a = np.ascontiguousarray(f1, np.float64).reshape(-1, 3); b = np.ascontiguousarray(f2, np.float64).reshape(-1, 3)
+    s1 = np.ascontiguousarray(sigma1, np.float64).reshape(-1); s2 = np.ascontiguousarray(sigma2, np.float64).reshape(-1)
+    smp = np.ascontiguousarray(samples, np.int32).reshape(n_prob, -1, 5); ns = smp.shape[1]
+    r = dict(best_sample=np.zeros(n_prob, np.int32), best_model=np.zeros((n_prob, 3, 4)), best_count=np.zeros(n_prob, np.int32),
+             iterations=np.zeros(n_prob, np.int32), consumed=np.zeros(n_prob, np.int32), inlier_mask=np.zeros(len(a), np.uint8))
+    if per_sample:
+        r.update(sample_model=np.zeros((n_prob, ns, 3, 4)), sample_valid=np.zeros((n_prob, ns), np.uint8),
+                 sample_count=np.zeros((n_prob, ns), np.int32))
+    P = CCentralRelRansacProblems(n_prob, *[x.ctypes.data for x in (ptr, a, b, s1, s2, smp)], ns)
+    R = CRelRansacResult(*[r[k].ctypes.data if k in r else None for k, _ in CRelRansacResult._fields_])
+    ctx.check(lib().cvb_ransac_central_relative_pose_batch(ctx.handle, C.byref(P), float(threshold), int(max_iterations), float(probability),
+                                                           C.byref(R)))
     return r

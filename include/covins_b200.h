@@ -427,6 +427,62 @@ CVB_API int cvb_ransac_noncentral_relative_pose_batch(cvb_ctx* ctx, const cvb_re
                                                       double probability, cvb_rel_ransac_result* r);
 
 /*
+ * The central relative-pose RANSAC of RelNonCentralPosSolver::computePose (5-point, RelNonCentralPosSolver.cpp:343-377: opengv's
+ * Stewénius solver inside FrameRelativePoseSacProblem, run after each of the six pairwise matchings of
+ * computeNonCentralRelPose) for a batch of problems in one launch, from the caller's samples: 5-point solve, scoring, the
+ * sequential model selection of opengv's Ransac::computeModel and the inlier mask of the selected model.  Samples stay an input.
+ *   Model: [R|t] row-major 3x4 with X1 = R X2 + t, |t| = 1 (cvb_score_relative_pose_batch's [R12|t12] convention).
+ *   Hypothesis of a sample (5 problem-local indices), with only + - * / and sqrt, fixed iteration counts and fixed summation
+ *   order (bit-identical to a -ffp-contract=off C restatement):
+ *     1. q_i = vec(f1_i f2_i^T) (row-major, q_i . vec(E) = f1^T E f2).  Householder QR of Q^T (9x5); null-space basis
+ *        X, Y, Z, W = H_0..H_4 e_5..e_8.  The sample is invalid if min_k |r_kk| < 1e-10 max_k |r_kk|.
+ *     2. E = xX + yY + zZ + W; the nine entries of 2 E E^T E - tr(E E^T) E and det E give a 10x20 coefficient matrix in
+ *        Nistér's monomial order (Nistér 2004, §3).
+ *     3. Gauss-Jordan elimination of its left 10x10 block with partial pivoting (largest |value|, first row on ties); the
+ *        sample is invalid if a pivot is below 1e-10 times the largest |entry| of the matrix.  B(z) has rows <e> - z<f>,
+ *        <g> - z<h>, <i> - z<j>; n(z) = det B(z) has degree 10.  Real roots of n inside the Cauchy bound (invalid if it is not
+ *        finite): the real roots of n', n'', ... bracket those of n, so the roots of n^(9), n^(8), ..., n are found in turn,
+ *        one per sign change between consecutive roots of the previous derivative, by 64 bisection steps and 4 Newton steps
+ *        kept inside the bracket.  Per root, in ascending z: (x, y, 1) ~ the largest cross product of two rows of B(z) (the
+ *        first on ties), then at most 6 Gauss-Newton steps on the ten cubics in (x, y, z) (the first step that does not
+ *        lower their squared residual is undone and ends the polish), then E.
+ *     4. E scaled to tr(E E^T) / 2 = 1.  b = the largest of E's three column cross products (the first on ties), normalised:
+ *        the unit left null vector.  R_+- = cof(E) -+ [b]x E (cof(E)_ij = (-1)^(i+j) M_ij, not transposed): both are rotations
+ *        whatever the sign of E.  Candidates in this order: (R_+, b), (R_+, -b), (R_-, b), (R_-, -b).
+ *     5. quality = sum over the sample's 5 correspondences, in sample order, of (1 - f1 . X/|X|) + (1 - f2 . r2/|r2|), X and
+ *        r2 = R^T (X - t) from the score's triangulation.  The strictly lowest finite quality over roots x candidates wins.
+ *     The sample is also invalid if no real root or no finite candidate exists, the problem has fewer than 5 correspondences,
+ *     an index repeats within the sample, a bearing of the sample is not finite, or the model is not finite.
+ *     ASSUMPTIONS (opengv is not in the tree): Stewénius' eigen-decomposition is replaced by Nistér's polynomial, and only its
+ *     real roots are kept, where opengv takes the real parts of all ten complex solutions; |t| = 1, where opengv scales t by
+ *     E's largest singular value (the score does not depend on |t|); the quality test of
+ *     CentralRelativePoseSacProblem::computeModelCoefficients runs on the sample's points only.  Every solution satisfies the
+ *     five epipolar constraints, so on noise-free data several can tie near zero quality and rounding decides between them:
+ *     the chosen hypothesis of one sample need not be the true pose.
+ *   Score of correspondence i: exactly cvb_score_relative_pose_batch's per-correspondence score (the same device function),
+ *   inlier iff score < threshold.
+ *   Selection: as cvb_ransac_noncentral_relative_pose_batch with sample size 5.
+ * Inputs: correspondences concatenated over problems (prob_ptr[n_prob+1], prob_ptr[0] = 0): unit bearings f1[i], f2[i],
+ * sigma1[i], sigma2[i] as in cvb_score_relative_pose_batch; samples [n_prob][n_samples][5], indices local to their problem (the
+ * samples of a problem with fewer than 5 correspondences are not read).
+ * Outputs: cvb_rel_ransac_result, as cvb_ransac_noncentral_relative_pose_batch.
+ * Errors: CVB_ERR_INVALID before any launch for negative sizes, null required pointers, a decreasing prob_ptr, an out-of-range
+ * sample index, or per-sample outputs not requested together; n_prob = 0 succeeds.
+ */
+typedef struct cvb_central_rel_ransac_problems {
+  int32_t n_prob;
+  const int32_t* prob_ptr;   /* [n_prob+1], prob_ptr[0] = 0 */
+  const double* f1;          /* [N][3] unit bearings, camera 1 */
+  const double* f2;          /* [N][3] unit bearings, camera 2 */
+  const double* sigma1;      /* [N] */
+  const double* sigma2;      /* [N] */
+  const int32_t* samples;    /* [n_prob][n_samples][5], problem-local indices */
+  int32_t n_samples;
+} cvb_central_rel_ransac_problems;
+CVB_API int cvb_ransac_central_relative_pose_batch(cvb_ctx* ctx, const cvb_central_rel_ransac_problems* p, double threshold,
+                                                   int max_iterations, double probability, cvb_rel_ransac_result* r);
+
+/*
  * Optimization::OptimizeRelativePose(kf1, kf2, matches1, T12, th2) (optimization_be.cpp:620-831): the 6-dof refinement of
  * the relative pose T12 from the matched landmark pairs, both ceres::Solve calls (5 + 5 iterations, DOGLEG, CauchyLoss(1))
  * and the outlier purge between them, in one call.  The caller (shim) flattens, per residual pair r (the reference's

@@ -11,7 +11,11 @@ With --relative, the non-central relative-pose (17-point) RANSAC instead, at 5 %
   (b) host 17-point solves with the oracle (the first max_iterations samples of every problem, one thread), plus the oracle's
       selection over them (host scoring per camera pair, placerec.ransac_select);
   (c) the oracle RANSAC on the host cores.
-  python tools/ransac_timing.py [--reps 100] [--outlier 0.5] [--relative]"""
+With --central, the central relative-pose (5-point) RANSAC, n_prob 1, 6 and 60 (one and ten candidates x six pairings), 300 and
+1000 correspondences, 5 % and 30 % outliers:
+  (a) cvb_ransac_central_relative_pose_batch (whole call, and kernel time from torch.profiler);
+  (c) the oracle RANSAC on the host cores.
+  python tools/ransac_timing.py [--reps 100] [--outlier 0.5] [--relative | --central]"""
 import argparse
 import os
 import subprocess
@@ -32,9 +36,12 @@ def main():
     ap.add_argument("--n", type=int, default=1000)
     ap.add_argument("--samples", type=int, default=400)
     ap.add_argument("--relative", action="store_true", help="time the non-central relative-pose (17-point) RANSAC")
+    ap.add_argument("--central", action="store_true", help="time the central relative-pose (5-point) RANSAC")
     a = ap.parse_args()
     if a.relative:
         return relative(a)
+    if a.central:
+        return central(a)
     import torch
     import covins_b200
     from covins_b200 import placerec as PR
@@ -148,6 +155,50 @@ def relative(a):
             print(f"relative | outliers {outlier:.0%} | n_prob {n_prob:2d} x {a.n} corr, {a.samples} samples: iterations used "
                   f"{got['iterations'].min()}-{got['iterations'].max()} | (a) call {t_a:.3f} ms, kernel {k_a:.3f} ms | (b) host 17-pt solves + "
                   f"selection {t_b:.3f} ms | (c) oracle RANSAC on {os.cpu_count()} host cores {t_c:.3f} ms")
+    ctx.close()
+
+
+def central(a):
+    import torch
+    import covins_b200
+    from covins_b200 import placerec as PR
+    from oracle import ransac_rel5 as orel
+    from test_ransac_central import _batch
+    from torch.profiler import profile, ProfilerActivity
+    assert torch.cuda.is_available(), "needs a CUDA device"
+    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"], capture_output=True, text=True)
+    print(f"GPU: {torch.cuda.get_device_name(0)} | {q.stdout.strip()} | host cores: {os.cpu_count()}")
+    ctx = covins_b200.Context(0)
+    thr, max_it, prob = 9.0, 300, 0.99
+    kw = dict(threshold=thr, max_iterations=max_it, probability=prob)
+    for n in (300, 1000):
+        for outlier in (0.05, 0.3):
+            for n_prob in (1, 6, 60):
+                b, _ = _batch(300 + n_prob, [(n, outlier, False)] * n_prob, a.samples, repeat_frac=0.0)
+                ref = orel.ransac_central_relative_pose(**b, **kw)
+                got = PR.ransac_central_relative_pose(ctx, **b, **kw)
+                for k in ref:
+                    assert np.array_equal(ref[k], got[k]), k
+                for _ in range(3):
+                    PR.ransac_central_relative_pose(ctx, **b, **kw)
+                reps = max(3, a.reps // 10)
+                torch.cuda.synchronize()
+                t0 = time.perf_counter()
+                for _ in range(reps):
+                    PR.ransac_central_relative_pose(ctx, **b, **kw)
+                t_a = (time.perf_counter() - t0) / reps * 1e3
+                with profile(activities=[ProfilerActivity.CUDA]) as pr:
+                    for _ in range(5):
+                        PR.ransac_central_relative_pose(ctx, **b, **kw)
+                ev = [e for e in pr.events() if "ransac_rel_kernel" in e.name]
+                k_a = np.mean([e.device_time for e in ev]) / 1e3 if ev else float("nan")
+                t0 = time.perf_counter()
+                for _ in range(3):
+                    orel.ransac_central_relative_pose(**b, **kw)
+                t_c = (time.perf_counter() - t0) / 3 * 1e3
+                print(f"central | {n} corr | outliers {outlier:.0%} | n_prob {n_prob:2d}, {a.samples} samples: iterations used "
+                      f"{got['iterations'].min()}-{got['iterations'].max()} | (a) call {t_a:.3f} ms, kernel {k_a:.3f} ms | "
+                      f"(c) oracle RANSAC on {os.cpu_count()} host cores {t_c:.3f} ms | bit-identical to the oracle")
     ctx.close()
 
 
