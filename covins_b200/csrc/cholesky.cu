@@ -361,26 +361,61 @@ __global__ void __launch_bounds__(TILE_THREADS, 1) tile_update_kernel(double* __
 
 // Factor the diagonal tile k in shared memory and invert the factor, one CTA of 512 threads.  This kernel is the serial
 // chain of the whole factorisation (one launch per tile column, nothing else can run before its panel is solved), so it
-// is organised around dependent-operation latency (DFMA, SHFL, STS→LDS and rsqrt latencies on the critical chain):
-//   Cholesky: blocked right-looking, 16-wide block columns.  Per block column
-//     (a) warp 0 factors the 16x16 diagonal block register-resident (lane = 2*row + half).  Per pivot the *unscaled*
-//         column goes through 128 B of shared memory and the update uses a_rj * a_cj / pivot, so the chain per pivot is
-//         STS → LDS → reciprocal → DMUL → DFMA (≈ 100 cycles); rsqrt and the L values are computed off the chain;
-//     (b) one thread per row below solves its 16 unknowns by substitution against the block (in place, no scratch);
-//     (c) the trailing sub-matrix gets its rank-16 update with 4x4 register tiles whose rows are interleaved with stride
-//         n/4 (conflict-free shared-memory operand loads); one thread owns the product of row sets {tr+i*S} x {tc+j*S}
-//         and scatters it to both triangles' canonical (row >= col) positions;
-//     meanwhile warp 15 inverts the 16x16 diagonal block (needed only by the inverse phase) off the critical path.
-//   Inverse: in place by recursive doubling (16 → 32 → 64 → 128): X21 = -C^-1 (B A^-1), 4x4 register tiles with
-//   interleaved columns, a padded scratch tile; the 16x16 diagonal inverses come from the factorisation.
+// is organised around the latency of that chain: the eight 16x16 diagonal blocks, each factored by one warp, with
+// everything that does not feed the next diagonal block done beside it.  Blocked right-looking Cholesky over the 16-wide
+// block columns jb, two CTA barriers per block column:
+//   step 1  warp 0 factors the diagonal block (jb, jb) register-resident (lane = 2*row + half).  Per pivot the *unscaled*
+//           column goes through 128 B of shared memory and the update uses a_rj * a_cj / pivot, so the chain per pivot is
+//           STS → LDS → rsqrt → DMUL → DFMA (rsqrt and the L values are computed off the chain).  Meanwhile the 12
+//           warps that do not share warp 0's scheduler (warp w runs on sub-partition w % 4) apply block column jb-1's
+//           rank-16 update to the trailing blocks (look-ahead: the diagonal block itself got it at the end of the previous
+//           step 2) and finish block row jb-1 of the inverse;
+//   step 2  one thread per row below solves its 16 unknowns by substitution against the diagonal block, and warp 0,
+//           which owns the rows of the next diagonal block, applies their update to that block at once.  Meanwhile warp
+//           15 inverts the diagonal block and 8 warps form P_jb = L[jb,:jb] X[:jb,:jb] for the inverse.
+// The inverse X = L^-1 is built behind the factor by the block-row recurrence X[j,:j] = -X[j,j] P_j, which follows from
+// XL = I and keeps the left residual |XL - I| small; X[j,j] comes from warp 15.  When the last diagonal block is factored
+// only block row 7 of X is left.  Every 16x16x16 product (trailing update, P_j, X[j,j] P_j) is two mma.sync.m16n8k16.f64
+// on one warp.  Results go to global memory as soon as they are final, off the chain: X's blocks from the registers that
+// formed them, L's block column jb-1 by the step-1 warps of block column jb.  L lives in the lower triangle of the tile `a`, the off-diagonal blocks of X
+// transposed in its upper triangle (X[j,c] as block (c,j)), the X[j,j] in `binv`.  Row strides ≡ 4 doubles mod 16 make
+// the fragment loads of a half-warp (rows g = 0..3, columns t = 0..3, or the transpose) hit 16 different banks.
 // L is written back to S, the inverse (row-major 128x128, zeros above the diagonal) to linv_k.  flag[0] |= 1 on a
 // non-positive pivot (matrix not positive definite → the caller raises mu, as Ceres does on LINEAR_SOLVER_FAILURE).
-constexpr int LDP = T + 1;
 constexpr int PB = 16;
+constexpr int NB = T / PB;      // block columns of the tile
+constexpr int LDP = T + 4;      // row stride of the tile in shared memory
+constexpr int BLD = PB + 4;     // row stride of binv and of the P_j scratch
 constexpr int POTRF_THREADS = 512;
-constexpr int POTRF_WORKERS = POTRF_THREADS - 32;   // warp 15 inverts the diagonal blocks
-constexpr int TMP_DOUBLES = 64 * 65;
-constexpr size_t kPotrfSmem = ((size_t)T * LDP + (size_t)TMP_DOUBLES + (size_t)(T / PB) * PB * PB + 5 * PB) * sizeof(double);
+constexpr int POTRF_WARPS = POTRF_THREADS / 32;
+constexpr size_t kPotrfSmem =
+    ((size_t)T * LDP + (size_t)NB * PB * BLD + (size_t)(T - PB) * BLD + 5 * PB) * sizeof(double);   // 174208 B
+
+// c[h] += A B^T over one 16x16x16 block, as two m16n8k16 (c[h] = columns 8h.. of the output, in dmma16816's C-fragment
+// order).  A(r,k) = A[r lda + k] (negated when NEG: exact); B(n,k) = B[n ldb + k], or B[k ldb + n] when BT.
+template <bool NEG, bool BT>
+__device__ __forceinline__ void mma16(double (&c)[2][4], const double* A, int lda, const double* B, int ldb) {
+  const int lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
+  double a[8];
+#pragma unroll
+  for (int e = 0; e < 8; e++) {
+    const double v = A[(g + 8 * (e & 1)) * lda + t + 4 * (e >> 1)];
+    a[e] = NEG ? -v : v;
+  }
+#pragma unroll
+  for (int h = 0; h < 2; h++) {
+    double b[4];
+#pragma unroll
+    for (int e = 0; e < 4; e++) b[e] = BT ? B[(t + 4 * e) * ldb + 8 * h + g] : B[(8 * h + g) * ldb + t + 4 * e];
+    dmma16816(c[h], a, b);
+  }
+}
+// offset of element c[h][e] of mma16's output in a 16x16 block with row stride ld (TR: the block stored transposed)
+template <bool TR>
+__device__ __forceinline__ int frag_off(int h, int e, int ld) {
+  const int lane = threadIdx.x & 31, r = (lane >> 2) + 8 * (e >> 1), c = 8 * h + 2 * (lane & 3) + (e & 1);
+  return TR ? c * ld + r : r * ld + c;
+}
 
 #define POTRF_MARK(i)                                     \
   do {                                                    \
@@ -391,13 +426,55 @@ __global__ void __launch_bounds__(POTRF_THREADS, 1) potrf_inv_kernel(double* __r
                                                                      double* __restrict__ linv_k, int* __restrict__ flag,
                                                                      long long* __restrict__ prof, int prof_fine) {
   extern __shared__ __align__(16) double smem_d[];
-  double* a = smem_d;                     // [T][LDP]
-  double* tmp = smem_d + T * LDP;         // scratch of the inverse phase
-  double* binv = tmp + TMP_DOUBLES;       // [8][16][16] inverses of the diagonal 16x16 blocks of L
-  double* colbuf = binv + (T / PB) * PB * PB;   // [2][2*PB] pivot-column exchange (second half: dummy slots)
-  double* rdbuf = colbuf + 4 * PB;              // [PB] reciprocal diagonal of the current diagonal block
+  double* a = smem_d;                          // [T][LDP]: L on and below the diagonal, X^T above it
+  double* binv = a + T * LDP;                  // [NB][PB][BLD]: X[j,j] = L[j,j]^-1
+  double* pt = binv + NB * PB * BLD;           // [T - PB][BLD]: P_j^T
+  double* colbuf = pt + (T - PB) * BLD;        // [2][2*PB] pivot-column exchange (second half: dummy slots)
+  double* rdbuf = colbuf + 4 * PB;             // [PB] reciprocal diagonal of the current diagonal block
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   double* At = S + (size_t)k * T * ld + (size_t)k * T;
+  auto blk = [&](int i, int j) { return a + i * PB * LDP + j * PB; };
+  // A(i,m) -= L(i,jb) L(m,jb)^T on one 16x16 block (one warp)
+  auto update_block = [&](int i, int m, int jb) {
+    double* C = blk(i, m);
+    double c[2][4];
+#pragma unroll
+    for (int h = 0; h < 2; h++)
+#pragma unroll
+      for (int e = 0; e < 4; e++) c[h][e] = C[frag_off<false>(h, e, LDP)];
+    mma16<true, false>(c, blk(i, jb), LDP, blk(m, jb), LDP);
+#pragma unroll
+    for (int h = 0; h < 2; h++)
+#pragma unroll
+      for (int e = 0; e < 4; e++) C[frag_off<false>(h, e, LDP)] = c[h][e];
+  };
+  // L's block column jb (rows >= 16 jb, on and below the diagonal) from shared memory to S
+  auto store_l = [&](int jb, int u0, int nthr) {
+    const int c0 = jb * PB;
+    for (int u = u0; u < (T - c0) * (PB / 2); u += nthr) {
+      const int r = c0 + u / (PB / 2), c = c0 + 2 * (u % (PB / 2));
+      if (c + 1 <= r)
+        *reinterpret_cast<double2*>(At + (size_t)r * ld + c) = make_double2(a[r * LDP + c], a[r * LDP + c + 1]);
+      else if (c <= r)
+        At[(size_t)r * ld + c] = a[r * LDP + c];
+    }
+  };
+  // X[j,c] = -X[j,j] P_j[:,c] (one warp): kept transposed as block (c,j) for the later P's, and written to linv_k
+  auto finish_x = [&](int j, int c) {
+    double x[2][4] = {};
+    mma16<true, false>(x, binv + j * PB * BLD, BLD, pt + c * PB * BLD, BLD);
+    double* D = blk(c, j);
+#pragma unroll
+    for (int h = 0; h < 2; h++)
+#pragma unroll
+      for (int e = 0; e < 4; e++) D[frag_off<true>(h, e, LDP)] = x[h][e];
+#pragma unroll
+    for (int h = 0; h < 2; h++)
+#pragma unroll
+      for (int e = 0; e < 4; e += 2)
+        *reinterpret_cast<double2*>(linv_k + (size_t)(j * PB) * T + c * PB + frag_off<false>(h, e, T)) =
+            make_double2(x[h][e], x[h][e + 1]);
+  };
   POTRF_MARK(0);
   {
     // all 16 16-byte loads of a thread are in flight before the first use (one L2/HBM round trip for the tile)
@@ -416,13 +493,13 @@ __global__ void __launch_bounds__(POTRF_THREADS, 1) potrf_inv_kernel(double* __r
   }
   __syncthreads();
   POTRF_MARK(1);
-  // ---------------- Cholesky ----------------
-  long long t_a = 0, acc_a = 0, acc_ab = 0, acc_b = 0, acc_c = 0;   // fine profile (thread 0 only), kept in registers
-  for (int jb = 0; jb < T / PB; jb++) {
+  long long t_a = 0, acc_a = 0, acc_1 = 0, acc_2 = 0;   // fine profile (thread 0 only), kept in registers
+  for (int jb = 0; jb < NB; jb++) {
     const int c0 = jb * PB, nbelow = T - c0 - PB;
     if (prof_fine && tid == 0) t_a = clock64();
+    // ---------------- step 1 ----------------
     if (warp == 0) {
-      // (a) the 16x16 diagonal block.  Branch-free pivot loop: every lane stores one value per step (lanes of the other
+      // the 16x16 diagonal block.  Branch-free pivot loop: every lane stores one value per step (lanes of the other
       // column half into a dummy slot), readers mask by row index; a non-positive pivot only sets a flag bit.
       const int r = lane >> 1, hf = lane & 1;
       double v[8];
@@ -463,12 +540,38 @@ __global__ void __launch_bounds__(POTRF_THREADS, 1) potrf_inv_kernel(double* __r
 #pragma unroll
       for (int c = 0; c < 8; c++) a[(c0 + r) * LDP + c0 + hf * 8 + c] = (hf * 8 + c <= r) ? v[c] : 0.0;
       if (prof_fine && tid == 0) acc_a += clock64() - t_a;
+    } else if ((warp & 3) != 0) {
+      // The 12 warps that do not share warp 0's scheduler (warps 4, 8, 12 stay idle: they would take issue slots from
+      // the pivot chain): block column jb-1's update of the trailing blocks (i, m), jb <= m <= i, (jb, jb) excepted
+      // (numbered row by row), then the blocks X[jb-1, c], c < jb-1, of the inverse, then L's block column jb-1.
+      // In block column 0 they write the zeros of X right of its diagonal blocks instead.
+      const int w = warp - (warp >> 2) - 1, nw = POTRF_WARPS * 3 / 4;
+      if (jb == 0) {
+        for (int u = w * 32 + lane; u < T * T / 2; u += nw * 32) {
+          const int r = u / (T / 2), c = (u % (T / 2)) * 2;
+          if (c >= (r | (PB - 1)) + 1) reinterpret_cast<double2*>(linv_k)[u] = make_double2(0.0, 0.0);
+        }
+      } else {
+        const int nt = NB - jb, nupd = nt * (nt + 1) / 2 - 1;
+#pragma unroll 1
+        for (int u = w; u < nupd + jb - 1; u += nw) {
+          if (u < nupd) {
+            int i = 0;
+            while ((i + 1) * (i + 2) / 2 <= u + 1) i++;
+            update_block(jb + i, jb + (u + 1 - i * (i + 1) / 2), jb - 1);
+          } else {
+            finish_x(jb - 1, u - nupd);
+          }
+        }
+        store_l(jb - 1, w * 32 + lane, nw * 32);
+      }
     }
     __syncthreads();
-    if (prof_fine && tid == 0) { const long long tt = clock64(); acc_ab += tt - t_a; t_a = tt; }
-    if (warp == POTRF_THREADS / 32 - 1) {
-      // inverse of the diagonal block, off the critical path: lane j (< 16) builds column j of Ljj^-1 by forward
-      // substitution in axpy form (16 dependent steps, the row updates of a step are independent)
+    if (prof_fine && tid == 0) { const long long tt = clock64(); acc_1 += tt - t_a; t_a = tt; }
+    // ---------------- step 2 ----------------
+    if (warp == POTRF_WARPS - 1) {
+      // inverse of the diagonal block: lane j (< 16) builds column j of Ljj^-1 by forward substitution in axpy form
+      // (16 dependent steps, the row updates of a step are independent)
       if (lane < PB) {
         const int j = lane;
         double res[PB];
@@ -482,151 +585,62 @@ __global__ void __launch_bounds__(POTRF_THREADS, 1) potrf_inv_kernel(double* __r
           for (int q = m + 1; q < PB; q++) res[q] -= a[(c0 + q) * LDP + c0 + m] * xm;
         }
 #pragma unroll
-        for (int q = 0; q < PB; q++) binv[(jb * PB + q) * PB + j] = res[q];   // Linv_block[q][j]
-      }
-    } else if (nbelow > 0) {
-      // (b) panel: row r of X solves X Ljj^T = A(r, block), one thread per row, in place
-      if (tid < nbelow) {
-        const int r = c0 + PB + tid;
-        double x[PB];
-#pragma unroll
-        for (int m = 0; m < PB; m++) x[m] = a[r * LDP + c0 + m];
-#pragma unroll
-        for (int m = 0; m < PB; m++) {
-          const double xm = x[m] * rdbuf[m];
-          x[m] = xm;
-#pragma unroll
-          for (int q = m + 1; q < PB; q++) x[q] -= a[(c0 + q) * LDP + c0 + m] * xm;
+        for (int q = 0; q < PB; q++) {
+          binv[(jb * PB + q) * BLD + j] = res[q];   // Linv_block[q][j]
+          linv_k[(size_t)(c0 + q) * T + c0 + j] = (q >= j) ? res[q] : 0.0;
         }
-#pragma unroll
-        for (int m = 0; m < PB; m++) a[r * LDP + c0 + m] = x[m];
       }
-    }
-    __syncthreads();   // (the last block column has no panel; warp 15 still finishes its inverse before the barrier)
-    if (prof_fine && tid == 0) { const long long tt = clock64(); acc_b += tt - t_a; t_a = tt; }
-    if (nbelow > 0) {
-      // (c) trailing update A[r][c] -= sum_{m<16} L[r][c0+m] L[c][c0+m] for r >= c >= c0+16
-      const int Sx = nbelow / 4, ntiles = Sx * (Sx + 1) / 2, base = c0 + PB;
-      if (tid < POTRF_WORKERS)
-        for (int u = tid; u < ntiles; u += POTRF_WORKERS) {
-          int tr = (int)((sqrtf(8.0f * (float)u + 1.0f) - 1.0f) * 0.5f);
-          while ((tr + 1) * (tr + 2) / 2 <= u) tr++;
-          while (tr * (tr + 1) / 2 > u) tr--;
-          const int tc = u - tr * (tr + 1) / 2;   // tc <= tr
-          const double* P = a + (base + tr) * LDP + c0;
-          const double* Q = a + (base + tc) * LDP + c0;
-          double g[4][4];
+    } else if (warp >= 4 && (warp & 3) != 0) {
+      // P_jb^T: P_jb[:, c] = sum_{m = c..jb-1} L(jb,m) X(m,c) for c < jb, in increasing m (on the 8 warps 5-7, 9-11,
+      // 13-14: not beside warp 0 on its scheduler)
+      for (int c = warp - 4 - (warp >> 2); c < jb; c += 8) {
+        double p[2][4] = {};
+        mma16<false, true>(p, blk(jb, c), LDP, binv + c * PB * BLD, BLD);
+        for (int m = c + 1; m < jb; m++) mma16<false, false>(p, blk(jb, m), LDP, blk(c, m), LDP);
+        double* D = pt + c * PB * BLD;
 #pragma unroll
-          for (int i = 0; i < 4; i++)
+        for (int h = 0; h < 2; h++)
 #pragma unroll
-            for (int j = 0; j < 4; j++) g[i][j] = 0.0;
-#pragma unroll 4
-          for (int m = 0; m < PB; m++) {
-            double pv[4], qv[4];
+          for (int e = 0; e < 4; e++) D[frag_off<true>(h, e, BLD)] = p[h][e];
+      }
+    } else if (tid < nbelow) {
+      // panel: row r of X solves X Ljj^T = A(r, block), one thread per row, in place
+      const int r = c0 + PB + tid;
+      double x[PB];
 #pragma unroll
-            for (int i = 0; i < 4; i++) { pv[i] = P[i * Sx * LDP + m]; qv[i] = Q[i * Sx * LDP + m]; }
-#pragma unroll
-            for (int i = 0; i < 4; i++)
-#pragma unroll
-              for (int j = 0; j < 4; j++) g[i][j] += pv[i] * qv[j];
-          }
-          // g[i][j] = <row tr+i*Sx, row tc+j*Sx>: canonical position is (larger row index, smaller row index)
-#pragma unroll
-          for (int i = 0; i < 4; i++)
-#pragma unroll
-            for (int j = 0; j < 4; j++) {
-              const int ri = base + tr + i * Sx, cj = base + tc + j * Sx;
-              if (j <= i) a[ri * LDP + cj] -= g[i][j];
-              else if (tr != tc) a[cj * LDP + ri] -= g[i][j];
-            }
-        }
-      __syncthreads();
-      if (prof_fine && tid == 0) acc_c += clock64() - t_a;
-    }
-  }
-  POTRF_MARK(2);
-  if (prof_fine && tid == 0) { prof[6] = acc_a; prof[7] = acc_ab; prof[8] = acc_b; prof[9] = acc_c; }
-  for (int u = tid; u < T * T / 2; u += POTRF_THREADS) {
-    const int r = u / (T / 2), c = (u % (T / 2)) * 2;
-    if (c + 1 <= r)
-      *reinterpret_cast<double2*>(At + (size_t)r * ld + c) = make_double2(a[r * LDP + c], a[r * LDP + c + 1]);
-    else if (c <= r)
-      At[(size_t)r * ld + c] = a[r * LDP + c];
-  }
-  __syncthreads();
-  POTRF_MARK(3);
-  // ---------------- inverse of L, in place ----------------
-  // level 0: the diagonal 16x16 blocks were inverted during the factorisation
-  for (int u = tid; u < (T / PB) * PB * PB; u += POTRF_THREADS) {
-    const int blk = u / (PB * PB), r = (u / PB) % PB, c = u % PB;
-    a[(blk * PB + r) * LDP + blk * PB + c] = binv[u];
-  }
-  __syncthreads();
-  // levels h = 16, 32, 64: for each pair (A = inv at [p,p], C = inv at [p+h,p+h], B at [p+h,p]):
-  //   tmp = B * A  (A lower triangular),  B <- -C * tmp  (C lower triangular).  A thread owns rows r0..r0+3 and the
-  //   interleaved columns {ct + j*h/4}: lanes run along ct → conflict-free operand loads.
-  for (int h = PB; h < T; h *= 2) {
-    const int npairs = T / (2 * h), h4 = h / 4, ldt = h + 1;
-    for (int u = tid; u < npairs * h4 * h4; u += POTRF_THREADS) {
-      const int pr = u / (h4 * h4), r0 = 4 * ((u / h4) % h4), ct = u % h4;
-      const int p0 = pr * 2 * h;
-      double c4[4][4];
-#pragma unroll
-      for (int i = 0; i < 4; i++)
-#pragma unroll
-        for (int j = 0; j < 4; j++) c4[i][j] = 0.0;
-      // (B A)[r][c] = sum_m B[r][m] A[m][c]; A[m][c] = 0 for m < c, the smallest column of the thread is ct
-      const double* Bp = a + (p0 + h + r0) * LDP + p0;
-      const double* Ap = a + p0 * LDP + p0 + ct;
-      for (int m = ct; m < h; m++) {
-        double bv[4], av[4];
-#pragma unroll
-        for (int i = 0; i < 4; i++) { bv[i] = Bp[i * LDP + m]; av[i] = Ap[m * LDP + i * h4]; }
-#pragma unroll
-        for (int i = 0; i < 4; i++)
-#pragma unroll
-          for (int j = 0; j < 4; j++) c4[i][j] += bv[i] * av[j];
+      for (int m = 0; m < PB; m += 2) {
+        const double2 v = *reinterpret_cast<const double2*>(a + r * LDP + c0 + m);
+        x[m] = v.x;
+        x[m + 1] = v.y;
       }
 #pragma unroll
-      for (int i = 0; i < 4; i++)
+      for (int m = 0; m < PB; m++) {
+        const double xm = x[m] * rdbuf[m];
+        x[m] = xm;
 #pragma unroll
-        for (int j = 0; j < 4; j++) tmp[pr * h * ldt + (r0 + i) * ldt + ct + j * h4] = c4[i][j];
+        for (int q = m + 1; q < PB; q++) x[q] -= a[(c0 + q) * LDP + c0 + m] * xm;
+      }
+#pragma unroll
+      for (int m = 0; m < PB; m += 2) *reinterpret_cast<double2*>(a + r * LDP + c0 + m) = make_double2(x[m], x[m + 1]);
+    }
+    if (warp == 0 && nbelow > 0) {   // the next diagonal block gets this block column's update now (its rows are warp 0's)
+      __syncwarp();
+      update_block(jb + 1, jb + 1, jb);
     }
     __syncthreads();
-    for (int u = tid; u < npairs * h4 * h4; u += POTRF_THREADS) {
-      const int pr = u / (h4 * h4), r0 = 4 * ((u / h4) % h4), ct = u % h4;
-      const int p0 = pr * 2 * h;
-      double c4[4][4];
-#pragma unroll
-      for (int i = 0; i < 4; i++)
-#pragma unroll
-        for (int j = 0; j < 4; j++) c4[i][j] = 0.0;
-      // (C tmp)[r][c] = sum_{m <= r} C[r][m] tmp[m][c]   (C[r][m] = 0 above the diagonal)
-      const double* Cp = a + (p0 + h + r0) * LDP + p0 + h;
-      const double* Tp = tmp + pr * h * ldt + ct;
-      for (int m = 0; m < r0 + 4; m++) {
-        double cv[4], tv[4];
-#pragma unroll
-        for (int i = 0; i < 4; i++) { cv[i] = Cp[i * LDP + m]; tv[i] = Tp[m * ldt + i * h4]; }
-#pragma unroll
-        for (int i = 0; i < 4; i++)
-#pragma unroll
-          for (int j = 0; j < 4; j++) c4[i][j] += cv[i] * tv[j];
-      }
-#pragma unroll
-      for (int i = 0; i < 4; i++)
-#pragma unroll
-        for (int j = 0; j < 4; j++) a[(p0 + h + r0 + i) * LDP + p0 + ct + j * h4] = -c4[i][j];
-    }
-    __syncthreads();
+    if (prof_fine && tid == 0) { const long long tt = clock64(); acc_2 += tt - t_a; t_a = tt; }
+    if (jb == NB / 2 - 1) POTRF_MARK(2);
+    if (jb == NB - 3) POTRF_MARK(3);
   }
   POTRF_MARK(4);
-  for (int u = tid; u < T * T / 2; u += POTRF_THREADS) {
-    const int r = u / (T / 2), c = (u % (T / 2)) * 2;
-    reinterpret_cast<double2*>(linv_k)[u] =
-        make_double2((c <= r) ? a[r * LDP + c] : 0.0, (c + 1 <= r) ? a[r * LDP + c + 1] : 0.0);
+  // block row NB-1 of the inverse, the last diagonal block of L
+  if (warp < NB - 1) finish_x(NB - 1, warp);
+  else store_l(NB - 1, tid - (NB - 1) * 32, POTRF_THREADS - (NB - 1) * 32);
+  if (prof != nullptr) {
+    __syncthreads();
+    POTRF_MARK(5);
+    if (prof_fine && tid == 0) { prof[6] = acc_a; prof[7] = acc_1; prof[8] = acc_2; prof[9] = clock64() - t_a; }
   }
-  POTRF_MARK(5);
 }
 
 // Triangular solves.  One launch per tile column; every CTA recomputes the tiny diagonal product (128x128 mat-vec with
@@ -1216,8 +1230,10 @@ int solve(cvb_ctx* ctx, const double* L, const double* linv, double* b, double* 
 // ---- test/diagnostic entry: solve A x = b for a host SPD matrix (row-major n x n) with the BA factorisation ----
 // Latency of the diagonal-tile kernel (the serial chain of the tiled factorisation): factors `reps` copies of a synthetic
 // SPD tile back to back; us_per_tile = average launch-to-launch time; phase_cycles[0..5] = clock64 marks of the last
-// launch relative to its start (loaded, factored, L stored, inverted, Linv stored); summed over the 8 block columns:
-// [6] = inside the 16x16 diagonal-block step, [7] = the same incl. the closing barrier, [8] = panel, [9] = trailing update.
+// launch relative to its start (loaded, 4 and 6 of the 8 block columns factored, factored, inverted); summed over the 8
+// block columns: [6] = the 16x16 diagonal-block factorisations, [7] = step 1 (diagonal block beside the trailing update)
+// incl. its barrier, [8] = step 2 (panel beside the inverse's products) incl. its barrier; [9] = the inverse's last block
+// row after the last block column.
 extern "C" int cvb_microbench_potrf(cvb_ctx* ctx, int reps, double* us_per_tile, int64_t* phase_cycles) {
   if (!ctx || reps < 1 || !us_per_tile) return CVB_ERR_INVALID;
   CVB_GUARD(ctx);

@@ -8,7 +8,8 @@ from covins_b200._lib import lib
 ctx = covins_b200.Context(0)
 us = C.c_double(); ph = np.zeros(10, np.int64)
 ctx.check(lib().cvb_microbench_potrf(ctx.handle, 200, C.byref(us), ph.ctypes.data_as(C.c_void_p)))
-names = ["start", "loaded", "factored", "L stored", "inverted", "Linv stored", "sum diag-block steps", "sum (a)+barrier", "sum panel (b)", "sum trailing (c)"]
+names = ["start", "loaded", "4 block cols factored", "6 block cols factored", "factored", "inverted",
+         "sum diag-block steps", "sum step 1 + barrier", "sum step 2 + barrier", "last inverse block row"]
 print(f"potrf_inv_kernel: {us.value:.1f} us per tile (back-to-back launches)")
 for n, v in zip(names, ph):
     print(f"  {n:22s} {int(v):8d} cycles")
