@@ -1033,36 +1033,55 @@ struct NonCentralRelativePoseRansacResult {
   int n_inliers = 0, iterations = 0, samples_used = 0;
   std::vector<uint8_t> inliers;     // n flags of the selected model
 };
-inline std::vector<NonCentralRelativePoseRansacResult> RansacNonCentralRelativePose(Context& ctx,
-                                                                                   const std::vector<NonCentralRelativePoseRansacProblem>& problems,
-                                                                                   double threshold, int max_iterations, double probability = 0.99) {
-  const int n_prob = (int)problems.size();
-  const size_t n_samples = n_prob ? problems[0].samples.size() / 17 : 0;
-  std::vector<int32_t> ptr(n_prob + 1, 0), cp1(n_prob + 1, 0), cp2(n_prob + 1, 0), cam1, cam2, samples;
+namespace detail {
+// a batch of non-central problems flattened into the arrays of cvb_rel_ransac_problems
+struct FlatRelProblems {
+  std::vector<int32_t> ptr, cp1, cp2, cam1, cam2, samples;
   std::vector<double> f1, f2, s1, s2, co1, cr1, co2, cr2;
+  int32_t n_samples = 0;
+  cvb_rel_ransac_problems view() const {
+    return cvb_rel_ransac_problems{(int32_t)ptr.size() - 1, ptr.data(), f1.data(), f2.data(), s1.data(), s2.data(), cam1.data(), cam2.data(),
+                                   cp1.data(), co1.data(), cr1.data(), cp2.data(), co2.data(), cr2.data(), samples.data(), n_samples};
+  }
+};
+inline FlatRelProblems flatten_rel_problems(const std::vector<NonCentralRelativePoseRansacProblem>& problems, const char* what) {
+  const int n_prob = (int)problems.size();
+  FlatRelProblems F;
+  const size_t n_samples = n_prob ? problems[0].samples.size() / 17 : 0;
+  F.n_samples = (int32_t)n_samples;
+  F.ptr.assign(n_prob + 1, 0); F.cp1.assign(n_prob + 1, 0); F.cp2.assign(n_prob + 1, 0);
   for (int i = 0; i < n_prob; i++) {
     const NonCentralRelativePoseRansacProblem& p = problems[i];
     const size_t n = p.sigma1.size();
     if (p.samples.size() != 17 * n_samples || p.bearings1.size() != 3 * n || p.bearings2.size() != 3 * n || p.sigma2.size() != n ||
         p.cam1.size() != n || p.cam2.size() != n || p.rig1_rotations.size() != 3 * p.rig1_offsets.size() ||
         p.rig2_rotations.size() != 3 * p.rig2_offsets.size() || p.rig1_offsets.size() % 3 || p.rig2_offsets.size() % 3)
-      throw std::invalid_argument("covins_b200::RansacNonCentralRelativePose: inconsistent problem sizes");
-    ptr[i + 1] = ptr[i] + (int32_t)n;
-    cp1[i + 1] = cp1[i] + (int32_t)(p.rig1_offsets.size() / 3);
-    cp2[i + 1] = cp2[i] + (int32_t)(p.rig2_offsets.size() / 3);
-    f1.insert(f1.end(), p.bearings1.begin(), p.bearings1.end()); f2.insert(f2.end(), p.bearings2.begin(), p.bearings2.end());
-    s1.insert(s1.end(), p.sigma1.begin(), p.sigma1.end()); s2.insert(s2.end(), p.sigma2.begin(), p.sigma2.end());
-    cam1.insert(cam1.end(), p.cam1.begin(), p.cam1.end()); cam2.insert(cam2.end(), p.cam2.begin(), p.cam2.end());
-    co1.insert(co1.end(), p.rig1_offsets.begin(), p.rig1_offsets.end()); cr1.insert(cr1.end(), p.rig1_rotations.begin(), p.rig1_rotations.end());
-    co2.insert(co2.end(), p.rig2_offsets.begin(), p.rig2_offsets.end()); cr2.insert(cr2.end(), p.rig2_rotations.begin(), p.rig2_rotations.end());
-    samples.insert(samples.end(), p.samples.begin(), p.samples.end());
+      throw std::invalid_argument(std::string("covins_b200::") + what + ": inconsistent problem sizes");
+    F.ptr[i + 1] = F.ptr[i] + (int32_t)n;
+    F.cp1[i + 1] = F.cp1[i] + (int32_t)(p.rig1_offsets.size() / 3);
+    F.cp2[i + 1] = F.cp2[i] + (int32_t)(p.rig2_offsets.size() / 3);
+    F.f1.insert(F.f1.end(), p.bearings1.begin(), p.bearings1.end()); F.f2.insert(F.f2.end(), p.bearings2.begin(), p.bearings2.end());
+    F.s1.insert(F.s1.end(), p.sigma1.begin(), p.sigma1.end()); F.s2.insert(F.s2.end(), p.sigma2.begin(), p.sigma2.end());
+    F.cam1.insert(F.cam1.end(), p.cam1.begin(), p.cam1.end()); F.cam2.insert(F.cam2.end(), p.cam2.begin(), p.cam2.end());
+    F.co1.insert(F.co1.end(), p.rig1_offsets.begin(), p.rig1_offsets.end()); F.cr1.insert(F.cr1.end(), p.rig1_rotations.begin(), p.rig1_rotations.end());
+    F.co2.insert(F.co2.end(), p.rig2_offsets.begin(), p.rig2_offsets.end()); F.cr2.insert(F.cr2.end(), p.rig2_rotations.begin(), p.rig2_rotations.end());
+    F.samples.insert(F.samples.end(), p.samples.begin(), p.samples.end());
   }
+  return F;
+}
+}  // namespace detail
+
+inline std::vector<NonCentralRelativePoseRansacResult> RansacNonCentralRelativePose(Context& ctx,
+                                                                                   const std::vector<NonCentralRelativePoseRansacProblem>& problems,
+                                                                                   double threshold, int max_iterations, double probability = 0.99) {
+  const int n_prob = (int)problems.size();
+  const detail::FlatRelProblems F = detail::flatten_rel_problems(problems, "RansacNonCentralRelativePose");
+  const std::vector<int32_t>& ptr = F.ptr;
   const size_t m = n_prob > 0 ? n_prob : 1;
   std::vector<int32_t> best(m), cnt(m), iters(m), used(m);
   std::vector<double> models(12 * m);
   std::vector<uint8_t> mask(ptr[n_prob] > 0 ? ptr[n_prob] : 1);
-  cvb_rel_ransac_problems P{n_prob,     ptr.data(), f1.data(), f2.data(), s1.data(),  s2.data(),  cam1.data(),    cam2.data(),
-                            cp1.data(), co1.data(), cr1.data(), cp2.data(), co2.data(), cr2.data(), samples.data(), (int32_t)n_samples};
+  const cvb_rel_ransac_problems P = F.view();
   cvb_rel_ransac_result R{best.data(), models.data(), cnt.data(), iters.data(), used.data(), mask.data(), nullptr, nullptr, nullptr};
   ctx.check(cvb_ransac_noncentral_relative_pose_batch(ctx.get(), &P, threshold, max_iterations, probability, &R),
             "cvb_ransac_noncentral_relative_pose_batch");
@@ -1071,6 +1090,39 @@ inline std::vector<NonCentralRelativePoseRansacResult> RansacNonCentralRelativeP
     out[i].best_sample = best[i]; out[i].n_inliers = cnt[i]; out[i].iterations = iters[i]; out[i].samples_used = used[i];
     std::copy(models.begin() + 12 * i, models.begin() + 12 * (i + 1), out[i].model.begin());
     out[i].inliers.assign(mask.begin() + ptr[i], mask.begin() + ptr[i + 1]);
+  }
+  return out;
+}
+
+// The sampling-based 6x6 covariance of RelNonCentralPosSolver::computeNonCentralRelPose (RelNonCentralPosSolver.cpp:199,236,
+// 276-279) for a batch of candidates in one call (cvb_noncentral_relative_pose_covariance_batch), in place of the loop of up to
+// 300 host 17-point solves per candidate.  problems[i] are the candidate's correspondences and rigs, with samples = the
+// covariance samples (17 local indices each, normally drawn from ransac_results[i].inliers); the reference model is
+// ransac_results[i].model (all zeros when the RANSAC found none: the problem is skipped, n_valid = 0).  Per sample a 17-point
+// re-solve and its deviation [2 vec(q); t_s - t_ref], q the quaternion of R_ref^T R_s; cov = the mean of delta delta^T over the
+// valid samples (0 when none is).  cov (row-major, rotation then translation) is what LoopConstraint::cov_mat takes;
+// PoseGraphOptimization whitens the loop edge with it and needs it positive definite.
+struct RelativePoseCovariance {
+  std::array<double, 36> cov{};
+  int n_valid = 0;
+};
+inline std::vector<RelativePoseCovariance> NonCentralRelativePoseCovariance(Context& ctx, const std::vector<NonCentralRelativePoseRansacProblem>& problems,
+                                                                            const std::vector<NonCentralRelativePoseRansacResult>& ransac_results) {
+  const int n_prob = (int)problems.size();
+  if (ransac_results.size() != problems.size())
+    throw std::invalid_argument("covins_b200::NonCentralRelativePoseCovariance: one RANSAC result per problem");
+  const detail::FlatRelProblems F = detail::flatten_rel_problems(problems, "NonCentralRelativePoseCovariance");
+  const size_t m = n_prob > 0 ? n_prob : 1;
+  std::vector<double> ref(12 * m), cov(36 * m);
+  std::vector<int32_t> nv(m);
+  for (int i = 0; i < n_prob; i++) std::copy(ransac_results[i].model.begin(), ransac_results[i].model.end(), ref.begin() + 12 * i);
+  const cvb_rel_ransac_problems P = F.view();
+  cvb_rel_cov_result R{cov.data(), nv.data(), nullptr, nullptr};
+  ctx.check(cvb_noncentral_relative_pose_covariance_batch(ctx.get(), &P, ref.data(), &R), "cvb_noncentral_relative_pose_covariance_batch");
+  std::vector<RelativePoseCovariance> out(n_prob);
+  for (int i = 0; i < n_prob; i++) {
+    std::copy(cov.begin() + 36 * i, cov.begin() + 36 * (i + 1), out[i].cov.begin());
+    out[i].n_valid = nv[i];
   }
   return out;
 }

@@ -7,6 +7,10 @@
 // RelNonCentralPosSolver::computePose (cvb_ransac_central_relative_pose_batch): a central problem is a non-central one with a
 // single identity camera per side.
 //
+// The 17-point solver also serves the sampling-based 6x6 covariance of computeNonCentralRelPose
+// (cvb_noncentral_relative_pose_covariance_batch, rel_cov_solve_kernel / rel_cov_reduce_kernel at the end of the file;
+// oracle/relpose_cov_oracle.c restates it).
+//
 // One CTA per problem, both rigs staged in shared memory.  Samples are taken in waves of kWave: each warp solves one sample at
 // a time (lane k owns column k of A^T in its warp's shared-memory area, every norm and dot product is a sequential sum inside
 // one lane), then every warp scores the wave's hypotheses against all correspondences (camera-pair models in the warp's area,
@@ -739,11 +743,13 @@ bool ptr_ok(const int32_t* p, int n) {
   return true;
 }
 
-// every sample index of a problem with at least k correspondences in [0, n); the samples of smaller problems are not read
-int check_samples(cvb_ctx* ctx, const char* name, const int32_t* samples, const int32_t* prob_ptr, int n_prob, int ns, int k) {
+// every sample index of a problem with at least k correspondences in [0, n); the samples of smaller problems, and of problems
+// flagged in skip (nullable), are not read
+int check_samples(cvb_ctx* ctx, const char* name, const int32_t* samples, const int32_t* prob_ptr, int n_prob, int ns, int k,
+                  const uint8_t* skip = nullptr) {
   for (int i = 0; i < n_prob; i++) {
     const int n = prob_ptr[i + 1] - prob_ptr[i];
-    if (n < k) continue;
+    if (n < k || (skip && skip[i])) continue;
     const int32_t* s = samples + k * (size_t)i * ns;
     for (size_t j = 0; j < k * (size_t)ns; j++)
       CVB_REQUIRE(ctx, s[j] >= 0 && s[j] < n, "%s: sample index %d out of range [0, %d) in problem %d", name, s[j], n, i);
@@ -753,6 +759,47 @@ int check_samples(cvb_ctx* ctx, const char* name, const int32_t* samples, const 
 
 // staging offsets of the inputs (camera arrays unused by a central problem)
 struct RelIn { size_t ptr, f1, f2, s1, s2, c1, c2, cp1, cp2, rig1, rig2, smp; };
+
+// the argument checks of a non-central problem batch (n_prob > 0) shared by the RANSAC and the covariance calls, up to the
+// samples; with_sigma: sigma1 / sigma2 are read.  Sets *max_pairs to the largest rig1 x rig2 camera-pair count.
+int check_rel_problems(cvb_ctx* ctx, const char* name, const cvb_rel_ransac_problems* p, bool with_sigma, int* max_pairs) {
+  const int n_prob = p->n_prob;
+  CVB_REQUIRE(ctx, ptr_ok(p->prob_ptr, n_prob), "%s: prob_ptr does not start at 0 or decreases", name);
+  CVB_REQUIRE(ctx, ptr_ok(p->cam_ptr1, n_prob) && ptr_ok(p->cam_ptr2, n_prob), "%s: cam_ptr1 / cam_ptr2 does not start at 0 or decreases", name);
+  *max_pairs = 0;
+  for (int i = 0; i < n_prob; i++) {
+    const int nc1 = p->cam_ptr1[i + 1] - p->cam_ptr1[i], nc2 = p->cam_ptr2[i + 1] - p->cam_ptr2[i];
+    CVB_REQUIRE(ctx, nc1 <= kMaxCams && nc2 <= kMaxCams, "%s: problem %d has a rig of more than %d cameras", name, i, kMaxCams);
+    *max_pairs = nc1 * nc2 > *max_pairs ? nc1 * nc2 : *max_pairs;
+  }
+  const size_t N = (size_t)p->prob_ptr[n_prob], NC1 = (size_t)p->cam_ptr1[n_prob], NC2 = (size_t)p->cam_ptr2[n_prob];
+  CVB_REQUIRE(ctx, N == 0 || (p->f1 && p->f2 && (!with_sigma || (p->sigma1 && p->sigma2)) && p->cam1 && p->cam2), "%s: null correspondence arrays", name);
+  CVB_REQUIRE(ctx, (NC1 == 0 || (p->cam_off1 && p->cam_rot1)) && (NC2 == 0 || (p->cam_off2 && p->cam_rot2)), "%s: null rig arrays", name);
+  CVB_REQUIRE(ctx, p->n_samples == 0 || p->samples, "%s: null samples", name);
+  for (int i = 0; i < n_prob; i++) {
+    const int o = p->prob_ptr[i], n = p->prob_ptr[i + 1] - o;
+    const int nc1 = p->cam_ptr1[i + 1] - p->cam_ptr1[i], nc2 = p->cam_ptr2[i + 1] - p->cam_ptr2[i];
+    for (int j = o; j < o + n; j++)
+      CVB_REQUIRE(ctx, p->cam1[j] >= 0 && p->cam1[j] < nc1 && p->cam2[j] >= 0 && p->cam2[j] < nc2,
+                  "%s: correspondence %d of problem %d names camera (%d, %d) outside its rigs (%d, %d cameras)", name, j - o, i, p->cam1[j],
+                  p->cam2[j], nc1, nc2);
+  }
+  return CVB_OK;
+}
+
+// both rigs of a non-central batch into St, each camera as its offset (3) directly followed by its rotation (9, row-major)
+void stage_rigs(Stager& St, const cvb_rel_ransac_problems* p, RelIn& in) {
+  const size_t NC1 = (size_t)p->cam_ptr1[p->n_prob], NC2 = (size_t)p->cam_ptr2[p->n_prob];
+  in.rig1 = St.reserve(NC1 * 96); in.rig2 = St.reserve(NC2 * 96);
+  for (size_t j = 0; j < NC1; j++) {
+    memcpy(St.h.data() + in.rig1 + 96 * j, p->cam_off1 + 3 * j, 24);
+    memcpy(St.h.data() + in.rig1 + 96 * j + 24, p->cam_rot1 + 9 * j, 72);
+  }
+  for (size_t j = 0; j < NC2; j++) {
+    memcpy(St.h.data() + in.rig2 + 96 * j, p->cam_off2 + 3 * j, 24);
+    memcpy(St.h.data() + in.rig2 + 96 * j + 24, p->cam_rot2 + 9 * j, 72);
+  }
+}
 
 // the tail shared by both calls: outputs staged after the inputs in St, one upload, one launch of ransac_rel_kernel<Sv>, one
 // download
@@ -804,6 +851,117 @@ int run_rel_ransac(cvb_ctx* ctx, Stager& St, const RelIn& in, int n_prob, int ns
   return CVB_OK;
 }
 
+// ---- the sampling-based covariance of a 17-point model (cvb_noncentral_relative_pose_covariance_batch) ----
+// Solve: a problem's samples are spread over ceil(n_samples / kCovPerCta) CTAs (one linear grid over all problems), each
+// with both rigs and the reference model in shared memory and one warp per sample through rel17; lane 0 writes the sample's
+// deviation and valid flag to a workspace.  Reduce: one CTA per problem, thread (r, c) sums delta_r delta_c over the valid
+// samples in sample order.
+constexpr int kCovPerCta = 4;   // samples (and warps) per solve CTA, chosen by measurement (DESIGN §9, K11e)
+constexpr int kCovReduceThreads = 64, kCovChunk = 256;
+
+struct CovDev {
+  const int* prob_ptr; const double* f1; const double* f2; const int* cam1; const int* cam2;
+  const int* cam_ptr1; const int* cam_ptr2; const double* rig1; const double* rig2;   // rigs: [cam][12] offset then Rc
+  const int* samples; const double* ref_model;
+  int n_samples, ctas_per_prob;
+  double* delta; uint8_t* valid;   // [n_prob][n_samples][6], [n_prob][n_samples]
+  double* cov; int* n_valid;       // [n_prob][36], [n_prob]
+};
+
+// q = (x, y, z, w) of a rotation matrix m (row-major) in Eigen's branch for the largest diagonal entry i
+template <int i>
+__device__ __forceinline__ void quat_diag_branch(const double* m, double* q) {
+  constexpr int j = (i + 1) % 3, k = (j + 1) % 3;
+  double t = __dsqrt_rn(add(sub(sub(m[4 * i], m[4 * j]), m[4 * k]), 1.0));
+  q[i] = mul(0.5, t);
+  t = __ddiv_rn(0.5, t);
+  q[3] = mul(sub(m[3 * k + j], m[3 * j + k]), t);
+  q[j] = mul(add(m[3 * j + i], m[3 * i + j]), t);
+  q[k] = mul(add(m[3 * k + i], m[3 * i + k]), t);
+}
+
+// delta = [2 vec(q); t_s - t_ref], q the quaternion of R_ref^T R_s (Eigen's matrix-to-quaternion branches), w >= 0
+__device__ void rel_deviation(const double* ref, const double* M, double* d) {
+  double m[9], q[4];
+  for (int r = 0; r < 3; r++)
+    for (int c = 0; c < 3; c++) m[3 * r + c] = add(add(mul(ref[r], M[c]), mul(ref[4 + r], M[4 + c])), mul(ref[8 + r], M[8 + c]));
+  const double tr = add(add(m[0], m[4]), m[8]);
+  if (tr > 0.0) {
+    double t = __dsqrt_rn(add(tr, 1.0));
+    q[3] = mul(0.5, t);
+    t = __ddiv_rn(0.5, t);
+    q[0] = mul(sub(m[7], m[5]), t); q[1] = mul(sub(m[2], m[6]), t); q[2] = mul(sub(m[3], m[1]), t);
+  } else {
+    const int i = m[8] > (m[4] > m[0] ? m[4] : m[0]) ? 2 : (m[4] > m[0] ? 1 : 0);
+    if (i == 0) quat_diag_branch<0>(m, q);
+    else if (i == 1) quat_diag_branch<1>(m, q);
+    else quat_diag_branch<2>(m, q);
+  }
+  const double s = q[3] < 0.0 ? -2.0 : 2.0;
+  for (int r = 0; r < 3; r++) {
+    d[r] = mul(s, q[r]);
+    d[3 + r] = sub(M[4 * r + 3], ref[4 * r + 3]);
+  }
+}
+
+__global__ void __launch_bounds__(kThreads) rel_cov_solve_kernel(CovDev D) {
+  extern __shared__ double dyn[];
+  const int pi = blockIdx.x / D.ctas_per_prob, chunk = blockIdx.x % D.ctas_per_prob;
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, nw = blockDim.x >> 5;
+  const int off = D.prob_ptr[pi], n = D.prob_ptr[pi + 1] - off;
+  const int nc1 = D.cam_ptr1[pi + 1] - D.cam_ptr1[pi], nc2 = D.cam_ptr2[pi + 1] - D.cam_ptr2[pi];
+  __shared__ double rig1[kMaxCams * 12], rig2[kMaxCams * 12], ref[12], w_model[kWarps][12];
+  __shared__ int rigs_finite, skip;
+  for (int i = tid; i < 12 * nc1; i += blockDim.x) rig1[i] = D.rig1[12 * (size_t)D.cam_ptr1[pi] + i];
+  for (int i = tid; i < 12 * nc2; i += blockDim.x) rig2[i] = D.rig2[12 * (size_t)D.cam_ptr2[pi] + i];
+  if (tid < 12) ref[tid] = D.ref_model[12 * (size_t)pi + tid];
+  __syncthreads();
+  if (tid == 0) {
+    int fin = 1, zero = 1;
+    for (int i = 0; i < 12 * nc1; i++) fin &= isfinite(rig1[i]);
+    for (int i = 0; i < 12 * nc2; i++) fin &= isfinite(rig2[i]);
+    for (int i = 0; i < 12; i++) zero &= ref[i] == 0.0;
+    rigs_finite = fin; skip = zero;
+  }
+  __syncthreads();
+  const ProbView P{n, D.f1 + 3 * (size_t)off, D.f2 + 3 * (size_t)off, D.cam1 + off, D.cam2 + off, rig1, rig2, rigs_finite != 0};
+  double* W = dyn + (size_t)warp * kSolveArea;
+  const int s_end = min((chunk + 1) * kCovPerCta, D.n_samples);
+  for (int s = chunk * kCovPerCta + warp; s < s_end; s += nw) {
+    const size_t g = (size_t)pi * D.n_samples + s;
+    const bool v = !skip && Solver17::solve(D.samples + kSample * g, P, W, w_model[warp], lane);   // a skipped problem's samples are not read
+    __syncwarp();
+    if (lane == 0) {
+      double d[6] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0};
+      if (v) rel_deviation(ref, w_model[warp], d);
+      for (int i = 0; i < 6; i++) D.delta[6 * g + i] = d[i];
+      D.valid[g] = (uint8_t)v;
+    }
+    __syncwarp();
+  }
+}
+
+__global__ void __launch_bounds__(kCovReduceThreads) rel_cov_reduce_kernel(CovDev D) {
+  const int pi = blockIdx.x, tid = threadIdx.x, r = tid / 6, c = tid % 6;
+  __shared__ double sd[kCovChunk * 6];
+  __shared__ uint8_t sv[kCovChunk];
+  double acc = 0.0;
+  int nv = 0;
+  for (int base = 0; base < D.n_samples; base += kCovChunk) {
+    const int m = min(kCovChunk, D.n_samples - base);
+    const size_t g0 = (size_t)pi * D.n_samples + base;
+    for (int i = tid; i < 6 * m; i += kCovReduceThreads) sd[i] = D.delta[6 * g0 + i];
+    for (int i = tid; i < m; i += kCovReduceThreads) sv[i] = D.valid[g0 + i];
+    __syncthreads();
+    if (tid < 36)
+      for (int i = 0; i < m; i++)
+        if (sv[i]) { acc = add(acc, mul(sd[6 * i + r], sd[6 * i + c])); nv++; }
+    __syncthreads();
+  }
+  if (tid < 36) D.cov[36 * (size_t)pi + tid] = nv > 0 ? __ddiv_rn(acc, (double)nv) : 0.0;
+  if (tid == 0) D.n_valid[pi] = nv;
+}
+
 }  // namespace
 
 extern "C" int cvb_ransac_noncentral_relative_pose_batch(cvb_ctx* ctx, const cvb_rel_ransac_problems* p, double threshold, int max_iterations,
@@ -818,43 +976,17 @@ extern "C" int cvb_ransac_noncentral_relative_pose_batch(cvb_ctx* ctx, const cvb
               "ransac_noncentral_relative_pose: null required pointer");
   CVB_REQUIRE(ctx, (r->sample_model != nullptr) == (r->sample_valid != nullptr) && (r->sample_model != nullptr) == (r->sample_count != nullptr),
               "ransac_noncentral_relative_pose: sample_model / sample_valid / sample_count are requested together");
-  CVB_REQUIRE(ctx, ptr_ok(p->prob_ptr, n_prob), "ransac_noncentral_relative_pose: prob_ptr does not start at 0 or decreases");
-  CVB_REQUIRE(ctx, ptr_ok(p->cam_ptr1, n_prob) && ptr_ok(p->cam_ptr2, n_prob), "ransac_noncentral_relative_pose: cam_ptr1 / cam_ptr2 does not start at 0 or decreases");
   int max_pairs = 0;
-  for (int i = 0; i < n_prob; i++) {
-    const int nc1 = p->cam_ptr1[i + 1] - p->cam_ptr1[i], nc2 = p->cam_ptr2[i + 1] - p->cam_ptr2[i];
-    CVB_REQUIRE(ctx, nc1 <= kMaxCams && nc2 <= kMaxCams, "ransac_noncentral_relative_pose: problem %d has a rig of more than %d cameras", i, kMaxCams);
-    max_pairs = nc1 * nc2 > max_pairs ? nc1 * nc2 : max_pairs;
-  }
-  const size_t N = (size_t)p->prob_ptr[n_prob], NC1 = (size_t)p->cam_ptr1[n_prob], NC2 = (size_t)p->cam_ptr2[n_prob];
-  CVB_REQUIRE(ctx, N == 0 || (p->f1 && p->f2 && p->sigma1 && p->sigma2 && p->cam1 && p->cam2), "ransac_noncentral_relative_pose: null correspondence arrays");
-  CVB_REQUIRE(ctx, (NC1 == 0 || (p->cam_off1 && p->cam_rot1)) && (NC2 == 0 || (p->cam_off2 && p->cam_rot2)), "ransac_noncentral_relative_pose: null rig arrays");
-  CVB_REQUIRE(ctx, ns == 0 || p->samples, "ransac_noncentral_relative_pose: null samples");
-  for (int i = 0; i < n_prob; i++) {
-    const int o = p->prob_ptr[i], n = p->prob_ptr[i + 1] - o;
-    const int nc1 = p->cam_ptr1[i + 1] - p->cam_ptr1[i], nc2 = p->cam_ptr2[i + 1] - p->cam_ptr2[i];
-    for (int j = o; j < o + n; j++)
-      CVB_REQUIRE(ctx, p->cam1[j] >= 0 && p->cam1[j] < nc1 && p->cam2[j] >= 0 && p->cam2[j] < nc2,
-                  "ransac_noncentral_relative_pose: correspondence %d of problem %d names camera (%d, %d) outside its rigs (%d, %d cameras)", j - o, i,
-                  p->cam1[j], p->cam2[j], nc1, nc2);
-  }
+  if (const int rc = check_rel_problems(ctx, "ransac_noncentral_relative_pose", p, true, &max_pairs)) return rc;
   if (const int rc = check_samples(ctx, "ransac_noncentral_relative_pose", p->samples, p->prob_ptr, n_prob, ns, kSample)) return rc;
-  const size_t S_all = (size_t)n_prob * ns;
+  const size_t N = (size_t)p->prob_ptr[n_prob], S_all = (size_t)n_prob * ns;
   Stager St;
   RelIn in{};
   in.ptr = St.put(p->prob_ptr, ((size_t)n_prob + 1) * 4); in.f1 = St.put(p->f1, N * 24); in.f2 = St.put(p->f2, N * 24);
   in.s1 = St.put(p->sigma1, N * 8); in.s2 = St.put(p->sigma2, N * 8); in.c1 = St.put(p->cam1, N * 4); in.c2 = St.put(p->cam2, N * 4);
   in.cp1 = St.put(p->cam_ptr1, ((size_t)n_prob + 1) * 4); in.cp2 = St.put(p->cam_ptr2, ((size_t)n_prob + 1) * 4);
   in.smp = St.put(p->samples, S_all * kSample * 4);
-  in.rig1 = St.reserve(NC1 * 96); in.rig2 = St.reserve(NC2 * 96);
-  for (size_t j = 0; j < NC1; j++) {   // camera: offset (3) directly followed by the rotation (9, row-major)
-    memcpy(St.h.data() + in.rig1 + 96 * j, p->cam_off1 + 3 * j, 24);
-    memcpy(St.h.data() + in.rig1 + 96 * j + 24, p->cam_rot1 + 9 * j, 72);
-  }
-  for (size_t j = 0; j < NC2; j++) {
-    memcpy(St.h.data() + in.rig2 + 96 * j, p->cam_off2 + 3 * j, 24);
-    memcpy(St.h.data() + in.rig2 + 96 * j + 24, p->cam_rot2 + 9 * j, 72);
-  }
+  stage_rigs(St, p, in);
   return run_rel_ransac<Solver17>(ctx, St, in, n_prob, ns, N, max_pairs, threshold, max_iterations, probability, r);
 }
 
@@ -880,4 +1012,78 @@ extern "C" int cvb_ransac_central_relative_pose_batch(cvb_ctx* ctx, const cvb_ce
   in.ptr = St.put(p->prob_ptr, ((size_t)n_prob + 1) * 4); in.f1 = St.put(p->f1, N * 24); in.f2 = St.put(p->f2, N * 24);
   in.s1 = St.put(p->sigma1, N * 8); in.s2 = St.put(p->sigma2, N * 8); in.smp = St.put(p->samples, (size_t)n_prob * ns * kSample5 * 4);
   return run_rel_ransac<Solver5>(ctx, St, in, n_prob, ns, N, 1, threshold, max_iterations, probability, r);
+}
+
+extern "C" int cvb_noncentral_relative_pose_covariance_batch(cvb_ctx* ctx, const cvb_rel_ransac_problems* p, const double* ref_model,
+                                                             cvb_rel_cov_result* r) {
+  if (!ctx) return CVB_ERR_INVALID;
+  CVB_GUARD(ctx);
+  CVB_REQUIRE(ctx, p && r && p->n_prob >= 0 && p->n_samples >= 0, "noncentral_relative_pose_covariance: bad arguments");
+  const int n_prob = p->n_prob, ns = p->n_samples;
+  if (n_prob == 0) return CVB_OK;
+  CVB_REQUIRE(ctx, p->prob_ptr && p->cam_ptr1 && p->cam_ptr2 && ref_model && r->cov && r->n_valid,
+              "noncentral_relative_pose_covariance: null required pointer");
+  CVB_REQUIRE(ctx, (r->sample_delta != nullptr) == (r->sample_valid != nullptr),
+              "noncentral_relative_pose_covariance: sample_delta / sample_valid are requested together");
+  int max_pairs = 0;   // unused: the covariance does not score
+  if (const int rc = check_rel_problems(ctx, "noncentral_relative_pose_covariance", p, false, &max_pairs)) return rc;
+  // the reference models: all zeros (skipped), or finite with a rotation R
+  std::vector<uint8_t> skip(n_prob);
+  for (int i = 0; i < n_prob; i++) {
+    const double* M = ref_model + 12 * (size_t)i;
+    bool zero = true, finite = true;
+    for (int k = 0; k < 12; k++) { zero &= M[k] == 0.0; finite &= isfinite(M[k]) != 0; }
+    skip[i] = zero;
+    if (zero) continue;
+    CVB_REQUIRE(ctx, finite, "noncentral_relative_pose_covariance: reference model of problem %d is not finite", i);
+    double dev = 0.0;
+    for (int a = 0; a < 3; a++)
+      for (int b = 0; b < 3; b++) {
+        const double g = M[a] * M[b] + M[4 + a] * M[4 + b] + M[8 + a] * M[8 + b] - (a == b ? 1.0 : 0.0);
+        dev = fabs(g) > dev ? fabs(g) : dev;
+      }
+    CVB_REQUIRE(ctx, dev <= 1e-6, "noncentral_relative_pose_covariance: R of the reference model of problem %d is not a rotation (max |R^T R - I| = %g)", i,
+                dev);
+  }
+  if (const int rc = check_samples(ctx, "noncentral_relative_pose_covariance", p->samples, p->prob_ptr, n_prob, ns, kSample, skip.data())) return rc;
+  const size_t N = (size_t)p->prob_ptr[n_prob], S_all = (size_t)n_prob * ns;
+  const bool all = r->sample_delta != nullptr;
+  Stager St;
+  RelIn in{};
+  in.ptr = St.put(p->prob_ptr, ((size_t)n_prob + 1) * 4); in.f1 = St.put(p->f1, N * 24); in.f2 = St.put(p->f2, N * 24);
+  in.c1 = St.put(p->cam1, N * 4); in.c2 = St.put(p->cam2, N * 4);
+  in.cp1 = St.put(p->cam_ptr1, ((size_t)n_prob + 1) * 4); in.cp2 = St.put(p->cam_ptr2, ((size_t)n_prob + 1) * 4);
+  in.smp = St.put(p->samples, S_all * kSample * 4);
+  stage_rigs(St, p, in);
+  const size_t o_ref = St.put(ref_model, (size_t)n_prob * 96);
+  const size_t in_bytes = St.h.size();
+  const size_t o_cov = St.reserve((size_t)n_prob * 288), o_nv = St.reserve((size_t)n_prob * 4), o_d = St.reserve(S_all * 48), o_v = St.reserve(S_all);
+  const size_t total = St.h.size();
+  unsigned char* d = (unsigned char*)cvb_ws(ctx, WS_GS6, total);
+  unsigned char* hpin = (unsigned char*)cvb_pinned(ctx, total);
+  if (!d || !hpin) return CVB_ERR_CUDA;
+  memcpy(hpin, St.h.data(), in_bytes);
+  CovDev D{};
+  D.prob_ptr = (const int*)(d + in.ptr); D.f1 = (const double*)(d + in.f1); D.f2 = (const double*)(d + in.f2);
+  D.cam1 = (const int*)(d + in.c1); D.cam2 = (const int*)(d + in.c2); D.cam_ptr1 = (const int*)(d + in.cp1); D.cam_ptr2 = (const int*)(d + in.cp2);
+  D.rig1 = (const double*)(d + in.rig1); D.rig2 = (const double*)(d + in.rig2); D.samples = (const int*)(d + in.smp);
+  D.ref_model = (const double*)(d + o_ref);
+  D.n_samples = ns; D.ctas_per_prob = (ns + kCovPerCta - 1) / kCovPerCta;
+  D.delta = (double*)(d + o_d); D.valid = d + o_v; D.cov = (double*)(d + o_cov); D.n_valid = (int*)(d + o_nv);
+  cudaStream_t st = ctx->stream;
+  CVB_CUDA(ctx, cudaMemcpyAsync(d, hpin, in_bytes, cudaMemcpyHostToDevice, st));
+  if (ns > 0) {
+    const long long grid = (long long)n_prob * D.ctas_per_prob;
+    CVB_REQUIRE(ctx, grid <= INT32_MAX, "noncentral_relative_pose_covariance: %lld solve CTAs exceed the grid limit", grid);
+    constexpr int kSolveWarps = kCovPerCta < kWarps ? kCovPerCta : kWarps;
+    rel_cov_solve_kernel<<<(unsigned)grid, 32 * kSolveWarps, (size_t)kSolveWarps * kSolveArea * sizeof(double), st>>>(D);
+    CVB_CHECK_LAUNCH(ctx);
+  }
+  rel_cov_reduce_kernel<<<n_prob, kCovReduceThreads, 0, st>>>(D);
+  CVB_CHECK_LAUNCH(ctx);
+  CVB_CUDA(ctx, cudaMemcpyAsync(hpin + o_cov, d + o_cov, (all ? total : o_d) - o_cov, cudaMemcpyDeviceToHost, st));
+  CVB_CUDA(ctx, cudaStreamSynchronize(st));
+  memcpy(r->cov, hpin + o_cov, (size_t)n_prob * 288); memcpy(r->n_valid, hpin + o_nv, (size_t)n_prob * 4);
+  if (all) { memcpy(r->sample_delta, hpin + o_d, S_all * 48); memcpy(r->sample_valid, hpin + o_v, S_all); }
+  return CVB_OK;
 }

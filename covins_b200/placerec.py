@@ -9,6 +9,8 @@ the C-ABI:
   ransac_noncentral_relative_pose(...) ↔ the 17-point RANSAC of RelNonCentralPosSolver::computeNonCentralRelPose from
                                   caller-supplied samples
   ransac_central_relative_pose(...) ↔ the 5-point RANSAC of RelNonCentralPosSolver::computePose from caller-supplied samples
+  relative_pose_covariance(...) ↔ the sampling-based 6x6 covariance of RelNonCentralPosSolver::computeNonCentralRelPose (17-point
+                                  re-solves from caller-supplied samples)
 
 `KfView` flattens what the reference reads of a Keyframe (the C++ shim does the same from the containers)."""
 from __future__ import annotations
@@ -262,4 +264,36 @@ def ransac_central_relative_pose(ctx: Context, prob_ptr, f1, f2, sigma1, sigma2,
     R = CRelRansacResult(*[r[k].ctypes.data if k in r else None for k, _ in CRelRansacResult._fields_])
     ctx.check(lib().cvb_ransac_central_relative_pose_batch(ctx.handle, C.byref(P), float(threshold), int(max_iterations), float(probability),
                                                            C.byref(R)))
+    return r
+
+
+class CRelCovResult(C.Structure):
+    _fields_ = [(k, c_vp) for k in ("cov", "n_valid", "sample_delta", "sample_valid")]
+
+
+def relative_pose_covariance(ctx: Context, prob_ptr, f1, f2, cam1, cam2, cam_ptr1, cam_off1, cam_rot1, cam_ptr2, cam_off2, cam_rot2, samples,
+                             ref_model, per_sample=False, sigma1=None, sigma2=None):
+    """The sampling-based 6x6 covariance of RelNonCentralPosSolver::computeNonCentralRelPose for a batch of problems
+    (cvb_noncentral_relative_pose_covariance_batch): a 17-point re-solve per sample, its deviation
+    delta = [2 vec(q); t_s - t_ref] (q the quaternion of R_ref^T R_s, w >= 0) from the reference model, and
+    cov = sum delta delta^T / n_valid over the valid samples, on the GPU.  Arguments as ransac_noncentral_relative_pose (sigma1 /
+    sigma2 are accepted and not read); samples [n_prob, n_samples, 17] problem-local indices, normally drawn from the inlier
+    mask of the RANSAC; ref_model [n_prob,3,4] (X1 = R X2 + t), normally its best_model (all zeros: the problem is skipped).
+    → dict(cov [n_prob,6,6] (rotation then translation), n_valid [n_prob]) and, with per_sample, sample_delta
+    [n_prob,n_samples,6], sample_valid [n_prob,n_samples]."""
+    ptr = np.ascontiguousarray(prob_ptr, np.int32); n_prob = len(ptr) - 1
+    a = np.ascontiguousarray(f1, np.float64).reshape(-1, 3); b = np.ascontiguousarray(f2, np.float64).reshape(-1, 3)
+    c1 = np.ascontiguousarray(cam1, np.int32).reshape(-1); c2 = np.ascontiguousarray(cam2, np.int32).reshape(-1)
+    cp1 = np.ascontiguousarray(cam_ptr1, np.int32); cp2 = np.ascontiguousarray(cam_ptr2, np.int32)
+    co1 = np.ascontiguousarray(cam_off1, np.float64).reshape(-1, 3); cr1 = np.ascontiguousarray(cam_rot1, np.float64).reshape(-1, 9)
+    co2 = np.ascontiguousarray(cam_off2, np.float64).reshape(-1, 3); cr2 = np.ascontiguousarray(cam_rot2, np.float64).reshape(-1, 9)
+    smp = np.ascontiguousarray(samples, np.int32).reshape(n_prob, -1, 17); ns = smp.shape[1]
+    ref = np.ascontiguousarray(ref_model, np.float64).reshape(n_prob, 12)
+    r = dict(cov=np.zeros((n_prob, 6, 6)), n_valid=np.zeros(n_prob, np.int32))
+    if per_sample:
+        r.update(sample_delta=np.zeros((n_prob, ns, 6)), sample_valid=np.zeros((n_prob, ns), np.uint8))
+    P = CRelRansacProblems(n_prob, ptr.ctypes.data, a.ctypes.data, b.ctypes.data, None, None,
+                           *[x.ctypes.data for x in (c1, c2, cp1, co1, cr1, cp2, co2, cr2, smp)], ns)
+    R = CRelCovResult(*[r[k].ctypes.data if k in r else None for k, _ in CRelCovResult._fields_])
+    ctx.check(lib().cvb_noncentral_relative_pose_covariance_batch(ctx.handle, C.byref(P), ref.ctypes.data, C.byref(R)))
     return r

@@ -483,6 +483,47 @@ CVB_API int cvb_ransac_central_relative_pose_batch(cvb_ctx* ctx, const cvb_centr
                                                    int max_iterations, double probability, cvb_rel_ransac_result* r);
 
 /*
+ * The sampling-based 6x6 covariance of the non-central relative pose (RelNonCentralPosSolver::computeNonCentralRelPose,
+ * RelNonCentralPosSolver.cpp:199,236,276-279: up to 300 17-point re-solves on subsets of the selected model's inliers, the
+ * matrix that becomes LoopConstraint::cov_mat) for a batch of problems (candidates), from the caller's samples.  Sampling
+ * stays with the caller: the samples are normally drawn from the inlier mask of cvb_ransac_noncentral_relative_pose_batch,
+ * but their indices need not be inliers.
+ *   Inputs per problem: the correspondences and rigs of cvb_rel_ransac_problems (sigma1 / sigma2 are not read and may be
+ *   null), samples [n_prob][n_samples][17], and a reference model ref_model [n_prob][12] = [R_ref|t_ref] (X1 = R X2 + t,
+ *   normally the problem's best_model).
+ *   Per sample: the 17-point hypothesis [R_s|t_s] of cvb_ransac_noncentral_relative_pose_batch, with exactly its rules for
+ *   an invalid sample (an invalid sample is skipped and not counted).  Its deviation from the reference is
+ *     delta = [dtheta; dt], dtheta = 2 vec(q), q = (x, y, z, w) the quaternion of R_ref^T R_s by Eigen's matrix-to-quaternion
+ *     branches (trace > 0, else the largest diagonal entry), negated if w < 0; dt = t_s - t_ref.
+ *   Per problem: cov = (1 / n_valid) sum delta delta^T over the valid samples, summed in sample order; cov = 0 when
+ *   n_valid = 0.  A problem whose reference model is all zeros (a RANSAC without a model) is skipped: n_valid = 0, and its
+ *   samples are not read.
+ *   Only + - * / and sqrt as non-fused operations and fixed summation orders: the results are bit-identical to a
+ *   -ffp-contract=off C restatement, and cov is exactly symmetric.
+ *   ASSUMPTIONS (robopt and opengv are not in the tree):
+ *     - rotation first, right-side deviation, 2 vec(q) rather than Log: cov is in the coordinates of the residual it whitens,
+ *       the pose-graph between factor e = [2 vec(q_m^-1 q_hat); t_hat - t_m].  (robopt's quaternion::Minus may be a left-side
+ *       Log instead.)
+ *     - the second moment about the reference, divided by n_valid: the mean is not subtracted and the divisor is not n - 1.
+ *     - minimal 17-point re-solves, not a non-minimal solver.
+ * Outputs: cov [n_prob][36] row-major, n_valid [n_prob]; on request (both or neither) every sample's delta
+ * [n_prob][n_samples][6] (0 for an invalid sample) and valid flag.
+ * Errors: CVB_ERR_INVALID before any launch for the errors of cvb_ransac_noncentral_relative_pose_batch (negative sizes, null
+ * required pointers, a decreasing prob_ptr / cam_ptr1 / cam_ptr2, an out-of-range sample index of a problem that is read, a
+ * camera index outside its rig, a rig of more than CVB_REL_MAX_CAMS cameras, per-sample outputs not requested together), and
+ * for a non-zero reference model that is not finite or whose R is not a rotation (max |R^T R - I| > 1e-6); n_prob = 0
+ * succeeds.
+ */
+typedef struct cvb_rel_cov_result {
+  double* cov;               /* [n_prob][36] row-major, dtheta then dt */
+  int32_t* n_valid;          /* [n_prob] */
+  double* sample_delta;      /* [n_prob][n_samples][6] nullable */
+  uint8_t* sample_valid;     /* [n_prob][n_samples]    nullable together */
+} cvb_rel_cov_result;
+CVB_API int cvb_noncentral_relative_pose_covariance_batch(cvb_ctx* ctx, const cvb_rel_ransac_problems* p, const double* ref_model,
+                                                          cvb_rel_cov_result* r);
+
+/*
  * Optimization::OptimizeRelativePose(kf1, kf2, matches1, T12, th2) (optimization_be.cpp:620-831): the 6-dof refinement of
  * the relative pose T12 from the matched landmark pairs, both ceres::Solve calls (5 + 5 iterations, DOGLEG, CauchyLoss(1))
  * and the outlier purge between them, in one call.  The caller (shim) flattens, per residual pair r (the reference's

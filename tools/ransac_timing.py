@@ -15,7 +15,12 @@ With --central, the central relative-pose (5-point) RANSAC, n_prob 1, 6 and 60 (
 1000 correspondences, 5 % and 30 % outliers:
   (a) cvb_ransac_central_relative_pose_batch (whole call, and kernel time from torch.profiler);
   (c) the oracle RANSAC on the host cores.
-  python tools/ransac_timing.py [--reps 100] [--outlier 0.5] [--relative | --central]"""
+With --covariance, the sampling-based 6x6 covariance of the non-central relative pose (17-point re-solves), n_prob 1, 8 and 32,
+1000 correspondences, 3-camera rigs per side, 300 samples per problem drawn from the inliers, reference model = the true pose:
+  (a) cvb_noncentral_relative_pose_covariance_batch (whole call, and the device time of its two kernels from torch.profiler);
+  (c) the oracle on one host thread and on all host cores (OpenMP over the samples).
+Every result of a timed call is checked bit-identical to the oracle.
+  python tools/ransac_timing.py [--reps 100] [--outlier 0.5] [--relative | --central | --covariance]"""
 import argparse
 import os
 import subprocess
@@ -37,7 +42,10 @@ def main():
     ap.add_argument("--samples", type=int, default=400)
     ap.add_argument("--relative", action="store_true", help="time the non-central relative-pose (17-point) RANSAC")
     ap.add_argument("--central", action="store_true", help="time the central relative-pose (5-point) RANSAC")
+    ap.add_argument("--covariance", action="store_true", help="time the non-central relative pose's sampling-based covariance")
     a = ap.parse_args()
+    if a.covariance:
+        return covariance(a)
     if a.relative:
         return relative(a)
     if a.central:
@@ -199,6 +207,53 @@ def central(a):
                 print(f"central | {n} corr | outliers {outlier:.0%} | n_prob {n_prob:2d}, {a.samples} samples: iterations used "
                       f"{got['iterations'].min()}-{got['iterations'].max()} | (a) call {t_a:.3f} ms, kernel {k_a:.3f} ms | "
                       f"(c) oracle RANSAC on {os.cpu_count()} host cores {t_c:.3f} ms | bit-identical to the oracle")
+    ctx.close()
+
+
+def covariance(a):
+    import torch
+    import covins_b200
+    from covins_b200 import placerec as PR
+    from oracle import relpose_cov as ocov
+    from test_relpose_covariance import _batch, _truth
+    from torch.profiler import profile, ProfilerActivity
+    assert torch.cuda.is_available(), "needs a CUDA device"
+    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"], capture_output=True, text=True)
+    print(f"GPU: {torch.cuda.get_device_name(0)} | {q.stdout.strip()} | host cores: {os.cpu_count()}")
+    ctx = covins_b200.Context(0)
+    ns = 300
+    for n_prob in (1, 8, 32):
+        b, probs = _batch(400 + n_prob, [(a.n, 3, 3, False)] * n_prob, ns, noise=1e-3, outlier_frac=0.3)
+        ref = _truth(probs)
+        want = ocov.noncentral_relative_pose_covariance(**b, ref_model=ref)
+
+        def call():
+            got = PR.relative_pose_covariance(ctx, **b, ref_model=ref)
+            for k in want:
+                assert np.array_equal(got[k].view(np.uint8), want[k].view(np.uint8)), k
+        for _ in range(3):
+            call()
+        reps = max(3, a.reps)
+        t0 = time.perf_counter()
+        for _ in range(reps):
+            call()
+        t_a = (time.perf_counter() - t0) / reps * 1e3
+        with profile(activities=[ProfilerActivity.CUDA]) as pr:
+            for _ in range(10):
+                call()
+        ev = [e for e in pr.events() if "rel_cov_" in e.name]
+        k_solve = np.sum([e.device_time for e in ev if "solve" in e.name]) / 10 / 1e3
+        k_red = np.sum([e.device_time for e in ev if "reduce" in e.name]) / 10 / 1e3
+        t_c = {}
+        for threads in (1, 0):
+            reps_c = 3
+            t0 = time.perf_counter()
+            for _ in range(reps_c):
+                ocov.noncentral_relative_pose_covariance(**b, ref_model=ref, threads=threads)
+            t_c[threads] = (time.perf_counter() - t0) / reps_c * 1e3
+        print(f"covariance | n_prob {n_prob:2d} x {a.n} corr, {ns} samples, valid {want['n_valid'].min()}-{want['n_valid'].max()} | "
+              f"(a) call {t_a:.3f} ms, kernels {k_solve + k_red:.3f} ms (solve {k_solve:.3f}, reduce {k_red:.3f}) | (c) oracle on 1 host "
+              f"thread {t_c[1]:.2f} ms, on {os.cpu_count()} host cores {t_c[0]:.2f} ms | bit-identical to the oracle")
     ctx.close()
 
 
