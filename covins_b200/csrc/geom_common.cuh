@@ -1,8 +1,10 @@
 // geom_common.cuh — helpers shared by the geometric-verification translation units (geom_kernels.cu, ransac_abs.cu,
-// ransac_rel.cu): the host staging block and the device arithmetic, including the per-correspondence absolute-pose score
-// (score_abs_kernel, ransac_abs_kernel), the relative-pose score (score_rel_kernel, ransac_rel_kernel) and the 3x3 inverse of
-// both RANSAC solvers.  Every device operation is an explicit round-to-nearest non-fused intrinsic, so results are
-// reproducible bit for bit against a plain IEEE evaluation compiled with -ffp-contract=off.
+// ransac_rel.cu): the host staging block and the device arithmetic, including the cross product, the largest-cross-product
+// null vector of a rank-2 3x3 (P3P's eigenvectors, the 5-point solver's roots and baseline), the per-correspondence
+// absolute-pose score (score_abs_kernel, ransac_abs_kernel), the relative-pose score (score_rel_kernel, ransac_rel_kernel) and
+// the 3x3 inverse of the RANSAC solvers.  Every device operation is an explicit round-to-nearest non-fused intrinsic, so
+// results are reproducible bit for bit against a plain IEEE evaluation compiled with -ffp-contract=off.  The RANSAC around the
+// solvers is in ransac_common.cuh.
 #pragma once
 #include <cuda_runtime.h>
 #include <string.h>
@@ -28,6 +30,25 @@ __device__ __forceinline__ double add(double a, double b) { return __dadd_rn(a, 
 __device__ __forceinline__ double sub(double a, double b) { return __dsub_rn(a, b); }
 __device__ __forceinline__ double dot3(double a0, double a1, double a2, const double* p) {
   return add(add(mul(a0, p[0]), mul(a1, p[1])), mul(a2, p[2]));
+}
+__device__ __forceinline__ void cross3(const double* a, const double* b, double* o) {
+  o[0] = sub(mul(a[1], b[2]), mul(a[2], b[1]));
+  o[1] = sub(mul(a[2], b[0]), mul(a[0], b[2]));
+  o[2] = sub(mul(a[0], b[1]), mul(a[1], b[0]));
+}
+__device__ __forceinline__ bool finite3(const double* v) { return isfinite(v[0]) && isfinite(v[1]) && isfinite(v[2]); }
+// the largest of the three cross products r0 x r1, r0 x r2, r1 x r2 (the first on ties) and its squared norm
+__device__ __forceinline__ double cross_max(const double* r0, const double* r1, const double* r2, double* v) {
+  double c[3][3];
+  cross3(r0, r1, c[0]); cross3(r0, r2, c[1]); cross3(r1, r2, c[2]);
+  double best = dot3(c[0][0], c[0][1], c[0][2], c[0]);
+  v[0] = c[0][0]; v[1] = c[0][1]; v[2] = c[0][2];
+#pragma unroll
+  for (int j = 1; j < 3; j++) {
+    const double nj = dot3(c[j][0], c[j][1], c[j][2], c[j]);
+    if (nj > best) { best = nj; v[0] = c[j][0]; v[1] = c[j][1]; v[2] = c[j][2]; }
+  }
+  return best;
 }
 
 // inverseSolution = [R^T | -R^T t] of a 3x4 [R|t] body-in-world model (row-major)

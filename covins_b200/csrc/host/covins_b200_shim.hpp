@@ -981,6 +981,28 @@ struct AbsolutePoseRansacResult {
   int n_inliers = 0, iterations = 0, samples_used = 0;
   std::vector<uint8_t> inliers;     // n flags of the selected model
 };
+namespace detail {
+// one RANSAC call fn on the flattened problems P (ptr: their correspondence ranges) → the per-problem results (Out:
+// AbsolutePoseRansacResult or NonCentralRelativePoseRansacResult)
+template <class Out, class Problems, class Result>
+std::vector<Out> ransac(Context& ctx, int (*fn)(cvb_ctx*, const Problems*, double, int, double, Result*), const char* what, const Problems& P,
+                        const std::vector<int32_t>& ptr, double threshold, int max_iterations, double probability) {
+  const int n_prob = (int)ptr.size() - 1;
+  const size_t m = n_prob > 0 ? n_prob : 1;
+  std::vector<int32_t> best(m), cnt(m), iters(m), used(m);
+  std::vector<double> models(12 * m);
+  std::vector<uint8_t> mask(ptr[n_prob] > 0 ? ptr[n_prob] : 1);
+  Result R{best.data(), models.data(), cnt.data(), iters.data(), used.data(), mask.data(), nullptr, nullptr, nullptr};
+  ctx.check(fn(ctx.get(), &P, threshold, max_iterations, probability, &R), what);
+  std::vector<Out> out(n_prob);
+  for (int i = 0; i < n_prob; i++) {
+    out[i].best_sample = best[i]; out[i].n_inliers = cnt[i]; out[i].iterations = iters[i]; out[i].samples_used = used[i];
+    std::copy(models.begin() + 12 * i, models.begin() + 12 * (i + 1), out[i].model.begin());
+    out[i].inliers.assign(mask.begin() + ptr[i], mask.begin() + ptr[i + 1]);
+  }
+  return out;
+}
+}  // namespace detail
 inline std::vector<AbsolutePoseRansacResult> RansacAbsolutePose(Context& ctx, const std::vector<AbsolutePoseRansacProblem>& problems, double threshold,
                                                                  int max_iterations, double probability = 0.99) {
   const int n_prob = (int)problems.size();
@@ -999,20 +1021,10 @@ inline std::vector<AbsolutePoseRansacResult> RansacAbsolutePose(Context& ctx, co
     cam_rot.insert(cam_rot.end(), p.cam_rotation, p.cam_rotation + 9);
     samples.insert(samples.end(), p.samples.begin(), p.samples.end());
   }
-  const size_t m = n_prob > 0 ? n_prob : 1;
-  std::vector<int32_t> best(m), cnt(m), iters(m), used(m);
-  std::vector<double> models(12 * m);
-  std::vector<uint8_t> mask(ptr[n_prob] > 0 ? ptr[n_prob] : 1);
-  cvb_abs_ransac_problems P{n_prob, ptr.data(), pts.data(), f.data(), sigma.data(), cam_off.data(), cam_rot.data(), samples.data(), (int32_t)n_samples};
-  cvb_abs_ransac_result R{best.data(), models.data(), cnt.data(), iters.data(), used.data(), mask.data(), nullptr, nullptr, nullptr};
-  ctx.check(cvb_ransac_absolute_pose_batch(ctx.get(), &P, threshold, max_iterations, probability, &R), "cvb_ransac_absolute_pose_batch");
-  std::vector<AbsolutePoseRansacResult> out(n_prob);
-  for (int i = 0; i < n_prob; i++) {
-    out[i].best_sample = best[i]; out[i].n_inliers = cnt[i]; out[i].iterations = iters[i]; out[i].samples_used = used[i];
-    std::copy(models.begin() + 12 * i, models.begin() + 12 * (i + 1), out[i].model.begin());
-    out[i].inliers.assign(mask.begin() + ptr[i], mask.begin() + ptr[i + 1]);
-  }
-  return out;
+  const cvb_abs_ransac_problems P{n_prob, ptr.data(), pts.data(), f.data(), sigma.data(), cam_off.data(), cam_rot.data(), samples.data(),
+                                  (int32_t)n_samples};
+  return detail::ransac<AbsolutePoseRansacResult>(ctx, cvb_ransac_absolute_pose_batch, "cvb_ransac_absolute_pose_batch", P, ptr, threshold,
+                                                  max_iterations, probability);
 }
 
 // The 17-point non-central relative-pose RANSAC of RelNonCentralPosSolver::computeNonCentralRelPose (RelNonCentralPosSolver.cpp:
@@ -1074,24 +1086,9 @@ inline FlatRelProblems flatten_rel_problems(const std::vector<NonCentralRelative
 inline std::vector<NonCentralRelativePoseRansacResult> RansacNonCentralRelativePose(Context& ctx,
                                                                                    const std::vector<NonCentralRelativePoseRansacProblem>& problems,
                                                                                    double threshold, int max_iterations, double probability = 0.99) {
-  const int n_prob = (int)problems.size();
   const detail::FlatRelProblems F = detail::flatten_rel_problems(problems, "RansacNonCentralRelativePose");
-  const std::vector<int32_t>& ptr = F.ptr;
-  const size_t m = n_prob > 0 ? n_prob : 1;
-  std::vector<int32_t> best(m), cnt(m), iters(m), used(m);
-  std::vector<double> models(12 * m);
-  std::vector<uint8_t> mask(ptr[n_prob] > 0 ? ptr[n_prob] : 1);
-  const cvb_rel_ransac_problems P = F.view();
-  cvb_rel_ransac_result R{best.data(), models.data(), cnt.data(), iters.data(), used.data(), mask.data(), nullptr, nullptr, nullptr};
-  ctx.check(cvb_ransac_noncentral_relative_pose_batch(ctx.get(), &P, threshold, max_iterations, probability, &R),
-            "cvb_ransac_noncentral_relative_pose_batch");
-  std::vector<NonCentralRelativePoseRansacResult> out(n_prob);
-  for (int i = 0; i < n_prob; i++) {
-    out[i].best_sample = best[i]; out[i].n_inliers = cnt[i]; out[i].iterations = iters[i]; out[i].samples_used = used[i];
-    std::copy(models.begin() + 12 * i, models.begin() + 12 * (i + 1), out[i].model.begin());
-    out[i].inliers.assign(mask.begin() + ptr[i], mask.begin() + ptr[i + 1]);
-  }
-  return out;
+  return detail::ransac<NonCentralRelativePoseRansacResult>(ctx, cvb_ransac_noncentral_relative_pose_batch, "cvb_ransac_noncentral_relative_pose_batch",
+                                                            F.view(), F.ptr, threshold, max_iterations, probability);
 }
 
 // The sampling-based 6x6 covariance of RelNonCentralPosSolver::computeNonCentralRelPose (RelNonCentralPosSolver.cpp:199,236,
@@ -1152,20 +1149,9 @@ inline std::vector<NonCentralRelativePoseRansacResult> RansacCentralRelativePose
     s1.insert(s1.end(), p.sigma1.begin(), p.sigma1.end()); s2.insert(s2.end(), p.sigma2.begin(), p.sigma2.end());
     samples.insert(samples.end(), p.samples.begin(), p.samples.end());
   }
-  const size_t m = n_prob > 0 ? n_prob : 1;
-  std::vector<int32_t> best(m), cnt(m), iters(m), used(m);
-  std::vector<double> models(12 * m);
-  std::vector<uint8_t> mask(ptr[n_prob] > 0 ? ptr[n_prob] : 1);
-  cvb_central_rel_ransac_problems P{n_prob, ptr.data(), f1.data(), f2.data(), s1.data(), s2.data(), samples.data(), (int32_t)n_samples};
-  cvb_rel_ransac_result R{best.data(), models.data(), cnt.data(), iters.data(), used.data(), mask.data(), nullptr, nullptr, nullptr};
-  ctx.check(cvb_ransac_central_relative_pose_batch(ctx.get(), &P, threshold, max_iterations, probability, &R), "cvb_ransac_central_relative_pose_batch");
-  std::vector<NonCentralRelativePoseRansacResult> out(n_prob);
-  for (int i = 0; i < n_prob; i++) {
-    out[i].best_sample = best[i]; out[i].n_inliers = cnt[i]; out[i].iterations = iters[i]; out[i].samples_used = used[i];
-    std::copy(models.begin() + 12 * i, models.begin() + 12 * (i + 1), out[i].model.begin());
-    out[i].inliers.assign(mask.begin() + ptr[i], mask.begin() + ptr[i + 1]);
-  }
-  return out;
+  const cvb_central_rel_ransac_problems P{n_prob, ptr.data(), f1.data(), f2.data(), s1.data(), s2.data(), samples.data(), (int32_t)n_samples};
+  return detail::ransac<NonCentralRelativePoseRansacResult>(ctx, cvb_ransac_central_relative_pose_batch, "cvb_ransac_central_relative_pose_batch", P,
+                                                            ptr, threshold, max_iterations, probability);
 }
 
 // Resident-map descriptor database (cvb_db_*): the ORB descriptors of the map's keyframes live in HBM; the candidate

@@ -2,34 +2,23 @@
 // caller-supplied samples: P3P per sample, the fourth-point choice, scoring and the sequential model selection of opengv's
 // Ransac::computeModel, for a batch of problems (candidate keyframes) in one launch (SURVEY §8a V1).
 //
-// One CTA per problem.  Samples are taken in waves of kWave: the first kWave threads solve one sample each, every warp scores
-// the wave's hypotheses against all correspondences (warp-shuffle integer counts), thread 0 replays the selection over the
-// wave in sample order, and the CTA stops as soon as the adaptive bound ends the selection, so opengv's early stop saves the
-// solver and scoring work of the samples it never reads.  The CTA then writes the best model's inlier mask.
+// One CTA per problem, driven by ransac_cta (ransac_common.cuh, shared with ransac_rel.cu): the waves of kWave samples, the
+// scoring, the selection with its early stop and the inlier mask.  This file supplies the solver: in each wave the first kWave
+// threads solve one sample each; a hypothesis is scored by its inverse (abs_inverse, abs_score in geom_common.cuh).
 //
 // P3P is Lambda Twist (Persson & Nordberg, ECCV 2018): Newton iterations for one root of the cubic det(D1 + g D2) = 0, the
 // eigen-decomposition of the degenerate conic D1 + g D2 with its known zero eigenvalue, two quadratics, Newton refinement of
 // the depths, the pose from a 3x3 inverse.  Only + - * / and sqrt as explicit non-fused intrinsics, fixed iteration counts:
 // the results are bit-identical to the plain IEEE restatement compiled with -ffp-contract=off (oracle/ransac_oracle.c).
-#include <float.h>
-#include <math.h>
-
-#include "cvb_internal.cuh"
-#include "geom_common.cuh"
+#include "ransac_common.cuh"
 
 namespace {
 
-constexpr int kThreads = 256, kWave = 64;
 constexpr int kCubicNewtonIters = 30, kDepthNewtonIters = 5;
 
 __device__ __forceinline__ double dv(double a, double b) { return __ddiv_rn(a, b); }
 __device__ __forceinline__ double sq(double a) { return __dsqrt_rn(a); }
 __device__ __forceinline__ double dotv(const double* a, const double* b) { return dot3(a[0], a[1], a[2], b); }
-__device__ __forceinline__ void cross3(const double* a, const double* b, double* o) {
-  o[0] = sub(mul(a[1], b[2]), mul(a[2], b[1]));
-  o[1] = sub(mul(a[2], b[0]), mul(a[0], b[2]));
-  o[2] = sub(mul(a[0], b[1]), mul(a[1], b[0]));
-}
 
 // symmetric 3x3 as (s00, s01, s02, s11, s12, s22) → cofactors in the same layout
 __device__ __forceinline__ void sym_cof(const double* s, double* c) {
@@ -74,15 +63,8 @@ __device__ double cubic_root(double b, double c, double d) {
 // unit eigenvector of symmetric A for eigenvalue e: the largest cross product of two rows of A - eI
 __device__ void eigvec(const double* A, double e, double* v) {
   const double r0[3] = {sub(A[0], e), A[1], A[2]}, r1[3] = {A[1], sub(A[3], e), A[4]}, r2[3] = {A[2], A[4], sub(A[5], e)};
-  double c0[3], c1[3], c2[3];
-  cross3(r0, r1, c0); cross3(r0, r2, c1); cross3(r1, r2, c2);
-  const double n0 = dotv(c0, c0), n1 = dotv(c1, c1), n2 = dotv(c2, c2);
-  const double* best = c0;
-  double bn = n0;
-  if (n1 > bn) { bn = n1; best = c1; }
-  if (n2 > bn) { bn = n2; best = c2; }
-  const double s = sq(bn);
-  for (int i = 0; i < 3; i++) v[i] = dv(best[i], s);
+  const double s = sq(cross_max(r0, r1, r2, v));
+  for (int i = 0; i < 3; i++) v[i] = dv(v[i], s);
 }
 
 __device__ __forceinline__ double depth_residual(const double* L, const double* a, const double* b) {
@@ -240,94 +222,43 @@ __device__ bool hypothesis(const int* s, int n, const double* pts, const double*
 struct RansacDev {
   const int* prob_ptr; const double* pts; const double* f; const double* sigma; const double* cam;   // cam: [n_prob][12] offset, Rc
   const int* samples;
-  int n_samples, max_iterations;
-  double threshold, log_p;
-  int* best_sample; double* best_model; int* best_count; int* iterations; int* consumed;
-  uint8_t* inlier_mask;                                    // nullable
-  double* sample_model; uint8_t* sample_valid; int* sample_count;   // nullable together
+  RansacOut o;
+};
+
+// problem blockIdx.x for ransac_cta
+struct AbsProblem {
+  const double *P, *F, *S, *cam;
+  const int* samples;   // [n_samples][4] of this problem
+  int n, n_samples;
+  __device__ AbsProblem(const RansacDev& D, int pi, int off)
+      : P(D.pts + 3 * (size_t)off), F(D.f + 3 * (size_t)off), S(D.sigma + off), cam(D.cam + 12 * (size_t)pi),
+        samples(D.samples + 4 * (size_t)pi * D.o.n_samples), n(D.prob_ptr[pi + 1] - off), n_samples(D.o.n_samples) {}
+  // the first kWave threads solve one sample each
+  __device__ void solve_wave(int base, double (*w_model)[12], int* w_valid) const {
+    const int tid = threadIdx.x;
+    if (tid >= kWave) return;
+    const int s = base + tid;
+    double M[12];
+    for (int i = 0; i < 12; i++) M[i] = 0.0;
+    bool v = false;
+    if (s < n_samples) v = hypothesis(samples + 4 * (size_t)s, n, P, F, cam, M);
+    if (!v)
+      for (int i = 0; i < 12; i++) M[i] = 0.0;
+    for (int i = 0; i < 12; i++) w_model[tid][i] = M[i];
+    w_valid[tid] = v;
+  }
+  // the score of correspondence i under M
+  __device__ auto scorer(const double* M) const {
+    double Ri[9], ti[3];
+    abs_inverse(M, Ri, ti);
+    return [=](int i) { return abs_score(Ri, ti, P + 3 * (size_t)i, F + 3 * (size_t)i, S[i], cam); };
+  }
 };
 
 __global__ void __launch_bounds__(kThreads) ransac_abs_kernel(RansacDev D) {
-  const int pi = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const int off = D.prob_ptr[pi], n = D.prob_ptr[pi + 1] - off;
-  const double* P = D.pts + 3 * (size_t)off;
-  const double* F = D.f + 3 * (size_t)off;
-  const double* S = D.sigma + off;
-  const double* cam = D.cam + 12 * (size_t)pi;
-  const bool all = D.sample_model != nullptr;
-  __shared__ double w_model[kWave][12];
-  __shared__ int w_valid[kWave], w_count[kWave];
-  __shared__ double best_model[12], k_bound;
-  __shared__ int best, best_n, it, used, running;
-  __shared__ long long skipped;
-  if (tid == 0) {
-    best = -1; best_n = 0; it = 0; used = 0; skipped = 0; k_bound = (double)D.max_iterations;
-    running = D.max_iterations > 0;
-    for (int i = 0; i < 12; i++) best_model[i] = 0.0;
-  }
-  __syncthreads();
-  const long long max_skip = 10LL * D.max_iterations;
-  for (int base = 0; base < D.n_samples && (running || all); base += kWave) {
-    if (tid < kWave) {
-      const int s = base + tid;
-      double M[12];
-      for (int i = 0; i < 12; i++) M[i] = 0.0;
-      bool v = false;
-      if (s < D.n_samples) v = hypothesis(D.samples + 4 * ((size_t)pi * D.n_samples + s), n, P, F, cam, M);
-      if (!v)
-        for (int i = 0; i < 12; i++) M[i] = 0.0;
-      for (int i = 0; i < 12; i++) w_model[tid][i] = M[i];
-      w_valid[tid] = v;
-    }
-    __syncthreads();
-    for (int h = warp; h < kWave; h += kThreads / 32) {
-      int cnt = 0;
-      if (w_valid[h]) {
-        double Ri[9], ti[3];
-        abs_inverse(w_model[h], Ri, ti);
-        for (int i = lane; i < n; i += 32) cnt += abs_score(Ri, ti, P + 3 * (size_t)i, F + 3 * (size_t)i, S[i], cam) < D.threshold;
-        for (int o = 16; o > 0; o >>= 1) cnt += __shfl_xor_sync(0xffffffffu, cnt, o);   // integer: order-independent
-      }
-      if (lane == 0) w_count[h] = cnt;
-    }
-    __syncthreads();
-    if (all && tid < kWave && base + tid < D.n_samples) {
-      const size_t g = (size_t)pi * D.n_samples + base + tid;
-      for (int i = 0; i < 12; i++) D.sample_model[12 * g + i] = w_model[tid][i];
-      D.sample_valid[g] = (uint8_t)w_valid[tid]; D.sample_count[g] = w_count[tid];
-    }
-    if (tid == 0) {   // placerec.ransac_select over the valid samples, opengv's skipped_count for the invalid ones
-      for (int h = 0; h < kWave && base + h < D.n_samples; h++) {
-        running = it < D.max_iterations && (double)it < k_bound && skipped < max_skip;
-        if (!running) break;
-        used++;
-        if (!w_valid[h]) { skipped++; continue; }
-        const int c = w_count[h];
-        if (c > best_n) {
-          best_n = c; best = base + h;
-          for (int i = 0; i < 12; i++) best_model[i] = w_model[h][i];
-          const double w = dv((double)c, (double)n);
-          double pno = sub(1.0, mul(mul(mul(w, w), w), w));
-          pno = pno > DBL_EPSILON ? pno : DBL_EPSILON;
-          pno = pno < 1.0 - DBL_EPSILON ? pno : 1.0 - DBL_EPSILON;
-          k_bound = dv(D.log_p, log(pno));
-        }
-        it++;
-      }
-      running = it < D.max_iterations && (double)it < k_bound && skipped < max_skip;
-    }
-    __syncthreads();
-  }
-  if (tid == 0) {
-    D.best_sample[pi] = best; D.best_count[pi] = best_n; D.iterations[pi] = it; D.consumed[pi] = used;
-    for (int i = 0; i < 12; i++) D.best_model[12 * (size_t)pi + i] = best_model[i];
-  }
-  if (D.inlier_mask) {
-    double Ri[9], ti[3];
-    abs_inverse(best_model, Ri, ti);
-    for (int i = tid; i < n; i += kThreads)
-      D.inlier_mask[off + i] = best >= 0 && abs_score(Ri, ti, P + 3 * (size_t)i, F + 3 * (size_t)i, S[i], cam) < D.threshold;
-  }
+  const int pi = blockIdx.x, off = D.prob_ptr[pi];
+  AbsProblem Pb(D, pi, off);
+  ransac_cta<4>(D.o, Pb, off, Pb.n);
 }
 
 }  // namespace
@@ -336,64 +267,25 @@ extern "C" int cvb_ransac_absolute_pose_batch(cvb_ctx* ctx, const cvb_abs_ransac
                                               double probability, cvb_abs_ransac_result* r) {
   if (!ctx) return CVB_ERR_INVALID;
   CVB_GUARD(ctx);
-  CVB_REQUIRE(ctx, p && r && p->n_prob >= 0 && p->n_samples >= 0 && max_iterations >= 0, "ransac_absolute_pose: bad arguments");
-  CVB_REQUIRE(ctx, max_iterations <= INT32_MAX / 10, "ransac_absolute_pose: max_iterations too large");
+  if (const int rc = check_ransac(ctx, "ransac_absolute_pose", p, max_iterations, r, 4)) return rc;
   const int n_prob = p->n_prob, ns = p->n_samples;
   if (n_prob == 0) return CVB_OK;
-  CVB_REQUIRE(ctx, p->prob_ptr && p->cam_off && p->cam_rot && r->best_sample && r->best_model && r->best_count && r->iterations && r->consumed,
-              "ransac_absolute_pose: null required pointer");
-  CVB_REQUIRE(ctx, (r->sample_model != nullptr) == (r->sample_valid != nullptr) && (r->sample_model != nullptr) == (r->sample_count != nullptr),
-              "ransac_absolute_pose: sample_model / sample_valid / sample_count are requested together");
-  CVB_REQUIRE(ctx, p->prob_ptr[0] == 0, "ransac_absolute_pose: prob_ptr[0] != 0");
-  for (int i = 0; i < n_prob; i++) CVB_REQUIRE(ctx, p->prob_ptr[i + 1] >= p->prob_ptr[i], "ransac_absolute_pose: prob_ptr decreases at %d", i);
+  CVB_REQUIRE(ctx, p->cam_off && p->cam_rot, "ransac_absolute_pose: null camera arrays");
   const size_t N = (size_t)p->prob_ptr[n_prob];
   CVB_REQUIRE(ctx, N == 0 || (p->pts && p->f && p->sigma), "ransac_absolute_pose: null correspondence arrays");
-  CVB_REQUIRE(ctx, ns == 0 || p->samples, "ransac_absolute_pose: null samples");
-  for (int i = 0; i < n_prob; i++) {
-    const int n = p->prob_ptr[i + 1] - p->prob_ptr[i];
-    if (n < 4) continue;   // every sample of such a problem is invalid; its indices are not read
-    const int32_t* s = p->samples + 4 * (size_t)i * ns;
-    for (size_t j = 0; j < 4 * (size_t)ns; j++)
-      CVB_REQUIRE(ctx, s[j] >= 0 && s[j] < n, "ransac_absolute_pose: sample index %d out of range [0, %d) in problem %d", s[j], n, i);
-  }
-  const size_t S_all = (size_t)n_prob * ns;
-  const bool all = r->sample_model != nullptr;
   Stager St;
   const size_t o_ptr = St.put(p->prob_ptr, ((size_t)n_prob + 1) * 4), o_pts = St.put(p->pts, N * 24), o_f = St.put(p->f, N * 24),
-               o_sg = St.put(p->sigma, N * 8), o_smp = St.put(p->samples, S_all * 16);
+               o_sg = St.put(p->sigma, N * 8), o_smp = St.put(p->samples, (size_t)n_prob * ns * 16);
   const size_t o_cam = St.reserve((size_t)n_prob * 96);
   for (int i = 0; i < n_prob; i++) {   // one camera per problem: offset (3) directly followed by the rotation (9, row-major)
     memcpy(St.h.data() + o_cam + 96 * (size_t)i, p->cam_off + 3 * (size_t)i, 24);
     memcpy(St.h.data() + o_cam + 96 * (size_t)i + 24, p->cam_rot + 9 * (size_t)i, 72);
   }
-  const size_t in_bytes = St.h.size();
-  const size_t o_bm = St.reserve((size_t)n_prob * 96), o_bs = St.reserve((size_t)n_prob * 4), o_bc = St.reserve((size_t)n_prob * 4),
-               o_it = St.reserve((size_t)n_prob * 4), o_us = St.reserve((size_t)n_prob * 4), o_mask = r->inlier_mask ? St.reserve(N) : 0,
-               o_sm = all ? St.reserve(S_all * 96) : 0, o_sv = all ? St.reserve(S_all) : 0, o_sc = all ? St.reserve(S_all * 4) : 0;
-  const size_t total = St.h.size();
-  unsigned char* d = (unsigned char*)cvb_ws(ctx, WS_GS5, total);
-  unsigned char* hpin = (unsigned char*)cvb_pinned(ctx, total);
-  if (!d || !hpin) return CVB_ERR_CUDA;
-  memcpy(hpin, St.h.data(), in_bytes);
-  RansacDev D{};
-  D.prob_ptr = (const int*)(d + o_ptr); D.pts = (const double*)(d + o_pts); D.f = (const double*)(d + o_f); D.sigma = (const double*)(d + o_sg);
-  D.cam = (const double*)(d + o_cam); D.samples = (const int*)(d + o_smp);
-  D.n_samples = ns; D.max_iterations = max_iterations; D.threshold = threshold; D.log_p = log(1.0 - probability);
-  D.best_sample = (int*)(d + o_bs); D.best_model = (double*)(d + o_bm); D.best_count = (int*)(d + o_bc); D.iterations = (int*)(d + o_it);
-  D.consumed = (int*)(d + o_us); D.inlier_mask = r->inlier_mask ? d + o_mask : nullptr;
-  if (all) { D.sample_model = (double*)(d + o_sm); D.sample_valid = d + o_sv; D.sample_count = (int*)(d + o_sc); }
-  cudaStream_t st = ctx->stream;
-  CVB_CUDA(ctx, cudaMemcpyAsync(d, hpin, in_bytes, cudaMemcpyHostToDevice, st));
-  ransac_abs_kernel<<<n_prob, kThreads, 0, st>>>(D);
-  CVB_CHECK_LAUNCH(ctx);
-  CVB_CUDA(ctx, cudaMemcpyAsync(hpin + o_bm, d + o_bm, total - o_bm, cudaMemcpyDeviceToHost, st));
-  CVB_CUDA(ctx, cudaStreamSynchronize(st));
-  memcpy(r->best_model, hpin + o_bm, (size_t)n_prob * 96); memcpy(r->best_sample, hpin + o_bs, (size_t)n_prob * 4);
-  memcpy(r->best_count, hpin + o_bc, (size_t)n_prob * 4); memcpy(r->iterations, hpin + o_it, (size_t)n_prob * 4);
-  memcpy(r->consumed, hpin + o_us, (size_t)n_prob * 4);
-  if (r->inlier_mask) memcpy(r->inlier_mask, hpin + o_mask, N);
-  if (all) {
-    memcpy(r->sample_model, hpin + o_sm, S_all * 96); memcpy(r->sample_valid, hpin + o_sv, S_all); memcpy(r->sample_count, hpin + o_sc, S_all * 4);
-  }
-  return CVB_OK;
+  const auto inputs = [&](unsigned char* d) {
+    RansacDev D{};
+    D.prob_ptr = (const int*)(d + o_ptr); D.pts = (const double*)(d + o_pts); D.f = (const double*)(d + o_f); D.sigma = (const double*)(d + o_sg);
+    D.cam = (const double*)(d + o_cam); D.samples = (const int*)(d + o_smp);
+    return D;
+  };
+  return run_ransac(ctx, WS_GS5, ransac_abs_kernel, 0, St, inputs, n_prob, ns, N, threshold, max_iterations, probability, r);
 }

@@ -11,25 +11,21 @@
 // (cvb_noncentral_relative_pose_covariance_batch, rel_cov_solve_kernel / rel_cov_reduce_kernel at the end of the file;
 // oracle/relpose_cov_oracle.c restates it).
 //
-// One CTA per problem, both rigs staged in shared memory.  Samples are taken in waves of kWave: each warp solves one sample at
-// a time (lane k owns column k of A^T in its warp's shared-memory area, every norm and dot product is a sequential sum inside
-// one lane), then every warp scores the wave's hypotheses against all correspondences (camera-pair models in the warp's area,
-// warp-shuffle integer counts), thread 0 replays the selection over the wave in sample order, and the CTA stops as soon as the
-// adaptive bound ends the selection.  The CTA then writes the selected model's inlier mask.
+// One CTA per problem, both rigs staged in shared memory, driven by ransac_cta (ransac_common.cuh, shared with ransac_abs.cu):
+// the waves of kWave samples, the scoring, the selection with its early stop and the inlier mask.  This file supplies the
+// solvers: in each wave a warp solves one sample at a time (lane k owns column k of A^T in its warp's shared-memory area, the
+// Householder QR warp_householder serves both solvers, every norm and dot product is a sequential sum inside one lane); a
+// hypothesis is scored through its camera-pair models in the warp's area.
 //
 // Only + - * / and sqrt as explicit non-fused intrinsics, fixed iteration counts: the results are bit-identical to the plain
 // IEEE restatement compiled with -ffp-contract=off (oracle/ransac_rel_oracle.c for the 17-point solver,
 // oracle/ransac_rel5_oracle.c for the 5-point one; their headers state the problems and their assumptions; so does
 // include/covins_b200.h).
-#include <float.h>
-#include <math.h>
-
-#include "cvb_internal.cuh"
-#include "geom_common.cuh"
+#include "ransac_common.cuh"
 
 namespace {
 
-constexpr int kThreads = 256, kWarps = kThreads / 32, kWave = 64, kSample = 17, kMaxCams = CVB_REL_MAX_CAMS;
+constexpr int kSample = 17, kMaxCams = CVB_REL_MAX_CAMS;
 constexpr int kPolarIters = 12;
 constexpr double kRankTol = 1e-10;
 // per-warp shared-memory area (doubles): the solver's arrays, or the camera-pair models (12 each) while scoring
@@ -37,13 +33,6 @@ constexpr int kLd = 19;   // leading dimension of A^T's columns (17 lanes hit di
 constexpr int oAt = 0, oDm = oAt + kSample * kLd, oX = oDm + kSample * 12, oAl = oX + 18, oVt = oAl + kSample, oGh = oVt + kSample,
               oR = oGh + kSample * 4, kSolveArea = oR + 9;
 constexpr int kPairArea = 12;
-constexpr unsigned kFull = 0xffffffffu;
-
-__device__ __forceinline__ void cross3(const double* a, const double* b, double* o) {
-  o[0] = sub(mul(a[1], b[2]), mul(a[2], b[1]));
-  o[1] = sub(mul(a[2], b[0]), mul(a[0], b[2]));
-  o[2] = sub(mul(a[0], b[1]), mul(a[1], b[0]));
-}
 
 // d = Rc f, m = c x d; cam = offset (3) then Rc (9, row-major)
 __device__ __forceinline__ void plucker(const double* cam, const double* f, double* d, double* m) {
@@ -66,7 +55,40 @@ __device__ void pair_model(const double* M, const double* cam1, const double* ca
   }
 }
 
-__device__ __forceinline__ bool finite3(const double* v) { return isfinite(v[0]) && isfinite(v[1]) && isfinite(v[2]); }
+// Householder QR of the kRows x kCols matrix in the warp's shared memory A, lane j owning column j (leading dimension kLd): step
+// k reflects rows k .. kRows - 1; v_k overwrites column k from row k, r_kk = al[k], |v_k|^2 = vt[k].  Returns the rank test,
+// every |r_kk| >= kRankTol * max |r_kk| and max |r_kk| > 0, which every lane evaluates on the same values (warp-uniform).
+template <int kRows, int kCols, int kLd>
+__device__ __forceinline__ bool warp_householder(double* A, double* al, double* vt, int lane) {
+  for (int k = 0; k < kCols; k++) {
+    if (lane == k) {
+      double* col = A + kLd * k;
+      double ss = 0.0;
+      for (int i = k; i < kRows; i++) ss = i == k ? mul(col[i], col[i]) : add(ss, mul(col[i], col[i]));
+      const double sigma = __dsqrt_rn(ss), ak = col[k];
+      const double alpha = ak >= 0.0 ? -sigma : sigma;
+      col[k] = sub(ak, alpha);
+      al[k] = alpha;
+      vt[k] = mul(2.0, add(ss, mul(fabs(ak), sigma)));
+    }
+    __syncwarp();
+    if (lane > k && lane < kCols) {
+      const double* v = A + kLd * k;
+      double* a = A + kLd * lane;
+      double dot = 0.0;
+      for (int i = k; i < kRows; i++) dot = i == k ? mul(v[i], a[i]) : add(dot, mul(v[i], a[i]));
+      const double c = __ddiv_rn(mul(2.0, dot), vt[k]);
+      for (int i = k; i < kRows; i++) a[i] = sub(a[i], mul(c, v[i]));
+    }
+    __syncwarp();
+  }
+  double rmax = 0.0;
+  for (int k = 0; k < kCols; k++) rmax = fabs(al[k]) > rmax ? fabs(al[k]) : rmax;
+  bool good = rmax > 0.0;
+  for (int k = 0; k < kCols; k++)
+    if (!(fabs(al[k]) >= mul(kRankTol, rmax))) good = false;
+  return good;
+}
 
 // the hypothesis of sample s (17 problem-local indices), solved by one warp in its area W; lane 0 writes the model.  Returns the
 // (warp-uniform) valid flag.
@@ -93,38 +115,7 @@ __device__ bool rel17(const int* s, int n, const double* F1, const double* F2, c
       }
   }
   __syncwarp();
-  // Householder QR of A^T: step k reflects rows k..17; v_k overwrites column k from row k, r_kk = al[k], |v_k|^2 = vt[k]
-  for (int k = 0; k < kSample; k++) {
-    if (lane == k) {
-      double* col = At + kLd * k;
-      double ss = 0.0;
-      for (int i = k; i < 18; i++) ss = i == k ? mul(col[i], col[i]) : add(ss, mul(col[i], col[i]));
-      const double sigma = __dsqrt_rn(ss), ak = col[k];
-      const double alpha = ak >= 0.0 ? -sigma : sigma;
-      col[k] = sub(ak, alpha);
-      al[k] = alpha;
-      vt[k] = mul(2.0, add(ss, mul(fabs(ak), sigma)));
-    }
-    __syncwarp();
-    if (lane > k && lane < kSample) {
-      const double* v = At + kLd * k;
-      double* a = At + kLd * lane;
-      double dot = 0.0;
-      for (int i = k; i < 18; i++) dot = i == k ? mul(v[i], a[i]) : add(dot, mul(v[i], a[i]));
-      const double c = __ddiv_rn(mul(2.0, dot), vt[k]);
-      for (int i = k; i < 18; i++) a[i] = sub(a[i], mul(c, v[i]));
-    }
-    __syncwarp();
-  }
-  int good = 0;
-  if (lane == 0) {   // rank: every |r_kk| >= kRankTol * max |r_kk|
-    double rmax = 0.0;
-    for (int k = 0; k < kSample; k++) rmax = fabs(al[k]) > rmax ? fabs(al[k]) : rmax;
-    good = rmax > 0.0;
-    for (int k = 0; k < kSample; k++)
-      if (!(fabs(al[k]) >= mul(kRankTol, rmax))) good = 0;
-  }
-  if (!__shfl_sync(kFull, good, 0)) return false;
+  if (!warp_householder<18, kSample, kLd>(At, al, vt, lane)) return false;   // QR of A^T (18 x 17)
   // x = H_0 H_1 ... H_16 e18 (every lane forms the same dot product; lane i updates x[i])
   if (lane < 18) x[lane] = lane == 17 ? 1.0 : 0.0;
   for (int k = kSample - 1; k >= 0; k--) {
@@ -137,6 +128,7 @@ __device__ bool rel17(const int* s, int n, const double* F1, const double* F2, c
     if (lane >= k && lane < 18) x[lane] = sub(x[lane], mul(c, v[lane]));
   }
   __syncwarp();
+  int good = 0;
   if (lane == 0) {   // R' = x[9:18] with det > 0, its polar factor by Newton from |R'|_F = sqrt(3)
     double X[9], Xi[9];
     for (int i = 0; i < 9; i++) X[i] = x[9 + i];
@@ -234,19 +226,6 @@ __device__ __forceinline__ double horner(const double* c, int d, double x) {
   return v;
 }
 __device__ __forceinline__ int sgn(double v) { return (v > 0.0) - (v < 0.0); }
-// the largest of the three cross products r0 x r1, r0 x r2, r1 x r2 (the first on ties) and its squared norm
-__device__ __forceinline__ double cross_max(const double* r0, const double* r1, const double* r2, double* v) {
-  double c[3][3];
-  cross3(r0, r1, c[0]); cross3(r0, r2, c[1]); cross3(r1, r2, c[2]);
-  double best = dot3(c[0][0], c[0][1], c[0][2], c[0]);
-  v[0] = c[0][0]; v[1] = c[0][1]; v[2] = c[0][2];
-#pragma unroll
-  for (int j = 1; j < 3; j++) {
-    const double nj = dot3(c[j][0], c[j][1], c[j][2], c[j]);
-    if (nj > best) { best = nj; v[0] = c[j][0]; v[1] = c[j][1]; v[2] = c[j][2]; }
-  }
-  return best;
-}
 
 // at most kPolish Gauss-Newton steps on the ten cubics A0 m(x, y, z) = 0 (A0 row-major) from v = (x, y, z); the first step that
 // does not lower |F|^2 is undone and ends the polish.  The monomials are recomputed per row (the same expressions as the oracle's
@@ -316,37 +295,7 @@ __device__ bool rel5(const int* s, int n, const double* F1, const double* F2, do
       for (int c = 0; c < 3; c++) Qt[9 * lane + 3 * r + c] = mul(a[r], b[c]);
   }
   __syncwarp();
-  for (int k = 0; k < kSample5; k++) {
-    if (lane == k) {
-      double* col = Qt + 9 * k;
-      double ss = 0.0;
-      for (int i = k; i < 9; i++) ss = i == k ? mul(col[i], col[i]) : add(ss, mul(col[i], col[i]));
-      const double sigma = __dsqrt_rn(ss), ak = col[k];
-      const double alpha = ak >= 0.0 ? -sigma : sigma;
-      col[k] = sub(ak, alpha);
-      al[k] = alpha;
-      vt[k] = mul(2.0, add(ss, mul(fabs(ak), sigma)));
-    }
-    __syncwarp();
-    if (lane > k && lane < kSample5) {
-      const double* v = Qt + 9 * k;
-      double* a = Qt + 9 * lane;
-      double dot = 0.0;
-      for (int i = k; i < 9; i++) dot = i == k ? mul(v[i], a[i]) : add(dot, mul(v[i], a[i]));
-      const double c = __ddiv_rn(mul(2.0, dot), vt[k]);
-      for (int i = k; i < 9; i++) a[i] = sub(a[i], mul(c, v[i]));
-    }
-    __syncwarp();
-  }
-  int good = 0;
-  if (lane == 0) {
-    double rmax = 0.0;
-    for (int k = 0; k < kSample5; k++) rmax = fabs(al[k]) > rmax ? fabs(al[k]) : rmax;
-    good = rmax > 0.0;
-    for (int k = 0; k < kSample5; k++)
-      if (!(fabs(al[k]) >= mul(kRankTol, rmax))) good = 0;
-  }
-  if (!__shfl_sync(kFull, good, 0)) return false;
+  if (!warp_householder<9, kSample5, 9>(Qt, al, vt, lane)) return false;
   if (lane < 4) {   // basis vector `lane` = H_0 ... H_4 e_{5+lane}
     double x[9];
 #pragma unroll
@@ -566,6 +515,7 @@ __device__ bool rel5(const int* s, int n, const double* F1, const double* F2, do
     qual[lane] = best;
   }
   __syncwarp();
+  int good = 0;
   if (lane == 0) {   // the strictly lowest finite quality, roots in ascending order
     double best = INFINITY;
     int k = -1;
@@ -610,11 +560,8 @@ struct RelDev {
   const int* prob_ptr; const double* f1; const double* f2; const double* s1; const double* s2; const int* cam1; const int* cam2;
   const int* cam_ptr1; const int* cam_ptr2; const double* rig1; const double* rig2;   // rigs: [cam][12] offset then Rc
   const int* samples;
-  int n_samples, max_iterations, area;   // area: doubles per warp in dynamic shared memory
-  double threshold, log_p;
-  int* best_sample; double* best_model; int* best_count; int* iterations; int* consumed;
-  uint8_t* inlier_mask;                                    // nullable
-  double* sample_model; uint8_t* sample_valid; int* sample_count;   // nullable together
+  int area;   // doubles per warp in dynamic shared memory
+  RansacOut o;
 };
 
 // the camera-pair models of M for every pair (j1, j2) at P[12 (j1 nc2 + j2)], formed by the lanes of one warp
@@ -623,38 +570,52 @@ __device__ __forceinline__ void warp_pair_models(const double* M, const double* 
   __syncwarp();
 }
 
+// problem blockIdx.x for ransac_cta: its inputs, the rigs in shared memory and the warp's area W, which holds the solver's arrays
+// while a sample is solved and the camera-pair models of the hypothesis being scored
+template <class Sv>
+struct RelProblem {
+  ProbView P;
+  const double *S1, *S2;
+  int nc1, nc2;
+  const int* samples;   // [n_samples][Sv::kSample] of this problem
+  int n_samples;
+  double* W;
+  int warp, lane;
+  // each warp solves one sample at a time
+  __device__ void solve_wave(int base, double (*w_model)[12], int* w_valid) const {
+    for (int h = warp; h < kWave; h += kWarps) {
+      const int s = base + h;
+      bool v = false;
+      if (s < n_samples) v = Sv::solve(samples + Sv::kSample * (size_t)s, P, W, w_model[h], lane);
+      __syncwarp();
+      if (lane == 0) {
+        if (!v)
+          for (int i = 0; i < 12; i++) w_model[h][i] = 0.0;
+        w_valid[h] = v;
+      }
+    }
+  }
+  // the score of correspondence i under M (called by every lane of the warp)
+  __device__ auto scorer(const double* M) const {
+    warp_pair_models(M, P.rig1, nc1, P.rig2, nc2, W, lane);
+    return [this](int i) { return rel_score(W + kPairArea * (Sv::kCentral ? 0 : P.C1[i] * nc2 + P.C2[i]), P.F1, P.F2, S1, S2, i); };
+  }
+};
+
 // Sv: Solver17 (non-central, rigs and camera indices from D) or Solver5 (central: one identity camera per side)
 template <class Sv>
 __global__ void __launch_bounds__(kThreads) ransac_rel_kernel(RelDev D) {
-  constexpr int kS = Sv::kSample;
   extern __shared__ double dyn[];
-  const int pi = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int pi = blockIdx.x, tid = threadIdx.x;
   const int off = D.prob_ptr[pi], n = D.prob_ptr[pi + 1] - off;
   const int nc1 = Sv::kCentral ? 1 : D.cam_ptr1[pi + 1] - D.cam_ptr1[pi], nc2 = Sv::kCentral ? 1 : D.cam_ptr2[pi + 1] - D.cam_ptr2[pi];
-  const double* F1 = D.f1 + 3 * (size_t)off;
-  const double* F2 = D.f2 + 3 * (size_t)off;
-  const double* S1 = D.s1 + off;
-  const double* S2 = D.s2 + off;
-  const int* C1 = Sv::kCentral ? nullptr : D.cam1 + off;
-  const int* C2 = Sv::kCentral ? nullptr : D.cam2 + off;
-  double* W = dyn + (size_t)warp * D.area;
-  const bool all = D.sample_model != nullptr;
   __shared__ double rig1[kMaxCams * 12], rig2[kMaxCams * 12];
-  __shared__ double w_model[kWave][12];
-  __shared__ int w_valid[kWave], w_count[kWave];
-  __shared__ double best_model[12], k_bound;
-  __shared__ int best, best_n, it, used, running, rigs_finite;
-  __shared__ long long skipped;
+  __shared__ int rigs_finite;
   if (Sv::kCentral) {   // camera: offset 0, rotation I
     for (int i = tid; i < 12; i += kThreads) rig1[i] = rig2[i] = i == 3 || i == 7 || i == 11 ? 1.0 : 0.0;
   } else {
     for (int i = tid; i < 12 * nc1; i += kThreads) rig1[i] = D.rig1[12 * (size_t)D.cam_ptr1[pi] + i];
     for (int i = tid; i < 12 * nc2; i += kThreads) rig2[i] = D.rig2[12 * (size_t)D.cam_ptr2[pi] + i];
-  }
-  if (tid == 0) {
-    best = -1; best_n = 0; it = 0; used = 0; skipped = 0; k_bound = (double)D.max_iterations;
-    running = D.max_iterations > 0;
-    for (int i = 0; i < 12; i++) best_model[i] = 0.0;
   }
   __syncthreads();
   if (tid == 0) {
@@ -664,97 +625,11 @@ __global__ void __launch_bounds__(kThreads) ransac_rel_kernel(RelDev D) {
     rigs_finite = fin;
   }
   __syncthreads();
-  const ProbView P{n, F1, F2, C1, C2, rig1, rig2, rigs_finite != 0};
-  const long long max_skip = 10LL * D.max_iterations;
-  for (int base = 0; base < D.n_samples && (running || all); base += kWave) {
-    for (int h = warp; h < kWave; h += kWarps) {
-      const int s = base + h;
-      bool v = false;
-      if (s < D.n_samples)
-        v = Sv::solve(D.samples + kS * ((size_t)pi * D.n_samples + s), P, W, w_model[h], lane);
-      __syncwarp();
-      if (lane == 0) {
-        if (!v)
-          for (int i = 0; i < 12; i++) w_model[h][i] = 0.0;
-        w_valid[h] = v;
-      }
-    }
-    __syncthreads();
-    for (int h = warp; h < kWave; h += kWarps) {
-      int cnt = 0;
-      if (w_valid[h]) {
-        warp_pair_models(w_model[h], rig1, nc1, rig2, nc2, W, lane);
-        for (int i = lane; i < n; i += 32) {
-          const double* q = W + kPairArea * (Sv::kCentral ? 0 : C1[i] * nc2 + C2[i]);
-          cnt += rel_score(q, F1, F2, S1, S2, i) < D.threshold;
-        }
-        for (int o = 16; o > 0; o >>= 1) cnt += __shfl_xor_sync(kFull, cnt, o);   // integer: order-independent
-        __syncwarp();
-      }
-      if (lane == 0) w_count[h] = cnt;
-    }
-    __syncthreads();
-    if (all && tid < kWave && base + tid < D.n_samples) {
-      const size_t g = (size_t)pi * D.n_samples + base + tid;
-      for (int i = 0; i < 12; i++) D.sample_model[12 * g + i] = w_model[tid][i];
-      D.sample_valid[g] = (uint8_t)w_valid[tid]; D.sample_count[g] = w_count[tid];
-    }
-    if (tid == 0) {   // placerec.ransac_select over the valid samples, opengv's skipped_count for the invalid ones
-      for (int h = 0; h < kWave && base + h < D.n_samples; h++) {
-        running = it < D.max_iterations && (double)it < k_bound && skipped < max_skip;
-        if (!running) break;
-        used++;
-        if (!w_valid[h]) { skipped++; continue; }
-        const int c = w_count[h];
-        if (c > best_n) {
-          best_n = c; best = base + h;
-          for (int i = 0; i < 12; i++) best_model[i] = w_model[h][i];
-          const double w = __ddiv_rn((double)c, (double)n);
-          double wp = w;
-          for (int e = 1; e < kS; e++) wp = mul(wp, w);
-          double pno = sub(1.0, wp);
-          pno = pno > DBL_EPSILON ? pno : DBL_EPSILON;
-          pno = pno < 1.0 - DBL_EPSILON ? pno : 1.0 - DBL_EPSILON;
-          k_bound = __ddiv_rn(D.log_p, log(pno));
-        }
-        it++;
-      }
-      running = it < D.max_iterations && (double)it < k_bound && skipped < max_skip;
-    }
-    __syncthreads();
-  }
-  if (tid == 0) {
-    D.best_sample[pi] = best; D.best_count[pi] = best_n; D.iterations[pi] = it; D.consumed[pi] = used;
-    for (int i = 0; i < 12; i++) D.best_model[12 * (size_t)pi + i] = best_model[i];
-  }
-  if (D.inlier_mask) {
-    if (best >= 0) warp_pair_models(best_model, rig1, nc1, rig2, nc2, W, lane);   // every warp its own copy
-    for (int i = tid; i < n; i += kThreads) {
-      const double* q = W + kPairArea * (Sv::kCentral ? 0 : C1[i] * nc2 + C2[i]);
-      D.inlier_mask[off + i] = best >= 0 && rel_score(q, F1, F2, S1, S2, i) < D.threshold;
-    }
-  }
-}
-
-bool ptr_ok(const int32_t* p, int n) {
-  if (p[0] != 0) return false;
-  for (int i = 0; i < n; i++)
-    if (p[i + 1] < p[i]) return false;
-  return true;
-}
-
-// every sample index of a problem with at least k correspondences in [0, n); the samples of smaller problems, and of problems
-// flagged in skip (nullable), are not read
-int check_samples(cvb_ctx* ctx, const char* name, const int32_t* samples, const int32_t* prob_ptr, int n_prob, int ns, int k,
-                  const uint8_t* skip = nullptr) {
-  for (int i = 0; i < n_prob; i++) {
-    const int n = prob_ptr[i + 1] - prob_ptr[i];
-    if (n < k || (skip && skip[i])) continue;
-    const int32_t* s = samples + k * (size_t)i * ns;
-    for (size_t j = 0; j < k * (size_t)ns; j++)
-      CVB_REQUIRE(ctx, s[j] >= 0 && s[j] < n, "%s: sample index %d out of range [0, %d) in problem %d", name, s[j], n, i);
-  }
-  return CVB_OK;
+  RelProblem<Sv> Pb{ProbView{n, D.f1 + 3 * (size_t)off, D.f2 + 3 * (size_t)off, Sv::kCentral ? nullptr : D.cam1 + off,
+                             Sv::kCentral ? nullptr : D.cam2 + off, rig1, rig2, rigs_finite != 0},
+                    D.s1 + off, D.s2 + off, nc1, nc2, D.samples + Sv::kSample * (size_t)pi * D.o.n_samples, D.o.n_samples,
+                    dyn + (size_t)(tid >> 5) * D.area, tid >> 5, tid & 31};
+  ransac_cta<Sv::kSample>(D.o, Pb, off, n);
 }
 
 // staging offsets of the inputs (camera arrays unused by a central problem)
@@ -801,54 +676,30 @@ void stage_rigs(Stager& St, const cvb_rel_ransac_problems* p, RelIn& in) {
   }
 }
 
-// the tail shared by both calls: outputs staged after the inputs in St, one upload, one launch of ransac_rel_kernel<Sv>, one
-// download
+// ransac_rel_kernel<Sv> on the inputs staged in St (max_pairs: the largest camera-pair count of a problem)
 template <class Sv>
 int run_rel_ransac(cvb_ctx* ctx, Stager& St, const RelIn& in, int n_prob, int ns, size_t N, int max_pairs, double threshold, int max_iterations,
                    double probability, cvb_rel_ransac_result* r) {
-  const size_t S_all = (size_t)n_prob * ns;
-  const bool all = r->sample_model != nullptr;
-  const size_t in_bytes = St.h.size();
-  const size_t o_bm = St.reserve((size_t)n_prob * 96), o_bs = St.reserve((size_t)n_prob * 4), o_bc = St.reserve((size_t)n_prob * 4),
-               o_it = St.reserve((size_t)n_prob * 4), o_us = St.reserve((size_t)n_prob * 4), o_mask = r->inlier_mask ? St.reserve(N) : 0,
-               o_sm = all ? St.reserve(S_all * 96) : 0, o_sv = all ? St.reserve(S_all) : 0, o_sc = all ? St.reserve(S_all * 4) : 0;
-  const size_t total = St.h.size();
-  unsigned char* d = (unsigned char*)cvb_ws(ctx, WS_GS6, total);
-  unsigned char* hpin = (unsigned char*)cvb_pinned(ctx, total);
-  if (!d || !hpin) return CVB_ERR_CUDA;
-  memcpy(hpin, St.h.data(), in_bytes);
-  RelDev D{};
-  D.prob_ptr = (const int*)(d + in.ptr); D.f1 = (const double*)(d + in.f1); D.f2 = (const double*)(d + in.f2);
-  D.s1 = (const double*)(d + in.s1); D.s2 = (const double*)(d + in.s2); D.samples = (const int*)(d + in.smp);
-  if (!Sv::kCentral) {
-    D.cam1 = (const int*)(d + in.c1); D.cam2 = (const int*)(d + in.c2); D.cam_ptr1 = (const int*)(d + in.cp1); D.cam_ptr2 = (const int*)(d + in.cp2);
-    D.rig1 = (const double*)(d + in.rig1); D.rig2 = (const double*)(d + in.rig2);
-  }
-  D.n_samples = ns; D.max_iterations = max_iterations; D.threshold = threshold; D.log_p = log(1.0 - probability);
-  D.area = Sv::kArea > kPairArea * max_pairs ? Sv::kArea : kPairArea * max_pairs;
-  D.best_sample = (int*)(d + o_bs); D.best_model = (double*)(d + o_bm); D.best_count = (int*)(d + o_bc); D.iterations = (int*)(d + o_it);
-  D.consumed = (int*)(d + o_us); D.inlier_mask = r->inlier_mask ? d + o_mask : nullptr;
-  if (all) { D.sample_model = (double*)(d + o_sm); D.sample_valid = d + o_sv; D.sample_count = (int*)(d + o_sc); }
+  const int area = Sv::kArea > kPairArea * max_pairs ? Sv::kArea : kPairArea * max_pairs;
   constexpr int kMaxPairs = Sv::kCentral ? 1 : kMaxCams * kMaxCams;
   constexpr int kMaxArea = Sv::kArea > kPairArea * kMaxPairs ? Sv::kArea : kPairArea * kMaxPairs;
   static cvb_once_per_device once;
   if (once.first(ctx->device)) {
     CVB_CUDA(ctx, cudaFuncSetAttribute(ransac_rel_kernel<Sv>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(kWarps * kMaxArea * sizeof(double))));
   }
-  cudaStream_t st = ctx->stream;
-  CVB_CUDA(ctx, cudaMemcpyAsync(d, hpin, in_bytes, cudaMemcpyHostToDevice, st));
-  ransac_rel_kernel<Sv><<<n_prob, kThreads, (size_t)kWarps * D.area * sizeof(double), st>>>(D);
-  CVB_CHECK_LAUNCH(ctx);
-  CVB_CUDA(ctx, cudaMemcpyAsync(hpin + o_bm, d + o_bm, total - o_bm, cudaMemcpyDeviceToHost, st));
-  CVB_CUDA(ctx, cudaStreamSynchronize(st));
-  memcpy(r->best_model, hpin + o_bm, (size_t)n_prob * 96); memcpy(r->best_sample, hpin + o_bs, (size_t)n_prob * 4);
-  memcpy(r->best_count, hpin + o_bc, (size_t)n_prob * 4); memcpy(r->iterations, hpin + o_it, (size_t)n_prob * 4);
-  memcpy(r->consumed, hpin + o_us, (size_t)n_prob * 4);
-  if (r->inlier_mask) memcpy(r->inlier_mask, hpin + o_mask, N);
-  if (all) {
-    memcpy(r->sample_model, hpin + o_sm, S_all * 96); memcpy(r->sample_valid, hpin + o_sv, S_all); memcpy(r->sample_count, hpin + o_sc, S_all * 4);
-  }
-  return CVB_OK;
+  const auto inputs = [&](unsigned char* d) {
+    RelDev D{};
+    D.prob_ptr = (const int*)(d + in.ptr); D.f1 = (const double*)(d + in.f1); D.f2 = (const double*)(d + in.f2);
+    D.s1 = (const double*)(d + in.s1); D.s2 = (const double*)(d + in.s2); D.samples = (const int*)(d + in.smp);
+    if (!Sv::kCentral) {
+      D.cam1 = (const int*)(d + in.c1); D.cam2 = (const int*)(d + in.c2); D.cam_ptr1 = (const int*)(d + in.cp1); D.cam_ptr2 = (const int*)(d + in.cp2);
+      D.rig1 = (const double*)(d + in.rig1); D.rig2 = (const double*)(d + in.rig2);
+    }
+    D.area = area;
+    return D;
+  };
+  return run_ransac(ctx, WS_GS6, ransac_rel_kernel<Sv>, (size_t)kWarps * area * sizeof(double), St, inputs, n_prob, ns, N, threshold,
+                    max_iterations, probability, r);
 }
 
 // ---- the sampling-based covariance of a 17-point model (cvb_noncentral_relative_pose_covariance_batch) ----
@@ -968,17 +819,12 @@ extern "C" int cvb_ransac_noncentral_relative_pose_batch(cvb_ctx* ctx, const cvb
                                                          double probability, cvb_rel_ransac_result* r) {
   if (!ctx) return CVB_ERR_INVALID;
   CVB_GUARD(ctx);
-  CVB_REQUIRE(ctx, p && r && p->n_prob >= 0 && p->n_samples >= 0 && max_iterations >= 0, "ransac_noncentral_relative_pose: bad arguments");
-  CVB_REQUIRE(ctx, max_iterations <= INT32_MAX / 10, "ransac_noncentral_relative_pose: max_iterations too large");
+  if (const int rc = check_ransac(ctx, "ransac_noncentral_relative_pose", p, max_iterations, r, kSample)) return rc;
   const int n_prob = p->n_prob, ns = p->n_samples;
   if (n_prob == 0) return CVB_OK;
-  CVB_REQUIRE(ctx, p->prob_ptr && p->cam_ptr1 && p->cam_ptr2 && r->best_sample && r->best_model && r->best_count && r->iterations && r->consumed,
-              "ransac_noncentral_relative_pose: null required pointer");
-  CVB_REQUIRE(ctx, (r->sample_model != nullptr) == (r->sample_valid != nullptr) && (r->sample_model != nullptr) == (r->sample_count != nullptr),
-              "ransac_noncentral_relative_pose: sample_model / sample_valid / sample_count are requested together");
+  CVB_REQUIRE(ctx, p->cam_ptr1 && p->cam_ptr2, "ransac_noncentral_relative_pose: null cam_ptr1 / cam_ptr2");
   int max_pairs = 0;
   if (const int rc = check_rel_problems(ctx, "ransac_noncentral_relative_pose", p, true, &max_pairs)) return rc;
-  if (const int rc = check_samples(ctx, "ransac_noncentral_relative_pose", p->samples, p->prob_ptr, n_prob, ns, kSample)) return rc;
   const size_t N = (size_t)p->prob_ptr[n_prob], S_all = (size_t)n_prob * ns;
   Stager St;
   RelIn in{};
@@ -994,19 +840,11 @@ extern "C" int cvb_ransac_central_relative_pose_batch(cvb_ctx* ctx, const cvb_ce
                                                       double probability, cvb_rel_ransac_result* r) {
   if (!ctx) return CVB_ERR_INVALID;
   CVB_GUARD(ctx);
-  CVB_REQUIRE(ctx, p && r && p->n_prob >= 0 && p->n_samples >= 0 && max_iterations >= 0, "ransac_central_relative_pose: bad arguments");
-  CVB_REQUIRE(ctx, max_iterations <= INT32_MAX / 10, "ransac_central_relative_pose: max_iterations too large");
+  if (const int rc = check_ransac(ctx, "ransac_central_relative_pose", p, max_iterations, r, kSample5)) return rc;
   const int n_prob = p->n_prob, ns = p->n_samples;
   if (n_prob == 0) return CVB_OK;
-  CVB_REQUIRE(ctx, p->prob_ptr && r->best_sample && r->best_model && r->best_count && r->iterations && r->consumed,
-              "ransac_central_relative_pose: null required pointer");
-  CVB_REQUIRE(ctx, (r->sample_model != nullptr) == (r->sample_valid != nullptr) && (r->sample_model != nullptr) == (r->sample_count != nullptr),
-              "ransac_central_relative_pose: sample_model / sample_valid / sample_count are requested together");
-  CVB_REQUIRE(ctx, ptr_ok(p->prob_ptr, n_prob), "ransac_central_relative_pose: prob_ptr does not start at 0 or decreases");
   const size_t N = (size_t)p->prob_ptr[n_prob];
   CVB_REQUIRE(ctx, N == 0 || (p->f1 && p->f2 && p->sigma1 && p->sigma2), "ransac_central_relative_pose: null correspondence arrays");
-  CVB_REQUIRE(ctx, ns == 0 || p->samples, "ransac_central_relative_pose: null samples");
-  if (const int rc = check_samples(ctx, "ransac_central_relative_pose", p->samples, p->prob_ptr, n_prob, ns, kSample5)) return rc;
   Stager St;
   RelIn in{};
   in.ptr = St.put(p->prob_ptr, ((size_t)n_prob + 1) * 4); in.f1 = St.put(p->f1, N * 24); in.f2 = St.put(p->f2, N * 24);

@@ -174,9 +174,25 @@ class CAbsRansacProblems(C.Structure):
                [("n_samples", C.c_int32)]
 
 
-class CAbsRansacResult(C.Structure):
+class CRansacResult(C.Structure):
+    """cvb_abs_ransac_result and cvb_rel_ransac_result (the same layout)"""
     _fields_ = [(k, c_vp) for k in ("best_sample", "best_model", "best_count", "iterations", "consumed", "inlier_mask", "sample_model",
                                     "sample_valid", "sample_count")]
+
+
+CAbsRansacResult = CRelRansacResult = CRansacResult   # the names of the per-call result structs, kept for existing callers
+
+
+def _ransac(ctx, fn, P, n_prob, ns, n, threshold, max_iterations, probability, per_sample):
+    """one RANSAC call fn on the problems P (n_prob problems, ns samples each, n correspondences) → its result dict"""
+    r = dict(best_sample=np.zeros(n_prob, np.int32), best_model=np.zeros((n_prob, 3, 4)), best_count=np.zeros(n_prob, np.int32),
+             iterations=np.zeros(n_prob, np.int32), consumed=np.zeros(n_prob, np.int32), inlier_mask=np.zeros(n, np.uint8))
+    if per_sample:
+        r.update(sample_model=np.zeros((n_prob, ns, 3, 4)), sample_valid=np.zeros((n_prob, ns), np.uint8),
+                 sample_count=np.zeros((n_prob, ns), np.int32))
+    R = CRansacResult(*[r[k].ctypes.data if k in r else None for k, _ in CRansacResult._fields_])
+    ctx.check(fn(ctx.handle, C.byref(P), float(threshold), int(max_iterations), float(probability), C.byref(R)))
+    return r
 
 
 def ransac_absolute_pose(ctx: Context, prob_ptr, pts, bearings, sigma, cam_off, cam_rot, samples, threshold, max_iterations, probability=0.99,
@@ -191,24 +207,13 @@ def ransac_absolute_pose(ctx: Context, prob_ptr, pts, bearings, sigma, cam_off, 
     s = np.ascontiguousarray(sigma, np.float64).reshape(-1)
     co = np.ascontiguousarray(cam_off, np.float64).reshape(n_prob, 3); cr = np.ascontiguousarray(cam_rot, np.float64).reshape(n_prob, 9)
     smp = np.ascontiguousarray(samples, np.int32).reshape(n_prob, -1, 4); ns = smp.shape[1]
-    r = dict(best_sample=np.zeros(n_prob, np.int32), best_model=np.zeros((n_prob, 3, 4)), best_count=np.zeros(n_prob, np.int32),
-             iterations=np.zeros(n_prob, np.int32), consumed=np.zeros(n_prob, np.int32), inlier_mask=np.zeros(len(p), np.uint8))
-    if per_sample:
-        r.update(sample_model=np.zeros((n_prob, ns, 3, 4)), sample_valid=np.zeros((n_prob, ns), np.uint8),
-                 sample_count=np.zeros((n_prob, ns), np.int32))
     P = CAbsRansacProblems(n_prob, ptr.ctypes.data, p.ctypes.data, f.ctypes.data, s.ctypes.data, co.ctypes.data, cr.ctypes.data, smp.ctypes.data, ns)
-    R = CAbsRansacResult(*[r[k].ctypes.data if k in r else None for k, _ in CAbsRansacResult._fields_])
-    ctx.check(lib().cvb_ransac_absolute_pose_batch(ctx.handle, C.byref(P), float(threshold), int(max_iterations), float(probability), C.byref(R)))
-    return r
+    return _ransac(ctx, lib().cvb_ransac_absolute_pose_batch, P, n_prob, ns, len(p), threshold, max_iterations, probability, per_sample)
 
 
 class CRelRansacProblems(C.Structure):
     _fields_ = [("n_prob", C.c_int32)] + [(k, c_vp) for k in ("prob_ptr", "f1", "f2", "sigma1", "sigma2", "cam1", "cam2", "cam_ptr1", "cam_off1",
                                                                "cam_rot1", "cam_ptr2", "cam_off2", "cam_rot2", "samples")] + [("n_samples", C.c_int32)]
-
-
-class CRelRansacResult(CAbsRansacResult):
-    pass
 
 
 def ransac_noncentral_relative_pose(ctx: Context, prob_ptr, f1, f2, sigma1, sigma2, cam1, cam2, cam_ptr1, cam_off1, cam_rot1, cam_ptr2, cam_off2,
@@ -228,16 +233,8 @@ def ransac_noncentral_relative_pose(ctx: Context, prob_ptr, f1, f2, sigma1, sigm
     co1 = np.ascontiguousarray(cam_off1, np.float64).reshape(-1, 3); cr1 = np.ascontiguousarray(cam_rot1, np.float64).reshape(-1, 9)
     co2 = np.ascontiguousarray(cam_off2, np.float64).reshape(-1, 3); cr2 = np.ascontiguousarray(cam_rot2, np.float64).reshape(-1, 9)
     smp = np.ascontiguousarray(samples, np.int32).reshape(n_prob, -1, 17); ns = smp.shape[1]
-    r = dict(best_sample=np.zeros(n_prob, np.int32), best_model=np.zeros((n_prob, 3, 4)), best_count=np.zeros(n_prob, np.int32),
-             iterations=np.zeros(n_prob, np.int32), consumed=np.zeros(n_prob, np.int32), inlier_mask=np.zeros(len(a), np.uint8))
-    if per_sample:
-        r.update(sample_model=np.zeros((n_prob, ns, 3, 4)), sample_valid=np.zeros((n_prob, ns), np.uint8),
-                 sample_count=np.zeros((n_prob, ns), np.int32))
     P = CRelRansacProblems(n_prob, *[x.ctypes.data for x in (ptr, a, b, s1, s2, c1, c2, cp1, co1, cr1, cp2, co2, cr2, smp)], ns)
-    R = CRelRansacResult(*[r[k].ctypes.data if k in r else None for k, _ in CRelRansacResult._fields_])
-    ctx.check(lib().cvb_ransac_noncentral_relative_pose_batch(ctx.handle, C.byref(P), float(threshold), int(max_iterations), float(probability),
-                                                              C.byref(R)))
-    return r
+    return _ransac(ctx, lib().cvb_ransac_noncentral_relative_pose_batch, P, n_prob, ns, len(a), threshold, max_iterations, probability, per_sample)
 
 
 class CCentralRelRansacProblems(C.Structure):
@@ -255,16 +252,8 @@ def ransac_central_relative_pose(ctx: Context, prob_ptr, f1, f2, sigma1, sigma2,
     a = np.ascontiguousarray(f1, np.float64).reshape(-1, 3); b = np.ascontiguousarray(f2, np.float64).reshape(-1, 3)
     s1 = np.ascontiguousarray(sigma1, np.float64).reshape(-1); s2 = np.ascontiguousarray(sigma2, np.float64).reshape(-1)
     smp = np.ascontiguousarray(samples, np.int32).reshape(n_prob, -1, 5); ns = smp.shape[1]
-    r = dict(best_sample=np.zeros(n_prob, np.int32), best_model=np.zeros((n_prob, 3, 4)), best_count=np.zeros(n_prob, np.int32),
-             iterations=np.zeros(n_prob, np.int32), consumed=np.zeros(n_prob, np.int32), inlier_mask=np.zeros(len(a), np.uint8))
-    if per_sample:
-        r.update(sample_model=np.zeros((n_prob, ns, 3, 4)), sample_valid=np.zeros((n_prob, ns), np.uint8),
-                 sample_count=np.zeros((n_prob, ns), np.int32))
     P = CCentralRelRansacProblems(n_prob, *[x.ctypes.data for x in (ptr, a, b, s1, s2, smp)], ns)
-    R = CRelRansacResult(*[r[k].ctypes.data if k in r else None for k, _ in CRelRansacResult._fields_])
-    ctx.check(lib().cvb_ransac_central_relative_pose_batch(ctx.handle, C.byref(P), float(threshold), int(max_iterations), float(probability),
-                                                           C.byref(R)))
-    return r
+    return _ransac(ctx, lib().cvb_ransac_central_relative_pose_batch, P, n_prob, ns, len(a), threshold, max_iterations, probability, per_sample)
 
 
 class CRelCovResult(C.Structure):

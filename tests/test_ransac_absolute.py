@@ -10,18 +10,11 @@ import subprocess
 import numpy as np
 import pytest
 
-from covins_b200 import placerec as PR, synth
+from covins_b200 import placerec as PR
 from oracle import ransac as orr
+from ransac_helpers import _build_shim, _check_selection, _gpu_vs_oracle, _rand_rot
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-
-
-def _rand_rot(rng):
-    q = rng.normal(size=4); q /= np.linalg.norm(q)
-    w, x, y, z = q
-    return np.array([[1 - 2 * (y * y + z * z), 2 * (x * y - z * w), 2 * (x * z + y * w)],
-                     [2 * (x * y + z * w), 1 - 2 * (x * x + z * z), 2 * (y * z - x * w)],
-                     [2 * (x * z - y * w), 2 * (y * z + x * w), 1 - 2 * (x * x + y * y)]])
+S = 4
 
 
 def _rot_err(A, B):
@@ -146,39 +139,11 @@ def _batch(seed, sizes, n_samples, outlier_frac=0.3):
                 cam_rot=np.stack([p["Rc"] for p in probs]), samples=samples), probs
 
 
-def _expected_selection(valid, count, n, max_iterations, probability):
-    """placerec.ransac_select over the valid samples in order (opengv's skipped_count: at most 10 * max_iterations invalid ones)"""
-    idx, skipped, stop = [], 0, len(valid)
-    for s in range(len(valid)):
-        if skipped >= 10 * max_iterations:
-            stop = s
-            break
-        if valid[s]:
-            idx.append(s)
-        else:
-            skipped += 1
-    best, it = PR.ransac_select(np.asarray(count)[idx], n, 4, max_iterations, probability)
-    consumed = (idx[it - 1] + 1 if it > 0 else 0) if it < len(idx) else stop
-    return (idx[best] if best >= 0 else -1), it, consumed
-
-
-def _check_selection(b, r, max_iterations, probability):
-    ptr = b["prob_ptr"]
-    for i in range(len(ptr) - 1):
-        n = ptr[i + 1] - ptr[i]
-        best, it, consumed = _expected_selection(r["sample_valid"][i], r["sample_count"][i], n, max_iterations, probability)
-        assert (r["best_sample"][i], r["iterations"][i], r["consumed"][i]) == (best, it, consumed), i
-        if best >= 0:
-            assert r["best_count"][i] == r["sample_count"][i][best] and np.array_equal(r["best_model"][i], r["sample_model"][i][best])
-        else:
-            assert r["best_count"][i] == 0 and not r["best_model"][i].any() and not r["inlier_mask"][ptr[i]:ptr[i + 1]].any()
-
-
 def test_oracle_selection_equals_ransac_select():
     b, _ = _batch(3, [0, 3, 4, 57, 400, 400], 400, outlier_frac=0.6)
     for thr, max_it, prob in ((25.0, 300, 0.99), (25.0, 300, 0.999999), (25.0, 7, 0.99), (1e-3, 40, 0.99)):
         r = orr.ransac_absolute_pose(**b, threshold=thr, max_iterations=max_it, probability=prob, per_sample=True)
-        _check_selection(b, r, max_it, prob)
+        _check_selection(b, r, S, max_it, prob)
         lazy = orr.ransac_absolute_pose(**b, threshold=thr, max_iterations=max_it, probability=prob)
         for k in ("best_sample", "best_model", "best_count", "iterations", "consumed", "inlier_mask"):
             assert np.array_equal(lazy[k], r[k]), k
@@ -187,27 +152,19 @@ def test_oracle_selection_equals_ransac_select():
     b2 = {k: (v.copy() if isinstance(v, np.ndarray) else v) for k, v in b.items()}
     b2["samples"][:, :60, 3] = b2["samples"][:, :60, 0]
     r = orr.ransac_absolute_pose(**b2, threshold=25.0, max_iterations=2, per_sample=True)
-    _check_selection(b2, r, 2, 0.99)
+    _check_selection(b2, r, S, 2, 0.99)
     assert r["consumed"][4] == 20 and r["iterations"][4] == 0 and r["best_sample"][4] == -1
     # problems with fewer than 4 correspondences never have a hypothesis
     assert not r["sample_valid"][:2].any() and r["sample_valid"][2].any()
 
 
 # ------------------------------------------------------------------------------------------------- GPU (C-ABI)
-def _gpu_vs_oracle(ctx, b, thr, max_it, prob):
-    g = PR.ransac_absolute_pose(ctx, **b, threshold=thr, max_iterations=max_it, probability=prob, per_sample=True)
-    r = orr.ransac_absolute_pose(**b, threshold=thr, max_iterations=max_it, probability=prob, per_sample=True)
-    for k in r:
-        assert np.array_equal(g[k], r[k]), k
-    return g
-
-
 @pytest.mark.gpu
 def test_gpu_equals_oracle_bitwise(ctx):
     b, _ = _batch(7, [0, 3, 4, 57, 1000, 2000], 350)
     for thr, max_it, prob in ((25.0, 300, 0.99), (25.0, 300, 0.999999), (0.5, 300, 0.99), (25.0, 3, 0.99)):
-        g = _gpu_vs_oracle(ctx, b, thr, max_it, prob)
-        _check_selection(b, g, max_it, prob)
+        g = _gpu_vs_oracle(ctx, PR.ransac_absolute_pose, orr.ransac_absolute_pose, b, thr, max_it, prob)
+        _check_selection(b, g, S, max_it, prob)
     assert g["sample_valid"][3:].sum() > 500 and (g["sample_valid"][3:] == 0).sum() > 60
     # the selected model through the existing scoring kernel: same count and mask (shared per-correspondence score)
     ptr = b["prob_ptr"]
@@ -233,7 +190,7 @@ def test_gpu_noise_free_scene_gives_ground_truth(ctx):
     b = dict(prob_ptr=np.concatenate([[0], np.cumsum(sizes)]).astype(np.int32), pts=np.concatenate([p["pts"] for p in probs]),
              bearings=np.concatenate([p["f"] for p in probs]), sigma=np.concatenate([p["sigma"] for p in probs]),
              cam_off=np.stack([p["c"] for p in probs]), cam_rot=np.stack([p["Rc"] for p in probs]), samples=samples)
-    g = _gpu_vs_oracle(ctx, b, 1.0, 300, 0.99)
+    g = _gpu_vs_oracle(ctx, PR.ransac_absolute_pose, orr.ransac_absolute_pose, b, 1.0, 300, 0.99)
     ptr = b["prob_ptr"]
     for i, p in enumerate(probs):
         assert g["best_sample"][i] >= 0 and g["iterations"][i] < 60
@@ -248,21 +205,23 @@ def test_gpu_bad_arguments_are_refused(ctx):
     b, _ = _batch(5, [0, 57, 100], 20)
     keep = []
 
-    def call(n_prob=3, ns=20, max_it=300, **over):
+    def call(n_prob=3, ns=20, max_it=300, per_sample=(False, False, False), **over):
         a = {k: np.ascontiguousarray(v) for k, v in b.items()}
         a.update(over)
         keep.append(a)
         res = {k: np.zeros(s, dt) for k, s, dt in (("bs", 3, np.int32), ("bm", 36, np.float64), ("bc", 3, np.int32), ("it", 3, np.int32),
-                                                    ("us", 3, np.int32))}
+                                                    ("us", 3, np.int32), ("sm", 3 * 20 * 12, np.float64), ("sv", 60, np.uint8), ("sc", 60, np.int32))}
         keep.append(res)
         ptr = lambda k: a[k].ctypes.data if a[k] is not None else None
         P = PR.CAbsRansacProblems(n_prob, ptr("prob_ptr"), ptr("pts"), ptr("bearings"), ptr("sigma"), ptr("cam_off"), ptr("cam_rot"), ptr("samples"), ns)
-        R = PR.CAbsRansacResult(res["bs"].ctypes.data, res["bm"].ctypes.data, res["bc"].ctypes.data, res["it"].ctypes.data, res["us"].ctypes.data,
-                                None, None, None, None)
+        opt = [res[k].ctypes.data if on else None for k, on in zip(("sm", "sv", "sc"), per_sample)]
+        R = PR.CRansacResult(res["bs"].ctypes.data, res["bm"].ctypes.data, res["bc"].ctypes.data, res["it"].ctypes.data, res["us"].ctypes.data,
+                             None, *opt)
         return lib().cvb_ransac_absolute_pose_batch(ctx.handle, C.byref(P), 25.0, max_it, 0.99, C.byref(R))
 
-    assert call() == 0
+    assert call() == 0 and call(per_sample=(True, True, True)) == 0
     assert call(n_prob=0) == 0
+    assert call(per_sample=(True, False, True)) == 1 and call(per_sample=(False, False, True)) == 1
     bad = b["samples"].copy(); bad[1, 7, 2] = 57
     assert call(samples=bad) == 1
     bad = b["samples"].copy(); bad[2, 0, 0] = -1
@@ -274,24 +233,16 @@ def test_gpu_bad_arguments_are_refused(ctx):
 
 
 # ------------------------------------------------------------------------------------------------- C++ wrapper
-def _build_shim(out):
-    import covins_b200
-    if not os.path.exists(covins_b200.LIB_PATH):
-        covins_b200.build()
-    subprocess.check_call(["g++", "-O2", "-std=c++17", "-Wall", "-Werror", "-o", out, os.path.join(ROOT, "tests", "cpp", "shim_ransac_test.cpp"),
-                           "-L" + os.path.join(ROOT, "covins_b200"), "-lcovins_b200", "-Wl,-rpath," + os.path.join(ROOT, "covins_b200")])
-
-
 def test_shim_ransac_compiles_and_links(tmp_path):
     exe = str(tmp_path / "shim_ransac_test")
-    _build_shim(exe)
+    _build_shim("shim_ransac_test.cpp", exe)
     assert os.path.exists(exe)
 
 
 @pytest.mark.gpu
 def test_shim_ransac_equals_python_path(ctx, tmp_path):
     exe = str(tmp_path / "shim_ransac_test")
-    _build_shim(exe)
+    _build_shim("shim_ransac_test.cpp", exe)
     b, _ = _batch(9, [57, 0, 1000, 4], 320)
     for k, v in b.items():
         np.ascontiguousarray(v).tofile(tmp_path / f"{k}.bin")

@@ -14,17 +14,9 @@ import pytest
 from covins_b200 import placerec as PR
 from oracle import geom as og
 from oracle import ransac_rel as orel
+from ransac_helpers import _build_shim, _check_selection, _gpu_vs_oracle, _rand_rot
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 S = 17
-
-
-def _rand_rot(rng):
-    q = rng.normal(size=4); q /= np.linalg.norm(q)
-    w, x, y, z = q
-    return np.array([[1 - 2 * (y * y + z * z), 2 * (x * y - z * w), 2 * (x * z + y * w)],
-                     [2 * (x * y + z * w), 1 - 2 * (x * x + z * z), 2 * (y * z - x * w)],
-                     [2 * (x * z - y * w), 2 * (y * z + x * w), 1 - 2 * (x * x + y * y)]])
 
 
 def _rig(rng, ncam, central=False):
@@ -181,40 +173,12 @@ def test_identity_rig_score_equals_central_scoring_oracle():
 
 
 # ------------------------------------------------------------------------------------------------- selection (CPU)
-def _expected_selection(valid, count, n, max_iterations, probability):
-    """placerec.ransac_select over the valid samples in order (at most 10 * max_iterations invalid ones are skipped)"""
-    idx, skipped, stop = [], 0, len(valid)
-    for s in range(len(valid)):
-        if skipped >= 10 * max_iterations:
-            stop = s
-            break
-        if valid[s]:
-            idx.append(s)
-        else:
-            skipped += 1
-    best, it = PR.ransac_select(np.asarray(count)[idx], n, S, max_iterations, probability)
-    consumed = (idx[it - 1] + 1 if it > 0 else 0) if it < len(idx) else stop
-    return (idx[best] if best >= 0 else -1), it, consumed
-
-
-def _check_selection(b, r, max_iterations, probability):
-    ptr = b["prob_ptr"]
-    for i in range(len(ptr) - 1):
-        n = ptr[i + 1] - ptr[i]
-        best, it, consumed = _expected_selection(r["sample_valid"][i], r["sample_count"][i], n, max_iterations, probability)
-        assert (r["best_sample"][i], r["iterations"][i], r["consumed"][i]) == (best, it, consumed), i
-        if best >= 0:
-            assert r["best_count"][i] == r["sample_count"][i][best] and np.array_equal(r["best_model"][i], r["sample_model"][i][best])
-        else:
-            assert r["best_count"][i] == 0 and not r["best_model"][i].any() and not r["inlier_mask"][ptr[i]:ptr[i + 1]].any()
-
-
 def test_oracle_selection_equals_ransac_select():
     specs = [(0, 1, 1, False), (16, 2, 3, False), (17, 3, 3, False), (120, 3, 3, False), (120, 3, 2, True), (200, 4, 3, False)]
     b, _ = _batch(4, specs, 200, outlier_frac=0.05)
     for thr, max_it, prob in ((9.0, 150, 0.99), (9.0, 150, 0.999999), (9.0, 5, 0.99), (1e-3, 40, 0.99)):
         r = orel.ransac_noncentral_relative_pose(**b, threshold=thr, max_iterations=max_it, probability=prob, per_sample=True)
-        _check_selection(b, r, max_it, prob)
+        _check_selection(b, r, S, max_it, prob)
         lazy = orel.ransac_noncentral_relative_pose(**b, threshold=thr, max_iterations=max_it, probability=prob)
         for k in lazy:
             assert np.array_equal(lazy[k], r[k]), k
@@ -225,7 +189,7 @@ def test_oracle_selection_equals_ransac_select():
     b2 = {k: (v.copy() if isinstance(v, np.ndarray) else v) for k, v in b.items()}
     b2["samples"][:, :60, 16] = b2["samples"][:, :60, 0]
     r = orel.ransac_noncentral_relative_pose(**b2, threshold=9.0, max_iterations=2, per_sample=True)
-    _check_selection(b2, r, 2, 0.99)
+    _check_selection(b2, r, S, 2, 0.99)
     assert r["consumed"][3] == 20 and r["iterations"][3] == 0 and r["best_sample"][3] == -1
 
 
@@ -234,20 +198,12 @@ GPU_SPECS = [(0, 1, 1, False), (16, 2, 2, False), (17, 3, 3, False), (18, 1, 4, 
              (2000, 3, 3, False), (300, 2, 4, False)]
 
 
-def _gpu_vs_oracle(ctx, b, thr, max_it, prob):
-    g = PR.ransac_noncentral_relative_pose(ctx, **b, threshold=thr, max_iterations=max_it, probability=prob, per_sample=True)
-    r = orel.ransac_noncentral_relative_pose(**b, threshold=thr, max_iterations=max_it, probability=prob, per_sample=True)
-    for k in r:
-        assert np.array_equal(g[k], r[k]), k
-    return g
-
-
 @pytest.mark.gpu
 def test_gpu_equals_oracle_bitwise(ctx):
     b, _ = _batch(7, GPU_SPECS, 150)
     for thr, max_it, prob in ((9.0, 100, 0.99), (9.0, 100, 0.999999), (0.5, 100, 0.99), (9.0, 3, 0.99)):
-        g = _gpu_vs_oracle(ctx, b, thr, max_it, prob)
-        _check_selection(b, g, max_it, prob)
+        g = _gpu_vs_oracle(ctx, PR.ransac_noncentral_relative_pose, orel.ransac_noncentral_relative_pose, b, thr, max_it, prob)
+        _check_selection(b, g, S, max_it, prob)
     assert g["sample_valid"].sum() > 500 and (g["sample_valid"][2:] == 0).sum() > 100
     assert not g["sample_valid"][4].any()                                          # the central-rig problem
     # the selected model through the existing scoring kernel, one camera pair at a time: same count and mask
@@ -283,7 +239,7 @@ def test_gpu_equals_oracle_bitwise(ctx):
 @pytest.mark.gpu
 def test_gpu_noise_free_scene_gives_ground_truth(ctx):
     b, probs = _batch(11, [(1000, 3, 3, False), (300, 2, 3, False), (1000, 4, 4, False)], 300, outlier_frac=0.1, repeat_frac=0.0)
-    g = _gpu_vs_oracle(ctx, b, 1.0, 300, 0.99)
+    g = _gpu_vs_oracle(ctx, PR.ransac_noncentral_relative_pose, orel.ransac_noncentral_relative_pose, b, 1.0, 300, 0.99)
     ptr = b["prob_ptr"]
     for i, p in enumerate(probs):
         assert g["best_sample"][i] >= 0 and g["iterations"][i] < 100
@@ -309,8 +265,8 @@ def test_gpu_bad_arguments_are_refused(ctx):
         P = PR.CRelRansacProblems(n_prob, *[ptr(k) for k in ("prob_ptr", "f1", "f2", "sigma1", "sigma2", "cam1", "cam2", "cam_ptr1", "cam_off1",
                                                              "cam_rot1", "cam_ptr2", "cam_off2", "cam_rot2", "samples")], ns)
         opt = [res[k].ctypes.data if on else None for k, on in zip(("sm", "sv", "sc"), per_sample)]
-        R = PR.CRelRansacResult(res["bs"].ctypes.data, res["bm"].ctypes.data, res["bc"].ctypes.data, res["it"].ctypes.data, res["us"].ctypes.data,
-                                None, *opt)
+        R = PR.CRansacResult(res["bs"].ctypes.data, res["bm"].ctypes.data, res["bc"].ctypes.data, res["it"].ctypes.data, res["us"].ctypes.data,
+                             None, *opt)
         return lib().cvb_ransac_noncentral_relative_pose_batch(ctx.handle, C.byref(P), 9.0, max_it, 0.99, C.byref(R))
 
     assert call() == 0 and call(per_sample=(True, True, True)) == 0
@@ -336,24 +292,16 @@ def test_gpu_bad_arguments_are_refused(ctx):
 
 
 # ------------------------------------------------------------------------------------------------- C++ wrapper
-def _build_shim(out):
-    import covins_b200
-    if not os.path.exists(covins_b200.LIB_PATH):
-        covins_b200.build()
-    subprocess.check_call(["g++", "-O2", "-std=c++17", "-Wall", "-Werror", "-o", out, os.path.join(ROOT, "tests", "cpp", "shim_ransac_rel_test.cpp"),
-                           "-L" + os.path.join(ROOT, "covins_b200"), "-lcovins_b200", "-Wl,-rpath," + os.path.join(ROOT, "covins_b200")])
-
-
 def test_shim_ransac_rel_compiles_and_links(tmp_path):
     exe = str(tmp_path / "shim_ransac_rel_test")
-    _build_shim(exe)
+    _build_shim("shim_ransac_rel_test.cpp", exe)
     assert os.path.exists(exe)
 
 
 @pytest.mark.gpu
 def test_shim_ransac_rel_equals_python_path(ctx, tmp_path):
     exe = str(tmp_path / "shim_ransac_rel_test")
-    _build_shim(exe)
+    _build_shim("shim_ransac_rel_test.cpp", exe)
     b, _ = _batch(9, [(300, 3, 3, False), (0, 1, 1, False), (1000, 2, 4, False), (17, 1, 2, False)], 120, outlier_frac=0.1)
     for k, v in b.items():
         np.ascontiguousarray(v).tofile(tmp_path / f"{k}.bin")

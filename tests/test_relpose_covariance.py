@@ -15,9 +15,9 @@ from scipy.spatial.transform import Rotation
 
 from covins_b200 import placerec as PR
 from oracle import relpose_cov as ocov
-from test_ransac_relative import _problem, _rand_rot
+from ransac_helpers import _build_shim, _rand_rot
+from test_ransac_relative import _problem
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 S = 17
 
 
@@ -292,24 +292,16 @@ def test_gpu_bad_arguments_are_refused(ctx):
 
 
 # ------------------------------------------------------------------------------------------------- C++ wrapper
-def _build_shim(out):
-    import covins_b200
-    if not os.path.exists(covins_b200.LIB_PATH):
-        covins_b200.build()
-    subprocess.check_call(["g++", "-O2", "-std=c++17", "-Wall", "-Werror", "-o", out, os.path.join(ROOT, "tests", "cpp", "shim_relpose_cov_test.cpp"),
-                           "-L" + os.path.join(ROOT, "covins_b200"), "-lcovins_b200", "-Wl,-rpath," + os.path.join(ROOT, "covins_b200")])
-
-
 def test_shim_relpose_cov_compiles_and_links(tmp_path):
     exe = str(tmp_path / "shim_relpose_cov_test")
-    _build_shim(exe)
+    _build_shim("shim_relpose_cov_test.cpp", exe)
     assert os.path.exists(exe)
 
 
 @pytest.mark.gpu
 def test_shim_relpose_cov_equals_python_path_and_feeds_pgo(ctx, tmp_path):
     exe = str(tmp_path / "shim_relpose_cov_test")
-    _build_shim(exe)
+    _build_shim("shim_relpose_cov_test.cpp", exe)
     rng = np.random.default_rng(25)
     b, probs = _batch(26, [(800, 3, 3, False), (0, 1, 1, False), (600, 2, 4, False), (500, 3, 2, False)], 200, noise=1e-3, outlier_frac=0.2)
     ptr = b["prob_ptr"]
