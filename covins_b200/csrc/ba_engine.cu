@@ -1266,7 +1266,7 @@ int engine_setup(Engine& E, const cvb_ba_problem* p, const cvb_ba_options* o) {
   // (a tile shared by two chains would carry the first chain's pose clique along the whole second chain).
   E.h_off_pose.resize(K); E.h_off_sb.assign(K, 0);
   int n_sb_pad = 0, n_total = 0;
-  std::vector<std::pair<int, int>> sb_ranges;   // [begin, end) column range of every chain (for the column groups)
+  std::vector<int> group_of_tile;   // column group of every tile cvb_chol::nd_layout() laid out (tiles 0, 1, ...)
   if (!E.visual_only) {
     std::vector<int> parent(K);
     std::iota(parent.begin(), parent.end(), 0);
@@ -1277,18 +1277,16 @@ int engine_setup(Engine& E, const cvb_ba_problem* p, const cvb_ba_options* o) {
     }
     std::vector<int> comp_size(K, 0);
     for (int k = 0; k < K; k++) comp_size[find(k)]++;
-    int cursor = 0;
     std::vector<int> roots;
+    std::vector<std::vector<int>> members;
     for (int root = 0; root < K; root++) {          // chains with >= 2 keyframes, in order of their first keyframe
       if (find(root) != root || comp_size[root] < 2) continue;
       roots.push_back(root);
-      cursor = ((cursor + TT - 1) / TT) * TT;
-      const int begin = cursor;
+      members.emplace_back();
       for (int k = root; k < K; k++)
-        if (find(k) == root) { E.h_off_sb[k] = cursor; cursor += 9; }
-      sb_ranges.emplace_back(begin, cursor);
+        if (find(k) == root) members.back().push_back(k);
     }
-    cursor = ((cursor + TT - 1) / TT) * TT;
+    int cursor = cvb_chol::nd_layout(members, 9, E.h_off_sb, group_of_tile) * TT;
     for (int k = 0; k < K; k++)                     // keyframes without an IMU factor: isolated speed-bias blocks
       if (comp_size[find(k)] < 2) { E.h_off_sb[k] = cursor; cursor += 9; }
     n_sb_pad = ((cursor + TT - 1) / TT) * TT;
@@ -1328,15 +1326,14 @@ int engine_setup(Engine& E, const cvb_ba_problem* p, const cvb_ba_options* o) {
     std::vector<int> roots;
     for (int r = 0; r < K; r++)
       if (find(r) == r && comp_size[r] >= 64) roots.push_back(r);
-    int cursor = 0;
-    for (int r : roots) {                                             // interiors of the big chains: one column group each
-      cursor = ((cursor + TT - 1) / TT) * TT;
-      const int begin = cursor;
+    std::vector<std::vector<int>> members;                            // interiors of the big chains: one column group each
+    for (int r : roots) {
+      members.emplace_back();
       for (int k = r; k < K; k++)
-        if (find(k) == r && !border[k]) { E.h_off_pose[k] = cursor; cursor += 6; }
-      if (cursor > begin) sb_ranges.emplace_back(begin, cursor);
+        if (find(k) == r && !border[k]) members.back().push_back(k);
+      if (members.back().empty()) members.pop_back();
     }
-    cursor = ((cursor + TT - 1) / TT) * TT;
+    int cursor = cvb_chol::nd_layout(members, 6, E.h_off_pose, group_of_tile) * TT;
     for (int k = 0; k < K; k++)                                       // small components: main sequence
       if (comp_size[find(k)] < 64) { E.h_off_pose[k] = cursor; cursor += 6; }
     for (int r : roots) {                                             // per-chain border segments
@@ -1394,8 +1391,7 @@ int engine_setup(Engine& E, const cvb_ba_problem* p, const cvb_ba_options* o) {
   }
   // column groups (IMU chains) first: the owner map of a distributed factorisation follows them
   std::vector<int> col_group(nt, -1);
-  for (size_t g = 0; g < sb_ranges.size(); g++)
-    for (int t = sb_ranges[g].first / TT; t <= (sb_ranges[g].second - 1) / TT; t++) col_group[t] = (int)g;
+  std::copy(group_of_tile.begin(), group_of_tile.end(), col_group.begin());
   // ownership of the tile columns (world > 1): an IMU chain's speed-bias columns — a pure latency chain — stay on one
   // rank, the remaining (pose) columns go round the ranks in blocks of COVINS_B200_DIST_BLOCK columns (default 6: every
   // change of owner puts a flag + a 128 KB NVLink copy on the critical chain; tools/mgpu_block_sweep.py)

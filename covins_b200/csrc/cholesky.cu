@@ -23,6 +23,7 @@
 #include <stdlib.h>
 
 #include <algorithm>
+#include <map>
 
 namespace cvb_chol {
 
@@ -122,12 +123,11 @@ constexpr size_t kSyrkSmem = (size_t)GEMM_STAGES * (64 + 64) * LDS * sizeof(doub
 // A(i,k) <- A(i,k) * Linv_k^T for the structurally non-zero row tiles i of tile column k (rows[]).  Two CTAs per tile,
 // each owns 64 full rows (it has consumed all of them as the A operand before it overwrites them).
 // `panel` = first row tile of the column (the column's row tiles are contiguous in the packed array).
-__global__ void __launch_bounds__(TRSM_THREADS, 2) trsm_kernel(double* __restrict__ panel,
-                                                                const double* __restrict__ linv_k) {
+__device__ __forceinline__ void trsm_tile(double* __restrict__ tile, const double* __restrict__ linv_k) {
   extern __shared__ __align__(16) double smem_d[];
   constexpr size_t ld = T;
   const int half = blockIdx.x & 1;
-  double* At = panel + (size_t)(blockIdx.x >> 1) * TT + (size_t)half * 64 * T;
+  double* At = tile + (size_t)half * 64 * T;
   double acc[2][4][4];
   gemm_abt_64<128>(At, ld, linv_k, T, acc, smem_d);
   __syncthreads();   // every warp is done reading this CTA's rows (they were all staged through shared memory)
@@ -141,6 +141,18 @@ __global__ void __launch_bounds__(TRSM_THREADS, 2) trsm_kernel(double* __restric
         const int r = wm * 32 + a * 16 + h * 8 + (lane >> 2), c = wn * 32 + b * 8 + (lane & 3) * 2;
         *reinterpret_cast<double2*>(At + (size_t)r * ld + c) = make_double2(acc[a][b][2 * h], acc[a][b][2 * h + 1]);
       }
+}
+__global__ void __launch_bounds__(TRSM_THREADS, 2) trsm_kernel(double* __restrict__ panel,
+                                                                const double* __restrict__ linv_k) {
+  trsm_tile(panel + (size_t)(blockIdx.x >> 1) * TT, linv_k);
+}
+// The same for the panel tiles of a level (TilePlan::h_lvl_trsm_*): two CTAs per packed tile tiles[t], each tile with the
+// inverse of its own column cols[t].
+__global__ void __launch_bounds__(TRSM_THREADS, 2) trsm_level_kernel(double* __restrict__ S, const double* __restrict__ linv,
+                                                                      const int* __restrict__ tiles,
+                                                                      const int* __restrict__ cols) {
+  const int t = blockIdx.x >> 1;
+  trsm_tile(S + (size_t)tiles[t] * TT, linv + (size_t)cols[t] * TT);
 }
 
 // The two small products of the critical chain (see factor(): "chain column"), one 128x128 tile each:
@@ -247,10 +259,9 @@ constexpr int TILE_STAGES = 3;
 constexpr int TILE_STAGE = 2 * T * KC;   // doubles per ring stage: 128 rows of A(i,k), then 128 rows of A(j,k)
 constexpr size_t kTileSmem = (TT + (size_t)TILE_STAGES * TILE_STAGE) * sizeof(double);   // 229376 B → 1 CTA / SM
 
-__global__ void __launch_bounds__(TILE_THREADS, 1) tile_update_kernel(double* __restrict__ S, const int* __restrict__ tile_of,
-                                                                      int nt, int k0, const int* __restrict__ pi,
-                                                                      const int* __restrict__ pj,
-                                                                      const int* __restrict__ pmask) {
+__device__ __forceinline__ void tile_update(double* __restrict__ S, const int* __restrict__ tile_of, int nt, int k0,
+                                            const int* __restrict__ pi, const int* __restrict__ pj,
+                                            const int* __restrict__ pmask) {
   extern __shared__ __align__(128) double smem_d[];
   __shared__ const double* s_ai[32];   // operand tiles A(i,k), A(j,k) of the pair's panels, in increasing k
   __shared__ const double* s_aj[32];
@@ -358,6 +369,21 @@ __global__ void __launch_bounds__(TILE_THREADS, 1) tile_update_kernel(double* __
           *reinterpret_cast<const double2*>(Cs + r * T + ((s ^ ((r & 1) << 2)) << 1));
   }
 }
+__global__ void __launch_bounds__(TILE_THREADS, 1) tile_update_kernel(double* __restrict__ S, const int* __restrict__ tile_of,
+                                                                      int nt, int k0, const int* __restrict__ pi,
+                                                                      const int* __restrict__ pj,
+                                                                      const int* __restrict__ pmask) {
+  tile_update(S, tile_of, nt, k0, pi, pj, pmask);
+}
+// The same for a level's merged update list (TilePlan::h_lvl_pair_*): each pair with its own first panel pk0[].
+__global__ void __launch_bounds__(TILE_THREADS, 1) tile_update_level_kernel(double* __restrict__ S,
+                                                                            const int* __restrict__ tile_of, int nt,
+                                                                            const int* __restrict__ pk0,
+                                                                            const int* __restrict__ pi,
+                                                                            const int* __restrict__ pj,
+                                                                            const int* __restrict__ pmask) {
+  tile_update(S, tile_of, nt, pk0[blockIdx.x], pi, pj, pmask);
+}
 
 // Factor the diagonal tile k in shared memory and invert the factor, one CTA of 512 threads.  This kernel is the serial
 // chain of the whole factorisation (one launch per tile column, nothing else can run before its panel is solved), so it
@@ -422,9 +448,8 @@ __device__ __forceinline__ int frag_off(int h, int e, int ld) {
     if (prof != nullptr && tid == 0) prof[i] = clock64(); \
   } while (0)
 
-__global__ void __launch_bounds__(POTRF_THREADS, 1) potrf_inv_kernel(double* __restrict__ S, size_t ld, int k,
-                                                                     double* __restrict__ linv_k, int* __restrict__ flag,
-                                                                     long long* __restrict__ prof, int prof_fine) {
+__device__ __forceinline__ void potrf_inv(double* __restrict__ S, size_t ld, int k, double* __restrict__ linv_k,
+                                          int* __restrict__ flag, long long* __restrict__ prof, int prof_fine) {
   extern __shared__ __align__(16) double smem_d[];
   double* a = smem_d;                          // [T][LDP]: L on and below the diagonal, X^T above it
   double* binv = a + T * LDP;                  // [NB][PB][BLD]: X[j,j] = L[j,j]^-1
@@ -642,6 +667,18 @@ __global__ void __launch_bounds__(POTRF_THREADS, 1) potrf_inv_kernel(double* __r
     if (prof_fine && tid == 0) { prof[6] = acc_a; prof[7] = acc_1; prof[8] = acc_2; prof[9] = clock64() - t_a; }
   }
 }
+__global__ void __launch_bounds__(POTRF_THREADS, 1) potrf_inv_kernel(double* __restrict__ S, size_t ld, int k,
+                                                                     double* __restrict__ linv_k, int* __restrict__ flag,
+                                                                     long long* __restrict__ prof, int prof_fine) {
+  potrf_inv(S, ld, k, linv_k, flag, prof, prof_fine);
+}
+// The diagonal tiles of the columns c0 .. c0 + gridDim.x - 1 of a level (packed storage), one CTA each.
+__global__ void __launch_bounds__(POTRF_THREADS, 1) potrf_inv_level_kernel(double* __restrict__ S,
+                                                                           const int* __restrict__ tile_of, int nt, int c0,
+                                                                           double* __restrict__ linv, int* __restrict__ flag) {
+  const int k = c0 + blockIdx.x;
+  potrf_inv(S + (size_t)tile_of[(size_t)k * nt + k] * TT, (size_t)T, 0, linv + (size_t)k * TT, flag, nullptr, 0);
+}
 
 // Triangular solves.  One launch per tile column; every CTA recomputes the tiny diagonal product (128x128 mat-vec with
 // the stored tile inverse) and then updates its own off-diagonal tile.  512 threads, all loads of a mat-vec are issued
@@ -719,6 +756,51 @@ __global__ void __launch_bounds__(SOLVE_THREADS) bwd_kernel(const double* __rest
   const int i = cols[blockIdx.x - 1];
   matvec_cols(L + (size_t)tile_of[(size_t)k * nt + i] * TT, ld, xk, upd, part);
   if (tid < T) y[(size_t)i * T + tid] -= upd[tid];
+}
+
+// Level steps of the solve (TilePlan::h_lvl_ptr: columns c0 .. c0 + nc - 1, none of which touches another's rows of b / y).
+// diag_level_kernel: CTA c forms y_k = Linv_k b_k (FWD) or x_k = Linv_k^T y_k (backward) for k = c0 + c.
+template <bool FWD>
+__global__ void __launch_bounds__(SOLVE_THREADS) diag_level_kernel(const double* __restrict__ linv, int c0,
+                                                                   const double* __restrict__ in, double* __restrict__ out) {
+  __shared__ double vk[T], rk[T], part[4 * T];
+  const int tid = threadIdx.x, k = c0 + blockIdx.x;
+  if (tid < T) vk[tid] = in[(size_t)k * T + tid];
+  __syncthreads();
+  if (FWD) {
+    matvec_rows(linv + (size_t)k * TT, T, vk, rk);
+    __syncthreads();
+  } else {
+    matvec_cols(linv + (size_t)k * TT, T, vk, rk, part);
+  }
+  if (tid < T) out[(size_t)k * T + tid] = rk[tid];
+}
+// gather_level_kernel: CTA per target tile i (targets[]) subtracts the level's products from its rows, one product at a
+// time in the order of the column-by-column solve: forward b_i -= L(i,k) y_k in increasing k, backward
+// y_i -= L(k,i)^T x_k in decreasing k.  v = y (forward) or x (backward) of the level's columns, r = b or y.
+template <bool FWD>
+__global__ void __launch_bounds__(SOLVE_THREADS) gather_level_kernel(const double* __restrict__ L, const int* __restrict__ tile_of,
+                                                                     int nt, int c0, int nc, const double* __restrict__ v,
+                                                                     double* __restrict__ r, const int* __restrict__ targets) {
+  __shared__ double vk[T], upd[T], part[4 * T];
+  const int tid = threadIdx.x, i = targets[blockIdx.x];
+  double ri = tid < T ? r[(size_t)i * T + tid] : 0.0;
+  for (int s = 0; s < nc; s++) {
+    const int k = FWD ? c0 + s : c0 + nc - 1 - s;
+    const int t = FWD ? tile_of[(size_t)i * nt + k] : tile_of[(size_t)k * nt + i];
+    if (t < 0) continue;
+    __syncthreads();   // the previous product is done with vk / upd
+    if (tid < T) vk[tid] = v[(size_t)k * T + tid];
+    __syncthreads();
+    if (FWD) {
+      matvec_rows(L + (size_t)t * TT, T, vk, upd);
+      __syncthreads();
+    } else {
+      matvec_cols(L + (size_t)t * TT, T, vk, upd, part);
+    }
+    if (tid < T) ri -= upd[tid];
+  }
+  if (tid < T) r[(size_t)i * T + tid] = ri;
 }
 
 // Symbolic phase (host): tile-level structure of L from the tile-level structure of S (lower, nt x nt, row-major
@@ -816,6 +898,90 @@ void TilePlan::build(int nt_, std::vector<uint8_t> mask, std::vector<int> col_gr
   }
   // flops this rank executes: one 128^3 GEMM (2 flop per MAC) per trsm tile and per (target tile, panel) update
   flops = 2.0 * T * T * T * (n_trsm + n_upd);
+  // Levels: a group column joins the run of the previous column when that is a group column too, no column of the run has
+  // row tile k, and every row tile i of k first appeared in the run less than 32 columns before k (a target (i, j) then
+  // receives panels from at most 32 consecutive columns).
+  h_lvl_ptr.assign(1, 0);
+  {
+    std::vector<int> first(nt, -1);   // per row tile: first column of the current run that has it
+    int c0 = 0;
+    for (int k = 0; k < nt; k++) {
+      bool join = k > c0 && in_group(k) && in_group(c0);
+      for (int c = c0; join && c < k; c++) join = !tile(k, c);
+      for (int q = h_col_ptr[k]; join && q < h_col_ptr[k + 1]; q++)
+        join = first[h_row_idx[q]] < 0 || k - first[h_row_idx[q]] < 32;
+      if (!join && k > 0) {
+        h_lvl_ptr.push_back(k);
+        for (int c = c0; c < k; c++)
+          for (int q = h_col_ptr[c]; q < h_col_ptr[c + 1]; q++) first[h_row_idx[q]] = -1;
+        c0 = k;
+      }
+      for (int q = h_col_ptr[k]; q < h_col_ptr[k + 1]; q++)
+        if (first[h_row_idx[q]] < 0) first[h_row_idx[q]] = k;
+    }
+    if (nt > 0) h_lvl_ptr.push_back(nt);
+  }
+  const int n_lvl = (int)h_lvl_ptr.size() - 1;
+  h_lvl_pair_ptr.assign(1, 0); h_lvl_pair_i.clear(); h_lvl_pair_j.clear(); h_lvl_pair_k0.clear(); h_lvl_pair_mask.clear();
+  h_lvl_trsm_ptr.assign(1, 0); h_lvl_trsm_tile.clear(); h_lvl_trsm_col.clear();
+  h_lvl_fwd_ptr.assign(1, 0); h_lvl_fwd_idx.clear(); h_lvl_bwd_ptr.assign(1, 0); h_lvl_bwd_idx.clear();
+  for (int l = 0; l < n_lvl; l++) {
+    const int c0 = h_lvl_ptr[l], c1 = in_group(c0) ? h_lvl_ptr[l + 1] : c0;   // lists for the group levels only
+    // merged update list: the group columns' width-1 lists (panel k alone), targets in their order (column j, then row i)
+    std::map<std::pair<int, int>, std::pair<int, int>> pairs;   // (j, i) -> (first panel, mask)
+    for (int k = c0; k < c1; k++)
+      for (int p = h_pair_ptr[k]; p < h_pair_ptr[k + 1]; p++) {
+        auto it = pairs.find({h_pair_j[p], h_pair_i[p]});
+        if (it == pairs.end()) pairs[{h_pair_j[p], h_pair_i[p]}] = {k, 1};
+        else it->second.second = (int)((unsigned)it->second.second | 1u << (k - it->second.first));
+      }
+    for (const auto& e : pairs) {
+      h_lvl_pair_j.push_back(e.first.first);
+      h_lvl_pair_i.push_back(e.first.second);
+      h_lvl_pair_k0.push_back(e.second.first);
+      h_lvl_pair_mask.push_back(e.second.second);
+    }
+    h_lvl_pair_ptr.push_back((int)h_lvl_pair_i.size());
+    std::vector<int> fwd, bwd;
+    for (int k = c0; k < c1; k++) {
+      const bool has_next = h_col_ptr[k + 1] > h_col_ptr[k] && h_row_idx[h_col_ptr[k]] == k + 1;
+      for (int q = h_col_ptr[k]; q < h_col_ptr[k + 1]; q++) {
+        fwd.push_back(h_row_idx[q]);
+        if (has_next && q == h_col_ptr[k]) continue;
+        h_lvl_trsm_tile.push_back(h_col_base[k] + 1 + (q - h_col_ptr[k]));
+        h_lvl_trsm_col.push_back(k);
+      }
+      bwd.insert(bwd.end(), h_rowc_idx.begin() + h_rowc_ptr[k], h_rowc_idx.begin() + h_rowc_ptr[k + 1]);
+    }
+    h_lvl_trsm_ptr.push_back((int)h_lvl_trsm_tile.size());
+    for (std::vector<int>* v : {&fwd, &bwd}) {
+      std::sort(v->begin(), v->end());
+      v->erase(std::unique(v->begin(), v->end()), v->end());
+    }
+    h_lvl_fwd_idx.insert(h_lvl_fwd_idx.end(), fwd.begin(), fwd.end());
+    h_lvl_fwd_ptr.push_back((int)h_lvl_fwd_idx.size());
+    h_lvl_bwd_idx.insert(h_lvl_bwd_idx.end(), bwd.begin(), bwd.end());
+    h_lvl_bwd_ptr.push_back((int)h_lvl_bwd_idx.size());
+  }
+}
+
+int nd_layout(const std::vector<std::vector<int>>& members, int bw, std::vector<int>& off, std::vector<int>& group_of_tile) {
+  const int per = T / bw;
+  const auto level = [](int p) { return __builtin_ctz(~(unsigned)p); };
+  int n_level = 0;
+  for (const auto& m : members)
+    for (int p = 0; p * per < (int)m.size(); p++) n_level = std::max(n_level, level(p) + 1);
+  group_of_tile.clear();
+  for (int lv = 0; lv < n_level; lv++)
+    for (size_t g = 0; g < members.size(); g++)
+      for (int p = 0; p * per < (int)members[g].size(); p++) {
+        if (level(p) != lv) continue;
+        const int tile = (int)group_of_tile.size();
+        for (int q = p * per; q < std::min((p + 1) * per, (int)members[g].size()); q++)
+          off[members[g][q]] = tile * T + (q - p * per) * bw;
+        group_of_tile.push_back((int)g);
+      }
+  return (int)group_of_tile.size();
 }
 
 int TilePlan::upload(cvb_ctx* ctx, cudaStream_t st) {
@@ -828,7 +994,11 @@ int TilePlan::upload(cvb_ctx* ctx, cudaStream_t st) {
   };
   int rc;
   if ((rc = up(&d_row_idx, h_row_idx)) || (rc = up(&d_pair_i, h_pair_i)) || (rc = up(&d_pair_j, h_pair_j)) ||
-      (rc = up(&d_pair_mask, h_pair_mask)) || (rc = up(&d_rowc_idx, h_rowc_idx)) || (rc = up(&d_tile_of, h_tile_of)))
+      (rc = up(&d_pair_mask, h_pair_mask)) || (rc = up(&d_rowc_idx, h_rowc_idx)) || (rc = up(&d_tile_of, h_tile_of)) ||
+      (rc = up(&d_lvl_pair_i, h_lvl_pair_i)) || (rc = up(&d_lvl_pair_j, h_lvl_pair_j)) ||
+      (rc = up(&d_lvl_pair_k0, h_lvl_pair_k0)) || (rc = up(&d_lvl_pair_mask, h_lvl_pair_mask)) ||
+      (rc = up(&d_lvl_trsm_tile, h_lvl_trsm_tile)) || (rc = up(&d_lvl_trsm_col, h_lvl_trsm_col)) ||
+      (rc = up(&d_lvl_fwd_idx, h_lvl_fwd_idx)) || (rc = up(&d_lvl_bwd_idx, h_lvl_bwd_idx)))
     return rc;
   CVB_CUDA(ctx, cudaStreamSynchronize(st));
   return CVB_OK;
@@ -842,6 +1012,11 @@ void TilePlan::release() {
   if (d_rowc_idx) cudaFree(d_rowc_idx);
   if (d_tile_of) cudaFree(d_tile_of);
   d_row_idx = d_pair_i = d_pair_j = d_pair_mask = d_rowc_idx = d_tile_of = nullptr;
+  for (int** d : {&d_lvl_pair_i, &d_lvl_pair_j, &d_lvl_pair_k0, &d_lvl_pair_mask, &d_lvl_trsm_tile, &d_lvl_trsm_col,
+                  &d_lvl_fwd_idx, &d_lvl_bwd_idx}) {
+    if (*d) cudaFree(*d);
+    *d = nullptr;
+  }
 }
 
 int FactorStreams::create(cvb_ctx* ctx, int nt) {
@@ -926,6 +1101,9 @@ int factor(cvb_ctx* ctx, double* S, double* linv, int* d_flag, const TilePlan& p
     CVB_CUDA(ctx, cudaFuncSetAttribute(potrf_inv_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kPotrfSmem));
     CVB_CUDA(ctx, cudaFuncSetAttribute(chain_gemm_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kChainSmem));
     CVB_CUDA(ctx, cudaFuncSetAttribute(chain_gemm_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kChainSmem));
+    CVB_CUDA(ctx, cudaFuncSetAttribute(trsm_level_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kTrsmSmem));
+    CVB_CUDA(ctx, cudaFuncSetAttribute(tile_update_level_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kTileSmem));
+    CVB_CUDA(ctx, cudaFuncSetAttribute(potrf_inv_level_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kPotrfSmem));
   }
   const int nt = plan.nt;
   const bool dist = dv != nullptr && dv->world > 1 && !plan.h_owner.empty();
@@ -989,7 +1167,62 @@ int factor(cvb_ctx* ctx, double* S, double* linv, int* d_flag, const TilePlan& p
       }
     return CVB_OK;
   };
+  // Level schedule of the column groups (single GPU and replicated plans; TilePlan::h_lvl_ptr): the columns of a level are
+  // independent, so each level is three batched launches on the main stream — every diagonal tile, every panel tile, the
+  // merged update list — instead of a chain step per column.  Per tile the kernels and the order of the products are those
+  // of the column-by-column schedule, so the results are bit-identical to it.  The one product the column-by-column
+  // schedule leaves to the chain, S(k+1,k+1) -= L(k+1,k) L(k+1,k)^T when the level's last column k has row tile k+1, is
+  // made the chain's way too (chain_gemm_kernel), after the merged list, as is the solve of tile (k+1,k).
+  auto run_level = [&](int l) -> int {
+    const int c0 = plan.h_lvl_ptr[l], nc = plan.h_lvl_ptr[l + 1] - c0, kl = c0 + nc - 1;
+    if (sf_live) {   // the main sequence's chain and bulk streams join the main stream
+      CVB_CUDA(ctx, cudaEventRecord(fs.fork_fast, sf));
+      CVB_CUDA(ctx, cudaStreamWaitEvent(st, fs.fork_fast, 0));
+      sf_live = false;
+    }
+    if (last_bulk >= 0) CVB_CUDA(ctx, cudaStreamWaitEvent(st, ev[5 * last_bulk + 1], 0));
+    last_bulk = prev_chain = -1;
+    auto mark = [&](int e) {   // one event per stage of the level (the trace gives it to each of the level's columns)
+      if (tr) cudaEventRecord(tev[(size_t)c0 * 5 + e], st);
+    };
+    mark(0);
+    potrf_inv_level_kernel<<<nc, POTRF_THREADS, kPotrfSmem, st>>>(S, plan.d_tile_of, nt, c0, linv, d_flag);
+    CVB_CHECK_LAUNCH(ctx);
+    mark(1);
+    double* diag = S + (size_t)plan.h_col_base[kl] * TT;
+    const bool has_next = plan.h_col_ptr[kl + 1] > plan.h_col_ptr[kl] && plan.h_row_idx[plan.h_col_ptr[kl]] == kl + 1;
+    if (has_next) {
+      chain_gemm_kernel<0><<<T / CHAIN_ROWS, T, kChainSmem, st>>>(diag + TT, diag + TT, linv + (size_t)kl * TT);
+      CVB_CHECK_LAUNCH(ctx);
+    }
+    const int t0 = plan.h_lvl_trsm_ptr[l], ntr = plan.h_lvl_trsm_ptr[l + 1] - t0;
+    if (ntr > 0) {
+      trsm_level_kernel<<<2 * ntr, TRSM_THREADS, kTrsmSmem, st>>>(S, linv, plan.d_lvl_trsm_tile + t0, plan.d_lvl_trsm_col + t0);
+      CVB_CHECK_LAUNCH(ctx);
+    }
+    mark(2);
+    const int p0 = plan.h_lvl_pair_ptr[l], np = plan.h_lvl_pair_ptr[l + 1] - p0;
+    if (np > 0) {
+      tile_update_level_kernel<<<np, TILE_THREADS, kTileSmem, st>>>(S, plan.d_tile_of, nt, plan.d_lvl_pair_k0 + p0,
+                                                                    plan.d_lvl_pair_i + p0, plan.d_lvl_pair_j + p0,
+                                                                    plan.d_lvl_pair_mask + p0);
+      CVB_CHECK_LAUNCH(ctx);
+    }
+    if (has_next) {
+      chain_gemm_kernel<1><<<T / CHAIN_ROWS, T, kChainSmem, st>>>(S + (size_t)plan.h_col_base[kl + 1] * TT, diag + TT, diag + TT);
+      CVB_CHECK_LAUNCH(ctx);
+    }
+    mark(3);
+    return CVB_OK;
+  };
+  int lvl = 0;
   for (int k = 0; k < nt; k++) {
+    while (plan.h_lvl_ptr[lvl + 1] <= k) lvl++;
+    if (!dist && plan.level_is_group(lvl)) {
+      if ((rc_join = run_level(lvl))) return rc_join;
+      k = plan.h_lvl_ptr[lvl + 1] - 1;
+      continue;
+    }
     const int grp = n_gs > 0 ? plan.h_col_group[k] : -1;
     cudaStream_t s = st;
     if (grp >= 0) {
@@ -1036,8 +1269,11 @@ int factor(cvb_ctx* ctx, double* S, double* linv, int* d_flag, const TilePlan& p
     // a list that starts with (k+1,k+1) (at a block's last column) holds the block's earlier panels for it: they go on the
     // chain stream, before the chain's own product and potrf(k+1)
     const bool diag_pair = np > 0 && plan.h_pair_i[p0] == k + 1 && plan.h_pair_j[p0] == k + 1;
-    // A. tile (k,k) is final: column k-1's contribution came with the chain, the others were waited for by the previous
-    //    chain step (below) — nothing to wait for here
+    // A. tile (k,k) is final: when the previous chain column is k-1, its contribution came with the chain and the others
+    //    were waited for by its chain step (below).  Otherwise (a column group in nested-dissection order: the group's
+    //    previous column is a lower level and may have row tile k) that column's updates of tile (k,k) ran on the work
+    //    stream as ordinary list pairs, so they are waited for here.
+    if (pc >= 0 && pc != k - 1) CVB_CUDA(ctx, cudaStreamWaitEvent(cs, ev[5 * pc + 4], 0));
     if (mine) {
       potrf_inv_kernel<<<1, POTRF_THREADS, kPotrfSmem, cs>>>(diag, (size_t)T, 0, linv_k, d_flag, nullptr, 0);
       CVB_CHECK_LAUNCH(ctx);
@@ -1145,13 +1381,15 @@ int factor(cvb_ctx* ctx, double* S, double* linv, int* d_flag, const TilePlan& p
       // n_pairs / n_work_pairs: pairs of column k's update list / of its work-stream part; t_bulk_us: end of the bulk
       // update launched at column k (a block's last column), -1 if none
       fprintf(f, "k,group,owner,n_rows,n_pairs,n_work_pairs,t_start_us,t_panel_ready_us,t_trsm_us,t_syrk_a_us,t_bulk_us\n");
-      for (int k = 0; k < nt; k++) {
+      for (int k = 0, l = 0; k < nt; k++) {
+        while (plan.h_lvl_ptr[l + 1] <= k) l++;
+        const int ke = !dist && plan.level_is_group(l) ? plan.h_lvl_ptr[l] : k;   // column whose events time column k
         float t[5];
         for (int e = 0; e < 5; e++) {
           t[e] = -1.f;
-          if (cudaEventQuery(tev[(size_t)k * 5 + e]) == cudaSuccess) {
+          if (cudaEventQuery(tev[(size_t)ke * 5 + e]) == cudaSuccess) {
             float ms = 0.f;
-            if (cudaEventElapsedTime(&ms, tev[(size_t)nt * 5], tev[(size_t)k * 5 + e]) == cudaSuccess) t[e] = ms * 1e3f;
+            if (cudaEventElapsedTime(&ms, tev[(size_t)nt * 5], tev[(size_t)ke * 5 + e]) == cudaSuccess) t[e] = ms * 1e3f;
           }
         }
         fprintf(f, "%d,%d,%d,%d,%d,%d,%.1f,%.1f,%.1f,%.1f,%.1f\n", k, plan.h_col_group.empty() ? -1 : plan.h_col_group[k],
@@ -1168,60 +1406,44 @@ int factor(cvb_ctx* ctx, double* S, double* linv, int* d_flag, const TilePlan& p
 
 // solves L L^T x = b; b is destroyed, tmp is scratch (n_pad), result in x
 int solve(cvb_ctx* ctx, const double* L, const double* linv, double* b, double* tmp, double* x,
-          const TilePlan& plan, cudaStream_t st, const FactorStreams& fs) {
-  const int nt = plan.nt;
-  // The leading tile columns that belong to independent column groups (IMU chains, TilePlan::h_col_group) touch only
-  // their own chain's rows of b / y, so the chains' substitution steps — pure launch-latency chains — run concurrently
-  // on the group streams, forward before and backward after the sequential part.
-  const int n_gs = plan.h_col_group.empty() ? 0 : fs.n_group;
-  int n_grouped = 0;
-  while (n_gs > 0 && n_grouped < nt && plan.h_col_group[n_grouped] >= 0) n_grouped++;
-  for (int k = n_grouped; k < nt; k++)
-    if (n_gs > 0 && plan.h_col_group[k] >= 0) { n_grouped = 0; break; }   // groups must be a prefix; else run sequentially
-  std::vector<char> used(n_gs > 0 ? n_gs : 1, 0);
-  auto fork = [&]() -> int {
-    CVB_CUDA(ctx, cudaEventRecord(fs.fork, st));
-    std::fill(used.begin(), used.end(), 0);
-    return CVB_OK;
-  };
-  auto stream_of = [&](int k, cudaStream_t* s) -> int {
-    const int g = plan.h_col_group[k] % n_gs;
-    if (!used[g]) {
-      CVB_CUDA(ctx, cudaStreamWaitEvent(fs.group[g], fs.fork, 0));
-      used[g] = 1;
-    }
-    *s = fs.group[g];
-    return CVB_OK;
-  };
-  auto join = [&]() -> int {
-    for (int g = 0; g < n_gs; g++)
-      if (used[g]) {
-        CVB_CUDA(ctx, cudaEventRecord(fs.join[g], fs.group[g]));
-        CVB_CUDA(ctx, cudaStreamWaitEvent(st, fs.join[g], 0));
+          const TilePlan& plan, cudaStream_t st, const FactorStreams& /*fs*/) {
+  const int nt = plan.nt, n_lvl = (int)plan.h_lvl_ptr.size() - 1;
+  // One step per level (TilePlan::h_lvl_ptr): a level's columns touch none of each other's rows of b / y, so a level of
+  // several columns is two launches — its diagonal products, then the gather into its target rows — and a single column
+  // is one (fwd_kernel / bwd_kernel).
+  for (int l = 0; l < n_lvl; l++) {
+    const int c0 = plan.h_lvl_ptr[l], nc = plan.h_lvl_ptr[l + 1] - c0;
+    if (nc > 1) {
+      const int t0 = plan.h_lvl_fwd_ptr[l], ntg = plan.h_lvl_fwd_ptr[l + 1] - t0;
+      diag_level_kernel<true><<<nc, SOLVE_THREADS, 0, st>>>(linv, c0, b, tmp);
+      CVB_CHECK_LAUNCH(ctx);
+      if (ntg > 0) {
+        gather_level_kernel<true><<<ntg, SOLVE_THREADS, 0, st>>>(L, plan.d_tile_of, nt, c0, nc, tmp, b, plan.d_lvl_fwd_idx + t0);
+        CVB_CHECK_LAUNCH(ctx);
       }
-    return CVB_OK;
-  };
-  int rc;
-  if (n_grouped > 0 && (rc = fork())) return rc;
-  for (int k = 0; k < nt; k++) {
-    cudaStream_t s = st;
-    if (k < n_grouped && (rc = stream_of(k, &s))) return rc;
-    if (k == n_grouped && n_grouped > 0 && (rc = join())) return rc;
-    const int m = plan.h_col_ptr[k + 1] - plan.h_col_ptr[k];
-    fwd_kernel<<<1 + m, SOLVE_THREADS, 0, s>>>(L + (size_t)(plan.h_col_base[k] + 1) * TT, k, linv, b, tmp,
-                                               plan.d_row_idx + plan.h_col_ptr[k]);
+      continue;
+    }
+    const int m = plan.h_col_ptr[c0 + 1] - plan.h_col_ptr[c0];
+    fwd_kernel<<<1 + m, SOLVE_THREADS, 0, st>>>(L + (size_t)(plan.h_col_base[c0] + 1) * TT, c0, linv, b, tmp,
+                                                plan.d_row_idx + plan.h_col_ptr[c0]);
     CVB_CHECK_LAUNCH(ctx);
   }
-  if (n_grouped == nt && n_grouped > 0 && (rc = join())) return rc;
-  for (int k = nt - 1; k >= 0; k--) {
-    cudaStream_t s = st;
-    if (k == n_grouped - 1 && (rc = fork())) return rc;
-    if (k < n_grouped && (rc = stream_of(k, &s))) return rc;
-    const int m = plan.h_rowc_ptr[k + 1] - plan.h_rowc_ptr[k];
-    bwd_kernel<<<1 + m, SOLVE_THREADS, 0, s>>>(L, plan.d_tile_of, nt, k, linv, tmp, x, plan.d_rowc_idx + plan.h_rowc_ptr[k]);
+  for (int l = n_lvl - 1; l >= 0; l--) {
+    const int c0 = plan.h_lvl_ptr[l], nc = plan.h_lvl_ptr[l + 1] - c0;
+    if (nc > 1) {
+      const int t0 = plan.h_lvl_bwd_ptr[l], ntg = plan.h_lvl_bwd_ptr[l + 1] - t0;
+      diag_level_kernel<false><<<nc, SOLVE_THREADS, 0, st>>>(linv, c0, tmp, x);
+      CVB_CHECK_LAUNCH(ctx);
+      if (ntg > 0) {
+        gather_level_kernel<false><<<ntg, SOLVE_THREADS, 0, st>>>(L, plan.d_tile_of, nt, c0, nc, x, tmp, plan.d_lvl_bwd_idx + t0);
+        CVB_CHECK_LAUNCH(ctx);
+      }
+      continue;
+    }
+    const int m = plan.h_rowc_ptr[c0 + 1] - plan.h_rowc_ptr[c0];
+    bwd_kernel<<<1 + m, SOLVE_THREADS, 0, st>>>(L, plan.d_tile_of, nt, c0, linv, tmp, x, plan.d_rowc_idx + plan.h_rowc_ptr[c0]);
     CVB_CHECK_LAUNCH(ctx);
   }
-  if (n_grouped > 0 && (rc = join())) return rc;
   return CVB_OK;
 }
 

@@ -30,6 +30,21 @@ struct TilePlan {
   std::vector<int> h_rowc_ptr, h_rowc_idx;         // per tile row k: non-zero column tiles i < k (backward solve)
   std::vector<int> h_col_group;                    // optional, per tile column: id (>= 0) of an independent column group
                                                    // (its columns share no tile with other groups), -1 = main sequence
+  // Levels: the tile columns cut into runs [h_lvl_ptr[l], h_lvl_ptr[l + 1]) of mutually independent columns (no column of
+  // a run has a row tile inside the run).  Column-group columns form maximal runs, capped so that the panels a target tile
+  // receives from one run span at most 32 columns; every other column is a run of its own.  The columns of a run are
+  // factored together (factor(), single GPU and replicated plans) and substituted together (solve()).  Per group level
+  // (the lists of every other level are empty):
+  //   merged update list: every (target, panel) product of its columns' width-1 pair lists once, per target pair (i >= j)
+  //     the first panel h_lvl_pair_k0 and bit q of h_lvl_pair_mask = panel k0 + q;
+  //   trsm list: the packed index and column of every panel tile of its columns but the first one of a column whose first
+  //     row tile is the next column (that tile is the chain's, see factor());
+  //   fwd / bwd targets: the row tiles i of its columns (forward solve) / the column tiles i < k of its rows (backward).
+  std::vector<int> h_lvl_ptr;
+  std::vector<int> h_lvl_pair_ptr, h_lvl_pair_i, h_lvl_pair_j, h_lvl_pair_k0, h_lvl_pair_mask;
+  std::vector<int> h_lvl_trsm_ptr, h_lvl_trsm_tile, h_lvl_trsm_col;
+  std::vector<int> h_lvl_fwd_ptr, h_lvl_fwd_idx, h_lvl_bwd_ptr, h_lvl_bwd_idx;
+  bool level_is_group(int l) const { return !h_col_group.empty() && h_col_group[h_lvl_ptr[l]] >= 0; }
   // Packed tile storage: only the tiles of L's structure exist.  Column k's tiles are contiguous — the diagonal tile at
   // h_col_base[k], then its row tiles in h_row_idx order — so a panel is one contiguous block (one peer copy when the
   // factorisation is distributed).  h_tile_of[i * nt + j] = packed index of tile (i >= j) or -1.
@@ -40,6 +55,8 @@ struct TilePlan {
   int my_rank = 0;
   int *d_row_idx = nullptr, *d_pair_i = nullptr, *d_pair_j = nullptr, *d_pair_mask = nullptr, *d_rowc_idx = nullptr,
       *d_tile_of = nullptr;
+  int *d_lvl_pair_i = nullptr, *d_lvl_pair_j = nullptr, *d_lvl_pair_k0 = nullptr, *d_lvl_pair_mask = nullptr,
+      *d_lvl_trsm_tile = nullptr, *d_lvl_trsm_col = nullptr, *d_lvl_fwd_idx = nullptr, *d_lvl_bwd_idx = nullptr;
   long n_tiles_L = 0;
   double flops = 0.0;   // flops of one numeric factorisation with this plan
   // col_group (optional, nt entries): h_col_group.  owner (optional, nt entries) + rank: distributed plan.  flops = the
@@ -50,6 +67,15 @@ struct TilePlan {
   int upload(cvb_ctx* ctx, cudaStream_t st);
   void release();
 };
+
+// Tile layout of the column groups (IMU chains' speed-bias blocks; pose-graph chain interiors), starting at tile 0.
+// members[g] = the blocks of group g in order (block ids, bw columns each).  Whole blocks per tile (128 / bw of them), so
+// that a block stays contiguous when the tiles are permuted.  A group's tile at position p has level = the number of
+// trailing one bits of p (nested dissection of a chain by cyclic reduction: the tiles of one level couple only to tiles
+// of higher levels, so each level is a run of independent tile columns — TilePlan::h_lvl_ptr); the tiles go level by
+// level, and inside a level group by group.  Writes off[block] = its first column and group_of_tile[t] = the group of
+// tile t; returns the number of tiles.
+int nd_layout(const std::vector<std::vector<int>>& members, int bw, std::vector<int>& off, std::vector<int>& group_of_tile);
 
 // Extra streams/events of a factorisation (all events with timing disabled), made by create() for a plan of nt tile
 // columns and released by destroy() or the destructor.
