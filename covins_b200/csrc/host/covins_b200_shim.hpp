@@ -984,16 +984,16 @@ struct AbsolutePoseRansacResult {
 namespace detail {
 // one RANSAC call fn on the flattened problems P (ptr: their correspondence ranges) → the per-problem results (Out:
 // AbsolutePoseRansacResult or NonCentralRelativePoseRansacResult)
-template <class Out, class Problems, class Result>
-std::vector<Out> ransac(Context& ctx, int (*fn)(cvb_ctx*, const Problems*, double, int, double, Result*), const char* what, const Problems& P,
-                        const std::vector<int32_t>& ptr, double threshold, int max_iterations, double probability) {
+// call(&R) runs the RANSAC call into the result struct R
+template <class Out, class Result, class Call>
+std::vector<Out> ransac_results(const std::vector<int32_t>& ptr, const Call& call) {
   const int n_prob = (int)ptr.size() - 1;
   const size_t m = n_prob > 0 ? n_prob : 1;
   std::vector<int32_t> best(m), cnt(m), iters(m), used(m);
   std::vector<double> models(12 * m);
   std::vector<uint8_t> mask(ptr[n_prob] > 0 ? ptr[n_prob] : 1);
   Result R{best.data(), models.data(), cnt.data(), iters.data(), used.data(), mask.data(), nullptr, nullptr, nullptr};
-  ctx.check(fn(ctx.get(), &P, threshold, max_iterations, probability, &R), what);
+  call(&R);
   std::vector<Out> out(n_prob);
   for (int i = 0; i < n_prob; i++) {
     out[i].best_sample = best[i]; out[i].n_inliers = cnt[i]; out[i].iterations = iters[i]; out[i].samples_used = used[i];
@@ -1002,29 +1002,73 @@ std::vector<Out> ransac(Context& ctx, int (*fn)(cvb_ctx*, const Problems*, doubl
   }
   return out;
 }
-}  // namespace detail
-inline std::vector<AbsolutePoseRansacResult> RansacAbsolutePose(Context& ctx, const std::vector<AbsolutePoseRansacProblem>& problems, double threshold,
-                                                                 int max_iterations, double probability = 0.99) {
-  const int n_prob = (int)problems.size();
-  const size_t n_samples = n_prob ? problems[0].samples.size() / 4 : 0;
-  std::vector<int32_t> ptr(n_prob + 1, 0), samples;
+template <class Out, class Problems, class Result>
+std::vector<Out> ransac(Context& ctx, int (*fn)(cvb_ctx*, const Problems*, double, int, double, Result*), const char* what, const Problems& P,
+                        const std::vector<int32_t>& ptr, double threshold, int max_iterations, double probability) {
+  return ransac_results<Out, Result>(ptr, [&](Result* R) { ctx.check(fn(ctx.get(), &P, threshold, max_iterations, probability, R), what); });
+}
+// the seeded form: P.samples = NULL, one seed per problem
+template <class Out, class Problems, class Result>
+std::vector<Out> ransac_seeded(Context& ctx, int (*fn)(cvb_ctx*, const Problems*, const uint64_t*, double, int, double, Result*, int32_t*),
+                               const char* what, const Problems& P, const std::vector<int32_t>& ptr, const std::vector<uint64_t>& seeds,
+                               double threshold, int max_iterations, double probability) {
+  if (seeds.size() != ptr.size() - 1) throw std::invalid_argument(std::string("covins_b200: ") + what + ": one seed per problem");
+  return ransac_results<Out, Result>(
+      ptr, [&](Result* R) { ctx.check(fn(ctx.get(), &P, seeds.data(), threshold, max_iterations, probability, R, nullptr), what); });
+}
+// every problem's samples left empty, as the seeded calls require
+template <class Problem>
+void require_no_samples(const std::vector<Problem>& problems, const char* what) {
+  for (const Problem& p : problems)
+    if (!p.samples.empty()) throw std::invalid_argument(std::string("covins_b200::") + what + ": the seeded form draws the samples; leave them empty");
+}
+// a batch of absolute-pose problems flattened into the arrays of cvb_abs_ransac_problems
+struct FlatAbsProblems {
+  std::vector<int32_t> ptr, samples;
   std::vector<double> pts, f, sigma, cam_off, cam_rot;
+  int32_t n_samples = 0;
+  cvb_abs_ransac_problems view() const {
+    return cvb_abs_ransac_problems{(int32_t)ptr.size() - 1, ptr.data(), pts.data(), f.data(), sigma.data(), cam_off.data(), cam_rot.data(),
+                                   samples.empty() ? nullptr : samples.data(), n_samples};
+  }
+};
+inline FlatAbsProblems flatten_abs_problems(const std::vector<AbsolutePoseRansacProblem>& problems) {
+  const int n_prob = (int)problems.size();
+  FlatAbsProblems F;
+  const size_t n_samples = n_prob ? problems[0].samples.size() / 4 : 0;
+  F.n_samples = (int32_t)n_samples;
+  F.ptr.assign(n_prob + 1, 0);
   for (int i = 0; i < n_prob; i++) {
     const AbsolutePoseRansacProblem& p = problems[i];
     if (p.samples.size() != 4 * n_samples || p.points.size() != 3 * p.sigma_angles.size() || p.bearings.size() != 3 * p.sigma_angles.size())
       throw std::invalid_argument("covins_b200::RansacAbsolutePose: inconsistent problem sizes");
-    ptr[i + 1] = ptr[i] + (int32_t)p.sigma_angles.size();
-    pts.insert(pts.end(), p.points.begin(), p.points.end());
-    f.insert(f.end(), p.bearings.begin(), p.bearings.end());
-    sigma.insert(sigma.end(), p.sigma_angles.begin(), p.sigma_angles.end());
-    cam_off.insert(cam_off.end(), p.cam_offset, p.cam_offset + 3);
-    cam_rot.insert(cam_rot.end(), p.cam_rotation, p.cam_rotation + 9);
-    samples.insert(samples.end(), p.samples.begin(), p.samples.end());
+    F.ptr[i + 1] = F.ptr[i] + (int32_t)p.sigma_angles.size();
+    F.pts.insert(F.pts.end(), p.points.begin(), p.points.end());
+    F.f.insert(F.f.end(), p.bearings.begin(), p.bearings.end());
+    F.sigma.insert(F.sigma.end(), p.sigma_angles.begin(), p.sigma_angles.end());
+    F.cam_off.insert(F.cam_off.end(), p.cam_offset, p.cam_offset + 3);
+    F.cam_rot.insert(F.cam_rot.end(), p.cam_rotation, p.cam_rotation + 9);
+    F.samples.insert(F.samples.end(), p.samples.begin(), p.samples.end());
   }
-  const cvb_abs_ransac_problems P{n_prob, ptr.data(), pts.data(), f.data(), sigma.data(), cam_off.data(), cam_rot.data(), samples.data(),
-                                  (int32_t)n_samples};
-  return detail::ransac<AbsolutePoseRansacResult>(ctx, cvb_ransac_absolute_pose_batch, "cvb_ransac_absolute_pose_batch", P, ptr, threshold,
+  return F;
+}
+}  // namespace detail
+inline std::vector<AbsolutePoseRansacResult> RansacAbsolutePose(Context& ctx, const std::vector<AbsolutePoseRansacProblem>& problems, double threshold,
+                                                                 int max_iterations, double probability = 0.99) {
+  const detail::FlatAbsProblems F = detail::flatten_abs_problems(problems);
+  return detail::ransac<AbsolutePoseRansacResult>(ctx, cvb_ransac_absolute_pose_batch, "cvb_ransac_absolute_pose_batch", F.view(), F.ptr, threshold,
                                                   max_iterations, probability);
+}
+// The same RANSAC with the samples drawn on the GPU (cvb_ransac_absolute_pose_seeded_batch): one seed per problem (e.g. from
+// std::random_device, or fixed for reproducible runs), every problem's samples left empty.  The selection draws until opengv's
+// bound ends it; a problem with fewer than 4 correspondences draws nothing (best_sample = -1, iterations = samples_used = 0).
+inline std::vector<AbsolutePoseRansacResult> RansacAbsolutePose(Context& ctx, const std::vector<AbsolutePoseRansacProblem>& problems,
+                                                                 const std::vector<uint64_t>& seeds, double threshold, int max_iterations,
+                                                                 double probability = 0.99) {
+  detail::require_no_samples(problems, "RansacAbsolutePose");
+  const detail::FlatAbsProblems F = detail::flatten_abs_problems(problems);
+  return detail::ransac_seeded<AbsolutePoseRansacResult>(ctx, cvb_ransac_absolute_pose_seeded_batch, "cvb_ransac_absolute_pose_seeded_batch", F.view(),
+                                                         F.ptr, seeds, threshold, max_iterations, probability);
 }
 
 // The 17-point non-central relative-pose RANSAC of RelNonCentralPosSolver::computeNonCentralRelPose (RelNonCentralPosSolver.cpp:
@@ -1053,7 +1097,8 @@ struct FlatRelProblems {
   int32_t n_samples = 0;
   cvb_rel_ransac_problems view() const {
     return cvb_rel_ransac_problems{(int32_t)ptr.size() - 1, ptr.data(), f1.data(), f2.data(), s1.data(), s2.data(), cam1.data(), cam2.data(),
-                                   cp1.data(), co1.data(), cr1.data(), cp2.data(), co2.data(), cr2.data(), samples.data(), n_samples};
+                                   cp1.data(), co1.data(), cr1.data(), cp2.data(), co2.data(), cr2.data(), samples.empty() ? nullptr : samples.data(),
+                                   n_samples};
   }
 };
 inline FlatRelProblems flatten_rel_problems(const std::vector<NonCentralRelativePoseRansacProblem>& problems, const char* what) {
@@ -1090,6 +1135,18 @@ inline std::vector<NonCentralRelativePoseRansacResult> RansacNonCentralRelativeP
   return detail::ransac<NonCentralRelativePoseRansacResult>(ctx, cvb_ransac_noncentral_relative_pose_batch, "cvb_ransac_noncentral_relative_pose_batch",
                                                             F.view(), F.ptr, threshold, max_iterations, probability);
 }
+// The same RANSAC with the samples drawn on the GPU (cvb_ransac_noncentral_relative_pose_seeded_batch): one seed per problem,
+// every problem's samples left empty (as RansacAbsolutePose's seeded form).
+inline std::vector<NonCentralRelativePoseRansacResult> RansacNonCentralRelativePose(Context& ctx,
+                                                                                   const std::vector<NonCentralRelativePoseRansacProblem>& problems,
+                                                                                   const std::vector<uint64_t>& seeds, double threshold,
+                                                                                   int max_iterations, double probability = 0.99) {
+  detail::require_no_samples(problems, "RansacNonCentralRelativePose");
+  const detail::FlatRelProblems F = detail::flatten_rel_problems(problems, "RansacNonCentralRelativePose");
+  return detail::ransac_seeded<NonCentralRelativePoseRansacResult>(ctx, cvb_ransac_noncentral_relative_pose_seeded_batch,
+                                                                   "cvb_ransac_noncentral_relative_pose_seeded_batch", F.view(), F.ptr, seeds, threshold,
+                                                                   max_iterations, probability);
+}
 
 // The sampling-based 6x6 covariance of RelNonCentralPosSolver::computeNonCentralRelPose (RelNonCentralPosSolver.cpp:199,236,
 // 276-279) for a batch of candidates in one call (cvb_noncentral_relative_pose_covariance_batch), in place of the loop of up to
@@ -1116,6 +1173,41 @@ inline std::vector<RelativePoseCovariance> NonCentralRelativePoseCovariance(Cont
   const cvb_rel_ransac_problems P = F.view();
   cvb_rel_cov_result R{cov.data(), nv.data(), nullptr, nullptr};
   ctx.check(cvb_noncentral_relative_pose_covariance_batch(ctx.get(), &P, ref.data(), &R), "cvb_noncentral_relative_pose_covariance_batch");
+  std::vector<RelativePoseCovariance> out(n_prob);
+  for (int i = 0; i < n_prob; i++) {
+    std::copy(cov.begin() + 36 * i, cov.begin() + 36 * (i + 1), out[i].cov.begin());
+    out[i].n_valid = nv[i];
+  }
+  return out;
+}
+// The same covariance with the samples drawn on the GPU (cvb_noncentral_relative_pose_covariance_seeded_batch): n_samples
+// subsets of 17 (the reference's 300) of ransac_results[i].inliers per candidate, drawn from seeds[i] (the seed of the
+// candidate's RANSAC may be reused: the two draw from separate streams); every problem's samples left empty.  A candidate with
+// fewer than 17 inliers, or without a model, gets n_valid = 0.
+inline std::vector<RelativePoseCovariance> NonCentralRelativePoseCovariance(Context& ctx, const std::vector<NonCentralRelativePoseRansacProblem>& problems,
+                                                                            const std::vector<NonCentralRelativePoseRansacResult>& ransac_results,
+                                                                            int n_samples, const std::vector<uint64_t>& seeds) {
+  const int n_prob = (int)problems.size();
+  if (ransac_results.size() != problems.size() || seeds.size() != problems.size())
+    throw std::invalid_argument("covins_b200::NonCentralRelativePoseCovariance: one RANSAC result and one seed per problem");
+  detail::require_no_samples(problems, "NonCentralRelativePoseCovariance");
+  detail::FlatRelProblems F = detail::flatten_rel_problems(problems, "NonCentralRelativePoseCovariance");
+  F.n_samples = n_samples;
+  const size_t m = n_prob > 0 ? n_prob : 1;
+  std::vector<double> ref(12 * m), cov(36 * m);
+  std::vector<int32_t> nv(m);
+  std::vector<uint8_t> mask;
+  for (int i = 0; i < n_prob; i++) {
+    if (ransac_results[i].inliers.size() != problems[i].sigma1.size())
+      throw std::invalid_argument("covins_b200::NonCentralRelativePoseCovariance: one inlier flag per correspondence");
+    std::copy(ransac_results[i].model.begin(), ransac_results[i].model.end(), ref.begin() + 12 * i);
+    mask.insert(mask.end(), ransac_results[i].inliers.begin(), ransac_results[i].inliers.end());
+  }
+  if (mask.empty()) mask.push_back(0);
+  const cvb_rel_ransac_problems P = F.view();
+  cvb_rel_cov_result R{cov.data(), nv.data(), nullptr, nullptr};
+  ctx.check(cvb_noncentral_relative_pose_covariance_seeded_batch(ctx.get(), &P, ref.data(), mask.data(), seeds.data(), &R, nullptr),
+            "cvb_noncentral_relative_pose_covariance_seeded_batch");
   std::vector<RelativePoseCovariance> out(n_prob);
   for (int i = 0; i < n_prob; i++) {
     std::copy(cov.begin() + 36 * i, cov.begin() + 36 * (i + 1), out[i].cov.begin());
@@ -1152,6 +1244,29 @@ inline std::vector<NonCentralRelativePoseRansacResult> RansacCentralRelativePose
   const cvb_central_rel_ransac_problems P{n_prob, ptr.data(), f1.data(), f2.data(), s1.data(), s2.data(), samples.data(), (int32_t)n_samples};
   return detail::ransac<NonCentralRelativePoseRansacResult>(ctx, cvb_ransac_central_relative_pose_batch, "cvb_ransac_central_relative_pose_batch", P,
                                                             ptr, threshold, max_iterations, probability);
+}
+// The same RANSAC with the samples drawn on the GPU (cvb_ransac_central_relative_pose_seeded_batch): one seed per problem,
+// every problem's samples left empty (as RansacAbsolutePose's seeded form).
+inline std::vector<NonCentralRelativePoseRansacResult> RansacCentralRelativePose(Context& ctx, const std::vector<CentralRelativePoseRansacProblem>& problems,
+                                                                                const std::vector<uint64_t>& seeds, double threshold, int max_iterations,
+                                                                                double probability = 0.99) {
+  detail::require_no_samples(problems, "RansacCentralRelativePose");
+  const int n_prob = (int)problems.size();
+  std::vector<int32_t> ptr(n_prob + 1, 0);
+  std::vector<double> f1, f2, s1, s2;
+  for (int i = 0; i < n_prob; i++) {
+    const CentralRelativePoseRansacProblem& p = problems[i];
+    const size_t n = p.sigma1.size();
+    if (p.bearings1.size() != 3 * n || p.bearings2.size() != 3 * n || p.sigma2.size() != n)
+      throw std::invalid_argument("covins_b200::RansacCentralRelativePose: inconsistent problem sizes");
+    ptr[i + 1] = ptr[i] + (int32_t)n;
+    f1.insert(f1.end(), p.bearings1.begin(), p.bearings1.end()); f2.insert(f2.end(), p.bearings2.begin(), p.bearings2.end());
+    s1.insert(s1.end(), p.sigma1.begin(), p.sigma1.end()); s2.insert(s2.end(), p.sigma2.begin(), p.sigma2.end());
+  }
+  const cvb_central_rel_ransac_problems P{n_prob, ptr.data(), f1.data(), f2.data(), s1.data(), s2.data(), nullptr, 0};
+  return detail::ransac_seeded<NonCentralRelativePoseRansacResult>(ctx, cvb_ransac_central_relative_pose_seeded_batch,
+                                                                   "cvb_ransac_central_relative_pose_seeded_batch", P, ptr, seeds, threshold, max_iterations,
+                                                                   probability);
 }
 
 // Resident-map descriptor database (cvb_db_*): the ORB descriptors of the map's keyframes live in HBM; the candidate

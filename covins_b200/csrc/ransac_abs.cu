@@ -228,20 +228,19 @@ struct RansacDev {
 // problem blockIdx.x for ransac_cta
 struct AbsProblem {
   const double *P, *F, *S, *cam;
-  const int* samples;   // [n_samples][4] of this problem
-  int n, n_samples;
+  int n;
   __device__ AbsProblem(const RansacDev& D, int pi, int off)
-      : P(D.pts + 3 * (size_t)off), F(D.f + 3 * (size_t)off), S(D.sigma + off), cam(D.cam + 12 * (size_t)pi),
-        samples(D.samples + 4 * (size_t)pi * D.o.n_samples), n(D.prob_ptr[pi + 1] - off), n_samples(D.o.n_samples) {}
+      : P(D.pts + 3 * (size_t)off), F(D.f + 3 * (size_t)off), S(D.sigma + off), cam(D.cam + 12 * (size_t)pi), n(D.prob_ptr[pi + 1] - off) {}
   // the first kWave threads solve one sample each
-  __device__ void solve_wave(int base, double (*w_model)[12], int* w_valid) const {
+  template <class Src>
+  __device__ void solve_wave(const Src& src, int base, double (*w_model)[12], int* w_valid) const {
     const int tid = threadIdx.x;
     if (tid >= kWave) return;
     const int s = base + tid;
     double M[12];
     for (int i = 0; i < 12; i++) M[i] = 0.0;
     bool v = false;
-    if (s < n_samples) v = hypothesis(samples + 4 * (size_t)s, n, P, F, cam, M);
+    if (src.has(s)) v = hypothesis(src.sample(s), n, P, F, cam, M);
     if (!v)
       for (int i = 0; i < 12; i++) M[i] = 0.0;
     for (int i = 0; i < 12; i++) w_model[tid][i] = M[i];
@@ -255,27 +254,27 @@ struct AbsProblem {
   }
 };
 
+// Src: SuppliedSamples<4> (cvb_ransac_absolute_pose_batch) or SeededSamples<4> (cvb_ransac_absolute_pose_seeded_batch)
+template <class Src>
 __global__ void __launch_bounds__(kThreads) ransac_abs_kernel(RansacDev D) {
   const int pi = blockIdx.x, off = D.prob_ptr[pi];
+  const int* samples = D.samples + 4 * (size_t)pi * D.o.n_samples;   // supplied: this problem's
   AbsProblem Pb(D, pi, off);
-  ransac_cta<4>(D.o, Pb, off, Pb.n);
+  ransac_cta<4>(D.o, Pb, sample_source<Src>(D.o, samples, pi, Pb.n), off, Pb.n);
 }
 
-}  // namespace
-
-extern "C" int cvb_ransac_absolute_pose_batch(cvb_ctx* ctx, const cvb_abs_ransac_problems* p, double threshold, int max_iterations,
-                                              double probability, cvb_abs_ransac_result* r) {
-  if (!ctx) return CVB_ERR_INVALID;
-  CVB_GUARD(ctx);
-  if (const int rc = check_ransac(ctx, "ransac_absolute_pose", p, max_iterations, r, 4)) return rc;
+// cvb_ransac_absolute_pose_batch (seeded = false) and cvb_ransac_absolute_pose_seeded_batch
+int abs_ransac(cvb_ctx* ctx, const char* name, const cvb_abs_ransac_problems* p, bool seeded, const uint64_t* seed, double threshold, int max_iterations,
+               double probability, cvb_abs_ransac_result* r, int32_t* drawn) {
+  if (const int rc = check_ransac(ctx, name, p, max_iterations, r, 4, seeded, seed)) return rc;
   const int n_prob = p->n_prob, ns = p->n_samples;
   if (n_prob == 0) return CVB_OK;
-  CVB_REQUIRE(ctx, p->cam_off && p->cam_rot, "ransac_absolute_pose: null camera arrays");
+  CVB_REQUIRE(ctx, p->cam_off && p->cam_rot, "%s: null camera arrays", name);
   const size_t N = (size_t)p->prob_ptr[n_prob];
-  CVB_REQUIRE(ctx, N == 0 || (p->pts && p->f && p->sigma), "ransac_absolute_pose: null correspondence arrays");
+  CVB_REQUIRE(ctx, N == 0 || (p->pts && p->f && p->sigma), "%s: null correspondence arrays", name);
   Stager St;
   const size_t o_ptr = St.put(p->prob_ptr, ((size_t)n_prob + 1) * 4), o_pts = St.put(p->pts, N * 24), o_f = St.put(p->f, N * 24),
-               o_sg = St.put(p->sigma, N * 8), o_smp = St.put(p->samples, (size_t)n_prob * ns * 16);
+               o_sg = St.put(p->sigma, N * 8), o_smp = seeded ? St.put(seed, (size_t)n_prob * 8) : St.put(p->samples, (size_t)n_prob * ns * 16);
   const size_t o_cam = St.reserve((size_t)n_prob * 96);
   for (int i = 0; i < n_prob; i++) {   // one camera per problem: offset (3) directly followed by the rotation (9, row-major)
     memcpy(St.h.data() + o_cam + 96 * (size_t)i, p->cam_off + 3 * (size_t)i, 24);
@@ -284,8 +283,28 @@ extern "C" int cvb_ransac_absolute_pose_batch(cvb_ctx* ctx, const cvb_abs_ransac
   const auto inputs = [&](unsigned char* d) {
     RansacDev D{};
     D.prob_ptr = (const int*)(d + o_ptr); D.pts = (const double*)(d + o_pts); D.f = (const double*)(d + o_f); D.sigma = (const double*)(d + o_sg);
-    D.cam = (const double*)(d + o_cam); D.samples = (const int*)(d + o_smp);
+    D.cam = (const double*)(d + o_cam);
+    if (seeded) D.o.seed = (const unsigned long long*)(d + o_smp);
+    else D.samples = (const int*)(d + o_smp);
     return D;
   };
-  return run_ransac(ctx, WS_GS5, ransac_abs_kernel, 0, St, inputs, n_prob, ns, N, threshold, max_iterations, probability, r);
+  if (seeded)
+    return run_ransac(ctx, WS_GS5, ransac_abs_kernel<SeededSamples<4>>, 0, St, inputs, n_prob, ns, N, threshold, max_iterations, probability, r, drawn, 4);
+  return run_ransac(ctx, WS_GS5, ransac_abs_kernel<SuppliedSamples<4>>, 0, St, inputs, n_prob, ns, N, threshold, max_iterations, probability, r);
+}
+
+}  // namespace
+
+extern "C" int cvb_ransac_absolute_pose_batch(cvb_ctx* ctx, const cvb_abs_ransac_problems* p, double threshold, int max_iterations,
+                                              double probability, cvb_abs_ransac_result* r) {
+  if (!ctx) return CVB_ERR_INVALID;
+  CVB_GUARD(ctx);
+  return abs_ransac(ctx, "ransac_absolute_pose", p, false, nullptr, threshold, max_iterations, probability, r, nullptr);
+}
+
+extern "C" int cvb_ransac_absolute_pose_seeded_batch(cvb_ctx* ctx, const cvb_abs_ransac_problems* p, const uint64_t* seed, double threshold,
+                                                     int max_iterations, double probability, cvb_abs_ransac_result* r, int32_t* drawn) {
+  if (!ctx) return CVB_ERR_INVALID;
+  CVB_GUARD(ctx);
+  return abs_ransac(ctx, "ransac_absolute_pose_seeded", p, true, seed, threshold, max_iterations, probability, r, drawn);
 }

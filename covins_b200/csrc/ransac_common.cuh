@@ -1,8 +1,9 @@
 // ransac_common.cuh — the RANSAC shared by ransac_abs.cu (GP3P) and ransac_rel.cu (17-point and 5-point): on the device, everything
-// of a problem's CTA from the selection state to the inlier mask (ransac_cta); on the host, the argument checks (check_ransac)
-// and the staging, upload, launch, download and copy-out of a call (run_ransac).  The kernels supply only what differs: their
-// per-problem setup, how a wave of samples is solved, the preparation of a hypothesis for scoring and the per-correspondence
-// score.
+// of a problem's CTA from the selection state to the inlier mask (ransac_cta) and the two sources of samples it reads
+// (SuppliedSamples: the caller's, SeededSamples: drawn per wave from the problem's seed by seeded_sample); on the host, the
+// argument checks (check_ransac) and the staging, upload, launch, download and copy-out of a call (run_ransac).  The kernels
+// supply only what differs: their per-problem setup, how a wave of samples is solved, the preparation of a hypothesis for
+// scoring and the per-correspondence score.
 #pragma once
 #include <float.h>
 #include <math.h>
@@ -22,18 +23,105 @@ struct RansacOut {
   int* best_sample; double* best_model; int* best_count; int* iterations; int* consumed;
   uint8_t* inlier_mask;                                             // nullable
   double* sample_model; uint8_t* sample_valid; int* sample_count;   // nullable together
+  const unsigned long long* seed; int* drawn;                       // seeded calls: [n_prob], [n_prob][n_samples][kS] (nullable)
 };
 
+// ---- the seeded sampler (include/covins_b200.h, "Seeded samples"; oracle/sampler_oracle.c restates it) ----
+// Philox4x64-10 (Salmon et al., SC'11; Random123's philox4x64 and numpy.random.Philox): counter c, key (k0, k1)
+__device__ __forceinline__ void philox4x64_10(unsigned long long* c, unsigned long long k0, unsigned long long k1) {
+#pragma unroll
+  for (int r = 0; r < 10; r++) {
+    if (r > 0) { k0 += 0x9E3779B97F4A7C15ull; k1 += 0xBB67AE8584CAA73Bull; }
+    const unsigned long long m0 = 0xD2E7470EE14C6C93ull, m1 = 0xCA5A826395121157ull;
+    const unsigned long long hi0 = __umul64hi(m0, c[0]), lo0 = m0 * c[0], hi1 = __umul64hi(m1, c[2]), lo1 = m1 * c[2];
+    const unsigned long long c1 = c[1], c3 = c[3];
+    c[0] = hi1 ^ c1 ^ k0; c[1] = lo1; c[2] = hi0 ^ c3 ^ k1; c[3] = lo0;
+  }
+}
+
+// Sample s of key (seed, stream): the ordered kS-subset of [0, m) (m >= kS) by a partial Fisher-Yates shuffle of the identity,
+// j = i + (u_i (m - i)) >> 32, u_0, u_1, ... the 32-bit halves (low first) of the words of Philox blocks (s, 0, 0, 0),
+// (s, 1, 0, 0), ...  Instead of an m-sized permutation, the kS positions written so far are kept as (position, value) pairs
+// in registers; the last pair of a position holds its value.
+template <int kS>
+__device__ __forceinline__ void seeded_sample(unsigned long long seed, unsigned long long stream, unsigned m, unsigned long long s, int* out) {
+  unsigned pos[kS], val[kS];
+  unsigned long long blk[4];
+#pragma unroll
+  for (int i = 0; i < kS; i++) {
+    if (i % 8 == 0) {
+      blk[0] = s; blk[1] = (unsigned long long)(i / 8); blk[2] = 0; blk[3] = 0;
+      philox4x64_10(blk, seed, stream);
+    }
+    const unsigned long long w = blk[(i % 8) / 2];
+    const unsigned u = i % 2 ? (unsigned)(w >> 32) : (unsigned)w;
+    const unsigned j = (unsigned)i + (unsigned)(((unsigned long long)u * (m - (unsigned)i)) >> 32);
+    unsigned vi = (unsigned)i, vj = j;
+#pragma unroll
+    for (int e = 0; e < i; e++) {
+      if (pos[e] == (unsigned)i) vi = val[e];
+      if (pos[e] == j) vj = val[e];
+    }
+    out[i] = (int)vj;                  // perm[i] <-> perm[j]; position i is never read again
+    pos[i] = j; val[i] = vi;
+  }
+}
+
+// The caller's samples of a problem ([n_samples][kS], read from global memory)
+template <int kS>
+struct SuppliedSamples {
+  static constexpr bool kSeeded = false;
+  static constexpr int kSize = kS;
+  const int* samples;
+  int n_samples;
+  __device__ void draw(int) const {}
+  __device__ bool has(int s) const { return s < n_samples; }
+  __device__ const int* sample(int s) const { return samples + kS * (size_t)s; }
+};
+
+// Samples drawn on the device: before a wave is solved, thread t < kWave draws sample base + t of the problem (stream 0, m = n)
+// into shared memory, and copies it to drawn[s] for s < n_samples.  A problem with fewer than kS correspondences has none.
+template <int kS>
+struct SeededSamples {
+  static constexpr bool kSeeded = true;
+  static constexpr int kSize = kS;
+  int (*w_smp)[kS];
+  unsigned long long seed;
+  int n, n_samples;
+  int* drawn;   // this problem's [n_samples][kS], nullable
+  __device__ void draw(int base) const {
+    const int t = threadIdx.x, s = base + t;
+    if (t >= kWave || n < kS) return;
+    seeded_sample<kS>(seed, 0, (unsigned)n, (unsigned long long)s, w_smp[t]);
+    if (drawn && s < n_samples)
+      for (int i = 0; i < kS; i++) drawn[kS * (size_t)s + i] = w_smp[t][i];
+  }
+  __device__ bool has(int) const { return n >= kS; }
+  __device__ const int* sample(int s) const { return w_smp[s % kWave]; }
+};
+
+// the sample source Src of problem pi (n correspondences) of a RANSAC call; samples: the problem's supplied samples
+template <class Src>
+__device__ __forceinline__ Src sample_source(const RansacOut& D, const int* samples, int pi, int n) {
+  if constexpr (Src::kSeeded) {
+    __shared__ int w_smp[kWave][Src::kSize];
+    return Src{w_smp, D.seed[pi], n, D.n_samples, D.drawn ? D.drawn + (size_t)Src::kSize * pi * D.n_samples : nullptr};
+  } else {
+    return Src{samples, D.n_samples};
+  }
+}
+
 // The RANSAC of problem blockIdx.x (n correspondences from off, kS indices per sample) after the kernel's per-problem setup.
-// Samples are taken in waves of kWave: Pb.solve_wave(base, w_model, w_valid) writes the models (zero if invalid) and valid flags
-// of samples base .. base + kWave - 1; every warp scores the wave's valid hypotheses against all correspondences (Pb.scorer(M),
-// called by every lane of the warp, prepares hypothesis M and returns the score of correspondence i under it; warp-shuffle
-// integer counts); thread 0 replays
+// Samples are taken in waves of kWave: src.draw(base) prepares them (seeded: draws them), Pb.solve_wave(src, base, w_model,
+// w_valid) writes the models (zero if invalid) and valid flags of samples base .. base + kWave - 1; every warp scores the wave's
+// valid hypotheses against all correspondences (Pb.scorer(M), called by every lane of the warp, prepares hypothesis M and returns
+// the score of correspondence i under it; warp-shuffle integer counts); thread 0 replays
 // opengv's Ransac::computeModel over the wave in sample order, and the CTA stops as soon as the adaptive bound ends the selection
 // (unless the per-sample outputs are requested), so the early stop saves the solver and scoring work of the samples it never
-// reads.  The CTA then writes the result and the selected model's inlier mask.
-template <int kS, class Problem>
-__device__ __forceinline__ void ransac_cta(const RansacOut& D, Problem& Pb, int off, int n) {
+// reads.  Supplied samples also end the selection when they run out; seeded ones never do (a problem with fewer than kS
+// correspondences draws none and selects nothing).  The CTA then writes the result and the selected model's inlier mask.
+template <int kS, class Src, class Problem>
+__device__ __forceinline__ void ransac_cta(const RansacOut& D, Problem& Pb, const Src& src, int off, int n) {
   const int pi = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const bool all = D.sample_model != nullptr;
   __shared__ double w_model[kWave][12];
@@ -43,13 +131,17 @@ __device__ __forceinline__ void ransac_cta(const RansacOut& D, Problem& Pb, int 
   __shared__ long long skipped;
   if (tid == 0) {
     best = -1; best_n = 0; it = 0; used = 0; skipped = 0; k_bound = (double)D.max_iterations;
-    running = D.max_iterations > 0;
+    running = D.max_iterations > 0 && (!Src::kSeeded || n >= kS);
     for (int i = 0; i < 12; i++) best_model[i] = 0.0;
   }
   __syncthreads();
   const long long max_skip = 10LL * D.max_iterations;
-  for (int base = 0; base < D.n_samples && (running || all); base += kWave) {
-    Pb.solve_wave(base, w_model, w_valid);
+  for (int base = 0; Src::kSeeded ? running || (all && base < D.n_samples) : base < D.n_samples && (running || all); base += kWave) {
+    if constexpr (Src::kSeeded) {
+      src.draw(base);
+      __syncthreads();
+    }
+    Pb.solve_wave(src, base, w_model, w_valid);
     __syncthreads();
     for (int h = warp; h < kWave; h += kWarps) {
       int cnt = 0;
@@ -68,7 +160,7 @@ __device__ __forceinline__ void ransac_cta(const RansacOut& D, Problem& Pb, int 
       D.sample_valid[g] = (uint8_t)w_valid[tid]; D.sample_count[g] = w_count[tid];
     }
     if (tid == 0) {   // placerec.ransac_select over the valid samples, opengv's skipped_count for the invalid ones
-      for (int h = 0; h < kWave && base + h < D.n_samples; h++) {
+      for (int h = 0; h < kWave && src.has(base + h); h++) {
         running = it < D.max_iterations && (double)it < k_bound && skipped < max_skip;
         if (!running) break;
         used++;
@@ -87,7 +179,8 @@ __device__ __forceinline__ void ransac_cta(const RansacOut& D, Problem& Pb, int 
         }
         it++;
       }
-      running = it < D.max_iterations && (double)it < k_bound && skipped < max_skip;
+      // (a seeded problem with fewer than kS correspondences never starts: it would draw forever)
+      running = (!Src::kSeeded || n >= kS) && it < D.max_iterations && (double)it < k_bound && skipped < max_skip;
     }
     __syncthreads();
   }
@@ -127,33 +220,43 @@ int check_samples(cvb_ctx* ctx, const char* name, const int32_t* samples, const 
 }
 
 // The argument checks of a RANSAC call that do not depend on its problem type: the sizes, the result pointers, prob_ptr and the
-// samples (k indices each).  With n_prob = 0 only the sizes are checked.
+// samples (k indices each).  With n_prob = 0 only the sizes are checked.  A seeded call (seeded) instead takes no samples and
+// one seed per problem.
 template <class Problems, class Result>
-int check_ransac(cvb_ctx* ctx, const char* name, const Problems* p, int max_iterations, const Result* r, int k) {
+int check_ransac(cvb_ctx* ctx, const char* name, const Problems* p, int max_iterations, const Result* r, int k, bool seeded = false,
+                 const uint64_t* seed = nullptr) {
   CVB_REQUIRE(ctx, p && r && p->n_prob >= 0 && p->n_samples >= 0 && max_iterations >= 0, "%s: bad arguments", name);
   CVB_REQUIRE(ctx, max_iterations <= INT32_MAX / 10, "%s: max_iterations too large", name);
+  CVB_REQUIRE(ctx, !seeded || !p->samples, "%s: samples must be NULL (the samples are drawn from the seeds)", name);
+  CVB_REQUIRE(ctx, !seeded || max_iterations <= (INT32_MAX - kWave) / 11, "%s: max_iterations too large", name);   // sample numbers fit an int
   const int n_prob = p->n_prob, ns = p->n_samples;
   if (n_prob == 0) return CVB_OK;
   CVB_REQUIRE(ctx, p->prob_ptr && r->best_sample && r->best_model && r->best_count && r->iterations && r->consumed, "%s: null required pointer", name);
   CVB_REQUIRE(ctx, (r->sample_model != nullptr) == (r->sample_valid != nullptr) && (r->sample_model != nullptr) == (r->sample_count != nullptr),
               "%s: sample_model / sample_valid / sample_count are requested together", name);
   CVB_REQUIRE(ctx, ptr_ok(p->prob_ptr, n_prob), "%s: prob_ptr does not start at 0 or decreases", name);
+  if (seeded) {
+    CVB_REQUIRE(ctx, seed, "%s: null seed", name);
+    return CVB_OK;
+  }
   CVB_REQUIRE(ctx, ns == 0 || p->samples, "%s: null samples", name);
   return check_samples(ctx, name, p->samples, p->prob_ptr, n_prob, ns, k);
 }
 
 // The rest of a RANSAC call whose inputs are staged in St: its outputs staged after them, one upload into workspace slot
 // ws_slot, one launch of kernel (one CTA per problem, smem bytes of dynamic shared memory) with the device struct
-// inputs(device block) and its common part filled here, one download, the copy-out into r.
+// inputs(device block) and its common part filled here, one download, the copy-out into r.  A seeded call may also ask for
+// its drawn samples (drawn, k indices each, -1 where not drawn).
 template <class Dev, class Result, class Inputs>
 int run_ransac(cvb_ctx* ctx, int ws_slot, void (*kernel)(Dev), size_t smem, Stager& St, const Inputs& inputs, int n_prob, int ns, size_t N,
-               double threshold, int max_iterations, double probability, Result* r) {
+               double threshold, int max_iterations, double probability, Result* r, int32_t* drawn = nullptr, int k = 0) {
   const size_t S_all = (size_t)n_prob * ns;
   const bool all = r->sample_model != nullptr;
   const size_t in_bytes = St.h.size();
   const size_t o_bm = St.reserve((size_t)n_prob * 96), o_bs = St.reserve((size_t)n_prob * 4), o_bc = St.reserve((size_t)n_prob * 4),
                o_it = St.reserve((size_t)n_prob * 4), o_us = St.reserve((size_t)n_prob * 4), o_mask = r->inlier_mask ? St.reserve(N) : 0,
-               o_sm = all ? St.reserve(S_all * 96) : 0, o_sv = all ? St.reserve(S_all) : 0, o_sc = all ? St.reserve(S_all * 4) : 0;
+               o_sm = all ? St.reserve(S_all * 96) : 0, o_sv = all ? St.reserve(S_all) : 0, o_sc = all ? St.reserve(S_all * 4) : 0,
+               o_dr = drawn ? St.reserve(S_all * k * 4) : 0;
   const size_t total = St.h.size();
   unsigned char* d = (unsigned char*)cvb_ws(ctx, ws_slot, total);
   unsigned char* hpin = (unsigned char*)cvb_pinned(ctx, total);
@@ -167,6 +270,10 @@ int run_ransac(cvb_ctx* ctx, int ws_slot, void (*kernel)(Dev), size_t smem, Stag
   if (all) { O.sample_model = (double*)(d + o_sm); O.sample_valid = d + o_sv; O.sample_count = (int*)(d + o_sc); }
   cudaStream_t st = ctx->stream;
   CVB_CUDA(ctx, cudaMemcpyAsync(d, hpin, in_bytes, cudaMemcpyHostToDevice, st));
+  if (drawn) {
+    O.drawn = (int*)(d + o_dr);
+    CVB_CUDA(ctx, cudaMemsetAsync(d + o_dr, 0xff, S_all * k * 4, st));
+  }
   kernel<<<n_prob, kThreads, smem, st>>>(D);
   CVB_CHECK_LAUNCH(ctx);
   CVB_CUDA(ctx, cudaMemcpyAsync(hpin + o_bm, d + o_bm, total - o_bm, cudaMemcpyDeviceToHost, st));
@@ -178,6 +285,7 @@ int run_ransac(cvb_ctx* ctx, int ws_slot, void (*kernel)(Dev), size_t smem, Stag
   if (all) {
     memcpy(r->sample_model, hpin + o_sm, S_all * 96); memcpy(r->sample_valid, hpin + o_sv, S_all); memcpy(r->sample_count, hpin + o_sc, S_all * 4);
   }
+  if (drawn) memcpy(drawn, hpin + o_dr, S_all * k * 4);
   return CVB_OK;
 }
 

@@ -21,6 +21,8 @@
 // IEEE restatement compiled with -ffp-contract=off (oracle/ransac_rel_oracle.c for the 17-point solver,
 // oracle/ransac_rel5_oracle.c for the 5-point one; their headers state the problems and their assumptions; so does
 // include/covins_b200.h).
+#include <type_traits>
+
 #include "ransac_common.cuh"
 
 namespace {
@@ -577,16 +579,15 @@ struct RelProblem {
   ProbView P;
   const double *S1, *S2;
   int nc1, nc2;
-  const int* samples;   // [n_samples][Sv::kSample] of this problem
-  int n_samples;
   double* W;
   int warp, lane;
   // each warp solves one sample at a time
-  __device__ void solve_wave(int base, double (*w_model)[12], int* w_valid) const {
+  template <class Src>
+  __device__ void solve_wave(const Src& src, int base, double (*w_model)[12], int* w_valid) const {
     for (int h = warp; h < kWave; h += kWarps) {
       const int s = base + h;
       bool v = false;
-      if (s < n_samples) v = Sv::solve(samples + Sv::kSample * (size_t)s, P, W, w_model[h], lane);
+      if (src.has(s)) v = Sv::solve(src.sample(s), P, W, w_model[h], lane);
       __syncwarp();
       if (lane == 0) {
         if (!v)
@@ -602,8 +603,9 @@ struct RelProblem {
   }
 };
 
-// Sv: Solver17 (non-central, rigs and camera indices from D) or Solver5 (central: one identity camera per side)
-template <class Sv>
+// Sv: Solver17 (non-central, rigs and camera indices from D) or Solver5 (central: one identity camera per side); Src:
+// SuppliedSamples<Sv::kSample> or SeededSamples<Sv::kSample>
+template <class Sv, class Src>
 __global__ void __launch_bounds__(kThreads) ransac_rel_kernel(RelDev D) {
   extern __shared__ double dyn[];
   const int pi = blockIdx.x, tid = threadIdx.x;
@@ -627,17 +629,16 @@ __global__ void __launch_bounds__(kThreads) ransac_rel_kernel(RelDev D) {
   __syncthreads();
   RelProblem<Sv> Pb{ProbView{n, D.f1 + 3 * (size_t)off, D.f2 + 3 * (size_t)off, Sv::kCentral ? nullptr : D.cam1 + off,
                              Sv::kCentral ? nullptr : D.cam2 + off, rig1, rig2, rigs_finite != 0},
-                    D.s1 + off, D.s2 + off, nc1, nc2, D.samples + Sv::kSample * (size_t)pi * D.o.n_samples, D.o.n_samples,
-                    dyn + (size_t)(tid >> 5) * D.area, tid >> 5, tid & 31};
-  ransac_cta<Sv::kSample>(D.o, Pb, off, n);
+                    D.s1 + off, D.s2 + off, nc1, nc2, dyn + (size_t)(tid >> 5) * D.area, tid >> 5, tid & 31};
+  ransac_cta<Sv::kSample>(D.o, Pb, sample_source<Src>(D.o, D.samples + Sv::kSample * (size_t)pi * D.o.n_samples, pi, n), off, n);
 }
 
 // staging offsets of the inputs (camera arrays unused by a central problem)
 struct RelIn { size_t ptr, f1, f2, s1, s2, c1, c2, cp1, cp2, rig1, rig2, smp; };
 
 // the argument checks of a non-central problem batch (n_prob > 0) shared by the RANSAC and the covariance calls, up to the
-// samples; with_sigma: sigma1 / sigma2 are read.  Sets *max_pairs to the largest rig1 x rig2 camera-pair count.
-int check_rel_problems(cvb_ctx* ctx, const char* name, const cvb_rel_ransac_problems* p, bool with_sigma, int* max_pairs) {
+// samples; with_sigma: sigma1 / sigma2 are read; with_samples: the samples are (the sample-supplied calls).  Sets *max_pairs to the largest rig1 x rig2 camera-pair count.
+int check_rel_problems(cvb_ctx* ctx, const char* name, const cvb_rel_ransac_problems* p, bool with_sigma, bool with_samples, int* max_pairs) {
   const int n_prob = p->n_prob;
   CVB_REQUIRE(ctx, ptr_ok(p->prob_ptr, n_prob), "%s: prob_ptr does not start at 0 or decreases", name);
   CVB_REQUIRE(ctx, ptr_ok(p->cam_ptr1, n_prob) && ptr_ok(p->cam_ptr2, n_prob), "%s: cam_ptr1 / cam_ptr2 does not start at 0 or decreases", name);
@@ -650,7 +651,7 @@ int check_rel_problems(cvb_ctx* ctx, const char* name, const cvb_rel_ransac_prob
   const size_t N = (size_t)p->prob_ptr[n_prob], NC1 = (size_t)p->cam_ptr1[n_prob], NC2 = (size_t)p->cam_ptr2[n_prob];
   CVB_REQUIRE(ctx, N == 0 || (p->f1 && p->f2 && (!with_sigma || (p->sigma1 && p->sigma2)) && p->cam1 && p->cam2), "%s: null correspondence arrays", name);
   CVB_REQUIRE(ctx, (NC1 == 0 || (p->cam_off1 && p->cam_rot1)) && (NC2 == 0 || (p->cam_off2 && p->cam_rot2)), "%s: null rig arrays", name);
-  CVB_REQUIRE(ctx, p->n_samples == 0 || p->samples, "%s: null samples", name);
+  CVB_REQUIRE(ctx, !with_samples || p->n_samples == 0 || p->samples, "%s: null samples", name);
   for (int i = 0; i < n_prob; i++) {
     const int o = p->prob_ptr[i], n = p->prob_ptr[i + 1] - o;
     const int nc1 = p->cam_ptr1[i + 1] - p->cam_ptr1[i], nc2 = p->cam_ptr2[i + 1] - p->cam_ptr2[i];
@@ -676,21 +677,24 @@ void stage_rigs(Stager& St, const cvb_rel_ransac_problems* p, RelIn& in) {
   }
 }
 
-// ransac_rel_kernel<Sv> on the inputs staged in St (max_pairs: the largest camera-pair count of a problem)
-template <class Sv>
+// ransac_rel_kernel<Sv, Src> on the inputs staged in St (max_pairs: the largest camera-pair count of a problem; a seeded call's
+// seeds at in.smp, its drawn samples to drawn)
+template <class Sv, class Src>
 int run_rel_ransac(cvb_ctx* ctx, Stager& St, const RelIn& in, int n_prob, int ns, size_t N, int max_pairs, double threshold, int max_iterations,
-                   double probability, cvb_rel_ransac_result* r) {
+                   double probability, cvb_rel_ransac_result* r, int32_t* drawn = nullptr) {
   const int area = Sv::kArea > kPairArea * max_pairs ? Sv::kArea : kPairArea * max_pairs;
   constexpr int kMaxPairs = Sv::kCentral ? 1 : kMaxCams * kMaxCams;
   constexpr int kMaxArea = Sv::kArea > kPairArea * kMaxPairs ? Sv::kArea : kPairArea * kMaxPairs;
   static cvb_once_per_device once;
   if (once.first(ctx->device)) {
-    CVB_CUDA(ctx, cudaFuncSetAttribute(ransac_rel_kernel<Sv>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(kWarps * kMaxArea * sizeof(double))));
+    CVB_CUDA(ctx, cudaFuncSetAttribute(ransac_rel_kernel<Sv, Src>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(kWarps * kMaxArea * sizeof(double))));
   }
   const auto inputs = [&](unsigned char* d) {
     RelDev D{};
     D.prob_ptr = (const int*)(d + in.ptr); D.f1 = (const double*)(d + in.f1); D.f2 = (const double*)(d + in.f2);
-    D.s1 = (const double*)(d + in.s1); D.s2 = (const double*)(d + in.s2); D.samples = (const int*)(d + in.smp);
+    D.s1 = (const double*)(d + in.s1); D.s2 = (const double*)(d + in.s2);
+    if (Src::kSeeded) D.o.seed = (const unsigned long long*)(d + in.smp);
+    else D.samples = (const int*)(d + in.smp);
     if (!Sv::kCentral) {
       D.cam1 = (const int*)(d + in.c1); D.cam2 = (const int*)(d + in.c2); D.cam_ptr1 = (const int*)(d + in.cp1); D.cam_ptr2 = (const int*)(d + in.cp2);
       D.rig1 = (const double*)(d + in.rig1); D.rig2 = (const double*)(d + in.rig2);
@@ -698,8 +702,8 @@ int run_rel_ransac(cvb_ctx* ctx, Stager& St, const RelIn& in, int n_prob, int ns
     D.area = area;
     return D;
   };
-  return run_ransac(ctx, WS_GS6, ransac_rel_kernel<Sv>, (size_t)kWarps * area * sizeof(double), St, inputs, n_prob, ns, N, threshold,
-                    max_iterations, probability, r);
+  return run_ransac(ctx, WS_GS6, ransac_rel_kernel<Sv, Src>, (size_t)kWarps * area * sizeof(double), St, inputs, n_prob, ns, N, threshold,
+                    max_iterations, probability, r, drawn, Sv::kSample);
 }
 
 // ---- the sampling-based covariance of a 17-point model (cvb_noncentral_relative_pose_covariance_batch) ----
@@ -717,6 +721,10 @@ struct CovDev {
   int n_samples, ctas_per_prob;
   double* delta; uint8_t* valid;   // [n_prob][n_samples][6], [n_prob][n_samples]
   double* cov; int* n_valid;       // [n_prob][36], [n_prob]
+};
+// the seeded call's solve: the inlier mask [N], the seeds [n_prob] and the drawn samples (nullable) instead of samples
+struct CovSeededDev : CovDev {
+  const uint8_t* mask; const unsigned long long* seed; int* drawn;
 };
 
 // q = (x, y, z, w) of a rotation matrix m (row-major) in Eigen's branch for the largest diagonal entry i
@@ -755,7 +763,12 @@ __device__ void rel_deviation(const double* ref, const double* M, double* d) {
   }
 }
 
-__global__ void __launch_bounds__(kThreads) rel_cov_solve_kernel(CovDev D) {
+// Dev = CovSeededDev: the seeded form (cvb_noncentral_relative_pose_covariance_seeded_batch).  Its CTA counts the problem's
+// inliers m in the mask; a problem with m < 17 is skipped like one without a reference model.  For sample s, lane 0 draws the
+// ranks (stream 1, [0, m)), and the warp maps each rank j to the j-th inlier in ascending order with one ballot scan of the mask.
+template <class Dev>
+__global__ void __launch_bounds__(kThreads) rel_cov_solve_kernel(Dev D) {
+  constexpr bool kSeeded = !std::is_same<Dev, CovDev>::value;
   extern __shared__ double dyn[];
   const int pi = blockIdx.x / D.ctas_per_prob, chunk = blockIdx.x % D.ctas_per_prob;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, nw = blockDim.x >> 5;
@@ -766,6 +779,14 @@ __global__ void __launch_bounds__(kThreads) rel_cov_solve_kernel(CovDev D) {
   for (int i = tid; i < 12 * nc1; i += blockDim.x) rig1[i] = D.rig1[12 * (size_t)D.cam_ptr1[pi] + i];
   for (int i = tid; i < 12 * nc2; i += blockDim.x) rig2[i] = D.rig2[12 * (size_t)D.cam_ptr2[pi] + i];
   if (tid < 12) ref[tid] = D.ref_model[12 * (size_t)pi + tid];
+  [[maybe_unused]] __shared__ int n_inl, w_smp[kSeeded ? kWarps : 1][kSample];
+  if constexpr (kSeeded) {
+    if (tid == 0) n_inl = 0;
+    __syncthreads();
+    int c = 0;
+    for (int i = tid; i < n; i += blockDim.x) c += D.mask[off + i] != 0;
+    atomicAdd(&n_inl, c);   // integer: order-independent
+  }
   __syncthreads();
   if (tid == 0) {
     int fin = 1, zero = 1;
@@ -773,6 +794,7 @@ __global__ void __launch_bounds__(kThreads) rel_cov_solve_kernel(CovDev D) {
     for (int i = 0; i < 12 * nc2; i++) fin &= isfinite(rig2[i]);
     for (int i = 0; i < 12; i++) zero &= ref[i] == 0.0;
     rigs_finite = fin; skip = zero;
+    if constexpr (kSeeded) skip |= n_inl < kSample;
   }
   __syncthreads();
   const ProbView P{n, D.f1 + 3 * (size_t)off, D.f2 + 3 * (size_t)off, D.cam1 + off, D.cam2 + off, rig1, rig2, rigs_finite != 0};
@@ -780,7 +802,30 @@ __global__ void __launch_bounds__(kThreads) rel_cov_solve_kernel(CovDev D) {
   const int s_end = min((chunk + 1) * kCovPerCta, D.n_samples);
   for (int s = chunk * kCovPerCta + warp; s < s_end; s += nw) {
     const size_t g = (size_t)pi * D.n_samples + s;
-    const bool v = !skip && Solver17::solve(D.samples + kSample * g, P, W, w_model[warp], lane);   // a skipped problem's samples are not read
+    bool v;
+    if constexpr (kSeeded) {
+      if (!skip) {
+        if (lane == 0) seeded_sample<kSample>(D.seed[pi], 1, (unsigned)n_inl, (unsigned long long)s, w_smp[warp]);
+        __syncwarp();
+        const int r = lane < kSample ? w_smp[warp][lane] : -1;
+        int idx = -1;
+        for (int b = 0, c = 0; b < n; b += 32) {   // c: inliers before correspondence b
+          const unsigned bal = __ballot_sync(kFull, b + lane < n && D.mask[off + b + lane]);
+          const int cnt = __popc(bal);
+          if (r >= c && r < c + cnt) idx = b + (int)__fns(bal, 0, r - c + 1);
+          c += cnt;
+        }
+        __syncwarp();
+        if (lane < kSample) {
+          w_smp[warp][lane] = idx;
+          if (D.drawn) D.drawn[kSample * g + lane] = idx;
+        }
+        __syncwarp();
+      }
+      v = !skip && Solver17::solve(w_smp[warp], P, W, w_model[warp], lane);
+    } else {
+      v = !skip && Solver17::solve(D.samples + kSample * g, P, W, w_model[warp], lane);   // a skipped problem's samples are not read
+    }
     __syncwarp();
     if (lane == 0) {
       double d[6] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0};
@@ -813,58 +858,92 @@ __global__ void __launch_bounds__(kCovReduceThreads) rel_cov_reduce_kernel(CovDe
   if (tid == 0) D.n_valid[pi] = nv;
 }
 
-}  // namespace
-
-extern "C" int cvb_ransac_noncentral_relative_pose_batch(cvb_ctx* ctx, const cvb_rel_ransac_problems* p, double threshold, int max_iterations,
-                                                         double probability, cvb_rel_ransac_result* r) {
-  if (!ctx) return CVB_ERR_INVALID;
-  CVB_GUARD(ctx);
-  if (const int rc = check_ransac(ctx, "ransac_noncentral_relative_pose", p, max_iterations, r, kSample)) return rc;
+// cvb_ransac_noncentral_relative_pose_batch (seeded = false) and cvb_ransac_noncentral_relative_pose_seeded_batch
+int noncentral_ransac(cvb_ctx* ctx, const char* name, const cvb_rel_ransac_problems* p, bool seeded, const uint64_t* seed, double threshold,
+                      int max_iterations, double probability, cvb_rel_ransac_result* r, int32_t* drawn) {
+  if (const int rc = check_ransac(ctx, name, p, max_iterations, r, kSample, seeded, seed)) return rc;
   const int n_prob = p->n_prob, ns = p->n_samples;
   if (n_prob == 0) return CVB_OK;
-  CVB_REQUIRE(ctx, p->cam_ptr1 && p->cam_ptr2, "ransac_noncentral_relative_pose: null cam_ptr1 / cam_ptr2");
+  CVB_REQUIRE(ctx, p->cam_ptr1 && p->cam_ptr2, "%s: null cam_ptr1 / cam_ptr2", name);
   int max_pairs = 0;
-  if (const int rc = check_rel_problems(ctx, "ransac_noncentral_relative_pose", p, true, &max_pairs)) return rc;
+  if (const int rc = check_rel_problems(ctx, name, p, true, !seeded, &max_pairs)) return rc;
   const size_t N = (size_t)p->prob_ptr[n_prob], S_all = (size_t)n_prob * ns;
   Stager St;
   RelIn in{};
   in.ptr = St.put(p->prob_ptr, ((size_t)n_prob + 1) * 4); in.f1 = St.put(p->f1, N * 24); in.f2 = St.put(p->f2, N * 24);
   in.s1 = St.put(p->sigma1, N * 8); in.s2 = St.put(p->sigma2, N * 8); in.c1 = St.put(p->cam1, N * 4); in.c2 = St.put(p->cam2, N * 4);
   in.cp1 = St.put(p->cam_ptr1, ((size_t)n_prob + 1) * 4); in.cp2 = St.put(p->cam_ptr2, ((size_t)n_prob + 1) * 4);
-  in.smp = St.put(p->samples, S_all * kSample * 4);
+  in.smp = seeded ? St.put(seed, (size_t)n_prob * 8) : St.put(p->samples, S_all * kSample * 4);
   stage_rigs(St, p, in);
-  return run_rel_ransac<Solver17>(ctx, St, in, n_prob, ns, N, max_pairs, threshold, max_iterations, probability, r);
+  if (seeded)
+    return run_rel_ransac<Solver17, SeededSamples<kSample>>(ctx, St, in, n_prob, ns, N, max_pairs, threshold, max_iterations, probability, r, drawn);
+  return run_rel_ransac<Solver17, SuppliedSamples<kSample>>(ctx, St, in, n_prob, ns, N, max_pairs, threshold, max_iterations, probability, r);
+}
+
+// cvb_ransac_central_relative_pose_batch (seeded = false) and cvb_ransac_central_relative_pose_seeded_batch
+int central_ransac(cvb_ctx* ctx, const char* name, const cvb_central_rel_ransac_problems* p, bool seeded, const uint64_t* seed, double threshold,
+                   int max_iterations, double probability, cvb_rel_ransac_result* r, int32_t* drawn) {
+  if (const int rc = check_ransac(ctx, name, p, max_iterations, r, kSample5, seeded, seed)) return rc;
+  const int n_prob = p->n_prob, ns = p->n_samples;
+  if (n_prob == 0) return CVB_OK;
+  const size_t N = (size_t)p->prob_ptr[n_prob];
+  CVB_REQUIRE(ctx, N == 0 || (p->f1 && p->f2 && p->sigma1 && p->sigma2), "%s: null correspondence arrays", name);
+  Stager St;
+  RelIn in{};
+  in.ptr = St.put(p->prob_ptr, ((size_t)n_prob + 1) * 4); in.f1 = St.put(p->f1, N * 24); in.f2 = St.put(p->f2, N * 24);
+  in.s1 = St.put(p->sigma1, N * 8); in.s2 = St.put(p->sigma2, N * 8);
+  in.smp = seeded ? St.put(seed, (size_t)n_prob * 8) : St.put(p->samples, (size_t)n_prob * ns * kSample5 * 4);
+  if (seeded)
+    return run_rel_ransac<Solver5, SeededSamples<kSample5>>(ctx, St, in, n_prob, ns, N, 1, threshold, max_iterations, probability, r, drawn);
+  return run_rel_ransac<Solver5, SuppliedSamples<kSample5>>(ctx, St, in, n_prob, ns, N, 1, threshold, max_iterations, probability, r);
+}
+
+}  // namespace
+
+extern "C" int cvb_ransac_noncentral_relative_pose_batch(cvb_ctx* ctx, const cvb_rel_ransac_problems* p, double threshold, int max_iterations,
+                                                         double probability, cvb_rel_ransac_result* r) {
+  if (!ctx) return CVB_ERR_INVALID;
+  CVB_GUARD(ctx);
+  return noncentral_ransac(ctx, "ransac_noncentral_relative_pose", p, false, nullptr, threshold, max_iterations, probability, r, nullptr);
+}
+
+extern "C" int cvb_ransac_noncentral_relative_pose_seeded_batch(cvb_ctx* ctx, const cvb_rel_ransac_problems* p, const uint64_t* seed,
+                                                                double threshold, int max_iterations, double probability, cvb_rel_ransac_result* r,
+                                                                int32_t* drawn) {
+  if (!ctx) return CVB_ERR_INVALID;
+  CVB_GUARD(ctx);
+  return noncentral_ransac(ctx, "ransac_noncentral_relative_pose_seeded", p, true, seed, threshold, max_iterations, probability, r, drawn);
 }
 
 extern "C" int cvb_ransac_central_relative_pose_batch(cvb_ctx* ctx, const cvb_central_rel_ransac_problems* p, double threshold, int max_iterations,
                                                       double probability, cvb_rel_ransac_result* r) {
   if (!ctx) return CVB_ERR_INVALID;
   CVB_GUARD(ctx);
-  if (const int rc = check_ransac(ctx, "ransac_central_relative_pose", p, max_iterations, r, kSample5)) return rc;
-  const int n_prob = p->n_prob, ns = p->n_samples;
-  if (n_prob == 0) return CVB_OK;
-  const size_t N = (size_t)p->prob_ptr[n_prob];
-  CVB_REQUIRE(ctx, N == 0 || (p->f1 && p->f2 && p->sigma1 && p->sigma2), "ransac_central_relative_pose: null correspondence arrays");
-  Stager St;
-  RelIn in{};
-  in.ptr = St.put(p->prob_ptr, ((size_t)n_prob + 1) * 4); in.f1 = St.put(p->f1, N * 24); in.f2 = St.put(p->f2, N * 24);
-  in.s1 = St.put(p->sigma1, N * 8); in.s2 = St.put(p->sigma2, N * 8); in.smp = St.put(p->samples, (size_t)n_prob * ns * kSample5 * 4);
-  return run_rel_ransac<Solver5>(ctx, St, in, n_prob, ns, N, 1, threshold, max_iterations, probability, r);
+  return central_ransac(ctx, "ransac_central_relative_pose", p, false, nullptr, threshold, max_iterations, probability, r, nullptr);
 }
 
-extern "C" int cvb_noncentral_relative_pose_covariance_batch(cvb_ctx* ctx, const cvb_rel_ransac_problems* p, const double* ref_model,
-                                                             cvb_rel_cov_result* r) {
+extern "C" int cvb_ransac_central_relative_pose_seeded_batch(cvb_ctx* ctx, const cvb_central_rel_ransac_problems* p, const uint64_t* seed,
+                                                             double threshold, int max_iterations, double probability, cvb_rel_ransac_result* r,
+                                                             int32_t* drawn) {
   if (!ctx) return CVB_ERR_INVALID;
   CVB_GUARD(ctx);
-  CVB_REQUIRE(ctx, p && r && p->n_prob >= 0 && p->n_samples >= 0, "noncentral_relative_pose_covariance: bad arguments");
+  return central_ransac(ctx, "ransac_central_relative_pose_seeded", p, true, seed, threshold, max_iterations, probability, r, drawn);
+}
+
+namespace {
+
+// cvb_noncentral_relative_pose_covariance_batch (seeded = false) and cvb_noncentral_relative_pose_covariance_seeded_batch
+int rel_cov(cvb_ctx* ctx, const char* name, const cvb_rel_ransac_problems* p, const double* ref_model, bool seeded, const uint8_t* inlier_mask,
+            const uint64_t* seed, cvb_rel_cov_result* r, int32_t* drawn) {
+  CVB_REQUIRE(ctx, p && r && p->n_prob >= 0 && p->n_samples >= 0, "%s: bad arguments", name);
+  CVB_REQUIRE(ctx, !seeded || !p->samples, "%s: samples must be NULL (the samples are drawn from the seeds)", name);
   const int n_prob = p->n_prob, ns = p->n_samples;
   if (n_prob == 0) return CVB_OK;
-  CVB_REQUIRE(ctx, p->prob_ptr && p->cam_ptr1 && p->cam_ptr2 && ref_model && r->cov && r->n_valid,
-              "noncentral_relative_pose_covariance: null required pointer");
-  CVB_REQUIRE(ctx, (r->sample_delta != nullptr) == (r->sample_valid != nullptr),
-              "noncentral_relative_pose_covariance: sample_delta / sample_valid are requested together");
+  CVB_REQUIRE(ctx, p->prob_ptr && p->cam_ptr1 && p->cam_ptr2 && ref_model && r->cov && r->n_valid, "%s: null required pointer", name);
+  CVB_REQUIRE(ctx, !seeded || (inlier_mask && seed), "%s: null inlier_mask / seed", name);
+  CVB_REQUIRE(ctx, (r->sample_delta != nullptr) == (r->sample_valid != nullptr), "%s: sample_delta / sample_valid are requested together", name);
   int max_pairs = 0;   // unused: the covariance does not score
-  if (const int rc = check_rel_problems(ctx, "noncentral_relative_pose_covariance", p, false, &max_pairs)) return rc;
+  if (const int rc = check_rel_problems(ctx, name, p, false, !seeded, &max_pairs)) return rc;
   // the reference models: all zeros (skipped), or finite with a rotation R
   std::vector<uint8_t> skip(n_prob);
   for (int i = 0; i < n_prob; i++) {
@@ -873,17 +952,17 @@ extern "C" int cvb_noncentral_relative_pose_covariance_batch(cvb_ctx* ctx, const
     for (int k = 0; k < 12; k++) { zero &= M[k] == 0.0; finite &= isfinite(M[k]) != 0; }
     skip[i] = zero;
     if (zero) continue;
-    CVB_REQUIRE(ctx, finite, "noncentral_relative_pose_covariance: reference model of problem %d is not finite", i);
+    CVB_REQUIRE(ctx, finite, "%s: reference model of problem %d is not finite", name, i);
     double dev = 0.0;
     for (int a = 0; a < 3; a++)
       for (int b = 0; b < 3; b++) {
         const double g = M[a] * M[b] + M[4 + a] * M[4 + b] + M[8 + a] * M[8 + b] - (a == b ? 1.0 : 0.0);
         dev = fabs(g) > dev ? fabs(g) : dev;
       }
-    CVB_REQUIRE(ctx, dev <= 1e-6, "noncentral_relative_pose_covariance: R of the reference model of problem %d is not a rotation (max |R^T R - I| = %g)", i,
-                dev);
+    CVB_REQUIRE(ctx, dev <= 1e-6, "%s: R of the reference model of problem %d is not a rotation (max |R^T R - I| = %g)", name, i, dev);
   }
-  if (const int rc = check_samples(ctx, "noncentral_relative_pose_covariance", p->samples, p->prob_ptr, n_prob, ns, kSample, skip.data())) return rc;
+  if (!seeded)
+    if (const int rc = check_samples(ctx, name, p->samples, p->prob_ptr, n_prob, ns, kSample, skip.data())) return rc;
   const size_t N = (size_t)p->prob_ptr[n_prob], S_all = (size_t)n_prob * ns;
   const bool all = r->sample_delta != nullptr;
   Stager St;
@@ -891,37 +970,65 @@ extern "C" int cvb_noncentral_relative_pose_covariance_batch(cvb_ctx* ctx, const
   in.ptr = St.put(p->prob_ptr, ((size_t)n_prob + 1) * 4); in.f1 = St.put(p->f1, N * 24); in.f2 = St.put(p->f2, N * 24);
   in.c1 = St.put(p->cam1, N * 4); in.c2 = St.put(p->cam2, N * 4);
   in.cp1 = St.put(p->cam_ptr1, ((size_t)n_prob + 1) * 4); in.cp2 = St.put(p->cam_ptr2, ((size_t)n_prob + 1) * 4);
-  in.smp = St.put(p->samples, S_all * kSample * 4);
+  in.smp = seeded ? St.put(seed, (size_t)n_prob * 8) : St.put(p->samples, S_all * kSample * 4);
+  const size_t o_mask = seeded ? St.put(inlier_mask, N) : 0;
   stage_rigs(St, p, in);
   const size_t o_ref = St.put(ref_model, (size_t)n_prob * 96);
   const size_t in_bytes = St.h.size();
-  const size_t o_cov = St.reserve((size_t)n_prob * 288), o_nv = St.reserve((size_t)n_prob * 4), o_d = St.reserve(S_all * 48), o_v = St.reserve(S_all);
+  const size_t o_cov = St.reserve((size_t)n_prob * 288), o_nv = St.reserve((size_t)n_prob * 4), o_d = St.reserve(S_all * 48), o_v = St.reserve(S_all),
+               o_dr = drawn ? St.reserve(S_all * kSample * 4) : 0;
   const size_t total = St.h.size();
   unsigned char* d = (unsigned char*)cvb_ws(ctx, WS_GS6, total);
   unsigned char* hpin = (unsigned char*)cvb_pinned(ctx, total);
   if (!d || !hpin) return CVB_ERR_CUDA;
   memcpy(hpin, St.h.data(), in_bytes);
-  CovDev D{};
+  CovSeededDev D{};   // the sample-supplied solve and the reduce take its CovDev part
   D.prob_ptr = (const int*)(d + in.ptr); D.f1 = (const double*)(d + in.f1); D.f2 = (const double*)(d + in.f2);
   D.cam1 = (const int*)(d + in.c1); D.cam2 = (const int*)(d + in.c2); D.cam_ptr1 = (const int*)(d + in.cp1); D.cam_ptr2 = (const int*)(d + in.cp2);
-  D.rig1 = (const double*)(d + in.rig1); D.rig2 = (const double*)(d + in.rig2); D.samples = (const int*)(d + in.smp);
+  D.rig1 = (const double*)(d + in.rig1); D.rig2 = (const double*)(d + in.rig2);
+  if (seeded) {
+    D.seed = (const unsigned long long*)(d + in.smp); D.mask = d + o_mask; D.drawn = drawn ? (int*)(d + o_dr) : nullptr;
+  } else {
+    D.samples = (const int*)(d + in.smp);
+  }
   D.ref_model = (const double*)(d + o_ref);
   D.n_samples = ns; D.ctas_per_prob = (ns + kCovPerCta - 1) / kCovPerCta;
   D.delta = (double*)(d + o_d); D.valid = d + o_v; D.cov = (double*)(d + o_cov); D.n_valid = (int*)(d + o_nv);
   cudaStream_t st = ctx->stream;
   CVB_CUDA(ctx, cudaMemcpyAsync(d, hpin, in_bytes, cudaMemcpyHostToDevice, st));
+  if (drawn) CVB_CUDA(ctx, cudaMemsetAsync(d + o_dr, 0xff, S_all * kSample * 4, st));
   if (ns > 0) {
     const long long grid = (long long)n_prob * D.ctas_per_prob;
-    CVB_REQUIRE(ctx, grid <= INT32_MAX, "noncentral_relative_pose_covariance: %lld solve CTAs exceed the grid limit", grid);
+    CVB_REQUIRE(ctx, grid <= INT32_MAX, "%s: %lld solve CTAs exceed the grid limit", name, grid);
     constexpr int kSolveWarps = kCovPerCta < kWarps ? kCovPerCta : kWarps;
-    rel_cov_solve_kernel<<<(unsigned)grid, 32 * kSolveWarps, (size_t)kSolveWarps * kSolveArea * sizeof(double), st>>>(D);
+    const size_t smem = (size_t)kSolveWarps * kSolveArea * sizeof(double);
+    if (seeded) rel_cov_solve_kernel<CovSeededDev><<<(unsigned)grid, 32 * kSolveWarps, smem, st>>>(D);
+    else rel_cov_solve_kernel<CovDev><<<(unsigned)grid, 32 * kSolveWarps, smem, st>>>(static_cast<const CovDev&>(D));
     CVB_CHECK_LAUNCH(ctx);
   }
-  rel_cov_reduce_kernel<<<n_prob, kCovReduceThreads, 0, st>>>(D);
+  rel_cov_reduce_kernel<<<n_prob, kCovReduceThreads, 0, st>>>(static_cast<const CovDev&>(D));
   CVB_CHECK_LAUNCH(ctx);
-  CVB_CUDA(ctx, cudaMemcpyAsync(hpin + o_cov, d + o_cov, (all ? total : o_d) - o_cov, cudaMemcpyDeviceToHost, st));
+  CVB_CUDA(ctx, cudaMemcpyAsync(hpin + o_cov, d + o_cov, (all || drawn ? total : o_d) - o_cov, cudaMemcpyDeviceToHost, st));
   CVB_CUDA(ctx, cudaStreamSynchronize(st));
   memcpy(r->cov, hpin + o_cov, (size_t)n_prob * 288); memcpy(r->n_valid, hpin + o_nv, (size_t)n_prob * 4);
   if (all) { memcpy(r->sample_delta, hpin + o_d, S_all * 48); memcpy(r->sample_valid, hpin + o_v, S_all); }
+  if (drawn) memcpy(drawn, hpin + o_dr, S_all * kSample * 4);
   return CVB_OK;
+}
+
+}  // namespace
+
+extern "C" int cvb_noncentral_relative_pose_covariance_batch(cvb_ctx* ctx, const cvb_rel_ransac_problems* p, const double* ref_model,
+                                                             cvb_rel_cov_result* r) {
+  if (!ctx) return CVB_ERR_INVALID;
+  CVB_GUARD(ctx);
+  return rel_cov(ctx, "noncentral_relative_pose_covariance", p, ref_model, false, nullptr, nullptr, r, nullptr);
+}
+
+extern "C" int cvb_noncentral_relative_pose_covariance_seeded_batch(cvb_ctx* ctx, const cvb_rel_ransac_problems* p, const double* ref_model,
+                                                                    const uint8_t* inlier_mask, const uint64_t* seed, cvb_rel_cov_result* r,
+                                                                    int32_t* drawn) {
+  if (!ctx) return CVB_ERR_INVALID;
+  CVB_GUARD(ctx);
+  return rel_cov(ctx, "noncentral_relative_pose_covariance_seeded", p, ref_model, true, inlier_mask, seed, r, drawn);
 }

@@ -11,6 +11,8 @@ the C-ABI:
   ransac_central_relative_pose(...) ↔ the 5-point RANSAC of RelNonCentralPosSolver::computePose from caller-supplied samples
   relative_pose_covariance(...) ↔ the sampling-based 6x6 covariance of RelNonCentralPosSolver::computeNonCentralRelPose (17-point
                                   re-solves from caller-supplied samples)
+  ransac_*_seeded(...), relative_pose_covariance_seeded(...) ↔ the same calls with the samples drawn on the GPU from one seed
+                                  per problem, as the reference draws its own (include/covins_b200.h, "Seeded samples")
 
 `KfView` flattens what the reference reads of a Keyframe (the C++ shim does the same from the containers)."""
 from __future__ import annotations
@@ -183,16 +185,30 @@ class CRansacResult(C.Structure):
 CAbsRansacResult = CRelRansacResult = CRansacResult   # the names of the per-call result structs, kept for existing callers
 
 
-def _ransac(ctx, fn, P, n_prob, ns, n, threshold, max_iterations, probability, per_sample):
-    """one RANSAC call fn on the problems P (n_prob problems, ns samples each, n correspondences) → its result dict"""
+def _ransac(ctx, fn, P, n_prob, ns, n, threshold, max_iterations, probability, per_sample, seeds=None, k=0, want_drawn=False):
+    """one RANSAC call fn on the problems P (n_prob problems, ns samples each, n correspondences) → its result dict; with seeds
+    (a seeded call fn, sample size k) also drawn [n_prob, ns, k] when want_drawn"""
     r = dict(best_sample=np.zeros(n_prob, np.int32), best_model=np.zeros((n_prob, 3, 4)), best_count=np.zeros(n_prob, np.int32),
              iterations=np.zeros(n_prob, np.int32), consumed=np.zeros(n_prob, np.int32), inlier_mask=np.zeros(n, np.uint8))
     if per_sample:
         r.update(sample_model=np.zeros((n_prob, ns, 3, 4)), sample_valid=np.zeros((n_prob, ns), np.uint8),
                  sample_count=np.zeros((n_prob, ns), np.int32))
     R = CRansacResult(*[r[k].ctypes.data if k in r else None for k, _ in CRansacResult._fields_])
-    ctx.check(fn(ctx.handle, C.byref(P), float(threshold), int(max_iterations), float(probability), C.byref(R)))
+    if seeds is None:
+        ctx.check(fn(ctx.handle, C.byref(P), float(threshold), int(max_iterations), float(probability), C.byref(R)))
+        return r
+    if want_drawn:
+        r["drawn"] = np.full((n_prob, ns, k), -1, np.int32)
+    ctx.check(fn(ctx.handle, C.byref(P), seeds.ctypes.data, float(threshold), int(max_iterations), float(probability), C.byref(R),
+                 r["drawn"].ctypes.data if want_drawn else None))
     return r
+
+
+def _seeds(seeds, n_prob):
+    s = np.ascontiguousarray(seeds, np.uint64).reshape(-1)
+    if len(s) != n_prob:
+        raise ValueError(f"{len(s)} seeds for {n_prob} problems")
+    return s
 
 
 def ransac_absolute_pose(ctx: Context, prob_ptr, pts, bearings, sigma, cam_off, cam_rot, samples, threshold, max_iterations, probability=0.99,
@@ -209,6 +225,20 @@ def ransac_absolute_pose(ctx: Context, prob_ptr, pts, bearings, sigma, cam_off, 
     smp = np.ascontiguousarray(samples, np.int32).reshape(n_prob, -1, 4); ns = smp.shape[1]
     P = CAbsRansacProblems(n_prob, ptr.ctypes.data, p.ctypes.data, f.ctypes.data, s.ctypes.data, co.ctypes.data, cr.ctypes.data, smp.ctypes.data, ns)
     return _ransac(ctx, lib().cvb_ransac_absolute_pose_batch, P, n_prob, ns, len(p), threshold, max_iterations, probability, per_sample)
+
+
+def ransac_absolute_pose_seeded(ctx: Context, prob_ptr, pts, bearings, sigma, cam_off, cam_rot, seeds, threshold, max_iterations, probability=0.99,
+                                per_sample=False, n_samples=0, want_drawn=False):
+    """ransac_absolute_pose with the samples drawn on the GPU (cvb_ransac_absolute_pose_seeded_batch): seeds [n_prob] uint64, one per
+    problem; the selection draws until opengv's bound ends it.  n_samples sizes the per-sample outputs (per_sample) and drawn
+    [n_prob, n_samples, 4] (want_drawn: the drawn indices, -1 where not drawn)."""
+    ptr = np.ascontiguousarray(prob_ptr, np.int32); n_prob = len(ptr) - 1
+    p = np.ascontiguousarray(pts, np.float64).reshape(-1, 3); f = np.ascontiguousarray(bearings, np.float64).reshape(-1, 3)
+    s = np.ascontiguousarray(sigma, np.float64).reshape(-1)
+    co = np.ascontiguousarray(cam_off, np.float64).reshape(n_prob, 3); cr = np.ascontiguousarray(cam_rot, np.float64).reshape(n_prob, 9)
+    P = CAbsRansacProblems(n_prob, ptr.ctypes.data, p.ctypes.data, f.ctypes.data, s.ctypes.data, co.ctypes.data, cr.ctypes.data, None, int(n_samples))
+    return _ransac(ctx, lib().cvb_ransac_absolute_pose_seeded_batch, P, n_prob, int(n_samples), len(p), threshold, max_iterations, probability,
+                   per_sample, _seeds(seeds, n_prob), 4, want_drawn)
 
 
 class CRelRansacProblems(C.Structure):
@@ -237,6 +267,23 @@ def ransac_noncentral_relative_pose(ctx: Context, prob_ptr, f1, f2, sigma1, sigm
     return _ransac(ctx, lib().cvb_ransac_noncentral_relative_pose_batch, P, n_prob, ns, len(a), threshold, max_iterations, probability, per_sample)
 
 
+def ransac_noncentral_relative_pose_seeded(ctx: Context, prob_ptr, f1, f2, sigma1, sigma2, cam1, cam2, cam_ptr1, cam_off1, cam_rot1, cam_ptr2,
+                                           cam_off2, cam_rot2, seeds, threshold, max_iterations, probability=0.99, per_sample=False, n_samples=0,
+                                           want_drawn=False):
+    """ransac_noncentral_relative_pose with the samples drawn on the GPU (cvb_ransac_noncentral_relative_pose_seeded_batch); seeds,
+    n_samples and want_drawn as ransac_absolute_pose_seeded (drawn [n_prob, n_samples, 17])."""
+    ptr = np.ascontiguousarray(prob_ptr, np.int32); n_prob = len(ptr) - 1
+    a = np.ascontiguousarray(f1, np.float64).reshape(-1, 3); b = np.ascontiguousarray(f2, np.float64).reshape(-1, 3)
+    s1 = np.ascontiguousarray(sigma1, np.float64).reshape(-1); s2 = np.ascontiguousarray(sigma2, np.float64).reshape(-1)
+    c1 = np.ascontiguousarray(cam1, np.int32).reshape(-1); c2 = np.ascontiguousarray(cam2, np.int32).reshape(-1)
+    cp1 = np.ascontiguousarray(cam_ptr1, np.int32); cp2 = np.ascontiguousarray(cam_ptr2, np.int32)
+    co1 = np.ascontiguousarray(cam_off1, np.float64).reshape(-1, 3); cr1 = np.ascontiguousarray(cam_rot1, np.float64).reshape(-1, 9)
+    co2 = np.ascontiguousarray(cam_off2, np.float64).reshape(-1, 3); cr2 = np.ascontiguousarray(cam_rot2, np.float64).reshape(-1, 9)
+    P = CRelRansacProblems(n_prob, *[x.ctypes.data for x in (ptr, a, b, s1, s2, c1, c2, cp1, co1, cr1, cp2, co2, cr2)], None, int(n_samples))
+    return _ransac(ctx, lib().cvb_ransac_noncentral_relative_pose_seeded_batch, P, n_prob, int(n_samples), len(a), threshold, max_iterations,
+                   probability, per_sample, _seeds(seeds, n_prob), 17, want_drawn)
+
+
 class CCentralRelRansacProblems(C.Structure):
     _fields_ = [("n_prob", C.c_int32)] + [(k, c_vp) for k in ("prob_ptr", "f1", "f2", "sigma1", "sigma2", "samples")] + [("n_samples", C.c_int32)]
 
@@ -254,6 +301,18 @@ def ransac_central_relative_pose(ctx: Context, prob_ptr, f1, f2, sigma1, sigma2,
     smp = np.ascontiguousarray(samples, np.int32).reshape(n_prob, -1, 5); ns = smp.shape[1]
     P = CCentralRelRansacProblems(n_prob, *[x.ctypes.data for x in (ptr, a, b, s1, s2, smp)], ns)
     return _ransac(ctx, lib().cvb_ransac_central_relative_pose_batch, P, n_prob, ns, len(a), threshold, max_iterations, probability, per_sample)
+
+
+def ransac_central_relative_pose_seeded(ctx: Context, prob_ptr, f1, f2, sigma1, sigma2, seeds, threshold, max_iterations, probability=0.99,
+                                        per_sample=False, n_samples=0, want_drawn=False):
+    """ransac_central_relative_pose with the samples drawn on the GPU (cvb_ransac_central_relative_pose_seeded_batch); seeds,
+    n_samples and want_drawn as ransac_absolute_pose_seeded (drawn [n_prob, n_samples, 5])."""
+    ptr = np.ascontiguousarray(prob_ptr, np.int32); n_prob = len(ptr) - 1
+    a = np.ascontiguousarray(f1, np.float64).reshape(-1, 3); b = np.ascontiguousarray(f2, np.float64).reshape(-1, 3)
+    s1 = np.ascontiguousarray(sigma1, np.float64).reshape(-1); s2 = np.ascontiguousarray(sigma2, np.float64).reshape(-1)
+    P = CCentralRelRansacProblems(n_prob, *[x.ctypes.data for x in (ptr, a, b, s1, s2)], None, int(n_samples))
+    return _ransac(ctx, lib().cvb_ransac_central_relative_pose_seeded_batch, P, n_prob, int(n_samples), len(a), threshold, max_iterations,
+                   probability, per_sample, _seeds(seeds, n_prob), 5, want_drawn)
 
 
 class CRelCovResult(C.Structure):
@@ -285,4 +344,32 @@ def relative_pose_covariance(ctx: Context, prob_ptr, f1, f2, cam1, cam2, cam_ptr
                            *[x.ctypes.data for x in (c1, c2, cp1, co1, cr1, cp2, co2, cr2, smp)], ns)
     R = CRelCovResult(*[r[k].ctypes.data if k in r else None for k, _ in CRelCovResult._fields_])
     ctx.check(lib().cvb_noncentral_relative_pose_covariance_batch(ctx.handle, C.byref(P), ref.ctypes.data, C.byref(R)))
+    return r
+
+
+def relative_pose_covariance_seeded(ctx: Context, prob_ptr, f1, f2, cam1, cam2, cam_ptr1, cam_off1, cam_rot1, cam_ptr2, cam_off2, cam_rot2,
+                                    inlier_mask, seeds, ref_model, n_samples=300, per_sample=False, want_drawn=False, sigma1=None, sigma2=None):
+    """relative_pose_covariance with the samples drawn on the GPU (cvb_noncentral_relative_pose_covariance_seeded_batch): n_samples
+    17-point subsets per problem of its inliers in inlier_mask [N] (normally the RANSAC's), drawn from seeds [n_prob] uint64.
+    A problem with fewer than 17 inliers or a zero ref_model gets n_valid 0.  want_drawn: also drawn [n_prob, n_samples, 17], the
+    problem-local correspondence indices (-1 where not drawn)."""
+    ptr = np.ascontiguousarray(prob_ptr, np.int32); n_prob = len(ptr) - 1
+    a = np.ascontiguousarray(f1, np.float64).reshape(-1, 3); b = np.ascontiguousarray(f2, np.float64).reshape(-1, 3)
+    c1 = np.ascontiguousarray(cam1, np.int32).reshape(-1); c2 = np.ascontiguousarray(cam2, np.int32).reshape(-1)
+    cp1 = np.ascontiguousarray(cam_ptr1, np.int32); cp2 = np.ascontiguousarray(cam_ptr2, np.int32)
+    co1 = np.ascontiguousarray(cam_off1, np.float64).reshape(-1, 3); cr1 = np.ascontiguousarray(cam_rot1, np.float64).reshape(-1, 9)
+    co2 = np.ascontiguousarray(cam_off2, np.float64).reshape(-1, 3); cr2 = np.ascontiguousarray(cam_rot2, np.float64).reshape(-1, 9)
+    mask = np.ascontiguousarray(inlier_mask, np.uint8).reshape(-1)
+    ref = np.ascontiguousarray(ref_model, np.float64).reshape(n_prob, 12)
+    seeds = _seeds(seeds, n_prob); ns = int(n_samples)
+    r = dict(cov=np.zeros((n_prob, 6, 6)), n_valid=np.zeros(n_prob, np.int32))
+    if per_sample:
+        r.update(sample_delta=np.zeros((n_prob, ns, 6)), sample_valid=np.zeros((n_prob, ns), np.uint8))
+    if want_drawn:
+        r["drawn"] = np.full((n_prob, ns, 17), -1, np.int32)
+    P = CRelRansacProblems(n_prob, ptr.ctypes.data, a.ctypes.data, b.ctypes.data, None, None,
+                           *[x.ctypes.data for x in (c1, c2, cp1, co1, cr1, cp2, co2, cr2)], None, ns)
+    R = CRelCovResult(*[r[k].ctypes.data if k in r else None for k, _ in CRelCovResult._fields_])
+    ctx.check(lib().cvb_noncentral_relative_pose_covariance_seeded_batch(ctx.handle, C.byref(P), ref.ctypes.data, mask.ctypes.data, seeds.ctypes.data,
+                                                                         C.byref(R), r["drawn"].ctypes.data if want_drawn else None))
     return r

@@ -524,6 +524,48 @@ CVB_API int cvb_noncentral_relative_pose_covariance_batch(cvb_ctx* ctx, const cv
                                                           cvb_rel_cov_result* r);
 
 /*
+ * Seeded samples: the four calls above with the samples drawn on the device from one 64-bit seed per problem, so the call
+ * sites need no sampler of their own (opengv draws inside Ransac::computeModel, and computeNonCentralRelPose draws its
+ * covariance subsets itself, RelNonCentralPosSolver.cpp:199,236).
+ *   Sampler (this project's own definition; oracle/sampler_oracle.c restates it):
+ *     Generator: Philox4x64-10 (Salmon et al., SC'11), the bit generator of numpy.random.Philox, with key (seed_p, stream):
+ *     seed_p the problem's seed, stream 0 for RANSAC samples and 1 for covariance samples (one seed per candidate serves
+ *     both).  Sample s of a problem uses counters (s, b, 0, 0), b = 0, 1, ...; each block gives four 64-bit words, each
+ *     word two 32-bit values, low half first: the stream u_0, u_1, ...  (One block serves sample sizes 4 and 5, three serve 17.)
+ *     Ordered k-subset of [0, m): a partial Fisher-Yates shuffle of the identity permutation; for i = 0 .. k-1,
+ *     j = i + (uint32)(((uint64)u_i * (m - i)) >> 32), swap perm[i] and perm[j], sample[i] = perm[i].  A sample never repeats
+ *     an index.  A problem's samples depend only on (seed_p, stream, m, k, s): it gives the same results alone or anywhere
+ *     in a batch, and sample s is drawn without drawing samples 0 .. s-1.
+ *     ASSUMPTION (opengv's std::mt19937 is seeded from the clock, so no reference run can be replayed): only the
+ *     distribution is kept.  Like opengv's shuffle, the subsets are uniform up to a bias of at most m / 2^32.
+ *   RANSAC (m = n, indices local to the problem): the selection of the sample-supplied call, never limited by a sample
+ *   count: samples are drawn until opengv's bound ends it (max_iterations valid samples, the adaptive bound, or
+ *   10 * max_iterations skipped).  A problem with fewer than k correspondences (4, 17, 5) draws nothing: iterations =
+ *   consumed = 0, best_sample = -1 (opengv's getSamples returns an empty selection and computeModel stops).  p->samples must
+ *   be NULL; p->n_samples only sizes the optional per-sample outputs (sample_model / sample_valid / sample_count, which
+ *   cover samples 0 .. n_samples-1 whether or not the selection reads them) and drawn.
+ *   Covariance (m = the problem's number of inliers in inlier_mask [N]; index j of a subset means the j-th inlier in
+ *   ascending correspondence order): p->n_samples subsets per problem (the reference's 300).  A problem with fewer than 17
+ *   inliers, or with an all-zero ref_model, draws nothing and gets n_valid = 0.
+ *   drawn (nullable): [n_prob][n_samples][k] the drawn samples as problem-local correspondence indices, -1 in the rows that
+ *   were not drawn.
+ * Errors: those of the sample-supplied twin except the sample-index check, and CVB_ERR_INVALID before any launch for a
+ * non-null p->samples, a null seed with n_prob > 0, (covariance) a null inlier_mask, or (RANSAC) max_iterations above
+ * (INT32_MAX - 64) / 11, so that every sample number the selection can reach (at most 11 * max_iterations) fits an int32.
+ */
+CVB_API int cvb_ransac_absolute_pose_seeded_batch(cvb_ctx* ctx, const cvb_abs_ransac_problems* p, const uint64_t* seed, double threshold,
+                                                  int max_iterations, double probability, cvb_abs_ransac_result* r, int32_t* drawn);
+CVB_API int cvb_ransac_noncentral_relative_pose_seeded_batch(cvb_ctx* ctx, const cvb_rel_ransac_problems* p, const uint64_t* seed,
+                                                             double threshold, int max_iterations, double probability,
+                                                             cvb_rel_ransac_result* r, int32_t* drawn);
+CVB_API int cvb_ransac_central_relative_pose_seeded_batch(cvb_ctx* ctx, const cvb_central_rel_ransac_problems* p, const uint64_t* seed,
+                                                          double threshold, int max_iterations, double probability,
+                                                          cvb_rel_ransac_result* r, int32_t* drawn);
+CVB_API int cvb_noncentral_relative_pose_covariance_seeded_batch(cvb_ctx* ctx, const cvb_rel_ransac_problems* p, const double* ref_model,
+                                                                 const uint8_t* inlier_mask, const uint64_t* seed, cvb_rel_cov_result* r,
+                                                                 int32_t* drawn);
+
+/*
  * Optimization::OptimizeRelativePose(kf1, kf2, matches1, T12, th2) (optimization_be.cpp:620-831): the 6-dof refinement of
  * the relative pose T12 from the matched landmark pairs, both ceres::Solve calls (5 + 5 iterations, DOGLEG, CauchyLoss(1))
  * and the outlier purge between them, in one call.  The caller (shim) flattens, per residual pair r (the reference's

@@ -20,7 +20,13 @@ With --covariance, the sampling-based 6x6 covariance of the non-central relative
   (a) cvb_noncentral_relative_pose_covariance_batch (whole call, and the device time of its two kernels from torch.profiler);
   (c) the oracle on one host thread and on all host cores (OpenMP over the samples).
 Every result of a timed call is checked bit-identical to the oracle.
-  python tools/ransac_timing.py [--reps 100] [--outlier 0.5] [--relative | --central | --covariance]"""
+With --seeded, each of the four calls in its seeded form (samples drawn on the GPU from one seed per problem) against the
+sample-supplied form given the same samples (the first --samples the seeded call drew; the covariance: 300 drawn from the
+true inliers), timed alternately in one session at the sizes above (absolute: 1, 8, 32 x 1000; 17-point: 5 % and 30 % outliers
+x 1, 8, 32; 5-point: 1000 correspondences, 5 % and 30 % x 1, 6, 60; covariance: 1, 8, 32): the whole call (host clock around
+the synchronous call, median of --reps) and its kernels' device time (torch.profiler).  Both calls' results are checked
+identical.
+  python tools/ransac_timing.py [--reps 100] [--outlier 0.5] [--relative | --central | --covariance | --seeded]"""
 import argparse
 import os
 import subprocess
@@ -43,7 +49,10 @@ def main():
     ap.add_argument("--relative", action="store_true", help="time the non-central relative-pose (17-point) RANSAC")
     ap.add_argument("--central", action="store_true", help="time the central relative-pose (5-point) RANSAC")
     ap.add_argument("--covariance", action="store_true", help="time the non-central relative pose's sampling-based covariance")
+    ap.add_argument("--seeded", action="store_true", help="time the seeded calls against the sample-supplied ones")
     a = ap.parse_args()
+    if a.seeded:
+        return seeded(a)
     if a.covariance:
         return covariance(a)
     if a.relative:
@@ -254,6 +263,79 @@ def covariance(a):
         print(f"covariance | n_prob {n_prob:2d} x {a.n} corr, {ns} samples, valid {want['n_valid'].min()}-{want['n_valid'].max()} | "
               f"(a) call {t_a:.3f} ms, kernels {k_solve + k_red:.3f} ms (solve {k_solve:.3f}, reduce {k_red:.3f}) | (c) oracle on 1 host "
               f"thread {t_c[1]:.2f} ms, on {os.cpu_count()} host cores {t_c[0]:.2f} ms | bit-identical to the oracle")
+    ctx.close()
+
+
+def seeded(a):
+    import torch
+    import covins_b200
+    from covins_b200 import placerec as PR
+    import test_ransac_absolute as TA
+    import test_ransac_central as TC
+    import test_ransac_relative as TR
+    import test_relpose_covariance as TV
+    from torch.profiler import profile, ProfilerActivity
+    assert torch.cuda.is_available(), "needs a CUDA device"
+    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"], capture_output=True, text=True)
+    print(f"GPU: {torch.cuda.get_device_name(0)} | {q.stdout.strip()}")
+    ctx = covins_b200.Context(0)
+    drop = lambda b: {k: v for k, v in b.items() if k != "samples"}
+    ns, max_it = a.samples, 300
+
+    def compare(label, seeded_call, supplied_call, kernel_names):
+        got_s, got_p = seeded_call(), supplied_call()
+        for k in got_p:
+            assert np.array_equal(np.ascontiguousarray(got_s[k]).view(np.uint8), np.ascontiguousarray(got_p[k]).view(np.uint8)), (label, k)
+        t = {"seeded": [], "supplied": []}
+        for _ in range(3):
+            seeded_call(); supplied_call()
+        for _ in range(a.reps):                       # alternately
+            for key, fn in (("seeded", seeded_call), ("supplied", supplied_call)):
+                t0 = time.perf_counter(); fn(); t[key].append((time.perf_counter() - t0) * 1e3)
+        kern = {}
+        for key, fn in (("seeded", seeded_call), ("supplied", supplied_call)):
+            with profile(activities=[ProfilerActivity.CUDA]) as pr:
+                for _ in range(10):
+                    fn()
+            ev = [e for e in pr.events() if kernel_names[key](e.name)]
+            kern[key] = np.sum([e.device_time for e in ev]) / 10 / 1e3
+        it = got_s.get("iterations")
+        extra = f" | iterations {it.min()}-{it.max()}" if it is not None else f" | valid {got_s['n_valid'].min()}-{got_s['n_valid'].max()}"
+        print(f"{label}{extra} | call: seeded {np.median(t['seeded']):.3f} ms, supplied {np.median(t['supplied']):.3f} ms | kernels: seeded "
+              f"{kern['seeded']:.3f} ms, supplied {kern['supplied']:.3f} ms | identical")
+
+    def ransac(label, gpu_seeded, gpu_supplied, b, n_prob, thr, k_names):
+        seeds = np.arange(1, n_prob + 1, dtype=np.uint64) * np.uint64(0x9E3779B97F4A7C15)
+        kw = dict(threshold=thr, max_iterations=max_it, probability=0.99)
+        drawn = gpu_seeded(ctx, **b, seeds=seeds, **kw, per_sample=True, n_samples=ns, want_drawn=True)["drawn"]
+        compare(label, lambda: gpu_seeded(ctx, **b, seeds=seeds, **kw), lambda: gpu_supplied(ctx, **b, samples=drawn, **kw),
+                {"seeded": lambda s: "Seeded" in s, "supplied": lambda s: "Supplied" in s})
+
+    for n_prob in (1, 8, 32):
+        b = drop(TA._batch(100 + n_prob, [a.n] * n_prob, 10, outlier_frac=a.outlier)[0])
+        ransac(f"absolute | n_prob {n_prob:2d} x {a.n}, outliers {a.outlier:.0%}", PR.ransac_absolute_pose_seeded, PR.ransac_absolute_pose, b, n_prob, 25.0,
+               None)
+    for outlier in (0.05, 0.3):
+        for n_prob in (1, 8, 32):
+            b = drop(TR._batch(200 + n_prob, [(a.n, 3, 3, False)] * n_prob, 1, outlier_frac=outlier, repeat_frac=0.0)[0])
+            ransac(f"17-point | n_prob {n_prob:2d} x {a.n}, outliers {outlier:.0%}", PR.ransac_noncentral_relative_pose_seeded,
+                   PR.ransac_noncentral_relative_pose, b, n_prob, 9.0, None)
+    for outlier in (0.05, 0.3):
+        for n_prob in (1, 6, 60):
+            b = drop(TC._batch(300 + n_prob, [(a.n, outlier, False)] * n_prob, 1, repeat_frac=0.0)[0])
+            ransac(f"5-point | n_prob {n_prob:2d} x {a.n}, outliers {outlier:.0%}", PR.ransac_central_relative_pose_seeded, PR.ransac_central_relative_pose,
+                   b, n_prob, 9.0, None)
+    for n_prob in (1, 8, 32):
+        b, probs = TV._batch(400 + n_prob, [(a.n, 3, 3, False)] * n_prob, 1, noise=1e-3, outlier_frac=0.3)
+        b = drop(b)
+        mask = np.concatenate([p["inlier"] for p in probs]).astype(np.uint8)
+        ref = TV._truth(probs)
+        seeds = np.arange(1, n_prob + 1, dtype=np.uint64)
+        drawn = PR.relative_pose_covariance_seeded(ctx, **b, inlier_mask=mask, seeds=seeds, ref_model=ref, n_samples=300, want_drawn=True)["drawn"]
+        compare(f"covariance | n_prob {n_prob:2d} x {a.n}, 300 samples",
+                lambda: PR.relative_pose_covariance_seeded(ctx, **b, inlier_mask=mask, seeds=seeds, ref_model=ref, n_samples=300),
+                lambda: PR.relative_pose_covariance(ctx, **b, samples=drawn, ref_model=ref),
+                {"seeded": lambda s: "rel_cov_" in s and "CovDev>" not in s, "supplied": lambda s: "rel_cov_" in s and "CovSeededDev" not in s})
     ctx.close()
 
 
