@@ -57,6 +57,12 @@ int cvb_fail(cvb_ctx* ctx, int code, const char* fmt, ...);
 void* cvb_ws(cvb_ctx* ctx, int slot, size_t bytes);          // returns nullptr on failure (ctx->err set)
 void* cvb_pinned(cvb_ctx* ctx, size_t bytes);
 
+// match_kernels.cu: the fused 2-NN + ratio filter of cvb_match_hamming_batch for n_pairs pairs of keyframes of one device
+// descriptor table d_desc in one launch on ctx->stream.  d_pairs [n_pairs][5] = (query row0, query rows, train row0, train rows,
+// output offset); pair s writes match_train / match_dist [offset + query] and n_matches [s]; max_nq: the largest query count.
+int cvb_match_hamming_pairs_dev(cvb_ctx* ctx, const uint8_t* d_desc, const int32_t* d_pairs, int n_pairs, int max_nq, float thr, float ratio,
+                                int32_t* d_match_train, float* d_match_dist, int32_t* d_n_matches);
+
 #define CVB_CUDA(ctx, call)                                                                         \
   do {                                                                                              \
     cudaError_t e_ = (call);                                                                        \

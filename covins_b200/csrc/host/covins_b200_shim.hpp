@@ -1148,6 +1148,100 @@ inline std::vector<NonCentralRelativePoseRansacResult> RansacNonCentralRelativeP
                                                                    max_iterations, probability);
 }
 
+// RelNonCentralPosSolver::computeNonCentralRelPose's whole verification of a query keyframe's candidates in one call
+// (cvb_verify_noncentral_relative_pose_seeded_batch): per pairing the ORB matching and a seeded 5-point RANSAC, per candidate a
+// seeded 17-point RANSAC on the pairings' 5-point inliers and the seeded covariance, with one upload and one download.
+// keyframes: flat views of every keyframe the rigs use (n rows of descriptors_add_ [32], bearings_add_ [3] and sigma each);
+// a pairing names two of them and their cameras in the candidate's rigs.  One seed per pairing (seeds5) and per candidate.
+struct VerifyKeyframeView {
+  const uint8_t* desc; const double* bearings; const double* sigma; int n;
+};
+struct VerifyPairing { int kf1, kf2, cam1, cam2; };
+struct VerifyCandidate {
+  std::vector<double> rig1_offsets, rig1_rotations, rig2_offsets, rig2_rotations;   // 3 / 9 (row-major) per camera
+  std::vector<VerifyPairing> pairings;
+};
+struct VerifyParams {
+  float img_match_thres = 0.f, ratio_thres = 0.f;
+  double threshold5 = 0.0; int max_iterations5 = 0;
+  double threshold17 = 0.0; int max_iterations17 = 0;
+  double probability = 0.99; int n_cov_samples = 300;
+};
+struct VerifyPairingResult {
+  int n_matches = 0, best_sample = -1, n_inliers = 0, iterations = 0, samples_used = 0;
+  std::array<double, 12> model{};   // 5-point [R|t], |t| = 1
+};
+struct VerifyCandidateResult {
+  int best_sample = -1, n_inliers = 0, iterations = 0, samples_used = 0, n_valid = 0;
+  std::array<double, 12> model{};   // 17-point [R|t], X1 = R X2 + t (rig frames)
+  std::array<double, 36> cov{};
+};
+struct VerifyCorrespondence { int pairing, row1, row2, inlier5, inlier17; };
+struct VerifyResult {
+  std::vector<VerifyPairingResult> pairings;            // all candidates' pairings in order
+  std::vector<VerifyCandidateResult> candidates;
+  std::vector<VerifyCorrespondence> correspondences;    // every match, pairing then match order
+};
+inline VerifyResult VerifyNonCentralRelativePose(Context& ctx, const std::vector<VerifyKeyframeView>& keyframes,
+                                                 const std::vector<VerifyCandidate>& candidates, const VerifyParams& params,
+                                                 const std::vector<uint64_t>& seeds5, const std::vector<uint64_t>& seeds) {
+  const int n_kf = (int)keyframes.size(), C = (int)candidates.size();
+  std::vector<int32_t> kf_ptr(n_kf + 1, 0), cp1(C + 1, 0), cp2(C + 1, 0), pair_ptr(C + 1, 0), pairs;
+  std::vector<uint8_t> desc;
+  std::vector<double> bear, sig, co1, cr1, co2, cr2;
+  for (int k = 0; k < n_kf; k++) {
+    const VerifyKeyframeView& v = keyframes[k];
+    kf_ptr[k + 1] = kf_ptr[k] + v.n;
+    desc.insert(desc.end(), v.desc, v.desc + 32 * (size_t)v.n);
+    bear.insert(bear.end(), v.bearings, v.bearings + 3 * (size_t)v.n);
+    sig.insert(sig.end(), v.sigma, v.sigma + v.n);
+  }
+  size_t bound = 0;
+  for (int c = 0; c < C; c++) {
+    const VerifyCandidate& cd = candidates[c];
+    if (cd.rig1_rotations.size() != 3 * cd.rig1_offsets.size() || cd.rig2_rotations.size() != 3 * cd.rig2_offsets.size() ||
+        cd.rig1_offsets.size() % 3 || cd.rig2_offsets.size() % 3)
+      throw std::invalid_argument("covins_b200::VerifyNonCentralRelativePose: inconsistent rig sizes");
+    cp1[c + 1] = cp1[c] + (int32_t)(cd.rig1_offsets.size() / 3); cp2[c + 1] = cp2[c] + (int32_t)(cd.rig2_offsets.size() / 3);
+    co1.insert(co1.end(), cd.rig1_offsets.begin(), cd.rig1_offsets.end()); cr1.insert(cr1.end(), cd.rig1_rotations.begin(), cd.rig1_rotations.end());
+    co2.insert(co2.end(), cd.rig2_offsets.begin(), cd.rig2_offsets.end()); cr2.insert(cr2.end(), cd.rig2_rotations.begin(), cd.rig2_rotations.end());
+    pair_ptr[c + 1] = pair_ptr[c] + (int32_t)cd.pairings.size();
+    for (const VerifyPairing& q : cd.pairings) {
+      pairs.insert(pairs.end(), {q.kf1, q.kf2, q.cam1, q.cam2});
+      if (q.kf1 >= 0 && q.kf1 < n_kf) bound += (size_t)keyframes[q.kf1].n;
+    }
+  }
+  const int P = pair_ptr[C];
+  if (seeds5.size() != (size_t)P || seeds.size() != (size_t)C)
+    throw std::invalid_argument("covins_b200::VerifyNonCentralRelativePose: one seed per pairing and per candidate");
+  std::vector<int32_t> nm(P), bs5(P), bc5(P), it5(P), us5(P), bs(C), bc(C), it(C), us(C), nv(C), corr(5 * bound);
+  std::vector<double> bm5(12 * (size_t)P), bm(12 * (size_t)C), cov(36 * (size_t)C);
+  cvb_verify_keyframes K{n_kf, kf_ptr.data(), desc.data(), bear.data(), sig.data()};
+  cvb_verify_candidates D{C, cp1.data(), co1.data(), cr1.data(), cp2.data(), co2.data(), cr2.data(), pair_ptr.data(), pairs.data()};
+  cvb_verify_params prm{params.img_match_thres, params.ratio_thres, params.threshold5, params.max_iterations5, params.threshold17,
+                        params.max_iterations17, params.probability, params.n_cov_samples};
+  cvb_verify_result R{nm.data(), bs5.data(), bm5.data(), bc5.data(), it5.data(), us5.data(), bs.data(), bm.data(), bc.data(), it.data(), us.data(),
+                      cov.data(), nv.data(), corr.data(), (int32_t)bound, 0};
+  ctx.check(cvb_verify_noncentral_relative_pose_seeded_batch(ctx.get(), &K, &D, &prm, seeds5.data(), seeds.data(), &R),
+            "cvb_verify_noncentral_relative_pose_seeded_batch");
+  VerifyResult out;
+  out.pairings.resize(P); out.candidates.resize(C);
+  for (int q = 0; q < P; q++) {
+    VerifyPairingResult& o = out.pairings[q];
+    o.n_matches = nm[q]; o.best_sample = bs5[q]; o.n_inliers = bc5[q]; o.iterations = it5[q]; o.samples_used = us5[q];
+    std::copy(bm5.begin() + 12 * (size_t)q, bm5.begin() + 12 * (size_t)(q + 1), o.model.begin());
+  }
+  for (int c = 0; c < C; c++) {
+    VerifyCandidateResult& o = out.candidates[c];
+    o.best_sample = bs[c]; o.n_inliers = bc[c]; o.iterations = it[c]; o.samples_used = us[c]; o.n_valid = nv[c];
+    std::copy(bm.begin() + 12 * (size_t)c, bm.begin() + 12 * (size_t)(c + 1), o.model.begin());
+    std::copy(cov.begin() + 36 * (size_t)c, cov.begin() + 36 * (size_t)(c + 1), o.cov.begin());
+  }
+  for (int j = 0; j < R.n_total; j++)
+    out.correspondences.push_back({corr[5 * j], corr[5 * j + 1], corr[5 * j + 2], corr[5 * j + 3], corr[5 * j + 4]});
+  return out;
+}
+
 // The sampling-based 6x6 covariance of RelNonCentralPosSolver::computeNonCentralRelPose (RelNonCentralPosSolver.cpp:199,236,
 // 276-279) for a batch of candidates in one call (cvb_noncentral_relative_pose_covariance_batch), in place of the loop of up to
 // 300 host 17-point solves per candidate.  problems[i] are the candidate's correspondences and rigs, with samples = the

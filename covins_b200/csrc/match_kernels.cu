@@ -4,6 +4,8 @@
 //                                      placerec_gen_be.cpp:82-100, RelNonCentralPosSolver.cpp:303-324)
 //   scan_kernel<L2Metric,…>        K2  brute-force L2 k-NN on u8 SIFT    (exact result of the FLANN call sites)
 //   fused filter epilogue              placerec_gen_be.cpp:102-114
+//   scan_kernel<HammingMetric,…,PAIRS> K1 over a list of keyframe pairs, each with its own query rows (the pairwise matchings
+//                                      of computeNonCentralRelPose, cvb_match_hamming_pairs_dev)
 //   scan_kernel<HammingMetric,…,DM> + dm_assign_kernel
 //                                  K3  DenseMatcher<LandmarkMatchingAlgorithm> (placerec_be.cpp:85-90)
 //
@@ -34,7 +36,7 @@ namespace {
 constexpr int kThreads = 128;
 constexpr int kStages = 2;
 
-enum { MODE_BF = 0, MODE_DM = 1 };
+enum { MODE_BF = 0, MODE_DM = 1, MODE_PAIRS = 2 };
 
 struct ScanParams {
   const uint8_t* q;
@@ -56,6 +58,9 @@ struct ScanParams {
   int32_t* match_train;
   float* match_dist;
   int32_t* n_matches;
+  // MODE_PAIRS: segment s is the pair pairs[5s .. 5s+4] = (query row0, query count, train row0, train count, output offset) of
+  // one descriptor table q (t = q); its filter outputs are at match_train / match_dist[output offset + query]
+  const int32_t* pairs;
 };
 
 __device__ __forceinline__ uint4 ld_nc_u4(const void* p) {
@@ -217,8 +222,12 @@ __global__ void __launch_bounds__(kThreads) scan_kernel(const ScanParams p) {
   const int tid = threadIdx.x;
   const int seg = blockIdx.x / p.splits;
   const int split = blockIdx.x - seg * p.splits;
-  const int s0 = p.seg_ptr[seg];
-  const int len = p.seg_ptr[seg + 1] - s0;
+  const int32_t* pr = MODE == MODE_PAIRS ? p.pairs + 5 * seg : nullptr;
+  const int s0 = MODE == MODE_PAIRS ? pr[2] : p.seg_ptr[seg];
+  const int len = MODE == MODE_PAIRS ? pr[3] : p.seg_ptr[seg + 1] - s0;
+  const int nq = MODE == MODE_PAIRS ? pr[1] : p.nq;
+  const uint8_t* qsrc = MODE == MODE_PAIRS ? p.q + (size_t)pr[0] * M::kRowBytes : p.q;
+  if (MODE == MODE_PAIRS && (int)blockIdx.y * (kThreads * QPT) >= nq) return;   // CTA-uniform, before any barrier
   const int r0 = min(len, split * p.chunk);
   const int r1 = min(len, r0 + p.chunk);
   const int ntiles = (r1 - r0 + M::kTileRows - 1) / M::kTileRows;
@@ -231,10 +240,10 @@ __global__ void __launch_bounds__(kThreads) scan_kernel(const ScanParams p) {
 #pragma unroll
   for (int j = 0; j < QPT; j++) {
     const int qi = blockIdx.y * (kThreads * QPT) + j * kThreads + tid;
-    active[j] = qi < p.nq;
+    active[j] = qi < nq;
     if (MODE == MODE_DM && active[j] && p.skipA) active[j] = p.skipA[qi] == 0;
-    const int ql = min(qi, p.nq - 1);
-    M::load_q(q[j], p.q + (size_t)ql * M::kRowBytes);
+    const int ql = min(qi, nq - 1);
+    M::load_q(q[j], qsrc + (size_t)ql * M::kRowBytes);
 #pragma unroll
     for (int c = 0; c < K; c++) {
       wd[j][c] = (MODE == MODE_DM) ? p.ithr : INT_MAX;
@@ -317,7 +326,7 @@ __global__ void __launch_bounds__(kThreads) scan_kernel(const ScanParams p) {
 #pragma unroll
   for (int j = 0; j < QPT; j++) {
     const int qi = blockIdx.y * (kThreads * QPT) + j * kThreads + tid;
-    const bool valid = qi < p.nq;
+    const bool valid = qi < nq;
     if (MODE == MODE_DM) {
       if (valid) {
         const size_t o = ((size_t)seg * p.nq + qi) * K;
@@ -347,7 +356,7 @@ __global__ void __launch_bounds__(kThreads) scan_kernel(const ScanParams p) {
         const float dm = M::fdist(wd[j][0]);
         const float dn = M::fdist(wd[j][K >= 2 ? 1 : 0]);
         ok = ratio_test(wi[j][0], wi[j][K >= 2 ? 1 : 0], dm, dn, p.thr, p.ratio);
-        const size_t o = (size_t)seg * p.nq + qi;
+        const size_t o = MODE == MODE_PAIRS ? (size_t)pr[4] + qi : (size_t)seg * p.nq + qi;
         p.match_train[o] = ok ? wi[j][0] : -1;
         p.match_dist[o] = ok ? dm : FLT_MAX;
       }
@@ -797,6 +806,22 @@ int stage_inputs(cvb_ctx* ctx, const void* q, size_t qbytes, const void* t, size
 }
 
 }  // namespace
+
+// The fused 2-NN + filter of cvb_match_hamming_batch for n_pairs (query keyframe, train keyframe) pairs of one device descriptor
+// table in one launch (cvb_internal.cuh).  Each pair is an independent scan, so the results are those of cvb_match_hamming_batch
+// with n_seg = 1 on the pair's rows.  On ctx->stream; n_matches is zeroed here.
+int cvb_match_hamming_pairs_dev(cvb_ctx* ctx, const uint8_t* d_desc, const int32_t* d_pairs, int n_pairs, int max_nq, float thr, float ratio,
+                                int32_t* d_match_train, float* d_match_dist, int32_t* d_n_matches) {
+  cudaStream_t st = ctx->stream;
+  CVB_CUDA(ctx, cudaMemsetAsync(d_n_matches, 0, sizeof(int32_t) * n_pairs, st));
+  if (n_pairs == 0 || max_nq == 0) return CVB_OK;
+  const Plan pl = make_plan<HammingMetric>(max_nq, n_pairs, 0, ctx->sm_count, 4, false);
+  ScanParams sp{};
+  sp.q = d_desc; sp.nq = max_nq; sp.t = d_desc; sp.n_seg = n_pairs; sp.splits = 1; sp.chunk = INT_MAX;   // one split: the whole train keyframe
+  sp.filter = 1; sp.thr = thr; sp.ratio = ratio;
+  sp.match_train = d_match_train; sp.match_dist = d_match_dist; sp.n_matches = d_n_matches; sp.pairs = d_pairs;
+  return pl.qpt == 1 ? launch_scan<HammingMetric, 1, 2, MODE_PAIRS>(ctx, sp, pl, st) : launch_scan<HammingMetric, 4, 2, MODE_PAIRS>(ctx, sp, pl, st);
+}
 
 // ------------------------------------------------------------------------------------------------
 // Landmark::ComputeDescriptor (src/covins_backend/landmark_be.cpp:49-92), batched: one warp per landmark.  For every

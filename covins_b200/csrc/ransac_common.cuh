@@ -243,9 +243,22 @@ int check_ransac(cvb_ctx* ctx, const char* name, const Problems* p, int max_iter
   return check_samples(ctx, name, p->samples, p->prob_ptr, n_prob, ns, k);
 }
 
+// the selection parameters of a RANSAC call
+inline void set_selection(RansacOut& O, int ns, int max_iterations, double threshold, double probability) {
+  O.n_samples = ns; O.max_iterations = max_iterations; O.threshold = threshold; O.log_p = log(1.0 - probability);
+}
+
+// The launcher: kernel on device inputs and outputs D (one CTA per problem, smem bytes of dynamic shared memory) on ctx's stream.
+template <class Dev>
+int launch_ransac(cvb_ctx* ctx, void (*kernel)(Dev), size_t smem, const Dev& D, int n_prob) {
+  kernel<<<n_prob, kThreads, smem, ctx->stream>>>(D);
+  CVB_CHECK_LAUNCH(ctx);
+  return CVB_OK;
+}
+
 // The rest of a RANSAC call whose inputs are staged in St: its outputs staged after them, one upload into workspace slot
-// ws_slot, one launch of kernel (one CTA per problem, smem bytes of dynamic shared memory) with the device struct
-// inputs(device block) and its common part filled here, one download, the copy-out into r.  A seeded call may also ask for
+// ws_slot, launch_ransac of kernel with the device struct inputs(device block) and its common part filled here, one download,
+// the copy-out into r.  A seeded call may also ask for
 // its drawn samples (drawn, k indices each, -1 where not drawn).
 template <class Dev, class Result, class Inputs>
 int run_ransac(cvb_ctx* ctx, int ws_slot, void (*kernel)(Dev), size_t smem, Stager& St, const Inputs& inputs, int n_prob, int ns, size_t N,
@@ -264,7 +277,7 @@ int run_ransac(cvb_ctx* ctx, int ws_slot, void (*kernel)(Dev), size_t smem, Stag
   memcpy(hpin, St.h.data(), in_bytes);
   Dev D = inputs(d);
   RansacOut& O = D.o;
-  O.n_samples = ns; O.max_iterations = max_iterations; O.threshold = threshold; O.log_p = log(1.0 - probability);
+  set_selection(O, ns, max_iterations, threshold, probability);
   O.best_sample = (int*)(d + o_bs); O.best_model = (double*)(d + o_bm); O.best_count = (int*)(d + o_bc); O.iterations = (int*)(d + o_it);
   O.consumed = (int*)(d + o_us); O.inlier_mask = r->inlier_mask ? d + o_mask : nullptr;
   if (all) { O.sample_model = (double*)(d + o_sm); O.sample_valid = d + o_sv; O.sample_count = (int*)(d + o_sc); }
@@ -274,8 +287,7 @@ int run_ransac(cvb_ctx* ctx, int ws_slot, void (*kernel)(Dev), size_t smem, Stag
     O.drawn = (int*)(d + o_dr);
     CVB_CUDA(ctx, cudaMemsetAsync(d + o_dr, 0xff, S_all * k * 4, st));
   }
-  kernel<<<n_prob, kThreads, smem, st>>>(D);
-  CVB_CHECK_LAUNCH(ctx);
+  if (const int rc = launch_ransac(ctx, kernel, smem, D, n_prob)) return rc;
   CVB_CUDA(ctx, cudaMemcpyAsync(hpin + o_bm, d + o_bm, total - o_bm, cudaMemcpyDeviceToHost, st));
   CVB_CUDA(ctx, cudaStreamSynchronize(st));
   memcpy(r->best_model, hpin + o_bm, (size_t)n_prob * 96); memcpy(r->best_sample, hpin + o_bs, (size_t)n_prob * 4);

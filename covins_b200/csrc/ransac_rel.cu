@@ -21,7 +21,10 @@
 // IEEE restatement compiled with -ffp-contract=off (oracle/ransac_rel_oracle.c for the 17-point solver,
 // oracle/ransac_rel5_oracle.c for the 5-point one; their headers state the problems and their assumptions; so does
 // include/covins_b200.h).
+#include <algorithm>
 #include <type_traits>
+
+#include <cub/block/block_scan.cuh>
 
 #include "ransac_common.cuh"
 
@@ -677,18 +680,27 @@ void stage_rigs(Stager& St, const cvb_rel_ransac_problems* p, RelIn& in) {
   }
 }
 
-// ransac_rel_kernel<Sv, Src> on the inputs staged in St (max_pairs: the largest camera-pair count of a problem; a seeded call's
-// seeds at in.smp, its drawn samples to drawn)
+// the per-warp area (doubles) of ransac_rel_kernel<Sv, Src> for a batch whose largest camera-pair count is max_pairs; the
+// kernel's dynamic shared-memory limit is raised to the largest possible area on first use per device
 template <class Sv, class Src>
-int run_rel_ransac(cvb_ctx* ctx, Stager& St, const RelIn& in, int n_prob, int ns, size_t N, int max_pairs, double threshold, int max_iterations,
-                   double probability, cvb_rel_ransac_result* r, int32_t* drawn = nullptr) {
-  const int area = Sv::kArea > kPairArea * max_pairs ? Sv::kArea : kPairArea * max_pairs;
+int rel_ransac_area(cvb_ctx* ctx, int max_pairs, int* area) {
   constexpr int kMaxPairs = Sv::kCentral ? 1 : kMaxCams * kMaxCams;
   constexpr int kMaxArea = Sv::kArea > kPairArea * kMaxPairs ? Sv::kArea : kPairArea * kMaxPairs;
   static cvb_once_per_device once;
   if (once.first(ctx->device)) {
     CVB_CUDA(ctx, cudaFuncSetAttribute(ransac_rel_kernel<Sv, Src>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(kWarps * kMaxArea * sizeof(double))));
   }
+  *area = Sv::kArea > kPairArea * max_pairs ? Sv::kArea : kPairArea * max_pairs;
+  return CVB_OK;
+}
+
+// ransac_rel_kernel<Sv, Src> on the inputs staged in St (max_pairs: the largest camera-pair count of a problem; a seeded call's
+// seeds at in.smp, its drawn samples to drawn)
+template <class Sv, class Src>
+int run_rel_ransac(cvb_ctx* ctx, Stager& St, const RelIn& in, int n_prob, int ns, size_t N, int max_pairs, double threshold, int max_iterations,
+                   double probability, cvb_rel_ransac_result* r, int32_t* drawn = nullptr) {
+  int area = 0;
+  if (const int rc = rel_ransac_area<Sv, Src>(ctx, max_pairs, &area)) return rc;
   const auto inputs = [&](unsigned char* d) {
     RelDev D{};
     D.prob_ptr = (const int*)(d + in.ptr); D.f1 = (const double*)(d + in.f1); D.f2 = (const double*)(d + in.f2);
@@ -1031,4 +1043,282 @@ extern "C" int cvb_noncentral_relative_pose_covariance_seeded_batch(cvb_ctx* ctx
   if (!ctx) return CVB_ERR_INVALID;
   CVB_GUARD(ctx);
   return rel_cov(ctx, "noncentral_relative_pose_covariance_seeded", p, ref_model, true, inlier_mask, seed, r, drawn);
+}
+
+// ---- the verification chain of cvb_verify_noncentral_relative_pose_seeded_batch on the device ----
+// The matcher's pair-list scan (match_kernels.cu), verify_gather_kernel (matches -> 5-point problems), ransac_rel_kernel<Solver5>,
+// verify_merge_kernel (5-point inliers -> 17-point problems), ransac_rel_kernel<Solver17>, rel_cov_solve_kernel / rel_cov_reduce_kernel
+// and verify_list_kernel (the correspondence list), all on device buffers of one workspace.  The correspondence arrays are sized
+// by the host-known bound sum over pairings of rows(kf1); the problems are packed to the front in pairing (candidate) order.
+namespace {
+
+constexpr int kGlueThreads = 256;
+using GlueScan = cub::BlockScan<int, kGlueThreads>;
+
+// emit(i, rank) for every i < n with flag(i), rank = the number of flagged indices before i (a CTA-wide scan in chunks of
+// kGlueThreads); returns the number of flagged indices to every thread
+template <class Flag, class Emit>
+__device__ int scan_emit(int n, const Flag& flag, const Emit& emit) {
+  __shared__ typename GlueScan::TempStorage tmp;
+  __shared__ int carry;
+  __syncthreads();
+  if (threadIdx.x == 0) carry = 0;
+  __syncthreads();
+  for (int b = 0; b < n; b += kGlueThreads) {
+    const int i = b + threadIdx.x;
+    const int f = i < n && flag(i);
+    int rank, total;
+    GlueScan(tmp).ExclusiveSum(f, rank, total);
+    if (f) emit(i, carry + rank);
+    __syncthreads();
+    if (threadIdx.x == 0) carry += total;
+    __syncthreads();
+  }
+  return carry;
+}
+
+struct VerifyDev {
+  const double* bearings; const double* sigma;          // keyframe table [R][3], [R]
+  const int* pair_rows;                                  // [P][5] the matcher's pair table: query row0, rows, train row0, rows, offset
+  const int* pair_cams;                                  // [P][2]
+  const int* pair_ptr;                                   // [C+1]
+  const int* match_train; const int* n_matches;          // the matcher's outputs
+  int* prob_ptr5; double *f1_5, *f2_5, *s1_5, *s2_5; int *row1, *row2;   // 5-point problems [P+1], [N5] ...
+  const uint8_t* mask5; const int* count5;
+  int* prob_ptr17; double *f1_17, *f2_17, *s1_17, *s2_17; int *cam1_17, *cam2_17;
+  int* pos17;                                            // [N5] the 17-point correspondence of a 5-point inlier, -1 otherwise
+  const uint8_t* mask17;
+  int* corr; int corr_cap;                               // [corr_cap][5] (nullable)
+};
+
+// one CTA per pairing: its problem's offset (the matches of the pairings before it), prob_ptr5, and its matches in query order
+__global__ void __launch_bounds__(kGlueThreads) verify_gather_kernel(VerifyDev V) {
+  const int p = blockIdx.x;
+  __shared__ int off;
+  if (threadIdx.x == 0) {
+    int o = 0;
+    for (int q = 0; q < p; q++) o += V.n_matches[q];
+    off = o;
+    if (p == 0) V.prob_ptr5[0] = 0;
+    V.prob_ptr5[p + 1] = o + V.n_matches[p];
+  }
+  __syncthreads();
+  const int* pr = V.pair_rows + 5 * p;
+  const int q0 = pr[0], t0 = pr[2], o = off;
+  const int* mt = V.match_train + pr[4];
+  scan_emit(pr[1], [&](int i) { return mt[i] >= 0; }, [&](int i, int r) {
+    const int j = o + r, t = mt[i];
+    const size_t a = (size_t)q0 + i, b = (size_t)t0 + t;
+    for (int k = 0; k < 3; k++) { V.f1_5[3 * (size_t)j + k] = V.bearings[3 * a + k]; V.f2_5[3 * (size_t)j + k] = V.bearings[3 * b + k]; }
+    V.s1_5[j] = V.sigma[a]; V.s2_5[j] = V.sigma[b]; V.row1[j] = i; V.row2[j] = t;
+  });
+}
+
+// one CTA per candidate: its 17-point problem, the 5-point inliers of its pairings in order.  Its offset sums the 5-point
+// best_count of the pairings before it: best_count is the number of set flags in the selected model's inlier mask (ransac_cta
+// scores the same model with the same device function for both).
+__global__ void __launch_bounds__(kGlueThreads) verify_merge_kernel(VerifyDev V) {
+  const int c = blockIdx.x, pb = V.pair_ptr[c], pe = V.pair_ptr[c + 1];
+  __shared__ int off;
+  if (threadIdx.x == 0) {
+    int o = 0, m = 0;
+    for (int q = 0; q < pb; q++) o += V.count5[q];
+    for (int q = pb; q < pe; q++) m += V.count5[q];
+    off = o;
+    if (c == 0) V.prob_ptr17[0] = 0;
+    V.prob_ptr17[c + 1] = o + m;
+  }
+  __syncthreads();
+  int j0 = off;
+  for (int q = pb; q < pe; q++) {
+    const int b5 = V.prob_ptr5[q], n5 = V.prob_ptr5[q + 1] - b5, c1 = V.pair_cams[2 * q], c2 = V.pair_cams[2 * q + 1];
+    for (int i = threadIdx.x; i < n5; i += kGlueThreads) V.pos17[b5 + i] = -1;
+    __syncthreads();
+    j0 += scan_emit(n5, [&](int i) { return V.mask5[b5 + i] != 0; }, [&](int i, int r) {
+      const size_t j = (size_t)j0 + r, a = (size_t)b5 + i;
+      for (int k = 0; k < 3; k++) { V.f1_17[3 * j + k] = V.f1_5[3 * a + k]; V.f2_17[3 * j + k] = V.f2_5[3 * a + k]; }
+      V.s1_17[j] = V.s1_5[a]; V.s2_17[j] = V.s2_5[a]; V.cam1_17[j] = c1; V.cam2_17[j] = c2;
+      V.pos17[a] = (int)j;
+    });
+  }
+}
+
+// one CTA per pairing: its entries of the correspondence list (those below corr_cap)
+__global__ void __launch_bounds__(kGlueThreads) verify_list_kernel(VerifyDev V) {
+  const int p = blockIdx.x, b = V.prob_ptr5[p], e = min(V.prob_ptr5[p + 1], V.corr_cap);
+  for (int j = b + threadIdx.x; j < e; j += kGlueThreads) {
+    int* o = V.corr + 5 * (size_t)j;
+    const int k = V.pos17[j];
+    o[0] = p; o[1] = V.row1[j]; o[2] = V.row2[j]; o[3] = V.mask5[j]; o[4] = k >= 0 ? V.mask17[k] : 0;
+  }
+}
+
+int verify_noncentral(cvb_ctx* ctx, const cvb_verify_keyframes* kf, const cvb_verify_candidates* cd, const cvb_verify_params* prm,
+                      const uint64_t* seed5, const uint64_t* seed, cvb_verify_result* r) {
+  const char* name = "verify_noncentral_relative_pose_seeded";
+  constexpr int kMaxIt = (INT32_MAX - kWave) / 11;   // the seeded RANSAC's limit: every sample number fits an int
+  CVB_REQUIRE(ctx, kf && cd && prm && r && kf->n_kf >= 0 && cd->n_cand >= 0, "%s: bad arguments", name);
+  CVB_REQUIRE(ctx, prm->max_iterations5 >= 0 && prm->max_iterations5 <= kMaxIt && prm->max_iterations17 >= 0 && prm->max_iterations17 <= kMaxIt,
+              "%s: max_iterations5 / max_iterations17 outside [0, %d]", name, kMaxIt);
+  CVB_REQUIRE(ctx, prm->n_cov_samples >= 0 && r->corr_cap >= 0, "%s: negative n_cov_samples / corr_cap", name);
+  const int n_kf = kf->n_kf, C = cd->n_cand;
+  r->n_total = 0;
+  if (C == 0) return CVB_OK;
+  CVB_REQUIRE(ctx, kf->kf_ptr && cd->cam_ptr1 && cd->cam_ptr2 && cd->pair_ptr && seed, "%s: null required pointer", name);
+  CVB_REQUIRE(ctx, r->n_matches && r->best_sample5 && r->best_model5 && r->best_count5 && r->iterations5 && r->consumed5 && r->best_sample &&
+                   r->best_model && r->best_count && r->iterations && r->consumed && r->cov && r->n_valid, "%s: null result pointer", name);
+  CVB_REQUIRE(ctx, ptr_ok(kf->kf_ptr, n_kf), "%s: kf_ptr does not start at 0 or decreases", name);
+  CVB_REQUIRE(ctx, ptr_ok(cd->pair_ptr, C), "%s: pair_ptr does not start at 0 or decreases", name);
+  CVB_REQUIRE(ctx, ptr_ok(cd->cam_ptr1, C) && ptr_ok(cd->cam_ptr2, C), "%s: cam_ptr1 / cam_ptr2 does not start at 0 or decreases", name);
+  const size_t R = (size_t)kf->kf_ptr[n_kf];
+  const int P = cd->pair_ptr[C];
+  CVB_REQUIRE(ctx, R == 0 || (kf->desc && kf->bearings && kf->sigma), "%s: null keyframe arrays", name);
+  CVB_REQUIRE(ctx, P == 0 || (cd->pairs && seed5), "%s: null pairs / seed5", name);
+  const size_t NC1 = (size_t)cd->cam_ptr1[C], NC2 = (size_t)cd->cam_ptr2[C];
+  CVB_REQUIRE(ctx, (NC1 == 0 || (cd->cam_off1 && cd->cam_rot1)) && (NC2 == 0 || (cd->cam_off2 && cd->cam_rot2)), "%s: null rig arrays", name);
+  // the pair table of the matcher and the bound of the correspondence arrays
+  std::vector<int32_t> rows((size_t)P * 5), cams((size_t)P * 2);
+  size_t B = 0;
+  int max_pairs = 0, max_nq = 0;
+  for (int c = 0; c < C; c++) {
+    const int nc1 = cd->cam_ptr1[c + 1] - cd->cam_ptr1[c], nc2 = cd->cam_ptr2[c + 1] - cd->cam_ptr2[c];
+    CVB_REQUIRE(ctx, nc1 <= kMaxCams && nc2 <= kMaxCams, "%s: candidate %d has a rig of more than %d cameras", name, c, kMaxCams);
+    max_pairs = nc1 * nc2 > max_pairs ? nc1 * nc2 : max_pairs;
+    for (int q = cd->pair_ptr[c]; q < cd->pair_ptr[c + 1]; q++) {
+      const int32_t* e = cd->pairs + 4 * (size_t)q;
+      CVB_REQUIRE(ctx, e[0] >= 0 && e[0] < n_kf && e[1] >= 0 && e[1] < n_kf, "%s: pairing %d names keyframe (%d, %d) outside [0, %d)", name, q, e[0],
+                  e[1], n_kf);
+      CVB_REQUIRE(ctx, e[2] >= 0 && e[2] < nc1 && e[3] >= 0 && e[3] < nc2, "%s: pairing %d names camera (%d, %d) outside its rigs (%d, %d cameras)",
+                  name, q, e[2], e[3], nc1, nc2);
+      const int nq = kf->kf_ptr[e[0] + 1] - kf->kf_ptr[e[0]];
+      int32_t* w = rows.data() + 5 * (size_t)q;
+      w[0] = kf->kf_ptr[e[0]]; w[1] = nq; w[2] = kf->kf_ptr[e[1]]; w[3] = kf->kf_ptr[e[1] + 1] - kf->kf_ptr[e[1]]; w[4] = (int32_t)B;
+      cams[2 * (size_t)q] = e[2]; cams[2 * (size_t)q + 1] = e[3];
+      B += (size_t)nq;
+      max_nq = nq > max_nq ? nq : max_nq;
+    }
+  }
+  CVB_REQUIRE(ctx, B <= INT32_MAX, "%s: %zu query rows over the pairings exceed the int32 range", name, B);
+  const int ns = prm->n_cov_samples, ctas_per_cand = (ns + kCovPerCta - 1) / kCovPerCta;
+  CVB_REQUIRE(ctx, (long long)C * ctas_per_cand <= INT32_MAX, "%s: %lld covariance CTAs exceed the grid limit", name, (long long)C * ctas_per_cand);
+  const size_t S_all = (size_t)C * ns, L = r->corr ? std::min(B, (size_t)r->corr_cap) : 0;
+  // device block: inputs (uploaded), scratch, outputs (downloaded)
+  Stager St;
+  RelIn in{};
+  const size_t o_desc = St.put(kf->desc, R * 32), o_bear = St.put(kf->bearings, R * 24), o_sig = St.put(kf->sigma, R * 8);
+  const size_t o_rows = St.put(rows.data(), (size_t)P * 20), o_cams = St.put(cams.data(), (size_t)P * 8);
+  const size_t o_pp = St.put(cd->pair_ptr, ((size_t)C + 1) * 4);
+  in.cp1 = St.put(cd->cam_ptr1, ((size_t)C + 1) * 4); in.cp2 = St.put(cd->cam_ptr2, ((size_t)C + 1) * 4);
+  cvb_rel_ransac_problems rp{};
+  rp.n_prob = C; rp.cam_ptr1 = cd->cam_ptr1; rp.cam_off1 = cd->cam_off1; rp.cam_rot1 = cd->cam_rot1;
+  rp.cam_ptr2 = cd->cam_ptr2; rp.cam_off2 = cd->cam_off2; rp.cam_rot2 = cd->cam_rot2;
+  stage_rigs(St, &rp, in);
+  const size_t o_seed5 = St.put(seed5, (size_t)P * 8), o_seed = St.put(seed, (size_t)C * 8);
+  const size_t in_bytes = St.h.size();
+  // scratch and outputs: device offsets only (the host block holds the inputs, and the outputs from in_bytes on)
+  size_t top = in_bytes;
+  const auto res = [&](size_t bytes) {
+    const size_t o = (top + 15) & ~size_t(15);
+    top = o + bytes;
+    return o;
+  };
+  const size_t o_mt = res(B * 4), o_md = res(B * 4);
+  const size_t o_f15 = res(B * 24), o_f25 = res(B * 24), o_s15 = res(B * 8), o_s25 = res(B * 8);
+  const size_t o_r1 = res(B * 4), o_r2 = res(B * 4), o_m5 = res(B), o_pos = res(B * 4);
+  const size_t o_f117 = res(B * 24), o_f217 = res(B * 24), o_s117 = res(B * 8), o_s217 = res(B * 8);
+  const size_t o_c117 = res(B * 4), o_c217 = res(B * 4), o_m17 = res(B), o_pp17 = res(((size_t)C + 1) * 4);
+  const size_t o_d = res(S_all * 48), o_v = res(S_all);
+  const size_t o_out = res(0);
+  const size_t o_nm = res((size_t)P * 4), o_pp5 = res(((size_t)P + 1) * 4), o_bs5 = res((size_t)P * 4),
+               o_bm5 = res((size_t)P * 96), o_bc5 = res((size_t)P * 4), o_it5 = res((size_t)P * 4), o_us5 = res((size_t)P * 4);
+  const size_t o_bs = res((size_t)C * 4), o_bm = res((size_t)C * 96), o_bc = res((size_t)C * 4), o_it = res((size_t)C * 4),
+               o_us = res((size_t)C * 4), o_cov = res((size_t)C * 288), o_nv = res((size_t)C * 4), o_corr = res(L * 20);
+  const size_t total = top, out_bytes = total - o_out;
+  unsigned char* d = (unsigned char*)cvb_ws(ctx, WS_GS6, total);
+  unsigned char* hpin = (unsigned char*)cvb_pinned(ctx, in_bytes + out_bytes);
+  if (!d || !hpin) return CVB_ERR_CUDA;
+  memcpy(hpin, St.h.data(), in_bytes);
+  unsigned char* hout = hpin + in_bytes;
+  cudaStream_t st = ctx->stream;
+  CVB_CUDA(ctx, cudaMemcpyAsync(d, hpin, in_bytes, cudaMemcpyHostToDevice, st));
+  VerifyDev V{};
+  V.bearings = (const double*)(d + o_bear); V.sigma = (const double*)(d + o_sig);
+  V.pair_rows = (const int*)(d + o_rows); V.pair_cams = (const int*)(d + o_cams); V.pair_ptr = (const int*)(d + o_pp);
+  V.match_train = (const int*)(d + o_mt); V.n_matches = (const int*)(d + o_nm);
+  V.prob_ptr5 = (int*)(d + o_pp5); V.f1_5 = (double*)(d + o_f15); V.f2_5 = (double*)(d + o_f25); V.s1_5 = (double*)(d + o_s15);
+  V.s2_5 = (double*)(d + o_s25); V.row1 = (int*)(d + o_r1); V.row2 = (int*)(d + o_r2); V.mask5 = d + o_m5; V.count5 = (const int*)(d + o_bc5);
+  V.prob_ptr17 = (int*)(d + o_pp17); V.f1_17 = (double*)(d + o_f117); V.f2_17 = (double*)(d + o_f217); V.s1_17 = (double*)(d + o_s117);
+  V.s2_17 = (double*)(d + o_s217); V.cam1_17 = (int*)(d + o_c117); V.cam2_17 = (int*)(d + o_c217); V.pos17 = (int*)(d + o_pos);
+  V.mask17 = d + o_m17; V.corr = (int*)(d + o_corr); V.corr_cap = (int)L;
+  // 1. matches
+  if (const int rc = cvb_match_hamming_pairs_dev(ctx, d + o_desc, V.pair_rows, P, max_nq, prm->img_match_thres, prm->ratio_thres, (int*)(d + o_mt),
+                                                 (float*)(d + o_md), (int*)(d + o_nm)))
+    return rc;
+  if (P == 0) CVB_CUDA(ctx, cudaMemsetAsync(d + o_pp5, 0, 4, st));
+  // 2. the 5-point problems and their RANSACs
+  if (P > 0) {
+    verify_gather_kernel<<<P, kGlueThreads, 0, st>>>(V);
+    CVB_CHECK_LAUNCH(ctx);
+    RelDev D{};
+    D.prob_ptr = V.prob_ptr5; D.f1 = V.f1_5; D.f2 = V.f2_5; D.s1 = V.s1_5; D.s2 = V.s2_5;
+    set_selection(D.o, 0, prm->max_iterations5, prm->threshold5, prm->probability);
+    D.o.seed = (const unsigned long long*)(d + o_seed5);
+    D.o.best_sample = (int*)(d + o_bs5); D.o.best_model = (double*)(d + o_bm5); D.o.best_count = (int*)(d + o_bc5);
+    D.o.iterations = (int*)(d + o_it5); D.o.consumed = (int*)(d + o_us5); D.o.inlier_mask = d + o_m5;
+    if (const int rc = rel_ransac_area<Solver5, SeededSamples<kSample5>>(ctx, 1, &D.area)) return rc;
+    if (const int rc = launch_ransac(ctx, ransac_rel_kernel<Solver5, SeededSamples<kSample5>>, (size_t)kWarps * D.area * sizeof(double), D, P)) return rc;
+  }
+  // 3. the 17-point problems and their RANSACs
+  verify_merge_kernel<<<C, kGlueThreads, 0, st>>>(V);
+  CVB_CHECK_LAUNCH(ctx);
+  RelDev D{};
+  D.prob_ptr = V.prob_ptr17; D.f1 = V.f1_17; D.f2 = V.f2_17; D.s1 = V.s1_17; D.s2 = V.s2_17; D.cam1 = V.cam1_17; D.cam2 = V.cam2_17;
+  D.cam_ptr1 = (const int*)(d + in.cp1); D.cam_ptr2 = (const int*)(d + in.cp2); D.rig1 = (const double*)(d + in.rig1); D.rig2 = (const double*)(d + in.rig2);
+  set_selection(D.o, 0, prm->max_iterations17, prm->threshold17, prm->probability);
+  D.o.seed = (const unsigned long long*)(d + o_seed);
+  D.o.best_sample = (int*)(d + o_bs); D.o.best_model = (double*)(d + o_bm); D.o.best_count = (int*)(d + o_bc);
+  D.o.iterations = (int*)(d + o_it); D.o.consumed = (int*)(d + o_us); D.o.inlier_mask = d + o_m17;
+  if (const int rc = rel_ransac_area<Solver17, SeededSamples<kSample>>(ctx, max_pairs, &D.area)) return rc;
+  if (const int rc = launch_ransac(ctx, ransac_rel_kernel<Solver17, SeededSamples<kSample>>, (size_t)kWarps * D.area * sizeof(double), D, C)) return rc;
+  // 4. the covariance from the 17-point inlier mask in place
+  CovSeededDev Q{};
+  Q.prob_ptr = V.prob_ptr17; Q.f1 = V.f1_17; Q.f2 = V.f2_17; Q.cam1 = V.cam1_17; Q.cam2 = V.cam2_17;
+  Q.cam_ptr1 = D.cam_ptr1; Q.cam_ptr2 = D.cam_ptr2; Q.rig1 = D.rig1; Q.rig2 = D.rig2; Q.ref_model = D.o.best_model;
+  Q.n_samples = ns; Q.ctas_per_prob = ctas_per_cand;
+  Q.delta = (double*)(d + o_d); Q.valid = d + o_v; Q.cov = (double*)(d + o_cov); Q.n_valid = (int*)(d + o_nv);
+  Q.mask = V.mask17; Q.seed = D.o.seed;
+  if (ns > 0) {
+    constexpr int kSolveWarps = kCovPerCta < kWarps ? kCovPerCta : kWarps;
+    rel_cov_solve_kernel<CovSeededDev><<<(unsigned)(C * ctas_per_cand), 32 * kSolveWarps, (size_t)kSolveWarps * kSolveArea * sizeof(double), st>>>(Q);
+    CVB_CHECK_LAUNCH(ctx);
+  }
+  rel_cov_reduce_kernel<<<C, kCovReduceThreads, 0, st>>>(static_cast<const CovDev&>(Q));
+  CVB_CHECK_LAUNCH(ctx);
+  // 5. the correspondence list
+  if (L > 0) {
+    verify_list_kernel<<<P, kGlueThreads, 0, st>>>(V);
+    CVB_CHECK_LAUNCH(ctx);
+  }
+  CVB_CUDA(ctx, cudaMemcpyAsync(hout, d + o_out, out_bytes, cudaMemcpyDeviceToHost, st));
+  CVB_CUDA(ctx, cudaStreamSynchronize(st));
+  const auto get = [&](void* dst, size_t off, size_t bytes) { if (bytes) memcpy(dst, hout + (off - o_out), bytes); };
+  get(r->n_matches, o_nm, (size_t)P * 4); get(r->best_sample5, o_bs5, (size_t)P * 4); get(r->best_model5, o_bm5, (size_t)P * 96);
+  get(r->best_count5, o_bc5, (size_t)P * 4); get(r->iterations5, o_it5, (size_t)P * 4); get(r->consumed5, o_us5, (size_t)P * 4);
+  get(r->best_sample, o_bs, (size_t)C * 4); get(r->best_model, o_bm, (size_t)C * 96); get(r->best_count, o_bc, (size_t)C * 4);
+  get(r->iterations, o_it, (size_t)C * 4); get(r->consumed, o_us, (size_t)C * 4); get(r->cov, o_cov, (size_t)C * 288); get(r->n_valid, o_nv, (size_t)C * 4);
+  int32_t n_total = 0;
+  get(&n_total, o_pp5 + (size_t)P * 4, 4);
+  r->n_total = n_total;
+  if (r->corr && (size_t)n_total <= L) get(r->corr, o_corr, (size_t)n_total * 20);
+  return CVB_OK;
+}
+
+}  // namespace
+
+extern "C" int cvb_verify_noncentral_relative_pose_seeded_batch(cvb_ctx* ctx, const cvb_verify_keyframes* kf, const cvb_verify_candidates* cand,
+                                                                const cvb_verify_params* prm, const uint64_t* seed5, const uint64_t* seed,
+                                                                cvb_verify_result* r) {
+  if (!ctx) return CVB_ERR_INVALID;
+  CVB_GUARD(ctx);
+  return verify_noncentral(ctx, kf, cand, prm, seed5, seed, r);
 }

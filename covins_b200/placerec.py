@@ -13,6 +13,8 @@ the C-ABI:
                                   re-solves from caller-supplied samples)
   ransac_*_seeded(...), relative_pose_covariance_seeded(...) ↔ the same calls with the samples drawn on the GPU from one seed
                                   per problem, as the reference draws its own (include/covins_b200.h, "Seeded samples")
+  verify_noncentral_relative_pose_seeded(...) ↔ the whole verification of RelNonCentralPosSolver::computeNonCentralRelPose
+                                  (pairwise matching, 5-point and 17-point RANSAC, covariance) for all candidates in one call
 
 `KfView` flattens what the reference reads of a Keyframe (the C++ shim does the same from the containers)."""
 from __future__ import annotations
@@ -372,4 +374,65 @@ def relative_pose_covariance_seeded(ctx: Context, prob_ptr, f1, f2, cam1, cam2, 
     R = CRelCovResult(*[r[k].ctypes.data if k in r else None for k, _ in CRelCovResult._fields_])
     ctx.check(lib().cvb_noncentral_relative_pose_covariance_seeded_batch(ctx.handle, C.byref(P), ref.ctypes.data, mask.ctypes.data, seeds.ctypes.data,
                                                                          C.byref(R), r["drawn"].ctypes.data if want_drawn else None))
+    return r
+
+
+class CVerifyKeyframes(C.Structure):
+    _fields_ = [("n_kf", C.c_int32)] + [(k, c_vp) for k in ("kf_ptr", "desc", "bearings", "sigma")]
+
+
+class CVerifyCandidates(C.Structure):
+    _fields_ = [("n_cand", C.c_int32)] + [(k, c_vp) for k in ("cam_ptr1", "cam_off1", "cam_rot1", "cam_ptr2", "cam_off2", "cam_rot2", "pair_ptr",
+                                                               "pairs")]
+
+
+class CVerifyParams(C.Structure):
+    _fields_ = [("img_match_thres", C.c_float), ("ratio_thres", C.c_float), ("threshold5", C.c_double), ("max_iterations5", C.c_int32),
+                ("threshold17", C.c_double), ("max_iterations17", C.c_int32), ("probability", C.c_double), ("n_cov_samples", C.c_int32)]
+
+
+class CVerifyResult(C.Structure):
+    _fields_ = [(k, c_vp) for k in ("n_matches", "best_sample5", "best_model5", "best_count5", "iterations5", "consumed5", "best_sample", "best_model",
+                                    "best_count", "iterations", "consumed", "cov", "n_valid", "corr")] + \
+               [("corr_cap", C.c_int32), ("n_total", C.c_int32)]
+
+
+def verify_noncentral_relative_pose_seeded(ctx: Context, kf_ptr, desc, bearings, sigma, cam_ptr1, cam_off1, cam_rot1, cam_ptr2, cam_off2, cam_rot2,
+                                           pair_ptr, pairs, seeds5, seeds, img_match_thres, ratio_thres, threshold5, max_iterations5, threshold17,
+                                           max_iterations17, probability=0.99, n_cov_samples=300, corr_cap=None):
+    """RelNonCentralPosSolver::computeNonCentralRelPose's verification of place-recognition candidates in one call
+    (cvb_verify_noncentral_relative_pose_seeded_batch): per pairing (kf1, kf2, cam1, cam2) the fused 2-NN + ratio filter of
+    match_candidates_hamming and a seeded 5-point RANSAC on its matches; per candidate a seeded 17-point RANSAC on the pairings'
+    5-point inliers and the seeded covariance on its inliers.  Keyframe table: kf_ptr [n_kf+1] row offsets into desc [R,32] u8,
+    bearings [R,3], sigma [R].  Candidates: rigs as ransac_noncentral_relative_pose (cam_ptr1 [n_cand+1], ...), pair_ptr
+    [n_cand+1], pairs [n_pairings,4] (kf1, kf2, cam1, cam2); seeds5 [n_pairings], seeds [n_cand] uint64.
+    corr_cap: capacity of the correspondence list (None: room for every match, 0: no list).
+    → dict(n_matches, best_sample5, best_model5 [P,3,4], best_count5, iterations5, consumed5 (per pairing); best_sample,
+    best_model [C,3,4], best_count, iterations, consumed, cov [C,6,6], n_valid (per candidate); n_total; and, unless
+    corr_cap = 0 or n_total > corr_cap, corr [n_total,5] = (pairing, row1, row2, inlier5, inlier17))."""
+    kp = np.ascontiguousarray(kf_ptr, np.int32); n_kf = len(kp) - 1
+    dsc = np.ascontiguousarray(desc, np.uint8).reshape(-1, 32); f = np.ascontiguousarray(bearings, np.float64).reshape(-1, 3)
+    sg = np.ascontiguousarray(sigma, np.float64).reshape(-1)
+    cp1 = np.ascontiguousarray(cam_ptr1, np.int32); cp2 = np.ascontiguousarray(cam_ptr2, np.int32); n_cand = len(cp1) - 1
+    co1 = np.ascontiguousarray(cam_off1, np.float64).reshape(-1, 3); cr1 = np.ascontiguousarray(cam_rot1, np.float64).reshape(-1, 9)
+    co2 = np.ascontiguousarray(cam_off2, np.float64).reshape(-1, 3); cr2 = np.ascontiguousarray(cam_rot2, np.float64).reshape(-1, 9)
+    pp = np.ascontiguousarray(pair_ptr, np.int32); pr = np.ascontiguousarray(pairs, np.int32).reshape(-1, 4); P = len(pr)
+    s5 = _seeds(seeds5, P); s17 = _seeds(seeds, n_cand)
+    if corr_cap is None:
+        corr_cap = int(sum(kp[a + 1] - kp[a] for a in pr[:, 0])) if P and n_kf > 0 and pr[:, 0].min() >= 0 and pr[:, 0].max() < n_kf else 0
+    r = dict(n_matches=np.zeros(P, np.int32), best_sample5=np.zeros(P, np.int32), best_model5=np.zeros((P, 3, 4)), best_count5=np.zeros(P, np.int32),
+             iterations5=np.zeros(P, np.int32), consumed5=np.zeros(P, np.int32), best_sample=np.zeros(n_cand, np.int32),
+             best_model=np.zeros((n_cand, 3, 4)), best_count=np.zeros(n_cand, np.int32), iterations=np.zeros(n_cand, np.int32),
+             consumed=np.zeros(n_cand, np.int32), cov=np.zeros((n_cand, 6, 6)), n_valid=np.zeros(n_cand, np.int32))
+    corr = np.zeros((max(int(corr_cap), 1), 5), np.int32)
+    K = CVerifyKeyframes(n_kf, *[x.ctypes.data for x in (kp, dsc, f, sg)])
+    D = CVerifyCandidates(n_cand, *[x.ctypes.data for x in (cp1, co1, cr1, cp2, co2, cr2, pp, pr)])
+    Pm = CVerifyParams(float(img_match_thres), float(ratio_thres), float(threshold5), int(max_iterations5), float(threshold17), int(max_iterations17),
+                       float(probability), int(n_cov_samples))
+    R = CVerifyResult(*[r[k].ctypes.data for k, _ in CVerifyResult._fields_[:13]], corr.ctypes.data if corr_cap else None, int(corr_cap), 0)
+    ctx.check(lib().cvb_verify_noncentral_relative_pose_seeded_batch(ctx.handle, C.byref(K), C.byref(D), C.byref(Pm), s5.ctypes.data,
+                                                                     s17.ctypes.data, C.byref(R)))
+    r["n_total"] = int(R.n_total)
+    if corr_cap and R.n_total <= corr_cap:
+        r["corr"] = corr[:R.n_total].copy()
     return r

@@ -566,6 +566,92 @@ CVB_API int cvb_noncentral_relative_pose_covariance_seeded_batch(cvb_ctx* ctx, c
                                                                  int32_t* drawn);
 
 /*
+ * The COVINS_G verification of place-recognition candidates (RelNonCentralPosSolver::computeNonCentralRelPose: pairwise ORB
+ * matching, a 5-point RANSAC per pairing, one 17-point RANSAC per candidate on their inliers, the sampling-based covariance)
+ * for all candidates of one query keyframe in one call: one upload, every stage on the ctx's stream, one download.
+ *   Semantics: exactly the composition of the calls above on the same inputs and seeds:
+ *     1. Matches of pairing (kf1, kf2, cam1, cam2): cvb_match_hamming_batch(query = the rows of kf1, train = the rows of kf2,
+ *        img_match_thres, ratio_thres); the accepted rows are kept in query order.  n_matches is its count.
+ *     2. 5-point problem of the pairing, one correspondence per match: f1 = bearings[row of kf1], f2 = bearings[row of kf2],
+ *        sigma1 / sigma2 likewise; solved by cvb_ransac_central_relative_pose_seeded_batch (threshold5, max_iterations5,
+ *        probability) with seed5[pairing].
+ *     3. 17-point problem of a candidate: its pairings in order, of each the matches in the 5-point model's inlier mask in
+ *        match order, with camera indices (cam1, cam2) of the pairing; solved by cvb_ransac_noncentral_relative_pose_seeded_batch
+ *        (threshold17, max_iterations17, probability) with seed[candidate] and the candidate's rigs.
+ *        ASSUMPTION (the reference source is not in the tree): the inlier sets of the 5-point RANSACs feed the 17-point one
+ *        in this order; the caller chooses the pairings (the reference uses six).
+ *     4. Covariance: cvb_noncentral_relative_pose_covariance_seeded_batch with n_cov_samples samples (the reference's 300),
+ *        ref_model = the 17-point best_model, its inlier mask and seed[candidate].
+ *   So a pairing with fewer than 5 matches selects nothing and contributes no correspondence, a candidate with fewer than 17
+ *   merged correspondences gets best_sample = -1 and n_valid = 0, and a keyframe with fewer than 2 rows has no accepted match.
+ * Inputs:
+ *   Keyframe table (every keyframe any rig uses, once): kf_ptr [n_kf+1] row offsets (kf_ptr[0] = 0) into desc [R][32] (ORB
+ *   rows), bearings [R][3] (unit, in the keyframe's camera frame) and sigma [R] (the score's per-keypoint sigma).
+ *   Candidates: rigs cam_ptr1 / cam_off1 / cam_rot1 and cam_ptr2 / ... as in cvb_rel_ransac_problems (rig 1 is normally the
+ *   query keyframe's rig, the same for every candidate); pair_ptr [n_cand+1] the candidate's pairings, pairs [n_pairings][4] =
+ *   (kf1, kf2, cam1, cam2): kf1 / kf2 index the keyframe table, cam1 / cam2 are those keyframes' cameras in the candidate's
+ *   rigs.  seed5 [n_pairings], seed [n_cand] (stream 0 for the 17-point RANSAC, stream 1 for the covariance).
+ * Outputs (cvb_verify_result): per pairing n_matches and the 5-point best_sample / best_model / best_count / iterations /
+ * consumed; per candidate the 17-point best_sample / best_model / best_count / iterations / consumed, cov [36] and n_valid;
+ * n_total, the number of matches over all pairings; and, when corr is not null and n_total <= corr_cap, the correspondence list
+ * corr [n_total][5] = (pairing, row1, row2, inlier5, inlier17) in pairing then match order (row1 / row2 local to kf1 / kf2;
+ * inlier17 is the 17-point inlier flag of a correspondence that entered the 17-point problem, else 0).  With n_total >
+ * corr_cap only n_total is written.
+ * Errors: CVB_ERR_INVALID before any launch for negative sizes, null required pointers, a decreasing kf_ptr / pair_ptr /
+ * cam_ptr1 / cam_ptr2, a keyframe or camera index out of range, a rig of more than CVB_REL_MAX_CAMS cameras, a null seed5 /
+ * seed, a negative n_cov_samples or corr_cap, or max_iterations5 / max_iterations17 outside [0, (INT32_MAX - 64) / 11];
+ * n_cand = 0 succeeds.
+ */
+typedef struct cvb_verify_keyframes {
+  int32_t n_kf;
+  const int32_t* kf_ptr;     /* [n_kf+1] */
+  const uint8_t* desc;       /* [R][32] */
+  const double* bearings;    /* [R][3] */
+  const double* sigma;       /* [R] */
+} cvb_verify_keyframes;
+typedef struct cvb_verify_candidates {
+  int32_t n_cand;
+  const int32_t* cam_ptr1;   /* [n_cand+1] */
+  const double* cam_off1;    /* [cam_ptr1[n_cand]][3] */
+  const double* cam_rot1;    /* [cam_ptr1[n_cand]][9] row-major */
+  const int32_t* cam_ptr2;   /* [n_cand+1] */
+  const double* cam_off2;    /* [cam_ptr2[n_cand]][3] */
+  const double* cam_rot2;    /* [cam_ptr2[n_cand]][9] */
+  const int32_t* pair_ptr;   /* [n_cand+1] */
+  const int32_t* pairs;      /* [pair_ptr[n_cand]][4] kf1, kf2, cam1, cam2 */
+} cvb_verify_candidates;
+typedef struct cvb_verify_params {
+  float img_match_thres, ratio_thres;
+  double threshold5;
+  int32_t max_iterations5;
+  double threshold17;
+  int32_t max_iterations17;
+  double probability;
+  int32_t n_cov_samples;
+} cvb_verify_params;
+typedef struct cvb_verify_result {
+  int32_t* n_matches;        /* [n_pairings] */
+  int32_t* best_sample5;     /* [n_pairings] */
+  double* best_model5;       /* [n_pairings][12] */
+  int32_t* best_count5;      /* [n_pairings] */
+  int32_t* iterations5;      /* [n_pairings] */
+  int32_t* consumed5;        /* [n_pairings] */
+  int32_t* best_sample;      /* [n_cand] */
+  double* best_model;        /* [n_cand][12] */
+  int32_t* best_count;       /* [n_cand] */
+  int32_t* iterations;       /* [n_cand] */
+  int32_t* consumed;         /* [n_cand] */
+  double* cov;               /* [n_cand][36] */
+  int32_t* n_valid;          /* [n_cand] */
+  int32_t* corr;             /* [corr_cap][5] nullable */
+  int32_t corr_cap;
+  int32_t n_total;           /* written */
+} cvb_verify_result;
+CVB_API int cvb_verify_noncentral_relative_pose_seeded_batch(cvb_ctx* ctx, const cvb_verify_keyframes* kf, const cvb_verify_candidates* cand,
+                                                             const cvb_verify_params* prm, const uint64_t* seed5, const uint64_t* seed,
+                                                             cvb_verify_result* r);
+
+/*
  * Optimization::OptimizeRelativePose(kf1, kf2, matches1, T12, th2) (optimization_be.cpp:620-831): the 6-dof refinement of
  * the relative pose T12 from the matched landmark pairs, both ceres::Solve calls (5 + 5 iterations, DOGLEG, CauchyLoss(1))
  * and the outlier purge between them, in one call.  The caller (shim) flattens, per residual pair r (the reference's
