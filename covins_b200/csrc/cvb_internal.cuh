@@ -63,6 +63,31 @@ void* cvb_pinned(cvb_ctx* ctx, size_t bytes);
 int cvb_match_hamming_pairs_dev(cvb_ctx* ctx, const uint8_t* d_desc, const int32_t* d_pairs, int n_pairs, int max_nq, float thr, float ratio,
                                 int32_t* d_match_train, float* d_match_dist, int32_t* d_n_matches);
 
+// ransac_abs.cu: the seeded GP3P RANSAC of cvb_ransac_absolute_pose_seeded_batch on device inputs and outputs (one CTA per
+// problem on ctx->stream).  d_cam [n_prob][12] = camera offset (3) then rotation (9, row-major); d_inlier_mask nullable.
+int cvb_abs_ransac_seeded_dev(cvb_ctx* ctx, int n_prob, const int32_t* d_prob_ptr, const double* d_pts, const double* d_f, const double* d_sigma,
+                              const double* d_cam, const uint64_t* d_seed, double threshold, int max_iterations, double probability,
+                              int32_t* d_best_sample, double* d_best_model, int32_t* d_best_count, int32_t* d_iterations, int32_t* d_consumed,
+                              uint8_t* d_inlier_mask);
+
+// relpose.cu: one problem of cvb_optimize_relative_pose in device memory (all pointers device).  pose_in [7]; removed [n];
+// out [27] = T12_out [7], n_inliers, the two solves' iterations, the cost-history length and the history [16].
+struct cvb_relcam {
+  double intr[4], dist[4];
+  int cam, dm;
+  double xi;
+};
+struct cvb_relpose_dev {
+  int n;
+  const double* pA; const double* pB; const float* kpA; const float* kpB; const double* sA; const double* sB;
+  cvb_relcam camA, camB;
+  const double* pose_in; uint8_t* removed; double* out;
+};
+constexpr int CVB_RELPOSE_OUT = 27;
+// refines the n_prob problems d_probs [n_prob] (device) in one launch on ctx->stream, one CTA each; a problem with n < 12 gets
+// cvb_optimize_relative_pose's early result (T12_out = pose_in, nothing removed, zero counts)
+int cvb_relpose_batch_dev(cvb_ctx* ctx, const cvb_relpose_dev* d_probs, int n_prob, double th_outlier_align);
+
 #define CVB_CUDA(ctx, call)                                                                         \
   do {                                                                                              \
     cudaError_t e_ = (call);                                                                        \

@@ -20,6 +20,7 @@
 #include "ba_math.cuh"
 #include "cvb_internal.cuh"
 #include "geom_common.cuh"
+#include "ransac_common.cuh"
 
 namespace {
 
@@ -287,9 +288,10 @@ __global__ void __launch_bounds__(256) score_rel_kernel(const double* __restrict
   if ((threadIdx.x & 31) == 0 && in) atomicAdd(n_inliers + h, in);
 }
 
-size_t stage_kf(Stager& S, const cvb_kf_view* v, size_t off[9]) {
+// with_desc = false: the descriptor rows are staged elsewhere by the caller, who sets off[2]
+size_t stage_kf(Stager& S, const cvb_kf_view* v, size_t off[9], bool with_desc = true) {
   const size_t n = (size_t)v->n;
-  off[0] = S.put(v->kp, n * 8); off[1] = S.put(v->octave, n * 4); off[2] = S.put(v->desc, n * 32); off[3] = S.put(v->lm_valid, n);
+  off[0] = S.put(v->kp, n * 8); off[1] = S.put(v->octave, n * 4); off[2] = with_desc ? S.put(v->desc, n * 32) : 0; off[3] = S.put(v->lm_valid, n);
   off[4] = S.put(v->lm_pos, n * 24); off[5] = S.put(v->lm_maxdist, n * 8); off[6] = S.put(v->lm_desc, n * 32);
   off[7] = S.put(v->grid_ptr, (GRID_COLS * GRID_ROWS + 1) * 4);
   off[8] = S.put(v->grid_idx, (size_t)v->grid_ptr[GRID_COLS * GRID_ROWS] * 4);
@@ -501,3 +503,379 @@ int cvb_search_by_projection(cvb_ctx* ctx, const cvb_kf_view* kf, const int32_t*
 }
 
 }  // extern "C"
+
+// ---- the COVINS verification chain of cvb_verify_landmark_candidates_seeded_batch on the device ----
+// The DenseMatcher scan and assignment (cvb_landmark_match_batch_dev), lmv_gather_kernel (matches -> RANSAC problems),
+// ransac_abs_kernel<SeededSamples<4>> (cvb_abs_ransac_seeded_dev), lmv_pose_kernel (gate, T12 / T21, already-masks),
+// search_se3_kernel, lmv_residual_kernel (LandmarkVector -> residual pairs) and relpose_kernel (cvb_relpose_batch_dev), all on
+// device buffers of one workspace.  The per-candidate arrays are sized by the host-known bound n_cand x n_query; the RANSAC
+// problems are packed to the front in candidate order.  The DevPair and relpose records hold pointers that depend only on
+// sizes, so the host fills them; the device writes their T12 / T21 and n.
+namespace {
+
+struct LmvDev {
+  int nq, min_matches, min_inliers;
+  const int* seg;                                       // [C+1] the candidates' rows in the concatenated B
+  const int* outA; const int* outB; const int* n_out;   // the matcher's matches, per segment ordered by B
+  const double* q_bear; const double* q_sig;            // query [nq][3], [nq]
+  const uint8_t* q_valid; const double* q_pos; const float* q_kp; const float* q_oct;
+  double q_Tsc[16], TcwA[16];
+  const double* TcwB;                                   // [C][16]
+  int* row;                                             // [C][nq] the idxB matched to query keypoint i, or -1
+  int* prob_ptr; double* pts; double* f; double* sg; int* srcA;   // the RANSAC problems, packed
+  const int* best_sample; const double* best_model; const int* best_count; const uint8_t* mask;
+  uint8_t* already1; uint8_t* stage; int* match12;      // [C][nq]
+  double* T12; double* T21; double* pose_in;            // [C][16], [C][16], [C][7]
+  double* pA; double* pB; float* kA; float* kB; double* sA; double* sB;   // residual pairs of candidate c from c * nq
+  int* n_corr;
+};
+
+// rows 0..2 of A * B (4x4 row-major), each entry four products summed left to right; row 3 = 0 0 0 1
+__device__ void mul44_rn(const double* A, const double* B, double* O) {
+  for (int r = 0; r < 3; r++)
+    for (int c = 0; c < 4; c++)
+      O[4 * r + c] = add(add(add(mul(A[4 * r], B[c]), mul(A[4 * r + 1], B[4 + c])), mul(A[4 * r + 2], B[8 + c])), mul(A[4 * r + 3], B[12 + c]));
+  O[12] = O[13] = O[14] = 0.0; O[15] = 1.0;
+}
+// [R^T | -R^T t] of rows 0..2 of T, the shim's inv_rigid order; row 3 = 0 0 0 1
+__device__ void rigid_inv_rn(const double* T, double* I) {
+  for (int r = 0; r < 3; r++)
+    for (int c = 0; c < 3; c++) I[4 * r + c] = T[4 * c + r];
+  for (int r = 0; r < 3; r++) I[4 * r + 3] = -add(add(mul(T[r], T[3]), mul(T[4 + r], T[7])), mul(T[8 + r], T[11]));
+  I[12] = I[13] = I[14] = 0.0; I[15] = 1.0;
+}
+// the shim's transform_to_pose7: [qx, qy, qz, qw, x, y, z] by Eigen's matrix-to-quaternion branches
+__device__ void pose7_rn(const double* T, double* out) {
+  double q[4];
+  const double tr = add(add(T[0], T[5]), T[10]);
+  if (tr > 0) {
+    double t = __dsqrt_rn(add(tr, 1.0));
+    q[3] = mul(0.5, t);
+    t = __ddiv_rn(0.5, t);
+    q[0] = mul(sub(T[9], T[6]), t); q[1] = mul(sub(T[2], T[8]), t); q[2] = mul(sub(T[4], T[1]), t);
+  } else {
+    int i = 0;
+    if (T[5] > T[0]) i = 1;
+    if (T[10] > T[5 * i]) i = 2;
+    const int j = (i + 1) % 3, k = (j + 1) % 3;
+    double t = __dsqrt_rn(add(sub(sub(T[5 * i], T[5 * j]), T[5 * k]), 1.0));
+    q[i] = mul(0.5, t);
+    t = __ddiv_rn(0.5, t);
+    q[3] = mul(sub(T[4 * k + j], T[4 * j + k]), t);
+    q[j] = mul(add(T[4 * j + i], T[4 * i + j]), t);
+    q[k] = mul(add(T[4 * k + i], T[4 * i + k]), t);
+  }
+  for (int c = 0; c < 4; c++) out[c] = q[c];
+  out[4] = T[3]; out[5] = T[7]; out[6] = T[11];
+}
+
+// one CTA per candidate: its matches scattered into the dense row idxA -> idxB, then (n_matches >= min_matches) compacted in
+// ascending idxA into its RANSAC problem, at the offset of the used matches of the candidates before it
+__global__ void __launch_bounds__(kGlueThreads) lmv_gather_kernel(LmvDev V, const DevPair* __restrict__ pairs) {
+  const int c = blockIdx.x, nq = V.nq;
+  __shared__ int off, use;
+  if (threadIdx.x == 0) {
+    int o = 0;
+    for (int q = 0; q < c; q++) o += V.n_out[q] >= V.min_matches ? V.n_out[q] : 0;
+    off = o;
+    use = V.n_out[c] >= V.min_matches;
+    if (c == 0) V.prob_ptr[0] = 0;
+    V.prob_ptr[c + 1] = o + (use ? V.n_out[c] : 0);
+  }
+  int* row = V.row + (size_t)c * nq;
+  for (int i = threadIdx.x; i < nq; i += kGlueThreads) row[i] = -1;
+  __syncthreads();
+  const int s0 = V.seg[c], m = V.n_out[c];
+  for (int k = threadIdx.x; k < m; k += kGlueThreads) row[V.outA[s0 + k]] = V.outB[s0 + k];
+  __syncthreads();
+  if (!use) return;
+  const double* lm = pairs[c].k2.lm_pos;
+  const int o = off;
+  scan_emit(nq, [&](int i) { return row[i] >= 0; }, [&](int i, int r) {
+    const size_t j = (size_t)o + r, b = (size_t)row[i];
+    for (int k = 0; k < 3; k++) { V.pts[3 * j + k] = lm[3 * b + k]; V.f[3 * j + k] = V.q_bear[3 * (size_t)i + k]; }
+    V.sg[j] = V.q_sig[i]; V.srcA[j] = i;
+  });
+}
+
+// one CTA per candidate: the gate, T12 / T21 (also into its DevPair) and the refinement's start pose, then the already-masks and
+// stages 1 / 2.  A candidate that stops gets all-ones masks, so the search finds nothing for it.
+__global__ void __launch_bounds__(kGlueThreads) lmv_pose_kernel(LmvDev V, DevPair* __restrict__ pairs) {
+  const int c = blockIdx.x, nq = V.nq;
+  DevPair& P = pairs[c];
+  __shared__ int go;
+  if (threadIdx.x == 0) {
+    go = V.best_sample[c] >= 0 && V.best_count[c] >= V.min_inliers;
+    double T12[16], T21[16], p7[7];
+    for (int i = 0; i < 16; i++) T12[i] = T21[i] = 0.0;
+    for (int i = 0; i < 7; i++) p7[i] = 0.0;
+    if (go) {
+      double M[16], A[16], B[16], Cw[16];
+      for (int i = 0; i < 12; i++) M[i] = V.best_model[12 * (size_t)c + i];
+      M[12] = M[13] = M[14] = 0.0; M[15] = 1.0;
+      mul44_rn(M, V.q_Tsc, A);      // T_wc of the query camera
+      rigid_inv_rn(A, B);           // T_c1_w
+      rigid_inv_rn(P.k2.Tcw, Cw);   // T_w_c2
+      mul44_rn(B, Cw, T12);
+      rigid_inv_rn(T12, T21);
+      pose7_rn(T12, p7);
+    }
+    for (int i = 0; i < 16; i++) { P.T12[i] = T12[i]; P.T21[i] = T21[i]; V.T12[16 * (size_t)c + i] = T12[i]; V.T21[16 * (size_t)c + i] = T21[i]; }
+    for (int i = 0; i < 7; i++) V.pose_in[7 * (size_t)c + i] = p7[i];
+  }
+  __syncthreads();
+  const bool g = go;
+  const int n2 = P.k2.n;
+  uint8_t* a1 = V.already1 + (size_t)c * nq;
+  uint8_t* a2 = const_cast<uint8_t*>(P.already2);
+  uint8_t* st = V.stage + (size_t)c * nq;
+  const int* row = V.row + (size_t)c * nq;
+  for (int i = threadIdx.x; i < nq; i += kGlueThreads) { a1[i] = !g; st[i] = row[i] >= 0; }
+  for (int b = threadIdx.x; b < n2; b += kGlueThreads) a2[b] = !g;
+  __syncthreads();
+  if (!g) return;
+  for (int j = V.prob_ptr[c] + threadIdx.x; j < V.prob_ptr[c + 1]; j += kGlueThreads)
+    if (V.mask[j]) {
+      const int i = V.srcA[j];
+      a1[i] = 1; a2[row[i]] = 1; st[i] = 2;
+    }
+}
+
+// one CTA per candidate: the LandmarkVector (RANSAC inliers, then the search's matches: stage 3) and, in ascending query
+// keypoint, the residual pairs of its entries whose two landmarks are valid; n into the candidate's relpose record
+__global__ void __launch_bounds__(kGlueThreads) lmv_residual_kernel(LmvDev V, const DevPair* __restrict__ pairs, cvb_relpose_dev* __restrict__ recs) {
+  const int c = blockIdx.x, nq = V.nq;
+  const DevPair& P = pairs[c];
+  const size_t base = (size_t)c * nq;
+  const int* row = V.row + base;
+  const int* ms = P.match12;
+  uint8_t* st = V.stage + base;
+  int* m12 = V.match12 + base;
+  for (int i = threadIdx.x; i < nq; i += kGlueThreads) {
+    int b = -1;
+    if (st[i] == 2) b = row[i];
+    else if (ms[i] >= 0) { b = ms[i]; st[i] = 3; }
+    m12[i] = b;
+  }
+  __syncthreads();
+  const uint8_t* v2 = P.k2.lm_valid;
+  const double* lm2 = P.k2.lm_pos;
+  const float* kp2 = P.k2.kp;
+  const float* oc2 = P.k2.octave;
+  const double* TB = V.TcwB + 16 * (size_t)c;
+  const int n = scan_emit(nq, [&](int i) { const int b = m12[i]; return b >= 0 && V.q_valid[i] && v2[b]; }, [&](int i, int r) {
+    const size_t j = base + r, b = (size_t)m12[i];
+    rt_apply(V.TcwA, V.q_pos + 3 * (size_t)i, V.pA + 3 * j);
+    rt_apply(TB, lm2 + 3 * b, V.pB + 3 * j);
+    V.kA[2 * j] = V.q_kp[2 * (size_t)i]; V.kA[2 * j + 1] = V.q_kp[2 * (size_t)i + 1];
+    V.kB[2 * j] = kp2[2 * b]; V.kB[2 * j + 1] = kp2[2 * b + 1];
+    V.sA[j] = mul((double)__fadd_rn(V.q_oct[i], 1.0f), 2.0);   // (keypoints_aors_[i][1] + 1) * 2.0: a float sum, then double
+    V.sB[j] = mul((double)__fadd_rn(oc2[b], 1.0f), 2.0);
+  });
+  if (threadIdx.x == 0) { recs[c].n = n; V.n_corr[c] = n; }
+}
+
+// the shim's mul4 / inv_rigid (host, no fused multiply-add)
+void host_mul4(const double* A, const double* B, double* O) {
+  for (int r = 0; r < 4; r++)
+    for (int c = 0; c < 4; c++) {
+      double s = 0;
+      for (int k = 0; k < 4; k++) s += A[4 * r + k] * B[4 * k + c];
+      O[4 * r + c] = s;
+    }
+}
+void host_inv_rigid(const double* T, double* I) {
+  for (int i = 0; i < 16; i++) I[i] = i % 5 == 0 ? 1.0 : 0.0;
+  for (int r = 0; r < 3; r++)
+    for (int c = 0; c < 3; c++) I[4 * r + c] = T[4 * c + r];
+  for (int r = 0; r < 3; r++) I[4 * r + 3] = -(I[4 * r] * T[3] + I[4 * r + 1] * T[7] + I[4 * r + 2] * T[11]);
+}
+
+cvb_relcam relcam(const cvb_landmark_kf* k) {
+  cvb_relcam c{};
+  for (int i = 0; i < 4; i++) { c.intr[i] = k->intr[i]; c.dist[i] = k->dist[i]; }
+  c.cam = k->cam_model; c.dm = k->dist_model; c.xi = k->xi;
+  return c;
+}
+
+int verify_landmark(cvb_ctx* ctx, const cvb_landmark_kf* q, const cvb_landmark_kf* cand, int C, const cvb_landmark_verify_params* prm,
+                    const uint64_t* seed, cvb_landmark_verify_result* r) {
+  const char* name = "verify_landmark_candidates_seeded";
+  constexpr int kMaxIt = (INT32_MAX - kWave) / 11;   // the seeded RANSAC's limit: every sample number fits an int
+  CVB_REQUIRE(ctx, q && prm && r && C >= 0, "%s: bad arguments", name);
+  CVB_REQUIRE(ctx, prm->num_best >= 1 && prm->num_best <= 4, "%s: num_best must be in 1..4", name);
+  CVB_REQUIRE(ctx, prm->thr > 0.f && prm->thr <= 257.f, "%s: distance threshold out of range", name);
+  CVB_REQUIRE(ctx, prm->max_iterations >= 0 && prm->max_iterations <= kMaxIt, "%s: max_iterations outside [0, %d]", name, kMaxIt);
+  CVB_REQUIRE(ctx, prm->search.num_octaves >= 1 && prm->search.scale_factor > 1.0 && prm->search.th > 0.0, "%s: bad search parameters", name);
+  if (C == 0) return CVB_OK;
+  CVB_REQUIRE(ctx, cand && seed, "%s: null candidates / seed", name);
+  CVB_REQUIRE(ctx, r->n_matches && r->best_sample && r->best_model && r->best_count && r->iterations && r->consumed && r->T12 && r->T21 &&
+                   r->n_found && r->n_corr && r->T12_out && r->n_inliers && r->solve_iterations, "%s: null result pointer", name);
+  CVB_REQUIRE(ctx, kf_ok(&q->view), "%s: malformed keyframe view (query)", name);
+  const int nq = q->view.n;
+  CVB_REQUIRE(ctx, nq == 0 || (q->bearings && q->sigma_angle), "%s: null query bearings / sigma_angle", name);
+  std::vector<int32_t> seg((size_t)C + 1, 0);
+  for (int c = 0; c < C; c++) {
+    CVB_REQUIRE(ctx, kf_ok(&cand[c].view), "%s: malformed keyframe view (cand[%d])", name, c);
+    CVB_REQUIRE(ctx, (int64_t)seg[c] + cand[c].view.n <= INT32_MAX, "%s: candidate rows exceed the int32 range", name);
+    seg[c + 1] = seg[c] + cand[c].view.n;
+  }
+  CVB_REQUIRE(ctx, (int64_t)C * nq <= INT32_MAX, "%s: n_cand x n_query exceeds the int32 range", name);
+  for (int c = -1; c < C; c++) {   // OptimizeRelativePose's model checks (optimization_be.cpp:684-688, :705-707)
+    const cvb_landmark_kf* k = c < 0 ? q : cand + c;
+    if (k->cam_model < 0 || k->cam_model > 1) return cvb_fail(ctx, CVB_ERR_UNSUPPORTED, "Unknown projection type.");
+    if (k->dist_model < 0 || k->dist_model > 2) return cvb_fail(ctx, CVB_ERR_UNSUPPORTED, "Unknown distortion type.");
+  }
+  const size_t NB = (size_t)seg[C], L = (size_t)C * nq;
+  // the refinement's camera poses: TcwA = (T_ws1 T_sc1)^-1, TcwB = (T_ws2 T_sc1)^-1, as the shim forms them
+  double TA[16], TcwA[16];
+  host_mul4(q->T_ws, q->T_sc, TA);
+  host_inv_rigid(TA, TcwA);
+  std::vector<double> TcwB((size_t)C * 16);
+  std::vector<double> cam((size_t)C * 12);
+  for (int c = 0; c < C; c++) {
+    double TB[16];
+    host_mul4(cand[c].T_ws, q->T_sc, TB);
+    host_inv_rigid(TB, &TcwB[16 * (size_t)c]);
+    for (int k = 0; k < 3; k++) cam[12 * (size_t)c + k] = q->T_sc[4 * k + 3];   // one camera per problem: c, then Rc row-major
+    for (int a = 0; a < 3; a++)
+      for (int b = 0; b < 3; b++) cam[12 * (size_t)c + 3 + 3 * a + b] = q->T_sc[4 * a + b];
+  }
+  // device block: inputs (uploaded), scratch, outputs (downloaded)
+  Stager St;
+  size_t off1[9];
+  stage_kf(St, &q->view, off1);
+  std::vector<size_t> off2((size_t)C * 9);
+  for (int c = 0; c < C; c++) stage_kf(St, &cand[c].view, &off2[(size_t)c * 9], false);   // descriptors: the DenseMatcher's B below
+  const size_t o_bear = St.put(q->bearings, (size_t)nq * 24), o_sig = St.put(q->sigma_angle, (size_t)nq * 8);
+  std::vector<uint8_t> skipA(nq), skipB(NB);
+  for (int i = 0; i < nq; i++) skipA[i] = !q->view.lm_valid[i];
+  const size_t o_skA = St.put(skipA.data(), (size_t)nq), o_B = St.reserve(NB * 32), o_skB = St.reserve(NB);
+  for (int c = 0; c < C; c++) {
+    const size_t n = (size_t)cand[c].view.n;
+    if (n == 0) continue;
+    memcpy(St.h.data() + o_B + 32 * (size_t)seg[c], cand[c].view.desc, n * 32);
+    for (size_t b = 0; b < n; b++) St.h[o_skB + seg[c] + b] = !cand[c].view.lm_valid[b];
+  }
+  for (int c = 0; c < C; c++) off2[(size_t)c * 9 + 2] = o_B + 32 * (size_t)seg[c];   // the search reads its rows of B
+  const size_t o_seg = St.put(seg.data(), ((size_t)C + 1) * 4), o_seed = St.put(seed, (size_t)C * 8), o_cam = St.put(cam.data(), (size_t)C * 96);
+  const size_t o_TB = St.put(TcwB.data(), (size_t)C * 128);
+  const size_t o_pairs = St.reserve((size_t)C * sizeof(DevPair)), o_recs = St.reserve((size_t)C * sizeof(cvb_relpose_dev));
+  const size_t in_bytes = St.h.size();
+  size_t top = in_bytes;
+  const auto res = [&](size_t bytes) {
+    const size_t o = (top + 15) & ~size_t(15);
+    top = o + bytes;
+    return o;
+  };
+  const size_t o_oA = res(NB * 4), o_oB = res(NB * 4), o_oD = res(NB * 4), o_row = res(L * 4), o_pp = res(((size_t)C + 1) * 4);
+  const size_t o_pts = res(L * 24), o_f = res(L * 24), o_sg = res(L * 8), o_src = res(L * 4), o_mask = res(L);
+  const size_t o_a1 = res(L), o_a2 = res(NB), o_m1 = res(L * 4), o_m2 = res(NB * 4), o_ms = res(L * 4);
+  const size_t o_pA = res(L * 24), o_pB = res(L * 24), o_kA = res(L * 8), o_kB = res(L * 8), o_sA = res(L * 8), o_sB = res(L * 8);
+  const size_t o_pose = res((size_t)C * 56);
+  const size_t o_out = res(0);
+  const size_t o_nm = res((size_t)C * 4), o_bs = res((size_t)C * 4), o_bm = res((size_t)C * 96), o_bc = res((size_t)C * 4), o_it = res((size_t)C * 4),
+               o_us = res((size_t)C * 4), o_T12 = res((size_t)C * 128), o_T21 = res((size_t)C * 128), o_nf = res((size_t)C * 4),
+               o_nc = res((size_t)C * 4), o_ro = res((size_t)C * CVB_RELPOSE_OUT * 8);
+  const size_t o_m12 = res(L * 4), o_st = res(L), o_rem = res(L);
+  const size_t total = top;
+  const size_t out_end = r->removed ? total : r->stage ? o_rem : r->match12 ? o_st : o_m12;   // the nullable outputs only on request
+  unsigned char* d = (unsigned char*)cvb_ws(ctx, WS_GS0, total);
+  unsigned char* hpin = (unsigned char*)cvb_pinned(ctx, in_bytes + (out_end - o_out));
+  if (!d || !hpin) return CVB_ERR_CUDA;
+  // the records the device reads and completes
+  DevKf d1;
+  fill_dev(d1, &q->view, d, off1);
+  DevPair* hp = reinterpret_cast<DevPair*>(St.h.data() + o_pairs);
+  cvb_relpose_dev* hr = reinterpret_cast<cvb_relpose_dev*>(St.h.data() + o_recs);
+  for (int c = 0; c < C; c++) {
+    DevPair& P = hp[c];
+    memset(&P, 0, sizeof(P));
+    fill_dev(P.k2, &cand[c].view, d, &off2[(size_t)c * 9]);
+    P.already1 = d + o_a1 + (size_t)c * nq; P.already2 = d + o_a2 + seg[c];
+    P.match1 = (int*)(d + o_m1) + (size_t)c * nq; P.match2 = (int*)(d + o_m2) + seg[c];
+    P.match12 = (int*)(d + o_ms) + (size_t)c * nq; P.n_found = (int*)(d + o_nf) + c;
+    cvb_relpose_dev& R = hr[c];
+    memset(&R, 0, sizeof(R));
+    const size_t b = (size_t)c * nq;
+    R.pA = (const double*)(d + o_pA) + 3 * b; R.pB = (const double*)(d + o_pB) + 3 * b; R.kpA = (const float*)(d + o_kA) + 2 * b;
+    R.kpB = (const float*)(d + o_kB) + 2 * b; R.sA = (const double*)(d + o_sA) + b; R.sB = (const double*)(d + o_sB) + b;
+    R.camA = relcam(q); R.camB = relcam(cand + c);
+    R.pose_in = (const double*)(d + o_pose) + 7 * (size_t)c; R.removed = d + o_rem + b; R.out = (double*)(d + o_ro) + CVB_RELPOSE_OUT * (size_t)c;
+  }
+  memcpy(hpin, St.h.data(), in_bytes);
+  unsigned char* hout = hpin + in_bytes;
+  cudaStream_t st = ctx->stream;
+  CVB_CUDA(ctx, cudaMemcpyAsync(d, hpin, in_bytes, cudaMemcpyHostToDevice, st));
+  LmvDev V{};
+  V.nq = nq; V.min_matches = prm->min_matches; V.min_inliers = prm->min_ransac_inliers;
+  V.seg = (const int*)(d + o_seg); V.outA = (const int*)(d + o_oA); V.outB = (const int*)(d + o_oB); V.n_out = (const int*)(d + o_nm);
+  V.q_bear = (const double*)(d + o_bear); V.q_sig = (const double*)(d + o_sig);
+  V.q_valid = d1.lm_valid; V.q_pos = d1.lm_pos; V.q_kp = d1.kp; V.q_oct = d1.octave;
+  memcpy(V.q_Tsc, q->T_sc, sizeof(V.q_Tsc)); memcpy(V.TcwA, TcwA, sizeof(V.TcwA));
+  V.TcwB = (const double*)(d + o_TB); V.row = (int*)(d + o_row);
+  V.prob_ptr = (int*)(d + o_pp); V.pts = (double*)(d + o_pts); V.f = (double*)(d + o_f); V.sg = (double*)(d + o_sg); V.srcA = (int*)(d + o_src);
+  V.best_sample = (const int*)(d + o_bs); V.best_model = (const double*)(d + o_bm); V.best_count = (const int*)(d + o_bc); V.mask = d + o_mask;
+  V.already1 = d + o_a1; V.stage = d + o_st; V.match12 = (int*)(d + o_m12);
+  V.T12 = (double*)(d + o_T12); V.T21 = (double*)(d + o_T21); V.pose_in = (double*)(d + o_pose);
+  V.pA = (double*)(d + o_pA); V.pB = (double*)(d + o_pB); V.kA = (float*)(d + o_kA); V.kB = (float*)(d + o_kB);
+  V.sA = (double*)(d + o_sA); V.sB = (double*)(d + o_sB); V.n_corr = (int*)(d + o_nc);
+  DevPair* d_pairs = reinterpret_cast<DevPair*>(d + o_pairs);
+  cvb_relpose_dev* d_recs = reinterpret_cast<cvb_relpose_dev*>(d + o_recs);
+  // 1. DenseMatcher
+  if (NB > 0) {
+    if (const int rc = cvb_landmark_match_batch_dev(ctx, d + off1[2], d + o_skA, nq, d + o_B, d + o_skB, V.seg, seg.data(), C, prm->thr, prm->num_best,
+                                                    (int*)(d + o_oA), (int*)(d + o_oB), (float*)(d + o_oD), (int*)(d + o_nm), nullptr))
+      return rc;
+  } else {
+    CVB_CUDA(ctx, cudaMemsetAsync(d + o_nm, 0, (size_t)C * 4, st));
+  }
+  // 2. the RANSAC problems and their RANSACs
+  lmv_gather_kernel<<<C, kGlueThreads, 0, st>>>(V, d_pairs);
+  CVB_CHECK_LAUNCH(ctx);
+  if (const int rc = cvb_abs_ransac_seeded_dev(ctx, C, V.prob_ptr, V.pts, V.f, V.sg, (const double*)(d + o_cam), (const uint64_t*)(d + o_seed),
+                                               prm->threshold, prm->max_iterations, prm->probability, (int*)(d + o_bs), (double*)(d + o_bm),
+                                               (int*)(d + o_bc), (int*)(d + o_it), (int*)(d + o_us), d + o_mask))
+    return rc;
+  // 3. gate, T12 / T21, already-masks
+  lmv_pose_kernel<<<C, kGlueThreads, 0, st>>>(V, d_pairs);
+  CVB_CHECK_LAUNCH(ctx);
+  // 4. SearchBySE3
+  search_se3_kernel<<<C, 256, 0, st>>>(d1, d_pairs, prm->search.th, prm->search.desc_th_low, prm->search.scale_factor, prm->search.num_octaves);
+  CVB_CHECK_LAUNCH(ctx);
+  // 5. the residual pairs and the refinement
+  lmv_residual_kernel<<<C, kGlueThreads, 0, st>>>(V, d_pairs, d_recs);
+  CVB_CHECK_LAUNCH(ctx);
+  if (const int rc = cvb_relpose_batch_dev(ctx, d_recs, C, prm->th_outlier_align)) return rc;
+  CVB_CUDA(ctx, cudaMemcpyAsync(hout, d + o_out, out_end - o_out, cudaMemcpyDeviceToHost, st));
+  CVB_CUDA(ctx, cudaStreamSynchronize(st));
+  const auto at = [&](size_t off) { return hout + (off - o_out); };
+  memcpy(r->n_matches, at(o_nm), (size_t)C * 4); memcpy(r->best_sample, at(o_bs), (size_t)C * 4); memcpy(r->best_model, at(o_bm), (size_t)C * 96);
+  memcpy(r->best_count, at(o_bc), (size_t)C * 4); memcpy(r->iterations, at(o_it), (size_t)C * 4); memcpy(r->consumed, at(o_us), (size_t)C * 4);
+  memcpy(r->T12, at(o_T12), (size_t)C * 128); memcpy(r->T21, at(o_T21), (size_t)C * 128); memcpy(r->n_found, at(o_nf), (size_t)C * 4);
+  memcpy(r->n_corr, at(o_nc), (size_t)C * 4);
+  const double* ro = (const double*)at(o_ro);
+  for (int c = 0; c < C; c++) {
+    const double* o = ro + CVB_RELPOSE_OUT * (size_t)c;
+    for (int k = 0; k < 7; k++) r->T12_out[7 * (size_t)c + k] = o[k];
+    r->n_inliers[c] = (int32_t)o[7];
+    r->solve_iterations[2 * (size_t)c] = (int32_t)o[8]; r->solve_iterations[2 * (size_t)c + 1] = (int32_t)o[9];
+  }
+  if (r->match12) memcpy(r->match12, at(o_m12), L * 4);
+  if (r->stage) memcpy(r->stage, at(o_st), L);
+  if (r->removed) {   // defined for r < n_corr; the rest of a candidate's row is 0
+    memset(r->removed, 0, L);
+    for (int c = 0; c < C; c++) memcpy(r->removed + (size_t)c * nq, at(o_rem) + (size_t)c * nq, (size_t)r->n_corr[c]);
+  }
+  return CVB_OK;
+}
+
+}  // namespace
+
+extern "C" int cvb_verify_landmark_candidates_seeded_batch(cvb_ctx* ctx, const cvb_landmark_kf* query, const cvb_landmark_kf* cand, int n_cand,
+                                                           const cvb_landmark_verify_params* prm, const uint64_t* seed,
+                                                           cvb_landmark_verify_result* r) {
+  if (!ctx) return CVB_ERR_INVALID;
+  CVB_GUARD(ctx);
+  return verify_landmark(ctx, query, cand, n_cand, prm, seed, r);
+}

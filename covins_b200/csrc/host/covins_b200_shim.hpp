@@ -76,6 +76,9 @@ struct Adapter {
   // (ORB-SLAM3 agents only send pinhole + radtan, orb_slam3/src/KeyFrame.cc:64-65); specialise for the real Keyframe:
   //   cam = kf.camera_->getType() == aslam::Camera::Type::kUnifiedProjection, dist from getDistortion().getType().
   static void camera_model(const KF& kf, int* cam, int* dist, double* xi) { (void)kf; *cam = 0; *dist = 0; *xi = 0.0; }
+  // the unit bearing vector [n][3] (camera frame) and sigma angle [n] of every keypoint, what Se3Solver::projectiveAlignment reads of
+  // the query keyframe (FrameAbsolutePoseSacProblem's getSigmaAngle); specialise for the real Keyframe
+  static void bearings(const KF& kf, double* f, double* sigma_angle) { kf.GetBearings(f, sigma_angle); }
   // raw IMU samples of the KF's preintegration (robopt PreintegrationBase::getReadingsByIndex / getTimeDiffByIndex,
   // keyframe_base.cpp:145-173) and its first reading + noise (keyframe_be.cpp:187-203)
   static size_t imu_count(const KF& kf) { return kf.ImuDt().size(); }
@@ -797,6 +800,34 @@ struct KfViewStorage {
   }
 };
 
+namespace detail {
+// the flat view of a keyframe that SearchBySE3 reads (KfViewStorage)
+template <class KFPtr>
+inline void flatten_kf_view(const KFPtr& kf, KfViewStorage& S) {
+  const size_t n = kf->keypoints_distorted_.size();
+  S.kp.resize(2 * n); S.octave.resize(n); S.desc.resize(32 * n); S.lm_valid.assign(n, 0); S.lm_pos.assign(3 * n, 0.0);
+  S.lm_maxdist.assign(n, 1.0); S.lm_desc.assign(32 * n, 0);
+  const auto lms = kf->GetLandmarks();
+  for (size_t i = 0; i < n; i++) {
+    S.kp[2 * i] = kf->keypoints_distorted_[i][0]; S.kp[2 * i + 1] = kf->keypoints_distorted_[i][1];
+    S.octave[i] = kf->keypoints_aors_[i][1];
+    std::copy(kf->GetDescriptor(i), kf->GetDescriptor(i) + 32, S.desc.begin() + 32 * i);
+    if (lms[i] && !lms[i]->IsInvalid()) {
+      S.lm_valid[i] = 1;
+      const auto p = lms[i]->GetWorldPos();
+      for (int c = 0; c < 3; c++) S.lm_pos[3 * i + c] = p[c];
+      S.lm_maxdist[i] = lms[i]->GetMaxDistance();
+      std::copy(lms[i]->GetDescriptorPtr(), lms[i]->GetDescriptorPtr() + 32, S.lm_desc.begin() + 32 * i);
+    }
+  }
+  const auto Tcw = kf->GetPoseTcw();
+  for (int r = 0; r < 4; r++) for (int c = 0; c < 4; c++) S.v.Tcw[4 * r + c] = Tcw(r, c);
+  for (int r = 0; r < 3; r++) for (int c = 0; c < 3; c++) S.v.K[3 * r + c] = kf->calibration_K(r, c);
+  S.v.img[0] = kf->img_dim_x_min_; S.v.img[1] = kf->img_dim_x_max_; S.v.img[2] = kf->img_dim_y_min_; S.v.img[3] = kf->img_dim_y_max_;
+  S.assign_grid(kf->image_width(), kf->image_height());
+}
+}  // namespace detail
+
 // FeatureMatcher::SearchBySE3(pKF1, pKF2, matches12, T12, th) (feature_matcher_be.cpp:293-498) for a batch of candidates:
 // matches12[p] is updated in place exactly as the reference does (:485-496: matches12[i] = mapPoints2[idx2]); returns the
 // number of matches found per candidate.  KF is touched through the member names the reference class has
@@ -808,29 +839,7 @@ template <class KFPtr, class LandmarkVector, class Transform4>
 inline std::vector<int> SearchBySE3(Context& ctx, const KFPtr& kf1, const std::vector<KFPtr>& kf2, std::vector<LandmarkVector>& matches12,
                                     const std::vector<Transform4>& T12, const std::vector<Transform4>& T21, double th,
                                     int desc_matching_th_low, int num_octaves, double scale_factor) {
-  auto flatten = [](const KFPtr& kf, KfViewStorage& S) {
-    const size_t n = kf->keypoints_distorted_.size();
-    S.kp.resize(2 * n); S.octave.resize(n); S.desc.resize(32 * n); S.lm_valid.assign(n, 0); S.lm_pos.assign(3 * n, 0.0);
-    S.lm_maxdist.assign(n, 1.0); S.lm_desc.assign(32 * n, 0);
-    const auto lms = kf->GetLandmarks();
-    for (size_t i = 0; i < n; i++) {
-      S.kp[2 * i] = kf->keypoints_distorted_[i][0]; S.kp[2 * i + 1] = kf->keypoints_distorted_[i][1];
-      S.octave[i] = kf->keypoints_aors_[i][1];
-      std::copy(kf->GetDescriptor(i), kf->GetDescriptor(i) + 32, S.desc.begin() + 32 * i);
-      if (lms[i] && !lms[i]->IsInvalid()) {
-        S.lm_valid[i] = 1;
-        const auto p = lms[i]->GetWorldPos();
-        for (int c = 0; c < 3; c++) S.lm_pos[3 * i + c] = p[c];
-        S.lm_maxdist[i] = lms[i]->GetMaxDistance();
-        std::copy(lms[i]->GetDescriptorPtr(), lms[i]->GetDescriptorPtr() + 32, S.lm_desc.begin() + 32 * i);
-      }
-    }
-    const auto Tcw = kf->GetPoseTcw();
-    for (int r = 0; r < 4; r++) for (int c = 0; c < 4; c++) S.v.Tcw[4 * r + c] = Tcw(r, c);
-    for (int r = 0; r < 3; r++) for (int c = 0; c < 3; c++) S.v.K[3 * r + c] = kf->calibration_K(r, c);
-    S.v.img[0] = kf->img_dim_x_min_; S.v.img[1] = kf->img_dim_x_max_; S.v.img[2] = kf->img_dim_y_min_; S.v.img[3] = kf->img_dim_y_max_;
-    S.assign_grid(kf->image_width(), kf->image_height());
-  };
+  const auto flatten = [](const KFPtr& kf, KfViewStorage& S) { detail::flatten_kf_view(kf, S); };
   const int n_pairs = (int)kf2.size();
   KfViewStorage S1;
   flatten(kf1, S1);
@@ -865,6 +874,105 @@ inline std::vector<int> SearchBySE3(Context& ctx, const KFPtr& kf1, const std::v
     found[p] = nf[p];
   }
   return found;
+}
+
+// The parameters of the COVINS verification (placerec_be.cpp:85-151 and the settings it reads).
+struct LandmarkVerifyParams {
+  float distance_threshold = 50.0f;   // LandmarkMatchingAlgorithm(50.0)
+  int num_best = 4;                   // DenseMatcher numBest
+  int matches_thres = 25;             // the nmatches discard (:93-99)
+  double ransac_threshold = 0.0;      // Se3Solver's RANSAC threshold
+  int ransac_max_iterations = 0;
+  double ransac_probability = 0.99;
+  int min_ransac_inliers = 0;         // the gate after the RANSAC
+  double search_radius_SE3 = 9.5;     // SearchBySE3
+  int desc_matching_th_low = 50;
+  int num_octaves = 1;
+  double scale_factor = 2.0;
+  double th_outlier_align = 1.3;      // OptimizeRelativePose
+};
+template <class Transform4>
+struct LandmarkVerifyOutcome {
+  int n_matches = 0, best_sample = -1, best_count = 0, n_found = 0, n_corr = 0, n_inliers = 0;
+  double T12_pose[7] = {0, 0, 0, 0, 0, 0, 0};   // [qx,qy,qz,qw, x,y,z] after OptimizeRelativePose (the start pose when n_inliers == 0)
+  Transform4 T12;                                // refined when n_inliers > 0, else as handed to the refinement (zero if the candidate stopped)
+};
+
+// The candidate loop of PlaceRecognition::ComputeSE3 (placerec_be.cpp:85-151: DenseMatcher, the nmatches discard,
+// Se3Solver::projectiveAlignment, SearchBySE3, OptimizeRelativePose) for every candidate of kf_query in one call
+// (cvb_verify_landmark_candidates_seeded_batch).  vvpMapPointMatches[c] is written as the reference holds it after
+// OptimizeRelativePose: kf_query's keypoint i -> the candidate's landmark (GetLandmarks()[b]) of the LandmarkVector handed to the
+// refinement, with the reference's purge quirk applied (matches1[r] = nullptr for every purged RESIDUAL index r,
+// optimization_be.cpp:815); all null for a candidate that stops before SearchBySE3.  The acceptance test stays with the caller.
+// Members used beyond SearchBySE3's: KF::GetPoseTws / GetStateExtrinsics and, through Adapter<KF>, the camera, its model and the
+// query's bearing vectors and sigma angles (Adapter<KF>::bearings).
+template <class KFPtr, class LandmarkVector, class Transform4>
+inline std::vector<LandmarkVerifyOutcome<Transform4>> VerifyLandmarkCandidates(Context& ctx, const KFPtr& kf_query, const std::vector<KFPtr>& candidates,
+                                                                               std::vector<LandmarkVector>& vvpMapPointMatches,
+                                                                               const LandmarkVerifyParams& P, const std::vector<uint64_t>& seeds) {
+  using KF = typename std::decay<decltype(*kf_query)>::type;
+  const int C = (int)candidates.size();
+  if ((int)seeds.size() != C) {
+    std::printf("FATAL: VerifyLandmarkCandidates: %d seeds for %d candidates\n", (int)seeds.size(), C);
+    std::exit(-1);
+  }
+  const auto fill = [](const KFPtr& kf, KfViewStorage& S, cvb_landmark_kf& k) {
+    detail::flatten_kf_view(kf, S);
+    k.view = *S.view();
+    const auto Tws = kf->GetPoseTws(), Tsc = kf->GetStateExtrinsics();
+    for (int r = 0; r < 4; r++) for (int c = 0; c < 4; c++) { k.T_ws[4 * r + c] = Tws(r, c); k.T_sc[4 * r + c] = Tsc(r, c); }
+    if (!Adapter<KF>::camera(*kf, k.intr, k.dist)) {
+      std::printf("FATAL: Unknown projection type.\n");                                              // optimization_be.cpp:705-707
+      std::exit(-1);
+    }
+    Adapter<KF>::camera_model(*kf, &k.cam_model, &k.dist_model, &k.xi);
+  };
+  KfViewStorage Sq;
+  cvb_landmark_kf q{};
+  fill(kf_query, Sq, q);
+  const int nq = q.view.n;
+  std::vector<double> bear(3 * (size_t)nq), sig((size_t)nq);
+  Adapter<KF>::bearings(*kf_query, bear.data(), sig.data());
+  q.bearings = bear.data(); q.sigma_angle = sig.data();
+  std::vector<KfViewStorage> S(C);
+  std::vector<cvb_landmark_kf> cand(C > 0 ? C : 1);
+  for (int c = 0; c < C; c++) fill(candidates[c], S[c], cand[c]);
+  cvb_landmark_verify_params prm{P.distance_threshold, P.num_best, P.matches_thres, P.ransac_threshold, P.ransac_max_iterations,
+                                 P.ransac_probability, P.min_ransac_inliers,
+                                 {P.search_radius_SE3, P.desc_matching_th_low, P.num_octaves, P.scale_factor}, P.th_outlier_align};
+  const size_t Cn = C > 0 ? (size_t)C : 1, L = (size_t)C * nq + 1;
+  std::vector<int32_t> n_matches(Cn), best_sample(Cn), best_count(Cn), iterations(Cn), consumed(Cn), n_found(Cn), n_corr(Cn), n_inliers(Cn),
+      solve_it(2 * Cn), match12(L);
+  std::vector<double> best_model(12 * Cn), T12(16 * Cn), T21(16 * Cn), T12_out(7 * Cn);
+  std::vector<uint8_t> stage(L), removed(L);
+  cvb_landmark_verify_result res{n_matches.data(), best_sample.data(), best_model.data(), best_count.data(), iterations.data(), consumed.data(),
+                                 T12.data(), T21.data(), n_found.data(), n_corr.data(), T12_out.data(), n_inliers.data(), solve_it.data(),
+                                 match12.data(), stage.data(), removed.data()};
+  ctx.check(cvb_verify_landmark_candidates_seeded_batch(ctx.get(), &q, cand.data(), C, &prm, seeds.data(), &res),
+            "cvb_verify_landmark_candidates_seeded_batch");
+  vvpMapPointMatches.assign(C, LandmarkVector(nq));
+  std::vector<LandmarkVerifyOutcome<Transform4>> out(C);
+  for (int c = 0; c < C; c++) {
+    const auto lms2 = candidates[c]->GetLandmarks();
+    LandmarkVector& v = vvpMapPointMatches[c];
+    for (int i = 0; i < nq; i++) {
+      const int32_t b = match12[(size_t)c * nq + i];
+      if (b >= 0) v[i] = lms2[b];
+    }
+    for (int r = 0; r < n_corr[c]; r++)
+      if (removed[(size_t)c * nq + r]) v[r] = nullptr;                                               // matches1[r], r = residual index (:815)
+    auto& o = out[c];
+    o.n_matches = n_matches[c]; o.best_sample = best_sample[c]; o.best_count = best_count[c]; o.n_found = n_found[c];
+    o.n_corr = n_corr[c]; o.n_inliers = n_inliers[c];
+    for (int k = 0; k < 7; k++) o.T12_pose[k] = T12_out[7 * (size_t)c + k];
+    if (o.n_inliers > 0) {
+      o.T12 = detail::pose7_to_transform<Transform4>(o.T12_pose);                                  // :829
+    } else {
+      o.T12 = Transform4::Identity();
+      for (int r = 0; r < 4; r++) for (int k = 0; k < 4; k++) o.T12(r, k) = T12[16 * (size_t)c + 4 * r + k];
+    }
+  }
+  return out;
 }
 
 // FeatureMatcher::SearchByProjection(pKF, Tcw, vpPoints, vpMatched, th) (feature_matcher_be.cpp:168-291): loop landmarks projected

@@ -295,6 +295,18 @@ int abs_ransac(cvb_ctx* ctx, const char* name, const cvb_abs_ransac_problems* p,
 
 }  // namespace
 
+int cvb_abs_ransac_seeded_dev(cvb_ctx* ctx, int n_prob, const int32_t* d_prob_ptr, const double* d_pts, const double* d_f, const double* d_sigma,
+                              const double* d_cam, const uint64_t* d_seed, double threshold, int max_iterations, double probability,
+                              int32_t* d_best_sample, double* d_best_model, int32_t* d_best_count, int32_t* d_iterations, int32_t* d_consumed,
+                              uint8_t* d_inlier_mask) {
+  if (n_prob == 0) return CVB_OK;
+  RansacDev D{};
+  D.prob_ptr = d_prob_ptr; D.pts = d_pts; D.f = d_f; D.sigma = d_sigma; D.cam = d_cam;
+  set_outputs(D.o, 0, max_iterations, threshold, probability, d_best_sample, d_best_model, d_best_count, d_iterations, d_consumed, d_inlier_mask);
+  D.o.seed = (const unsigned long long*)d_seed;
+  return launch_ransac(ctx, ransac_abs_kernel<SeededSamples<4>>, 0, D, n_prob);
+}
+
 extern "C" int cvb_ransac_absolute_pose_batch(cvb_ctx* ctx, const cvb_abs_ransac_problems* p, double threshold, int max_iterations,
                                               double probability, cvb_abs_ransac_result* r) {
   if (!ctx) return CVB_ERR_INVALID;

@@ -8,6 +8,8 @@
 #include <float.h>
 #include <math.h>
 
+#include <cub/block/block_scan.cuh>
+
 #include "cvb_internal.cuh"
 #include "geom_common.cuh"
 
@@ -198,6 +200,32 @@ __device__ __forceinline__ void ransac_cta(const RansacOut& D, Problem& Pb, cons
   }
 }
 
+// ---- the glue kernels of the fused verification calls (ransac_rel.cu, geom_kernels.cu): one CTA of kGlueThreads per unit ----
+constexpr int kGlueThreads = 256;
+using GlueScan = cub::BlockScan<int, kGlueThreads>;
+
+// emit(i, rank) for every i < n with flag(i), rank = the number of flagged indices before i (a CTA-wide scan in chunks of
+// kGlueThreads); returns the number of flagged indices to every thread
+template <class Flag, class Emit>
+__device__ int scan_emit(int n, const Flag& flag, const Emit& emit) {
+  __shared__ typename GlueScan::TempStorage tmp;
+  __shared__ int carry;
+  __syncthreads();
+  if (threadIdx.x == 0) carry = 0;
+  __syncthreads();
+  for (int b = 0; b < n; b += kGlueThreads) {
+    const int i = b + threadIdx.x;
+    const int f = i < n && flag(i);
+    int rank, total;
+    GlueScan(tmp).ExclusiveSum(f, rank, total);
+    if (f) emit(i, carry + rank);
+    __syncthreads();
+    if (threadIdx.x == 0) carry += total;
+    __syncthreads();
+  }
+  return carry;
+}
+
 bool ptr_ok(const int32_t* p, int n) {
   if (p[0] != 0) return false;
   for (int i = 0; i < n; i++)
@@ -248,6 +276,14 @@ inline void set_selection(RansacOut& O, int ns, int max_iterations, double thres
   O.n_samples = ns; O.max_iterations = max_iterations; O.threshold = threshold; O.log_p = log(1.0 - probability);
 }
 
+// the selection parameters and the result pointers (device) of a RANSAC call; inlier_mask nullable
+inline void set_outputs(RansacOut& O, int ns, int max_iterations, double threshold, double probability, int* best_sample, double* best_model,
+                        int* best_count, int* iterations, int* consumed, uint8_t* inlier_mask) {
+  set_selection(O, ns, max_iterations, threshold, probability);
+  O.best_sample = best_sample; O.best_model = best_model; O.best_count = best_count; O.iterations = iterations; O.consumed = consumed;
+  O.inlier_mask = inlier_mask;
+}
+
 // The launcher: kernel on device inputs and outputs D (one CTA per problem, smem bytes of dynamic shared memory) on ctx's stream.
 template <class Dev>
 int launch_ransac(cvb_ctx* ctx, void (*kernel)(Dev), size_t smem, const Dev& D, int n_prob) {
@@ -277,9 +313,8 @@ int run_ransac(cvb_ctx* ctx, int ws_slot, void (*kernel)(Dev), size_t smem, Stag
   memcpy(hpin, St.h.data(), in_bytes);
   Dev D = inputs(d);
   RansacOut& O = D.o;
-  set_selection(O, ns, max_iterations, threshold, probability);
-  O.best_sample = (int*)(d + o_bs); O.best_model = (double*)(d + o_bm); O.best_count = (int*)(d + o_bc); O.iterations = (int*)(d + o_it);
-  O.consumed = (int*)(d + o_us); O.inlier_mask = r->inlier_mask ? d + o_mask : nullptr;
+  set_outputs(O, ns, max_iterations, threshold, probability, (int*)(d + o_bs), (double*)(d + o_bm), (int*)(d + o_bc), (int*)(d + o_it),
+              (int*)(d + o_us), r->inlier_mask ? d + o_mask : nullptr);
   if (all) { O.sample_model = (double*)(d + o_sm); O.sample_valid = d + o_sv; O.sample_count = (int*)(d + o_sc); }
   cudaStream_t st = ctx->stream;
   CVB_CUDA(ctx, cudaMemcpyAsync(d, hpin, in_bytes, cudaMemcpyHostToDevice, st));

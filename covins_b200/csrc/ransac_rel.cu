@@ -1052,31 +1052,6 @@ extern "C" int cvb_noncentral_relative_pose_covariance_seeded_batch(cvb_ctx* ctx
 // by the host-known bound sum over pairings of rows(kf1); the problems are packed to the front in pairing (candidate) order.
 namespace {
 
-constexpr int kGlueThreads = 256;
-using GlueScan = cub::BlockScan<int, kGlueThreads>;
-
-// emit(i, rank) for every i < n with flag(i), rank = the number of flagged indices before i (a CTA-wide scan in chunks of
-// kGlueThreads); returns the number of flagged indices to every thread
-template <class Flag, class Emit>
-__device__ int scan_emit(int n, const Flag& flag, const Emit& emit) {
-  __shared__ typename GlueScan::TempStorage tmp;
-  __shared__ int carry;
-  __syncthreads();
-  if (threadIdx.x == 0) carry = 0;
-  __syncthreads();
-  for (int b = 0; b < n; b += kGlueThreads) {
-    const int i = b + threadIdx.x;
-    const int f = i < n && flag(i);
-    int rank, total;
-    GlueScan(tmp).ExclusiveSum(f, rank, total);
-    if (f) emit(i, carry + rank);
-    __syncthreads();
-    if (threadIdx.x == 0) carry += total;
-    __syncthreads();
-  }
-  return carry;
-}
-
 struct VerifyDev {
   const double* bearings; const double* sigma;          // keyframe table [R][3], [R]
   const int* pair_rows;                                  // [P][5] the matcher's pair table: query row0, rows, train row0, rows, offset

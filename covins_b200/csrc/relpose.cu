@@ -6,7 +6,8 @@
 //   robopt::reprojection::RelativeEuclideanReprError<Camera, Distortion>  kNormal (camera A sees B's point through T12)
 //                                                                         kInverse (camera B sees A's point through T12^-1)
 // [A: robopt_open is not in the tree; formulas restated, oracle/relpose_oracle.py], CauchyLoss(1.0), dogleg, 5 + 5
-// iterations.  The whole call is ONE kernel launch of ONE CTA: every thread linearises a strided share of the
+// iterations.  The whole call is ONE kernel launch of ONE CTA (the kernel reads its problem record from blockIdx.x, so
+// cvb_relpose_batch_dev refines a batch of problems, one CTA each, in the same launch): every thread linearises a strided share of the
 // correspondences, the 6x6 normal equations are reduced in shared memory in a fixed order (bit-reproducible), and thread 0
 // runs the Ceres trust-region logic (Jacobi scaling, dogleg, accept/reject — the same restatement as ba_engine.cu) on the
 // 6x6 system between the passes; the outlier purge and the second solve follow inside the same launch.  The problem is far
@@ -21,16 +22,8 @@ namespace {
 
 using namespace bam;
 
-struct RelCam {
-  double intr[4], dist[4];
-  int cam, dm;
-  double xi;
-};
-struct RelDev {
-  int n;
-  const double* pA; const double* pB; const float* kpA; const float* kpB; const double* sA; const double* sB;
-  RelCam camA, camB;
-};
+using RelCam = cvb_relcam;
+using RelDev = cvb_relpose_dev;
 
 constexpr int NT = 256, NW = NT / 32, NACC = 28;   // 21 (J^T J lower) + 6 (J^T r) + 1 (cost)
 
@@ -283,13 +276,22 @@ __device__ void solve(const RelDev& P, const uint8_t* removed, TrState& S, doubl
   __syncthreads();
 }
 
-__global__ void __launch_bounds__(NT, 1) relpose_kernel(RelDev P, const double* __restrict__ pose_in, double th_outlier, uint8_t* __restrict__ removed,
-                                                        double* __restrict__ out /* pose[7], n_inliers, it1, it2, n_hist, hist[16] */) {
+// problem blockIdx.x of probs; out: pose[7], n_inliers, it1, it2, n_hist, hist[16]
+__global__ void __launch_bounds__(NT, 1) relpose_kernel(const RelDev* __restrict__ probs, double th_outlier) {
   __shared__ TrState S;
   __shared__ double wsum[NW][NACC];
   __shared__ double red[NACC];
   __shared__ int n_bad;
+  const RelDev& P = probs[blockIdx.x];   // read-only for the whole launch
   const int tid = threadIdx.x;
+  const double* __restrict__ pose_in = P.pose_in;
+  uint8_t* __restrict__ removed = P.removed;
+  double* __restrict__ out = P.out;
+  if (P.n < 12) {   // cvb_optimize_relative_pose's early result: fewer than 12 correspondences can never pass :821
+    for (int i = tid; i < P.n; i += NT) removed[i] = 0;
+    for (int i = tid; i < CVB_RELPOSE_OUT; i += NT) out[i] = i < 7 ? pose_in[i] : 0.0;
+    return;
+  }
   if (tid == 0) { for (int c = 0; c < 7; c++) S.pose[c] = pose_in[c]; S.n_hist = 0; n_bad = 0; }
   for (int i = tid; i < P.n; i += NT) removed[i] = 0;
   __syncthreads();
@@ -357,7 +359,8 @@ extern "C" int cvb_optimize_relative_pose(cvb_ctx* ctx, const cvb_relpose_proble
   }
   const size_t o_pA = 0, o_pB = o_pA + (size_t)n * 24, o_sA = o_pB + (size_t)n * 24, o_sB = o_sA + (size_t)n * 8, o_kA = o_sB + (size_t)n * 8,
                o_kB = o_kA + (size_t)n * 8, o_pose = o_kB + (size_t)n * 8, in_bytes = o_pose + 56;
-  const size_t o_out = (in_bytes + 15) & ~size_t(15), o_rem = o_out + 27 * 8, total = o_rem + (size_t)n;
+  const size_t o_rec = (in_bytes + 15) & ~size_t(15), o_out = (o_rec + sizeof(RelDev) + 15) & ~size_t(15), o_rem = o_out + CVB_RELPOSE_OUT * 8,
+               total = o_rem + (size_t)n;
   unsigned char* d = (unsigned char*)cvb_ws(ctx, WS_GS3, total);
   unsigned char* h = (unsigned char*)cvb_pinned(ctx, total);
   if (!d || !h) return CVB_ERR_CUDA;
@@ -365,16 +368,18 @@ extern "C" int cvb_optimize_relative_pose(cvb_ctx* ctx, const cvb_relpose_proble
   memcpy(h + o_sA, p->sigmaA, (size_t)n * 8); memcpy(h + o_sB, p->sigmaB, (size_t)n * 8);
   memcpy(h + o_kA, p->kpA, (size_t)n * 8); memcpy(h + o_kB, p->kpB, (size_t)n * 8);
   memcpy(h + o_pose, p->T12, 56);
-  RelDev D;
+  RelDev D{};
   D.n = n;
   D.pA = (const double*)(d + o_pA); D.pB = (const double*)(d + o_pB); D.sA = (const double*)(d + o_sA); D.sB = (const double*)(d + o_sB);
   D.kpA = (const float*)(d + o_kA); D.kpB = (const float*)(d + o_kB);
   for (int c = 0; c < 4; c++) { D.camA.intr[c] = p->intrA[c]; D.camA.dist[c] = p->distA[c]; D.camB.intr[c] = p->intrB[c]; D.camB.dist[c] = p->distB[c]; }
   D.camA.cam = p->cam_model_A; D.camA.dm = p->dist_model_A; D.camA.xi = p->xiA;
   D.camB.cam = p->cam_model_B; D.camB.dm = p->dist_model_B; D.camB.xi = p->xiB;
+  D.pose_in = (const double*)(d + o_pose); D.removed = d + o_rem; D.out = (double*)(d + o_out);
+  memcpy(h + o_rec, &D, sizeof(D));
   cudaStream_t st = ctx->stream;
-  CVB_CUDA(ctx, cudaMemcpyAsync(d, h, in_bytes, cudaMemcpyHostToDevice, st));
-  relpose_kernel<<<1, NT, 0, st>>>(D, (const double*)(d + o_pose), th_outlier_align, d + o_rem, (double*)(d + o_out));
+  CVB_CUDA(ctx, cudaMemcpyAsync(d, h, o_rec + sizeof(D), cudaMemcpyHostToDevice, st));
+  relpose_kernel<<<1, NT, 0, st>>>((const RelDev*)(d + o_rec), th_outlier_align);
   CVB_CHECK_LAUNCH(ctx);
   CVB_CUDA(ctx, cudaMemcpyAsync(h + o_out, d + o_out, total - o_out, cudaMemcpyDeviceToHost, st));
   CVB_CUDA(ctx, cudaStreamSynchronize(st));
@@ -383,5 +388,12 @@ extern "C" int cvb_optimize_relative_pose(cvb_ctx* ctx, const cvb_relpose_proble
   *n_inliers = (int32_t)out[7];
   if (removed) memcpy(removed, h + o_rem, (size_t)n);
   if (info) for (int i = 0; i < 19; i++) info[i] = out[8 + i];
+  return CVB_OK;
+}
+
+int cvb_relpose_batch_dev(cvb_ctx* ctx, const cvb_relpose_dev* d_probs, int n_prob, double th_outlier_align) {
+  if (n_prob == 0) return CVB_OK;
+  relpose_kernel<<<n_prob, NT, 0, ctx->stream>>>(d_probs, th_outlier_align);
+  CVB_CHECK_LAUNCH(ctx);
   return CVB_OK;
 }

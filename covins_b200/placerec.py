@@ -15,6 +15,8 @@ the C-ABI:
                                   per problem, as the reference draws its own (include/covins_b200.h, "Seeded samples")
   verify_noncentral_relative_pose_seeded(...) ↔ the whole verification of RelNonCentralPosSolver::computeNonCentralRelPose
                                   (pairwise matching, 5-point and 17-point RANSAC, covariance) for all candidates in one call
+  verify_landmark_candidates_seeded(...) ↔ the COVINS verification of PlaceRecognition::ComputeSE3 (DenseMatcher landmark
+                                  matching, GP3P RANSAC, SearchBySE3, OptimizeRelativePose) for all candidates in one call
 
 `KfView` flattens what the reference reads of a Keyframe (the C++ shim does the same from the containers)."""
 from __future__ import annotations
@@ -436,3 +438,80 @@ def verify_noncentral_relative_pose_seeded(ctx: Context, kf_ptr, desc, bearings,
     if corr_cap and R.n_total <= corr_cap:
         r["corr"] = corr[:R.n_total].copy()
     return r
+
+
+class CLandmarkKf(C.Structure):
+    _fields_ = [("view", CKfView), ("bearings", c_vp), ("sigma_angle", c_vp), ("T_ws", C.c_double * 16), ("T_sc", C.c_double * 16),
+                ("intr", C.c_double * 4), ("dist", C.c_double * 4), ("cam_model", C.c_int32), ("dist_model", C.c_int32), ("xi", C.c_double)]
+
+
+class CLandmarkVerifyParams(C.Structure):
+    _fields_ = [("thr", C.c_float), ("num_best", C.c_int32), ("min_matches", C.c_int32), ("threshold", C.c_double), ("max_iterations", C.c_int32),
+                ("probability", C.c_double), ("min_ransac_inliers", C.c_int32), ("search", CSearchParams), ("th_outlier_align", C.c_double)]
+
+
+class CLandmarkVerifyResult(C.Structure):
+    _fields_ = [(k, c_vp) for k in ("n_matches", "best_sample", "best_model", "best_count", "iterations", "consumed", "T12", "T21", "n_found", "n_corr",
+                                    "T12_out", "n_inliers", "solve_iterations", "match12", "stage", "removed")]
+
+
+class LandmarkKf:
+    """a keyframe of verify_landmark_candidates_seeded: the KfView SearchBySE3 reads, plus bearings [n,3] (unit, camera frame) and
+    sigma_angle [n] (read of the query only), T_ws / T_sc (4x4 body in world, camera in body) and the camera model
+    cam = dict(intr[4], dist[4], cam_model=0, dist_model=0, xi=0) of optimize_relative_pose"""
+
+    def __init__(self, view: KfView, T_ws, T_sc, cam: dict, bearings=None, sigma_angle=None):
+        self.view, self.cam = view, cam
+        self.T_ws = np.asarray(T_ws, np.float64).reshape(16); self.T_sc = np.asarray(T_sc, np.float64).reshape(16)
+        self.bearings = np.ascontiguousarray(np.zeros((view.n, 3)) if bearings is None else bearings, np.float64).reshape(view.n, 3)
+        self.sigma_angle = np.ascontiguousarray(np.ones(view.n) if sigma_angle is None else sigma_angle, np.float64).reshape(view.n)
+
+    def cstruct(self):
+        s = CLandmarkKf()
+        s.view = self.view.cstruct()
+        s.bearings, s.sigma_angle = self.bearings.ctypes.data, self.sigma_angle.ctypes.data
+        s.T_ws[:] = self.T_ws.tolist(); s.T_sc[:] = self.T_sc.tolist()
+        s.intr[:] = [float(x) for x in np.asarray(self.cam["intr"]).reshape(4)]; s.dist[:] = [float(x) for x in np.asarray(self.cam["dist"]).reshape(4)]
+        s.cam_model, s.dist_model, s.xi = int(self.cam.get("cam_model", 0)), int(self.cam.get("dist_model", 0)), float(self.cam.get("xi", 0.0))
+        return s
+
+
+def landmark_verify_prepared(ctx: Context, query: LandmarkKf, cands, seeds, min_matches, threshold, max_iterations, min_ransac_inliers, thr=50.0,
+                             num_best=4, probability=0.99, th=9.5, desc_th_low=50, num_octaves=1, scale_factor=2.0, th_outlier_align=1.3, detail=True):
+    """PlaceRecognition::ComputeSE3's verification of place-recognition candidates in one call
+    (cvb_verify_landmark_candidates_seeded_batch): DenseMatcher landmark matching of the query against every candidate, a seeded
+    GP3P RANSAC per candidate with at least min_matches matches, the gate (best_count >= min_ransac_inliers), SearchBySE3 and the
+    relative-pose refinement.  cands: LandmarkKf list, seeds [n_cand] uint64.  detail: also the [n_cand, n_query] outputs.
+    → dict(n_matches, best_sample, best_model [C,3,4], best_count, iterations, consumed, T12 / T21 [C,4,4], n_found, n_corr,
+    T12_out [C,7], n_inliers, solve_iterations [C,2]) and, with detail, match12 [C,nq] i32, stage [C,nq] u8 (0 none, 1 DenseMatcher
+    match not kept by the RANSAC, 2 RANSAC inlier, 3 added by SearchBySE3), removed [C,nq] u8 (by residual index, < n_corr).
+    Packs the arguments once and returns (call, result dict): call() runs the C call on them and returns the filled dict."""
+    C_, nq = len(cands), query.view.n
+    s = _seeds(seeds, C_)
+    r = dict(n_matches=np.zeros(C_, np.int32), best_sample=np.zeros(C_, np.int32), best_model=np.zeros((C_, 3, 4)), best_count=np.zeros(C_, np.int32),
+             iterations=np.zeros(C_, np.int32), consumed=np.zeros(C_, np.int32), T12=np.zeros((C_, 4, 4)), T21=np.zeros((C_, 4, 4)),
+             n_found=np.zeros(C_, np.int32), n_corr=np.zeros(C_, np.int32), T12_out=np.zeros((C_, 7)), n_inliers=np.zeros(C_, np.int32),
+             solve_iterations=np.zeros((C_, 2), np.int32))
+    if detail:
+        r.update(match12=np.zeros((C_, nq), np.int32), stage=np.zeros((C_, nq), np.uint8), removed=np.zeros((C_, nq), np.uint8))
+    q = query.cstruct()
+    arr = (CLandmarkKf * max(C_, 1))(*[c.cstruct() for c in cands])
+    prm = CLandmarkVerifyParams(float(thr), int(num_best), int(min_matches), float(threshold), int(max_iterations), float(probability),
+                                int(min_ransac_inliers), CSearchParams(float(th), int(desc_th_low), int(num_octaves), float(scale_factor)),
+                                float(th_outlier_align))
+    R = CLandmarkVerifyResult(*[r[k].ctypes.data if k in r else None for k, _ in CLandmarkVerifyResult._fields_])
+    keep = (q, arr, prm, R, s, query, cands)
+
+    def call():
+        ctx.check(lib().cvb_verify_landmark_candidates_seeded_batch(ctx.handle, C.byref(keep[0]), keep[1], C_, C.byref(keep[2]), keep[4].ctypes.data,
+                                                                    C.byref(keep[3])))
+        return r
+    return call, r
+
+
+def verify_landmark_candidates_seeded(ctx: Context, query: LandmarkKf, cands, seeds, min_matches, threshold, max_iterations, min_ransac_inliers,
+                                      **kw):
+    """PlaceRecognition::ComputeSE3's verification of place-recognition candidates in one call
+    (cvb_verify_landmark_candidates_seeded_batch); the arguments and result of landmark_verify_prepared, which see"""
+    call, _ = landmark_verify_prepared(ctx, query, cands, seeds, min_matches, threshold, max_iterations, min_ransac_inliers, **kw)
+    return call()

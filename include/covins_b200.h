@@ -652,6 +652,96 @@ CVB_API int cvb_verify_noncentral_relative_pose_seeded_batch(cvb_ctx* ctx, const
                                                              cvb_verify_result* r);
 
 /*
+ * The COVINS verification of place-recognition candidates (PlaceRecognition::ComputeSE3, placerec_be.cpp:63-220, up to the
+ * acceptance test: DenseMatcher landmark matching, the nmatches < matches_thres discard, Se3Solver's GP3P RANSAC,
+ * FeatureMatcher::SearchBySE3 and Optimization::OptimizeRelativePose) for all candidates of one query keyframe in one call: one
+ * upload, every stage on the ctx's stream, one download.
+ *   Semantics: exactly the composition of the calls above on the same inputs and seeds, n = query->view.n:
+ *     1. Matches: cvb_landmark_match_batch(A = query desc, skipA = !query lm_valid, B = the candidates' desc concatenated (one
+ *        segment each), skipB = !lm_valid, thr, num_best).  n_matches[c] = the candidate's match count.
+ *     2. RANSAC problem of candidate c: none if n_matches[c] < min_matches (placerec_be.cpp:93-99: nothing is drawn,
+ *        best_sample = -1); otherwise one correspondence per match in ascending idxA: pts = cand lm_pos[idxB] (world),
+ *        f = query bearings[idxA], sigma = query sigma_angle[idxA], camera = the query's T_sc (c = its translation, Rc = its
+ *        rotation).  Solved by cvb_ransac_absolute_pose_seeded_batch(threshold, max_iterations, probability) with seed[c].
+ *        ASSUMPTIONS (Se3Solver is not in the tree): it walks the LandmarkVector in keypoint order, and it takes world points and
+ *        the body-frame camera, as cvb_ransac_absolute_pose_batch does.  DenseMatcher gives each A at most one B, so the order
+ *        is well defined.
+ *     3. Gate: a candidate continues iff best_sample >= 0 && best_count >= min_ransac_inliers.  Then, M the model as a 4x4,
+ *        T12 = rigid_inv(M * query T_sc) * rigid_inv(cand view.Tcw) (T_c1_w times T_w_c2) and T21 = rigid_inv(T12), with
+ *        rigid_inv([R|t]) = [R^T | -R^T t]; every entry of a product is its four (rigid_inv: three) products summed left to
+ *        right without fused multiply-add, so a float64 restatement in the same order gives the same bits.  (The reference
+ *        computes T21 with Eigen's general inverse().)  A candidate that stops gets n_found = n_corr = n_inliers = 0, zero
+ *        T12 / T21 / T12_out and no entry after the RANSAC stage.
+ *     4. SearchBySE3: cvb_search_by_se3_batch(kf1 = query view, kf2 = candidate view, T12, T21, search) with already1[i] = 1
+ *        iff query keypoint i holds a RANSAC inlier and already2[b] = 1 iff candidate keypoint b is the idxB of one (the flat
+ *        form identifies a candidate landmark's GetFeatureIndex(kf2) with the keypoint b where it sits).  The LandmarkVector
+ *        after this stage: the RANSAC inliers (i -> idxB) plus the search's match12 (disjoint: the search skips already1).
+ *     5. Refinement: one residual pair per LandmarkVector entry (i -> b) in ascending i whose two landmarks are valid (query
+ *        lm_valid[i], cand lm_valid[b]; the reference skips a null or invalid landmark), as the shim's OptimizeRelativePose builds
+ *        it: pA_c = TcwA * query lm_pos[i], pB_c = TcwB * cand lm_pos[b], TcwA = rigid_inv(query T_ws * query T_sc), TcwB =
+ *        rigid_inv(cand T_ws * query T_sc) (kf1's extrinsics for both, optimization_be.cpp:643; these two are formed on the
+ *        host), kpA / kpB the two keypoints, sigma = (double)(octave + 1.0f) * 2.0, each keyframe's camera; T12 as [q, t] by
+ *        the shim's transform_to_pose7 (Eigen's matrix-to-quaternion branches).  Then cvb_optimize_relative_pose
+ *        (th_outlier_align) gives T12_out, n_inliers and removed.  The acceptance test (n_inliers against the reference's
+ *        threshold, the first accepted candidate) stays with the caller.
+ * Inputs: query and cand [n_cand] (cvb_landmark_kf: the cvb_kf_view of cvb_search_by_se3_batch plus bearings [n][3] (unit,
+ * camera frame), sigma_angle [n], T_ws / T_sc (row-major 4x4 body in world, camera in body) and the camera model of
+ * cvb_relpose_problem; only the query's bearings / sigma_angle / T_sc are read), seed [n_cand] (stream 0 of the seeded sampler).
+ * Outputs per candidate (cvb_landmark_verify_result): n_matches; the RANSAC's best_sample / best_model [12] / best_count /
+ * iterations / consumed; T12 / T21 [16] as used; n_found (the search's return value); n_corr (residual pairs); T12_out [7],
+ * n_inliers and solve_iterations [2] (the two ceres::Solve iteration counts).  Nullable, each [n_cand][n]: match12 (the
+ * LandmarkVector handed to the refinement: the candidate keypoint of query keypoint i, or -1), stage (u8: 0 none, 1 DenseMatcher
+ * match that is not a RANSAC inlier of a candidate that continues, 2 RANSAC inlier, 3 added by SearchBySE3) and removed (u8,
+ * indexed by the residual r < n_corr: the reference nulls matches1[r], optimization_be.cpp:815).
+ * Errors: CVB_ERR_INVALID before any launch for null required pointers, a malformed view, num_best outside 1..4, thr outside
+ * (0, 257], bad search parameters or max_iterations outside [0, (INT32_MAX - 64) / 11]; CVB_ERR_UNSUPPORTED ("Unknown
+ * projection type." / "Unknown distortion type.") for a camera or distortion model of the query or a candidate that
+ * cvb_optimize_relative_pose does not know; n_cand = 0 succeeds.
+ */
+typedef struct cvb_landmark_kf {
+  cvb_kf_view view;
+  const double* bearings;    /* [n][3] */
+  const double* sigma_angle; /* [n] */
+  double T_ws[16];           /* GetPoseTws(), row-major */
+  double T_sc[16];           /* GetStateExtrinsics(), row-major */
+  double intr[4], dist[4];
+  int32_t cam_model, dist_model;
+  double xi;
+} cvb_landmark_kf;
+typedef struct cvb_landmark_verify_params {
+  float thr;                 /* DenseMatcher distance threshold (50) */
+  int32_t num_best;          /* 1..4 (4) */
+  int32_t min_matches;       /* matches_thres */
+  double threshold;          /* RANSAC */
+  int32_t max_iterations;
+  double probability;
+  int32_t min_ransac_inliers;
+  cvb_search_params search;
+  double th_outlier_align;
+} cvb_landmark_verify_params;
+typedef struct cvb_landmark_verify_result {
+  int32_t* n_matches;        /* [n_cand] */
+  int32_t* best_sample;      /* [n_cand] */
+  double* best_model;        /* [n_cand][12] */
+  int32_t* best_count;       /* [n_cand] */
+  int32_t* iterations;       /* [n_cand] */
+  int32_t* consumed;         /* [n_cand] */
+  double* T12;               /* [n_cand][16] */
+  double* T21;               /* [n_cand][16] */
+  int32_t* n_found;          /* [n_cand] */
+  int32_t* n_corr;           /* [n_cand] */
+  double* T12_out;           /* [n_cand][7] */
+  int32_t* n_inliers;        /* [n_cand] */
+  int32_t* solve_iterations; /* [n_cand][2] */
+  int32_t* match12;          /* [n_cand][n] nullable */
+  uint8_t* stage;            /* [n_cand][n] nullable */
+  uint8_t* removed;          /* [n_cand][n] nullable */
+} cvb_landmark_verify_result;
+CVB_API int cvb_verify_landmark_candidates_seeded_batch(cvb_ctx* ctx, const cvb_landmark_kf* query, const cvb_landmark_kf* cand, int n_cand,
+                                                        const cvb_landmark_verify_params* prm, const uint64_t* seed,
+                                                        cvb_landmark_verify_result* r);
+
+/*
  * Optimization::OptimizeRelativePose(kf1, kf2, matches1, T12, th2) (optimization_be.cpp:620-831): the 6-dof refinement of
  * the relative pose T12 from the matched landmark pairs, both ceres::Solve calls (5 + 5 iterations, DOGLEG, CauchyLoss(1))
  * and the outlier purge between them, in one call.  The caller (shim) flattens, per residual pair r (the reference's
