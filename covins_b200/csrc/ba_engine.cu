@@ -155,6 +155,7 @@ struct Engine {
   int n_sb = 0;
   // vectors of size n_vec: [cam part n_c_pad | landmark part 3 L_in]
   DevArr<double> scale, colsq, diag, gvec, grad, sgrad, gn, step, xsol, yb, gs, tmp;
+  DevArr<double> scale0;   // 0/1 activity mask of this rank's columns: engine_begin derives `scale` from it
   DevArr<double> S, linv;
   DevArr<int> flag;
   DevArr<double> partials, scalars, rankmax;
@@ -195,7 +196,7 @@ struct Engine {
     edge_robust.free_();
     fb_hi.free_(); fb_lo.free_(); fb_ptr.free_(); ft_type.free_(); ft_fac.free_(); ft_rhi.free_(); ft_rlo.free_();
     sb_hi.free_(); sb_lo.free_(); sb_ptr.free_(); sp_a.free_(); sp_b.free_();
-    scale.free_(); colsq.free_(); diag.free_(); gvec.free_(); grad.free_(); sgrad.free_(); gn.free_(); step.free_();
+    scale.free_(); scale0.free_(); colsq.free_(); diag.free_(); gvec.free_(); grad.free_(); sgrad.free_(); gn.free_(); step.free_();
     xsol.free_(); yb.free_(); gs.free_(); tmp.free_();
     if (S_raw) { S.p = nullptr; linv.p = nullptr; }
     S.free_(); linv.free_(); flag.free_(); partials.free_();
@@ -1586,7 +1587,7 @@ int engine_setup(Engine& E, const cvb_ba_problem* p, const cvb_ba_options* o) {
   for (int c = 0; c < E.L_in; c++)   // landmark blocks are owned by rank (c % world); others stay inactive here
     if (c % E.world == E.rank)
       for (int a = 0; a < 3; a++) h_scale[(size_t)E.n_c_pad + 3 * (size_t)c + a] = 1.0;
-  if ((rc = upload(E, E.scale, h_scale))) return rc;
+  if ((rc = upload(E, E.scale0, h_scale)) || (rc = zalloc(E, E.scale, (size_t)E.n_vec))) return rc;
   if ((rc = upload(E, E.off_pose, E.h_off_pose)) || (rc = upload(E, E.off_sb, E.h_off_sb))) return rc;
   if ((rc = E.plan.upload(E.ctx, E.st))) return rc;
   if (E.world > 1) {
@@ -1784,7 +1785,10 @@ int linearize(Engine& E, double* cost) {
 }
 
 int engine_begin(Engine& E) {
-  // iteration 0 of TrustRegionMinimizer: evaluate, fix the Jacobi scaling at x0, re-linearise in the scaled space
+  // iteration 0 of TrustRegionMinimizer: evaluate, fix the Jacobi scaling at x0, re-linearise in the scaled space.
+  // The first evaluation must see the unscaled Jacobian, so `scale` starts from the activity mask every time: a restart
+  // that kept the previous solve's scaling would take the column norms of an already scaled Jacobian.
+  ENG_CUDA(cudaMemcpyAsync(E.scale.p, E.scale0.p, (size_t)E.n_vec * sizeof(double), cudaMemcpyDeviceToDevice, E.st));
   double c0;
   int rc = linearize(E, &c0);
   if (rc) return rc;
