@@ -89,6 +89,7 @@ SIGNATURES = {
     "cvb_ransac_central_relative_pose_seeded_batch": (C.c_int, [c_vp, c_vp, c_vp, C.c_double, C.c_int, C.c_double, c_vp, c_vp]),
     "cvb_noncentral_relative_pose_covariance_seeded_batch": (C.c_int, [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
     "cvb_verify_noncentral_relative_pose_seeded_batch": (C.c_int, [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
+    "cvb_verify_noncentral_relative_pose_sift_seeded_batch": (C.c_int, [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
     "cvb_verify_landmark_candidates_seeded_batch": (C.c_int, [c_vp, c_vp, c_vp, C.c_int, c_vp, c_vp, c_vp]),
     "cvb_ba_iterate": (C.c_int, [c_vp, C.c_int, C.POINTER(C.c_int)]),
     "cvb_ba_result_get": (C.c_int, [c_vp, c_vp, c_vp]),

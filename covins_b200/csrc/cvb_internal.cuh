@@ -60,8 +60,11 @@ void* cvb_pinned(cvb_ctx* ctx, size_t bytes);
 // match_kernels.cu: the fused 2-NN + ratio filter of cvb_match_hamming_batch for n_pairs pairs of keyframes of one device
 // descriptor table d_desc in one launch on ctx->stream.  d_pairs [n_pairs][5] = (query row0, query rows, train row0, train rows,
 // output offset); pair s writes match_train / match_dist [offset + query] and n_matches [s]; max_nq: the largest query count.
+// cvb_match_l2_pairs_dev: the same for cvb_match_l2_batch on the u8 SIFT layout, d_desc [rows][128] (16-byte aligned).
 int cvb_match_hamming_pairs_dev(cvb_ctx* ctx, const uint8_t* d_desc, const int32_t* d_pairs, int n_pairs, int max_nq, float thr, float ratio,
                                 int32_t* d_match_train, float* d_match_dist, int32_t* d_n_matches);
+int cvb_match_l2_pairs_dev(cvb_ctx* ctx, const uint8_t* d_desc, const int32_t* d_pairs, int n_pairs, int max_nq, float thr, float ratio,
+                           int32_t* d_match_train, float* d_match_dist, int32_t* d_n_matches);
 
 // ransac_abs.cu: the seeded GP3P RANSAC of cvb_ransac_absolute_pose_seeded_batch on device inputs and outputs (one CTA per
 // problem on ctx->stream).  d_cam [n_prob][12] = camera offset (3) then rotation (9, row-major); d_inlier_mask nullable.

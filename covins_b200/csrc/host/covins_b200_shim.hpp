@@ -1290,20 +1290,36 @@ struct VerifyResult {
   std::vector<VerifyCandidateResult> candidates;
   std::vector<VerifyCorrespondence> correspondences;    // every match, pairing then match order
 };
-inline VerifyResult VerifyNonCentralRelativePose(Context& ctx, const std::vector<VerifyKeyframeView>& keyframes,
-                                                 const std::vector<VerifyCandidate>& candidates, const VerifyParams& params,
-                                                 const std::vector<uint64_t>& seeds5, const std::vector<uint64_t>& seeds) {
-  const int n_kf = (int)keyframes.size(), C = (int)candidates.size();
-  std::vector<int32_t> kf_ptr(n_kf + 1, 0), cp1(C + 1, 0), cp2(C + 1, 0), pair_ptr(C + 1, 0), pairs;
-  std::vector<uint8_t> desc;
-  std::vector<double> bear, sig, co1, cr1, co2, cr2;
-  for (int k = 0; k < n_kf; k++) {
-    const VerifyKeyframeView& v = keyframes[k];
+
+// The same with SIFT descriptors (cvb_verify_noncentral_relative_pose_sift_seeded_batch): n rows of descriptors_add_ [128] as
+// CV_32F, integer-valued in [0, 255] as cv::xfeatures2d::SIFT writes them; each pairing is matched by exact L2 2-NN + the filter.
+struct VerifyKeyframeViewSIFT {
+  const float* desc; const double* bearings; const double* sigma; int n;
+};
+
+namespace detail {
+// the keyframe table of VerifyNonCentralRelativePose: the views' rows concatenated, kDim descriptor elements per row
+template <size_t kDim, class View, class T>
+void flatten_verify_keyframes(const std::vector<View>& keyframes, std::vector<int32_t>& kf_ptr, std::vector<T>& desc, std::vector<double>& bear,
+                              std::vector<double>& sig) {
+  kf_ptr.assign(keyframes.size() + 1, 0);
+  for (size_t k = 0; k < keyframes.size(); k++) {
+    const View& v = keyframes[k];
     kf_ptr[k + 1] = kf_ptr[k] + v.n;
-    desc.insert(desc.end(), v.desc, v.desc + 32 * (size_t)v.n);
+    desc.insert(desc.end(), v.desc, v.desc + kDim * (size_t)v.n);
     bear.insert(bear.end(), v.bearings, v.bearings + 3 * (size_t)v.n);
     sig.insert(sig.end(), v.sigma, v.sigma + v.n);
   }
+}
+
+// the candidates, rigs, parameters and results of VerifyNonCentralRelativePose around one C call: call(D, prm, R) runs it on
+// them (kf_ptr: the keyframe table's row offsets, which size the correspondence list)
+template <class Call>
+VerifyResult verify_noncentral(const std::vector<int32_t>& kf_ptr, const std::vector<VerifyCandidate>& candidates, const VerifyParams& params,
+                               const std::vector<uint64_t>& seeds5, const std::vector<uint64_t>& seeds, const Call& call) {
+  const int n_kf = (int)kf_ptr.size() - 1, C = (int)candidates.size();
+  std::vector<int32_t> cp1(C + 1, 0), cp2(C + 1, 0), pair_ptr(C + 1, 0), pairs;
+  std::vector<double> co1, cr1, co2, cr2;
   size_t bound = 0;
   for (int c = 0; c < C; c++) {
     const VerifyCandidate& cd = candidates[c];
@@ -1316,7 +1332,7 @@ inline VerifyResult VerifyNonCentralRelativePose(Context& ctx, const std::vector
     pair_ptr[c + 1] = pair_ptr[c] + (int32_t)cd.pairings.size();
     for (const VerifyPairing& q : cd.pairings) {
       pairs.insert(pairs.end(), {q.kf1, q.kf2, q.cam1, q.cam2});
-      if (q.kf1 >= 0 && q.kf1 < n_kf) bound += (size_t)keyframes[q.kf1].n;
+      if (q.kf1 >= 0 && q.kf1 < n_kf) bound += (size_t)(kf_ptr[q.kf1 + 1] - kf_ptr[q.kf1]);
     }
   }
   const int P = pair_ptr[C];
@@ -1324,14 +1340,12 @@ inline VerifyResult VerifyNonCentralRelativePose(Context& ctx, const std::vector
     throw std::invalid_argument("covins_b200::VerifyNonCentralRelativePose: one seed per pairing and per candidate");
   std::vector<int32_t> nm(P), bs5(P), bc5(P), it5(P), us5(P), bs(C), bc(C), it(C), us(C), nv(C), corr(5 * bound);
   std::vector<double> bm5(12 * (size_t)P), bm(12 * (size_t)C), cov(36 * (size_t)C);
-  cvb_verify_keyframes K{n_kf, kf_ptr.data(), desc.data(), bear.data(), sig.data()};
-  cvb_verify_candidates D{C, cp1.data(), co1.data(), cr1.data(), cp2.data(), co2.data(), cr2.data(), pair_ptr.data(), pairs.data()};
-  cvb_verify_params prm{params.img_match_thres, params.ratio_thres, params.threshold5, params.max_iterations5, params.threshold17,
-                        params.max_iterations17, params.probability, params.n_cov_samples};
+  const cvb_verify_candidates D{C, cp1.data(), co1.data(), cr1.data(), cp2.data(), co2.data(), cr2.data(), pair_ptr.data(), pairs.data()};
+  const cvb_verify_params prm{params.img_match_thres, params.ratio_thres, params.threshold5, params.max_iterations5, params.threshold17,
+                              params.max_iterations17, params.probability, params.n_cov_samples};
   cvb_verify_result R{nm.data(), bs5.data(), bm5.data(), bc5.data(), it5.data(), us5.data(), bs.data(), bm.data(), bc.data(), it.data(), us.data(),
                       cov.data(), nv.data(), corr.data(), (int32_t)bound, 0};
-  ctx.check(cvb_verify_noncentral_relative_pose_seeded_batch(ctx.get(), &K, &D, &prm, seeds5.data(), seeds.data(), &R),
-            "cvb_verify_noncentral_relative_pose_seeded_batch");
+  call(D, prm, R);
   VerifyResult out;
   out.pairings.resize(P); out.candidates.resize(C);
   for (int q = 0; q < P; q++) {
@@ -1348,6 +1362,38 @@ inline VerifyResult VerifyNonCentralRelativePose(Context& ctx, const std::vector
   for (int j = 0; j < R.n_total; j++)
     out.correspondences.push_back({corr[5 * j], corr[5 * j + 1], corr[5 * j + 2], corr[5 * j + 3], corr[5 * j + 4]});
   return out;
+}
+}  // namespace detail
+
+inline VerifyResult VerifyNonCentralRelativePose(Context& ctx, const std::vector<VerifyKeyframeView>& keyframes,
+                                                 const std::vector<VerifyCandidate>& candidates, const VerifyParams& params,
+                                                 const std::vector<uint64_t>& seeds5, const std::vector<uint64_t>& seeds) {
+  std::vector<int32_t> kf_ptr;
+  std::vector<uint8_t> desc;
+  std::vector<double> bear, sig;
+  detail::flatten_verify_keyframes<32>(keyframes, kf_ptr, desc, bear, sig);
+  return detail::verify_noncentral(kf_ptr, candidates, params, seeds5, seeds,
+                                   [&](const cvb_verify_candidates& D, const cvb_verify_params& prm, cvb_verify_result& R) {
+                                     const cvb_verify_keyframes K{(int32_t)keyframes.size(), kf_ptr.data(), desc.data(), bear.data(), sig.data()};
+                                     ctx.check(cvb_verify_noncentral_relative_pose_seeded_batch(ctx.get(), &K, &D, &prm, seeds5.data(), seeds.data(), &R),
+                                               "cvb_verify_noncentral_relative_pose_seeded_batch");
+                                   });
+}
+
+inline VerifyResult VerifyNonCentralRelativePose(Context& ctx, const std::vector<VerifyKeyframeViewSIFT>& keyframes,
+                                                 const std::vector<VerifyCandidate>& candidates, const VerifyParams& params,
+                                                 const std::vector<uint64_t>& seeds5, const std::vector<uint64_t>& seeds) {
+  std::vector<int32_t> kf_ptr;
+  std::vector<float> desc;
+  std::vector<double> bear, sig;
+  detail::flatten_verify_keyframes<128>(keyframes, kf_ptr, desc, bear, sig);
+  return detail::verify_noncentral(kf_ptr, candidates, params, seeds5, seeds,
+                                   [&](const cvb_verify_candidates& D, const cvb_verify_params& prm, cvb_verify_result& R) {
+                                     const cvb_verify_keyframes_sift K{(int32_t)keyframes.size(), kf_ptr.data(), desc.data(), bear.data(), sig.data()};
+                                     ctx.check(cvb_verify_noncentral_relative_pose_sift_seeded_batch(ctx.get(), &K, &D, &prm, seeds5.data(), seeds.data(),
+                                                                                                     &R),
+                                               "cvb_verify_noncentral_relative_pose_sift_seeded_batch");
+                                   });
 }
 
 // The sampling-based 6x6 covariance of RelNonCentralPosSolver::computeNonCentralRelPose (RelNonCentralPosSolver.cpp:199,236,

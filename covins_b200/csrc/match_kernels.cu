@@ -6,6 +6,7 @@
 //   fused filter epilogue              placerec_gen_be.cpp:102-114
 //   scan_kernel<HammingMetric,…,PAIRS> K1 over a list of keyframe pairs, each with its own query rows (the pairwise matchings
 //                                      of computeNonCentralRelPose, cvb_match_hamming_pairs_dev)
+//   scan_kernel<L2Metric,…,PAIRS>  K2 over such a list (the same matchings on SIFT rows, cvb_match_l2_pairs_dev)
 //   scan_kernel<HammingMetric,…,DM> + dm_assign_kernel
 //                                  K3  DenseMatcher<LandmarkMatchingAlgorithm> (placerec_be.cpp:85-90)
 //
@@ -807,20 +808,33 @@ int stage_inputs(cvb_ctx* ctx, const void* q, size_t qbytes, const void* t, size
 
 }  // namespace
 
-// The fused 2-NN + filter of cvb_match_hamming_batch for n_pairs (query keyframe, train keyframe) pairs of one device descriptor
-// table in one launch (cvb_internal.cuh).  Each pair is an independent scan, so the results are those of cvb_match_hamming_batch
-// with n_seg = 1 on the pair's rows.  On ctx->stream; n_matches is zeroed here.
-int cvb_match_hamming_pairs_dev(cvb_ctx* ctx, const uint8_t* d_desc, const int32_t* d_pairs, int n_pairs, int max_nq, float thr, float ratio,
-                                int32_t* d_match_train, float* d_match_dist, int32_t* d_n_matches) {
+// The fused 2-NN + filter of cvb_match_{hamming,l2}_batch for n_pairs (query keyframe, train keyframe) pairs of one device
+// descriptor table in one launch (cvb_internal.cuh).  Each pair is an independent scan, so the results are those of the batch
+// call with n_seg = 1 on the pair's rows.  On ctx->stream; n_matches is zeroed here.  QPT_BIG: as knn_dev<M, QPT_BIG>.
+namespace {
+template <class M, int QPT_BIG>
+int match_pairs_dev(cvb_ctx* ctx, const uint8_t* d_desc, const int32_t* d_pairs, int n_pairs, int max_nq, float thr, float ratio,
+                    int32_t* d_match_train, float* d_match_dist, int32_t* d_n_matches) {
   cudaStream_t st = ctx->stream;
   CVB_CUDA(ctx, cudaMemsetAsync(d_n_matches, 0, sizeof(int32_t) * n_pairs, st));
   if (n_pairs == 0 || max_nq == 0) return CVB_OK;
-  const Plan pl = make_plan<HammingMetric>(max_nq, n_pairs, 0, ctx->sm_count, 4, false);
+  const Plan pl = make_plan<M>(max_nq, n_pairs, 0, ctx->sm_count, QPT_BIG, false);
   ScanParams sp{};
   sp.q = d_desc; sp.nq = max_nq; sp.t = d_desc; sp.n_seg = n_pairs; sp.splits = 1; sp.chunk = INT_MAX;   // one split: the whole train keyframe
   sp.filter = 1; sp.thr = thr; sp.ratio = ratio;
   sp.match_train = d_match_train; sp.match_dist = d_match_dist; sp.n_matches = d_n_matches; sp.pairs = d_pairs;
-  return pl.qpt == 1 ? launch_scan<HammingMetric, 1, 2, MODE_PAIRS>(ctx, sp, pl, st) : launch_scan<HammingMetric, 4, 2, MODE_PAIRS>(ctx, sp, pl, st);
+  return pl.qpt == 1 ? launch_scan<M, 1, 2, MODE_PAIRS>(ctx, sp, pl, st) : launch_scan<M, QPT_BIG, 2, MODE_PAIRS>(ctx, sp, pl, st);
+}
+}  // namespace
+
+int cvb_match_hamming_pairs_dev(cvb_ctx* ctx, const uint8_t* d_desc, const int32_t* d_pairs, int n_pairs, int max_nq, float thr, float ratio,
+                                int32_t* d_match_train, float* d_match_dist, int32_t* d_n_matches) {
+  return match_pairs_dev<HammingMetric, 4>(ctx, d_desc, d_pairs, n_pairs, max_nq, thr, ratio, d_match_train, d_match_dist, d_n_matches);
+}
+
+int cvb_match_l2_pairs_dev(cvb_ctx* ctx, const uint8_t* d_desc, const int32_t* d_pairs, int n_pairs, int max_nq, float thr, float ratio,
+                           int32_t* d_match_train, float* d_match_dist, int32_t* d_n_matches) {
+  return match_pairs_dev<L2Metric, 2>(ctx, d_desc, d_pairs, n_pairs, max_nq, thr, ratio, d_match_train, d_match_dist, d_n_matches);
 }
 
 // ------------------------------------------------------------------------------------------------

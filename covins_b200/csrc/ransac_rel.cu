@@ -1128,9 +1128,31 @@ __global__ void __launch_bounds__(kGlueThreads) verify_list_kernel(VerifyDev V) 
   }
 }
 
-int verify_noncentral(cvb_ctx* ctx, const cvb_verify_keyframes* kf, const cvb_verify_candidates* cd, const cvb_verify_params* prm,
-                      const uint64_t* seed5, const uint64_t* seed, cvb_verify_result* r) {
-  const char* name = "verify_noncentral_relative_pose_seeded";
+// SIFT rows (CV_32F) to the u8 layout of the L2 scan in one pass; false if a value is not an integer in [0, 255] (NaN and
+// +-inf included).  This is quantize_u8_kernel's test rintf(v) == v && 0 <= v <= 255 (checked equal on every float bit
+// pattern), written without branches or conversions so that the loop vectorises and runs at copy speed: c = v + 1.5 * 2^23
+// rounds v to an integer held in c's low mantissa bits (|v| < 2^22), and c - 1.5 * 2^23 == v holds exactly when v is one.
+// Needs IEEE arithmetic (no -ffast-math).
+bool quantize_sift(const float* src, size_t n, uint8_t* dst) {
+  int bad = 0;
+  for (size_t i = 0; i < n; i++) {
+    const float v = src[i];
+    const float c = v + 12582912.f;
+    int32_t bits;
+    memcpy(&bits, &c, 4);
+    bad |= (c - 12582912.f != v) | (v < 0.f) | (v > 255.f);
+    dst[i] = (uint8_t)(bits - 0x4B400000);   // the bits of 1.5 * 2^23
+  }
+  return bad == 0;
+}
+
+// cvb_verify_noncentral_relative_pose{,_sift}_seeded_batch: KF is cvb_verify_keyframes (ORB rows, staged as they are, matched by
+// the Hamming pair scan) or cvb_verify_keyframes_sift (SIFT rows, checked and quantised to u8 while staged, matched by the L2 one)
+template <class KF>
+int verify_noncentral(cvb_ctx* ctx, const KF* kf, const cvb_verify_candidates* cd, const cvb_verify_params* prm, const uint64_t* seed5,
+                      const uint64_t* seed, cvb_verify_result* r) {
+  constexpr bool kSift = std::is_same<KF, cvb_verify_keyframes_sift>::value;
+  const char* name = kSift ? "verify_noncentral_relative_pose_sift_seeded" : "verify_noncentral_relative_pose_seeded";
   constexpr int kMaxIt = (INT32_MAX - kWave) / 11;   // the seeded RANSAC's limit: every sample number fits an int
   CVB_REQUIRE(ctx, kf && cd && prm && r && kf->n_kf >= 0 && cd->n_cand >= 0, "%s: bad arguments", name);
   CVB_REQUIRE(ctx, prm->max_iterations5 >= 0 && prm->max_iterations5 <= kMaxIt && prm->max_iterations17 >= 0 && prm->max_iterations17 <= kMaxIt,
@@ -1180,7 +1202,15 @@ int verify_noncentral(cvb_ctx* ctx, const cvb_verify_keyframes* kf, const cvb_ve
   // device block: inputs (uploaded), scratch, outputs (downloaded)
   Stager St;
   RelIn in{};
-  const size_t o_desc = St.put(kf->desc, R * 32), o_bear = St.put(kf->bearings, R * 24), o_sig = St.put(kf->sigma, R * 8);
+  size_t o_desc;
+  if constexpr (kSift) {
+    o_desc = St.reserve(R * 128);
+    if (!quantize_sift(kf->desc, R * 128, St.h.data() + o_desc))
+      return cvb_fail(ctx, CVB_ERR_UNSUPPORTED, "%s: SIFT descriptors must be integer-valued in [0,255] (cv::xfeatures2d::SIFT output)", name);
+  } else {
+    o_desc = St.put(kf->desc, R * 32);
+  }
+  const size_t o_bear = St.put(kf->bearings, R * 24), o_sig = St.put(kf->sigma, R * 8);
   const size_t o_rows = St.put(rows.data(), (size_t)P * 20), o_cams = St.put(cams.data(), (size_t)P * 8);
   const size_t o_pp = St.put(cd->pair_ptr, ((size_t)C + 1) * 4);
   in.cp1 = St.put(cd->cam_ptr1, ((size_t)C + 1) * 4); in.cp2 = St.put(cd->cam_ptr2, ((size_t)C + 1) * 4);
@@ -1226,8 +1256,9 @@ int verify_noncentral(cvb_ctx* ctx, const cvb_verify_keyframes* kf, const cvb_ve
   V.s2_17 = (double*)(d + o_s217); V.cam1_17 = (int*)(d + o_c117); V.cam2_17 = (int*)(d + o_c217); V.pos17 = (int*)(d + o_pos);
   V.mask17 = d + o_m17; V.corr = (int*)(d + o_corr); V.corr_cap = (int)L;
   // 1. matches
-  if (const int rc = cvb_match_hamming_pairs_dev(ctx, d + o_desc, V.pair_rows, P, max_nq, prm->img_match_thres, prm->ratio_thres, (int*)(d + o_mt),
-                                                 (float*)(d + o_md), (int*)(d + o_nm)))
+  const auto match_pairs = kSift ? cvb_match_l2_pairs_dev : cvb_match_hamming_pairs_dev;
+  if (const int rc = match_pairs(ctx, d + o_desc, V.pair_rows, P, max_nq, prm->img_match_thres, prm->ratio_thres, (int*)(d + o_mt), (float*)(d + o_md),
+                                 (int*)(d + o_nm)))
     return rc;
   if (P == 0) CVB_CUDA(ctx, cudaMemsetAsync(d + o_pp5, 0, 4, st));
   // 2. the 5-point problems and their RANSACs
@@ -1293,6 +1324,14 @@ int verify_noncentral(cvb_ctx* ctx, const cvb_verify_keyframes* kf, const cvb_ve
 extern "C" int cvb_verify_noncentral_relative_pose_seeded_batch(cvb_ctx* ctx, const cvb_verify_keyframes* kf, const cvb_verify_candidates* cand,
                                                                 const cvb_verify_params* prm, const uint64_t* seed5, const uint64_t* seed,
                                                                 cvb_verify_result* r) {
+  if (!ctx) return CVB_ERR_INVALID;
+  CVB_GUARD(ctx);
+  return verify_noncentral(ctx, kf, cand, prm, seed5, seed, r);
+}
+
+extern "C" int cvb_verify_noncentral_relative_pose_sift_seeded_batch(cvb_ctx* ctx, const cvb_verify_keyframes_sift* kf,
+                                                                     const cvb_verify_candidates* cand, const cvb_verify_params* prm,
+                                                                     const uint64_t* seed5, const uint64_t* seed, cvb_verify_result* r) {
   if (!ctx) return CVB_ERR_INVALID;
   CVB_GUARD(ctx);
   return verify_noncentral(ctx, kf, cand, prm, seed5, seed, r);

@@ -15,6 +15,7 @@ the C-ABI:
                                   per problem, as the reference draws its own (include/covins_b200.h, "Seeded samples")
   verify_noncentral_relative_pose_seeded(...) ↔ the whole verification of RelNonCentralPosSolver::computeNonCentralRelPose
                                   (pairwise matching, 5-point and 17-point RANSAC, covariance) for all candidates in one call
+  verify_noncentral_relative_pose_sift_seeded(...) ↔ the same with SIFT descriptors (exact L2 matching)
   verify_landmark_candidates_seeded(...) ↔ the COVINS verification of PlaceRecognition::ComputeSE3 (DenseMatcher landmark
                                   matching, GP3P RANSAC, SearchBySE3, OptimizeRelativePose) for all candidates in one call
 
@@ -412,8 +413,31 @@ def verify_noncentral_relative_pose_seeded(ctx: Context, kf_ptr, desc, bearings,
     → dict(n_matches, best_sample5, best_model5 [P,3,4], best_count5, iterations5, consumed5 (per pairing); best_sample,
     best_model [C,3,4], best_count, iterations, consumed, cov [C,6,6], n_valid (per candidate); n_total; and, unless
     corr_cap = 0 or n_total > corr_cap, corr [n_total,5] = (pairing, row1, row2, inlier5, inlier17))."""
+    return _verify_noncentral(ctx, "cvb_verify_noncentral_relative_pose_seeded_batch", np.ascontiguousarray(desc, np.uint8).reshape(-1, 32), kf_ptr,
+                              bearings, sigma, cam_ptr1, cam_off1, cam_rot1, cam_ptr2, cam_off2, cam_rot2, pair_ptr, pairs, seeds5, seeds,
+                              img_match_thres, ratio_thres, threshold5, max_iterations5, threshold17, max_iterations17, probability, n_cov_samples,
+                              corr_cap)
+
+
+def verify_noncentral_relative_pose_sift_seeded(ctx: Context, kf_ptr, desc, bearings, sigma, cam_ptr1, cam_off1, cam_rot1, cam_ptr2, cam_off2,
+                                                cam_rot2, pair_ptr, pairs, seeds5, seeds, img_match_thres, ratio_thres, threshold5, max_iterations5,
+                                                threshold17, max_iterations17, probability=0.99, n_cov_samples=300, corr_cap=None):
+    """verify_noncentral_relative_pose_seeded with SIFT descriptors (cvb_verify_noncentral_relative_pose_sift_seeded_batch): desc
+    [R,128] float32, integer-valued in [0,255] as cv::xfeatures2d::SIFT writes them (otherwise CVB_ERR_UNSUPPORTED); each pairing
+    is matched by the fused 2-NN + ratio filter of match_candidates_l2 (exact L2).  Other arguments and the result dict as
+    verify_noncentral_relative_pose_seeded; the reference's SIFT thresholds are about img_match_thres=500, ratio_thres=0.8."""
+    return _verify_noncentral(ctx, "cvb_verify_noncentral_relative_pose_sift_seeded_batch", np.ascontiguousarray(desc, np.float32).reshape(-1, 128),
+                              kf_ptr, bearings, sigma, cam_ptr1, cam_off1, cam_rot1, cam_ptr2, cam_off2, cam_rot2, pair_ptr, pairs, seeds5, seeds,
+                              img_match_thres, ratio_thres, threshold5, max_iterations5, threshold17, max_iterations17, probability, n_cov_samples,
+                              corr_cap)
+
+
+def _verify_noncentral(ctx: Context, fn, dsc, kf_ptr, bearings, sigma, cam_ptr1, cam_off1, cam_rot1, cam_ptr2, cam_off2, cam_rot2, pair_ptr, pairs,
+                       seeds5, seeds, img_match_thres, ratio_thres, threshold5, max_iterations5, threshold17, max_iterations17, probability,
+                       n_cov_samples, corr_cap):
+    """the body of verify_noncentral_relative_pose{,_sift}_seeded: the C call fn on the contiguous descriptor table dsc"""
     kp = np.ascontiguousarray(kf_ptr, np.int32); n_kf = len(kp) - 1
-    dsc = np.ascontiguousarray(desc, np.uint8).reshape(-1, 32); f = np.ascontiguousarray(bearings, np.float64).reshape(-1, 3)
+    f = np.ascontiguousarray(bearings, np.float64).reshape(-1, 3)
     sg = np.ascontiguousarray(sigma, np.float64).reshape(-1)
     cp1 = np.ascontiguousarray(cam_ptr1, np.int32); cp2 = np.ascontiguousarray(cam_ptr2, np.int32); n_cand = len(cp1) - 1
     co1 = np.ascontiguousarray(cam_off1, np.float64).reshape(-1, 3); cr1 = np.ascontiguousarray(cam_rot1, np.float64).reshape(-1, 9)
@@ -432,8 +456,7 @@ def verify_noncentral_relative_pose_seeded(ctx: Context, kf_ptr, desc, bearings,
     Pm = CVerifyParams(float(img_match_thres), float(ratio_thres), float(threshold5), int(max_iterations5), float(threshold17), int(max_iterations17),
                        float(probability), int(n_cov_samples))
     R = CVerifyResult(*[r[k].ctypes.data for k, _ in CVerifyResult._fields_[:13]], corr.ctypes.data if corr_cap else None, int(corr_cap), 0)
-    ctx.check(lib().cvb_verify_noncentral_relative_pose_seeded_batch(ctx.handle, C.byref(K), C.byref(D), C.byref(Pm), s5.ctypes.data,
-                                                                     s17.ctypes.data, C.byref(R)))
+    ctx.check(getattr(lib(), fn)(ctx.handle, C.byref(K), C.byref(D), C.byref(Pm), s5.ctypes.data, s17.ctypes.data, C.byref(R)))
     r["n_total"] = int(R.n_total)
     if corr_cap and R.n_total <= corr_cap:
         r["corr"] = corr[:R.n_total].copy()

@@ -652,6 +652,32 @@ CVB_API int cvb_verify_noncentral_relative_pose_seeded_batch(cvb_ctx* ctx, const
                                                              cvb_verify_result* r);
 
 /*
+ * The same verification with SIFT descriptors (the SIFT branch of computeNonCentralRelPose, RelNonCentralPosSolver.cpp:310-311):
+ * the keyframe table holds desc [R][128] CV_32F rows, as the reference holds descriptors_add_.
+ *   Semantics: exactly the composition of cvb_verify_noncentral_relative_pose_seeded_batch above on the same inputs and seeds,
+ *   except step 1: the matches of pairing (kf1, kf2, cam1, cam2) are cvb_match_l2_batch(query = the rows of kf1, train = the
+ *   rows of kf2 as one segment, dim = 128, img_match_thres, ratio_thres); the accepted rows are kept in query order.  Steps 2-4,
+ *   the outputs and the correspondence list are those of the ORB call.
+ *   Deviation from the reference: the matches are the exact brute-force L2 2-NN, where the reference calls FLANN (approximate and
+ *   randomised), as cvb_match_l2_batch documents.
+ * Errors: every CVB_ERR_INVALID case of cvb_verify_noncentral_relative_pose_seeded_batch; CVB_ERR_UNSUPPORTED for a descriptor
+ * value that is not an integer in [0, 255] (rintf(v) == v && 0 <= v <= 255, as cv::xfeatures2d::SIFT writes them; NaN and
+ * +-inf fail it).  Both before any launch: the descriptors are checked and quantised to u8 on the host while they are staged,
+ * so the call uploads R x 128 bytes of them.  n_cand = 0 succeeds.
+ * Usage: the thresholds are the caller's; the reference's SIFT configuration uses img_match_thres about 500 and ratio_thres 0.8.
+ */
+typedef struct cvb_verify_keyframes_sift {
+  int32_t n_kf;
+  const int32_t* kf_ptr;     /* [n_kf+1] */
+  const float* desc;         /* [R][128]  CV_32F rows as the reference holds descriptors_add_ */
+  const double* bearings;    /* [R][3] */
+  const double* sigma;       /* [R] */
+} cvb_verify_keyframes_sift;
+CVB_API int cvb_verify_noncentral_relative_pose_sift_seeded_batch(cvb_ctx* ctx, const cvb_verify_keyframes_sift* kf,
+                                                                  const cvb_verify_candidates* cand, const cvb_verify_params* prm,
+                                                                  const uint64_t* seed5, const uint64_t* seed, cvb_verify_result* r);
+
+/*
  * The COVINS verification of place-recognition candidates (PlaceRecognition::ComputeSE3, placerec_be.cpp:63-220, up to the
  * acceptance test: DenseMatcher landmark matching, the nmatches < matches_thres discard, Se3Solver's GP3P RANSAC,
  * FeatureMatcher::SearchBySE3 and Optimization::OptimizeRelativePose) for all candidates of one query keyframe in one call: one

@@ -7,7 +7,9 @@ covariance samples) at 1, 8 and 32 candidates and 5 % / 30 % wrong bearings:
 Both are timed alternately in one session: the whole call (host clock around the synchronous calls, median of --reps) and the
 device time of their kernels (torch.profiler, a separate run).  Every result of every timed call is checked identical between
 (a) and (b).  Prints the GPU name and power limit read in the same run; --out writes the table as JSON.
-  python tools/verify_timing.py [--reps 30] [--out verify_timing.json]"""
+--sift: the same with SIFT descriptors (300 keypoints per keyframe, the scene of tests/test_verify_relative_sift.py): (a) is
+cvb_verify_noncentral_relative_pose_sift_seeded_batch, (b) matches with one cvb_match_l2_batch per query keyframe.
+  python tools/verify_timing.py [--sift] [--reps 30] [--out verify_timing.json]"""
 import argparse
 import json
 import os
@@ -28,17 +30,19 @@ KEYS = ("n_matches", "best_sample5", "best_model5", "best_count5", "iterations5"
         "iterations", "consumed", "cov", "n_valid", "corr")
 
 
-def chain_existing_calls(ctx, S, prm, n_cov_samples):
-    """(b): the existing calls with the glue in numpy → the result dict of placerec.verify_noncentral_relative_pose_seeded"""
+def chain_existing_calls(ctx, S, prm, n_cov_samples, metric="hamming"):
+    """(b): the existing calls with the glue in numpy → the result dict of placerec.verify_noncentral_relative_pose_seeded
+    (metric="hamming", desc [R,32] u8) or verify_noncentral_relative_pose_sift_seeded (metric="l2", desc [R,128] float32)"""
     kp, desc, f, sg = S["kf_ptr"], S["desc"], S["bearings"], S["sigma"]
     pairs, pair_ptr = np.asarray(S["pairs"]).reshape(-1, 4), np.asarray(S["pair_ptr"])
     P = len(pairs)
+    match, dim = (M.match_candidates_hamming, 32) if metric == "hamming" else (M.match_candidates_l2, 128)
     mts, nm = [None] * P, np.zeros(P, np.int32)
     for a in np.unique(pairs[:, 0]):                       # one matcher call per query keyframe, its pairings as segments
         qs = np.flatnonzero(pairs[:, 0] == a)
         seg = np.concatenate([[0], np.cumsum([kp[b + 1] - kp[b] for b in pairs[qs, 1]])]).astype(np.int32)
-        t = np.concatenate([desc[kp[b]:kp[b + 1]] for b in pairs[qs, 1]]).reshape(-1, 32)
-        mt, _, n = M.match_candidates_hamming(ctx, desc[kp[a]:kp[a + 1]], t, seg, prm["img_match_thres"], prm["ratio_thres"])
+        t = np.concatenate([desc[kp[b]:kp[b + 1]] for b in pairs[qs, 1]]).reshape(-1, dim)
+        mt, _, n = match(ctx, desc[kp[a]:kp[a + 1]], t, seg, prm["img_match_thres"], prm["ratio_thres"])
         for i, q in enumerate(qs):
             mts[q], nm[q] = mt[i], n[i]
     rows = [np.flatnonzero(m >= 0) for m in mts]
@@ -75,10 +79,16 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--reps", type=int, default=30)
     ap.add_argument("--out", default="")
+    ap.add_argument("--sift", action="store_true", help="the SIFT scene (300 keypoints per keyframe) and the SIFT call")
     a = ap.parse_args()
     import torch
     from torch.profiler import profile, ProfilerActivity
-    from test_verify_relative import PRM, scene
+    if a.sift:
+        from test_verify_relative_sift import PRM, scene
+        verify, metric, n_kp = PR.verify_noncentral_relative_pose_sift_seeded, "l2", 300
+    else:
+        from test_verify_relative import PRM, scene
+        verify, metric, n_kp = PR.verify_noncentral_relative_pose_seeded, "hamming", 1000
     assert torch.cuda.is_available(), "needs a GPU"
     q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"], capture_output=True, text=True)
     gpu = q.stdout.strip().splitlines()[0] if q.returncode == 0 and q.stdout.strip() else torch.cuda.get_device_name(0)
@@ -87,9 +97,9 @@ def main():
     rows = []
     for outlier in (0.05, 0.3):
         for n_cand in (1, 8, 32):
-            S, _ = scene(100 + n_cand, n_cand, outlier=outlier)
-            fused = lambda: PR.verify_noncentral_relative_pose_seeded(ctx, **S, **PRM)   # noqa: E731
-            chain = lambda: chain_existing_calls(ctx, S, PRM, 300)                         # noqa: E731
+            S, _ = scene(100 + n_cand, n_cand, n_kp=n_kp, outlier=outlier)
+            fused = lambda: verify(ctx, **S, **PRM)                                        # noqa: E731
+            chain = lambda: chain_existing_calls(ctx, S, PRM, 300, metric=metric)          # noqa: E731
             ref = fused()
             assert _same(ref, chain()), "the fused call and the chain differ"
             for _ in range(3):
