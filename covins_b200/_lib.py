@@ -99,6 +99,8 @@ SIGNATURES = {
     "cvb_ba_destroy": (C.c_int, [c_vp]),
     "cvb_ba_solve": (C.c_int, [c_vp, c_vp, c_vp, c_vp]),
     "cvb_gba": (C.c_int, [c_vp, c_vp, c_vp, c_vp, c_vp]),
+    "cvb_covisibility": (C.c_int, [c_vp, C.c_int, C.c_int, c_vp, c_vp, c_vp, c_vp, C.c_int, c_vp, c_vp, c_vp, C.c_int64,
+                                   C.POINTER(C.c_int64)]),
 }
 
 

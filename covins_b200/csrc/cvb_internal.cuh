@@ -23,7 +23,7 @@ struct cvb_ctx {
   int64_t launches = 0;
   std::string err;
   // grow-only device workspaces (named slots so independent stages never alias)
-  cvb_buf ws[27];   // one per WS_* slot below
+  cvb_buf ws[29];   // one per WS_* slot below
   // pinned host staging
   void* h_pin = nullptr;
   size_t h_pin_cap = 0;
@@ -39,8 +39,9 @@ struct cvb_ctx {
 };
 
 enum { WS_Q = 0, WS_T, WS_SEG, WS_OUT0, WS_OUT1, WS_OUT2, WS_PART_I, WS_PART_D, WS_LIST_I, WS_LIST_D, WS_SKIPA,
-       WS_SKIPB, WS_TMP0, WS_TMP1, WS_FLAG, WS_MISC, WS_CHUNK_PS, WS_CHUNK_OFF, WS_GS0, WS_GS1, WS_GS2, WS_GS3, WS_GS4, WS_GS5, WS_GS6, WS_XT, WS_XT_TILE };
-static_assert(WS_XT_TILE < (int)(sizeof(cvb_ctx::ws) / sizeof(cvb_buf)), "cvb_ctx::ws has a buffer per workspace slot");
+       WS_SKIPB, WS_TMP0, WS_TMP1, WS_FLAG, WS_MISC, WS_CHUNK_PS, WS_CHUNK_OFF, WS_GS0, WS_GS1, WS_GS2, WS_GS3, WS_GS4, WS_GS5, WS_GS6, WS_XT, WS_XT_TILE,
+       WS_MG_EDGES, WS_MG_ROWS };
+static_assert(WS_MG_ROWS < (int)(sizeof(cvb_ctx::ws) / sizeof(cvb_buf)), "cvb_ctx::ws has a buffer per workspace slot");
 
 // cudaFuncSetAttribute applies to the CURRENT device: one flag per (call site, device), so that a process that opens contexts
 // on several GPUs raises the dynamic shared-memory limit on each of them
@@ -90,6 +91,13 @@ constexpr int CVB_RELPOSE_OUT = 27;
 // refines the n_prob problems d_probs [n_prob] (device) in one launch on ctx->stream, one CTA each; a problem with n < 12 gets
 // cvb_optimize_relative_pose's early result (T12_out = pose_in, nothing removed, zero counts)
 int cvb_relpose_batch_dev(cvb_ctx* ctx, const cvb_relpose_dev* d_probs, int n_prob, double th_outlier_align);
+
+// map_graph.cu: cvb_covisibility with the pair budget as an argument.  The shared-landmark pairs are expanded, sorted and
+// counted at most `pair_budget` at a time and the partial counts merged by key; the result does not depend on the budget
+// (tests force several chunks at small size through this argument; the public entry point passes the default).
+int cvb_covisibility_budgeted(cvb_ctx* ctx, int K, int L, const int32_t* lm_obs_ptr, const int32_t* obs_kf, const uint8_t* obs_skip,
+                              const uint8_t* lm_valid, int min_weight, int32_t* nbr_ptr, int32_t* nbr_kf, int32_t* nbr_w, int64_t cap,
+                              int64_t* n_total, int64_t pair_budget);
 
 #define CVB_CUDA(ctx, call)                                                                         \
   do {                                                                                              \

@@ -225,6 +225,42 @@ struct Flat {
   }
 };
 
+// The canonical flattening of a map's containers (SURVEY.md §8c), shared by every function that hands the map's structure
+// to the library: the valid keyframes in the map's id-sorted order with their index ...
+template <class KeyframePtr, class KF>
+inline void canonical_keyframes(const std::vector<KeyframePtr>& keyframes, std::map<const KF*, int>& kf_index, std::vector<KeyframePtr>& kfs) {
+  for (auto& kf : keyframes) {
+    if (kf->IsInvalid()) continue;
+    kf_index[kf.get()] = (int)kfs.size();
+    kfs.push_back(kf);
+  }
+}
+// ... and the valid landmarks in id order with the CSR of their observations by valid keyframes, each landmark's sorted by
+// keyframe index (the reference iterates a pointer-ordered std::map, typedefs_base.hpp:187).  on_obs(keyframe index,
+// feature id, landmark index) is called once per observation in CSR order.
+template <class LandmarkPtr, class KF, class OnObs>
+inline void flatten_observations(const std::vector<LandmarkPtr>& landmarks, const std::map<const KF*, int>& kf_index, std::vector<LandmarkPtr>& lms,
+                                 std::vector<int32_t>& lm_obs_ptr, std::vector<int32_t>& obs_kf, OnObs on_obs) {
+  lm_obs_ptr.push_back(0);
+  for (auto& lm : landmarks) {
+    if (lm->IsInvalid()) continue;
+    const auto observations = lm->GetObservations();
+    std::vector<std::pair<int, int>> ob;   // (kf index, feature id)
+    for (const auto& mit : observations) {
+      auto kfx = mit.first;
+      if (!kfx || kfx->IsInvalid()) continue;
+      ob.emplace_back(kf_index.at(kfx.get()), (int)mit.second);
+    }
+    std::sort(ob.begin(), ob.end());
+    for (auto& o : ob) {
+      obs_kf.push_back(o.first);
+      on_obs(o.first, o.second, (int)lms.size());
+    }
+    lm_obs_ptr.push_back((int32_t)obs_kf.size());
+    lms.push_back(lm);
+  }
+}
+
 }  // namespace detail
 
 // parameters the reference reads from covins_params (config/config_backend.yaml; SURVEY.md §5)
@@ -262,11 +298,7 @@ void GlobalBundleAdjustment(Context& ctx, MapPtr map, int interations_limit, dou
   detail::Flat F;
   std::map<const KF*, int> kf_index;
   std::vector<KeyframePtr> kfs;               // valid keyframes, canonical order
-  for (auto& kf : keyframes) {
-    if (kf->IsInvalid()) continue;
-    kf_index[kf.get()] = (int)kfs.size();
-    kfs.push_back(kf);
-  }
+  detail::canonical_keyframes(keyframes, kf_index, kfs);
   const int K = (int)kfs.size();
   F.pose.resize(7 * (size_t)K); F.sb.resize(9 * (size_t)K); F.extr.resize(7 * (size_t)K); F.intr.resize(4 * (size_t)K);
   F.dist.resize(4 * (size_t)K); F.pose_const.assign(K, 0); F.cam_of_kf.resize(K);
@@ -314,35 +346,21 @@ void GlobalBundleAdjustment(Context& ctx, MapPtr map, int interations_limit, dou
       F.imu_ptr.push_back((int32_t)F.imu_dt.size());
     }
   }
-  // landmarks + observations (canonical: observations sorted by keyframe index; the reference iterates a
-  // pointer-ordered std::map, typedefs_base.hpp:187)
+  // landmarks + observations (detail::flatten_observations: the canonical landmark order and observation CSR)
   struct ObsRef { KeyframePtr kf; int lm; int feat; };
   std::vector<ObsRef> obs_ref;
   using LandmarkPtr = typename std::decay<decltype(landmarks[0])>::type;
   std::vector<LandmarkPtr> lms;
-  F.lm_obs_ptr.push_back(0);
-  for (auto& lm : landmarks) {
-    if (lm->IsInvalid()) continue;
-    const auto observations = lm->GetObservations();
-    std::vector<std::pair<int, int>> ob;   // (kf index, feature id)
-    for (const auto& mit : observations) {
-      auto kfx = mit.first;
-      if (!kfx || kfx->IsInvalid()) continue;
-      ob.emplace_back(kf_index.at(kfx.get()), (int)mit.second);
-    }
-    std::sort(ob.begin(), ob.end());
+  detail::flatten_observations(landmarks, kf_index, lms, F.lm_obs_ptr, F.obs_kf, [&](int k, int feat, int l) {
+    auto& kfx = kfs[k];
+    const auto& kp = kfx->keypoints_distorted_[feat];
+    F.obs_uv.push_back((float)kp[0]); F.obs_uv.push_back((float)kp[1]);
+    F.obs_sigma.push_back((kfx->keypoints_aors_[feat][1] + 1) * 2.0);                              // :183-184, 477-478
+    obs_ref.push_back({kfx, l, feat});
+  });
+  for (auto& lm : lms) {
     const auto pos = lm->GetWorldPos();
     F.lm.push_back(pos[0]); F.lm.push_back(pos[1]); F.lm.push_back(pos[2]);
-    for (auto& o : ob) {
-      auto& kfx = kfs[o.first];
-      const auto& kp = kfx->keypoints_distorted_[o.second];
-      F.obs_kf.push_back(o.first);
-      F.obs_uv.push_back((float)kp[0]); F.obs_uv.push_back((float)kp[1]);
-      F.obs_sigma.push_back((kfx->keypoints_aors_[o.second][1] + 1) * 2.0);                         // :183-184, 477-478
-      obs_ref.push_back({kfx, (int)lms.size(), o.second});
-    }
-    F.lm_obs_ptr.push_back((int32_t)F.obs_kf.size());
-    lms.push_back(lm);
   }
   // loop edges (:236-254, 532-557): sqrt_info = diag(100 I3, 1e4 I3)
   if (P.gba_use_map_loop_constraints) {
@@ -403,6 +421,41 @@ void GlobalBundleAdjustment(Context& ctx, MapPtr map, int interations_limit, dou
   std::printf("--> Clean Map\n");
   map->Clean();                                                                                     // :614
   std::printf("--> done.\n+++ GBA: End +++\n");
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// Keyframe::UpdateCovisibilityConnections (keyframe_be.cpp:559-608) for every keyframe of the map in one call — what the
+// reference repeats keyframe by keyframe after a merge, a map load or a GBA round that erased observations.  Every valid
+// keyframe receives its connected keyframes, ordered by weight (GetConnectedKeyframes order), through one setter,
+// kf->SetCovisibility(keyframes, weights) (INTEGRATION.md shows it).  The graph is the canonical one cvb_covisibility
+// defines; min_weight 15 is the value the reference hard-codes.
+// ---------------------------------------------------------------------------------------------------------------
+template <class MapPtr>
+void UpdateCovisibilityConnections(Context& ctx, MapPtr map, int min_weight = 15) {
+  using KeyframePtr = typename std::decay<decltype(map->GetKeyframesVec()[0])>::type;
+  using KF = typename KeyframePtr::element_type;
+  auto landmarks = map->GetLandmarksVec();
+  using LandmarkPtr = typename std::decay<decltype(landmarks[0])>::type;
+  std::map<const KF*, int> kf_index;
+  std::vector<KeyframePtr> kfs;
+  detail::canonical_keyframes(map->GetKeyframesVec(), kf_index, kfs);
+  std::vector<LandmarkPtr> lms;
+  std::vector<int32_t> lm_obs_ptr, obs_kf;
+  detail::flatten_observations(landmarks, kf_index, lms, lm_obs_ptr, obs_kf, [](int, int, int) {});
+  const int K = (int)kfs.size(), L = (int)lms.size();
+  std::vector<int32_t> nbr_ptr((size_t)K + 1), nbr_kf, nbr_w;
+  int64_t n_total = 0, cap = 0;
+  do {   // the first call sizes the lists, the second fills them
+    cap = n_total;
+    nbr_kf.resize((size_t)cap + 1); nbr_w.resize((size_t)cap + 1);
+    ctx.check(cvb_covisibility(ctx.get(), K, L, lm_obs_ptr.data(), obs_kf.data(), nullptr, nullptr, min_weight, nbr_ptr.data(), nbr_kf.data(),
+                               nbr_w.data(), cap, &n_total), "cvb_covisibility");
+  } while (n_total > cap);
+  for (int k = 0; k < K; k++) {
+    std::vector<KeyframePtr> connected;
+    for (int t = nbr_ptr[k]; t < nbr_ptr[k + 1]; t++) connected.push_back(kfs[nbr_kf[t]]);
+    kfs[k]->SetCovisibility(connected, std::vector<int>(nbr_w.begin() + nbr_ptr[k], nbr_w.begin() + nbr_ptr[k + 1]));
+  }
 }
 
 // ---------------------------------------------------------------------------------------------------------------

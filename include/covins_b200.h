@@ -931,6 +931,33 @@ CVB_API int cvb_ba_solve(cvb_ctx* ctx, const cvb_ba_problem* p, const cvb_ba_opt
 CVB_API int cvb_gba(cvb_ctx* ctx, const cvb_ba_problem* p, const cvb_gba_options* g, cvb_ba_result* r,
                     uint8_t* obs_removed);
 
+/* ------------------------------------------------------------------------------------------------
+ * Map maintenance (SURVEY.md §8f rank 4)
+ * ---------------------------------------------------------------------------------------------- */
+
+/*
+ * Replaces Keyframe::UpdateCovisibilityConnections (keyframe_be.cpp:559-608) called for every keyframe of a map (after a
+ * merge, a map load, or a GBA round that erased observations): the whole covisibility graph in one call, on the
+ * landmark / observation CSR of cvb_ba_problem (lm_obs_ptr [L+1], obs_kf, obs_skip).  All pointers are host memory.
+ * The reference's result depends on the order the keyframes were updated in and, for equal weights, on pointer order; this
+ * call returns the canonical, order-independent graph:
+ *   1. an observation takes part iff obs_skip is NULL or 0 for it, and its landmark iff lm_valid is NULL or 1 for it;
+ *   2. w(i,j), i != j = the number of participating landmarks observed by both keyframes.  A keyframe appears at most
+ *      once per landmark (a duplicate is CVB_ERR_INVALID);
+ *   3. i and j are connected iff w(i,j) >= min_weight, or i has no neighbour reaching min_weight, w(i,j) > 0 and j is i's
+ *      best neighbour (largest weight, lowest index among equals), or the same with i and j exchanged (the reference's
+ *      "keep the single best one" with AddConnectedKeyframe on the other side);
+ *   4. keyframe i's list, nbr_kf / nbr_w [nbr_ptr[i], nbr_ptr[i+1]), holds its connected keyframes by weight descending,
+ *      then keyframe index ascending: GetConnectedKeyframes order, its first N entries GetBestCovisibilityKeyFrames(N).
+ * min_weight >= 1 (the reference hard-codes 15).  nbr_ptr [K+1] and *n_total (= nbr_ptr[K]) are always written; nbr_kf and
+ * nbr_w [cap] only when *n_total <= cap (call again with a larger cap otherwise); both may be NULL with cap == 0 to ask
+ * for the size.  K == 0 or no observations: an empty graph.  Integer arithmetic only: the output is bit-identical from
+ * run to run.  A pair or edge count beyond the 31-bit index range is CVB_ERR_UNSUPPORTED with the count in the message.
+ */
+CVB_API int cvb_covisibility(cvb_ctx* ctx, int K, int L, const int32_t* lm_obs_ptr, const int32_t* obs_kf,
+                             const uint8_t* obs_skip /*nullable*/, const uint8_t* lm_valid /*nullable*/, int min_weight,
+                             int32_t* nbr_ptr /*[K+1]*/, int32_t* nbr_kf, int32_t* nbr_w, int64_t cap, int64_t* n_total);
+
 #ifdef __cplusplus
 }
 #endif
