@@ -101,6 +101,8 @@ SIGNATURES = {
     "cvb_gba": (C.c_int, [c_vp, c_vp, c_vp, c_vp, c_vp]),
     "cvb_covisibility": (C.c_int, [c_vp, C.c_int, C.c_int, c_vp, c_vp, c_vp, c_vp, C.c_int, c_vp, c_vp, c_vp, C.c_int64,
                                    C.POINTER(C.c_int64)]),
+    "cvb_redundant_keyframes": (C.c_int, [c_vp, C.c_int, C.c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, C.c_double,
+                                          C.c_double, C.c_int, C.c_int, c_vp, C.POINTER(C.c_int32)]),
 }
 
 

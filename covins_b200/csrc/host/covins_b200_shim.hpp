@@ -459,6 +459,55 @@ void UpdateCovisibilityConnections(Context& ctx, MapPtr map, int min_weight = 15
 }
 
 // ---------------------------------------------------------------------------------------------------------------
+// The redundancy pruning of Map::Clean (map_be.cpp:745-811, the covins_prunemap service): the keyframes the sequential
+// culling pass removes, found in one cvb_redundant_keyframes call (the rule is in include/covins_b200.h).  Never culled:
+// the first keyframe of every agent and every keyframe a loop constraint names.  The culled keyframes are handed to the
+// reference's own kf->SetInvalid() in ascending canonical order (keyframe_be.cpp:413-440: the IMU samples go to the
+// successor), then the covisibility graph of what remains is rebuilt.  Landmark erasure stays with the caller's
+// map->Clean(), as after GlobalBundleAdjustment; th_red, max_time_dist and th_obs are the caller's values.
+// ---------------------------------------------------------------------------------------------------------------
+template <class MapPtr>
+void PruneRedundantKeyframes(Context& ctx, MapPtr map, double th_red, double max_time_dist, int th_obs = 3) {
+  using KeyframePtr = typename std::decay<decltype(map->GetKeyframesVec()[0])>::type;
+  using KF = typename KeyframePtr::element_type;
+  auto landmarks = map->GetLandmarksVec();
+  using LandmarkPtr = typename std::decay<decltype(landmarks[0])>::type;
+  std::map<const KF*, int> kf_index;
+  std::vector<KeyframePtr> kfs;
+  detail::canonical_keyframes(map->GetKeyframesVec(), kf_index, kfs);
+  std::vector<LandmarkPtr> lms;
+  std::vector<int32_t> lm_obs_ptr, obs_kf, obs_octave;
+  detail::flatten_observations(landmarks, kf_index, lms, lm_obs_ptr, obs_kf,
+                               [&](int k, int feat, int) { obs_octave.push_back((int32_t)kfs[k]->keypoints_aors_[feat][1]); });
+  const int K = (int)kfs.size(), L = (int)lms.size();
+  std::vector<int32_t> kf_pred((size_t)K, -1);
+  std::vector<double> kf_time((size_t)K);
+  std::vector<uint8_t> kf_protect((size_t)K, 0), culled((size_t)K + 1, 0);
+  for (int k = 0; k < K; k++) {
+    auto pred = kfs[k]->GetPredecessor();
+    if (pred) {
+      auto it = kf_index.find(pred.get());
+      if (it != kf_index.end()) kf_pred[k] = it->second;
+    }
+    kf_time[k] = (double)kfs[k]->timestamp_;
+    if (kfs[k]->id_.first == 0) kf_protect[k] = 1;   // an agent's first keyframe
+  }
+  for (const auto& lc : map->GetLoopConstraints())
+    for (const auto& kf : {lc.kf1, lc.kf2}) {
+      auto it = kf_index.find(kf.get());
+      if (it != kf_index.end()) kf_protect[it->second] = 1;
+    }
+  // octaves above the largest one present change no count: the map's own range is the histogram's
+  const int num_octaves = obs_octave.empty() ? 1 : 1 + *std::max_element(obs_octave.begin(), obs_octave.end());
+  ctx.check(cvb_redundant_keyframes(ctx.get(), K, L, lm_obs_ptr.data(), obs_kf.data(), obs_octave.data(), nullptr, nullptr, kf_pred.data(),
+                                    kf_time.data(), kf_protect.data(), th_red, max_time_dist, th_obs, num_octaves, culled.data(), nullptr),
+            "cvb_redundant_keyframes");
+  for (int k = 0; k < K; k++)
+    if (culled[k]) kfs[k]->SetInvalid();
+  UpdateCovisibilityConnections(ctx, map);
+}
+
+// ---------------------------------------------------------------------------------------------------------------
 // Optimization::PoseGraphOptimization — optimization_be.hpp:46-47.  PoseMap = std::map<idpair, Transform>.
 // ---------------------------------------------------------------------------------------------------------------
 template <class MapPtr, class PoseMap>

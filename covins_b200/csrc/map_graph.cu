@@ -340,3 +340,231 @@ extern "C" int cvb_covisibility(cvb_ctx* ctx, int K, int L, const int32_t* lm_ob
   return cvb_covisibility_budgeted(ctx, K, L, lm_obs_ptr, obs_kf, obs_skip, lm_valid, min_weight, nbr_ptr, nbr_kf, nbr_w, cap, n_total,
                                    MG_PAIR_BUDGET);
 }
+
+// ======================================================================================================================
+// K14 cvb_redundant_keyframes: the sequential culling pass of Map::Clean's redundancy pruning (include/covins_b200.h), as
+// parallel rounds that commit exactly the keyframes the sequential pass culls.
+//   state   hist[l * num_octaves + o] = keyframes not culled that observe l (participating) at octave o; pred_c[k] = pred_C(k);
+//           the undecided keyframes in a list.  A keyframe is undecided until it is kept or culled; the host keeps at once
+//           every keyframe that fails whatever C is (protected, n(k) = 0, no predecessor, no successor);
+//   round   pr_eval_kernel    one warp per undecided k evaluates the rule under the committed C.  A failure is final (adding
+//                             keyframes to C only lowers red_C and moves pred_C earlier): k is kept.  The keyframes that pass
+//                             form T; each writes itself into lowt[l] of its landmarks (64-bit atomicMin of (round, k), so
+//                             the slot needs no reset between rounds);
+//           pr_commit_kernel  k in T is culled iff no lower member of T shares a participating landmark with it and its
+//                             pred_C is not in T; a culled k's observations leave hist (integer atomics);
+//           pr_relink_kernel  pred_C[succ(k)] = pred_C[k] for the culled k, and the keyframes still undecided form the next
+//                             list.
+//   Why this is exact: a culled k's test depends only on culls below it; of those, the committed ones are exact by
+//   induction, and the members of T below k that are still undecided touch neither red_C(k) (no shared landmark) nor
+//   pred_C(k) (not its pred_C; any other ancestor is behind it), whether they are culled later or not.  A cull above k
+//   committed before k is decided shares no landmark with k either.  Two keyframes adjacent in a chain never commit in the
+//   same round (the lower is the higher's pred_C), so the re-links do not chain, and the lowest member of T always commits:
+//   the loop ends after at most as many rounds as there are undecided keyframes.
+// Integer arithmetic except the th_red and time comparisons (one rounded product, one rounded difference, each the same on
+// the host): the output is bit-identical from run to run.
+// ======================================================================================================================
+namespace {
+
+constexpr int PR_THREADS = 256;
+constexpr int PR_WARPS = PR_THREADS / 32;
+constexpr uint32_t PR_ROUND_TOP = 0xfffffffeu;   // lowt key (PR_ROUND_TOP - round) << 32 | k: a later round sorts lower
+
+__device__ __forceinline__ unsigned long long pr_key(int round, int k) {
+  return ((unsigned long long)(PR_ROUND_TOP - (uint32_t)round) << 32) | (uint32_t)k;
+}
+
+__global__ void __launch_bounds__(PR_THREADS) pr_hist_kernel(const int32_t* __restrict__ kf_h, int n, int32_t* hist) {
+  const int t = blockIdx.x * PR_THREADS + threadIdx.x;
+  if (t < n) atomicAdd(&hist[kf_h[t]], 1);
+}
+
+// kf_h[kf_ptr[k] .. kf_ptr[k+1]) = l * num_octaves + octave of k's participating observations
+__global__ void __launch_bounds__(PR_THREADS) pr_eval_kernel(const int32_t* __restrict__ und, int n_und, const int32_t* __restrict__ kf_ptr,
+                                                             const int32_t* __restrict__ kf_h, const int32_t* __restrict__ hist, int num_octaves,
+                                                             int th_obs, double th_red, double max_time_dist, const int32_t* __restrict__ succ,
+                                                             const int32_t* __restrict__ pred_c, const double* __restrict__ kf_time, int round,
+                                                             int32_t* mark, uint8_t* state, unsigned long long* lowt) {
+  const int w = blockIdx.x * PR_WARPS + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+  if (w >= n_und) return;
+  const int k = und[w], b = kf_ptr[k], e = kf_ptr[k + 1];
+  int red = 0;
+  for (int t = b + lane; t < e; t += 32) {
+    const int h = kf_h[t];
+    const int o = h % num_octaves, base = h - o;
+    const int top = min(o + 1, num_octaves - 1);
+    int others = -1;   // k itself is not culled and observes l at o <= o + 1
+    for (int q = 0; q <= top; q++) others += hist[base + q];
+    red += others >= th_obs;
+  }
+  for (int s = 16; s; s >>= 1) red += __shfl_xor_sync(0xffffffffu, red, s);
+  const bool pass = (double)red > __dmul_rn(th_red, (double)(e - b)) && __dsub_rn(kf_time[succ[k]], kf_time[pred_c[k]]) <= max_time_dist;
+  if (!pass) {
+    if (lane == 0) state[k] = 1;
+    return;
+  }
+  if (lane == 0) mark[k] = round;
+  const unsigned long long key = pr_key(round, k);
+  for (int t = b + lane; t < e; t += 32) atomicMin(&lowt[kf_h[t] / num_octaves], key);
+}
+
+__global__ void __launch_bounds__(PR_THREADS) pr_commit_kernel(const int32_t* __restrict__ und, int n_und, const int32_t* __restrict__ kf_ptr,
+                                                               const int32_t* __restrict__ kf_h, int num_octaves, const int32_t* __restrict__ pred_c,
+                                                               const int32_t* __restrict__ mark, const unsigned long long* __restrict__ lowt, int round,
+                                                               int32_t* hist, uint8_t* state) {
+  const int w = blockIdx.x * PR_WARPS + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+  if (w >= n_und) return;
+  const int k = und[w];
+  if (mark[k] != round) return;
+  const int b = kf_ptr[k], e = kf_ptr[k + 1];
+  const unsigned long long key = pr_key(round, k);
+  bool blocked = false;
+  if (lane == 0) {
+    const int p = pred_c[k];
+    blocked = mark[p] == round;
+  }
+  for (int t = b + lane; t < e && !blocked; t += 32) blocked = lowt[kf_h[t] / num_octaves] < key;   // a lower member of T observes l
+  if (__any_sync(0xffffffffu, blocked)) return;
+  if (lane == 0) state[k] = 2;
+  for (int t = b + lane; t < e; t += 32) atomicSub(&hist[kf_h[t]], 1);
+}
+
+__global__ void __launch_bounds__(PR_THREADS) pr_relink_kernel(const int32_t* __restrict__ und, int n_und, const int32_t* __restrict__ succ,
+                                                               const uint8_t* __restrict__ state, int32_t* pred_c, int32_t* und_next, int32_t* n_next) {
+  const int i = blockIdx.x * PR_THREADS + threadIdx.x;
+  if (i >= n_und) return;
+  const int k = und[i];
+  if (state[k] == 2) pred_c[succ[k]] = pred_c[k];
+  else if (state[k] == 0) und_next[atomicAdd(n_next, 1)] = k;
+}
+
+}  // namespace
+
+extern "C" int cvb_redundant_keyframes(cvb_ctx* ctx, int K, int L, const int32_t* lm_obs_ptr, const int32_t* obs_kf, const int32_t* obs_octave,
+                                       const uint8_t* obs_skip, const uint8_t* lm_valid, const int32_t* kf_pred, const double* kf_time,
+                                       const uint8_t* kf_protect, double th_red, double max_time_dist, int th_obs, int num_octaves, uint8_t* culled,
+                                       int32_t* n_rounds) {
+  if (!ctx) return CVB_ERR_INVALID;
+  CVB_GUARD(ctx);
+  CVB_REQUIRE(ctx, K >= 0 && L >= 0, "cvb_redundant_keyframes: negative size (K %d, L %d)", K, L);
+  CVB_REQUIRE(ctx, th_red >= 0.0 && th_red <= 1.0, "cvb_redundant_keyframes: th_red %g is not in [0, 1]", th_red);
+  CVB_REQUIRE(ctx, max_time_dist > 0.0, "cvb_redundant_keyframes: max_time_dist %g is not > 0", max_time_dist);
+  CVB_REQUIRE(ctx, th_obs >= 1, "cvb_redundant_keyframes: th_obs %d < 1", th_obs);
+  CVB_REQUIRE(ctx, num_octaves >= 1 && num_octaves <= 64, "cvb_redundant_keyframes: num_octaves %d is not in [1, 64]", num_octaves);
+  CVB_REQUIRE(ctx, lm_obs_ptr || L == 0, "cvb_redundant_keyframes: lm_obs_ptr is null");
+  CVB_REQUIRE(ctx, K == 0 || (kf_pred && kf_time && kf_protect && culled), "cvb_redundant_keyframes: kf_pred, kf_time, kf_protect and culled are required");
+  CVB_REQUIRE(ctx, L == 0 || lm_obs_ptr[0] == 0, "cvb_redundant_keyframes: lm_obs_ptr[0] = %d, not 0", L ? lm_obs_ptr[0] : 0);
+  for (int l = 0; l < L; l++)
+    CVB_REQUIRE(ctx, lm_obs_ptr[l + 1] >= lm_obs_ptr[l], "cvb_redundant_keyframes: lm_obs_ptr decreases at landmark %d", l);
+  const int n_obs = L ? lm_obs_ptr[L] : 0;
+  CVB_REQUIRE(ctx, (obs_kf && obs_octave) || n_obs == 0, "cvb_redundant_keyframes: obs_kf and obs_octave are required");
+  if ((int64_t)L * num_octaves > MG_INDEX_MAX)
+    return cvb_fail(ctx, CVB_ERR_UNSUPPORTED, "cvb_redundant_keyframes: %d landmarks x %d octaves exceed the 31-bit index range", L, num_octaves);
+
+  // the chains: successors, at most one per keyframe
+  std::vector<int32_t> succ((size_t)K, -1);
+  for (int k = 0; k < K; k++) {
+    const int p = kf_pred[k];
+    CVB_REQUIRE(ctx, p >= -1 && p < k, "cvb_redundant_keyframes: kf_pred[%d] = %d is not in [-1, %d)", k, p, k);
+    if (p < 0) continue;
+    CVB_REQUIRE(ctx, succ[p] < 0, "cvb_redundant_keyframes: keyframe %d has two successors (%d and %d)", p, succ[p], k);
+    succ[p] = k;
+  }
+  // one pass over the observations: validation and the participating ones per keyframe (counting sort by keyframe)
+  std::vector<int32_t> seen_in((size_t)K, -1), kf_ptr((size_t)K + 1, 0);
+  for (int l = 0; l < L; l++) {
+    const bool lm_in = !lm_valid || lm_valid[l];
+    for (int o = lm_obs_ptr[l]; o < lm_obs_ptr[l + 1]; o++) {
+      const int k = obs_kf[o];
+      CVB_REQUIRE(ctx, k >= 0 && k < K, "cvb_redundant_keyframes: obs_kf[%d] = %d outside [0, %d)", o, k, K);
+      CVB_REQUIRE(ctx, seen_in[k] != l, "cvb_redundant_keyframes: keyframe %d observes landmark %d twice", k, l);
+      CVB_REQUIRE(ctx, obs_octave[o] >= 0 && obs_octave[o] < num_octaves, "cvb_redundant_keyframes: obs_octave[%d] = %d outside [0, %d)", o,
+                  obs_octave[o], num_octaves);
+      seen_in[k] = l;
+      if (lm_in && !(obs_skip && obs_skip[o])) kf_ptr[k + 1]++;
+    }
+  }
+  if (n_rounds) *n_rounds = 0;
+  if (K == 0) return CVB_OK;
+  for (int k = 0; k < K; k++) kf_ptr[k + 1] += kf_ptr[k];
+  // every keyframe that fails whatever C is stays: protected, n(k) = 0, no predecessor, no successor
+  std::vector<uint8_t> state((size_t)K, 1);
+  std::vector<int32_t> und;
+  for (int k = 0; k < K; k++)
+    if (!kf_protect[k] && kf_ptr[k + 1] > kf_ptr[k] && kf_pred[k] >= 0 && succ[k] >= 0) {
+      state[k] = 0;
+      und.push_back(k);
+    }
+  std::fill(culled, culled + K, 0);
+  const int n0 = (int)und.size();
+  if (n0 == 0) return CVB_OK;
+  const int n_part = kf_ptr[K];
+  std::vector<int32_t> kf_h((size_t)n_part), fill(kf_ptr.begin(), kf_ptr.end() - 1);
+  for (int l = 0; l < L; l++) {
+    if (lm_valid && !lm_valid[l]) continue;
+    for (int o = lm_obs_ptr[l]; o < lm_obs_ptr[l + 1]; o++)
+      if (!(obs_skip && obs_skip[o])) kf_h[fill[obs_kf[o]]++] = l * num_octaves + obs_octave[o];
+  }
+
+  cudaStream_t st = ctx->stream;
+  const size_t n_bins = (size_t)L * num_octaves;
+  mg_carver cv;
+  int32_t *d_kf_ptr = nullptr, *d_kf_h = nullptr, *hist = nullptr, *pred_c = nullptr, *d_succ = nullptr, *mark = nullptr, *und_a = nullptr,
+          *und_b = nullptr, *d_cnt = nullptr;
+  double* d_time = nullptr;
+  uint8_t* d_state = nullptr;
+  unsigned long long* lowt = nullptr;
+  for (int pass = 0; pass < 2; pass++) {
+    cv.off = 0;
+    d_kf_ptr = cv.take<int32_t>((size_t)K + 1);
+    d_kf_h = cv.take<int32_t>((size_t)n_part);
+    pred_c = cv.take<int32_t>((size_t)K);
+    d_succ = cv.take<int32_t>((size_t)K);
+    d_time = cv.take<double>((size_t)K);
+    d_state = cv.take<uint8_t>((size_t)K);
+    und_a = cv.take<int32_t>((size_t)n0);
+    und_b = cv.take<int32_t>((size_t)n0);
+    hist = cv.take<int32_t>(n_bins);
+    d_cnt = cv.take<int32_t>((size_t)n0 + 1);   // round r counts its survivors in d_cnt[r]: no reset between rounds
+    mark = cv.take<int32_t>((size_t)K);
+    lowt = cv.take<unsigned long long>((size_t)L);
+    if (pass == 0 && !(cv.base = (char*)cvb_ws(ctx, WS_MG_PRUNE, cv.off))) return CVB_ERR_CUDA;
+  }
+  CVB_CUDA(ctx, cudaMemcpyAsync(d_kf_ptr, kf_ptr.data(), kf_ptr.size() * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+  CVB_CUDA(ctx, cudaMemcpyAsync(d_kf_h, kf_h.data(), kf_h.size() * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+  CVB_CUDA(ctx, cudaMemcpyAsync(pred_c, kf_pred, (size_t)K * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+  CVB_CUDA(ctx, cudaMemcpyAsync(d_succ, succ.data(), (size_t)K * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+  CVB_CUDA(ctx, cudaMemcpyAsync(d_time, kf_time, (size_t)K * sizeof(double), cudaMemcpyHostToDevice, st));
+  CVB_CUDA(ctx, cudaMemcpyAsync(d_state, state.data(), (size_t)K, cudaMemcpyHostToDevice, st));
+  CVB_CUDA(ctx, cudaMemcpyAsync(und_a, und.data(), (size_t)n0 * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+  // hist and d_cnt are adjacent: one memset zeroes both; mark = -1 and lowt = all ones match no round
+  CVB_CUDA(ctx, cudaMemsetAsync(hist, 0, (size_t)((char*)mark - (char*)hist), st));
+  CVB_CUDA(ctx, cudaMemsetAsync(mark, 0xff, (size_t)((char*)(lowt + L) - (char*)mark), st));
+  pr_hist_kernel<<<(unsigned)((n_part + PR_THREADS - 1) / PR_THREADS), PR_THREADS, 0, st>>>(d_kf_h, n_part, hist);
+  CVB_CHECK_LAUNCH(ctx);
+  int n_und = n0, round = 0;
+  while (n_und > 0) {
+    const unsigned warp_grid = (unsigned)((n_und + PR_WARPS - 1) / PR_WARPS);
+    pr_eval_kernel<<<warp_grid, PR_THREADS, 0, st>>>(und_a, n_und, d_kf_ptr, d_kf_h, hist, num_octaves, th_obs, th_red, max_time_dist, d_succ,
+                                                     pred_c, d_time, round, mark, d_state, lowt);
+    CVB_CHECK_LAUNCH(ctx);
+    pr_commit_kernel<<<warp_grid, PR_THREADS, 0, st>>>(und_a, n_und, d_kf_ptr, d_kf_h, num_octaves, pred_c, mark, lowt, round, hist, d_state);
+    CVB_CHECK_LAUNCH(ctx);
+    pr_relink_kernel<<<(unsigned)((n_und + PR_THREADS - 1) / PR_THREADS), PR_THREADS, 0, st>>>(und_a, n_und, d_succ, d_state, pred_c, und_b,
+                                                                                               d_cnt + round);
+    CVB_CHECK_LAUNCH(ctx);
+    int32_t next = 0;
+    CVB_CUDA(ctx, cudaMemcpyAsync(&next, d_cnt + round, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+    CVB_CUDA(ctx, cudaStreamSynchronize(st));
+    if (next >= n_und)   // the lowest member of T always commits: a round that decides nothing is a device fault
+      return cvb_fail(ctx, CVB_ERR_CUDA, "cvb_redundant_keyframes: round %d decided no keyframe (%d undecided)", round, n_und);
+    n_und = next;
+    std::swap(und_a, und_b);
+    round++;
+  }
+  CVB_CUDA(ctx, cudaMemcpyAsync(state.data(), d_state, (size_t)K, cudaMemcpyDeviceToHost, st));
+  CVB_CUDA(ctx, cudaStreamSynchronize(st));
+  for (int k = 0; k < K; k++) culled[k] = state[k] == 2;
+  if (n_rounds) *n_rounds = round;
+  return CVB_OK;
+}

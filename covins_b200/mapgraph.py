@@ -3,6 +3,8 @@
 `covisibility` is Keyframe::UpdateCovisibilityConnections (keyframe_be.cpp:559-608) for every keyframe of a map in one
 call: the canonical, order-independent graph include/covins_b200.h defines for cvb_covisibility, on the landmark /
 observation CSR of the flat bundle-adjustment problem (`lm_obs_ptr`, `obs_kf`, `obs_skip`).
+`redundant_keyframes` is the redundancy pruning of Map::Clean (map_be.cpp:745-811): the reference's sequential culling
+pass on the same CSR, reproduced exactly by parallel rounds (cvb_redundant_keyframes).
 """
 from __future__ import annotations
 
@@ -44,3 +46,31 @@ def covisibility(ctx: Context, lm_obs_ptr, obs_kf, K: int, obs_skip=None, lm_val
         if n_total.value <= cap:
             return nbr_ptr, nbr_kf[:n_total.value].copy(), nbr_w[:n_total.value].copy()
         cap = n_total.value
+
+
+def redundant_keyframes(ctx: Context, lm_obs_ptr, obs_kf, obs_octave, kf_pred, kf_time, kf_protect, th_red: float,
+                        max_time_dist: float, th_obs: int = 3, num_octaves: int = 8, obs_skip=None, lm_valid=None):
+    """→ (culled [K] u8, rounds): the keyframes the sequential redundancy-culling pass of Map::Clean (map_be.cpp:745-811)
+    removes, as include/covins_b200.h defines it for cvb_redundant_keyframes, and the number of parallel rounds the call
+    took.  obs_octave [n_obs] (obs_sigma / 2 - 1 of the GBA problem), kf_pred [K] (the chain predecessor, -1 for none),
+    kf_time [K], kf_protect [K] (1 = never culled); obs_skip / lm_valid as for covisibility."""
+    ptr = np.ascontiguousarray(lm_obs_ptr, np.int32)
+    kf = np.ascontiguousarray(obs_kf, np.int32)
+    octv = np.ascontiguousarray(obs_octave, np.int32)
+    assert ptr.ndim == 1 and len(ptr) >= 1 and kf.ndim == 1, "lm_obs_ptr is [L+1], obs_kf is [n_obs]"
+    L = len(ptr) - 1
+    assert len(kf) >= int(ptr[-1]) and octv.shape == kf.shape, "obs_kf / obs_octave are shorter than lm_obs_ptr[L]"
+    pred = np.ascontiguousarray(kf_pred, np.int32)
+    K = len(pred)
+    time = np.ascontiguousarray(kf_time, np.float64)
+    prot = np.ascontiguousarray(kf_protect, np.uint8)
+    assert time.shape == (K,) and prot.shape == (K,), "kf_time and kf_protect are [K]"
+    skip = _opt(obs_skip, len(kf), "obs_skip")
+    valid = _opt(lm_valid, L, "lm_valid")
+    p = lambda a: None if a is None else a.ctypes.data
+    culled = np.zeros(K, np.uint8)
+    rounds = C.c_int32(0)
+    ctx.check(lib().cvb_redundant_keyframes(ctx.handle, K, L, p(ptr), p(kf), p(octv), p(skip), p(valid), p(pred), p(time), p(prot),
+                                            float(th_red), float(max_time_dist), int(th_obs), int(num_octaves), p(culled),
+                                            C.byref(rounds)))
+    return culled, rounds.value

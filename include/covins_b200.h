@@ -958,6 +958,35 @@ CVB_API int cvb_covisibility(cvb_ctx* ctx, int K, int L, const int32_t* lm_obs_p
                              const uint8_t* obs_skip /*nullable*/, const uint8_t* lm_valid /*nullable*/, int min_weight,
                              int32_t* nbr_ptr /*[K+1]*/, int32_t* nbr_kf, int32_t* nbr_w, int64_t cap, int64_t* n_total);
 
+/*
+ * Redundancy pruning of Map::Clean (map_be.cpp:745-811, behind the covins_prunemap service): which keyframes the
+ * reference's sequential culling pass removes, in one call.  ASSUMPTION (parity unpinned beyond the source): the rule is
+ * restated from the ORB-SLAM3 KeyFrameCulling lineage that pass follows (oracle/prune_oracle.c carries the same text).
+ * Inputs: the landmark / observation CSR of cvb_ba_problem (lm_obs_ptr [L+1], obs_kf, nullable obs_skip / lm_valid with
+ * rule 1 of cvb_covisibility), obs_octave [n_obs] (the keypoint's octave, obs_sigma / 2 - 1 of the GBA problem),
+ * kf_pred [K] (the keyframe's predecessor in its agent's chain, -1 if none; kf_pred[k] < k, at most one successor per
+ * keyframe), kf_time [K], kf_protect [K] (1 = never culled).  All pointers are host memory.
+ * For a set C of keyframes culled so far:
+ *   Λ(k)      k's participating landmarks, fixed for the whole pass (landmarks are not erased); n(k) = |Λ(k)|;
+ *   red_C(k)  the number of l in Λ(k) observed by at least th_obs keyframes k' ∉ C, k' != k, with
+ *             octave(k', l) <= octave(k, l) + 1;
+ *   pred_C(k) k's nearest ancestor in its chain that is not in C; succ(k) its original successor.
+ * The pass: for k = 0 .. K-1 in index order, C <- C ∪ {k} iff k is not protected, n(k) > 0,
+ * (double)red_C(k) > th_red * (double)n(k), pred_C(k) and succ(k) both exist, and
+ * kf_time[succ(k)] - kf_time[pred_C(k)] <= max_time_dist.  culled [K] (uint8) = 1 for the members of the final C.
+ * Adding keyframes to C only lowers red_C and moves pred_C earlier, so the call evaluates it in parallel rounds whose commit
+ * rule reproduces the sequential pass exactly; *n_rounds (nullable) receives their number.  Integer arithmetic except the
+ * comparison against th_red and the time difference: the output is bit-identical from run to run.  CVB_ERR_INVALID, before
+ * any launch: a duplicate observer, an octave outside [0, num_octaves), kf_pred[k] >= k or < -1, two successors of one
+ * keyframe, th_red NaN or outside [0, 1], max_time_dist not > 0, th_obs < 1, num_octaves outside [1, 64], a decreasing
+ * lm_obs_ptr.  K == 0: nothing is culled.
+ */
+CVB_API int cvb_redundant_keyframes(cvb_ctx* ctx, int K, int L, const int32_t* lm_obs_ptr, const int32_t* obs_kf,
+                                    const int32_t* obs_octave, const uint8_t* obs_skip /*nullable*/,
+                                    const uint8_t* lm_valid /*nullable*/, const int32_t* kf_pred, const double* kf_time,
+                                    const uint8_t* kf_protect, double th_red, double max_time_dist, int th_obs,
+                                    int num_octaves, uint8_t* culled /*[K]*/, int32_t* n_rounds /*nullable*/);
+
 #ifdef __cplusplus
 }
 #endif
