@@ -1572,8 +1572,14 @@ int engine_setup(Engine& E, const cvb_ba_problem* p, const cvb_ba_options* o) {
     imu_repropagate_kernel<<<grid1(E.n_imu, 64), 64, 0, E.st>>>(E.n_imu, E.imu_j.p, d_ptr.p, d_dt.p, d_acc.p, d_gyr.p, d_a0.p,
                                                                d_g0.p, E.sb[0].p, d_noise.p, E.pre.p, E.flag.p);
     ENG_LAUNCH();
+    int flag = 0;
+    ENG_CUDA(cudaMemcpyAsync(&flag, E.flag.p, sizeof(int), cudaMemcpyDeviceToHost, E.st));
     ENG_CUDA(cudaStreamSynchronize(E.st));
     d_ptr.free_(); d_dt.free_(); d_acc.free_(); d_gyr.free_(); d_a0.free_(); d_g0.free_(); d_noise.free_();
+    // bit 2: a preintegrated covariance P that is not positive definite (e.g. a zero noise sigma in imu_noise); its
+    // sqrt_info would be meaningless, and the reference's chol(P^-1) fails on the same input
+    if (flag & 2)
+      return cvb_fail(ctx, CVB_ERR_NUMERIC, "IMU preintegration covariance is not positive definite (check imu_noise)");
   }
   lap("uploads");
   // ---- vectors, S ----

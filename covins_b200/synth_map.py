@@ -337,21 +337,13 @@ CONFIGS = {
 }
 
 
-def with_camera_model(p: dict, cam_model: int, dist_model: int, dist=None, xi: float = 0.0, seed: int = 0, pix_noise: float = 1.0):
-    """The same map observed through another GlobalEuclideanReprError<Camera, Distortion> instantiation
-    (optimization_be.cpp:186-231): cam_model 0 pinhole / 1 unified(xi), dist_model 0 radtan / 1 equidistant / 2 fisheye (FOV).
-    The inlier observations are re-projected from the ground truth with the new model (+ pixel noise); gross outliers keep
-    their random pixels."""
-    q = dict(p)
-    default = {0: EUROC_DIST, 1: np.array([-0.013, 0.02, -0.012, 0.002]), 2: np.array([0.93, 0.0, 0.0, 0.0])}[dist_model]
-    d = np.asarray(default if dist is None else dist, float)
-    rng = np.random.default_rng(seed)
-    R_ws = quat_to_rot(p["gt_pose"][:, :4]); t_ws = p["gt_pose"][:, 4:]
-    R_sc = quat_to_rot(p["extr"][0][:4]); t_sc = p["extr"][0][4:]
-    obs_lm = np.repeat(np.arange(p["L"]), np.diff(p["lm_obs_ptr"]))
-    k = p["obs_kf"]
-    ps = np.einsum("nji,nj->ni", R_ws[k], p["gt_lm"][obs_lm] - t_ws[k])
-    pc = (ps - t_sc) @ R_sc
+# default distortion coefficients per dist_model: EuRoC radtan, a mild equidistant lens, FOV with w = 0.93
+DEFAULT_DIST = {0: EUROC_DIST, 1: np.array([-0.013, 0.02, -0.012, 0.002]), 2: np.array([0.93, 0.0, 0.0, 0.0])}
+
+
+def project_model(pc, intr, d, cam_model: int, dist_model: int, xi: float = 0.0):
+    """camera-frame points pc [n,3] → pixels [n,2] through one GlobalEuclideanReprError<Camera, Distortion> model:
+    cam_model 0 pinhole / 1 unified(xi), dist_model 0 radtan / 1 equidistant / 2 fisheye (FOV)."""
     den = pc[:, 2] + (xi * np.linalg.norm(pc, axis=1) if cam_model == 1 else 0.0)
     x, y = pc[:, 0] / den, pc[:, 1] / den
     r2 = x * x + y * y
@@ -366,7 +358,24 @@ def with_camera_model(p: dict, cam_model: int, dist_model: int, dist=None, xi: f
         w = d[0]; c = 2 * np.tan(0.5 * w); r = np.sqrt(r2)
         s = np.where(r2 < 1e-5, c / w, np.arctan(c * r) / (w * np.maximum(r, 1e-12)))
         xd, yd = s * x, s * y
-    uv = np.stack([p["intr"][0][0] * xd + p["intr"][0][2], p["intr"][0][1] * yd + p["intr"][0][3]], -1) + rng.normal(0, pix_noise, (len(k), 2))
+    return np.stack([intr[0] * xd + intr[2], intr[1] * yd + intr[3]], -1)
+
+
+def with_camera_model(p: dict, cam_model: int, dist_model: int, dist=None, xi: float = 0.0, seed: int = 0, pix_noise: float = 1.0):
+    """The same map observed through another GlobalEuclideanReprError<Camera, Distortion> instantiation
+    (optimization_be.cpp:186-231): cam_model 0 pinhole / 1 unified(xi), dist_model 0 radtan / 1 equidistant / 2 fisheye (FOV).
+    The inlier observations are re-projected from the ground truth with the new model (+ pixel noise); gross outliers keep
+    their random pixels."""
+    q = dict(p)
+    d = np.asarray(DEFAULT_DIST[dist_model] if dist is None else dist, float)
+    rng = np.random.default_rng(seed)
+    R_ws = quat_to_rot(p["gt_pose"][:, :4]); t_ws = p["gt_pose"][:, 4:]
+    R_sc = quat_to_rot(p["extr"][0][:4]); t_sc = p["extr"][0][4:]
+    obs_lm = np.repeat(np.arange(p["L"]), np.diff(p["lm_obs_ptr"]))
+    k = p["obs_kf"]
+    ps = np.einsum("nji,nj->ni", R_ws[k], p["gt_lm"][obs_lm] - t_ws[k])
+    pc = (ps - t_sc) @ R_sc
+    uv = project_model(pc, p["intr"][0], d, cam_model, dist_model, xi) + rng.normal(0, pix_noise, (len(k), 2))
     keep = p["obs_is_outlier"]
     uv[keep] = p["obs_uv"][keep]
     q["obs_uv"] = uv.astype(np.float32)

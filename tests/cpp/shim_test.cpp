@@ -175,18 +175,20 @@ int main(int argc, char** argv) {
   auto imu_acc = rd<double>(dir, "imu_acc"); auto imu_gyr = rd<double>(dir, "imu_gyr"); auto a0 = rd<double>(dir, "imu_acc0");
   auto g0 = rd<double>(dir, "imu_gyr0"); auto noise = rd<double>(dir, "imu_noise");
   auto li = rd<int32_t>(dir, "loop_i"); auto lj = rd<int32_t>(dir, "loop_j"); auto lq = rd<double>(dir, "loop_q"); auto lt = rd<double>(dir, "loop_t");
+  auto cam_of_kf = rd<int32_t>(dir, "cam_of_kf");   // one calibration per keyframe's camera (all camera 0 when absent)
   const int K = (int)pose.size() / 7, L = (int)lm.size() / 3;
   auto map = std::make_shared<Map>();
   map->id_map_ = 0;
   std::vector<KeyframePtr> kfs(K);
   for (int k = 0; k < K; k++) {
+    const int cam = cam_of_kf.empty() ? 0 : cam_of_kf[k];
     auto kf = std::make_shared<Keyframe>();
     kf->id_ = {(size_t)kfid[k], (size_t)agent[k]};
     kf->T_w_s_ = pose7_to_T(&pose[7 * k]);
     kf->T_w_s_vio_ = kf->T_w_s_;
-    kf->T_s_c_ = pose7_to_T(&extr[0]);
+    kf->T_s_c_ = pose7_to_T(&extr[7 * cam]);
     for (int c = 0; c < 3; c++) { kf->velocity_[c] = sb[9 * k + c]; kf->bias_accel_[c] = sb[9 * k + 3 + c]; kf->bias_gyro_[c] = sb[9 * k + 6 + c]; }
-    for (int c = 0; c < 4; c++) { kf->intr[c] = intr[c]; kf->dist[c] = dist[c]; }
+    for (int c = 0; c < 4; c++) { kf->intr[c] = intr[4 * cam + c]; kf->dist[c] = dist[4 * cam + c]; }
     if (k > 0 && agent[k - 1] == agent[k]) { kf->pred = kfs[k - 1]; kfs[k - 1]->succ = kf; }
     kfs[k] = kf;
   }

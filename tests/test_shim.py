@@ -37,16 +37,22 @@ def _rel(a, b):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("mode,visual_only", [("gba", False), ("gba_visual", True)])
+@pytest.mark.parametrize("mode,visual_only", [("gba", False), ("gba_visual", True), ("gba_cams", False)])
 def test_shim_gba_equals_flat_api(ctx, tmp_path, mode, visual_only):
+    """gba_cams: the visual-inertial GBA on a map with one pinhole / radtan calibration per agent (intrinsics and
+    extrinsic differ): the shim gives every mock keyframe its own camera, the flat problem maps keyframes to cameras"""
     from covins_b200 import optimization as O, synth_map
     if not os.path.exists(EXE):
         build_shim_test()
     # few gross outliers: with ill-posed two-view landmarks in the problem the comparison across two different keyframe
     # orders (and therefore summation orders) is dominated by their sensitivity, not by the shim
     p = synth_map.make_map(seed=21, n_agents=2, kf_per_agent=40, n_lm=2000, outlier_frac=0.01)
+    if mode == "gba_cams":
+        from test_ba_map_shapes import per_agent_cameras
+        p = per_agent_cameras(p, [(0, 0, 0.0)] * 2, seed=22)
+        assert len({tuple(r) for r in p["intr"]}) == 2 and np.array_equal(p["cam_of_kf"], p["agent_of"])
     _dump(p, str(tmp_path))
-    subprocess.check_call([EXE, str(tmp_path), mode])
+    subprocess.check_call([EXE, str(tmp_path), "gba_visual" if visual_only else "gba"])
     ref = O.global_bundle_adjustment(ctx, p, iterations_limit=4, visual_only=visual_only)
     pose = np.fromfile(tmp_path / "out_pose.bin").reshape(-1, 7)
     lm = np.fromfile(tmp_path / "out_lm.bin").reshape(-1, 3)
