@@ -1543,37 +1543,34 @@ extern "C" int cvb_dense_cholesky_solve(cvb_ctx* ctx, const double* A, int n, co
       if (A[(size_t)i * n + j] != 0.0) hs[plan.tile_index(i / T, j / T) * TT + (size_t)(i % T) * T + (j % T)] = A[(size_t)i * n + j];
   for (int i = n; i < np; i++) hs[plan.tile_index(i / T, i / T) * TT + (size_t)(i % T) * T + (i % T)] = 1.0;
   for (int i = 0; i < n; i++) hb[i] = b[i];
-  double* dS = (double*)cvb_ws(ctx, WS_T, hs.size() * sizeof(double));
-  double* dl = (double*)cvb_ws(ctx, WS_Q, (size_t)np * T * sizeof(double));
-  double* dv = (double*)cvb_ws(ctx, WS_OUT0, (size_t)np * 3 * sizeof(double));
-  int* dflag = (int*)cvb_ws(ctx, WS_FLAG, 16);
-  if (!dS || !dl || !dv || !dflag) return CVB_ERR_CUDA;
-  CVB_CUDA(ctx, cudaMemcpyAsync(dS, hs.data(), hs.size() * sizeof(double), cudaMemcpyHostToDevice, st));
-  CVB_CUDA(ctx, cudaMemcpyAsync(dv, hb.data(), np * sizeof(double), cudaMemcpyHostToDevice, st));
+  cvb_block B(ctx, st);
+  double *dS, *db, *dl, *dy, *dx;
+  int* dflag;
+  B.in(dS, hs.data(), hs.size()); B.in(db, hb.data(), np);
+  B.tmp(dl, (size_t)np * T); B.tmp(dy, np);
+  B.out_host(dflag, 1); B.out_host(dx, np);
+  int rc;
+  if ((rc = B.place()) || (rc = B.upload())) return rc;
   cudaEvent_t e0, e1;
   cudaEventCreate(&e0);
   cudaEventCreate(&e1);
-  int rc = plan.upload(ctx, st);
-  if (rc) return rc;
+  if ((rc = plan.upload(ctx, st))) return rc;
   FactorStreams fs;
   if ((rc = fs.create(ctx, nt))) return rc;
   cudaEventRecord(e0, st);
   rc = factor(ctx, dS, dl, dflag, plan, st, fs);
   cudaEventRecord(e1, st);
   if (rc) return rc;
-  rc = solve(ctx, dS, dl, dv, dv + np, dv + 2 * np, plan, st, fs);
+  rc = solve(ctx, dS, dl, db, dy, dx, plan, st, fs);
   if (rc) return rc;
-  int flag = 0;
-  CVB_CUDA(ctx, cudaMemcpyAsync(&flag, dflag, sizeof(int), cudaMemcpyDeviceToHost, st));
-  CVB_CUDA(ctx, cudaMemcpyAsync(hb.data(), dv + 2 * np, np * sizeof(double), cudaMemcpyDeviceToHost, st));
-  CVB_CUDA(ctx, cudaStreamSynchronize(st));
+  if ((rc = B.download())) return rc;
   float ms = 0.f;
   cudaEventElapsedTime(&ms, e0, e1);
   cudaEventDestroy(e0);
   cudaEventDestroy(e1);
   if (factor_ms) *factor_ms = ms;
   plan.release();
-  if (flag) return cvb_fail(ctx, CVB_ERR_NUMERIC, "matrix is not positive definite");
-  for (int i = 0; i < n; i++) x[i] = hb[i];
+  if (*B.host(dflag)) return cvb_fail(ctx, CVB_ERR_NUMERIC, "matrix is not positive definite");
+  memcpy(x, B.host(dx), (size_t)n * sizeof(double));
   return CVB_OK;
 }

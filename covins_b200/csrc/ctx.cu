@@ -1,4 +1,4 @@
-// ctx.cu — context lifetime, error reporting, grow-only workspaces.
+// ctx.cu — context lifetime, error reporting.
 #include <stdarg.h>
 
 #include "cvb_internal.cuh"
@@ -11,47 +11,6 @@ int cvb_fail(cvb_ctx* ctx, int code, const char* fmt, ...) {
   va_end(ap);
   if (ctx) ctx->err = buf;
   return code;
-}
-
-void* cvb_ws(cvb_ctx* ctx, int slot, size_t bytes) {
-  cvb_buf& b = ctx->ws[slot];
-  if (bytes <= b.cap && b.p) return b.p;
-  size_t want = bytes < 256 ? 256 : bytes;
-  if (b.p) {
-    // previous users of the buffer may still be in flight on the ctx stream
-    cudaStreamSynchronize(ctx->stream);
-    cudaFree(b.p);
-    b.p = nullptr;
-    b.cap = 0;
-    want = want + want / 4;  // amortise regrowth
-  }
-  cudaError_t e = cudaMalloc(&b.p, want);
-  if (e != cudaSuccess) {
-    cvb_fail(ctx, CVB_ERR_CUDA, "cudaMalloc(%zu) failed: %s", want, cudaGetErrorString(e));
-    b.p = nullptr;
-    return nullptr;
-  }
-  b.cap = want;
-  return b.p;
-}
-
-void* cvb_pinned(cvb_ctx* ctx, size_t bytes) {
-  if (bytes <= ctx->h_pin_cap && ctx->h_pin) return ctx->h_pin;
-  if (ctx->h_pin) {
-    cudaStreamSynchronize(ctx->stream);
-    cudaFreeHost(ctx->h_pin);
-    ctx->h_pin = nullptr;
-    ctx->h_pin_cap = 0;
-  }
-  size_t want = bytes < 4096 ? 4096 : bytes + bytes / 4;
-  cudaError_t e = cudaMallocHost(&ctx->h_pin, want);
-  if (e != cudaSuccess) {
-    cvb_fail(ctx, CVB_ERR_CUDA, "cudaMallocHost(%zu) failed: %s", want, cudaGetErrorString(e));
-    ctx->h_pin = nullptr;
-    return nullptr;
-  }
-  ctx->h_pin_cap = want;
-  return ctx->h_pin;
 }
 
 extern "C" {
@@ -97,8 +56,6 @@ int cvb_ctx_destroy(cvb_ctx* ctx) {
   cudaSetDevice(ctx->device);
   cudaStreamSynchronize(ctx->stream);
   cvb_ba_free(ctx);
-  for (auto& b : ctx->ws)
-    if (b.p) cudaFree(b.p);
   if (ctx->h_pin) cudaFreeHost(ctx->h_pin);
   cudaStreamDestroy(ctx->stream);
   delete ctx;

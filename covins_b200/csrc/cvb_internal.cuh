@@ -4,6 +4,7 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
+#include <string.h>
 #include <atomic>
 #include <mutex>
 #include <string>
@@ -11,22 +12,16 @@
 
 #include "../../include/covins_b200.h"
 
-struct cvb_buf {
-  void* p = nullptr;
-  size_t cap = 0;
-};
-
 struct cvb_ctx {
   int device = 0;
   cudaStream_t stream = nullptr;
   int sm_count = 132;
   int64_t launches = 0;
   std::string err;
-  // grow-only device workspaces (named slots so independent stages never alias)
-  cvb_buf ws[30];   // one per WS_* slot below
-  // pinned host staging
+  // pinned host staging (grow-only), used by one cvb_block at a time (pin_busy)
   void* h_pin = nullptr;
   size_t h_pin_cap = 0;
+  bool pin_busy = false;
   void* ba = nullptr;  // BA state (owned by ba_*.cu)
   // resident operand tiles of a train set (set by the map database around its matching call, see tc_match.cu): when the
   // matcher is handed the packed rows `xt_for`, their pre-expanded tiles are at `xt` / `xt_seg_tile`
@@ -37,11 +32,6 @@ struct cvb_ctx {
   // threads — calls on one ctx are serialised, concurrency comes from one ctx per thread
   mutable std::recursive_mutex mtx;
 };
-
-enum { WS_Q = 0, WS_T, WS_SEG, WS_OUT0, WS_OUT1, WS_OUT2, WS_PART_I, WS_PART_D, WS_LIST_I, WS_LIST_D, WS_SKIPA,
-       WS_SKIPB, WS_TMP0, WS_TMP1, WS_FLAG, WS_MISC, WS_CHUNK_PS, WS_CHUNK_OFF, WS_GS0, WS_GS1, WS_GS2, WS_GS3, WS_GS4, WS_GS5, WS_GS6, WS_XT, WS_XT_TILE,
-       WS_MG_EDGES, WS_MG_ROWS, WS_MG_PRUNE };
-static_assert(WS_MG_PRUNE < (int)(sizeof(cvb_ctx::ws) / sizeof(cvb_buf)), "cvb_ctx::ws has a buffer per workspace slot");
 
 // cudaFuncSetAttribute applies to the CURRENT device: one flag per (call site, device), so that a process that opens contexts
 // on several GPUs raises the dynamic shared-memory limit on each of them
@@ -55,8 +45,62 @@ struct cvb_once_per_device {
 };
 
 int cvb_fail(cvb_ctx* ctx, int code, const char* fmt, ...);
-void* cvb_ws(cvb_ctx* ctx, int slot, size_t bytes);          // returns nullptr on failure (ctx->err set)
-void* cvb_pinned(cvb_ctx* ctx, size_t bytes);
+
+// One call's device memory: one allocation from the device's stream-ordered pool on the stream the call's work runs on
+// (st), freed there when the block goes out of scope, early returns included.  So the scratch of a nested call, or of a
+// _dev call on a caller's stream, is never shared with another call.  Arrays are bound to pointer variables, which place()
+// sets: the inputs, then the scratch, then the outputs, each in declaration order, every array on a 256-byte boundary.
+//   in(p, src, n)          uploaded by upload(); src == nullptr: filled through host(p) between place() and upload()
+//   tmp(p, n)              device only
+//   out(p, dst, n)         downloaded by download() and copied to dst; dst == nullptr: left on the device
+//   out_host(p, n, want)   downloaded (when want) for the call to read through host(p) after download()
+// download() moves one range, from the first output to the end of the last one wanted: optional outputs are declared last.
+// Nothing is zeroed; pool memory holds whatever an earlier user left.  Inputs and downloaded outputs are staged in the ctx's
+// pinned buffer, which one block holds at a time: a second staging block on the same ctx is refused.  A direct block
+// (staged = false) instead copies each input from its src and each output to its dst, one copy per array and no host copy:
+// for calls whose arrays are large (rows of descriptors, possibly in the caller's pinned memory); it has no host().
+struct cvb_block {
+  cvb_block(cvb_ctx* c, cudaStream_t s, bool staged = true) : ctx(c), st(s), staged(staged) {}
+  ~cvb_block() {
+    if (d) cudaFreeAsync(d, st);
+    if (h) ctx->pin_busy = false;
+  }
+  cvb_block(const cvb_block&) = delete;
+  cvb_block& operator=(const cvb_block&) = delete;
+
+  template <class T> void in(T*& p, const void* src, size_t n) { arrs.push_back({(void**)&p, n * sizeof(T), kIn, src, nullptr, true}); }
+  template <class T> void tmp(T*& p, size_t n) { arrs.push_back({(void**)&p, n * sizeof(T), kTmp, nullptr, nullptr, false}); }
+  template <class T> void out(T*& p, void* dst, size_t n) { arrs.push_back({(void**)&p, n * sizeof(T), kOut, nullptr, dst, dst != nullptr}); }
+  template <class T> void out_host(T*& p, size_t n, bool want = true) { arrs.push_back({(void**)&p, n * sizeof(T), kOut, nullptr, nullptr, want}); }
+
+  int place();      // the allocation; sets every bound pointer and copies the inputs' src into the pinned buffer
+  int upload();     // one H2D copy of the inputs
+  int download();   // one D2H copy of the wanted outputs, a synchronisation of st, the copies into the callers' arrays
+  // the pinned copy of bound input or output p
+  template <class T> T* host(const T* p) const {
+    const size_t o = (const unsigned char*)p - d;
+    return (T*)(o < out_lo ? h + o : h + in_hi + (o - out_lo));
+  }
+
+ private:
+  enum { kIn, kTmp, kOut };
+  struct Arr {
+    void** p;
+    size_t bytes;
+    int kind;
+    const void* src;
+    void* dst;
+    bool want;
+    size_t off;
+  };
+  cvb_ctx* ctx;
+  cudaStream_t st;
+  bool staged;
+  std::vector<Arr> arrs;
+  unsigned char* d = nullptr;   // device block
+  unsigned char* h = nullptr;   // pinned: [0, in_hi) the inputs, then [out_lo, out_hi) of the outputs
+  size_t in_hi = 0, out_lo = 0, out_hi = 0;
+};
 
 // match_kernels.cu: the fused 2-NN + ratio filter of cvb_match_hamming_batch for n_pairs pairs of keyframes of one device
 // descriptor table d_desc in one launch on ctx->stream.  d_pairs [n_pairs][5] = (query row0, query rows, train row0, train rows,
@@ -120,6 +164,81 @@ int cvb_covisibility_budgeted(cvb_ctx* ctx, int K, int L, const int32_t* lm_obs_
   do {                                                                   \
     if (!(cond)) return cvb_fail((ctx), CVB_ERR_INVALID, __VA_ARGS__);   \
   } while (0)
+
+// The context's pinned staging buffer, grown to at least `bytes` (nullptr on failure, ctx->err set).  It and the block's
+// functions are defined here, in the header, so that a translation unit built without ctx.cu (the Cholesky test
+// harnesses) needs only cvb_fail.
+inline void* cvb_pinned(cvb_ctx* ctx, size_t bytes) {
+  if (bytes <= ctx->h_pin_cap && ctx->h_pin) return ctx->h_pin;
+  if (ctx->h_pin) {
+    cudaStreamSynchronize(ctx->stream);
+    cudaFreeHost(ctx->h_pin);
+    ctx->h_pin = nullptr;
+    ctx->h_pin_cap = 0;
+  }
+  size_t want = bytes < 4096 ? 4096 : bytes + bytes / 4;
+  cudaError_t e = cudaMallocHost(&ctx->h_pin, want);
+  if (e != cudaSuccess) {
+    cvb_fail(ctx, CVB_ERR_CUDA, "cudaMallocHost(%zu) failed: %s", want, cudaGetErrorString(e));
+    ctx->h_pin = nullptr;
+    return nullptr;
+  }
+  ctx->h_pin_cap = want;
+  return ctx->h_pin;
+}
+
+inline int cvb_block::place() {
+  const auto align = [](size_t o) { return (o + 255) & ~size_t(255); };
+  size_t top = 0;
+  for (int kind : {kIn, kTmp, kOut}) {
+    if (kind == kOut) out_lo = out_hi = top = align(top);
+    for (Arr& a : arrs) {
+      if (a.kind != kind) continue;
+      a.off = align(top);
+      top = a.off + a.bytes;
+      if (kind == kIn) in_hi = top;
+      if (kind == kOut && a.want) out_hi = top;
+    }
+  }
+  if (staged && (in_hi || out_hi > out_lo)) {
+    if (ctx->pin_busy) return cvb_fail(ctx, CVB_ERR_INVALID, "host staging nested in another call's host staging on the same ctx");
+    if (!(h = (unsigned char*)cvb_pinned(ctx, in_hi + (out_hi - out_lo)))) return CVB_ERR_CUDA;
+    ctx->pin_busy = true;
+    for (const Arr& a : arrs)
+      if (a.kind == kIn && a.src && a.bytes) memcpy(h + a.off, a.src, a.bytes);
+  }
+  const cudaError_t e = cudaMallocAsync((void**)&d, top > 256 ? top : 256, st);
+  if (e != cudaSuccess) {
+    d = nullptr;
+    return cvb_fail(ctx, CVB_ERR_CUDA, "cudaMallocAsync(%zu) failed: %s", top, cudaGetErrorString(e));
+  }
+  for (const Arr& a : arrs) *a.p = d + a.off;
+  return CVB_OK;
+}
+
+inline int cvb_block::upload() {
+  if (staged) {
+    if (in_hi) CVB_CUDA(ctx, cudaMemcpyAsync(d, h, in_hi, cudaMemcpyHostToDevice, st));
+    return CVB_OK;
+  }
+  for (const Arr& a : arrs)
+    if (a.kind == kIn && a.src && a.bytes) CVB_CUDA(ctx, cudaMemcpyAsync(d + a.off, a.src, a.bytes, cudaMemcpyHostToDevice, st));
+  return CVB_OK;
+}
+
+inline int cvb_block::download() {
+  if (!staged) {
+    for (const Arr& a : arrs)
+      if (a.kind == kOut && a.dst && a.bytes) CVB_CUDA(ctx, cudaMemcpyAsync(a.dst, d + a.off, a.bytes, cudaMemcpyDeviceToHost, st));
+    CVB_CUDA(ctx, cudaStreamSynchronize(st));
+    return CVB_OK;
+  }
+  if (out_hi > out_lo) CVB_CUDA(ctx, cudaMemcpyAsync(h + in_hi, d + out_lo, out_hi - out_lo, cudaMemcpyDeviceToHost, st));
+  CVB_CUDA(ctx, cudaStreamSynchronize(st));
+  for (const Arr& a : arrs)
+    if (a.kind == kOut && a.dst && a.bytes) memcpy(a.dst, h + in_hi + (a.off - out_lo), a.bytes);
+  return CVB_OK;
+}
 
 static inline cudaStream_t cvb_stream(cvb_ctx* ctx, void* s) { return s ? (cudaStream_t)s : ctx->stream; }
 

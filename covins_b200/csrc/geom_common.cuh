@@ -1,5 +1,5 @@
 // geom_common.cuh — helpers shared by the geometric-verification translation units (geom_kernels.cu, ransac_abs.cu,
-// ransac_rel.cu): the host staging block and the device arithmetic, including the cross product, the largest-cross-product
+// ransac_rel.cu): the device arithmetic, including the cross product, the largest-cross-product
 // null vector of a rank-2 3x3 (P3P's eigenvectors, the 5-point solver's roots and baseline), the per-correspondence
 // absolute-pose score (score_abs_kernel, ransac_abs_kernel), the relative-pose score (score_rel_kernel, ransac_rel_kernel) and
 // the 3x3 inverse of the RANSAC solvers.  Every device operation is an explicit round-to-nearest non-fused intrinsic, so
@@ -12,18 +12,6 @@
 #include <vector>
 
 namespace {
-
-// host staging: everything of a call goes through ONE pinned block and ONE device block
-struct Stager {
-  std::vector<unsigned char> h;
-  size_t put(const void* p, size_t bytes) {
-    const size_t off = (h.size() + 15) & ~size_t(15);
-    h.resize(off + bytes);
-    if (p && bytes) memcpy(h.data() + off, p, bytes);
-    return off;
-  }
-  size_t reserve(size_t bytes) { return put(nullptr, bytes); }
-};
 
 __device__ __forceinline__ double mul(double a, double b) { return __dmul_rn(a, b); }
 __device__ __forceinline__ double add(double a, double b) { return __dadd_rn(a, b); }

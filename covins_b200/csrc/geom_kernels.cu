@@ -288,20 +288,15 @@ __global__ void __launch_bounds__(256) score_rel_kernel(const double* __restrict
   if ((threadIdx.x & 31) == 0 && in) atomicAdd(n_inliers + h, in);
 }
 
-// with_desc = false: the descriptor rows are staged elsewhere by the caller, who sets off[2]
-size_t stage_kf(Stager& S, const cvb_kf_view* v, size_t off[9], bool with_desc = true) {
+// keyframe view v into d: its arrays bound as inputs of B, its scalars copied (with_desc = false: the caller binds the
+// descriptor rows)
+void bind_kf(cvb_block& B, DevKf& d, const cvb_kf_view* v, bool with_desc = true) {
   const size_t n = (size_t)v->n;
-  off[0] = S.put(v->kp, n * 8); off[1] = S.put(v->octave, n * 4); off[2] = with_desc ? S.put(v->desc, n * 32) : 0; off[3] = S.put(v->lm_valid, n);
-  off[4] = S.put(v->lm_pos, n * 24); off[5] = S.put(v->lm_maxdist, n * 8); off[6] = S.put(v->lm_desc, n * 32);
-  off[7] = S.put(v->grid_ptr, (GRID_COLS * GRID_ROWS + 1) * 4);
-  off[8] = S.put(v->grid_idx, (size_t)v->grid_ptr[GRID_COLS * GRID_ROWS] * 4);
-  return off[8];
-}
-void fill_dev(DevKf& d, const cvb_kf_view* v, const unsigned char* base, const size_t off[9]) {
+  B.in(d.kp, v->kp, n * 2); B.in(d.octave, v->octave, n);
+  if (with_desc) B.in(d.desc, v->desc, n * 32);
+  B.in(d.lm_valid, v->lm_valid, n); B.in(d.lm_pos, v->lm_pos, n * 3); B.in(d.lm_maxdist, v->lm_maxdist, n); B.in(d.lm_desc, v->lm_desc, n * 32);
+  B.in(d.grid_ptr, v->grid_ptr, GRID_COLS * GRID_ROWS + 1); B.in(d.grid_idx, v->grid_idx, (size_t)v->grid_ptr[GRID_COLS * GRID_ROWS]);
   d.n = v->n;
-  d.kp = (const float*)(base + off[0]); d.octave = (const float*)(base + off[1]); d.desc = base + off[2]; d.lm_valid = base + off[3];
-  d.lm_pos = (const double*)(base + off[4]); d.lm_maxdist = (const double*)(base + off[5]); d.lm_desc = base + off[6];
-  d.grid_ptr = (const int*)(base + off[7]); d.grid_idx = (const int*)(base + off[8]);
   d.grid_w_inv = v->grid_w_inv; d.grid_h_inv = v->grid_h_inv;
   memcpy(d.K, v->K, sizeof(d.K)); memcpy(d.Tcw, v->Tcw, sizeof(d.Tcw)); memcpy(d.img, v->img, sizeof(d.img));
 }
@@ -338,48 +333,30 @@ int cvb_search_by_se3_batch(cvb_ctx* ctx, const cvb_kf_view* kf1, const cvb_kf_v
   }
   CVB_REQUIRE(ctx, n2_total == 0 || already2, "search_by_se3: already2 is null");
   const size_t n1 = (size_t)kf1->n;
-  // ---- stage inputs ----
-  Stager S;
-  size_t off1[9];
-  stage_kf(S, kf1, off1);
-  std::vector<size_t> off2((size_t)n_pairs * 9);
-  for (int p = 0; p < n_pairs; p++) stage_kf(S, kf2 + p, &off2[(size_t)p * 9]);
-  const size_t o_a1 = S.put(already1, (size_t)n_pairs * n1), o_a2 = S.put(already2, n2_total);
-  const size_t o_pairs = S.reserve((size_t)n_pairs * sizeof(DevPair));
-  const size_t in_bytes = S.h.size();
-  // outputs live behind the inputs in the same device block
-  const size_t o_m1 = S.reserve((size_t)n_pairs * n1 * 4), o_m2 = S.reserve(n2_total * 4), o_m12 = S.reserve((size_t)n_pairs * n1 * 4),
-               o_nf = S.reserve((size_t)n_pairs * 4);
-  const size_t total = S.h.size();
-  unsigned char* dbase = (unsigned char*)cvb_ws(ctx, WS_GS0, total);
-  unsigned char* hpin = (unsigned char*)cvb_pinned(ctx, total);
-  if (!dbase || !hpin) return CVB_ERR_CUDA;
-  DevKf d1;
-  fill_dev(d1, kf1, dbase, off1);
-  DevPair* hp = reinterpret_cast<DevPair*>(S.h.data() + o_pairs);
+  cvb_block B(ctx, ctx->stream);
+  DevKf d1{};
+  bind_kf(B, d1, kf1);
+  std::vector<DevPair> hp((size_t)n_pairs);   // the records the kernel reads, uploaded at d_pairs
+  for (int p = 0; p < n_pairs; p++) bind_kf(B, hp[p].k2, kf2 + p);
+  const uint8_t *d_a1, *d_a2;
+  DevPair* d_pairs;
+  int *d_m1, *d_m2, *d_m12, *d_nf;
+  B.in(d_a1, already1, (size_t)n_pairs * n1); B.in(d_a2, already2, n2_total); B.in(d_pairs, nullptr, n_pairs);
+  B.out(d_m1, match1, (size_t)n_pairs * n1); B.out(d_m2, match2, n2_total); B.out(d_m12, match12, (size_t)n_pairs * n1); B.out(d_nf, n_found, n_pairs);
+  if (const int rc = B.place()) return rc;
   size_t a2 = 0;
   for (int p = 0; p < n_pairs; p++) {
     DevPair& P = hp[p];
-    fill_dev(P.k2, kf2 + p, dbase, &off2[(size_t)p * 9]);
     memcpy(P.T12, T12 + 16 * (size_t)p, sizeof(P.T12)); memcpy(P.T21, T21 + 16 * (size_t)p, sizeof(P.T21));
-    P.already1 = dbase + o_a1 + (size_t)p * n1; P.already2 = dbase + o_a2 + a2;
-    P.match1 = (int*)(dbase + o_m1) + (size_t)p * n1; P.match2 = (int*)(dbase + o_m2) + a2;
-    P.match12 = (int*)(dbase + o_m12) + (size_t)p * n1; P.n_found = (int*)(dbase + o_nf) + p;
+    P.already1 = d_a1 + (size_t)p * n1; P.already2 = d_a2 + a2;
+    P.match1 = d_m1 + (size_t)p * n1; P.match2 = d_m2 + a2; P.match12 = d_m12 + (size_t)p * n1; P.n_found = d_nf + p;
     a2 += (size_t)kf2[p].n;
   }
-  memcpy(hpin, S.h.data(), in_bytes);
-  cudaStream_t st = ctx->stream;
-  CVB_CUDA(ctx, cudaMemcpyAsync(dbase, hpin, in_bytes, cudaMemcpyHostToDevice, st));
-  search_se3_kernel<<<n_pairs, 256, 0, st>>>(d1, reinterpret_cast<const DevPair*>(dbase + o_pairs), prm->th, prm->desc_th_low,
-                                             prm->scale_factor, prm->num_octaves);
+  memcpy(B.host(d_pairs), hp.data(), hp.size() * sizeof(DevPair));
+  if (const int rc = B.upload()) return rc;
+  search_se3_kernel<<<n_pairs, 256, 0, ctx->stream>>>(d1, d_pairs, prm->th, prm->desc_th_low, prm->scale_factor, prm->num_octaves);
   CVB_CHECK_LAUNCH(ctx);
-  CVB_CUDA(ctx, cudaMemcpyAsync(hpin + o_m1, dbase + o_m1, total - o_m1, cudaMemcpyDeviceToHost, st));
-  CVB_CUDA(ctx, cudaStreamSynchronize(st));
-  memcpy(match12, hpin + o_m12, (size_t)n_pairs * n1 * 4);
-  memcpy(n_found, hpin + o_nf, (size_t)n_pairs * 4);
-  if (match1) memcpy(match1, hpin + o_m1, (size_t)n_pairs * n1 * 4);
-  if (match2) memcpy(match2, hpin + o_m2, n2_total * 4);
-  return CVB_OK;
+  return B.download();
 }
 
 static int score_common(cvb_ctx* ctx, bool relative, const double* model, int n_hyp, const double* a, const double* b, const double* s1,
@@ -393,42 +370,31 @@ static int score_common(cvb_ctx* ctx, bool relative, const double* model, int n_
   for (int h = 0; h < n_hyp; h++) n_inliers[h] = 0;
   if (n_hyp == 0 || n == 0) return CVB_OK;
   const size_t hn = (size_t)n_hyp * n;
-  Stager S;
-  const size_t o_model = S.put(model, (size_t)n_hyp * 96), o_a = S.put(a, (size_t)n * 24), o_b = S.put(b, (size_t)n * 24),
-               o_s1 = S.put(s1, (size_t)n * 8);
-  size_t o_s2 = 0, o_cam = 0;
-  if (relative) o_s2 = S.put(s2, (size_t)n * 8);
-  else {   // one camera: offset (3) directly followed by the rotation (9, row-major)
-    double cam[12];
+  double cam[12];   // one camera: offset (3) directly followed by the rotation (9, row-major)
+  cvb_block B(ctx, ctx->stream);
+  const double *d_model, *d_a, *d_b, *d_s1, *d_s2, *d_cam;
+  int* d_cnt;
+  double* d_sc = nullptr;
+  uint8_t* d_in = nullptr;
+  B.in(d_model, model, (size_t)n_hyp * 12); B.in(d_a, a, (size_t)n * 3); B.in(d_b, b, (size_t)n * 3); B.in(d_s1, s1, n);
+  if (relative) {
+    B.in(d_s2, s2, n);
+  } else {
     memcpy(cam, cam_off, 24); memcpy(cam + 3, cam_rot, 72);
-    o_cam = S.put(cam, sizeof(cam));
+    B.in(d_cam, cam, 12);
   }
-  const size_t in_bytes = S.h.size();
-  const size_t o_cnt = S.reserve((size_t)n_hyp * 4), o_sc = scores ? S.reserve(hn * 8) : 0, o_in = inlier ? S.reserve(hn) : 0;
-  const size_t total = S.h.size();
-  unsigned char* d = (unsigned char*)cvb_ws(ctx, WS_GS1, total);
-  unsigned char* hpin = (unsigned char*)cvb_pinned(ctx, total);
-  if (!d || !hpin) return CVB_ERR_CUDA;
-  memcpy(hpin, S.h.data(), in_bytes);
+  B.out(d_cnt, n_inliers, n_hyp);
+  if (scores) B.out(d_sc, scores, hn);
+  if (inlier) B.out(d_in, inlier, hn);
+  if (const int rc = B.place()) return rc;
+  if (const int rc = B.upload()) return rc;
   cudaStream_t st = ctx->stream;
-  CVB_CUDA(ctx, cudaMemcpyAsync(d, hpin, in_bytes, cudaMemcpyHostToDevice, st));
-  CVB_CUDA(ctx, cudaMemsetAsync(d + o_cnt, 0, (size_t)n_hyp * 4, st));
+  CVB_CUDA(ctx, cudaMemsetAsync(d_cnt, 0, (size_t)n_hyp * 4, st));
   const dim3 grid((unsigned)((n + 255) / 256), (unsigned)n_hyp);
-  if (relative)
-    score_rel_kernel<<<grid, 256, 0, st>>>((const double*)(d + o_model), (const double*)(d + o_a), (const double*)(d + o_b), (const double*)(d + o_s1),
-                                           (const double*)(d + o_s2), n, threshold, scores ? (double*)(d + o_sc) : nullptr,
-                                           inlier ? d + o_in : nullptr, (int*)(d + o_cnt));
-  else
-    score_abs_kernel<<<grid, 256, 0, st>>>((const double*)(d + o_model), (const double*)(d + o_a), (const double*)(d + o_b), (const double*)(d + o_s1), n,
-                                           (const double*)(d + o_cam), threshold, scores ? (double*)(d + o_sc) : nullptr,
-                                           inlier ? d + o_in : nullptr, (int*)(d + o_cnt));
+  if (relative) score_rel_kernel<<<grid, 256, 0, st>>>(d_model, d_a, d_b, d_s1, d_s2, n, threshold, d_sc, d_in, d_cnt);
+  else score_abs_kernel<<<grid, 256, 0, st>>>(d_model, d_a, d_b, d_s1, n, d_cam, threshold, d_sc, d_in, d_cnt);
   CVB_CHECK_LAUNCH(ctx);
-  CVB_CUDA(ctx, cudaMemcpyAsync(hpin + o_cnt, d + o_cnt, total - o_cnt, cudaMemcpyDeviceToHost, st));
-  CVB_CUDA(ctx, cudaStreamSynchronize(st));
-  memcpy(n_inliers, hpin + o_cnt, (size_t)n_hyp * 4);
-  if (scores) memcpy(scores, hpin + o_sc, hn * 8);
-  if (inlier) memcpy(inlier, hpin + o_in, hn);
-  return CVB_OK;
+  return B.download();
 }
 
 int cvb_score_absolute_pose_batch(cvb_ctx* ctx, const double* model, int n_hyp, const double* pts, const double* f, const double* sigma,
@@ -460,44 +426,33 @@ int cvb_search_by_projection(cvb_ctx* ctx, const cvb_kf_view* kf, const int32_t*
               action && best_idx, "search_by_projection: null landmark arrays");
   for (int i = 0; i < m; i++) CVB_REQUIRE(ctx, lms->feat_idx[i] >= -1 && lms->feat_idx[i] < n, "search_by_projection: feat_idx out of range");
   for (int i = 0; i < n; i++) CVB_REQUIRE(ctx, kf_lm_cand[i] >= -1 && kf_lm_cand[i] < m, "search_by_projection: kf_lm_cand out of range");
-  Stager S;
-  const size_t ng = (size_t)kf->grid_ptr[GRID_COLS * GRID_ROWS];
-  const size_t o_kp = S.put(kf->kp, (size_t)n * 8), o_oc = S.put(kf->octave, (size_t)n * 4), o_de = S.put(kf->desc, (size_t)n * 32),
-               o_gp = S.put(kf->grid_ptr, (GRID_COLS * GRID_ROWS + 1) * 4), o_gi = S.put(kf->grid_idx, ng * 4);
-  const size_t o_hl = S.put(kf->lm_valid, (size_t)n), o_lc = S.put(kf_lm_cand, (size_t)n * 4), o_ma = S.put(matched, (size_t)n);
-  const size_t o_va = S.put(lms->valid, (size_t)m), o_po = S.put(lms->pos, (size_t)m * 24), o_no = S.put(lms->normal, (size_t)m * 24),
-               o_mi = S.put(lms->min_dist, (size_t)m * 8), o_mx = S.put(lms->max_dist, (size_t)m * 8), o_md = S.put(lms->max_distance, (size_t)m * 8),
-               o_ld = S.put(lms->desc, (size_t)m * 32), o_fi = S.put(lms->feat_idx, (size_t)m * 4), o_fe = S.put(lms->feat_idx, (size_t)m * 4);
-  const size_t in_bytes = S.h.size();
-  const size_t o_ci = S.reserve((size_t)m * kProjCap * 4), o_cd = S.reserve((size_t)m * kProjCap * 4), o_cn = S.reserve((size_t)m * 4);
-  const size_t o_out = S.reserve(0), o_ac = S.reserve((size_t)m * 4), o_bi = S.reserve((size_t)m * 4), o_nm = S.reserve(8);
-  const size_t total = S.h.size();
-  unsigned char* d = (unsigned char*)cvb_ws(ctx, WS_GS4, total);
-  unsigned char* hpin = (unsigned char*)cvb_pinned(ctx, total);
-  if (!d || !hpin) return CVB_ERR_CUDA;
+  cvb_block B(ctx, ctx->stream);
   DevKf K{};
-  K.n = n; K.kp = (const float*)(d + o_kp); K.octave = (const float*)(d + o_oc); K.desc = d + o_de; K.grid_ptr = (const int*)(d + o_gp);
-  K.grid_idx = (const int*)(d + o_gi); K.grid_w_inv = kf->grid_w_inv; K.grid_h_inv = kf->grid_h_inv;
-  memcpy(K.img, kf->img, sizeof(K.img));
   ProjDev P{};
-  P.m = m; P.valid = d + o_va; P.pos = (const double*)(d + o_po); P.normal = (const double*)(d + o_no); P.min_dist = (const double*)(d + o_mi);
-  P.max_dist = (const double*)(d + o_mx); P.max_distance = (const double*)(d + o_md); P.desc = d + o_ld; P.feat_idx = (const int*)(d + o_fi);
+  B.in(K.kp, kf->kp, (size_t)n * 2); B.in(K.octave, kf->octave, n); B.in(K.desc, kf->desc, (size_t)n * 32);
+  B.in(K.grid_ptr, kf->grid_ptr, GRID_COLS * GRID_ROWS + 1); B.in(K.grid_idx, kf->grid_idx, (size_t)kf->grid_ptr[GRID_COLS * GRID_ROWS]);
+  B.in(P.has_lm, kf->lm_valid, n); B.in(P.lm_cand, kf_lm_cand, n); B.in(P.matched, matched, n);
+  B.in(P.valid, lms->valid, m); B.in(P.pos, lms->pos, (size_t)m * 3); B.in(P.normal, lms->normal, (size_t)m * 3); B.in(P.min_dist, lms->min_dist, m);
+  B.in(P.max_dist, lms->max_dist, m); B.in(P.max_distance, lms->max_distance, m); B.in(P.desc, lms->desc, (size_t)m * 32);
+  B.in(P.feat_idx, lms->feat_idx, m); B.in(P.feat, lms->feat_idx, m);
+  B.tmp(P.cand_idx, (size_t)m * kProjCap); B.tmp(P.cand_dist, (size_t)m * kProjCap); B.tmp(P.cand_n, m);
+  B.out_host(P.action, m); B.out_host(P.best_idx, m); B.out_host(P.n_matches, 2);   // n_matches, then the overflow flag
+  if (const int rc = B.place()) return rc;
+  if (const int rc = B.upload()) return rc;
+  K.n = n; K.grid_w_inv = kf->grid_w_inv; K.grid_h_inv = kf->grid_h_inv;
+  memcpy(K.img, kf->img, sizeof(K.img));
+  P.m = m;
   memcpy(P.Tcw, Tcw, sizeof(P.Tcw)); memcpy(P.intr, intr, 32); memcpy(P.dist, dist, 32);
   P.xi = xi; P.cam = cam_model; P.dm = dist_model;
-  P.cand_idx = (int*)(d + o_ci); P.cand_dist = (int*)(d + o_cd); P.cand_n = (int*)(d + o_cn);
-  P.matched = d + o_ma; P.has_lm = d + o_hl; P.lm_cand = (int*)(d + o_lc); P.feat = (int*)(d + o_fe);
-  P.action = (int*)(d + o_ac); P.best_idx = (int*)(d + o_bi); P.n_matches = (int*)(d + o_nm); P.overflow = (int*)(d + o_nm) + 1;
-  memcpy(hpin, S.h.data(), in_bytes);
+  P.overflow = P.n_matches + 1;
   cudaStream_t st = ctx->stream;
-  CVB_CUDA(ctx, cudaMemcpyAsync(d, hpin, in_bytes, cudaMemcpyHostToDevice, st));
-  CVB_CUDA(ctx, cudaMemsetAsync(d + o_nm, 0, 8, st));
+  CVB_CUDA(ctx, cudaMemsetAsync(P.n_matches, 0, 8, st));
   search_proj_kernel<<<1, 256, 0, st>>>(K, P, prm->th, prm->desc_th_low, prm->scale_factor, prm->num_octaves);
   CVB_CHECK_LAUNCH(ctx);
-  CVB_CUDA(ctx, cudaMemcpyAsync(hpin + o_out, d + o_out, total - o_out, cudaMemcpyDeviceToHost, st));
-  CVB_CUDA(ctx, cudaStreamSynchronize(st));
-  const int* tail = (const int*)(hpin + o_nm);
+  if (const int rc = B.download()) return rc;
+  const int* tail = B.host(P.n_matches);
   if (tail[1]) return cvb_fail(ctx, CVB_ERR_UNSUPPORTED, "search_by_projection: more than %d keypoints in a search radius", kProjCap);
-  memcpy(action, hpin + o_ac, (size_t)m * 4); memcpy(best_idx, hpin + o_bi, (size_t)m * 4);
+  memcpy(action, B.host(P.action), (size_t)m * 4); memcpy(best_idx, B.host(P.best_idx), (size_t)m * 4);
   *n_matches = tail[0];
   return CVB_OK;
 }
@@ -508,7 +463,7 @@ int cvb_search_by_projection(cvb_ctx* ctx, const cvb_kf_view* kf, const int32_t*
 // The DenseMatcher scan and assignment (cvb_landmark_match_batch_dev), lmv_gather_kernel (matches -> RANSAC problems),
 // ransac_abs_kernel<SeededSamples<4>> (cvb_abs_ransac_seeded_dev), lmv_pose_kernel (gate, T12 / T21, already-masks),
 // search_se3_kernel, lmv_residual_kernel (LandmarkVector -> residual pairs) and relpose_kernel (cvb_relpose_batch_dev), all on
-// device buffers of one workspace.  The per-candidate arrays are sized by the host-known bound n_cand x n_query; the RANSAC
+// the arrays of one device block (cvb_block).  The per-candidate arrays are sized by the host-known bound n_cand x n_query; the RANSAC
 // problems are packed to the front in candidate order.  The DevPair and relpose records hold pointers that depend only on
 // sizes, so the host fills them; the device writes their T12 / T21 and n.
 namespace {
@@ -741,101 +696,76 @@ int verify_landmark(cvb_ctx* ctx, const cvb_landmark_kf* q, const cvb_landmark_k
     for (int a = 0; a < 3; a++)
       for (int b = 0; b < 3; b++) cam[12 * (size_t)c + 3 + 3 * a + b] = q->T_sc[4 * a + b];
   }
-  // device block: inputs (uploaded), scratch, outputs (downloaded)
-  Stager St;
-  size_t off1[9];
-  stage_kf(St, &q->view, off1);
-  std::vector<size_t> off2((size_t)C * 9);
-  for (int c = 0; c < C; c++) stage_kf(St, &cand[c].view, &off2[(size_t)c * 9], false);   // descriptors: the DenseMatcher's B below
-  const size_t o_bear = St.put(q->bearings, (size_t)nq * 24), o_sig = St.put(q->sigma_angle, (size_t)nq * 8);
-  std::vector<uint8_t> skipA(nq), skipB(NB);
+  std::vector<uint8_t> skipA(nq);
   for (int i = 0; i < nq; i++) skipA[i] = !q->view.lm_valid[i];
-  const size_t o_skA = St.put(skipA.data(), (size_t)nq), o_B = St.reserve(NB * 32), o_skB = St.reserve(NB);
+  // the device block; the DevPair records are completed here and by the device (T12 / T21), the relpose records by the device (n)
+  cvb_block B(ctx, ctx->stream);
+  DevKf d1{};
+  bind_kf(B, d1, &q->view);
+  std::vector<DevPair> hp((size_t)C);
+  for (int c = 0; c < C; c++) bind_kf(B, hp[c].k2, &cand[c].view, false);   // descriptors: the DenseMatcher's rows d_B below
+  LmvDev V{};
+  const uint8_t *d_skA, *d_B, *d_skB;
+  const uint64_t* d_seed;
+  const double* d_cam;
+  DevPair* d_pairs;
+  cvb_relpose_dev* d_recs;
+  int *d_oA, *d_oB, *d_mt1, *d_mt2, *d_ms, *d_nm, *d_bs, *d_bc, *d_it, *d_us, *d_nf;
+  float* d_oD;
+  double *d_bm, *d_ro;
+  uint8_t *d_mask, *d_a2, *d_rem;
+  B.in(V.q_bear, q->bearings, (size_t)nq * 3); B.in(V.q_sig, q->sigma_angle, nq);
+  B.in(d_skA, skipA.data(), nq); B.in(d_B, nullptr, NB * 32); B.in(d_skB, nullptr, NB);
+  B.in(V.seg, seg.data(), (size_t)C + 1); B.in(d_seed, seed, C); B.in(d_cam, cam.data(), cam.size()); B.in(V.TcwB, TcwB.data(), TcwB.size());
+  B.in(d_pairs, nullptr, C); B.in(d_recs, nullptr, C);
+  B.tmp(d_oA, NB); B.tmp(d_oB, NB); B.tmp(d_oD, NB); B.tmp(V.row, L); B.tmp(V.prob_ptr, (size_t)C + 1);
+  B.tmp(V.pts, L * 3); B.tmp(V.f, L * 3); B.tmp(V.sg, L); B.tmp(V.srcA, L); B.tmp(d_mask, L);
+  B.tmp(V.already1, L); B.tmp(d_a2, NB); B.tmp(d_mt1, L); B.tmp(d_mt2, NB); B.tmp(d_ms, L);
+  B.tmp(V.pA, L * 3); B.tmp(V.pB, L * 3); B.tmp(V.kA, L * 2); B.tmp(V.kB, L * 2); B.tmp(V.sA, L); B.tmp(V.sB, L);
+  B.tmp(V.pose_in, (size_t)C * 7);
+  B.out(d_nm, r->n_matches, C); B.out(d_bs, r->best_sample, C); B.out(d_bm, r->best_model, (size_t)C * 12); B.out(d_bc, r->best_count, C);
+  B.out(d_it, r->iterations, C); B.out(d_us, r->consumed, C); B.out(V.T12, r->T12, (size_t)C * 16); B.out(V.T21, r->T21, (size_t)C * 16);
+  B.out(d_nf, r->n_found, C); B.out(V.n_corr, r->n_corr, C); B.out_host(d_ro, (size_t)C * CVB_RELPOSE_OUT);
+  B.out(V.match12, r->match12, L); B.out(V.stage, r->stage, L); B.out_host(d_rem, L, r->removed != nullptr);   // the nullable outputs last
+  if (const int rc = B.place()) return rc;
+  uint8_t *hB = B.host(d_B), *hskB = B.host(d_skB);
+  cvb_relpose_dev* hr = B.host(d_recs);
   for (int c = 0; c < C; c++) {
     const size_t n = (size_t)cand[c].view.n;
-    if (n == 0) continue;
-    memcpy(St.h.data() + o_B + 32 * (size_t)seg[c], cand[c].view.desc, n * 32);
-    for (size_t b = 0; b < n; b++) St.h[o_skB + seg[c] + b] = !cand[c].view.lm_valid[b];
-  }
-  for (int c = 0; c < C; c++) off2[(size_t)c * 9 + 2] = o_B + 32 * (size_t)seg[c];   // the search reads its rows of B
-  const size_t o_seg = St.put(seg.data(), ((size_t)C + 1) * 4), o_seed = St.put(seed, (size_t)C * 8), o_cam = St.put(cam.data(), (size_t)C * 96);
-  const size_t o_TB = St.put(TcwB.data(), (size_t)C * 128);
-  const size_t o_pairs = St.reserve((size_t)C * sizeof(DevPair)), o_recs = St.reserve((size_t)C * sizeof(cvb_relpose_dev));
-  const size_t in_bytes = St.h.size();
-  size_t top = in_bytes;
-  const auto res = [&](size_t bytes) {
-    const size_t o = (top + 15) & ~size_t(15);
-    top = o + bytes;
-    return o;
-  };
-  const size_t o_oA = res(NB * 4), o_oB = res(NB * 4), o_oD = res(NB * 4), o_row = res(L * 4), o_pp = res(((size_t)C + 1) * 4);
-  const size_t o_pts = res(L * 24), o_f = res(L * 24), o_sg = res(L * 8), o_src = res(L * 4), o_mask = res(L);
-  const size_t o_a1 = res(L), o_a2 = res(NB), o_m1 = res(L * 4), o_m2 = res(NB * 4), o_ms = res(L * 4);
-  const size_t o_pA = res(L * 24), o_pB = res(L * 24), o_kA = res(L * 8), o_kB = res(L * 8), o_sA = res(L * 8), o_sB = res(L * 8);
-  const size_t o_pose = res((size_t)C * 56);
-  const size_t o_out = res(0);
-  const size_t o_nm = res((size_t)C * 4), o_bs = res((size_t)C * 4), o_bm = res((size_t)C * 96), o_bc = res((size_t)C * 4), o_it = res((size_t)C * 4),
-               o_us = res((size_t)C * 4), o_T12 = res((size_t)C * 128), o_T21 = res((size_t)C * 128), o_nf = res((size_t)C * 4),
-               o_nc = res((size_t)C * 4), o_ro = res((size_t)C * CVB_RELPOSE_OUT * 8);
-  const size_t o_m12 = res(L * 4), o_st = res(L), o_rem = res(L);
-  const size_t total = top;
-  const size_t out_end = r->removed ? total : r->stage ? o_rem : r->match12 ? o_st : o_m12;   // the nullable outputs only on request
-  unsigned char* d = (unsigned char*)cvb_ws(ctx, WS_GS0, total);
-  unsigned char* hpin = (unsigned char*)cvb_pinned(ctx, in_bytes + (out_end - o_out));
-  if (!d || !hpin) return CVB_ERR_CUDA;
-  // the records the device reads and completes
-  DevKf d1;
-  fill_dev(d1, &q->view, d, off1);
-  DevPair* hp = reinterpret_cast<DevPair*>(St.h.data() + o_pairs);
-  cvb_relpose_dev* hr = reinterpret_cast<cvb_relpose_dev*>(St.h.data() + o_recs);
-  for (int c = 0; c < C; c++) {
+    if (n) memcpy(hB + 32 * (size_t)seg[c], cand[c].view.desc, n * 32);
+    for (size_t b = 0; b < n; b++) hskB[seg[c] + b] = !cand[c].view.lm_valid[b];
     DevPair& P = hp[c];
-    memset(&P, 0, sizeof(P));
-    fill_dev(P.k2, &cand[c].view, d, &off2[(size_t)c * 9]);
-    P.already1 = d + o_a1 + (size_t)c * nq; P.already2 = d + o_a2 + seg[c];
-    P.match1 = (int*)(d + o_m1) + (size_t)c * nq; P.match2 = (int*)(d + o_m2) + seg[c];
-    P.match12 = (int*)(d + o_ms) + (size_t)c * nq; P.n_found = (int*)(d + o_nf) + c;
+    P.k2.desc = d_B + 32 * (size_t)seg[c];   // the search reads its rows of d_B
+    P.already1 = V.already1 + (size_t)c * nq; P.already2 = d_a2 + seg[c];
+    P.match1 = d_mt1 + (size_t)c * nq; P.match2 = d_mt2 + seg[c]; P.match12 = d_ms + (size_t)c * nq; P.n_found = d_nf + c;
     cvb_relpose_dev& R = hr[c];
     memset(&R, 0, sizeof(R));
     const size_t b = (size_t)c * nq;
-    R.pA = (const double*)(d + o_pA) + 3 * b; R.pB = (const double*)(d + o_pB) + 3 * b; R.kpA = (const float*)(d + o_kA) + 2 * b;
-    R.kpB = (const float*)(d + o_kB) + 2 * b; R.sA = (const double*)(d + o_sA) + b; R.sB = (const double*)(d + o_sB) + b;
+    R.pA = V.pA + 3 * b; R.pB = V.pB + 3 * b; R.kpA = V.kA + 2 * b; R.kpB = V.kB + 2 * b; R.sA = V.sA + b; R.sB = V.sB + b;
     R.camA = relcam(q); R.camB = relcam(cand + c);
-    R.pose_in = (const double*)(d + o_pose) + 7 * (size_t)c; R.removed = d + o_rem + b; R.out = (double*)(d + o_ro) + CVB_RELPOSE_OUT * (size_t)c;
+    R.pose_in = V.pose_in + 7 * (size_t)c; R.removed = d_rem + b; R.out = d_ro + CVB_RELPOSE_OUT * (size_t)c;
   }
-  memcpy(hpin, St.h.data(), in_bytes);
-  unsigned char* hout = hpin + in_bytes;
+  memcpy(B.host(d_pairs), hp.data(), hp.size() * sizeof(DevPair));
+  if (const int rc = B.upload()) return rc;
   cudaStream_t st = ctx->stream;
-  CVB_CUDA(ctx, cudaMemcpyAsync(d, hpin, in_bytes, cudaMemcpyHostToDevice, st));
-  LmvDev V{};
   V.nq = nq; V.min_matches = prm->min_matches; V.min_inliers = prm->min_ransac_inliers;
-  V.seg = (const int*)(d + o_seg); V.outA = (const int*)(d + o_oA); V.outB = (const int*)(d + o_oB); V.n_out = (const int*)(d + o_nm);
-  V.q_bear = (const double*)(d + o_bear); V.q_sig = (const double*)(d + o_sig);
+  V.outA = d_oA; V.outB = d_oB; V.n_out = d_nm;
   V.q_valid = d1.lm_valid; V.q_pos = d1.lm_pos; V.q_kp = d1.kp; V.q_oct = d1.octave;
   memcpy(V.q_Tsc, q->T_sc, sizeof(V.q_Tsc)); memcpy(V.TcwA, TcwA, sizeof(V.TcwA));
-  V.TcwB = (const double*)(d + o_TB); V.row = (int*)(d + o_row);
-  V.prob_ptr = (int*)(d + o_pp); V.pts = (double*)(d + o_pts); V.f = (double*)(d + o_f); V.sg = (double*)(d + o_sg); V.srcA = (int*)(d + o_src);
-  V.best_sample = (const int*)(d + o_bs); V.best_model = (const double*)(d + o_bm); V.best_count = (const int*)(d + o_bc); V.mask = d + o_mask;
-  V.already1 = d + o_a1; V.stage = d + o_st; V.match12 = (int*)(d + o_m12);
-  V.T12 = (double*)(d + o_T12); V.T21 = (double*)(d + o_T21); V.pose_in = (double*)(d + o_pose);
-  V.pA = (double*)(d + o_pA); V.pB = (double*)(d + o_pB); V.kA = (float*)(d + o_kA); V.kB = (float*)(d + o_kB);
-  V.sA = (double*)(d + o_sA); V.sB = (double*)(d + o_sB); V.n_corr = (int*)(d + o_nc);
-  DevPair* d_pairs = reinterpret_cast<DevPair*>(d + o_pairs);
-  cvb_relpose_dev* d_recs = reinterpret_cast<cvb_relpose_dev*>(d + o_recs);
+  V.best_sample = d_bs; V.best_model = d_bm; V.best_count = d_bc; V.mask = d_mask;
   // 1. DenseMatcher
   if (NB > 0) {
-    if (const int rc = cvb_landmark_match_batch_dev(ctx, d + off1[2], d + o_skA, nq, d + o_B, d + o_skB, V.seg, seg.data(), C, prm->thr, prm->num_best,
-                                                    (int*)(d + o_oA), (int*)(d + o_oB), (float*)(d + o_oD), (int*)(d + o_nm), nullptr))
+    if (const int rc = cvb_landmark_match_batch_dev(ctx, d1.desc, d_skA, nq, d_B, d_skB, V.seg, seg.data(), C, prm->thr, prm->num_best, d_oA, d_oB,
+                                                    d_oD, d_nm, nullptr))
       return rc;
   } else {
-    CVB_CUDA(ctx, cudaMemsetAsync(d + o_nm, 0, (size_t)C * 4, st));
+    CVB_CUDA(ctx, cudaMemsetAsync(d_nm, 0, (size_t)C * 4, st));
   }
   // 2. the RANSAC problems and their RANSACs
   lmv_gather_kernel<<<C, kGlueThreads, 0, st>>>(V, d_pairs);
   CVB_CHECK_LAUNCH(ctx);
-  if (const int rc = cvb_abs_ransac_seeded_dev(ctx, C, V.prob_ptr, V.pts, V.f, V.sg, (const double*)(d + o_cam), (const uint64_t*)(d + o_seed),
-                                               prm->threshold, prm->max_iterations, prm->probability, (int*)(d + o_bs), (double*)(d + o_bm),
-                                               (int*)(d + o_bc), (int*)(d + o_it), (int*)(d + o_us), d + o_mask))
+  if (const int rc = cvb_abs_ransac_seeded_dev(ctx, C, V.prob_ptr, V.pts, V.f, V.sg, d_cam, d_seed, prm->threshold, prm->max_iterations,
+                                               prm->probability, d_bs, d_bm, d_bc, d_it, d_us, d_mask))
     return rc;
   // 3. gate, T12 / T21, already-masks
   lmv_pose_kernel<<<C, kGlueThreads, 0, st>>>(V, d_pairs);
@@ -847,25 +777,17 @@ int verify_landmark(cvb_ctx* ctx, const cvb_landmark_kf* q, const cvb_landmark_k
   lmv_residual_kernel<<<C, kGlueThreads, 0, st>>>(V, d_pairs, d_recs);
   CVB_CHECK_LAUNCH(ctx);
   if (const int rc = cvb_relpose_batch_dev(ctx, d_recs, C, prm->th_outlier_align)) return rc;
-  CVB_CUDA(ctx, cudaMemcpyAsync(hout, d + o_out, out_end - o_out, cudaMemcpyDeviceToHost, st));
-  CVB_CUDA(ctx, cudaStreamSynchronize(st));
-  const auto at = [&](size_t off) { return hout + (off - o_out); };
-  memcpy(r->n_matches, at(o_nm), (size_t)C * 4); memcpy(r->best_sample, at(o_bs), (size_t)C * 4); memcpy(r->best_model, at(o_bm), (size_t)C * 96);
-  memcpy(r->best_count, at(o_bc), (size_t)C * 4); memcpy(r->iterations, at(o_it), (size_t)C * 4); memcpy(r->consumed, at(o_us), (size_t)C * 4);
-  memcpy(r->T12, at(o_T12), (size_t)C * 128); memcpy(r->T21, at(o_T21), (size_t)C * 128); memcpy(r->n_found, at(o_nf), (size_t)C * 4);
-  memcpy(r->n_corr, at(o_nc), (size_t)C * 4);
-  const double* ro = (const double*)at(o_ro);
+  if (const int rc = B.download()) return rc;
+  const double* ro = B.host(d_ro);
   for (int c = 0; c < C; c++) {
     const double* o = ro + CVB_RELPOSE_OUT * (size_t)c;
     for (int k = 0; k < 7; k++) r->T12_out[7 * (size_t)c + k] = o[k];
     r->n_inliers[c] = (int32_t)o[7];
     r->solve_iterations[2 * (size_t)c] = (int32_t)o[8]; r->solve_iterations[2 * (size_t)c + 1] = (int32_t)o[9];
   }
-  if (r->match12) memcpy(r->match12, at(o_m12), L * 4);
-  if (r->stage) memcpy(r->stage, at(o_st), L);
   if (r->removed) {   // defined for r < n_corr; the rest of a candidate's row is 0
     memset(r->removed, 0, L);
-    for (int c = 0; c < C; c++) memcpy(r->removed + (size_t)c * nq, at(o_rem) + (size_t)c * nq, (size_t)r->n_corr[c]);
+    for (int c = 0; c < C; c++) memcpy(r->removed + (size_t)c * nq, B.host(d_rem) + (size_t)c * nq, (size_t)r->n_corr[c]);
   }
   return CVB_OK;
 }

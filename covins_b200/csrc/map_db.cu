@@ -12,6 +12,11 @@
 #include "cvb_internal.cuh"
 #include "tc_match.cuh"
 
+struct cvb_buf {
+  void* p = nullptr;
+  size_t cap = 0;
+};
+
 struct cvb_db {
   int desc_bytes = 32;
   uint8_t* d_rows = nullptr;
@@ -237,8 +242,10 @@ int cvb_db_remove(cvb_ctx* ctx, cvb_db* db, int kf_index) {
   const int64_t a = db->seg_ptr[kf_index], b = db->seg_ptr[kf_index + 1], end = db->seg_ptr.back();
   const size_t tail = (size_t)(end - b) * db->desc_bytes, len = (size_t)(b - a);
   if (tail && len) {   // move the tail down through a scratch buffer (source and destination overlap)
-    void* tmp = cvb_ws(ctx, WS_GS2, tail);
-    if (!tmp) return CVB_ERR_CUDA;
+    cvb_block B(ctx, ctx->stream);
+    uint8_t* tmp;
+    B.tmp(tmp, tail);
+    if (const int rc = B.place()) return rc;
     CVB_CUDA(ctx, cudaMemcpyAsync(tmp, db->d_rows + (size_t)b * db->desc_bytes, tail, cudaMemcpyDeviceToDevice, ctx->stream));
     CVB_CUDA(ctx, cudaMemcpyAsync(db->d_rows + (size_t)a * db->desc_bytes, tmp, tail, cudaMemcpyDeviceToDevice, ctx->stream));
     CVB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
@@ -248,8 +255,10 @@ int cvb_db_remove(cvb_ctx* ctx, cvb_db* db, int kf_index) {
     const int ta = db->seg_tile[kf_index], tbn = db->seg_tile[kf_index + 1], tend = db->seg_tile.back();
     const size_t ttail = (size_t)(tend - tbn) * tb;
     if (ttail && tbn > ta) {
-      void* tmp = cvb_ws(ctx, WS_GS2, ttail);
-      if (!tmp) return CVB_ERR_CUDA;
+      cvb_block B(ctx, ctx->stream);
+      uint8_t* tmp;
+      B.tmp(tmp, ttail);
+      if (const int rc = B.place()) return rc;
       CVB_CUDA(ctx, cudaMemcpyAsync(tmp, db->d_xt + (size_t)tbn * tb, ttail, cudaMemcpyDeviceToDevice, ctx->stream));
       CVB_CUDA(ctx, cudaMemcpyAsync(db->d_xt + (size_t)ta * tb, tmp, ttail, cudaMemcpyDeviceToDevice, ctx->stream));
       CVB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));

@@ -141,18 +141,6 @@ int mg_bits(int64_t v) {   // bits that hold 0..v
   return b;
 }
 
-// carves one workspace slot into 256-byte aligned arrays: first pass sizes, second pass hands out pointers
-struct mg_carver {
-  char* base = nullptr;
-  size_t off = 0;
-  template <class T>
-  T* take(size_t n) {
-    T* p = base ? reinterpret_cast<T*>(base + off) : nullptr;
-    off += (n * sizeof(T) + 255) & ~size_t(255);
-    return p;
-  }
-};
-
 #define MG_CUB(ctx, call)                                                                                                         \
   do {                                                                                                                            \
     cudaError_t e_ = (call);                                                                                                      \
@@ -236,31 +224,18 @@ int cvb_covisibility_budgeted(cvb_ctx* ctx, int K, int L, const int32_t* lm_obs_
                                                  (int32_t*)nullptr, ::cuda::std::plus<int32_t>(), (int)acc_cap, st));
     temp_bytes = std::max(temp_bytes, tb);
   }
-  mg_carver c1;
-  int32_t *d_ptr = nullptr, *d_kf = nullptr, *d_num = nullptr, *acc_w = nullptr, *acc_w2 = nullptr;
-  int64_t* d_poff = nullptr;
-  uint64_t *keys_a = nullptr, *keys_b = nullptr, *acc_k = nullptr, *acc_k2 = nullptr;
-  void* d_temp = nullptr;
-  for (int pass = 0; pass < 2; pass++) {
-    c1.off = 0;
-    d_ptr = c1.take<int32_t>((size_t)n_lm + 1);
-    d_kf = c1.take<int32_t>(c_kf.size());
-    d_poff = c1.take<int64_t>((size_t)n_lm + 1);
-    keys_a = c1.take<uint64_t>((size_t)chunk);
-    keys_b = c1.take<uint64_t>((size_t)chunk);
-    acc_k = c1.take<uint64_t>((size_t)acc_cap);
-    acc_w = c1.take<int32_t>((size_t)acc_cap);
-    if (n_chunks > 1) {
-      acc_k2 = c1.take<uint64_t>((size_t)acc_cap);
-      acc_w2 = c1.take<int32_t>((size_t)acc_cap);
-    }
-    d_num = c1.take<int32_t>(1);
-    d_temp = c1.take<char>(temp_bytes);
-    if (pass == 0 && !(c1.base = (char*)cvb_ws(ctx, WS_MG_EDGES, c1.off))) return CVB_ERR_CUDA;
-  }
-  CVB_CUDA(ctx, cudaMemcpyAsync(d_ptr, c_ptr.data(), c_ptr.size() * sizeof(int32_t), cudaMemcpyHostToDevice, st));
-  CVB_CUDA(ctx, cudaMemcpyAsync(d_kf, c_kf.data(), c_kf.size() * sizeof(int32_t), cudaMemcpyHostToDevice, st));
-  CVB_CUDA(ctx, cudaMemcpyAsync(d_poff, c_poff.data(), c_poff.size() * sizeof(int64_t), cudaMemcpyHostToDevice, st));
+  cvb_block B1(ctx, st, false);   // direct: the observation lists are large
+  const int32_t *d_ptr, *d_kf;
+  const int64_t* d_poff;
+  int32_t *d_num, *acc_w, *acc_w2 = nullptr;
+  uint64_t *keys_a, *keys_b, *acc_k, *acc_k2 = nullptr;
+  char* d_temp;
+  B1.in(d_ptr, c_ptr.data(), c_ptr.size()); B1.in(d_kf, c_kf.data(), c_kf.size()); B1.in(d_poff, c_poff.data(), c_poff.size());
+  B1.tmp(keys_a, chunk); B1.tmp(keys_b, chunk); B1.tmp(acc_k, acc_cap); B1.tmp(acc_w, acc_cap);
+  if (n_chunks > 1) { B1.tmp(acc_k2, acc_cap); B1.tmp(acc_w2, acc_cap); }
+  B1.tmp(d_num, 1); B1.tmp(d_temp, temp_bytes);
+  if (const int rc = B1.place()) return rc;
+  if (const int rc = B1.upload()) return rc;
   int64_t n_edge = 0;
   for (int64_t c = 0; c < n_chunks; c++) {
     const int64_t p0 = c * chunk, cnt = std::min(chunk, n_pairs - p0);
@@ -293,26 +268,18 @@ int cvb_covisibility_budgeted(cvb_ctx* ctx, int K, int L, const int32_t* lm_obs_
   temp2 = std::max(temp2, tb);
   CVB_CUDA(ctx, cub::DeviceScan::ExclusiveSum(nullptr, tb, (const int32_t*)nullptr, (int32_t*)nullptr, K + 1, st));
   temp2 = std::max(temp2, tb);
-  mg_carver c2;
-  int32_t *strong = nullptr, *deg = nullptr, *d_nbr_ptr = nullptr, *d_nbr_kf = nullptr, *d_nbr_w = nullptr;
-  unsigned long long* best = nullptr;
-  uint64_t *row_a = nullptr, *row_b = nullptr;
-  size_t zero_bytes = 0;
-  for (int pass = 0; pass < 2; pass++) {
-    c2.off = 0;
-    strong = c2.take<int32_t>((size_t)K);
-    deg = c2.take<int32_t>((size_t)K + 1);   // [K] stays 0: the scan of K + 1 items puts the total at nbr_ptr[K]
-    best = c2.take<unsigned long long>((size_t)K);
-    zero_bytes = c2.off;
-    d_nbr_ptr = c2.take<int32_t>((size_t)K + 1);
-    row_a = c2.take<uint64_t>((size_t)n_dir);
-    row_b = c2.take<uint64_t>((size_t)n_dir);
-    d_nbr_kf = c2.take<int32_t>((size_t)n_dir);
-    d_nbr_w = c2.take<int32_t>((size_t)n_dir);
-    d_temp = c2.take<char>(temp2);
-    if (pass == 0 && !(c2.base = (char*)cvb_ws(ctx, WS_MG_ROWS, c2.off))) return CVB_ERR_CUDA;
-  }
-  CVB_CUDA(ctx, cudaMemsetAsync(strong, 0, zero_bytes, st));
+  cvb_block B2(ctx, st);
+  int32_t *strong, *deg, *d_nbr_ptr, *d_nbr_kf, *d_nbr_w;
+  unsigned long long* best;
+  uint64_t *row_a, *row_b;
+  B2.tmp(strong, K);
+  B2.tmp(deg, (size_t)K + 1);   // [K] stays 0: the scan of K + 1 items puts the total at nbr_ptr[K]
+  B2.tmp(best, K);
+  B2.tmp(d_nbr_ptr, (size_t)K + 1); B2.tmp(row_a, n_dir); B2.tmp(row_b, n_dir); B2.tmp(d_nbr_kf, n_dir); B2.tmp(d_nbr_w, n_dir);
+  B2.tmp(d_temp, temp2);
+  if (const int rc = B2.place()) return rc;
+  // strong, deg and best are adjacent: one memset zeroes the three
+  CVB_CUDA(ctx, cudaMemsetAsync(strong, 0, (size_t)((char*)d_nbr_ptr - (char*)strong), st));
   const unsigned edge_grid = (unsigned)((n_edge + MG_THREADS - 1) / MG_THREADS);
   mg_row_stats_kernel<<<edge_grid, MG_THREADS, 0, st>>>(acc_k, acc_w, (int)n_edge, bits_k, min_weight, strong, best);
   CVB_CHECK_LAUNCH(ctx);
@@ -508,35 +475,19 @@ extern "C" int cvb_redundant_keyframes(cvb_ctx* ctx, int K, int L, const int32_t
 
   cudaStream_t st = ctx->stream;
   const size_t n_bins = (size_t)L * num_octaves;
-  mg_carver cv;
-  int32_t *d_kf_ptr = nullptr, *d_kf_h = nullptr, *hist = nullptr, *pred_c = nullptr, *d_succ = nullptr, *mark = nullptr, *und_a = nullptr,
-          *und_b = nullptr, *d_cnt = nullptr;
-  double* d_time = nullptr;
-  uint8_t* d_state = nullptr;
-  unsigned long long* lowt = nullptr;
-  for (int pass = 0; pass < 2; pass++) {
-    cv.off = 0;
-    d_kf_ptr = cv.take<int32_t>((size_t)K + 1);
-    d_kf_h = cv.take<int32_t>((size_t)n_part);
-    pred_c = cv.take<int32_t>((size_t)K);
-    d_succ = cv.take<int32_t>((size_t)K);
-    d_time = cv.take<double>((size_t)K);
-    d_state = cv.take<uint8_t>((size_t)K);
-    und_a = cv.take<int32_t>((size_t)n0);
-    und_b = cv.take<int32_t>((size_t)n0);
-    hist = cv.take<int32_t>(n_bins);
-    d_cnt = cv.take<int32_t>((size_t)n0 + 1);   // round r counts its survivors in d_cnt[r]: no reset between rounds
-    mark = cv.take<int32_t>((size_t)K);
-    lowt = cv.take<unsigned long long>((size_t)L);
-    if (pass == 0 && !(cv.base = (char*)cvb_ws(ctx, WS_MG_PRUNE, cv.off))) return CVB_ERR_CUDA;
-  }
-  CVB_CUDA(ctx, cudaMemcpyAsync(d_kf_ptr, kf_ptr.data(), kf_ptr.size() * sizeof(int32_t), cudaMemcpyHostToDevice, st));
-  CVB_CUDA(ctx, cudaMemcpyAsync(d_kf_h, kf_h.data(), kf_h.size() * sizeof(int32_t), cudaMemcpyHostToDevice, st));
-  CVB_CUDA(ctx, cudaMemcpyAsync(pred_c, kf_pred, (size_t)K * sizeof(int32_t), cudaMemcpyHostToDevice, st));
-  CVB_CUDA(ctx, cudaMemcpyAsync(d_succ, succ.data(), (size_t)K * sizeof(int32_t), cudaMemcpyHostToDevice, st));
-  CVB_CUDA(ctx, cudaMemcpyAsync(d_time, kf_time, (size_t)K * sizeof(double), cudaMemcpyHostToDevice, st));
-  CVB_CUDA(ctx, cudaMemcpyAsync(d_state, state.data(), (size_t)K, cudaMemcpyHostToDevice, st));
-  CVB_CUDA(ctx, cudaMemcpyAsync(und_a, und.data(), (size_t)n0 * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+  cvb_block B(ctx, st, false);   // direct: the observation lists are large
+  const int32_t *d_kf_ptr, *d_kf_h, *d_succ;
+  const double* d_time;
+  int32_t *hist, *pred_c, *mark, *und_a, *und_b, *d_cnt;
+  uint8_t* d_state;
+  unsigned long long* lowt;
+  B.in(d_kf_ptr, kf_ptr.data(), kf_ptr.size()); B.in(d_kf_h, kf_h.data(), kf_h.size()); B.in(pred_c, kf_pred, K); B.in(d_succ, succ.data(), K);
+  B.in(d_time, kf_time, K); B.in(d_state, state.data(), K); B.in(und_a, und.data(), n0);
+  B.tmp(und_b, n0); B.tmp(hist, n_bins);
+  B.tmp(d_cnt, (size_t)n0 + 1);   // round r counts its survivors in d_cnt[r]: no reset between rounds
+  B.tmp(mark, K); B.tmp(lowt, L);
+  if (const int rc = B.place()) return rc;
+  if (const int rc = B.upload()) return rc;
   // hist and d_cnt are adjacent: one memset zeroes both; mark = -1 and lowt = all ones match no round
   CVB_CUDA(ctx, cudaMemsetAsync(hist, 0, (size_t)((char*)mark - (char*)hist), st));
   CVB_CUDA(ctx, cudaMemsetAsync(mark, 0xff, (size_t)((char*)(lowt + L) - (char*)mark), st));

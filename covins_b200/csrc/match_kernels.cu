@@ -731,13 +731,11 @@ int knn_dev(cvb_ctx* ctx, const uint8_t* d_q, int nq, const uint8_t* d_t, const 
       std::vector<int32_t> h_ps((size_t)n_ps + 1), h_off((size_t)n_ps);
       for (int c = 0; c <= n_ps; c++) h_ps[c] = (int32_t)std::min<int64_t>((int64_t)c * chunk, total);
       for (int c = 0; c < n_ps; c++) h_off[c] = (int32_t)((int64_t)c * chunk);
-      // own slots: WS_TMP0/WS_TMP1 hold the quantised descriptors of the host L2 path (l2_host) at this point
-      int32_t* d_ps = (int32_t*)cvb_ws(ctx, WS_CHUNK_PS, sizeof(int32_t) * (n_ps + 1));
-      int32_t* d_off = (int32_t*)cvb_ws(ctx, WS_CHUNK_OFF, sizeof(int32_t) * n_ps);
       const size_t pn = (size_t)n_ps * nq * k;
-      int32_t* part_i = (int32_t*)cvb_ws(ctx, WS_PART_I, pn * sizeof(int32_t));
-      int32_t* part_d = (int32_t*)cvb_ws(ctx, WS_PART_D, pn * sizeof(int32_t));
-      if (!d_ps || !d_off || !part_i || !part_d) return CVB_ERR_CUDA;
+      cvb_block B(ctx, st);
+      int32_t *d_ps, *d_off, *part_i, *part_d;
+      B.tmp(d_ps, (size_t)n_ps + 1); B.tmp(d_off, n_ps); B.tmp(part_i, pn); B.tmp(part_d, pn);
+      if ((rc = B.place())) return rc;
       CVB_CUDA(ctx, cudaMemcpyAsync(d_ps, h_ps.data(), sizeof(int32_t) * (n_ps + 1), cudaMemcpyHostToDevice, st));
       CVB_CUDA(ctx, cudaMemcpyAsync(d_off, h_off.data(), sizeof(int32_t) * n_ps, cudaMemcpyHostToDevice, st));
       CVB_CUDA(ctx, cudaStreamSynchronize(st));   // the host vectors go out of scope
@@ -768,9 +766,10 @@ int knn_dev(cvb_ctx* ctx, const uint8_t* d_q, int nq, const uint8_t* d_t, const 
     return dispatch_scan<M, QPT_BIG, MODE_BF>(ctx, sp, pl, k, st);
   }
   const size_t pn = (size_t)n_seg * pl.splits * nq * k;
-  int32_t* part_i = (int32_t*)cvb_ws(ctx, WS_PART_I, pn * sizeof(int32_t));
-  int32_t* part_d = (int32_t*)cvb_ws(ctx, WS_PART_D, pn * sizeof(int32_t));
-  if (!part_i || !part_d) return CVB_ERR_CUDA;
+  cvb_block B(ctx, st);
+  int32_t *part_i, *part_d;
+  B.tmp(part_i, pn); B.tmp(part_d, pn);
+  if ((rc = B.place())) return rc;
   sp.out_idx = part_i; sp.out_dist = part_d;
   rc = dispatch_scan<M, QPT_BIG, MODE_BF>(ctx, sp, pl, k, st);
   if (rc) return rc;
@@ -792,19 +791,6 @@ int host_rows(cvb_ctx* ctx, const int32_t* seg_ptr, int n_seg, size_t* rows) {
   return CVB_OK;
 }
 
-// Host-buffer staging helper: copies q, t, seg_ptr to device workspaces.
-int stage_inputs(cvb_ctx* ctx, const void* q, size_t qbytes, const void* t, size_t tbytes, const int32_t* seg_ptr,
-                 int n_seg, void** d_q, void** d_t, int32_t** d_seg) {
-  *d_q = cvb_ws(ctx, WS_Q, qbytes);
-  *d_t = cvb_ws(ctx, WS_T, tbytes);
-  *d_seg = (int32_t*)cvb_ws(ctx, WS_SEG, sizeof(int32_t) * (n_seg + 1));
-  if (!*d_q || !*d_t || !*d_seg) return CVB_ERR_CUDA;
-  if (qbytes) CVB_CUDA(ctx, cudaMemcpyAsync(*d_q, q, qbytes, cudaMemcpyHostToDevice, ctx->stream));
-  if (tbytes) CVB_CUDA(ctx, cudaMemcpyAsync(*d_t, t, tbytes, cudaMemcpyHostToDevice, ctx->stream));
-  CVB_CUDA(ctx, cudaMemcpyAsync(*d_seg, seg_ptr, sizeof(int32_t) * (n_seg + 1), cudaMemcpyHostToDevice,
-                                ctx->stream));
-  return CVB_OK;
-}
 
 }  // namespace
 
@@ -972,23 +958,17 @@ int cvb_knn_hamming_batch(cvb_ctx* ctx, const uint8_t* q, int nq, const uint8_t*
   size_t rows = 0;
   int rc = host_rows(ctx, seg_ptr, n_seg, &rows);
   if (rc) return rc;
-  void *d_q, *d_t;
-  int32_t* d_seg;
-  rc = stage_inputs(ctx, q, (size_t)nq * 32, t, rows * 32, seg_ptr, n_seg, &d_q, &d_t, &d_seg);
-  if (rc) return rc;
   const size_t on = (size_t)n_seg * nq * k;
-  int32_t* d_idx = (int32_t*)cvb_ws(ctx, WS_OUT0, on * 4);
-  int32_t* d_dist = (int32_t*)cvb_ws(ctx, WS_OUT1, on * 4);
-  if (!d_idx || !d_dist) return CVB_ERR_CUDA;
-  rc = cvb_knn_hamming_batch_dev(ctx, (const uint8_t*)d_q, nq, (const uint8_t*)d_t, d_seg, seg_ptr, n_seg, k, d_idx,
-                                 d_dist, nullptr);
+  cvb_block B(ctx, ctx->stream, false);   // direct: the descriptor rows are large
+  const uint8_t *d_q, *d_t;
+  const int32_t* d_seg;
+  int32_t *d_idx, *d_dist;
+  B.in(d_q, q, (size_t)nq * 32); B.in(d_t, t, rows * 32); B.in(d_seg, seg_ptr, (size_t)n_seg + 1);
+  B.out(d_idx, idx, on); B.out(d_dist, dist, on);
+  if ((rc = B.place()) || (rc = B.upload())) return rc;
+  rc = cvb_knn_hamming_batch_dev(ctx, d_q, nq, d_t, d_seg, seg_ptr, n_seg, k, d_idx, d_dist, nullptr);
   if (rc) return rc;
-  if (on) {
-    CVB_CUDA(ctx, cudaMemcpyAsync(idx, d_idx, on * 4, cudaMemcpyDeviceToHost, ctx->stream));
-    CVB_CUDA(ctx, cudaMemcpyAsync(dist, d_dist, on * 4, cudaMemcpyDeviceToHost, ctx->stream));
-  }
-  CVB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-  return CVB_OK;
+  return B.download();
 }
 
 int cvb_match_hamming_batch(cvb_ctx* ctx, const uint8_t* q, int nq, const uint8_t* t, const int32_t* seg_ptr,
@@ -1000,25 +980,18 @@ int cvb_match_hamming_batch(cvb_ctx* ctx, const uint8_t* q, int nq, const uint8_
   size_t rows = 0;
   int rc = host_rows(ctx, seg_ptr, n_seg, &rows);
   if (rc) return rc;
-  void *d_q, *d_t;
-  int32_t* d_seg;
-  rc = stage_inputs(ctx, q, (size_t)nq * 32, t, rows * 32, seg_ptr, n_seg, &d_q, &d_t, &d_seg);
-  if (rc) return rc;
   const size_t on = (size_t)n_seg * nq;
-  int32_t* d_mt = (int32_t*)cvb_ws(ctx, WS_OUT0, on * 4);
-  float* d_md = (float*)cvb_ws(ctx, WS_OUT1, on * 4);
-  int32_t* d_nm = (int32_t*)cvb_ws(ctx, WS_OUT2, (size_t)n_seg * 4);
-  if (!d_mt || !d_md || !d_nm) return CVB_ERR_CUDA;
-  rc = cvb_match_hamming_batch_dev(ctx, (const uint8_t*)d_q, nq, (const uint8_t*)d_t, d_seg, seg_ptr, n_seg, thr,
-                                   ratio, d_mt, d_md, d_nm, nullptr);
+  cvb_block B(ctx, ctx->stream, false);   // direct: the descriptor rows are large
+  const uint8_t *d_q, *d_t;
+  const int32_t* d_seg;
+  int32_t *d_mt, *d_nm;
+  float* d_md;
+  B.in(d_q, q, (size_t)nq * 32); B.in(d_t, t, rows * 32); B.in(d_seg, seg_ptr, (size_t)n_seg + 1);
+  B.out(d_mt, match_train, on); B.out(d_md, match_dist, on); B.out(d_nm, n_matches, n_seg);
+  if ((rc = B.place()) || (rc = B.upload())) return rc;
+  rc = cvb_match_hamming_batch_dev(ctx, d_q, nq, d_t, d_seg, seg_ptr, n_seg, thr, ratio, d_mt, d_md, d_nm, nullptr);
   if (rc) return rc;
-  if (on) {
-    CVB_CUDA(ctx, cudaMemcpyAsync(match_train, d_mt, on * 4, cudaMemcpyDeviceToHost, ctx->stream));
-    CVB_CUDA(ctx, cudaMemcpyAsync(match_dist, d_md, on * 4, cudaMemcpyDeviceToHost, ctx->stream));
-  }
-  CVB_CUDA(ctx, cudaMemcpyAsync(n_matches, d_nm, (size_t)n_seg * 4, cudaMemcpyDeviceToHost, ctx->stream));
-  CVB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-  return CVB_OK;
+  return B.download();
 }
 
 int cvb_knn_merge_shards_dev(cvb_ctx* ctx, const int32_t* d_idx_all, const void* d_dist_all, int dist_is_float,
@@ -1067,21 +1040,19 @@ int cvb_landmark_descriptor_batch(cvb_ctx* ctx, const uint8_t* cand, const int32
   if (n_lm == 0) return CVB_OK;
   const size_t rows = (size_t)lm_ptr[n_lm];
   CVB_REQUIRE(ctx, lm_ptr[0] == 0 && (rows == 0 || cand), "landmark_descriptor: bad lm_ptr / null candidates");
-  uint8_t* d_c = (uint8_t*)cvb_ws(ctx, WS_T, rows * 32);
-  int32_t* d_p = (int32_t*)cvb_ws(ctx, WS_SEG, sizeof(int32_t) * ((size_t)n_lm + 1));
-  int32_t* d_b = (int32_t*)cvb_ws(ctx, WS_OUT0, sizeof(int32_t) * (size_t)n_lm);
-  uint8_t* d_o = (uint8_t*)cvb_ws(ctx, WS_OUT1, (size_t)n_lm * 32);
-  if (!d_c || !d_p || !d_b || !d_o) return CVB_ERR_CUDA;
-  if (rows) CVB_CUDA(ctx, cudaMemcpyAsync(d_c, cand, rows * 32, cudaMemcpyHostToDevice, ctx->stream));
-  CVB_CUDA(ctx, cudaMemcpyAsync(d_p, lm_ptr, sizeof(int32_t) * ((size_t)n_lm + 1), cudaMemcpyHostToDevice, ctx->stream));
+  cvb_block B(ctx, ctx->stream, false);   // direct: the descriptor rows are large
+  const uint8_t* d_c;
+  const int32_t* d_p;
+  uint8_t* d_o;
+  int32_t* d_b;
   // landmarks without candidates keep their descriptor (the reference returns early): pass the caller's bytes through
-  CVB_CUDA(ctx, cudaMemcpyAsync(d_o, out_desc, (size_t)n_lm * 32, cudaMemcpyHostToDevice, ctx->stream));
-  int rc = cvb_landmark_descriptor_batch_dev(ctx, d_c, d_p, n_lm, d_b, d_o, nullptr);
-  if (rc) return rc;
-  CVB_CUDA(ctx, cudaMemcpyAsync(best_idx, d_b, sizeof(int32_t) * (size_t)n_lm, cudaMemcpyDeviceToHost, ctx->stream));
+  B.in(d_c, cand, rows * 32); B.in(d_p, lm_ptr, (size_t)n_lm + 1); B.in(d_o, out_desc, (size_t)n_lm * 32);
+  B.out(d_b, best_idx, n_lm);
+  int rc;
+  if ((rc = B.place()) || (rc = B.upload())) return rc;
+  if ((rc = cvb_landmark_descriptor_batch_dev(ctx, d_c, d_p, n_lm, d_b, d_o, nullptr))) return rc;
   CVB_CUDA(ctx, cudaMemcpyAsync(out_desc, d_o, (size_t)n_lm * 32, cudaMemcpyDeviceToHost, ctx->stream));
-  CVB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-  return CVB_OK;
+  return B.download();
 }
 
 int cvb_quantize_u8_dev(cvb_ctx* ctx, const float* d_src, int64_t n, uint8_t* d_dst, int32_t* d_bad, void* stream) {
@@ -1118,17 +1089,20 @@ static int l2_host(cvb_ctx* ctx, const float* q, int nq, const float* t, const i
   size_t rows = 0;
   int rc = host_rows(ctx, seg_ptr, n_seg, &rows);
   if (rc) return rc;
-  void *d_qf, *d_tf;
-  int32_t* d_seg;
-  rc = stage_inputs(ctx, q, (size_t)nq * dim * 4, t, rows * dim * 4, seg_ptr, n_seg, &d_qf, &d_tf, &d_seg);
+  const size_t on = (size_t)n_seg * nq * (filter ? 1 : k);
+  cvb_block B(ctx, ctx->stream, false);   // direct: the descriptor rows are large
+  const float *d_qf, *d_tf;
+  const int32_t* d_seg;
+  uint8_t *d_q8, *d_t8;
+  int32_t *d_bad, *d_i, *d_nm;
+  float* d_d;
+  B.in(d_qf, q, (size_t)nq * dim); B.in(d_tf, t, rows * dim); B.in(d_seg, seg_ptr, (size_t)n_seg + 1);
+  B.tmp(d_q8, (size_t)nq * dim); B.tmp(d_t8, rows * dim); B.tmp(d_bad, 2);
+  B.out(d_i, out_i, on); B.out(d_d, out_d, on); B.out(d_nm, filter ? n_matches : nullptr, n_seg);
+  if ((rc = B.place()) || (rc = B.upload())) return rc;
+  rc = cvb_quantize_u8_dev(ctx, d_qf, (int64_t)nq * dim, d_q8, d_bad, nullptr);
   if (rc) return rc;
-  uint8_t* d_q8 = (uint8_t*)cvb_ws(ctx, WS_TMP0, (size_t)nq * dim);
-  uint8_t* d_t8 = (uint8_t*)cvb_ws(ctx, WS_TMP1, rows * dim);
-  int32_t* d_bad = (int32_t*)cvb_ws(ctx, WS_FLAG, 2 * sizeof(int32_t));
-  if (!d_q8 || !d_t8 || !d_bad) return CVB_ERR_CUDA;
-  rc = cvb_quantize_u8_dev(ctx, (const float*)d_qf, (int64_t)nq * dim, d_q8, d_bad, nullptr);
-  if (rc) return rc;
-  rc = cvb_quantize_u8_dev(ctx, (const float*)d_tf, (int64_t)rows * dim, d_t8, d_bad + 1, nullptr);
+  rc = cvb_quantize_u8_dev(ctx, d_tf, (int64_t)rows * dim, d_t8, d_bad + 1, nullptr);
   if (rc) return rc;
   int32_t bad[2] = {0, 0};
   CVB_CUDA(ctx, cudaMemcpyAsync(bad, d_bad, sizeof(bad), cudaMemcpyDeviceToHost, ctx->stream));
@@ -1136,21 +1110,10 @@ static int l2_host(cvb_ctx* ctx, const float* q, int nq, const float* t, const i
   if (bad[0] || bad[1])
     return cvb_fail(ctx, CVB_ERR_UNSUPPORTED,
                     "L2 descriptors must be integer-valued in [0,255] (cv::xfeatures2d::SIFT output)");
-  const size_t on = (size_t)n_seg * nq * (filter ? 1 : k);
-  int32_t* d_i = (int32_t*)cvb_ws(ctx, WS_OUT0, on * 4);
-  float* d_d = (float*)cvb_ws(ctx, WS_OUT1, on * 4);
-  int32_t* d_nm = (int32_t*)cvb_ws(ctx, WS_OUT2, (size_t)n_seg * 4);
-  if (!d_i || !d_d || !d_nm) return CVB_ERR_CUDA;
   rc = knn_dev<L2Metric, 2>(ctx, d_q8, nq, d_t8, d_seg, seg_ptr, n_seg, k, d_i, d_d, filter, thr, ratio, d_i, d_d,
                             d_nm, ctx->stream);
   if (rc) return rc;
-  if (on) {
-    CVB_CUDA(ctx, cudaMemcpyAsync(out_i, d_i, on * 4, cudaMemcpyDeviceToHost, ctx->stream));
-    CVB_CUDA(ctx, cudaMemcpyAsync(out_d, d_d, on * 4, cudaMemcpyDeviceToHost, ctx->stream));
-  }
-  if (filter) CVB_CUDA(ctx, cudaMemcpyAsync(n_matches, d_nm, (size_t)n_seg * 4, cudaMemcpyDeviceToHost, ctx->stream));
-  CVB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-  return CVB_OK;
+  return B.download();
 }
 
 int cvb_knn_l2_batch(cvb_ctx* ctx, const float* q, int nq, const float* t, const int32_t* seg_ptr, int n_seg, int dim,
@@ -1185,9 +1148,12 @@ int cvb_landmark_match_batch_dev(cvb_ctx* ctx, const uint8_t* d_A, const uint8_t
   }
   const int ithr = (int)ceilf(thr);  // integer d: (float)d < thr  <=>  d < ceil(thr)
   const size_t ln = (size_t)n_seg * nA * num_best;
-  int32_t* li = (int32_t*)cvb_ws(ctx, WS_LIST_I, ln * 4);
-  int32_t* ld = (int32_t*)cvb_ws(ctx, WS_LIST_D, ln * 4);
-  if (!li || !ld) return CVB_ERR_CUDA;
+  const size_t smem = ((size_t)2 * nA * num_best + (size_t)2 * max_len) * sizeof(int32_t);
+  cvb_block B(ctx, st);
+  int32_t *li, *ld, *vi = nullptr, *vd = nullptr;
+  B.tmp(li, ln); B.tmp(ld, ln);
+  if (smem > 200 * 1024) { B.tmp(vi, total); B.tmp(vd, total); }
+  if ((rc = B.place())) return rc;
   Plan pl = make_plan<HammingMetric>(nA, n_seg, max_len, ctx->sm_count, 4, false);
   ScanParams sp{};
   sp.q = d_A; sp.nq = nA; sp.t = d_B; sp.seg_ptr = d_seg_ptr; sp.n_seg = n_seg;
@@ -1195,7 +1161,6 @@ int cvb_landmark_match_batch_dev(cvb_ctx* ctx, const uint8_t* d_A, const uint8_t
   sp.skipA = d_skipA; sp.skipB = d_skipB; sp.ithr = ithr;
   rc = dispatch_scan<HammingMetric, 4, MODE_DM>(ctx, sp, pl, num_best, st);
   if (rc) return rc;
-  const size_t smem = ((size_t)2 * nA * num_best + (size_t)2 * max_len) * sizeof(int32_t);
   if (smem <= 200 * 1024) {
     static size_t attr = 0;
     if (smem > attr) {
@@ -1206,9 +1171,6 @@ int cvb_landmark_match_batch_dev(cvb_ctx* ctx, const uint8_t* d_A, const uint8_t
     dm_assign_kernel<true><<<n_seg, 256, smem, st>>>(li, ld, nA, num_best, d_seg_ptr, ithr, nullptr, nullptr, d_outA,
                                                      d_outB, d_outD, d_n_out);
   } else {
-    int32_t* vi = (int32_t*)cvb_ws(ctx, WS_TMP0, (size_t)total * 4);
-    int32_t* vd = (int32_t*)cvb_ws(ctx, WS_TMP1, (size_t)total * 4);
-    if (!vi || !vd) return CVB_ERR_CUDA;
     dm_assign_kernel<false><<<n_seg, 256, 0, st>>>(li, ld, nA, num_best, d_seg_ptr, ithr, vi, vd, d_outA, d_outB,
                                                    d_outD, d_n_out);
   }
@@ -1225,38 +1187,19 @@ int cvb_landmark_match_batch(cvb_ctx* ctx, const uint8_t* A, const uint8_t* skip
   size_t rows = 0;
   int rc = host_rows(ctx, seg_ptr, n_seg, &rows);
   if (rc) return rc;
-  void *d_A, *d_B;
-  int32_t* d_seg;
-  rc = stage_inputs(ctx, A, (size_t)nA * 32, B, rows * 32, seg_ptr, n_seg, &d_A, &d_B, &d_seg);
+  cvb_block blk(ctx, ctx->stream, false);   // direct: the descriptor rows are large
+  const uint8_t *d_A, *d_B, *d_sA = nullptr, *d_sB = nullptr;
+  const int32_t* d_seg;
+  int32_t *d_oA, *d_oB, *d_n;
+  float* d_oD;
+  blk.in(d_A, A, (size_t)nA * 32); blk.in(d_B, B, rows * 32); blk.in(d_seg, seg_ptr, (size_t)n_seg + 1);
+  if (skipA) blk.in(d_sA, skipA, nA);
+  if (skipB) blk.in(d_sB, skipB, rows);
+  blk.out(d_oA, outA, rows); blk.out(d_oB, outB, rows); blk.out(d_oD, outD, rows); blk.out(d_n, n_out, n_seg);
+  if ((rc = blk.place()) || (rc = blk.upload())) return rc;
+  rc = cvb_landmark_match_batch_dev(ctx, d_A, d_sA, nA, d_B, d_sB, d_seg, seg_ptr, n_seg, thr, num_best, d_oA, d_oB, d_oD, d_n, nullptr);
   if (rc) return rc;
-  uint8_t* d_sA = nullptr;
-  uint8_t* d_sB = nullptr;
-  if (skipA) {
-    d_sA = (uint8_t*)cvb_ws(ctx, WS_SKIPA, (size_t)nA);
-    if (!d_sA) return CVB_ERR_CUDA;
-    if (nA) CVB_CUDA(ctx, cudaMemcpyAsync(d_sA, skipA, (size_t)nA, cudaMemcpyHostToDevice, ctx->stream));
-  }
-  if (skipB) {
-    d_sB = (uint8_t*)cvb_ws(ctx, WS_SKIPB, rows);
-    if (!d_sB) return CVB_ERR_CUDA;
-    if (rows) CVB_CUDA(ctx, cudaMemcpyAsync(d_sB, skipB, rows, cudaMemcpyHostToDevice, ctx->stream));
-  }
-  int32_t* d_oA = (int32_t*)cvb_ws(ctx, WS_OUT0, rows * 4);
-  int32_t* d_oB = (int32_t*)cvb_ws(ctx, WS_OUT1, rows * 4);
-  float* d_oD = (float*)cvb_ws(ctx, WS_OUT2, rows * 4);
-  int32_t* d_n = (int32_t*)cvb_ws(ctx, WS_MISC, (size_t)n_seg * 4);
-  if (!d_oA || !d_oB || !d_oD || !d_n) return CVB_ERR_CUDA;
-  rc = cvb_landmark_match_batch_dev(ctx, (const uint8_t*)d_A, d_sA, nA, (const uint8_t*)d_B, d_sB, d_seg, seg_ptr,
-                                    n_seg, thr, num_best, d_oA, d_oB, d_oD, d_n, nullptr);
-  if (rc) return rc;
-  if (rows) {
-    CVB_CUDA(ctx, cudaMemcpyAsync(outA, d_oA, rows * 4, cudaMemcpyDeviceToHost, ctx->stream));
-    CVB_CUDA(ctx, cudaMemcpyAsync(outB, d_oB, rows * 4, cudaMemcpyDeviceToHost, ctx->stream));
-    CVB_CUDA(ctx, cudaMemcpyAsync(outD, d_oD, rows * 4, cudaMemcpyDeviceToHost, ctx->stream));
-  }
-  CVB_CUDA(ctx, cudaMemcpyAsync(n_out, d_n, (size_t)n_seg * 4, cudaMemcpyDeviceToHost, ctx->stream));
-  CVB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-  return CVB_OK;
+  return blk.download();
 }
 
 }  // extern "C"

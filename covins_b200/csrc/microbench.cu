@@ -28,8 +28,10 @@ __global__ void __launch_bounds__(256) popc_kernel(int iters, uint32_t seed, uin
 extern "C" int cvb_microbench_popc(cvb_ctx* ctx, int iters, double* gpopc_per_s) {
   if (!ctx || !gpopc_per_s || iters <= 0) return CVB_ERR_INVALID;
   CVB_GUARD(ctx);
-  uint32_t* d = (uint32_t*)cvb_ws(ctx, WS_MISC, 256);
-  if (!d) return CVB_ERR_CUDA;
+  cvb_block B(ctx, ctx->stream);
+  uint32_t* d;
+  B.tmp(d, 1);
+  if (const int rc = B.place()) return rc;
   const int blocks = ctx->sm_count * 8;
   cudaEvent_t e0, e1;
   CVB_CUDA(ctx, cudaEventCreate(&e0));
@@ -118,8 +120,11 @@ __global__ void latency_kernel(double* out, double seed, int n) {
 extern "C" int cvb_microbench_latency(cvb_ctx* ctx, double* out8) {
   if (!ctx || !out8) return CVB_ERR_INVALID;
   CVB_GUARD(ctx);
-  double* d = (double*)cvb_ws(ctx, WS_MISC, 256);
-  if (!d) return CVB_ERR_CUDA;
+  double h[9];
+  cvb_block B(ctx, ctx->stream);
+  double* d;
+  B.out(d, h, 9);
+  if (const int rc = B.place()) return rc;
   cudaEvent_t e0, e1;
   CVB_CUDA(ctx, cudaEventCreate(&e0));
   CVB_CUDA(ctx, cudaEventCreate(&e1));
@@ -130,9 +135,7 @@ extern "C" int cvb_microbench_latency(cvb_ctx* ctx, double* out8) {
   latency_kernel<<<1, 32, 0, ctx->stream>>>(d, 1.0, n);
   CVB_CHECK_LAUNCH(ctx);
   CVB_CUDA(ctx, cudaEventRecord(e1, ctx->stream));
-  double h[9];
-  CVB_CUDA(ctx, cudaMemcpyAsync(h, d, sizeof(h), cudaMemcpyDeviceToHost, ctx->stream));
-  CVB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  if (const int rc = B.download()) return rc;
   float ms = 0.f;
   CVB_CUDA(ctx, cudaEventElapsedTime(&ms, e0, e1));
   for (int i = 0; i < 7; i++) out8[i] = h[i];
@@ -178,8 +181,10 @@ __global__ void __launch_bounds__(256) minmax_kernel(unsigned* out, unsigned see
 extern "C" int cvb_microbench_minmax(cvb_ctx* ctx, double* out2) {
   if (!ctx || !out2) return CVB_ERR_INVALID;
   CVB_GUARD(ctx);
-  unsigned* d = (unsigned*)cvb_ws(ctx, WS_MISC, 256);
-  if (!d) return CVB_ERR_CUDA;
+  cvb_block B(ctx, ctx->stream);
+  unsigned* d;
+  B.tmp(d, 1);
+  if (const int rc = B.place()) return rc;
   cudaEvent_t e0, e1;
   CVB_CUDA(ctx, cudaEventCreate(&e0));
   CVB_CUDA(ctx, cudaEventCreate(&e1));

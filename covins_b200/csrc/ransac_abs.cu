@@ -272,25 +272,16 @@ int abs_ransac(cvb_ctx* ctx, const char* name, const cvb_abs_ransac_problems* p,
   CVB_REQUIRE(ctx, p->cam_off && p->cam_rot, "%s: null camera arrays", name);
   const size_t N = (size_t)p->prob_ptr[n_prob];
   CVB_REQUIRE(ctx, N == 0 || (p->pts && p->f && p->sigma), "%s: null correspondence arrays", name);
-  Stager St;
-  const size_t o_ptr = St.put(p->prob_ptr, ((size_t)n_prob + 1) * 4), o_pts = St.put(p->pts, N * 24), o_f = St.put(p->f, N * 24),
-               o_sg = St.put(p->sigma, N * 8), o_smp = seeded ? St.put(seed, (size_t)n_prob * 8) : St.put(p->samples, (size_t)n_prob * ns * 16);
-  const size_t o_cam = St.reserve((size_t)n_prob * 96);
-  for (int i = 0; i < n_prob; i++) {   // one camera per problem: offset (3) directly followed by the rotation (9, row-major)
-    memcpy(St.h.data() + o_cam + 96 * (size_t)i, p->cam_off + 3 * (size_t)i, 24);
-    memcpy(St.h.data() + o_cam + 96 * (size_t)i + 24, p->cam_rot + 9 * (size_t)i, 72);
-  }
-  const auto inputs = [&](unsigned char* d) {
-    RansacDev D{};
-    D.prob_ptr = (const int*)(d + o_ptr); D.pts = (const double*)(d + o_pts); D.f = (const double*)(d + o_f); D.sigma = (const double*)(d + o_sg);
-    D.cam = (const double*)(d + o_cam);
-    if (seeded) D.o.seed = (const unsigned long long*)(d + o_smp);
-    else D.samples = (const int*)(d + o_smp);
-    return D;
-  };
+  const std::vector<double> cam = pack_cams(p->cam_off, p->cam_rot, n_prob);   // one camera per problem
+  cvb_block B(ctx, ctx->stream);
+  RansacDev D{};
+  B.in(D.prob_ptr, p->prob_ptr, (size_t)n_prob + 1); B.in(D.pts, p->pts, N * 3); B.in(D.f, p->f, N * 3); B.in(D.sigma, p->sigma, N);
+  if (seeded) B.in(D.o.seed, seed, n_prob);
+  else B.in(D.samples, p->samples, (size_t)n_prob * ns * 4);
+  B.in(D.cam, cam.data(), (size_t)n_prob * 12);
   if (seeded)
-    return run_ransac(ctx, WS_GS5, ransac_abs_kernel<SeededSamples<4>>, 0, St, inputs, n_prob, ns, N, threshold, max_iterations, probability, r, drawn, 4);
-  return run_ransac(ctx, WS_GS5, ransac_abs_kernel<SuppliedSamples<4>>, 0, St, inputs, n_prob, ns, N, threshold, max_iterations, probability, r);
+    return run_ransac(ctx, B, ransac_abs_kernel<SeededSamples<4>>, 0, D, n_prob, ns, N, threshold, max_iterations, probability, r, drawn, 4);
+  return run_ransac(ctx, B, ransac_abs_kernel<SuppliedSamples<4>>, 0, D, n_prob, ns, N, threshold, max_iterations, probability, r);
 }
 
 }  // namespace

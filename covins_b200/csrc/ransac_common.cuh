@@ -292,48 +292,35 @@ int launch_ransac(cvb_ctx* ctx, void (*kernel)(Dev), size_t smem, const Dev& D, 
   return CVB_OK;
 }
 
-// The rest of a RANSAC call whose inputs are staged in St: its outputs staged after them, one upload into workspace slot
-// ws_slot, launch_ransac of kernel with the device struct inputs(device block) and its common part filled here, one download,
-// the copy-out into r.  A seeded call may also ask for
-// its drawn samples (drawn, k indices each, -1 where not drawn).
-template <class Dev, class Result, class Inputs>
-int run_ransac(cvb_ctx* ctx, int ws_slot, void (*kernel)(Dev), size_t smem, Stager& St, const Inputs& inputs, int n_prob, int ns, size_t N,
-               double threshold, int max_iterations, double probability, Result* r, int32_t* drawn = nullptr, int k = 0) {
+// cameras as the kernels read them: each one's offset (3) directly followed by its rotation (9, row-major)
+inline std::vector<double> pack_cams(const double* off, const double* rot, size_t n) {
+  std::vector<double> c(n * 12);
+  for (size_t j = 0; j < n; j++) {
+    memcpy(&c[12 * j], off + 3 * j, 24);
+    memcpy(&c[12 * j + 3], rot + 9 * j, 72);
+  }
+  return c;
+}
+
+// The rest of a RANSAC call whose inputs are bound in B (to D's pointers): its outputs bound after them, one upload,
+// launch_ransac of kernel with D and its common part filled here, one download into r.  A seeded call may also ask for its
+// drawn samples (drawn, k indices each, -1 where not drawn).
+template <class Dev, class Result>
+int run_ransac(cvb_ctx* ctx, cvb_block& B, void (*kernel)(Dev), size_t smem, Dev& D, int n_prob, int ns, size_t N, double threshold,
+               int max_iterations, double probability, Result* r, int32_t* drawn = nullptr, int k = 0) {
   const size_t S_all = (size_t)n_prob * ns;
-  const bool all = r->sample_model != nullptr;
-  const size_t in_bytes = St.h.size();
-  const size_t o_bm = St.reserve((size_t)n_prob * 96), o_bs = St.reserve((size_t)n_prob * 4), o_bc = St.reserve((size_t)n_prob * 4),
-               o_it = St.reserve((size_t)n_prob * 4), o_us = St.reserve((size_t)n_prob * 4), o_mask = r->inlier_mask ? St.reserve(N) : 0,
-               o_sm = all ? St.reserve(S_all * 96) : 0, o_sv = all ? St.reserve(S_all) : 0, o_sc = all ? St.reserve(S_all * 4) : 0,
-               o_dr = drawn ? St.reserve(S_all * k * 4) : 0;
-  const size_t total = St.h.size();
-  unsigned char* d = (unsigned char*)cvb_ws(ctx, ws_slot, total);
-  unsigned char* hpin = (unsigned char*)cvb_pinned(ctx, total);
-  if (!d || !hpin) return CVB_ERR_CUDA;
-  memcpy(hpin, St.h.data(), in_bytes);
-  Dev D = inputs(d);
   RansacOut& O = D.o;
-  set_outputs(O, ns, max_iterations, threshold, probability, (int*)(d + o_bs), (double*)(d + o_bm), (int*)(d + o_bc), (int*)(d + o_it),
-              (int*)(d + o_us), r->inlier_mask ? d + o_mask : nullptr);
-  if (all) { O.sample_model = (double*)(d + o_sm); O.sample_valid = d + o_sv; O.sample_count = (int*)(d + o_sc); }
-  cudaStream_t st = ctx->stream;
-  CVB_CUDA(ctx, cudaMemcpyAsync(d, hpin, in_bytes, cudaMemcpyHostToDevice, st));
-  if (drawn) {
-    O.drawn = (int*)(d + o_dr);
-    CVB_CUDA(ctx, cudaMemsetAsync(d + o_dr, 0xff, S_all * k * 4, st));
-  }
+  set_selection(O, ns, max_iterations, threshold, probability);
+  B.out(O.best_model, r->best_model, (size_t)n_prob * 12); B.out(O.best_sample, r->best_sample, n_prob); B.out(O.best_count, r->best_count, n_prob);
+  B.out(O.iterations, r->iterations, n_prob); B.out(O.consumed, r->consumed, n_prob);
+  if (r->inlier_mask) B.out(O.inlier_mask, r->inlier_mask, N);
+  if (r->sample_model) { B.out(O.sample_model, r->sample_model, S_all * 12); B.out(O.sample_valid, r->sample_valid, S_all); B.out(O.sample_count, r->sample_count, S_all); }
+  if (drawn) B.out(O.drawn, drawn, S_all * k);
+  if (const int rc = B.place()) return rc;
+  if (const int rc = B.upload()) return rc;
+  if (drawn) CVB_CUDA(ctx, cudaMemsetAsync(O.drawn, 0xff, S_all * k * 4, ctx->stream));
   if (const int rc = launch_ransac(ctx, kernel, smem, D, n_prob)) return rc;
-  CVB_CUDA(ctx, cudaMemcpyAsync(hpin + o_bm, d + o_bm, total - o_bm, cudaMemcpyDeviceToHost, st));
-  CVB_CUDA(ctx, cudaStreamSynchronize(st));
-  memcpy(r->best_model, hpin + o_bm, (size_t)n_prob * 96); memcpy(r->best_sample, hpin + o_bs, (size_t)n_prob * 4);
-  memcpy(r->best_count, hpin + o_bc, (size_t)n_prob * 4); memcpy(r->iterations, hpin + o_it, (size_t)n_prob * 4);
-  memcpy(r->consumed, hpin + o_us, (size_t)n_prob * 4);
-  if (r->inlier_mask) memcpy(r->inlier_mask, hpin + o_mask, N);
-  if (all) {
-    memcpy(r->sample_model, hpin + o_sm, S_all * 96); memcpy(r->sample_valid, hpin + o_sv, S_all); memcpy(r->sample_count, hpin + o_sc, S_all * 4);
-  }
-  if (drawn) memcpy(drawn, hpin + o_dr, S_all * k * 4);
-  return CVB_OK;
+  return B.download();
 }
 
 }  // namespace

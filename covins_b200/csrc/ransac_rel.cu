@@ -637,8 +637,6 @@ __global__ void __launch_bounds__(kThreads) ransac_rel_kernel(RelDev D) {
 }
 
 // staging offsets of the inputs (camera arrays unused by a central problem)
-struct RelIn { size_t ptr, f1, f2, s1, s2, c1, c2, cp1, cp2, rig1, rig2, smp; };
-
 // the argument checks of a non-central problem batch (n_prob > 0) shared by the RANSAC and the covariance calls, up to the
 // samples; with_sigma: sigma1 / sigma2 are read; with_samples: the samples are (the sample-supplied calls).  Sets *max_pairs to the largest rig1 x rig2 camera-pair count.
 int check_rel_problems(cvb_ctx* ctx, const char* name, const cvb_rel_ransac_problems* p, bool with_sigma, bool with_samples, int* max_pairs) {
@@ -666,20 +664,6 @@ int check_rel_problems(cvb_ctx* ctx, const char* name, const cvb_rel_ransac_prob
   return CVB_OK;
 }
 
-// both rigs of a non-central batch into St, each camera as its offset (3) directly followed by its rotation (9, row-major)
-void stage_rigs(Stager& St, const cvb_rel_ransac_problems* p, RelIn& in) {
-  const size_t NC1 = (size_t)p->cam_ptr1[p->n_prob], NC2 = (size_t)p->cam_ptr2[p->n_prob];
-  in.rig1 = St.reserve(NC1 * 96); in.rig2 = St.reserve(NC2 * 96);
-  for (size_t j = 0; j < NC1; j++) {
-    memcpy(St.h.data() + in.rig1 + 96 * j, p->cam_off1 + 3 * j, 24);
-    memcpy(St.h.data() + in.rig1 + 96 * j + 24, p->cam_rot1 + 9 * j, 72);
-  }
-  for (size_t j = 0; j < NC2; j++) {
-    memcpy(St.h.data() + in.rig2 + 96 * j, p->cam_off2 + 3 * j, 24);
-    memcpy(St.h.data() + in.rig2 + 96 * j + 24, p->cam_rot2 + 9 * j, 72);
-  }
-}
-
 // the per-warp area (doubles) of ransac_rel_kernel<Sv, Src> for a batch whose largest camera-pair count is max_pairs; the
 // kernel's dynamic shared-memory limit is raised to the largest possible area on first use per device
 template <class Sv, class Src>
@@ -694,34 +678,20 @@ int rel_ransac_area(cvb_ctx* ctx, int max_pairs, int* area) {
   return CVB_OK;
 }
 
-// ransac_rel_kernel<Sv, Src> on the inputs staged in St (max_pairs: the largest camera-pair count of a problem; a seeded call's
-// seeds at in.smp, its drawn samples to drawn)
+// ransac_rel_kernel<Sv, Src> on the inputs bound in B to D (max_pairs: the largest camera-pair count of a problem; a seeded
+// call's drawn samples to drawn)
 template <class Sv, class Src>
-int run_rel_ransac(cvb_ctx* ctx, Stager& St, const RelIn& in, int n_prob, int ns, size_t N, int max_pairs, double threshold, int max_iterations,
+int run_rel_ransac(cvb_ctx* ctx, cvb_block& B, RelDev& D, int n_prob, int ns, size_t N, int max_pairs, double threshold, int max_iterations,
                    double probability, cvb_rel_ransac_result* r, int32_t* drawn = nullptr) {
-  int area = 0;
-  if (const int rc = rel_ransac_area<Sv, Src>(ctx, max_pairs, &area)) return rc;
-  const auto inputs = [&](unsigned char* d) {
-    RelDev D{};
-    D.prob_ptr = (const int*)(d + in.ptr); D.f1 = (const double*)(d + in.f1); D.f2 = (const double*)(d + in.f2);
-    D.s1 = (const double*)(d + in.s1); D.s2 = (const double*)(d + in.s2);
-    if (Src::kSeeded) D.o.seed = (const unsigned long long*)(d + in.smp);
-    else D.samples = (const int*)(d + in.smp);
-    if (!Sv::kCentral) {
-      D.cam1 = (const int*)(d + in.c1); D.cam2 = (const int*)(d + in.c2); D.cam_ptr1 = (const int*)(d + in.cp1); D.cam_ptr2 = (const int*)(d + in.cp2);
-      D.rig1 = (const double*)(d + in.rig1); D.rig2 = (const double*)(d + in.rig2);
-    }
-    D.area = area;
-    return D;
-  };
-  return run_ransac(ctx, WS_GS6, ransac_rel_kernel<Sv, Src>, (size_t)kWarps * area * sizeof(double), St, inputs, n_prob, ns, N, threshold,
-                    max_iterations, probability, r, drawn, Sv::kSample);
+  if (const int rc = rel_ransac_area<Sv, Src>(ctx, max_pairs, &D.area)) return rc;
+  return run_ransac(ctx, B, ransac_rel_kernel<Sv, Src>, (size_t)kWarps * D.area * sizeof(double), D, n_prob, ns, N, threshold, max_iterations,
+                    probability, r, drawn, Sv::kSample);
 }
 
 // ---- the sampling-based covariance of a 17-point model (cvb_noncentral_relative_pose_covariance_batch) ----
 // Solve: a problem's samples are spread over ceil(n_samples / kCovPerCta) CTAs (one linear grid over all problems), each
 // with both rigs and the reference model in shared memory and one warp per sample through rel17; lane 0 writes the sample's
-// deviation and valid flag to a workspace.  Reduce: one CTA per problem, thread (r, c) sums delta_r delta_c over the valid
+// deviation and valid flag to a scratch array.  Reduce: one CTA per problem, thread (r, c) sums delta_r delta_c over the valid
 // samples in sample order.
 constexpr int kCovPerCta = 4;   // samples (and warps) per solve CTA, chosen by measurement (DESIGN §9, K11e)
 constexpr int kCovReduceThreads = 64, kCovChunk = 256;
@@ -880,16 +850,18 @@ int noncentral_ransac(cvb_ctx* ctx, const char* name, const cvb_rel_ransac_probl
   int max_pairs = 0;
   if (const int rc = check_rel_problems(ctx, name, p, true, !seeded, &max_pairs)) return rc;
   const size_t N = (size_t)p->prob_ptr[n_prob], S_all = (size_t)n_prob * ns;
-  Stager St;
-  RelIn in{};
-  in.ptr = St.put(p->prob_ptr, ((size_t)n_prob + 1) * 4); in.f1 = St.put(p->f1, N * 24); in.f2 = St.put(p->f2, N * 24);
-  in.s1 = St.put(p->sigma1, N * 8); in.s2 = St.put(p->sigma2, N * 8); in.c1 = St.put(p->cam1, N * 4); in.c2 = St.put(p->cam2, N * 4);
-  in.cp1 = St.put(p->cam_ptr1, ((size_t)n_prob + 1) * 4); in.cp2 = St.put(p->cam_ptr2, ((size_t)n_prob + 1) * 4);
-  in.smp = seeded ? St.put(seed, (size_t)n_prob * 8) : St.put(p->samples, S_all * kSample * 4);
-  stage_rigs(St, p, in);
+  const std::vector<double> rig1 = pack_cams(p->cam_off1, p->cam_rot1, p->cam_ptr1[n_prob]), rig2 = pack_cams(p->cam_off2, p->cam_rot2, p->cam_ptr2[n_prob]);
+  cvb_block B(ctx, ctx->stream);
+  RelDev D{};
+  B.in(D.prob_ptr, p->prob_ptr, (size_t)n_prob + 1); B.in(D.f1, p->f1, N * 3); B.in(D.f2, p->f2, N * 3); B.in(D.s1, p->sigma1, N);
+  B.in(D.s2, p->sigma2, N); B.in(D.cam1, p->cam1, N); B.in(D.cam2, p->cam2, N);
+  B.in(D.cam_ptr1, p->cam_ptr1, (size_t)n_prob + 1); B.in(D.cam_ptr2, p->cam_ptr2, (size_t)n_prob + 1);
+  if (seeded) B.in(D.o.seed, seed, n_prob);
+  else B.in(D.samples, p->samples, S_all * kSample);
+  B.in(D.rig1, rig1.data(), rig1.size()); B.in(D.rig2, rig2.data(), rig2.size());
   if (seeded)
-    return run_rel_ransac<Solver17, SeededSamples<kSample>>(ctx, St, in, n_prob, ns, N, max_pairs, threshold, max_iterations, probability, r, drawn);
-  return run_rel_ransac<Solver17, SuppliedSamples<kSample>>(ctx, St, in, n_prob, ns, N, max_pairs, threshold, max_iterations, probability, r);
+    return run_rel_ransac<Solver17, SeededSamples<kSample>>(ctx, B, D, n_prob, ns, N, max_pairs, threshold, max_iterations, probability, r, drawn);
+  return run_rel_ransac<Solver17, SuppliedSamples<kSample>>(ctx, B, D, n_prob, ns, N, max_pairs, threshold, max_iterations, probability, r);
 }
 
 // cvb_ransac_central_relative_pose_batch (seeded = false) and cvb_ransac_central_relative_pose_seeded_batch
@@ -900,14 +872,15 @@ int central_ransac(cvb_ctx* ctx, const char* name, const cvb_central_rel_ransac_
   if (n_prob == 0) return CVB_OK;
   const size_t N = (size_t)p->prob_ptr[n_prob];
   CVB_REQUIRE(ctx, N == 0 || (p->f1 && p->f2 && p->sigma1 && p->sigma2), "%s: null correspondence arrays", name);
-  Stager St;
-  RelIn in{};
-  in.ptr = St.put(p->prob_ptr, ((size_t)n_prob + 1) * 4); in.f1 = St.put(p->f1, N * 24); in.f2 = St.put(p->f2, N * 24);
-  in.s1 = St.put(p->sigma1, N * 8); in.s2 = St.put(p->sigma2, N * 8);
-  in.smp = seeded ? St.put(seed, (size_t)n_prob * 8) : St.put(p->samples, (size_t)n_prob * ns * kSample5 * 4);
+  cvb_block B(ctx, ctx->stream);
+  RelDev D{};
+  B.in(D.prob_ptr, p->prob_ptr, (size_t)n_prob + 1); B.in(D.f1, p->f1, N * 3); B.in(D.f2, p->f2, N * 3); B.in(D.s1, p->sigma1, N);
+  B.in(D.s2, p->sigma2, N);
+  if (seeded) B.in(D.o.seed, seed, n_prob);
+  else B.in(D.samples, p->samples, (size_t)n_prob * ns * kSample5);
   if (seeded)
-    return run_rel_ransac<Solver5, SeededSamples<kSample5>>(ctx, St, in, n_prob, ns, N, 1, threshold, max_iterations, probability, r, drawn);
-  return run_rel_ransac<Solver5, SuppliedSamples<kSample5>>(ctx, St, in, n_prob, ns, N, 1, threshold, max_iterations, probability, r);
+    return run_rel_ransac<Solver5, SeededSamples<kSample5>>(ctx, B, D, n_prob, ns, N, 1, threshold, max_iterations, probability, r, drawn);
+  return run_rel_ransac<Solver5, SuppliedSamples<kSample5>>(ctx, B, D, n_prob, ns, N, 1, threshold, max_iterations, probability, r);
 }
 
 }  // namespace
@@ -976,42 +949,30 @@ int rel_cov(cvb_ctx* ctx, const char* name, const cvb_rel_ransac_problems* p, co
   if (!seeded)
     if (const int rc = check_samples(ctx, name, p->samples, p->prob_ptr, n_prob, ns, kSample, skip.data())) return rc;
   const size_t N = (size_t)p->prob_ptr[n_prob], S_all = (size_t)n_prob * ns;
-  const bool all = r->sample_delta != nullptr;
-  Stager St;
-  RelIn in{};
-  in.ptr = St.put(p->prob_ptr, ((size_t)n_prob + 1) * 4); in.f1 = St.put(p->f1, N * 24); in.f2 = St.put(p->f2, N * 24);
-  in.c1 = St.put(p->cam1, N * 4); in.c2 = St.put(p->cam2, N * 4);
-  in.cp1 = St.put(p->cam_ptr1, ((size_t)n_prob + 1) * 4); in.cp2 = St.put(p->cam_ptr2, ((size_t)n_prob + 1) * 4);
-  in.smp = seeded ? St.put(seed, (size_t)n_prob * 8) : St.put(p->samples, S_all * kSample * 4);
-  const size_t o_mask = seeded ? St.put(inlier_mask, N) : 0;
-  stage_rigs(St, p, in);
-  const size_t o_ref = St.put(ref_model, (size_t)n_prob * 96);
-  const size_t in_bytes = St.h.size();
-  const size_t o_cov = St.reserve((size_t)n_prob * 288), o_nv = St.reserve((size_t)n_prob * 4), o_d = St.reserve(S_all * 48), o_v = St.reserve(S_all),
-               o_dr = drawn ? St.reserve(S_all * kSample * 4) : 0;
-  const size_t total = St.h.size();
-  unsigned char* d = (unsigned char*)cvb_ws(ctx, WS_GS6, total);
-  unsigned char* hpin = (unsigned char*)cvb_pinned(ctx, total);
-  if (!d || !hpin) return CVB_ERR_CUDA;
-  memcpy(hpin, St.h.data(), in_bytes);
+  const int ctas_per_prob = (ns + kCovPerCta - 1) / kCovPerCta;
+  const long long grid = (long long)n_prob * ctas_per_prob;
+  CVB_REQUIRE(ctx, grid <= INT32_MAX, "%s: %lld solve CTAs exceed the grid limit", name, grid);
+  const std::vector<double> rig1 = pack_cams(p->cam_off1, p->cam_rot1, p->cam_ptr1[n_prob]), rig2 = pack_cams(p->cam_off2, p->cam_rot2, p->cam_ptr2[n_prob]);
+  cvb_block B(ctx, ctx->stream);
   CovSeededDev D{};   // the sample-supplied solve and the reduce take its CovDev part
-  D.prob_ptr = (const int*)(d + in.ptr); D.f1 = (const double*)(d + in.f1); D.f2 = (const double*)(d + in.f2);
-  D.cam1 = (const int*)(d + in.c1); D.cam2 = (const int*)(d + in.c2); D.cam_ptr1 = (const int*)(d + in.cp1); D.cam_ptr2 = (const int*)(d + in.cp2);
-  D.rig1 = (const double*)(d + in.rig1); D.rig2 = (const double*)(d + in.rig2);
+  B.in(D.prob_ptr, p->prob_ptr, (size_t)n_prob + 1); B.in(D.f1, p->f1, N * 3); B.in(D.f2, p->f2, N * 3); B.in(D.cam1, p->cam1, N); B.in(D.cam2, p->cam2, N);
+  B.in(D.cam_ptr1, p->cam_ptr1, (size_t)n_prob + 1); B.in(D.cam_ptr2, p->cam_ptr2, (size_t)n_prob + 1);
   if (seeded) {
-    D.seed = (const unsigned long long*)(d + in.smp); D.mask = d + o_mask; D.drawn = drawn ? (int*)(d + o_dr) : nullptr;
+    B.in(D.seed, seed, n_prob);
+    B.in(D.mask, inlier_mask, N);
   } else {
-    D.samples = (const int*)(d + in.smp);
+    B.in(D.samples, p->samples, S_all * kSample);
   }
-  D.ref_model = (const double*)(d + o_ref);
-  D.n_samples = ns; D.ctas_per_prob = (ns + kCovPerCta - 1) / kCovPerCta;
-  D.delta = (double*)(d + o_d); D.valid = d + o_v; D.cov = (double*)(d + o_cov); D.n_valid = (int*)(d + o_nv);
+  B.in(D.rig1, rig1.data(), rig1.size()); B.in(D.rig2, rig2.data(), rig2.size()); B.in(D.ref_model, ref_model, (size_t)n_prob * 12);
+  B.out(D.cov, r->cov, (size_t)n_prob * 36); B.out(D.n_valid, r->n_valid, n_prob); B.out(D.delta, r->sample_delta, S_all * 6);
+  B.out(D.valid, r->sample_valid, S_all);
+  if (drawn) B.out(D.drawn, drawn, S_all * kSample);
+  if (const int rc = B.place()) return rc;
+  if (const int rc = B.upload()) return rc;
+  D.n_samples = ns; D.ctas_per_prob = ctas_per_prob;
   cudaStream_t st = ctx->stream;
-  CVB_CUDA(ctx, cudaMemcpyAsync(d, hpin, in_bytes, cudaMemcpyHostToDevice, st));
-  if (drawn) CVB_CUDA(ctx, cudaMemsetAsync(d + o_dr, 0xff, S_all * kSample * 4, st));
+  if (drawn) CVB_CUDA(ctx, cudaMemsetAsync(D.drawn, 0xff, S_all * kSample * 4, st));
   if (ns > 0) {
-    const long long grid = (long long)n_prob * D.ctas_per_prob;
-    CVB_REQUIRE(ctx, grid <= INT32_MAX, "%s: %lld solve CTAs exceed the grid limit", name, grid);
     constexpr int kSolveWarps = kCovPerCta < kWarps ? kCovPerCta : kWarps;
     const size_t smem = (size_t)kSolveWarps * kSolveArea * sizeof(double);
     if (seeded) rel_cov_solve_kernel<CovSeededDev><<<(unsigned)grid, 32 * kSolveWarps, smem, st>>>(D);
@@ -1020,12 +981,7 @@ int rel_cov(cvb_ctx* ctx, const char* name, const cvb_rel_ransac_problems* p, co
   }
   rel_cov_reduce_kernel<<<n_prob, kCovReduceThreads, 0, st>>>(static_cast<const CovDev&>(D));
   CVB_CHECK_LAUNCH(ctx);
-  CVB_CUDA(ctx, cudaMemcpyAsync(hpin + o_cov, d + o_cov, (all || drawn ? total : o_d) - o_cov, cudaMemcpyDeviceToHost, st));
-  CVB_CUDA(ctx, cudaStreamSynchronize(st));
-  memcpy(r->cov, hpin + o_cov, (size_t)n_prob * 288); memcpy(r->n_valid, hpin + o_nv, (size_t)n_prob * 4);
-  if (all) { memcpy(r->sample_delta, hpin + o_d, S_all * 48); memcpy(r->sample_valid, hpin + o_v, S_all); }
-  if (drawn) memcpy(drawn, hpin + o_dr, S_all * kSample * 4);
-  return CVB_OK;
+  return B.download();
 }
 
 }  // namespace
@@ -1048,7 +1004,7 @@ extern "C" int cvb_noncentral_relative_pose_covariance_seeded_batch(cvb_ctx* ctx
 // ---- the verification chain of cvb_verify_noncentral_relative_pose_seeded_batch on the device ----
 // The matcher's pair-list scan (match_kernels.cu), verify_gather_kernel (matches -> 5-point problems), ransac_rel_kernel<Solver5>,
 // verify_merge_kernel (5-point inliers -> 17-point problems), ransac_rel_kernel<Solver17>, rel_cov_solve_kernel / rel_cov_reduce_kernel
-// and verify_list_kernel (the correspondence list), all on device buffers of one workspace.  The correspondence arrays are sized
+// and verify_list_kernel (the correspondence list), all on the arrays of one device block (cvb_block).  The correspondence arrays are sized
 // by the host-known bound sum over pairings of rows(kf1); the problems are packed to the front in pairing (candidate) order.
 namespace {
 
@@ -1199,99 +1155,67 @@ int verify_noncentral(cvb_ctx* ctx, const KF* kf, const cvb_verify_candidates* c
   const int ns = prm->n_cov_samples, ctas_per_cand = (ns + kCovPerCta - 1) / kCovPerCta;
   CVB_REQUIRE(ctx, (long long)C * ctas_per_cand <= INT32_MAX, "%s: %lld covariance CTAs exceed the grid limit", name, (long long)C * ctas_per_cand);
   const size_t S_all = (size_t)C * ns, L = r->corr ? std::min(B, (size_t)r->corr_cap) : 0;
-  // device block: inputs (uploaded), scratch, outputs (downloaded)
-  Stager St;
-  RelIn in{};
-  size_t o_desc;
+  std::vector<uint8_t> q8;   // the SIFT rows quantised; their check is an argument check, so it comes before the device block
   if constexpr (kSift) {
-    o_desc = St.reserve(R * 128);
-    if (!quantize_sift(kf->desc, R * 128, St.h.data() + o_desc))
+    q8.resize(R * 128);
+    if (!quantize_sift(kf->desc, R * 128, q8.data()))
       return cvb_fail(ctx, CVB_ERR_UNSUPPORTED, "%s: SIFT descriptors must be integer-valued in [0,255] (cv::xfeatures2d::SIFT output)", name);
-  } else {
-    o_desc = St.put(kf->desc, R * 32);
   }
-  const size_t o_bear = St.put(kf->bearings, R * 24), o_sig = St.put(kf->sigma, R * 8);
-  const size_t o_rows = St.put(rows.data(), (size_t)P * 20), o_cams = St.put(cams.data(), (size_t)P * 8);
-  const size_t o_pp = St.put(cd->pair_ptr, ((size_t)C + 1) * 4);
-  in.cp1 = St.put(cd->cam_ptr1, ((size_t)C + 1) * 4); in.cp2 = St.put(cd->cam_ptr2, ((size_t)C + 1) * 4);
-  cvb_rel_ransac_problems rp{};
-  rp.n_prob = C; rp.cam_ptr1 = cd->cam_ptr1; rp.cam_off1 = cd->cam_off1; rp.cam_rot1 = cd->cam_rot1;
-  rp.cam_ptr2 = cd->cam_ptr2; rp.cam_off2 = cd->cam_off2; rp.cam_rot2 = cd->cam_rot2;
-  stage_rigs(St, &rp, in);
-  const size_t o_seed5 = St.put(seed5, (size_t)P * 8), o_seed = St.put(seed, (size_t)C * 8);
-  const size_t in_bytes = St.h.size();
-  // scratch and outputs: device offsets only (the host block holds the inputs, and the outputs from in_bytes on)
-  size_t top = in_bytes;
-  const auto res = [&](size_t bytes) {
-    const size_t o = (top + 15) & ~size_t(15);
-    top = o + bytes;
-    return o;
-  };
-  const size_t o_mt = res(B * 4), o_md = res(B * 4);
-  const size_t o_f15 = res(B * 24), o_f25 = res(B * 24), o_s15 = res(B * 8), o_s25 = res(B * 8);
-  const size_t o_r1 = res(B * 4), o_r2 = res(B * 4), o_m5 = res(B), o_pos = res(B * 4);
-  const size_t o_f117 = res(B * 24), o_f217 = res(B * 24), o_s117 = res(B * 8), o_s217 = res(B * 8);
-  const size_t o_c117 = res(B * 4), o_c217 = res(B * 4), o_m17 = res(B), o_pp17 = res(((size_t)C + 1) * 4);
-  const size_t o_d = res(S_all * 48), o_v = res(S_all);
-  const size_t o_out = res(0);
-  const size_t o_nm = res((size_t)P * 4), o_pp5 = res(((size_t)P + 1) * 4), o_bs5 = res((size_t)P * 4),
-               o_bm5 = res((size_t)P * 96), o_bc5 = res((size_t)P * 4), o_it5 = res((size_t)P * 4), o_us5 = res((size_t)P * 4);
-  const size_t o_bs = res((size_t)C * 4), o_bm = res((size_t)C * 96), o_bc = res((size_t)C * 4), o_it = res((size_t)C * 4),
-               o_us = res((size_t)C * 4), o_cov = res((size_t)C * 288), o_nv = res((size_t)C * 4), o_corr = res(L * 20);
-  const size_t total = top, out_bytes = total - o_out;
-  unsigned char* d = (unsigned char*)cvb_ws(ctx, WS_GS6, total);
-  unsigned char* hpin = (unsigned char*)cvb_pinned(ctx, in_bytes + out_bytes);
-  if (!d || !hpin) return CVB_ERR_CUDA;
-  memcpy(hpin, St.h.data(), in_bytes);
-  unsigned char* hout = hpin + in_bytes;
-  cudaStream_t st = ctx->stream;
-  CVB_CUDA(ctx, cudaMemcpyAsync(d, hpin, in_bytes, cudaMemcpyHostToDevice, st));
+  const std::vector<double> rig1 = pack_cams(cd->cam_off1, cd->cam_rot1, NC1), rig2 = pack_cams(cd->cam_off2, cd->cam_rot2, NC2);
+  // device block: V, the 5-point RANSAC D5, the 17-point RANSAC D, the covariance Q
+  cvb_block blk(ctx, ctx->stream);
   VerifyDev V{};
-  V.bearings = (const double*)(d + o_bear); V.sigma = (const double*)(d + o_sig);
-  V.pair_rows = (const int*)(d + o_rows); V.pair_cams = (const int*)(d + o_cams); V.pair_ptr = (const int*)(d + o_pp);
-  V.match_train = (const int*)(d + o_mt); V.n_matches = (const int*)(d + o_nm);
-  V.prob_ptr5 = (int*)(d + o_pp5); V.f1_5 = (double*)(d + o_f15); V.f2_5 = (double*)(d + o_f25); V.s1_5 = (double*)(d + o_s15);
-  V.s2_5 = (double*)(d + o_s25); V.row1 = (int*)(d + o_r1); V.row2 = (int*)(d + o_r2); V.mask5 = d + o_m5; V.count5 = (const int*)(d + o_bc5);
-  V.prob_ptr17 = (int*)(d + o_pp17); V.f1_17 = (double*)(d + o_f117); V.f2_17 = (double*)(d + o_f217); V.s1_17 = (double*)(d + o_s117);
-  V.s2_17 = (double*)(d + o_s217); V.cam1_17 = (int*)(d + o_c117); V.cam2_17 = (int*)(d + o_c217); V.pos17 = (int*)(d + o_pos);
-  V.mask17 = d + o_m17; V.corr = (int*)(d + o_corr); V.corr_cap = (int)L;
+  RelDev D5{}, D{};
+  CovSeededDev Q{};
+  const uint8_t* d_desc;
+  int *d_mt, *d_nm;
+  float* d_md;
+  blk.in(d_desc, kSift ? (const void*)q8.data() : (const void*)kf->desc, R * (kSift ? 128 : 32));
+  blk.in(V.bearings, kf->bearings, R * 3); blk.in(V.sigma, kf->sigma, R);
+  blk.in(V.pair_rows, rows.data(), (size_t)P * 5); blk.in(V.pair_cams, cams.data(), (size_t)P * 2); blk.in(V.pair_ptr, cd->pair_ptr, (size_t)C + 1);
+  blk.in(D.cam_ptr1, cd->cam_ptr1, (size_t)C + 1); blk.in(D.cam_ptr2, cd->cam_ptr2, (size_t)C + 1);
+  blk.in(D.rig1, rig1.data(), rig1.size()); blk.in(D.rig2, rig2.data(), rig2.size());
+  blk.in(D5.o.seed, seed5, P); blk.in(D.o.seed, seed, C);
+  blk.tmp(d_mt, B); blk.tmp(d_md, B);
+  blk.tmp(V.f1_5, B * 3); blk.tmp(V.f2_5, B * 3); blk.tmp(V.s1_5, B); blk.tmp(V.s2_5, B);
+  blk.tmp(V.row1, B); blk.tmp(V.row2, B); blk.tmp(D5.o.inlier_mask, B); blk.tmp(V.pos17, B);
+  blk.tmp(V.f1_17, B * 3); blk.tmp(V.f2_17, B * 3); blk.tmp(V.s1_17, B); blk.tmp(V.s2_17, B);
+  blk.tmp(V.cam1_17, B); blk.tmp(V.cam2_17, B); blk.tmp(D.o.inlier_mask, B); blk.tmp(V.prob_ptr17, (size_t)C + 1);
+  blk.tmp(Q.delta, S_all * 6); blk.tmp(Q.valid, S_all);
+  blk.out(d_nm, r->n_matches, P); blk.out_host(V.prob_ptr5, (size_t)P + 1);
+  blk.out(D5.o.best_sample, r->best_sample5, P); blk.out(D5.o.best_model, r->best_model5, (size_t)P * 12); blk.out(D5.o.best_count, r->best_count5, P);
+  blk.out(D5.o.iterations, r->iterations5, P); blk.out(D5.o.consumed, r->consumed5, P);
+  blk.out(D.o.best_sample, r->best_sample, C); blk.out(D.o.best_model, r->best_model, (size_t)C * 12); blk.out(D.o.best_count, r->best_count, C);
+  blk.out(D.o.iterations, r->iterations, C); blk.out(D.o.consumed, r->consumed, C);
+  blk.out(Q.cov, r->cov, (size_t)C * 36); blk.out(Q.n_valid, r->n_valid, C); blk.out_host(V.corr, L * 5);
+  if (const int rc = blk.place()) return rc;
+  if (const int rc = blk.upload()) return rc;
+  cudaStream_t st = ctx->stream;
+  V.match_train = d_mt; V.n_matches = d_nm; V.mask5 = D5.o.inlier_mask; V.count5 = D5.o.best_count; V.mask17 = D.o.inlier_mask; V.corr_cap = (int)L;
   // 1. matches
   const auto match_pairs = kSift ? cvb_match_l2_pairs_dev : cvb_match_hamming_pairs_dev;
-  if (const int rc = match_pairs(ctx, d + o_desc, V.pair_rows, P, max_nq, prm->img_match_thres, prm->ratio_thres, (int*)(d + o_mt), (float*)(d + o_md),
-                                 (int*)(d + o_nm)))
-    return rc;
-  if (P == 0) CVB_CUDA(ctx, cudaMemsetAsync(d + o_pp5, 0, 4, st));
+  if (const int rc = match_pairs(ctx, d_desc, V.pair_rows, P, max_nq, prm->img_match_thres, prm->ratio_thres, d_mt, d_md, d_nm)) return rc;
+  if (P == 0) CVB_CUDA(ctx, cudaMemsetAsync(V.prob_ptr5, 0, 4, st));
   // 2. the 5-point problems and their RANSACs
   if (P > 0) {
     verify_gather_kernel<<<P, kGlueThreads, 0, st>>>(V);
     CVB_CHECK_LAUNCH(ctx);
-    RelDev D{};
-    D.prob_ptr = V.prob_ptr5; D.f1 = V.f1_5; D.f2 = V.f2_5; D.s1 = V.s1_5; D.s2 = V.s2_5;
-    set_selection(D.o, 0, prm->max_iterations5, prm->threshold5, prm->probability);
-    D.o.seed = (const unsigned long long*)(d + o_seed5);
-    D.o.best_sample = (int*)(d + o_bs5); D.o.best_model = (double*)(d + o_bm5); D.o.best_count = (int*)(d + o_bc5);
-    D.o.iterations = (int*)(d + o_it5); D.o.consumed = (int*)(d + o_us5); D.o.inlier_mask = d + o_m5;
-    if (const int rc = rel_ransac_area<Solver5, SeededSamples<kSample5>>(ctx, 1, &D.area)) return rc;
-    if (const int rc = launch_ransac(ctx, ransac_rel_kernel<Solver5, SeededSamples<kSample5>>, (size_t)kWarps * D.area * sizeof(double), D, P)) return rc;
+    D5.prob_ptr = V.prob_ptr5; D5.f1 = V.f1_5; D5.f2 = V.f2_5; D5.s1 = V.s1_5; D5.s2 = V.s2_5;
+    set_selection(D5.o, 0, prm->max_iterations5, prm->threshold5, prm->probability);
+    if (const int rc = rel_ransac_area<Solver5, SeededSamples<kSample5>>(ctx, 1, &D5.area)) return rc;
+    if (const int rc = launch_ransac(ctx, ransac_rel_kernel<Solver5, SeededSamples<kSample5>>, (size_t)kWarps * D5.area * sizeof(double), D5, P)) return rc;
   }
   // 3. the 17-point problems and their RANSACs
   verify_merge_kernel<<<C, kGlueThreads, 0, st>>>(V);
   CVB_CHECK_LAUNCH(ctx);
-  RelDev D{};
   D.prob_ptr = V.prob_ptr17; D.f1 = V.f1_17; D.f2 = V.f2_17; D.s1 = V.s1_17; D.s2 = V.s2_17; D.cam1 = V.cam1_17; D.cam2 = V.cam2_17;
-  D.cam_ptr1 = (const int*)(d + in.cp1); D.cam_ptr2 = (const int*)(d + in.cp2); D.rig1 = (const double*)(d + in.rig1); D.rig2 = (const double*)(d + in.rig2);
   set_selection(D.o, 0, prm->max_iterations17, prm->threshold17, prm->probability);
-  D.o.seed = (const unsigned long long*)(d + o_seed);
-  D.o.best_sample = (int*)(d + o_bs); D.o.best_model = (double*)(d + o_bm); D.o.best_count = (int*)(d + o_bc);
-  D.o.iterations = (int*)(d + o_it); D.o.consumed = (int*)(d + o_us); D.o.inlier_mask = d + o_m17;
   if (const int rc = rel_ransac_area<Solver17, SeededSamples<kSample>>(ctx, max_pairs, &D.area)) return rc;
   if (const int rc = launch_ransac(ctx, ransac_rel_kernel<Solver17, SeededSamples<kSample>>, (size_t)kWarps * D.area * sizeof(double), D, C)) return rc;
   // 4. the covariance from the 17-point inlier mask in place
-  CovSeededDev Q{};
   Q.prob_ptr = V.prob_ptr17; Q.f1 = V.f1_17; Q.f2 = V.f2_17; Q.cam1 = V.cam1_17; Q.cam2 = V.cam2_17;
   Q.cam_ptr1 = D.cam_ptr1; Q.cam_ptr2 = D.cam_ptr2; Q.rig1 = D.rig1; Q.rig2 = D.rig2; Q.ref_model = D.o.best_model;
   Q.n_samples = ns; Q.ctas_per_prob = ctas_per_cand;
-  Q.delta = (double*)(d + o_d); Q.valid = d + o_v; Q.cov = (double*)(d + o_cov); Q.n_valid = (int*)(d + o_nv);
   Q.mask = V.mask17; Q.seed = D.o.seed;
   if (ns > 0) {
     constexpr int kSolveWarps = kCovPerCta < kWarps ? kCovPerCta : kWarps;
@@ -1305,17 +1229,10 @@ int verify_noncentral(cvb_ctx* ctx, const KF* kf, const cvb_verify_candidates* c
     verify_list_kernel<<<P, kGlueThreads, 0, st>>>(V);
     CVB_CHECK_LAUNCH(ctx);
   }
-  CVB_CUDA(ctx, cudaMemcpyAsync(hout, d + o_out, out_bytes, cudaMemcpyDeviceToHost, st));
-  CVB_CUDA(ctx, cudaStreamSynchronize(st));
-  const auto get = [&](void* dst, size_t off, size_t bytes) { if (bytes) memcpy(dst, hout + (off - o_out), bytes); };
-  get(r->n_matches, o_nm, (size_t)P * 4); get(r->best_sample5, o_bs5, (size_t)P * 4); get(r->best_model5, o_bm5, (size_t)P * 96);
-  get(r->best_count5, o_bc5, (size_t)P * 4); get(r->iterations5, o_it5, (size_t)P * 4); get(r->consumed5, o_us5, (size_t)P * 4);
-  get(r->best_sample, o_bs, (size_t)C * 4); get(r->best_model, o_bm, (size_t)C * 96); get(r->best_count, o_bc, (size_t)C * 4);
-  get(r->iterations, o_it, (size_t)C * 4); get(r->consumed, o_us, (size_t)C * 4); get(r->cov, o_cov, (size_t)C * 288); get(r->n_valid, o_nv, (size_t)C * 4);
-  int32_t n_total = 0;
-  get(&n_total, o_pp5 + (size_t)P * 4, 4);
+  if (const int rc = blk.download()) return rc;
+  const int32_t n_total = blk.host(V.prob_ptr5)[P];
   r->n_total = n_total;
-  if (r->corr && (size_t)n_total <= L) get(r->corr, o_corr, (size_t)n_total * 20);
+  if (r->corr && (size_t)n_total <= L) memcpy(r->corr, blk.host(V.corr), (size_t)n_total * 20);
   return CVB_OK;
 }
 

@@ -357,36 +357,25 @@ extern "C" int cvb_optimize_relative_pose(cvb_ctx* ctx, const cvb_relpose_proble
     if (info) for (int i = 0; i < 19; i++) info[i] = 0.0;
     return CVB_OK;
   }
-  const size_t o_pA = 0, o_pB = o_pA + (size_t)n * 24, o_sA = o_pB + (size_t)n * 24, o_sB = o_sA + (size_t)n * 8, o_kA = o_sB + (size_t)n * 8,
-               o_kB = o_kA + (size_t)n * 8, o_pose = o_kB + (size_t)n * 8, in_bytes = o_pose + 56;
-  const size_t o_rec = (in_bytes + 15) & ~size_t(15), o_out = (o_rec + sizeof(RelDev) + 15) & ~size_t(15), o_rem = o_out + CVB_RELPOSE_OUT * 8,
-               total = o_rem + (size_t)n;
-  unsigned char* d = (unsigned char*)cvb_ws(ctx, WS_GS3, total);
-  unsigned char* h = (unsigned char*)cvb_pinned(ctx, total);
-  if (!d || !h) return CVB_ERR_CUDA;
-  memcpy(h + o_pA, p->pA_c, (size_t)n * 24); memcpy(h + o_pB, p->pB_c, (size_t)n * 24);
-  memcpy(h + o_sA, p->sigmaA, (size_t)n * 8); memcpy(h + o_sB, p->sigmaB, (size_t)n * 8);
-  memcpy(h + o_kA, p->kpA, (size_t)n * 8); memcpy(h + o_kB, p->kpB, (size_t)n * 8);
-  memcpy(h + o_pose, p->T12, 56);
+  cvb_block B(ctx, ctx->stream);
   RelDev D{};
+  RelDev* d_rec;
+  B.in(D.pA, p->pA_c, (size_t)n * 3); B.in(D.pB, p->pB_c, (size_t)n * 3); B.in(D.sA, p->sigmaA, n); B.in(D.sB, p->sigmaB, n);
+  B.in(D.kpA, p->kpA, (size_t)n * 2); B.in(D.kpB, p->kpB, (size_t)n * 2); B.in(D.pose_in, p->T12, 7); B.in(d_rec, nullptr, 1);
+  B.out_host(D.out, CVB_RELPOSE_OUT); B.out(D.removed, removed, n);
+  if (const int rc = B.place()) return rc;
   D.n = n;
-  D.pA = (const double*)(d + o_pA); D.pB = (const double*)(d + o_pB); D.sA = (const double*)(d + o_sA); D.sB = (const double*)(d + o_sB);
-  D.kpA = (const float*)(d + o_kA); D.kpB = (const float*)(d + o_kB);
   for (int c = 0; c < 4; c++) { D.camA.intr[c] = p->intrA[c]; D.camA.dist[c] = p->distA[c]; D.camB.intr[c] = p->intrB[c]; D.camB.dist[c] = p->distB[c]; }
   D.camA.cam = p->cam_model_A; D.camA.dm = p->dist_model_A; D.camA.xi = p->xiA;
   D.camB.cam = p->cam_model_B; D.camB.dm = p->dist_model_B; D.camB.xi = p->xiB;
-  D.pose_in = (const double*)(d + o_pose); D.removed = d + o_rem; D.out = (double*)(d + o_out);
-  memcpy(h + o_rec, &D, sizeof(D));
-  cudaStream_t st = ctx->stream;
-  CVB_CUDA(ctx, cudaMemcpyAsync(d, h, o_rec + sizeof(D), cudaMemcpyHostToDevice, st));
-  relpose_kernel<<<1, NT, 0, st>>>((const RelDev*)(d + o_rec), th_outlier_align);
+  *B.host(d_rec) = D;
+  if (const int rc = B.upload()) return rc;
+  relpose_kernel<<<1, NT, 0, ctx->stream>>>(d_rec, th_outlier_align);
   CVB_CHECK_LAUNCH(ctx);
-  CVB_CUDA(ctx, cudaMemcpyAsync(h + o_out, d + o_out, total - o_out, cudaMemcpyDeviceToHost, st));
-  CVB_CUDA(ctx, cudaStreamSynchronize(st));
-  const double* out = (const double*)(h + o_out);
+  if (const int rc = B.download()) return rc;
+  const double* out = B.host(D.out);
   for (int c = 0; c < 7; c++) T12_out[c] = out[c];
   *n_inliers = (int32_t)out[7];
-  if (removed) memcpy(removed, h + o_rem, (size_t)n);
   if (info) for (int i = 0; i < 19; i++) info[i] = out[8 + i];
   return CVB_OK;
 }

@@ -867,14 +867,16 @@ int launch(cvb_ctx* ctx, TcParams p, int metric, int k, cudaStream_t st) {
   if (parts > p.n_seg) parts = p.n_seg;
   p.parts = parts;
   if (metric == 0 && !(getenv("COVINS_B200_TC_XT") && !strcmp(getenv("COVINS_B200_TC_XT"), "0"))) {
+    cvb_block B(ctx, st);
     if (!p.xt) {
-      // no resident tile store for this train set (raw-pointer API): expand it into the workspace first (HBM-bound pre-pass)
+      // no resident tile store for this train set (raw-pointer API): expand it into the call's block first (HBM-bound pre-pass)
       CVB_REQUIRE(ctx, p.h_seg != nullptr, "tensor-core Hamming path needs the host copy of the segment table");
       std::vector<int32_t> h_tile;
       const int64_t n_tiles = tiles_of(p.h_seg, p.n_seg, &h_tile);
-      int32_t* d_tile = (int32_t*)cvb_ws(ctx, WS_XT_TILE, sizeof(int32_t) * ((size_t)p.n_seg + 1));
-      uint8_t* d_xt = (uint8_t*)cvb_ws(ctx, WS_XT, (size_t)n_tiles * xt::TILE_BYTES);
-      if (!d_tile || !d_xt) return CVB_ERR_CUDA;
+      int32_t* d_tile;
+      uint8_t* d_xt;
+      B.tmp(d_tile, (size_t)p.n_seg + 1); B.tmp(d_xt, (size_t)n_tiles * xt::TILE_BYTES);
+      if (const int rc = B.place()) return rc;
       CVB_CUDA(ctx, cudaMemcpyAsync(d_tile, h_tile.data(), sizeof(int32_t) * ((size_t)p.n_seg + 1), cudaMemcpyHostToDevice, st));
       CVB_CUDA(ctx, cudaStreamSynchronize(st));   // h_tile goes out of scope
       const int rc = expand_tiles(ctx, p.t, p.seg_ptr, d_tile, 0, p.n_seg, 0, (int)n_tiles, d_xt, st);

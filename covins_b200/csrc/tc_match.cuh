@@ -23,7 +23,7 @@ struct TcParams {
   float* match_dist;
   int32_t* n_matches;
   // Hamming only: the pre-expanded operand tiles of the train set (expand_tiles) and the first tile of every segment
-  // [n_seg + 1]; xt == nullptr → launch() expands into the workspace (needs h_seg, the host copy of seg_ptr)
+  // [n_seg + 1]; xt == nullptr → launch() expands into the call's device block (needs h_seg, the host copy of seg_ptr)
   const uint8_t* xt;
   const int32_t* seg_tile;
   const int32_t* h_seg;

@@ -14,7 +14,8 @@
  *   - functions without suffix take HOST buffers and include all H2D/D2H copies (synchronous on
  *     return); `_dev` variants take DEVICE pointers and enqueue on `stream` (a cudaStream_t passed as
  *     void*; NULL = the ctx's own stream) without synchronising.
- *   - a ctx owns one device, one stream, and grow-only device workspaces.  Every entry point makes the ctx's device
+ *   - a ctx owns one device, one stream and a pinned staging buffer; each call takes its device memory as one block from
+ *     the device's stream-ordered pool on the stream its work runs on.  Every entry point makes the ctx's device
  *     current for the calling thread and holds the ctx's lock for its duration: a ctx may be shared between host threads
  *     (calls are serialised per ctx); for concurrency use one ctx per host thread (the reference runs one
  *     place-recognition thread per agent, src/covins_backend/handler_be.cpp:52-56, and at most one optimisation per map).

@@ -14,8 +14,7 @@
 
 #include "../../covins_b200/csrc/cholesky.cuh"
 
-// the library's workspace and error helpers (referenced by cholesky.cu's device paths, never called here)
-void* cvb_ws(cvb_ctx*, int, size_t) { return nullptr; }
+// the library's error helper (referenced by cholesky.cu's device paths, never called here)
 int cvb_fail(cvb_ctx*, int code, const char*, ...) { return code; }
 
 static void put(FILE* f, const std::vector<int>& v) {
