@@ -16,7 +16,7 @@
 //   tile_update_kernel trailing tiles (i >= j > k): A(i,j) -= A(i,k) A(j,k)^T (one 128x128 tile per CTA, 128^3 DMMA GEMM
 //                      per panel; in blocks of kPanelBlock columns, all of a block's panels per visit to a tile — see
 //                      factor()); syrk_kernel does the same for the chain's diagonal pair, spread over 4 CTAs for latency
-// Solves use the stored tile inverses: forward L y = b, backward L^T x = y, one launch per tile column.
+// Solves use the stored tile inverses: forward L y = b, backward L^T x = y, one persistent launch per direction.
 // All reductions have a fixed order → bit-reproducible run to run.
 #include "cholesky.cuh"
 
@@ -680,127 +680,146 @@ __global__ void __launch_bounds__(POTRF_THREADS, 1) potrf_inv_level_kernel(doubl
   potrf_inv(S + (size_t)tile_of[(size_t)k * nt + k] * TT, (size_t)T, 0, linv + (size_t)k * TT, flag, nullptr, 0);
 }
 
-// Triangular solves.  One launch per tile column; every CTA recomputes the tiny diagonal product (128x128 mat-vec with
-// the stored tile inverse) and then updates its own off-diagonal tile.  512 threads, all loads of a mat-vec are issued
-// before the first use (32 independent coalesced loads per thread) — these kernels are latency-, not bandwidth-bound.
+// Triangular solves: one persistent kernel per direction, subst_kernel<true> for L y = b and subst_kernel<false> for
+// L^T x = y.  A CTA takes the next tile row from a global ticket (increasing row index forward, decreasing backward) and
+// forms it completely:
+//   forward  row i: r = b_i; r -= L(i,k) y_k for the non-zero tiles (i,k), k < i, in increasing k; y_i = Linv_i r;
+//   backward row k: r = y_k; r -= L(i,k)^T x_i for the non-zero tiles (i,k), i > k, in decreasing i; x_k = Linv_k^T r;
+// then publishes its result through a per-row flag.  Row r only waits for rows that the ticket handed out before r, to
+// CTAs that are already running and never wait for r, so the kernel cannot deadlock whatever the grid size or residency.
+// The subtractions are those of a column-by-column solve (one launch per tile column), in the same order and with the
+// same products (tile_dot), so the result is bit-identical to it and does not depend on the grid.  A row's tile inverse
+// goes to shared memory (cp.async) and each tile to registers before the row waits for the operand, and the next tile is
+// fetched into L2 meanwhile: once the operand is published the row reads 128 doubles and does on-chip work only.
+// A wait that exceeds kSolveWaitNs (a broken dependency, never a slow one) gives up: the row's result is written as NaN
+// and still published, so a fault shows up as a non-finite solution instead of a hang.
 constexpr int SOLVE_THREADS = 512;
+constexpr size_t kSolveSmem = TT * sizeof(double);   // the row's tile inverse: 128 KB → 1 CTA / SM
+constexpr unsigned long long kSolveWaitNs = 4ull * 1000 * 1000 * 1000;
 
-// out[r] = sum_c A[r][c] x[c]   (A row-major 128x128 with leading dimension lda; lanes run along c)
-__device__ __forceinline__ void matvec_rows(const double* __restrict__ A, size_t lda, const double* x, double* out) {
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;   // 16 warps x 8 rows
-  double v[8][4];
-#pragma unroll
-  for (int i = 0; i < 8; i++)
-#pragma unroll
-    for (int j = 0; j < 4; j++) v[i][j] = A[(size_t)(warp * 8 + i) * lda + lane + 32 * j];
-#pragma unroll
-  for (int i = 0; i < 8; i++) {
-    double s = (v[i][0] * x[lane] + v[i][1] * x[lane + 32]) + (v[i][2] * x[lane + 64] + v[i][3] * x[lane + 96]);
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
-    if (lane == 0) out[warp * 8 + i] = s;
-  }
-}
-// out[c] = sum_m A[m][c] x[m]   (threads run along c; 4 groups of 128 threads split m, partials combined in order)
-__device__ __forceinline__ void matvec_cols(const double* __restrict__ A, size_t lda, const double* x, double* out,
-                                            double* part /*[4][128]*/) {
-  const int c = threadIdx.x & 127, g = threadIdx.x >> 7;
-  double v[32];
-#pragma unroll
-  for (int i = 0; i < 32; i++) v[i] = A[(size_t)(g * 32 + i) * lda + c];
-  double s = 0.0;
-#pragma unroll
-  for (int i = 0; i < 32; i++) s += v[i] * x[g * 32 + i];
-  part[g * T + c] = s;
-  __syncthreads();
-  if (threadIdx.x < T) out[c] = (part[c] + part[T + c]) + (part[2 * T + c] + part[3 * T + c]);
-  __syncthreads();
-}
-
-// forward step k: y_k = Linv_k b_k (written by CTA 0), b_i -= L(i,k) y_k for the non-zero row tiles i > k (rows[])
-// `panel` = first row tile of column k (row tiles contiguous)
-__global__ void __launch_bounds__(SOLVE_THREADS) fwd_kernel(const double* __restrict__ panel, int k,
-                                                            const double* __restrict__ linv, double* __restrict__ b,
-                                                            double* __restrict__ y, const int* __restrict__ rows) {
-  constexpr size_t ld = T;
-  __shared__ double bk[T], yk[T], upd[T];
-  const int tid = threadIdx.x;
-  if (tid < T) bk[tid] = b[(size_t)k * T + tid];
-  __syncthreads();
-  matvec_rows(linv + (size_t)k * T * T, T, bk, yk);   // Linv is stored with zeros above the diagonal
-  __syncthreads();
-  if (blockIdx.x == 0) {
-    if (tid < T) y[(size_t)k * T + tid] = yk[tid];
-    return;
-  }
-  const int i = rows[blockIdx.x - 1];
-  matvec_rows(panel + (size_t)(blockIdx.x - 1) * TT, ld, yk, upd);
-  __syncthreads();
-  if (tid < T) b[(size_t)i * T + tid] -= upd[tid];
-}
-
-// backward step k: x_k = Linv_k^T y_k (CTA 0), y_i -= L(k,i)^T x_k for the non-zero column tiles i < k of row k (cols[])
-__global__ void __launch_bounds__(SOLVE_THREADS) bwd_kernel(const double* __restrict__ L, const int* __restrict__ tile_of, int nt,
-                                                            int k, const double* __restrict__ linv, double* __restrict__ y,
-                                                            double* __restrict__ x, const int* __restrict__ cols) {
-  constexpr size_t ld = T;
-  __shared__ double ykk[T], xk[T], upd[T], part[4 * T];
-  const int tid = threadIdx.x;
-  if (tid < T) ykk[tid] = y[(size_t)k * T + tid];
-  __syncthreads();
-  matvec_cols(linv + (size_t)k * T * T, T, ykk, xk, part);
-  if (blockIdx.x == 0) {
-    if (tid < T) x[(size_t)k * T + tid] = xk[tid];
-    return;
-  }
-  const int i = cols[blockIdx.x - 1];
-  matvec_cols(L + (size_t)tile_of[(size_t)k * nt + i] * TT, ld, xk, upd, part);
-  if (tid < T) y[(size_t)i * T + tid] -= upd[tid];
-}
-
-// Level steps of the solve (TilePlan::h_lvl_ptr: columns c0 .. c0 + nc - 1, none of which touches another's rows of b / y).
-// diag_level_kernel: CTA c forms y_k = Linv_k b_k (FWD) or x_k = Linv_k^T y_k (backward) for k = c0 + c.
+// FWD: out = A x, row r of A by the 32 lanes of a warp (16 warps x 8 rows), lanes along the columns.  Backward:
+// out = A^T x, threads along the columns, 4 groups of 128 threads split the rows, partials combined in order.  A is a
+// row-major 128x128 tile.  tile_load fetches this thread's 32 elements, tile_dot forms the products; out is complete for
+// every thread when tile_dot returns.
 template <bool FWD>
-__global__ void __launch_bounds__(SOLVE_THREADS) diag_level_kernel(const double* __restrict__ linv, int c0,
-                                                                   const double* __restrict__ in, double* __restrict__ out) {
-  __shared__ double vk[T], rk[T], part[4 * T];
-  const int tid = threadIdx.x, k = c0 + blockIdx.x;
-  if (tid < T) vk[tid] = in[(size_t)k * T + tid];
-  __syncthreads();
+__device__ __forceinline__ void tile_load(const double* __restrict__ A, double (&v)[32]) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, c = threadIdx.x & 127, g = threadIdx.x >> 7;
+#pragma unroll
+  for (int i = 0; i < 32; i++) v[i] = FWD ? A[(size_t)(warp * 8 + i / 4) * T + lane + 32 * (i % 4)] : A[(size_t)(g * 32 + i) * T + c];
+}
+template <bool FWD>
+__device__ __forceinline__ void tile_dot(const double (&v)[32], const double* x, double* out, double* part /*[4][128]*/) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, c = threadIdx.x & 127, g = threadIdx.x >> 7;
   if (FWD) {
-    matvec_rows(linv + (size_t)k * TT, T, vk, rk);
+    double s[8];
+#pragma unroll
+    for (int i = 0; i < 8; i++)
+      s[i] = (v[4 * i] * x[lane] + v[4 * i + 1] * x[lane + 32]) + (v[4 * i + 2] * x[lane + 64] + v[4 * i + 3] * x[lane + 96]);
+    // Each row is summed over the lanes by the butterfly s += (s of lane ^ o), o = 16, 8, 4, 2, 1, as lane 0 sees it.  At
+    // the first three steps the partners split the rows instead of both summing all of them (lane 16 h1 + 8 h2 + 4 h3 ends
+    // with row 4 h1 + 2 h2 + h3): 9 shuffles instead of 40, and as IEEE addition commutes, the same bits.
+    const int h1 = (lane >> 4) & 1, h2 = (lane >> 3) & 1, h3 = (lane >> 2) & 1;
+    double t[4], u[2];
+#pragma unroll
+    for (int j = 0; j < 4; j++) t[j] = (h1 ? s[4 + j] : s[j]) + __shfl_xor_sync(0xffffffffu, h1 ? s[j] : s[4 + j], 16);
+#pragma unroll
+    for (int j = 0; j < 2; j++) u[j] = (h2 ? t[2 + j] : t[j]) + __shfl_xor_sync(0xffffffffu, h2 ? t[j] : t[2 + j], 8);
+    double w = (h3 ? u[1] : u[0]) + __shfl_xor_sync(0xffffffffu, h3 ? u[0] : u[1], 4);
+    w += __shfl_xor_sync(0xffffffffu, w, 2);
+    w += __shfl_xor_sync(0xffffffffu, w, 1);
+    if ((lane & 3) == 0) out[warp * 8 + 4 * h1 + 2 * h2 + h3] = w;
     __syncthreads();
   } else {
-    matvec_cols(linv + (size_t)k * TT, T, vk, rk, part);
-  }
-  if (tid < T) out[(size_t)k * T + tid] = rk[tid];
-}
-// gather_level_kernel: CTA per target tile i (targets[]) subtracts the level's products from its rows, one product at a
-// time in the order of the column-by-column solve: forward b_i -= L(i,k) y_k in increasing k, backward
-// y_i -= L(k,i)^T x_k in decreasing k.  v = y (forward) or x (backward) of the level's columns, r = b or y.
-template <bool FWD>
-__global__ void __launch_bounds__(SOLVE_THREADS) gather_level_kernel(const double* __restrict__ L, const int* __restrict__ tile_of,
-                                                                     int nt, int c0, int nc, const double* __restrict__ v,
-                                                                     double* __restrict__ r, const int* __restrict__ targets) {
-  __shared__ double vk[T], upd[T], part[4 * T];
-  const int tid = threadIdx.x, i = targets[blockIdx.x];
-  double ri = tid < T ? r[(size_t)i * T + tid] : 0.0;
-  for (int s = 0; s < nc; s++) {
-    const int k = FWD ? c0 + s : c0 + nc - 1 - s;
-    const int t = FWD ? tile_of[(size_t)i * nt + k] : tile_of[(size_t)k * nt + i];
-    if (t < 0) continue;
-    __syncthreads();   // the previous product is done with vk / upd
-    if (tid < T) vk[tid] = v[(size_t)k * T + tid];
+    double s = 0.0;
+#pragma unroll
+    for (int i = 0; i < 32; i++) s += v[i] * x[g * 32 + i];
+    part[g * T + c] = s;
     __syncthreads();
-    if (FWD) {
-      matvec_rows(L + (size_t)t * TT, T, vk, upd);
-      __syncthreads();
-    } else {
-      matvec_cols(L + (size_t)t * TT, T, vk, upd, part);
-    }
-    if (tid < T) ri -= upd[tid];
+    if (threadIdx.x < T) out[c] = (part[c] + part[T + c]) + (part[2 * T + c] + part[3 * T + c]);
+    __syncthreads();
   }
-  if (tid < T) r[(size_t)i * T + tid] = ri;
+}
+__device__ __forceinline__ int ld_acquire_gpu(const int* p) {
+  int v;
+  asm volatile("ld.acquire.gpu.global.s32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
+  return v;
+}
+__device__ __forceinline__ void st_release_gpu(int* p, int v) {
+  asm volatile("st.release.gpu.global.s32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
+}
+__device__ __forceinline__ unsigned long long globaltimer_ns() {
+  unsigned long long t;
+  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+  return t;
+}
+
+// Rows r of the direction: operands / results in out (row r at out + r T), the rows' input in `in`.  ptr / idx: the
+// non-zero tiles of row r — forward, the column tiles k < r of tile row r (TilePlan::h_rowc_*, packed index from
+// tile_of); backward, the row tiles i > r of tile column r (TilePlan::h_col_ptr / h_row_idx, packed contiguously after
+// the diagonal tile: index r + 1 + q).  sync[0] = ticket, sync[1 + r] = row r published; zero at launch.
+template <bool FWD>
+__global__ void __launch_bounds__(SOLVE_THREADS, 1) subst_kernel(const double* __restrict__ L, const double* __restrict__ linv,
+                                                                 const int* __restrict__ ptr, const int* __restrict__ idx,
+                                                                 const int* __restrict__ tile_of, int nt, const double* in,
+                                                                 double* out, int* sync) {
+  extern __shared__ __align__(16) double linv_s[];   // [T][T]
+  __shared__ double xs[T], upd[T], part[4 * T];
+  __shared__ int s_ticket, s_fail;
+  const int tid = threadIdx.x;
+  for (;;) {
+    if (tid == 0) {
+      s_ticket = atomicAdd(sync, 1);
+      s_fail = 0;
+    }
+    __syncthreads();
+    if (s_ticket >= nt) return;
+    const int r = FWD ? s_ticket : nt - 1 - s_ticket;
+#pragma unroll
+    for (int it = 0; it < (int)(TT / 2 / SOLVE_THREADS); it++) {
+      const int u = 2 * (tid + it * SOLVE_THREADS);
+      cp_async16(linv_s + u, linv + (size_t)r * TT + u);
+    }
+    cp_async_commit();
+    double acc = tid < T ? in[(size_t)r * T + tid] : 0.0;
+    const int q0 = ptr[r], n = ptr[r + 1] - q0;
+    auto tile = [&](int s) {   // s-th product of the row
+      const int q = FWD ? q0 + s : q0 + n - 1 - s;
+      return L + (size_t)(FWD ? tile_of[(size_t)r * nt + idx[q]] : r + 1 + q) * TT;
+    };
+    for (int s = 0; s < n; s++) {
+      const int k = idx[FWD ? q0 + s : q0 + n - 1 - s];
+      double v[32];
+      tile_load<FWD>(tile(s), v);
+      if (s + 1 < n) {
+        const double* nx = tile(s + 1);
+#pragma unroll
+        for (int it = 0; it < (int)(TT / 16 / SOLVE_THREADS); it++)   // the tile's 128-byte lines
+          asm volatile("prefetch.global.L2 [%0];" ::"l"(nx + (size_t)(tid + it * SOLVE_THREADS) * 16));
+      }
+      if (tid == 0 && !s_fail && !ld_acquire_gpu(sync + 1 + k)) {
+        const unsigned long long t0 = globaltimer_ns();
+        while (!ld_acquire_gpu(sync + 1 + k))
+          if (globaltimer_ns() - t0 > kSolveWaitNs) {
+            s_fail = 1;
+            break;
+          }
+      }
+      __syncthreads();
+      if (tid < T) xs[tid] = __ldcg(out + (size_t)k * T + tid);
+      __syncthreads();
+      tile_dot<FWD>(v, xs, upd, part);
+      if (tid < T) acc -= upd[tid];
+    }
+    if (tid < T) xs[tid] = acc;
+    cp_async_wait<0>();
+    __syncthreads();
+    double v[32];
+    tile_load<FWD>(linv_s, v);   // stored with zeros above the diagonal
+    tile_dot<FWD>(v, xs, upd, part);
+    if (tid < T) out[(size_t)r * T + tid] = s_fail ? __longlong_as_double(0x7ff8000000000000ll) : upd[tid];
+    __syncthreads();
+    if (tid == 0) st_release_gpu(sync + 1 + r, 1);
+  }
 }
 
 // Symbolic phase (host): tile-level structure of L from the tile-level structure of S (lower, nt x nt, row-major
@@ -998,7 +1017,7 @@ int TilePlan::upload(cvb_ctx* ctx, cudaStream_t st) {
       (rc = up(&d_lvl_pair_i, h_lvl_pair_i)) || (rc = up(&d_lvl_pair_j, h_lvl_pair_j)) ||
       (rc = up(&d_lvl_pair_k0, h_lvl_pair_k0)) || (rc = up(&d_lvl_pair_mask, h_lvl_pair_mask)) ||
       (rc = up(&d_lvl_trsm_tile, h_lvl_trsm_tile)) || (rc = up(&d_lvl_trsm_col, h_lvl_trsm_col)) ||
-      (rc = up(&d_lvl_fwd_idx, h_lvl_fwd_idx)) || (rc = up(&d_lvl_bwd_idx, h_lvl_bwd_idx)))
+      (rc = up(&d_col_ptr, h_col_ptr)) || (rc = up(&d_rowc_ptr, h_rowc_ptr)))
     return rc;
   CVB_CUDA(ctx, cudaStreamSynchronize(st));
   return CVB_OK;
@@ -1013,7 +1032,7 @@ void TilePlan::release() {
   if (d_tile_of) cudaFree(d_tile_of);
   d_row_idx = d_pair_i = d_pair_j = d_pair_mask = d_rowc_idx = d_tile_of = nullptr;
   for (int** d : {&d_lvl_pair_i, &d_lvl_pair_j, &d_lvl_pair_k0, &d_lvl_pair_mask, &d_lvl_trsm_tile, &d_lvl_trsm_col,
-                  &d_lvl_fwd_idx, &d_lvl_bwd_idx}) {
+                  &d_col_ptr, &d_rowc_ptr}) {
     if (*d) cudaFree(*d);
     *d = nullptr;
   }
@@ -1036,6 +1055,8 @@ int FactorStreams::create(cvb_ctx* ctx, int nt) {
     CVB_CUDA(ctx, cudaEventCreateWithFlags(&join[g], cudaEventDisableTiming));
   }
   CVB_CUDA(ctx, cudaEventCreateWithFlags(&fork, cudaEventDisableTiming));
+  CVB_CUDA(ctx, cudaMalloc(&d_solve_sync, (size_t)2 * (nt + 1) * sizeof(int)));
+  solve_nt = nt;
   return CVB_OK;
 }
 
@@ -1054,6 +1075,9 @@ void FactorStreams::destroy() {
     join_aux[g] = join[g] = nullptr;
   }
   if (fork) cudaEventDestroy(fork);
+  if (d_solve_sync) cudaFree(d_solve_sync);
+  d_solve_sync = nullptr;
+  solve_nt = 0;
   bulk = fast = nullptr;
   fork_fast = fork = nullptr;
 }
@@ -1404,47 +1428,39 @@ int factor(cvb_ctx* ctx, double* S, double* linv, int* d_flag, const TilePlan& p
   return CVB_OK;
 }
 
-// solves L L^T x = b; b is destroyed, tmp is scratch (n_pad), result in x
-int solve(cvb_ctx* ctx, const double* L, const double* linv, double* b, double* tmp, double* x,
-          const TilePlan& plan, cudaStream_t st, const FactorStreams& /*fs*/) {
-  const int nt = plan.nt, n_lvl = (int)plan.h_lvl_ptr.size() - 1;
-  // One step per level (TilePlan::h_lvl_ptr): a level's columns touch none of each other's rows of b / y, so a level of
-  // several columns is two launches — its diagonal products, then the gather into its target rows — and a single column
-  // is one (fwd_kernel / bwd_kernel).
-  for (int l = 0; l < n_lvl; l++) {
-    const int c0 = plan.h_lvl_ptr[l], nc = plan.h_lvl_ptr[l + 1] - c0;
-    if (nc > 1) {
-      const int t0 = plan.h_lvl_fwd_ptr[l], ntg = plan.h_lvl_fwd_ptr[l + 1] - t0;
-      diag_level_kernel<true><<<nc, SOLVE_THREADS, 0, st>>>(linv, c0, b, tmp);
-      CVB_CHECK_LAUNCH(ctx);
-      if (ntg > 0) {
-        gather_level_kernel<true><<<ntg, SOLVE_THREADS, 0, st>>>(L, plan.d_tile_of, nt, c0, nc, tmp, b, plan.d_lvl_fwd_idx + t0);
-        CVB_CHECK_LAUNCH(ctx);
-      }
-      continue;
-    }
-    const int m = plan.h_col_ptr[c0 + 1] - plan.h_col_ptr[c0];
-    fwd_kernel<<<1 + m, SOLVE_THREADS, 0, st>>>(L + (size_t)(plan.h_col_base[c0] + 1) * TT, c0, linv, b, tmp,
-                                                plan.d_row_idx + plan.h_col_ptr[c0]);
-    CVB_CHECK_LAUNCH(ctx);
+// solves L L^T x = b; tmp is scratch (n_pad), result in x.  grid = CTAs per direction, 0 = as many as fit on the device
+// at once (solve()); the result does not depend on it.
+int solve_grid(cvb_ctx* ctx, const double* L, const double* linv, const double* b, double* tmp, double* x,
+               const TilePlan& plan, cudaStream_t st, const FactorStreams& fs, int grid) {
+  static cvb_once_per_device once;
+  if (once.first(ctx->device)) {
+    CVB_CUDA(ctx, cudaFuncSetAttribute(subst_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSolveSmem));
+    CVB_CUDA(ctx, cudaFuncSetAttribute(subst_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSolveSmem));
   }
-  for (int l = n_lvl - 1; l >= 0; l--) {
-    const int c0 = plan.h_lvl_ptr[l], nc = plan.h_lvl_ptr[l + 1] - c0;
-    if (nc > 1) {
-      const int t0 = plan.h_lvl_bwd_ptr[l], ntg = plan.h_lvl_bwd_ptr[l + 1] - t0;
-      diag_level_kernel<false><<<nc, SOLVE_THREADS, 0, st>>>(linv, c0, tmp, x);
-      CVB_CHECK_LAUNCH(ctx);
-      if (ntg > 0) {
-        gather_level_kernel<false><<<ntg, SOLVE_THREADS, 0, st>>>(L, plan.d_tile_of, nt, c0, nc, x, tmp, plan.d_lvl_bwd_idx + t0);
-        CVB_CHECK_LAUNCH(ctx);
-      }
-      continue;
-    }
-    const int m = plan.h_rowc_ptr[c0 + 1] - plan.h_rowc_ptr[c0];
-    bwd_kernel<<<1 + m, SOLVE_THREADS, 0, st>>>(L, plan.d_tile_of, nt, c0, linv, tmp, x, plan.d_rowc_idx + plan.h_rowc_ptr[c0]);
-    CVB_CHECK_LAUNCH(ctx);
+  const int nt = plan.nt;
+  CVB_REQUIRE(ctx, plan.d_rowc_ptr != nullptr && plan.d_col_ptr != nullptr, "tile plan not built / uploaded");
+  CVB_REQUIRE(ctx, fs.d_solve_sync != nullptr && fs.solve_nt >= nt, "factor streams not created for this plan");
+  if (nt == 0) return CVB_OK;
+  if (grid <= 0) {
+    int per_sm = 0, n_sm = 0;
+    CVB_CUDA(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, subst_kernel<true>, SOLVE_THREADS, kSolveSmem));
+    CVB_CUDA(ctx, cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, ctx->device));
+    grid = per_sm * n_sm;
   }
+  grid = std::max(1, std::min(grid, nt));
+  int* fsync = fs.d_solve_sync;   // forward: [0, nt], backward: [nt + 1, 2 nt + 1]
+  CVB_CUDA(ctx, cudaMemsetAsync(fsync, 0, (size_t)2 * (nt + 1) * sizeof(int), st));
+  subst_kernel<true><<<grid, SOLVE_THREADS, kSolveSmem, st>>>(L, linv, plan.d_rowc_ptr, plan.d_rowc_idx, plan.d_tile_of,
+                                                              nt, b, tmp, fsync);
+  CVB_CHECK_LAUNCH(ctx);
+  subst_kernel<false><<<grid, SOLVE_THREADS, kSolveSmem, st>>>(L, linv, plan.d_col_ptr, plan.d_row_idx, nullptr, nt, tmp,
+                                                               x, fsync + nt + 1);
+  CVB_CHECK_LAUNCH(ctx);
   return CVB_OK;
+}
+int solve(cvb_ctx* ctx, const double* L, const double* linv, double* b, double* tmp, double* x,
+          const TilePlan& plan, cudaStream_t st, const FactorStreams& fs) {
+  return solve_grid(ctx, L, linv, b, tmp, x, plan, st, fs, 0);
 }
 
 }  // namespace cvb_chol

@@ -15,7 +15,7 @@ constexpr int kPanelBlock = 4;
 // Tile-level structure of the factor: which 128x128 tiles of L are structurally non-zero, as launch lists.
 struct TilePlan {
   int nt = 0;
-  std::vector<int> h_col_ptr, h_row_idx;           // per tile column k: non-zero row tiles i > k
+  std::vector<int> h_col_ptr, h_row_idx;           // per tile column k: non-zero row tiles i > k (also the backward solve)
   // Trailing-update launch lists, issued after the panel of tile column k is solved: pairs (i >= j) of target tiles with
   // the panels each one receives, bit q of h_pair_mask = panel h_pair_k0[k] + q (the panel tiles (i,k') and (j,k') both
   // exist).  Width 1 (h_blk_end[k] == k + 1 and h_pair_k0[k] == k): the pairs of panel k.  Inside a block of
@@ -27,19 +27,19 @@ struct TilePlan {
   std::vector<int> h_pair_split;                   // per tile column k: how many of its pairs (listed first) go on the work
                                                    // stream (the next block's columns); the rest go on the bulk stream
   std::vector<int> h_blk_end;                      // per tile column k: one past the last column of its block
-  std::vector<int> h_rowc_ptr, h_rowc_idx;         // per tile row k: non-zero column tiles i < k (backward solve)
+  std::vector<int> h_rowc_ptr, h_rowc_idx;         // per tile row k: non-zero column tiles i < k (forward solve)
   std::vector<int> h_col_group;                    // optional, per tile column: id (>= 0) of an independent column group
                                                    // (its columns share no tile with other groups), -1 = main sequence
   // Levels: the tile columns cut into runs [h_lvl_ptr[l], h_lvl_ptr[l + 1]) of mutually independent columns (no column of
   // a run has a row tile inside the run).  Column-group columns form maximal runs, capped so that the panels a target tile
   // receives from one run span at most 32 columns; every other column is a run of its own.  The columns of a run are
-  // factored together (factor(), single GPU and replicated plans) and substituted together (solve()).  Per group level
+  // factored together (factor(), single GPU and replicated plans).  Per group level
   // (the lists of every other level are empty):
   //   merged update list: every (target, panel) product of its columns' width-1 pair lists once, per target pair (i >= j)
   //     the first panel h_lvl_pair_k0 and bit q of h_lvl_pair_mask = panel k0 + q;
   //   trsm list: the packed index and column of every panel tile of its columns but the first one of a column whose first
   //     row tile is the next column (that tile is the chain's, see factor());
-  //   fwd / bwd targets: the row tiles i of its columns (forward solve) / the column tiles i < k of its rows (backward).
+  //   fwd / bwd targets (host only): the row tiles i of its columns / the column tiles i < k of its rows.
   std::vector<int> h_lvl_ptr;
   std::vector<int> h_lvl_pair_ptr, h_lvl_pair_i, h_lvl_pair_j, h_lvl_pair_k0, h_lvl_pair_mask;
   std::vector<int> h_lvl_trsm_ptr, h_lvl_trsm_tile, h_lvl_trsm_col;
@@ -56,7 +56,7 @@ struct TilePlan {
   int *d_row_idx = nullptr, *d_pair_i = nullptr, *d_pair_j = nullptr, *d_pair_mask = nullptr, *d_rowc_idx = nullptr,
       *d_tile_of = nullptr;
   int *d_lvl_pair_i = nullptr, *d_lvl_pair_j = nullptr, *d_lvl_pair_k0 = nullptr, *d_lvl_pair_mask = nullptr,
-      *d_lvl_trsm_tile = nullptr, *d_lvl_trsm_col = nullptr, *d_lvl_fwd_idx = nullptr, *d_lvl_bwd_idx = nullptr;
+      *d_lvl_trsm_tile = nullptr, *d_lvl_trsm_col = nullptr, *d_col_ptr = nullptr, *d_rowc_ptr = nullptr;
   long n_tiles_L = 0;
   double flops = 0.0;   // flops of one numeric factorisation with this plan
   // col_group (optional, nt entries): h_col_group.  owner (optional, nt entries) + rank: distributed plan.  flops = the
@@ -93,6 +93,8 @@ struct FactorStreams {
   cudaStream_t group_aux[n_group] = {};   // second stream per group: rest of the panel + updates, beside the group's chain
   cudaEvent_t join_aux[n_group] = {};
   cudaEvent_t fork = nullptr, join[n_group] = {};
+  int* d_solve_sync = nullptr;       // solve(): per direction a row ticket and one published flag per tile row (2 (nt + 1))
+  int solve_nt = 0;
   int create(cvb_ctx* ctx, int nt);
   void destroy();
 };
