@@ -242,19 +242,39 @@ __global__ void __launch_bounds__(SYRK_THREADS, 3) syrk_kernel(double* __restric
   }
 }
 
+// The trailing update's pipeline (tile_update below) uses the mbarrier helpers of cvb_internal.cuh and these two arrivals.
+__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
+  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(cvb_smem_addr(bar)) : "memory");
+}
+// arrives on `bar` once every cp.async this thread issued before has landed (the arrival counts against the init count)
+__device__ __forceinline__ void mbar_arrive_cp_async(uint64_t* bar) {
+  asm volatile("cp.async.mbarrier.arrive.noinc.shared::cta.b64 [%0];" ::"r"(cvb_smem_addr(bar)) : "memory");
+}
+
 // The same update, one CTA per pair and the whole 128x128 tile per CTA: the throughput path (every update list except the
 // chain's diagonal pair, see factor()).  Per 16-wide K chunk a CTA stages 128 rows of each operand for 128x128x16 FMA —
-// half the operand bytes per FMA of the 64x64 quadrants above, whose L2→SM traffic bounded them.  8 warps of 64x32
-// (4 m16 x 4 n8 blocks; a thread holds 128 accumulator doubles, the four B fragments of a chunk and one m16 row of A
-// fragments at a time): 221 registers, 1 CTA/SM.  The operands come through a 3-stage cp.async ring that runs on across
-// the panels of the pair's mask (a chunk's stage is refilled with the next panel's chunks while the epilogue runs).
-// C lives in shared memory for the whole visit: it is copied in during the first chunks, each panel's product
-// (accumulated from zero over the K chunks in order) is subtracted from it on its own, in increasing panel order, and it
-// is written back once.  So the results are bit-identical to syrk_kernel's, with one C read and one C write per visit
-// instead of an L2 read-modify-write per panel.  Ring rows are 128 B, unpadded: segment s of a row r sits at
-// s ^ 2 (r & 3), which makes the fragment loads conflict-free; C rows are 1 KB, 16-byte segment s of row r at s ^ 4 (r & 1),
-// which makes the epilogue's double2 accesses conflict-free.  Shared memory: 128 KB of C + 3 x 32 KB ring (+ 512 B).
-constexpr int TILE_THREADS = 256;
+// half the operand bytes per FMA of the 64x64 quadrants above, whose L2→SM traffic bounded them.  The operands come
+// through a 3-stage ring that runs on across the panels of the pair's mask, fed by a warp-specialised pipeline with no
+// CTA barrier in the main loop:
+//   producer   warpgroup 2 (4 warps, 24 registers after setmaxnreg) issues each chunk's cp.asyncs (16 per thread) into a
+//              stage once the stage's `empty` barrier has completed, and arrives on its `full` barrier through
+//              cp.async.mbarrier.arrive.noinc, which fires when the thread's copies have landed;
+//   consumers  warpgroups 0 and 1 (8 warps of 64x32: 4 m16 x 4 n8 blocks, 240 registers after setmaxnreg) wait on `full`,
+//              load the whole chunk's fragments (32 A + 16 B doubles beside the 64 accumulator doubles), release the stage
+//              on `empty` (one arrival per warp) and only then issue the chunk's 16 DMMAs.  So the stage is refilled
+//              while the DMMAs run, and the warps drift apart instead of meeting at a barrier every chunk.
+// The CTA is launched with 168 registers per thread (384 threads, 1 CTA/SM), and 24 x 128 + 240 x 256 = 168 x 384: the
+// consumers take exactly what the producer gives back.
+// C lives in shared memory for the whole visit: the producer copies it in with the first four chunks, each panel's
+// product (accumulated from zero over the K chunks in order) is subtracted from it on its own, in increasing panel order,
+// and the consumers write it back once.  So the results are bit-identical to syrk_kernel's, with one C read and one C
+// write per visit instead of an L2 read-modify-write per panel.  Ring rows are 128 B, unpadded: segment s of a row r sits
+// at s ^ 2 (r & 3), which makes the fragment loads conflict-free; C rows are 1 KB, 16-byte segment s of row r at
+// s ^ 4 (r & 1), which makes the epilogue's double2 accesses conflict-free.  Shared memory: 128 KB of C + 3 x 32 KB ring
+// (+ 576 B), 1 CTA/SM.
+constexpr int TILE_CONSUMERS = 256;                   // warpgroups 0 and 1
+constexpr int TILE_PRODUCERS = 128;                   // warpgroup 2
+constexpr int TILE_THREADS = TILE_CONSUMERS + TILE_PRODUCERS;
 constexpr int TILE_STAGES = 3;
 constexpr int TILE_STAGE = 2 * T * KC;   // doubles per ring stage: 128 rows of A(i,k), then 128 rows of A(j,k)
 constexpr size_t kTileSmem = (TT + (size_t)TILE_STAGES * TILE_STAGE) * sizeof(double);   // 229376 B → 1 CTA / SM
@@ -265,6 +285,8 @@ __device__ __forceinline__ void tile_update(double* __restrict__ S, const int* _
   extern __shared__ __align__(128) double smem_d[];
   __shared__ const double* s_ai[32];   // operand tiles A(i,k), A(j,k) of the pair's panels, in increasing k
   __shared__ const double* s_aj[32];
+  __shared__ uint64_t full[TILE_STAGES], empty[TILE_STAGES];
+  __shared__ int s_nch;   // chunks of the visit, read by each role after the set-up barrier (a register would spill)
   constexpr int NCH = T / KC;
   double* Cs = smem_d;            // [T][T], swizzled
   double* ring = smem_d + TT;     // [TILE_STAGES][2 T][KC], swizzled
@@ -278,92 +300,110 @@ __device__ __forceinline__ void tile_update(double* __restrict__ S, const int* _
     s_ai[q] = S + (size_t)tile_of[(size_t)i * nt + k0 + tid] * TT;
     s_aj[q] = S + (size_t)tile_of[(size_t)j * nt + k0 + tid] * TT;
   }
+  // the two warps of 64x32 above the diagonal of a diagonal tile are idle: they never touch the ring
+  const int g = lane >> 2, t = lane & 3, wm = warp >> 2, wn = warp & 3;   // warp tile: rows 64 wm.., columns 32 wn..
+  const bool idle = diag && wm == 0 && wn >= 2;
+  if (tid == 0) s_nch = __popc(mask) * NCH;   // chunk c = K chunk c % NCH of the pair's panel c / NCH
+  if (tid < TILE_STAGES) {
+    cvb_mbar_init(&full[tid], TILE_PRODUCERS);
+    cvb_mbar_init(&empty[tid], diag ? TILE_CONSUMERS / 32 - 2 : TILE_CONSUMERS / 32);
+    cvb_fence_mbar_init();
+  }
   __syncthreads();
-  const int nch = __popc(mask) * NCH;   // chunk c = K chunk c % NCH of the pair's panel c / NCH
-  // a thread copies 16-byte segment `seg` of rows r0, r0 + 32, ... of both operands (r0 & 3 fixes the swizzle)
-  const int r0 = tid >> 3, seg = tid & 7;
-  const int so = r0 * KC + ((seg ^ ((r0 & 3) << 1)) << 1);
-  auto load_chunk = [&](int c) {
-    if (c < nch) {
+
+  if (tid >= TILE_CONSUMERS) {   // ---- producer warpgroup
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 24;");
+    const int nch = s_nch;
+    const int pt = tid - TILE_CONSUMERS;
+    // a thread copies 16-byte segment `seg` of rows r0, r0 + 16, ... of both operands (r0 & 3 fixes the swizzle), and
+    // 16-byte segment `cs` of rows rc, rc + 2, ... of C's part
+    const int r0 = pt >> 3, seg = pt & 7, rc = pt >> 6, cs = pt & 63;
+    const int so = r0 * KC + ((seg ^ ((r0 & 3) << 1)) << 1);
+#pragma unroll 1
+    for (int c = 0; c < nch; c++) {
+      const int st = c % TILE_STAGES;
+      if (c >= TILE_STAGES) cvb_mbar_wait(&empty[st], (c / TILE_STAGES - 1) & 1);   // chunk c - 3 has left the stage
       const size_t go = (size_t)r0 * T + (c % NCH) * KC + seg * 2;
       const double* ga = s_ai[c / NCH] + go;
       const double* gb = s_aj[c / NCH] + go;
-      double* As = ring + (c % TILE_STAGES) * TILE_STAGE + so;
+      double* As = ring + st * TILE_STAGE + so;
 #pragma unroll
-      for (int it = 0; it < T / 32; it++) cp_async16(As + it * 32 * KC, ga + (size_t)it * 32 * T);
+      for (int it = 0; it < T / 16; it++) cp_async16(As + it * 16 * KC, ga + (size_t)it * 16 * T);
 #pragma unroll
-      for (int it = 0; it < T / 32; it++) cp_async16(As + T * KC + it * 32 * KC, gb + (size_t)it * 32 * T);
+      for (int it = 0; it < T / 16; it++) cp_async16(As + T * KC + it * 16 * KC, gb + (size_t)it * 16 * T);
+      // rows 32 c .. 32 c + 31 of C join chunk c (c < 4): all of C has landed before the first epilogue (chunk 7).  The
+      // quadrant above the diagonal of a diagonal tile is neither read nor written.
+      if (c < 4 && !(diag && c < 2 && cs >= 32)) {
+        const int r = c * 32 + rc;
+        double* cd = Cs + r * T + ((cs ^ (rc << 2)) << 1);
+        const double* cg = C + (size_t)r * T + cs * 2;
+#pragma unroll
+        for (int it = 0; it < 16; it++) cp_async16(cd + it * 2 * T, cg + it * 2 * T);
+      }
+      mbar_arrive_cp_async(&full[st]);
     }
-    cp_async_commit();   // always commit (possibly empty) so the wait count below is uniform
-  };
-  // rows 32 part .. 32 part + 31 of C join the group of chunk part + 2 (part < 4): all of C has landed at chunk 5, before
-  // the first epilogue, and the copy overlaps the first chunks.  The quadrant above the diagonal of a diagonal tile is
-  // neither read nor written.
-  auto load_c = [&](int part) {
+    asm volatile("cp.async.wait_all;" ::: "memory");   // no copy outlives its issuing thread
+    return;
+  }
+
+  // ---- consumer warpgroups
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 240;");
+  if (!idle) {
+    const int nch = s_nch;
+    int cq[4];   // ring column of fragment K index t + 4 q (rows g + 8 n: the swizzle depends on g & 3 only)
 #pragma unroll
-    for (int it = 0; it < 8; it++) {
-      const int u = tid + it * TILE_THREADS, r = part * 32 + (u >> 6), s = u & 63;
-      if (!(diag && r < 64 && s >= 32)) cp_async16(Cs + r * T + ((s ^ ((r & 1) << 2)) << 1), C + (size_t)r * T + s * 2);
-    }
-  };
-  const int g = lane >> 2, t = lane & 3, wm = warp >> 2, wn = warp & 3;   // warp tile: rows 64 wm.., columns 32 wn..
-  const bool idle = diag && wm == 0 && wn >= 2;                             // above the diagonal of a diagonal tile
-  int cq[4];   // ring column of fragment K index t + 4 q (rows g + 8 n: the swizzle depends on g & 3 only)
+    for (int q = 0; q < 4; q++) cq[q] = t + 4 * (q ^ (g & 3));
+    double acc[4][4][4];
 #pragma unroll
-  for (int q = 0; q < 4; q++) cq[q] = t + 4 * (q ^ (g & 3));
-  double acc[4][4][4];
+    for (int a = 0; a < 4; a++)
 #pragma unroll
-  for (int a = 0; a < 4; a++)
+      for (int b = 0; b < 4; b++)
 #pragma unroll
-    for (int b = 0; b < 4; b++)
-#pragma unroll
-      for (int e = 0; e < 4; e++) acc[a][b][e] = 0.0;
-#pragma unroll
-  for (int c = 0; c < TILE_STAGES - 1; c++) load_chunk(c);
+        for (int e = 0; e < 4; e++) acc[a][b][e] = 0.0;
 #pragma unroll 1
-  for (int c = 0; c < nch; c++) {
-    cp_async_wait<TILE_STAGES - 2>();   // chunk c has landed
-    __syncthreads();                    // ... for every thread, and chunk c-1's stage is free again
-    if (c < 4) load_c(c);
-    load_chunk(c + TILE_STAGES - 1);
-    if (idle) continue;
-    const double* As = ring + (c % TILE_STAGES) * TILE_STAGE + (wm * 64 + g) * KC;
-    const double* Bs = ring + (c % TILE_STAGES) * TILE_STAGE + T * KC + (wn * 32 + g) * KC;
-    double b[4][4];
+    for (int c = 0; c < nch; c++) {
+      const int st = c % TILE_STAGES;
+      cvb_mbar_wait(&full[st], (c / TILE_STAGES) & 1);   // chunk c (and C's part c < 4) has landed
+      const double* As = ring + st * TILE_STAGE + (wm * 64 + g) * KC;
+      const double* Bs = ring + st * TILE_STAGE + T * KC + (wn * 32 + g) * KC;
+      double a[4][8], b[4][4];
 #pragma unroll
-    for (int bj = 0; bj < 4; bj++)
+      for (int bj = 0; bj < 4; bj++)
 #pragma unroll
-      for (int e = 0; e < 4; e++) b[bj][e] = Bs[bj * 8 * KC + cq[e]];
-#pragma unroll
-    for (int ai = 0; ai < 4; ai++) {
-      double a[8];
-#pragma unroll
-      for (int e = 0; e < 8; e++) a[e] = As[(ai * 16 + 8 * (e & 1)) * KC + cq[e >> 1]];
-#pragma unroll
-      for (int bj = 0; bj < 4; bj++) dmma16816(acc[ai][bj], a, b[bj]);
-    }
-    if (c % NCH == NCH - 1) {   // the panel is complete: subtract it, start the next one from zero
+        for (int e = 0; e < 4; e++) b[bj][e] = Bs[bj * 8 * KC + cq[e]];
 #pragma unroll
       for (int ai = 0; ai < 4; ai++)
 #pragma unroll
-        for (int bj = 0; bj < 4; bj++)
+        for (int e = 0; e < 8; e++) a[ai][e] = As[(ai * 16 + 8 * (e & 1)) * KC + cq[e >> 1]];
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&empty[st]);   // the warp's fragments are in registers: the stage may be refilled
 #pragma unroll
-          for (int h = 0; h < 2; h++) {
-            const int r = wm * 64 + ai * 16 + h * 8 + g, s = wn * 16 + bj * 4 + t;
-            double2* q = reinterpret_cast<double2*>(Cs + r * T + ((s ^ ((r & 1) << 2)) << 1));
-            double2 v = *q;
-            v.x -= acc[ai][bj][2 * h];
-            v.y -= acc[ai][bj][2 * h + 1];
-            *q = v;
-            acc[ai][bj][2 * h] = 0.0;
-            acc[ai][bj][2 * h + 1] = 0.0;
-          }
+      for (int ai = 0; ai < 4; ai++)
+#pragma unroll
+        for (int bj = 0; bj < 4; bj++) dmma16816(acc[ai][bj], a[ai], b[bj]);
+      if (c % NCH == NCH - 1) {   // the panel is complete: subtract it, start the next one from zero
+#pragma unroll
+        for (int ai = 0; ai < 4; ai++)
+#pragma unroll
+          for (int bj = 0; bj < 4; bj++)
+#pragma unroll
+            for (int h = 0; h < 2; h++) {
+              const int r = wm * 64 + ai * 16 + h * 8 + g, s = wn * 16 + bj * 4 + t;
+              double2* q = reinterpret_cast<double2*>(Cs + r * T + ((s ^ ((r & 1) << 2)) << 1));
+              double2 v = *q;
+              v.x -= acc[ai][bj][2 * h];
+              v.y -= acc[ai][bj][2 * h + 1];
+              *q = v;
+              acc[ai][bj][2 * h] = 0.0;
+              acc[ai][bj][2 * h + 1] = 0.0;
+            }
+      }
     }
   }
-  __syncthreads();   // every warp's last epilogue is in Cs
+  asm volatile("bar.sync 1, %0;" ::"n"(TILE_CONSUMERS) : "memory");   // every consumer warp's last epilogue is in Cs
 #pragma unroll 8
-  for (int it = 0; it < (int)(TT / 2 / TILE_THREADS); it++) {
-    const int u = tid + it * TILE_THREADS, r = u >> 6, s = u & 63;
+  for (int it = 0; it < (int)(TT / 2 / TILE_CONSUMERS); it++) {
+    const int u = tid + it * TILE_CONSUMERS, r = u >> 6, s = u & 63;
     if (!(diag && r < 64 && s >= 32))
       *reinterpret_cast<double2*>(C + (size_t)r * T + s * 2) =
           *reinterpret_cast<const double2*>(Cs + r * T + ((s ^ ((r & 1) << 2)) << 1));
