@@ -99,6 +99,11 @@ SIGNATURES = {
     "cvb_ba_destroy": (C.c_int, [c_vp]),
     "cvb_ba_solve": (C.c_int, [c_vp, c_vp, c_vp, c_vp]),
     "cvb_gba": (C.c_int, [c_vp, c_vp, c_vp, c_vp, c_vp]),
+    "cvb_group_create": (C.c_int, [c_vp, C.c_int, C.POINTER(c_vp)]),
+    "cvb_group_destroy": (C.c_int, [c_vp]),
+    "cvb_group_allreduce_diag": (C.c_int, [c_vp, c_vp, C.c_size_t, c_vp]),
+    "cvb_ba_solve_group": (C.c_int, [c_vp, c_vp, c_vp, C.c_int, c_vp]),
+    "cvb_gba_group": (C.c_int, [c_vp, c_vp, c_vp, C.c_int, c_vp, c_vp]),
     "cvb_covisibility": (C.c_int, [c_vp, C.c_int, C.c_int, c_vp, c_vp, c_vp, c_vp, C.c_int, c_vp, c_vp, c_vp, C.c_int64,
                                    C.POINTER(C.c_int64)]),
     "cvb_redundant_keyframes": (C.c_int, [c_vp, C.c_int, C.c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, C.c_double,

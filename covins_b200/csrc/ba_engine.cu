@@ -37,6 +37,9 @@
 
 #include <cub/cub.cuh>
 
+#include <thread>
+
+#include "ba_group.cuh"
 #include "ba_math.cuh"
 #include "cholesky.cuh"
 #include "cvb_internal.cuh"
@@ -122,8 +125,9 @@ struct Engine {
   DevArr<double> xbuf, flagd;
   int n_xt_all = 0, n_xt_own = 0;
   size_t n_tiles = 0;                           // tiles of L's structure = length of S in tiles
-  // peer access (CUDA IPC): S, linv and the panel flags of every rank are mapped here (cvb_ba_enable_p2p)
-  bool p2p = false;
+  // peer access: S, linv and the panel flags of every rank are mapped here (enable_p2p: through CUDA IPC, or handed over
+  // by an in-process group, peer_ipc = false)
+  bool p2p = false, peer_ipc = false;
   double* S_raw = nullptr;                      // cudaMalloc'ed (IPC-exportable) when world > 1, else pool memory
   double* linv_raw = nullptr;
   int* pflag_raw = nullptr;
@@ -201,7 +205,7 @@ struct Engine {
     if (S_raw) { S.p = nullptr; linv.p = nullptr; }
     S.free_(); linv.free_(); flag.free_(); partials.free_();
     scalars.free_(); rankmax.free_();
-    for (int g = 0; g < dv.world && p2p; g++) {
+    for (int g = 0; g < dv.world && p2p && peer_ipc; g++) {
       if (g == dv.rank) continue;
       if (dv.peer_S[g]) cudaIpcCloseMemHandle(dv.peer_S[g]);
       if (dv.peer_linv[g]) cudaIpcCloseMemHandle(dv.peer_linv[g]);
@@ -1192,6 +1196,24 @@ int build_schur_lists(Engine& E, const std::vector<int>& h_lm_ptr, int K) {
   return CVB_OK;
 }
 
+// the host-side checks of a problem (cvb_ba_create's refusals; the group drivers run them before starting any rank)
+int check_problem(cvb_ctx* ctx, const cvb_ba_problem* p, int visual_only) {
+  CVB_REQUIRE(ctx, p->K > 0, "problem has no keyframes");
+  const int K = p->K;
+  CVB_REQUIRE(ctx, p->n_imu >= 0 && p->n_edge >= 0 && p->L >= 0, "negative problem size");
+  if (!visual_only)
+    for (int f = 0; f < p->n_imu; f++)
+      CVB_REQUIRE(ctx, p->imu_i[f] >= 0 && p->imu_i[f] < K && p->imu_j[f] >= 0 && p->imu_j[f] < K && p->imu_i[f] != p->imu_j[f],
+                  "bad IMU factor indices");
+  for (int e = 0; e < p->n_edge; e++)
+    CVB_REQUIRE(ctx, p->edge_i[e] >= 0 && p->edge_i[e] < K && p->edge_j[e] >= 0 && p->edge_j[e] < K && p->edge_i[e] != p->edge_j[e],
+                "bad edge indices");
+  for (int l = 0; l < p->L; l++)
+    for (int ob = p->lm_obs_ptr[l]; ob < p->lm_obs_ptr[l + 1]; ob++)
+      CVB_REQUIRE(ctx, p->obs_kf[ob] >= 0 && p->obs_kf[ob] < K, "obs_kf out of range");
+  return CVB_OK;
+}
+
 int engine_setup(Engine& E, const cvb_ba_problem* p, const cvb_ba_options* o) {
   cvb_ctx* ctx = E.ctx;
   const bool trace = getenv("COVINS_B200_SETUP_TRACE") != nullptr;   // development aid: host-side phase times to stderr
@@ -1209,20 +1231,10 @@ int engine_setup(Engine& E, const cvb_ba_problem* p, const cvb_ba_options* o) {
   E.a2_edge = o->cauchy_edge > 0 ? o->cauchy_edge * o->cauchy_edge : 0.0;
   E.rank = o->rank;
   E.world = o->world > 0 ? o->world : 1;
-  CVB_REQUIRE(ctx, p->K > 0, "problem has no keyframes");
   CVB_REQUIRE(ctx, E.rank >= 0 && E.rank < E.world, "bad rank/world");
+  int rc = check_problem(ctx, p, E.visual_only);
+  if (rc) return rc;
   const int K = p->K;
-  CVB_REQUIRE(ctx, p->n_imu >= 0 && p->n_edge >= 0 && p->L >= 0, "negative problem size");
-  if (!E.visual_only)
-    for (int f = 0; f < p->n_imu; f++)
-      CVB_REQUIRE(ctx, p->imu_i[f] >= 0 && p->imu_i[f] < K && p->imu_j[f] >= 0 && p->imu_j[f] < K && p->imu_i[f] != p->imu_j[f],
-                  "bad IMU factor indices");
-  for (int e = 0; e < p->n_edge; e++)
-    CVB_REQUIRE(ctx, p->edge_i[e] >= 0 && p->edge_i[e] < K && p->edge_j[e] >= 0 && p->edge_j[e] < K && p->edge_i[e] != p->edge_j[e],
-                "bad edge indices");
-  for (int l = 0; l < p->L; l++)
-    for (int ob = p->lm_obs_ptr[l]; ob < p->lm_obs_ptr[l + 1]; ob++)
-      CVB_REQUIRE(ctx, p->obs_kf[ob] >= 0 && p->obs_kf[ob] < K, "obs_kf out of range");
   // ---- landmarks with >= 2 usable observations (opt.cpp:158-171, 438-453), observations of this rank's landmarks ----
   std::vector<int> lm_compact(p->L > 0 ? p->L : 0, -1);
   E.lm_of_compact.clear();
@@ -1485,7 +1497,6 @@ int engine_setup(Engine& E, const cvb_ba_problem* p, const cvb_ba_options* o) {
 
   lap("factor lists");
   // ---- uploads ----
-  int rc;
   E.h_const.assign(p->pose_const, p->pose_const + K);
   if ((rc = upload(E, E.pose[0], p->pose, (size_t)7 * K))) return rc;
   if ((rc = zalloc(E, E.pose[1], (size_t)7 * K))) return rc;
@@ -2085,6 +2096,117 @@ int engine_download(Engine& E, const cvb_ba_problem* p, cvb_ba_result* r) {
   return CVB_OK;
 }
 
+// Peer access for the multi-GPU path: every rank maps the packed S, tile inverses and panel flags of every other rank
+// (map_peers: the source of the peers' pointers, which reports through *opened whether this rank mapped them all), the
+// ranks agree through the installed collective that all of them did, and from then on the reduced camera system is
+// reduce-scattered by peer pull and the factorisation is distributed by tile columns.  unmap undoes map_peers when some
+// rank failed.
+int enable_p2p(Engine& E, bool ipc, const std::function<int(cvb_chol::DistView&, bool*)>& map_peers,
+               const std::function<void(cvb_chol::DistView&)>& unmap) {
+  if (E.world <= 1) return CVB_OK;
+  if (E.p2p) return CVB_OK;
+  if (!E.allreduce) return cvb_fail(E.ctx, CVB_ERR_INVALID, "cvb_ba_enable_p2p: install the all-reduce first (cvb_ba_set_allreduce)");
+  if (E.world > 16) return cvb_fail(E.ctx, CVB_ERR_UNSUPPORTED, "peer path supports up to 16 ranks");
+  if (E.g_factor) return cvb_fail(E.ctx, CVB_ERR_INVALID, "cvb_ba_enable_p2p must precede the first iterations");
+  cvb_chol::DistView dv;
+  dv.rank = E.rank; dv.world = E.world;
+  dv.peer_S[E.rank] = E.S_raw; dv.peer_linv[E.rank] = E.linv_raw; dv.peer_flag[E.rank] = E.pflag_raw;
+  bool opened = false;
+  int rc;
+  if ((rc = map_peers(dv, &opened))) return rc;
+  // everybody must have mapped everybody: min over ranks via the sum of (1 - opened)
+  {
+    DevArr<double> d_ok;
+    std::vector<double> v(1, opened ? 0.0 : 1.0);
+    if ((rc = upload(E, d_ok, v))) return rc;
+    if ((rc = ar(E, d_ok.p, 1))) return rc;
+    ENG_CUDA(cudaMemcpyAsync(v.data(), d_ok.p, sizeof(double), cudaMemcpyDeviceToHost, E.st));
+    ENG_CUDA(cudaStreamSynchronize(E.st));
+    d_ok.free_();
+    if (v[0] != 0.0) {
+      unmap(dv);
+      return cvb_fail(E.ctx, CVB_ERR_UNSUPPORTED, "peer mapping is not available between all ranks (all-reduce fallback stays in use)");
+    }
+  }
+  ENG_CUDA(cudaMalloc(&dv.d_epoch, sizeof(int)));
+  ENG_CUDA(cudaMemsetAsync(dv.d_epoch, 0, sizeof(int), E.st));
+  ENG_CUDA(cudaMalloc(&dv.d_peer_flag, sizeof(int*) * 16));
+  ENG_CUDA(cudaMemcpyAsync(dv.d_peer_flag, dv.peer_flag, sizeof(int*) * 16, cudaMemcpyHostToDevice, E.st));
+  ENG_CUDA(cudaMalloc(&E.d_peer_S, sizeof(double*) * 16));
+  ENG_CUDA(cudaMemcpyAsync(E.d_peer_S, dv.peer_S, sizeof(double*) * 16, cudaMemcpyHostToDevice, E.st));
+  ENG_CUDA(cudaStreamSynchronize(E.st));
+  // distributed plan: same structure, pair lists restricted to the tile columns this rank owns
+  E.plan.build(E.plan.nt, E.h_prefill, E.plan.h_col_group, &E.h_owner, E.rank);
+  if ((rc = E.plan.upload(E.ctx, E.st))) return rc;
+  E.dv = dv;
+  E.p2p = true;
+  E.peer_ipc = ipc;
+  return CVB_OK;
+}
+
+// The peers' pointers through CUDA IPC (one process per GPU on one NVLink node): every rank exports its three buffers and
+// gathers every rank's handles with the installed collective (each rank writes its bytes into its slot of a zeroed table,
+// the SUM all-reduce is the all-gather), then opens them.
+int enable_p2p_ipc(Engine& E) {
+  const auto close = [&E](cvb_chol::DistView& dv) {
+    for (int g = 0; g < E.world; g++) {
+      if (g == E.rank) continue;
+      if (dv.peer_S[g]) cudaIpcCloseMemHandle(dv.peer_S[g]);
+      if (dv.peer_linv[g]) cudaIpcCloseMemHandle(dv.peer_linv[g]);
+      if (dv.peer_flag[g]) cudaIpcCloseMemHandle(dv.peer_flag[g]);
+    }
+  };
+  const auto map_peers = [&E](cvb_chol::DistView& dv, bool* opened) {
+    constexpr int HB = (int)sizeof(cudaIpcMemHandle_t);   // 64
+    const int per_rank = 3 * HB + 1;                     // three handles + an "ok" byte
+    std::vector<double> table((size_t)E.world * per_rank, 0.0);
+    cudaIpcMemHandle_t hs[3];
+    bool ok = cudaIpcGetMemHandle(&hs[0], E.S_raw) == cudaSuccess && cudaIpcGetMemHandle(&hs[1], E.linv_raw) == cudaSuccess &&
+              cudaIpcGetMemHandle(&hs[2], E.pflag_raw) == cudaSuccess;
+    cudaGetLastError();
+    for (int q = 0; q < 3 && ok; q++)
+      for (int b = 0; b < HB; b++) table[(size_t)E.rank * per_rank + q * HB + b] = (double)reinterpret_cast<unsigned char*>(&hs[q])[b];
+    table[(size_t)E.rank * per_rank + 3 * HB] = ok ? 1.0 : 0.0;
+    DevArr<double> d_table;
+    int rc;
+    if ((rc = upload(E, d_table, table))) return rc;
+    if ((rc = ar(E, d_table.p, table.size()))) return rc;
+    ENG_CUDA(cudaMemcpyAsync(table.data(), d_table.p, table.size() * sizeof(double), cudaMemcpyDeviceToHost, E.st));
+    ENG_CUDA(cudaStreamSynchronize(E.st));
+    d_table.free_();
+    for (int g = 0; g < E.world; g++) ok = ok && table[(size_t)g * per_rank + 3 * HB] == 1.0;
+    *opened = ok;
+    for (int g = 0; g < E.world && ok; g++) {
+      if (g == E.rank) continue;
+      cudaIpcMemHandle_t ph[3];
+      for (int q = 0; q < 3; q++)
+        for (int b = 0; b < HB; b++) reinterpret_cast<unsigned char*>(&ph[q])[b] = (unsigned char)table[(size_t)g * per_rank + q * HB + b];
+      void* ptr[3] = {nullptr, nullptr, nullptr};
+      for (int q = 0; q < 3; q++)
+        if (cudaIpcOpenMemHandle(&ptr[q], ph[q], cudaIpcMemLazyEnablePeerAccess) != cudaSuccess) { *opened = false; cudaGetLastError(); }
+      dv.peer_S[g] = (double*)ptr[0]; dv.peer_linv[g] = (double*)ptr[1]; dv.peer_flag[g] = (int*)ptr[2];
+    }
+    return (int)CVB_OK;
+  };
+  return enable_p2p(E, true, map_peers, close);
+}
+
+// The peers' pointers from an in-process group (cvb_group_create enabled peer access between the ranks' devices).
+int enable_p2p_group(Engine& E, cvb_group* g, int rank) {
+  const auto map_peers = [&E, g, rank](cvb_chol::DistView& dv, bool* opened) {
+    const void* mine[3] = {E.S_raw, E.linv_raw, E.pflag_raw};
+    const void* all[3 * CVB_GROUP_MAX];
+    int rc = cvb_grp::exchange(g, rank, mine, 3, all);
+    if (rc) return cvb_fail(E.ctx, rc, "peer pointer exchange failed (group failed)");
+    for (int q = 0; q < E.world; q++) {
+      dv.peer_S[q] = (double*)all[3 * q]; dv.peer_linv[q] = (double*)all[3 * q + 1]; dv.peer_flag[q] = (int*)all[3 * q + 2];
+    }
+    *opened = true;
+    return (int)CVB_OK;
+  };
+  return enable_p2p(E, false, map_peers, [](cvb_chol::DistView&) {});
+}
+
 }  // namespace
 
 // =================================================================================================
@@ -2136,82 +2258,10 @@ int cvb_ba_set_allreduce(cvb_ba* h, cvb_allreduce_fn fn, void* user) {
   return CVB_OK;
 }
 
-// Peer access for the multi-GPU path (one process per GPU on one NVLink node): exports this rank's packed S, tile
-// inverses and panel flags through CUDA IPC, gathers every rank's handles with the installed collective (each rank writes
-// its bytes into its slot of a zeroed table, the SUM all-reduce is the all-gather) and maps the peers' buffers.  From then
-// on the reduced camera system is reduce-scattered by peer pull and the factorisation is distributed by tile columns.
 int cvb_ba_enable_p2p(cvb_ba* h) {
   if (!h) return CVB_ERR_INVALID;
   BaEnter enter(h);
-  Engine& E = h->E;
-  if (E.world <= 1) return CVB_OK;
-  if (E.p2p) return CVB_OK;
-  if (!E.allreduce) return cvb_fail(E.ctx, CVB_ERR_INVALID, "cvb_ba_enable_p2p: install the all-reduce first (cvb_ba_set_allreduce)");
-  if (E.world > 16) return cvb_fail(E.ctx, CVB_ERR_UNSUPPORTED, "peer path supports up to 16 ranks");
-  if (E.g_factor) return cvb_fail(E.ctx, CVB_ERR_INVALID, "cvb_ba_enable_p2p must precede the first iterations");
-  constexpr int HB = (int)sizeof(cudaIpcMemHandle_t);   // 64
-  const int per_rank = 3 * HB + 1;                     // three handles + an "ok" byte
-  std::vector<double> table((size_t)E.world * per_rank, 0.0);
-  cudaIpcMemHandle_t hs[3];
-  bool ok = cudaIpcGetMemHandle(&hs[0], E.S_raw) == cudaSuccess && cudaIpcGetMemHandle(&hs[1], E.linv_raw) == cudaSuccess &&
-            cudaIpcGetMemHandle(&hs[2], E.pflag_raw) == cudaSuccess;
-  cudaGetLastError();
-  for (int q = 0; q < 3 && ok; q++)
-    for (int b = 0; b < HB; b++) table[(size_t)E.rank * per_rank + q * HB + b] = (double)reinterpret_cast<unsigned char*>(&hs[q])[b];
-  table[(size_t)E.rank * per_rank + 3 * HB] = ok ? 1.0 : 0.0;
-  DevArr<double> d_table;
-  int rc;
-  if ((rc = upload(E, d_table, table))) return rc;
-  if ((rc = ar(E, d_table.p, table.size()))) return rc;
-  ENG_CUDA(cudaMemcpyAsync(table.data(), d_table.p, table.size() * sizeof(double), cudaMemcpyDeviceToHost, E.st));
-  ENG_CUDA(cudaStreamSynchronize(E.st));
-  d_table.free_();
-  for (int g = 0; g < E.world; g++) ok = ok && table[(size_t)g * per_rank + 3 * HB] == 1.0;
-  cvb_chol::DistView dv;
-  dv.rank = E.rank; dv.world = E.world;
-  double opened = ok ? 1.0 : 0.0;
-  for (int g = 0; g < E.world && ok; g++) {
-    if (g == E.rank) { dv.peer_S[g] = E.S_raw; dv.peer_linv[g] = E.linv_raw; dv.peer_flag[g] = E.pflag_raw; continue; }
-    cudaIpcMemHandle_t ph[3];
-    for (int q = 0; q < 3; q++)
-      for (int b = 0; b < HB; b++) reinterpret_cast<unsigned char*>(&ph[q])[b] = (unsigned char)table[(size_t)g * per_rank + q * HB + b];
-    void* ptr[3] = {nullptr, nullptr, nullptr};
-    for (int q = 0; q < 3; q++)
-      if (cudaIpcOpenMemHandle(&ptr[q], ph[q], cudaIpcMemLazyEnablePeerAccess) != cudaSuccess) { opened = 0.0; cudaGetLastError(); }
-    dv.peer_S[g] = (double*)ptr[0]; dv.peer_linv[g] = (double*)ptr[1]; dv.peer_flag[g] = (int*)ptr[2];
-  }
-  // everybody must have mapped everybody: min over ranks via the sum of (1 - opened)
-  {
-    DevArr<double> d_ok;
-    std::vector<double> v(1, 1.0 - opened);
-    if ((rc = upload(E, d_ok, v))) return rc;
-    if ((rc = ar(E, d_ok.p, 1))) return rc;
-    ENG_CUDA(cudaMemcpyAsync(v.data(), d_ok.p, sizeof(double), cudaMemcpyDeviceToHost, E.st));
-    ENG_CUDA(cudaStreamSynchronize(E.st));
-    d_ok.free_();
-    if (v[0] != 0.0) {
-      for (int g = 0; g < E.world; g++) {
-        if (g == E.rank) continue;
-        if (dv.peer_S[g]) cudaIpcCloseMemHandle(dv.peer_S[g]);
-        if (dv.peer_linv[g]) cudaIpcCloseMemHandle(dv.peer_linv[g]);
-        if (dv.peer_flag[g]) cudaIpcCloseMemHandle(dv.peer_flag[g]);
-      }
-      return cvb_fail(E.ctx, CVB_ERR_UNSUPPORTED, "CUDA IPC peer mapping is not available between all ranks (all-reduce fallback stays in use)");
-    }
-  }
-  ENG_CUDA(cudaMalloc(&dv.d_epoch, sizeof(int)));
-  ENG_CUDA(cudaMemsetAsync(dv.d_epoch, 0, sizeof(int), E.st));
-  ENG_CUDA(cudaMalloc(&dv.d_peer_flag, sizeof(int*) * 16));
-  ENG_CUDA(cudaMemcpyAsync(dv.d_peer_flag, dv.peer_flag, sizeof(int*) * 16, cudaMemcpyHostToDevice, E.st));
-  ENG_CUDA(cudaMalloc(&E.d_peer_S, sizeof(double*) * 16));
-  ENG_CUDA(cudaMemcpyAsync(E.d_peer_S, dv.peer_S, sizeof(double*) * 16, cudaMemcpyHostToDevice, E.st));
-  ENG_CUDA(cudaStreamSynchronize(E.st));
-  // distributed plan: same structure, pair lists restricted to the tile columns this rank owns
-  E.plan.build(E.plan.nt, E.h_prefill, E.plan.h_col_group, &E.h_owner, E.rank);
-  if ((rc = E.plan.upload(E.ctx, E.st))) return rc;
-  E.dv = dv;
-  E.p2p = true;
-  return CVB_OK;
+  return enable_p2p_ipc(h->E);
 }
 
 // Back to the state the problem was created with (the preintegrations were propagated at those biases), then iteration 0
@@ -2311,12 +2361,16 @@ int cvb_ba_solve(cvb_ctx* ctx, const cvb_ba_problem* p, const cvb_ba_options* o,
   return rc;
 }
 
-// Optimization::GlobalBundleAdjustment (optimization_be.cpp:56-618) on the flat problem: round 1 (5 iterations, loop
-// edges without loss) + outlier purge on the loss-corrected residual norms (:270-290), round 2 from the ORIGINAL
-// state (the reference re-reads the map at :325,454-457; round 1 only removes observations) with Cauchy(1) on loops.
-int cvb_gba(cvb_ctx* ctx, const cvb_ba_problem* p, const cvb_gba_options* g, cvb_ba_result* r, uint8_t* obs_removed) {
-  if (!ctx || !p || !g || !r) return CVB_ERR_INVALID;
-  CVB_GUARD(ctx);
+}  // extern "C"
+
+namespace {
+
+// The two rounds of Optimization::GlobalBundleAdjustment (optimization_be.cpp:56-618) on the flat problem, around two
+// solvers: round1(p1, o, norms) runs round 1 (5 iterations, loop edges without loss) and writes the loss-corrected
+// residual norm of every observation; round2(p2, o) is round 2 from the ORIGINAL state (the reference re-reads the map at
+// :325,454-457; round 1 only removes observations) with Cauchy(1) on loops, after the outlier purge of :270-290.
+template <class Round1, class Round2>
+int gba_rounds(const cvb_ba_problem* p, const cvb_gba_options* g, uint8_t* obs_removed, Round1 round1, Round2 round2) {
   std::vector<uint8_t> skip(p->n_obs > 0 ? p->n_obs : 1, 0), rb0(p->n_edge > 0 ? p->n_edge : 1, 0), rb1(p->n_edge > 0 ? p->n_edge : 1, 1);
   if (p->obs_skip) std::memcpy(skip.data(), p->obs_skip, (size_t)p->n_obs);
   cvb_ba_options o{};
@@ -2329,13 +2383,8 @@ int cvb_gba(cvb_ctx* ctx, const cvb_ba_problem* p, const cvb_gba_options* g, cvb
     cvb_ba_problem p1 = *p;
     p1.edge_robust = rb0.data();   // round 1: loop edges without loss (optimization_be.cpp:253)
     o.max_iterations = 5;          // :261
-    cvb_ba* h = nullptr;
-    if ((rc = cvb_ba_create(ctx, &p1, &o, &h))) return rc;
-    rc = cvb_ba_iterate(h, o.max_iterations, nullptr);
     std::vector<double> norms(p->n_obs > 0 ? p->n_obs : 1);
-    if (!rc) rc = cvb_ba_reproj_norms(h, norms.data(), p->n_obs);
-    cvb_ba_destroy(h);
-    if (rc) return rc;
+    if ((rc = round1(&p1, &o, norms.data()))) return rc;
     for (int i = 0; i < p->n_obs; i++)
       if (norms[i] > g->th_outlier) skip[i] = 1;   // th_gba_outlier_global, :277-281
   }
@@ -2345,7 +2394,163 @@ int cvb_gba(cvb_ctx* ctx, const cvb_ba_problem* p, const cvb_gba_options* g, cvb
   p2.obs_skip = skip.data();
   p2.edge_robust = rb1.data();     // round 2: loss_function on the loop edges (:555)
   o.max_iterations = g->iterations_limit;
-  return cvb_ba_solve(ctx, &p2, &o, r);
+  return round2(&p2, &o);
+}
+
+// One sharded solve over an in-process group: one host thread per rank runs create -> group all-reduce -> [peer path] ->
+// restart -> iterate on its context; then (after every rank's stream is idle) each rank's handle goes to done(rank, h)
+// and is destroyed.  The handles outlive the rank threads so that no rank frees buffers a peer may still read.
+int group_solve(cvb_group* g, const cvb_ba_problem* p, const cvb_ba_options* o_in, int peer_path,
+                const std::function<int(int, cvb_ba*)>& done) {
+  const int n = g->n;
+  std::vector<cvb_ba*> h(n, nullptr);
+  int rc = cvb_grp::run(g, [&](int r) {
+    cvb_ba_options o = *o_in;
+    o.rank = r;
+    o.world = n;
+    int rr = cvb_ba_create(g->ctx[r], p, &o, &h[r]);
+    if (!rr) rr = cvb_ba_set_allreduce(h[r], cvb_grp::allreduce, &g->bind[r]);
+    if (!rr && peer_path && n > 1) {
+      BaEnter enter(h[r]);
+      rr = enable_p2p_group(h[r]->E, g, r);
+    }
+    if (!rr) rr = cvb_ba_restart(h[r]);
+    if (!rr) rr = cvb_ba_iterate(h[r], o.max_iterations, nullptr);
+    return rr;
+  });
+  for (int r = 0; r < n; r++)
+    if (h[r]) {
+      BaEnter enter(h[r]);
+      cudaStreamSynchronize(h[r]->E.st);
+    }
+  for (int r = 0; r < n && !rc; r++) {
+    rc = done(r, h[r]);
+    if (rc && r) cvb_fail(g->ctx[0], rc, "rank %d: %s", r, g->ctx[r]->err.c_str());
+  }
+  for (int r = 0; r < n; r++) cvb_ba_destroy(h[r]);
+  return rc;
+}
+
+// every rank's result of a group solve, merged: rank 0's trajectory (checked bitwise against every other rank's), each
+// landmark from its owner
+int group_solve_merged(cvb_group* g, const cvb_ba_problem* p, const cvb_ba_options* o, int peer_path, cvb_ba_result* r,
+                       const std::function<int(int, cvb_ba*)>& extra = nullptr) {
+  const int n = g->n, K = p->K, L = p->L;
+  const int cap = std::max(o->max_iterations, 0) + 2;   // iteration 0 + one cost per iteration
+  struct Out {
+    std::vector<double> pose, sb, lm, hist;
+    std::vector<int32_t> owner;
+    std::vector<uint8_t> steps;
+    cvb_ba_result res{};
+  };
+  std::vector<Out> out(n);
+  int rc = group_solve(g, p, o, peer_path, [&](int q, cvb_ba* h) {
+    Out& x = out[q];
+    x.pose.resize(7 * (size_t)K); x.sb.resize(9 * (size_t)K); x.lm.resize(3 * (size_t)std::max(L, 1)); x.hist.resize(cap);
+    x.owner.resize(std::max(L, 1)); x.steps.resize(cap);
+    x.res.pose = x.pose.data(); x.res.speedbias = x.sb.data(); x.res.lm = x.lm.data(); x.res.lm_owner = x.owner.data();
+    x.res.cost_history = x.hist.data(); x.res.step_status = x.steps.data(); x.res.cost_history_cap = cap;
+    int rr = cvb_ba_result_get(h, p, &x.res);
+    if (!rr && extra) rr = extra(q, h);
+    return rr;
+  });
+  if (rc) return rc;
+  const Out& a = out[0];
+  for (int q = 1; q < n; q++) {
+    const Out& b = out[q];
+    const bool same = a.res.n_cost_history == b.res.n_cost_history && a.res.iterations == b.res.iterations &&
+                      a.res.termination == b.res.termination && a.pose == b.pose && a.sb == b.sb &&
+                      std::memcmp(a.hist.data(), b.hist.data(), sizeof(double) * a.res.n_cost_history) == 0 &&
+                      std::memcmp(a.steps.data(), b.steps.data(), (size_t)std::max(a.res.n_cost_history - 1, 0)) == 0;
+    if (!same) return cvb_fail(g->ctx[0], CVB_ERR_NUMERIC, "rank %d's poses, speed-biases or cost history differ from rank 0's", q);
+  }
+  if (r->pose) std::memcpy(r->pose, a.pose.data(), sizeof(double) * 7 * (size_t)K);
+  if (r->speedbias) std::memcpy(r->speedbias, a.sb.data(), sizeof(double) * 9 * (size_t)K);
+  for (int l = 0; l < L; l++) {
+    const int w = a.owner[l];
+    if (r->lm) std::memcpy(r->lm + 3 * (size_t)l, (w >= 0 ? out[w].lm.data() : a.lm.data()) + 3 * (size_t)l, 3 * sizeof(double));
+    if (r->lm_owner) r->lm_owner[l] = w;
+  }
+  r->iterations = a.res.iterations;
+  r->termination = a.res.termination;
+  r->initial_cost = a.res.initial_cost;
+  r->final_cost = a.res.final_cost;
+  r->n_cost_history = 0;
+  if (r->cost_history && r->cost_history_cap > 0) {
+    r->n_cost_history = std::min(r->cost_history_cap, a.res.n_cost_history);
+    std::memcpy(r->cost_history, a.hist.data(), sizeof(double) * r->n_cost_history);
+  }
+  if (r->step_status && r->cost_history_cap > 0)
+    std::memcpy(r->step_status, a.steps.data(), (size_t)std::min(r->cost_history_cap, std::max(a.res.n_cost_history - 1, 0)));
+  return CVB_OK;
+}
+
+int group_check(cvb_group* g, const cvb_ba_problem* p, int visual_only, const void* o, const cvb_ba_result* r, int peer_path) {
+  if (!g) return CVB_ERR_INVALID;
+  if (!p || !o || !r) return cvb_fail(g->ctx[0], CVB_ERR_INVALID, "NULL problem, options or result");
+  // The peer path needs a device per rank.  With two ranks on one device it stalled past the 20 s panel-wait bound (C1) and
+  // once ended away from the world = 1 solve without reporting a failure (DESIGN.md §6), so it is refused there.
+  if (peer_path)
+    for (int a = 0; a < g->n; a++)
+      for (int b = 0; b < a; b++)
+        if (g->ctx[a]->device == g->ctx[b]->device)
+          return cvb_fail(g->ctx[0], CVB_ERR_UNSUPPORTED, "peer path needs a device per rank: ranks %d and %d share device %d", b, a,
+                          g->ctx[a]->device);
+  return check_problem(g->ctx[0], p, visual_only);
+}
+
+}  // namespace
+
+extern "C" {
+
+int cvb_gba(cvb_ctx* ctx, const cvb_ba_problem* p, const cvb_gba_options* g, cvb_ba_result* r, uint8_t* obs_removed) {
+  if (!ctx || !p || !g || !r) return CVB_ERR_INVALID;
+  CVB_GUARD(ctx);
+  const auto round1 = [ctx, p](const cvb_ba_problem* p1, const cvb_ba_options* o, double* norms) {
+    cvb_ba* h = nullptr;
+    int rc = cvb_ba_create(ctx, p1, o, &h);
+    if (rc) return rc;
+    rc = cvb_ba_iterate(h, o->max_iterations, nullptr);
+    if (!rc) rc = cvb_ba_reproj_norms(h, norms, p->n_obs);
+    cvb_ba_destroy(h);
+    return rc;
+  };
+  const auto round2 = [ctx, r](const cvb_ba_problem* p2, const cvb_ba_options* o) { return cvb_ba_solve(ctx, p2, o, r); };
+  return gba_rounds(p, g, obs_removed, round1, round2);
+}
+
+int cvb_ba_solve_group(cvb_group* g, const cvb_ba_problem* p, const cvb_ba_options* o, int peer_path, cvb_ba_result* r) {
+  if (!g) return CVB_ERR_INVALID;
+  std::lock_guard<std::recursive_mutex> call_lk(g->call_mtx);   // the engines outlive the rank threads (group_solve)
+  int rc = group_check(g, p, o ? o->visual_only : 0, o, r, peer_path);
+  if (rc) return rc;
+  return group_solve_merged(g, p, o, peer_path, r);
+}
+
+int cvb_gba_group(cvb_group* g, const cvb_ba_problem* p, const cvb_gba_options* gba, int peer_path, cvb_ba_result* r,
+                  uint8_t* obs_removed) {
+  if (!g) return CVB_ERR_INVALID;
+  std::lock_guard<std::recursive_mutex> call_lk(g->call_mtx);
+  int rc = group_check(g, p, gba ? gba->visual_only : 0, gba, r, peer_path);
+  if (rc) return rc;
+  const auto round1 = [g, p, peer_path](const cvb_ba_problem* p1, const cvb_ba_options* o, double* norms) {
+    // each observation's norm from the rank that owns its landmark (the others report -1 for it)
+    std::vector<std::vector<double>> per(g->n, std::vector<double>(p->n_obs > 0 ? p->n_obs : 1));
+    cvb_ba_result r1{};
+    int rc = group_solve_merged(g, p1, o, peer_path, &r1,
+                                [&](int q, cvb_ba* h) { return cvb_ba_reproj_norms(h, per[q].data(), p->n_obs); });
+    if (rc) return rc;
+    for (int i = 0; i < p->n_obs; i++) {
+      norms[i] = -1.0;
+      for (int q = 0; q < g->n; q++)
+        if (per[q][i] != -1.0) norms[i] = per[q][i];
+    }
+    return (int)CVB_OK;
+  };
+  const auto round2 = [g, r, peer_path](const cvb_ba_problem* p2, const cvb_ba_options* o) {
+    return group_solve_merged(g, p2, o, peer_path, r);
+  };
+  return gba_rounds(p, gba, obs_removed, round1, round2);
 }
 
 }  // extern "C"

@@ -1158,16 +1158,19 @@ __global__ void wait_panel_kernel(const int* __restrict__ flag, const int* __res
 int factor(cvb_ctx* ctx, double* S, double* linv, int* d_flag, const TilePlan& plan, cudaStream_t st,
            const FactorStreams& fs, const DistView* dv) {
   static cvb_once_per_device once;
-  if (once.first(ctx->device)) {
-    CVB_CUDA(ctx, cudaFuncSetAttribute(trsm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kTrsmSmem));
-    CVB_CUDA(ctx, cudaFuncSetAttribute(syrk_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSyrkSmem));
-    CVB_CUDA(ctx, cudaFuncSetAttribute(tile_update_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kTileSmem));
-    CVB_CUDA(ctx, cudaFuncSetAttribute(potrf_inv_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kPotrfSmem));
-    CVB_CUDA(ctx, cudaFuncSetAttribute(chain_gemm_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kChainSmem));
-    CVB_CUDA(ctx, cudaFuncSetAttribute(chain_gemm_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kChainSmem));
-    CVB_CUDA(ctx, cudaFuncSetAttribute(trsm_level_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kTrsmSmem));
-    CVB_CUDA(ctx, cudaFuncSetAttribute(tile_update_level_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kTileSmem));
-    CVB_CUDA(ctx, cudaFuncSetAttribute(potrf_inv_level_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kPotrfSmem));
+  {
+    std::lock_guard<std::mutex> once_lk(once.mtx);
+    if (once.first(ctx->device)) {
+      CVB_CUDA(ctx, cudaFuncSetAttribute(trsm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kTrsmSmem));
+      CVB_CUDA(ctx, cudaFuncSetAttribute(syrk_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSyrkSmem));
+      CVB_CUDA(ctx, cudaFuncSetAttribute(tile_update_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kTileSmem));
+      CVB_CUDA(ctx, cudaFuncSetAttribute(potrf_inv_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kPotrfSmem));
+      CVB_CUDA(ctx, cudaFuncSetAttribute(chain_gemm_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kChainSmem));
+      CVB_CUDA(ctx, cudaFuncSetAttribute(chain_gemm_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kChainSmem));
+      CVB_CUDA(ctx, cudaFuncSetAttribute(trsm_level_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kTrsmSmem));
+      CVB_CUDA(ctx, cudaFuncSetAttribute(tile_update_level_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kTileSmem));
+      CVB_CUDA(ctx, cudaFuncSetAttribute(potrf_inv_level_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kPotrfSmem));
+    }
   }
   const int nt = plan.nt;
   const bool dist = dv != nullptr && dv->world > 1 && !plan.h_owner.empty();
@@ -1473,9 +1476,12 @@ int factor(cvb_ctx* ctx, double* S, double* linv, int* d_flag, const TilePlan& p
 int solve_grid(cvb_ctx* ctx, const double* L, const double* linv, const double* b, double* tmp, double* x,
                const TilePlan& plan, cudaStream_t st, const FactorStreams& fs, int grid) {
   static cvb_once_per_device once;
-  if (once.first(ctx->device)) {
-    CVB_CUDA(ctx, cudaFuncSetAttribute(subst_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSolveSmem));
-    CVB_CUDA(ctx, cudaFuncSetAttribute(subst_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSolveSmem));
+  {
+    std::lock_guard<std::mutex> once_lk(once.mtx);
+    if (once.first(ctx->device)) {
+      CVB_CUDA(ctx, cudaFuncSetAttribute(subst_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSolveSmem));
+      CVB_CUDA(ctx, cudaFuncSetAttribute(subst_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSolveSmem));
+    }
   }
   const int nt = plan.nt;
   CVB_REQUIRE(ctx, plan.d_rowc_ptr != nullptr && plan.d_col_ptr != nullptr, "tile plan not built / uploaded");

@@ -35,7 +35,11 @@ struct cvb_ctx {
 
 // cudaFuncSetAttribute applies to the CURRENT device: one flag per (call site, device), so that a process that opens contexts
 // on several GPUs raises the dynamic shared-memory limit on each of them
+// Call sites hold `mtx` around first() and the attribute set-up, so that a concurrent first call on the
+// same device (several contexts of one device driven from their own threads) waits until the attributes are set instead of
+// launching before them.
 struct cvb_once_per_device {
+  std::mutex mtx;
   std::atomic<bool> done[64];
   cvb_once_per_device() { for (auto& d : done) d.store(false); }
   bool first(int device) {

@@ -63,6 +63,36 @@ class Context {
 };
 
 // ---------------------------------------------------------------------------------------------------------------
+// Several GPUs from one process: one Context per rank and the cvb_group over them (cvb_group_create).  Ranks may share a
+// device.  The server builds one at start-up over its GPUs and hands it to the GlobalBundleAdjustment overload below.
+// ---------------------------------------------------------------------------------------------------------------
+class ContextGroup {
+ public:
+  explicit ContextGroup(const std::vector<int>& devices) {
+    std::vector<cvb_ctx*> raw;
+    for (int d : devices) {
+      ctxs_.push_back(std::make_unique<Context>(d));
+      raw.push_back(ctxs_.back()->get());
+    }
+    if (raw.empty()) throw std::runtime_error("covins_b200: a context group needs at least one device");
+    const int rc = cvb_group_create(raw.data(), (int)raw.size(), &g_);
+    if (rc != CVB_OK)
+      throw std::runtime_error(std::string("covins_b200: cvb_group_create failed: ") + cvb_last_error(raw[0]));
+  }
+  ~ContextGroup() { cvb_group_destroy(g_); }
+  ContextGroup(const ContextGroup&) = delete;
+  ContextGroup& operator=(const ContextGroup&) = delete;
+  cvb_group* get() const { return g_; }
+  int size() const { return (int)ctxs_.size(); }
+  Context& rank(int r) { return *ctxs_[r]; }   // rank 0's context carries the group calls' error messages
+  void check(int rc, const char* what) const { ctxs_[0]->check(rc, what); }
+
+ private:
+  std::vector<std::unique_ptr<Context>> ctxs_;
+  cvb_group* g_ = nullptr;
+};
+
+// ---------------------------------------------------------------------------------------------------------------
 // Adapter: the only place that touches third-party types of the real containers.  Default = mock containers.
 // ---------------------------------------------------------------------------------------------------------------
 template <class KF>
@@ -281,12 +311,12 @@ struct OptParams {
   int matches_thres = 25, matches_thres_merge = 25;     // placerec (placerec_gen_be.cpp:118-121)
 };
 
-// ---------------------------------------------------------------------------------------------------------------
-// Optimization::GlobalBundleAdjustment — same signature meaning as optimization_be.hpp:38-40.
-// ---------------------------------------------------------------------------------------------------------------
-template <class MapPtr>
-void GlobalBundleAdjustment(Context& ctx, MapPtr map, int interations_limit, double /*time_limit*/, bool visual_only = false,
-                            bool outlier_removal = true, bool /*estimate_bias*/ = false, const OptParams& P = OptParams()) {
+namespace detail {
+// Optimization::GlobalBundleAdjustment's flatten and write-back around one solver call:
+// solve(problem, gba options, result, obs_removed) -> cvb_status (cvb_gba on one context, cvb_gba_group on a group).
+template <class MapPtr, class Solve>
+void global_bundle_adjustment(MapPtr map, int interations_limit, bool visual_only, bool outlier_removal, const OptParams& P,
+                              Solve solve) {
   using KeyframePtr = typename std::decay<decltype(map->GetKeyframesVec()[0])>::type;
   using KF = typename KeyframePtr::element_type;
   using Transform = typename std::decay<decltype(map->GetKeyframesVec()[0]->GetPoseTws())>::type;
@@ -387,7 +417,7 @@ void GlobalBundleAdjustment(Context& ctx, MapPtr map, int interations_limit, dou
   cvb_ba_result res{};
   res.pose = o_pose.data(); res.speedbias = o_sb.data(); res.lm = o_lm.data(); res.lm_owner = owner.data();
   cvb_gba_options g{interations_limit, visual_only ? 1 : 0, outlier_removal ? 1 : 0, P.th_gba_outlier_global};
-  ctx.check(cvb_gba(ctx.get(), &prob, &g, &res, removed.data()), "cvb_gba");
+  solve(&prob, &g, &res, removed.data());
 
   // round-1 outlier purge, written into the map exactly like optimization_be.cpp:282-288
   size_t num_bad = 0;
@@ -421,6 +451,32 @@ void GlobalBundleAdjustment(Context& ctx, MapPtr map, int interations_limit, dou
   std::printf("--> Clean Map\n");
   map->Clean();                                                                                     // :614
   std::printf("--> done.\n+++ GBA: End +++\n");
+}
+}  // namespace detail
+
+// ---------------------------------------------------------------------------------------------------------------
+// Optimization::GlobalBundleAdjustment — same signature meaning as optimization_be.hpp:38-40.
+// ---------------------------------------------------------------------------------------------------------------
+template <class MapPtr>
+void GlobalBundleAdjustment(Context& ctx, MapPtr map, int interations_limit, double /*time_limit*/, bool visual_only = false,
+                            bool outlier_removal = true, bool /*estimate_bias*/ = false, const OptParams& P = OptParams()) {
+  detail::global_bundle_adjustment(map, interations_limit, visual_only, outlier_removal, P,
+                                   [&ctx](const cvb_ba_problem* p, const cvb_gba_options* g, cvb_ba_result* r, uint8_t* removed) {
+                                     ctx.check(cvb_gba(ctx.get(), p, g, r, removed), "cvb_gba");
+                                   });
+}
+
+// The same, with the merged map's landmarks sharded over the ranks of a ContextGroup (cvb_gba_group).  peer_path: reduce-scatter
+// by peer pull and the column-distributed factorisation (a device per rank; not yet verified on several devices, so off by
+// default), else the all-reduce of the packed reduced system.
+template <class MapPtr>
+void GlobalBundleAdjustment(ContextGroup& group, MapPtr map, int interations_limit, double /*time_limit*/, bool visual_only = false,
+                            bool outlier_removal = true, bool /*estimate_bias*/ = false, const OptParams& P = OptParams(),
+                            bool peer_path = false) {
+  detail::global_bundle_adjustment(map, interations_limit, visual_only, outlier_removal, P,
+                                   [&group, peer_path](const cvb_ba_problem* p, const cvb_gba_options* g, cvb_ba_result* r, uint8_t* removed) {
+                                     group.check(cvb_gba_group(group.get(), p, g, peer_path ? 1 : 0, r, removed), "cvb_gba_group");
+                                   });
 }
 
 // ---------------------------------------------------------------------------------------------------------------

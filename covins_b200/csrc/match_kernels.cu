@@ -590,9 +590,12 @@ template <class M, int QPT, int K, int MODE>
 int launch_scan(cvb_ctx* ctx, const ScanParams& sp, const Plan& pl, cudaStream_t st) {
   static cvb_once_per_device once;
   const size_t smem = scan_smem_bytes<M>();
-  if (once.first(ctx->device)) {
-    CVB_CUDA(ctx, cudaFuncSetAttribute(scan_kernel<M, QPT, K, MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                       (int)smem));
+  {
+    std::lock_guard<std::mutex> once_lk(once.mtx);
+    if (once.first(ctx->device)) {
+      CVB_CUDA(ctx, cudaFuncSetAttribute(scan_kernel<M, QPT, K, MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                         (int)smem));
+    }
   }
   dim3 grid((unsigned)(sp.n_seg * pl.splits), (unsigned)pl.qblocks);
   scan_kernel<M, QPT, K, MODE><<<grid, kThreads, smem, st>>>(sp);

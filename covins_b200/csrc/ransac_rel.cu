@@ -671,8 +671,11 @@ int rel_ransac_area(cvb_ctx* ctx, int max_pairs, int* area) {
   constexpr int kMaxPairs = Sv::kCentral ? 1 : kMaxCams * kMaxCams;
   constexpr int kMaxArea = Sv::kArea > kPairArea * kMaxPairs ? Sv::kArea : kPairArea * kMaxPairs;
   static cvb_once_per_device once;
-  if (once.first(ctx->device)) {
-    CVB_CUDA(ctx, cudaFuncSetAttribute(ransac_rel_kernel<Sv, Src>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(kWarps * kMaxArea * sizeof(double))));
+  {
+    std::lock_guard<std::mutex> once_lk(once.mtx);
+    if (once.first(ctx->device)) {
+      CVB_CUDA(ctx, cudaFuncSetAttribute(ransac_rel_kernel<Sv, Src>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(kWarps * kMaxArea * sizeof(double))));
+    }
   }
   *area = Sv::kArea > kPairArea * max_pairs ? Sv::kArea : kPairArea * max_pairs;
   return CVB_OK;

@@ -810,8 +810,11 @@ __global__ void __launch_bounds__(XTHREADS, 1) tc_xt_kernel(const TcParams p) {
 template <int K>
 int launch_xt(cvb_ctx* ctx, const TcParams& p, cudaStream_t st) {
   static cvb_once_per_device once;
-  if (once.first(ctx->device)) {
-    CVB_CUDA(ctx, cudaFuncSetAttribute(tc_xt_kernel<K>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes));
+  {
+    std::lock_guard<std::mutex> once_lk(once.mtx);
+    if (once.first(ctx->device)) {
+      CVB_CUDA(ctx, cudaFuncSetAttribute(tc_xt_kernel<K>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes));
+    }
   }
   tc_xt_kernel<K><<<p.nqb * p.parts, XTHREADS, kSmemBytes, st>>>(p);
   CVB_CHECK_LAUNCH(ctx);
@@ -842,8 +845,11 @@ template <class M, int K>
 int launch_tc(cvb_ctx* ctx, const TcParams& p, cudaStream_t st) {
   static cvb_once_per_device once;
   const size_t smem = smem_bytes<M>();
-  if (once.first(ctx->device)) {
-    CVB_CUDA(ctx, cudaFuncSetAttribute(tc_scan_kernel<M, K>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  {
+    std::lock_guard<std::mutex> once_lk(once.mtx);
+    if (once.first(ctx->device)) {
+      CVB_CUDA(ctx, cudaFuncSetAttribute(tc_scan_kernel<M, K>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    }
   }
   tc_scan_kernel<M, K><<<p.nqb * p.parts, NUM_THREADS, smem, st>>>(p);
   CVB_CHECK_LAUNCH(ctx);

@@ -4,6 +4,9 @@
   pose_graph_optimization(...)   ↔ Optimization::PoseGraphOptimization   (optimization_be.cpp:833-1086)
   BaSolver                       ↔ one ceres::Problem + ceres::Solve (create / iterate / result), used by bench.py
                                    and by the multi-GPU path (landmark-block sharding + all-reduce callback)
+  Group, solve_group(...), global_bundle_adjustment_group(...)
+                                 ↔ the same solves sharded over several contexts of this process (one host thread
+                                   per rank, in-process all-reduce in rank order, optional peer path)
 
 `problem` is the dict produced by covins_b200.synth_map (or by the C++ shim's flatten step): numpy arrays in the
 canonical orders of SURVEY.md §8c.
@@ -257,6 +260,74 @@ def global_bundle_adjustment(ctx: Context, p: dict, iterations_limit=10, visual_
     removed = np.zeros(max(flat.n_obs, 1), np.uint8)
     g = GbaOptions(int(iterations_limit), int(visual_only), int(outlier_removal), float(th_outlier))
     ctx.check(lib().cvb_gba(ctx.handle, C.byref(flat.s), C.byref(g), C.byref(res.r), removed.ctypes.data))
+    out = res.as_dict()
+    out["obs_removed"] = removed[:flat.n_obs].astype(bool)
+    return out
+
+
+GROUP_ALLREDUCE_CHUNK = 1 << 21   # CVB_GROUP_ALLREDUCE_CHUNK: doubles per chunk of the group all-reduce
+
+
+class Group:
+    """cvb_group over Contexts of this process: rank r = contexts[r].  Several contexts may share a device.  The group
+    does not own the contexts; close it before them."""
+
+    def __init__(self, contexts):
+        self.contexts = list(contexts)
+        self.ctx = self.contexts[0] if self.contexts else None
+        arr = (c_vp * max(len(self.contexts), 1))(*[c.handle for c in self.contexts])
+        self.h = c_vp()
+        rc = lib().cvb_group_create(arr, len(self.contexts), C.byref(self.h))
+        if rc != 0:
+            if self.ctx is None:
+                from ._lib import CvbError
+                raise CvbError(f"status {rc}: cvb_group_create")
+            self.ctx.check(rc)
+
+    @property
+    def n(self):
+        return len(self.contexts)
+
+    def allreduce_diag(self, bufs):
+        """the group all-reduce alone: bufs [n][count] float64 (rank r's buffer) → what every rank holds afterwards"""
+        x = np.ascontiguousarray(bufs, np.float64).reshape(self.n, -1)
+        out = np.zeros_like(x)
+        self.ctx.check(lib().cvb_group_allreduce_diag(self.h, x.ctypes.data, x.shape[1], out.ctypes.data))
+        return out
+
+    def close(self):
+        if self.h:
+            lib().cvb_group_destroy(self.h)
+            self.h = c_vp()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+def solve_group(group: Group, p: dict, max_iterations: int, visual_only=False, cauchy_reproj=1.0, cauchy_edge=1.0,
+                edges=None, obs_skip=None, peer_path=False):
+    """solve() sharded over the ranks of `group` (cvb_ba_solve_group): merged result, landmarks from their owners.
+    peer_path: reduce-scatter by peer pull + column-distributed factorisation (a device per rank; not yet verified on
+    several devices, so off by default) instead of the all-reduce of the packed reduced system."""
+    flat = _Flat(p, edges=edges, obs_skip=obs_skip, use_imu=not visual_only)
+    res = _Res(flat.K, flat.L)
+    o = BaOptions(int(max_iterations), int(visual_only), float(cauchy_reproj), float(cauchy_edge), 0, 1)
+    group.ctx.check(lib().cvb_ba_solve_group(group.h, C.byref(flat.s), C.byref(o), int(bool(peer_path)), C.byref(res.r)))
+    return res.as_dict()
+
+
+def global_bundle_adjustment_group(group: Group, p: dict, iterations_limit=10, visual_only=False, outlier_removal=True,
+                                   th_outlier=0.92, peer_path=False):
+    """global_bundle_adjustment() sharded over the ranks of `group` (cvb_gba_group)."""
+    flat = _Flat(p, use_imu=not visual_only)
+    res = _Res(flat.K, flat.L)
+    removed = np.zeros(max(flat.n_obs, 1), np.uint8)
+    g = GbaOptions(int(iterations_limit), int(visual_only), int(outlier_removal), float(th_outlier))
+    group.ctx.check(lib().cvb_gba_group(group.h, C.byref(flat.s), C.byref(g), int(bool(peer_path)), C.byref(res.r),
+                                        removed.ctypes.data))
     out = res.as_dict()
     out["obs_removed"] = removed[:flat.n_obs].astype(bool)
     return out

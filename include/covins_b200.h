@@ -42,6 +42,7 @@ typedef enum cvb_status {
 } cvb_status;
 
 typedef struct cvb_ctx cvb_ctx;
+typedef struct cvb_group cvb_group;   /* in-process rank group of the bundle adjustment (cvb_group_create) */
 
 CVB_API int cvb_version(void);
 CVB_API int cvb_ctx_create(int device, cvb_ctx** out);
@@ -807,6 +808,9 @@ CVB_API int cvb_microbench_minmax(cvb_ctx* ctx, double* out2);
 CVB_API int cvb_microbench_potrf(cvb_ctx* ctx, int reps, double* us_per_tile, int64_t* phase_cycles);
 /* Diagnostic: single-warp latencies (cycles per dependent DFMA, rsqrt, shuffle, ...), see microbench.cu. out8: double[8]. */
 CVB_API int cvb_microbench_latency(cvb_ctx* ctx, double* out8);
+/* Diagnostic: the group all-reduce of cvb_group_create alone.  in [n][count] (host): rank r's buffer; out [n][count] (host):
+ * what each rank holds afterwards (the rank-order sum, on every rank).  One host thread per rank, as in the group drivers. */
+CVB_API int cvb_group_allreduce_diag(cvb_group* g, const double* in, size_t count, double* out);
 
 /* diagnostic: solve A x = b (host SPD matrix, row-major n x n) with the BA factorisation (tiled FP64 Cholesky on
  * DMMA); *factor_ms (nullable) receives the device time of the factorisation. */
@@ -931,6 +935,47 @@ CVB_API int cvb_ba_solve(cvb_ctx* ctx, const cvb_ba_problem* p, const cvb_ba_opt
  * erases from the map (:285-287).  Edges are the map's loop constraints with sqrt_info diag(100 I3, 1e4 I3) (:238-240). */
 CVB_API int cvb_gba(cvb_ctx* ctx, const cvb_ba_problem* p, const cvb_gba_options* g, cvb_ba_result* r,
                     uint8_t* obs_removed);
+
+/*
+ * Multi-GPU from one process: a rank group over contexts of this process (rank r = ctxs[r]), for a server whose bundle
+ * adjustment runs on one of its own threads (no torchrun, no NCCL, no CUDA IPC).
+ *   cvb_group_create: 1 <= n <= 16 (the peer path's limit), no NULL context, no context twice -> else CVB_ERR_INVALID before
+ *   any device work.  Several contexts may be on one device (their ranks then share it).  For every pair of distinct devices
+ *   peer access is enabled both ways (with access to the peer's stream-ordered pool; process-wide, it stays enabled after
+ *   cvb_group_destroy); a pair without peer access (cudaDeviceCanAccessPeer) -> CVB_ERR_UNSUPPORTED naming the pair.
+ *   Messages go to ctxs[0].
+ *   Group all-reduce (what the drivers install through cvb_allreduce_fn): a host rendezvous of the n rank threads, after which
+ *   each rank's stream waits on events the others recorded after producing their buffers; a kernel on each rank reads the n
+ *   buffers (same device or peer access) and adds them in RANK ORDER 0..n-1 into rank-local scratch; a second rendezvous
+ *   with events, so that no rank overwrites a buffer a peer still reads, then the copy back.  Every rank holds bit-identical
+ *   sums, the same from run to run.  Buffers go in chunks of CVB_GROUP_ALLREDUCE_CHUNK doubles (bounded scratch: one chunk
+ *   per rank).
+ *   Failures: every rendezvous waits at most 20 s (the distributed factorisation's peer-flag bound).  A rank that fails marks
+ *   the group failed; the other ranks then return an error from their next rendezvous instead of blocking.  The drivers
+ *   join every rank thread and synchronise every rank's streams before they return: no host thread and no device work
+ *   outlives a call.  The error is returned with "rank r: <message of the first failure>" on ctxs[0].
+ *   Calls on one group are serialised (a second concurrent call waits); the group's contexts must not be used by other
+ *   threads during a group call.
+ * cvb_ba_solve_group / cvb_gba_group: cvb_ba_solve / cvb_gba sharded over the group (landmark blocks c % n, o->rank and
+ * o->world are ignored); one host thread per rank runs create -> group all-reduce -> [peer path] -> restart -> iterate.
+ *   peer_path != 0: the reduced camera system is reduce-scattered by peer pull and factorised by tile columns (as
+ *   cvb_ba_enable_p2p, with the peers' buffers handed over inside the process); 0: all-reduce of the packed tiles and a
+ *   replicated factorisation.  The peer path needs a device per rank: a group in which two ranks share a device refuses
+ *   peer_path != 0 with CVB_ERR_UNSUPPORTED before any thread or launch.  The in-process peer path has not been verified
+ *   against world 1 on several devices; the C++ shim and the Python wrappers leave it off by default.
+ *   cvb_gba_group: cvb_gba's two rounds; each observation's round-1 norm comes from the rank that owns its landmark, and the
+ *   outlier set is computed once, the same obs_skip for every rank in round 2.
+ *   Result: poses, speed-biases, cost history, steps, iterations and termination of rank 0, each landmark from its owner,
+ *   lm_owner filled in.  Every rank's poses, speed-biases and cost history must be bitwise equal -> else CVB_ERR_NUMERIC.
+ *   A group of one is bitwise equal to cvb_ba_solve / cvb_gba; larger groups equal them up to summation order.
+ *   A malformed problem is refused as cvb_ba_create refuses it, before any thread or launch.
+ */
+#define CVB_GROUP_ALLREDUCE_CHUNK (1 << 21)
+CVB_API int cvb_group_create(cvb_ctx* const* ctxs, int n, cvb_group** out);
+CVB_API int cvb_group_destroy(cvb_group* g);
+CVB_API int cvb_ba_solve_group(cvb_group* g, const cvb_ba_problem* p, const cvb_ba_options* o, int peer_path, cvb_ba_result* r);
+CVB_API int cvb_gba_group(cvb_group* g, const cvb_ba_problem* p, const cvb_gba_options* gba, int peer_path, cvb_ba_result* r,
+                          uint8_t* obs_removed);
 
 /* ------------------------------------------------------------------------------------------------
  * Map maintenance (SURVEY.md §8f rank 4)
