@@ -45,7 +45,8 @@ __device__ __forceinline__ void dmma16816(double (&c)[4], const double (&a)[8], 
                  "d"(b[0]), "d"(b[1]), "d"(b[2]), "d"(b[3]));
 }
 
-// acc(64 x BN) = A(64 x T) * B(BN x T)^T, both operands row-major with K contiguous (leading dims lda, ldb).
+// acc(64 x BN) = A(64 x T) * B(BN x T)^T, both operands row-major with K contiguous (leading dims lda, ldb); with
+// FROM_ACC the product is accumulated onto acc as it stands, K chunk by K chunk in increasing order.
 // 2 x BN/32 warps, 32x32 per warp = 2 (m16) x 4 (n8) m16n8k16 blocks, acc[i][j] = rows 16 i.., columns 8 j.. of the warp
 // tile in the C-fragment order of dmma16816.  m16n8k16 is Hopper's full-rate FP64 MMA shape: on an H100 SXM (400 W limit)
 // a register-only probe sustained 64 TFLOP/s with it (~128 FMA/clk/SM) and 34 TFLOP/s with the Ampere m8n8k4 shape, and
@@ -53,25 +54,26 @@ __device__ __forceinline__ void dmma16816(double (&c)[4], const double (&a)[8], 
 // MMA per block and chunk) through a STAGES-deep cp.async ring (one barrier per chunk).  Row stride 20 doubles (≡ 8 words
 // mod 32): the fragment loads of a half-warp (rows g = 0..3, columns t = 0..3) hit words 8g + 2t, conflict-free.  The CTA
 // is deliberately small (64 x 64 x 128 for syrk_kernel: 128 threads, 60 KB): three to four CTAs share an SM, so one CTA's
-// fixed costs — index fetch, pipeline fill, the C round trip of the epilogue, barrier bubbles — overlap the others' main
-// loops.  The throughput path of the trailing update (tile_update_kernel) takes the whole 128x128 tile per CTA instead:
-// it halves the operand bytes per FMA and keeps C in shared memory, so it has no per-panel C round trip to hide.
+// fixed costs — index fetch, pipeline fill, the C load and store, barrier bubbles — overlap the others' main loops.  The
+// throughput path of the trailing update (tile_update_kernel) takes the whole 128x128 tile per CTA instead: it halves
+// the operand bytes per FMA.
 constexpr int KC = 16;
 constexpr int LDS = KC + 4;
 constexpr int GEMM_STAGES = 3;
 
-template <int BN>
+template <int BN, bool FROM_ACC = false>
 __device__ __forceinline__ void gemm_abt_64(const double* __restrict__ A, size_t lda, const double* __restrict__ B,
                                             size_t ldb, double (&acc)[2][4][4], double* smem) {
   constexpr int WN = BN / 32, THREADS = 2 * WN * 32, STAGE = (64 + BN) * LDS, NCH = T / KC, UPR = KC / 2;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int wm = warp / WN, wn = warp % WN;
+  if (!FROM_ACC)
 #pragma unroll
-  for (int i = 0; i < 2; i++)
+    for (int i = 0; i < 2; i++)
 #pragma unroll
-    for (int j = 0; j < 4; j++)
+      for (int j = 0; j < 4; j++)
 #pragma unroll
-      for (int e = 0; e < 4; e++) acc[i][j][e] = 0.0;
+        for (int e = 0; e < 4; e++) acc[i][j][e] = 0.0;
   // a thread copies the same 16-byte segment of rows r0, r0 + RSTEP, ...: one base address per operand
   constexpr int RSTEP = THREADS / UPR;
   const int r0 = tid / UPR, seg = tid % UPR;
@@ -180,9 +182,9 @@ __global__ void __launch_bounds__(T, 1) chain_gemm_kernel(double* __restrict__ C
   cp_async_commit();
   cp_async_wait<0>();
   __syncthreads();
-  double acc[CHAIN_ROWS];
+  double acc[CHAIN_ROWS];   // MODE 1: -C (see tile_update), so the products are added and 0 - acc is stored
 #pragma unroll
-  for (int r = 0; r < CHAIN_ROWS; r++) acc[r] = 0.0;
+  for (int r = 0; r < CHAIN_ROWS; r++) acc[r] = MODE == 1 && j <= i0 + r ? -C[(size_t)(i0 + r) * T + j] : 0.0;
   const double* qrow = Qs + (size_t)j * CHAIN_LDQ;
 #pragma unroll 8
   for (int c = 0; c < T; c++) {
@@ -194,16 +196,16 @@ __global__ void __launch_bounds__(T, 1) chain_gemm_kernel(double* __restrict__ C
   for (int r = 0; r < CHAIN_ROWS; r++) {
     double* dst = C + (size_t)(i0 + r) * T + j;
     if (MODE == 0) *dst = acc[r];
-    else if (j <= i0 + r) *dst -= acc[r];
+    else if (j <= i0 + r) *dst = 0.0 - acc[r];
   }
 }
 
-// A(i,j) -= A(i,k) A(j,k)^T for the tile pairs (i >= j) pi[]/pj[] and the panels k = k0 + q of the bits q of pmask[]
-// (TilePlan::h_pair_mask), in increasing k, each panel's product subtracted on its own.  Used for the chain's diagonal pair
-// (factor()), where one tile is updated alone and latency counts: four CTAs per pair, one 64x64
-// quadrant each (consecutive CTAs share the pair's operands in L2); the quadrant above the diagonal of a diagonal tile is
-// skipped.  The quadrant (32 KB) is fetched into L2 at the start, so the first epilogue does not wait on HBM, and stays
-// there for the read-modify-write of the later panels: several panels per visit make one HBM round trip of C.
+// A(i,j) += (-A(i,k)) A(j,k)^T for the tile pairs (i >= j) pi[]/pj[] and the panels k = k0 + q of the bits q of pmask[]
+// (TilePlan::h_pair_mask), in increasing k, the K chunks of each panel in increasing order, in the accumulators that hold
+// the target for the whole visit (the convention of tile_update below, which gives the same bits).  Used for the chain's
+// diagonal pair (factor()), where one tile is updated alone and latency counts: four CTAs per pair, one 64x64 quadrant
+// each (consecutive CTAs share the pair's operands in L2); the quadrant above the diagonal of a diagonal tile is skipped.
+// The quadrant is read once at the start and written once at the end.
 __global__ void __launch_bounds__(SYRK_THREADS, 3) syrk_kernel(double* __restrict__ S, const int* __restrict__ tile_of, int nt,
                                                                 int k0, const int* __restrict__ pi, const int* __restrict__ pj,
                                                                 const int* __restrict__ pmask) {
@@ -213,33 +215,36 @@ __global__ void __launch_bounds__(SYRK_THREADS, 3) syrk_kernel(double* __restric
   const int i = pi[p], j = pj[p];
   if (i == j && qc > qr) return;
   double* C = S + (size_t)tile_of[(size_t)i * nt + j] * TT + (size_t)qr * 64 * T + qc * 64;
-#pragma unroll
-  for (int u = threadIdx.x; u < 64 * 4; u += SYRK_THREADS)   // 64 rows x 4 lines of 128 B
-    asm volatile("prefetch.global.L2 [%0];" ::"l"(C + (size_t)(u >> 2) * ld + (u & 3) * 16));
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, wm = warp >> 1, wn = warp & 1;
+  double* Cw = C + (size_t)(wm * 32 + (lane >> 2)) * ld + wn * 32 + (lane & 3) * 2;   // + (16 a + 8 h) ld + 8 b
+  double acc[2][4][4];
+#pragma unroll
+  for (int a = 0; a < 2; a++)
+#pragma unroll
+    for (int b = 0; b < 4; b++)
+#pragma unroll
+      for (int h = 0; h < 2; h++) {
+        const double2 v = *reinterpret_cast<const double2*>(Cw + (size_t)(a * 16 + h * 8) * ld + b * 8);
+        acc[a][b][2 * h] = -v.x;
+        acc[a][b][2 * h + 1] = -v.y;
+      }
   unsigned mask = (unsigned)pmask[p];
 #pragma unroll 1
   for (int k = k0; mask != 0; k++, mask >>= 1) {
     if (!(mask & 1u)) continue;
     const double* Ai = S + (size_t)tile_of[(size_t)i * nt + k] * TT + (size_t)qr * 64 * T;
     const double* Aj = S + (size_t)tile_of[(size_t)j * nt + k] * TT + (size_t)qc * 64 * T;
-    double acc[2][4][4];
     __syncthreads();   // every warp is done with the previous panel's last stages before the prologue refills them
-    gemm_abt_64<64>(Ai, ld, Aj, ld, acc, smem_d);
-#pragma unroll
-    for (int a = 0; a < 2; a++)
-#pragma unroll
-      for (int b = 0; b < 4; b++)
-#pragma unroll
-        for (int h = 0; h < 2; h++) {
-          const int r = wm * 32 + a * 16 + h * 8 + (lane >> 2), c = wn * 32 + b * 8 + (lane & 3) * 2;
-          double2* q = reinterpret_cast<double2*>(C + (size_t)r * ld + c);
-          double2 v = *q;
-          v.x -= acc[a][b][2 * h];
-          v.y -= acc[a][b][2 * h + 1];
-          *q = v;
-        }
+    gemm_abt_64<64, true>(Ai, ld, Aj, ld, acc, smem_d);
   }
+#pragma unroll
+  for (int a = 0; a < 2; a++)
+#pragma unroll
+    for (int b = 0; b < 4; b++)
+#pragma unroll
+      for (int h = 0; h < 2; h++)
+        *reinterpret_cast<double2*>(Cw + (size_t)(a * 16 + h * 8) * ld + b * 8) =
+            make_double2(0.0 - acc[a][b][2 * h], 0.0 - acc[a][b][2 * h + 1]);
 }
 
 // The trailing update's pipeline (tile_update below) uses the mbarrier helpers of cvb_internal.cuh and these two arrivals.
@@ -254,8 +259,8 @@ __device__ __forceinline__ void mbar_arrive_cp_async(uint64_t* bar) {
 // The same update, one CTA per pair and the whole 128x128 tile per CTA: the throughput path (every update list except the
 // chain's diagonal pair, see factor()).  Per 16-wide K chunk a CTA stages 128 rows of each operand for 128x128x16 FMA —
 // half the operand bytes per FMA of the 64x64 quadrants above, whose L2→SM traffic bounded them.  The operands come
-// through a 3-stage ring that runs on across the panels of the pair's mask, fed by a warp-specialised pipeline with no
-// CTA barrier in the main loop:
+// through a TILE_STAGES-deep ring that runs on across the panels of the pair's mask, fed by a warp-specialised pipeline
+// with no CTA barrier after the set-up:
 //   producer   warpgroup 2 (4 warps, 24 registers after setmaxnreg) issues each chunk's cp.asyncs (16 per thread) into a
 //              stage once the stage's `empty` barrier has completed, and arrives on its `full` barrier through
 //              cp.async.mbarrier.arrive.noinc, which fires when the thread's copies have landed;
@@ -265,31 +270,37 @@ __device__ __forceinline__ void mbar_arrive_cp_async(uint64_t* bar) {
 //              while the DMMAs run, and the warps drift apart instead of meeting at a barrier every chunk.
 // The CTA is launched with 168 registers per thread (384 threads, 1 CTA/SM), and 24 x 128 + 240 x 256 = 168 x 384: the
 // consumers take exactly what the producer gives back.
-// C lives in shared memory for the whole visit: the producer copies it in with the first four chunks, each panel's
-// product (accumulated from zero over the K chunks in order) is subtracted from it on its own, in increasing panel order,
-// and the consumers write it back once.  So the results are bit-identical to syrk_kernel's, with one C read and one C
-// write per visit instead of an L2 read-modify-write per panel.  Ring rows are 128 B, unpadded: segment s of a row r sits
-// at s ^ 2 (r & 3), which makes the fragment loads conflict-free; C rows are 1 KB, 16-byte segment s of row r at
-// s ^ 4 (r & 1), which makes the epilogue's double2 accesses conflict-free.  Shared memory: 128 KB of C + 3 x 32 KB ring
-// (+ 576 B), 1 CTA/SM.
+// The target lives in the accumulators for the whole visit.  Arithmetic convention of every trailing-update kernel
+// (this one, syrk_kernel, chain_gemm_kernel<1>): C <- C + (-A(i,k)) A(j,k)^T, the accumulator starting at C, the panels in
+// increasing k and the K chunks in increasing order inside each panel, no separate product per panel.  It is computed as
+// -C + A(i,k) A(j,k)^T and stored as 0 - acc: round-to-nearest is symmetric under negation, so every rounding is the
+// mirror image of the convention's and a non-zero result has its bits, at no cost inside the K loop; a zero is stored as
+// +0 (a +0 entry that receives only zero products stays +0).  Since the accumulation starts from the stored target,
+// applying a pair's panels in one visit or over several visits gives the same bits, which keeps the blocked,
+// column-by-column and column-group schedules bit-identical.  The convention costs accuracy: the sum is recursive, every
+// rounding at the magnitude of the running target, where a product per panel summed from zero and then subtracted
+// rounded mostly at the product's magnitude.  That product cannot be kept beside the target: the two take 128 registers
+// per thread each, more than the consumers' 240 (built that way, ptxas spills 712 B).  Each consumer warp loads
+// its 64x32 slice of -C from global memory before its first `full` wait, so the load overlaps the ring fill, and stores
+// it once at the end; the warps of a diagonal tile's upper quadrant stay idle, so that quadrant is neither read nor
+// written.  Ring rows are 128 B, unpadded: segment s of a row r sits at s ^ 2 (r & 3), which makes the fragment loads
+// conflict-free.  Shared memory: TILE_STAGES x 32 KB ring (+ 640 B), 1 CTA/SM.
 constexpr int TILE_CONSUMERS = 256;                   // warpgroups 0 and 1
 constexpr int TILE_PRODUCERS = 128;                   // warpgroup 2
 constexpr int TILE_THREADS = TILE_CONSUMERS + TILE_PRODUCERS;
-constexpr int TILE_STAGES = 3;
+constexpr int TILE_STAGES = 4;
 constexpr int TILE_STAGE = 2 * T * KC;   // doubles per ring stage: 128 rows of A(i,k), then 128 rows of A(j,k)
-constexpr size_t kTileSmem = (TT + (size_t)TILE_STAGES * TILE_STAGE) * sizeof(double);   // 229376 B → 1 CTA / SM
+constexpr size_t kTileSmem = (size_t)TILE_STAGES * TILE_STAGE * sizeof(double);
 
 __device__ __forceinline__ void tile_update(double* __restrict__ S, const int* __restrict__ tile_of, int nt, int k0,
                                             const int* __restrict__ pi, const int* __restrict__ pj,
                                             const int* __restrict__ pmask) {
-  extern __shared__ __align__(128) double smem_d[];
+  extern __shared__ __align__(128) double ring[];   // [TILE_STAGES][2 T][KC], swizzled
   __shared__ const double* s_ai[32];   // operand tiles A(i,k), A(j,k) of the pair's panels, in increasing k
   __shared__ const double* s_aj[32];
   __shared__ uint64_t full[TILE_STAGES], empty[TILE_STAGES];
   __shared__ int s_nch;   // chunks of the visit, read by each role after the set-up barrier (a register would spill)
   constexpr int NCH = T / KC;
-  double* Cs = smem_d;            // [T][T], swizzled
-  double* ring = smem_d + TT;     // [TILE_STAGES][2 T][KC], swizzled
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int i = pi[blockIdx.x], j = pj[blockIdx.x];
   const bool diag = i == j;
@@ -315,14 +326,13 @@ __device__ __forceinline__ void tile_update(double* __restrict__ S, const int* _
     asm volatile("setmaxnreg.dec.sync.aligned.u32 24;");
     const int nch = s_nch;
     const int pt = tid - TILE_CONSUMERS;
-    // a thread copies 16-byte segment `seg` of rows r0, r0 + 16, ... of both operands (r0 & 3 fixes the swizzle), and
-    // 16-byte segment `cs` of rows rc, rc + 2, ... of C's part
-    const int r0 = pt >> 3, seg = pt & 7, rc = pt >> 6, cs = pt & 63;
+    // a thread copies 16-byte segment `seg` of rows r0, r0 + 16, ... of both operands (r0 & 3 fixes the swizzle)
+    const int r0 = pt >> 3, seg = pt & 7;
     const int so = r0 * KC + ((seg ^ ((r0 & 3) << 1)) << 1);
 #pragma unroll 1
     for (int c = 0; c < nch; c++) {
       const int st = c % TILE_STAGES;
-      if (c >= TILE_STAGES) cvb_mbar_wait(&empty[st], (c / TILE_STAGES - 1) & 1);   // chunk c - 3 has left the stage
+      if (c >= TILE_STAGES) cvb_mbar_wait(&empty[st], (c / TILE_STAGES - 1) & 1);   // chunk c - TILE_STAGES has left
       const size_t go = (size_t)r0 * T + (c % NCH) * KC + seg * 2;
       const double* ga = s_ai[c / NCH] + go;
       const double* gb = s_aj[c / NCH] + go;
@@ -331,15 +341,6 @@ __device__ __forceinline__ void tile_update(double* __restrict__ S, const int* _
       for (int it = 0; it < T / 16; it++) cp_async16(As + it * 16 * KC, ga + (size_t)it * 16 * T);
 #pragma unroll
       for (int it = 0; it < T / 16; it++) cp_async16(As + T * KC + it * 16 * KC, gb + (size_t)it * 16 * T);
-      // rows 32 c .. 32 c + 31 of C join chunk c (c < 4): all of C has landed before the first epilogue (chunk 7).  The
-      // quadrant above the diagonal of a diagonal tile is neither read nor written.
-      if (c < 4 && !(diag && c < 2 && cs >= 32)) {
-        const int r = c * 32 + rc;
-        double* cd = Cs + r * T + ((cs ^ (rc << 2)) << 1);
-        const double* cg = C + (size_t)r * T + cs * 2;
-#pragma unroll
-        for (int it = 0; it < 16; it++) cp_async16(cd + it * 2 * T, cg + it * 2 * T);
-      }
       mbar_arrive_cp_async(&full[st]);
     }
     asm volatile("cp.async.wait_all;" ::: "memory");   // no copy outlives its issuing thread
@@ -348,66 +349,55 @@ __device__ __forceinline__ void tile_update(double* __restrict__ S, const int* _
 
   // ---- consumer warpgroups
   asm volatile("setmaxnreg.inc.sync.aligned.u32 240;");
-  if (!idle) {
-    const int nch = s_nch;
-    int cq[4];   // ring column of fragment K index t + 4 q (rows g + 8 n: the swizzle depends on g & 3 only)
+  if (idle) return;
+  const int nch = s_nch;
+  int cq[4];   // ring column of fragment K index t + 4 q (rows g + 8 n: the swizzle depends on g & 3 only)
 #pragma unroll
-    for (int q = 0; q < 4; q++) cq[q] = t + 4 * (q ^ (g & 3));
-    double acc[4][4][4];
+  for (int q = 0; q < 4; q++) cq[q] = t + 4 * (q ^ (g & 3));
+  // the warp's slice of -C in the C-fragment order of dmma16816: acc[ai][bj][2 h + x] = -C(r0 + 16 ai + 8 h,
+  // c0 + 8 bj + x), row r0 = 64 wm + g, column c0 = 32 wn + 2 t
+  double* Cw = C + (size_t)(wm * 64 + g) * T + wn * 32 + 2 * t;
+  double acc[4][4][4];
 #pragma unroll
-    for (int a = 0; a < 4; a++)
+  for (int ai = 0; ai < 4; ai++)
 #pragma unroll
-      for (int b = 0; b < 4; b++)
+    for (int bj = 0; bj < 4; bj++)
 #pragma unroll
-        for (int e = 0; e < 4; e++) acc[a][b][e] = 0.0;
-#pragma unroll 1
-    for (int c = 0; c < nch; c++) {
-      const int st = c % TILE_STAGES;
-      cvb_mbar_wait(&full[st], (c / TILE_STAGES) & 1);   // chunk c (and C's part c < 4) has landed
-      const double* As = ring + st * TILE_STAGE + (wm * 64 + g) * KC;
-      const double* Bs = ring + st * TILE_STAGE + T * KC + (wn * 32 + g) * KC;
-      double a[4][8], b[4][4];
-#pragma unroll
-      for (int bj = 0; bj < 4; bj++)
-#pragma unroll
-        for (int e = 0; e < 4; e++) b[bj][e] = Bs[bj * 8 * KC + cq[e]];
-#pragma unroll
-      for (int ai = 0; ai < 4; ai++)
-#pragma unroll
-        for (int e = 0; e < 8; e++) a[ai][e] = As[(ai * 16 + 8 * (e & 1)) * KC + cq[e >> 1]];
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&empty[st]);   // the warp's fragments are in registers: the stage may be refilled
-#pragma unroll
-      for (int ai = 0; ai < 4; ai++)
-#pragma unroll
-        for (int bj = 0; bj < 4; bj++) dmma16816(acc[ai][bj], a[ai], b[bj]);
-      if (c % NCH == NCH - 1) {   // the panel is complete: subtract it, start the next one from zero
-#pragma unroll
-        for (int ai = 0; ai < 4; ai++)
-#pragma unroll
-          for (int bj = 0; bj < 4; bj++)
-#pragma unroll
-            for (int h = 0; h < 2; h++) {
-              const int r = wm * 64 + ai * 16 + h * 8 + g, s = wn * 16 + bj * 4 + t;
-              double2* q = reinterpret_cast<double2*>(Cs + r * T + ((s ^ ((r & 1) << 2)) << 1));
-              double2 v = *q;
-              v.x -= acc[ai][bj][2 * h];
-              v.y -= acc[ai][bj][2 * h + 1];
-              *q = v;
-              acc[ai][bj][2 * h] = 0.0;
-              acc[ai][bj][2 * h + 1] = 0.0;
-            }
+      for (int h = 0; h < 2; h++) {
+        const double2 v = *reinterpret_cast<const double2*>(Cw + (size_t)(ai * 16 + h * 8) * T + bj * 8);
+        acc[ai][bj][2 * h] = -v.x;
+        acc[ai][bj][2 * h + 1] = -v.y;
       }
-    }
+#pragma unroll 1
+  for (int c = 0; c < nch; c++) {
+    const int st = c % TILE_STAGES;
+    cvb_mbar_wait(&full[st], (c / TILE_STAGES) & 1);   // chunk c has landed
+    const double* As = ring + st * TILE_STAGE + (wm * 64 + g) * KC;
+    const double* Bs = ring + st * TILE_STAGE + T * KC + (wn * 32 + g) * KC;
+    double a[4][8], b[4][4];
+#pragma unroll
+    for (int bj = 0; bj < 4; bj++)
+#pragma unroll
+      for (int e = 0; e < 4; e++) b[bj][e] = Bs[bj * 8 * KC + cq[e]];
+#pragma unroll
+    for (int ai = 0; ai < 4; ai++)
+#pragma unroll
+      for (int e = 0; e < 8; e++) a[ai][e] = As[(ai * 16 + 8 * (e & 1)) * KC + cq[e >> 1]];
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&empty[st]);   // the warp's fragments are in registers: the stage may be refilled
+#pragma unroll
+    for (int ai = 0; ai < 4; ai++)
+#pragma unroll
+      for (int bj = 0; bj < 4; bj++) dmma16816(acc[ai][bj], a[ai], b[bj]);
   }
-  asm volatile("bar.sync 1, %0;" ::"n"(TILE_CONSUMERS) : "memory");   // every consumer warp's last epilogue is in Cs
-#pragma unroll 8
-  for (int it = 0; it < (int)(TT / 2 / TILE_CONSUMERS); it++) {
-    const int u = tid + it * TILE_CONSUMERS, r = u >> 6, s = u & 63;
-    if (!(diag && r < 64 && s >= 32))
-      *reinterpret_cast<double2*>(C + (size_t)r * T + s * 2) =
-          *reinterpret_cast<const double2*>(Cs + r * T + ((s ^ ((r & 1) << 2)) << 1));
-  }
+#pragma unroll
+  for (int ai = 0; ai < 4; ai++)
+#pragma unroll
+    for (int bj = 0; bj < 4; bj++)
+#pragma unroll
+      for (int h = 0; h < 2; h++)
+        *reinterpret_cast<double2*>(Cw + (size_t)(ai * 16 + h * 8) * T + bj * 8) =
+            make_double2(0.0 - acc[ai][bj][2 * h], 0.0 - acc[ai][bj][2 * h + 1]);
 }
 __global__ void __launch_bounds__(TILE_THREADS, 1) tile_update_kernel(double* __restrict__ S, const int* __restrict__ tile_of,
                                                                       int nt, int k0, const int* __restrict__ pi,

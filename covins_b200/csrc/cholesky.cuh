@@ -8,9 +8,9 @@ namespace cvb_chol {
 
 constexpr int T = 128;  // tile edge
 // Width of the outer block of the main sequence: the trailing update of the tiles past a block applies all of the block's
-// panels in one visit to each tile (one C round trip to HBM per block instead of per panel).  4 was the fastest of 2, 3
-// and 4 at C3 with the whole-tile update kernel (DESIGN.md §9).
-constexpr int kPanelBlock = 4;
+// panels in one visit to each tile (one C round trip to HBM per block instead of per panel).  6 and 8 were equally fast
+// at C3 and 1 % faster than 4 once the update kept its target in registers (DESIGN.md §9).
+constexpr int kPanelBlock = 6;
 
 // Tile-level structure of the factor: which 128x128 tiles of L are structurally non-zero, as launch lists.
 struct TilePlan {
