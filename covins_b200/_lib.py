@@ -54,6 +54,10 @@ SIGNATURES = {
     "cvb_db_match_hamming": (C.c_int, [c_vp, c_vp, c_vp, C.c_int, C.c_float, C.c_float, c_vp, c_vp, c_vp, c_vp, c_vp,
                                        C.c_int, C.POINTER(C.c_int32)]),
     "cvb_db_match_hamming_dev": (C.c_int, [c_vp, c_vp, c_vp, C.c_int, C.c_float, C.c_float, c_vp, c_vp, c_vp, c_vp]),
+    "cvb_db_append_sift": (C.c_int, [c_vp, c_vp, c_vp, c_vp, C.c_int]),
+    "cvb_db_match_l2": (C.c_int, [c_vp, c_vp, c_vp, C.c_int, C.c_float, C.c_float, c_vp, c_vp, c_vp, c_vp, c_vp,
+                                  C.c_int, C.POINTER(C.c_int32)]),
+    "cvb_db_match_l2_dev": (C.c_int, [c_vp, c_vp, c_vp, C.c_int, C.c_float, C.c_float, c_vp, c_vp, c_vp, c_vp]),
     "cvb_knn_l2_batch": (C.c_int, [c_vp, c_vp, C.c_int, c_vp, c_vp, C.c_int, C.c_int, C.c_int, c_vp, c_vp]),
     "cvb_knn_l2_u8_batch_dev": (C.c_int, [c_vp, c_vp, C.c_int, c_vp, c_vp, c_vp, C.c_int, C.c_int, C.c_int, c_vp, c_vp, c_vp]),
     "cvb_match_l2_batch": (C.c_int, [c_vp, c_vp, C.c_int, c_vp, c_vp, C.c_int, C.c_int, C.c_float, C.c_float, c_vp, c_vp, c_vp]),

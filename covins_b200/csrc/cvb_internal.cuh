@@ -114,6 +114,13 @@ int cvb_match_hamming_pairs_dev(cvb_ctx* ctx, const uint8_t* d_desc, const int32
                                 int32_t* d_match_train, float* d_match_dist, int32_t* d_n_matches);
 int cvb_match_l2_pairs_dev(cvb_ctx* ctx, const uint8_t* d_desc, const int32_t* d_pairs, int n_pairs, int max_nq, float thr, float ratio,
                            int32_t* d_match_train, float* d_match_dist, int32_t* d_n_matches);
+// cvb_match_l2_u8_dev: cvb_match_l2_batch on device u8 SIFT rows (the layout cvb_knn_l2_u8_batch_dev takes); outputs as
+// cvb_match_hamming_batch_dev.  The map database matches its SIFT keyframes through it.
+int cvb_match_l2_u8_dev(cvb_ctx* ctx, const uint8_t* d_q, int nq, const uint8_t* d_t, const int32_t* d_seg_ptr, const int32_t* h_seg_ptr,
+                        int n_seg, float thr, float ratio, int32_t* d_match_train, float* d_match_dist, int32_t* d_n_matches, void* stream);
+
+// ransac_rel.cu: SIFT rows (CV_32F) to the u8 layout of the L2 kernels on the host; false if a value is not an integer in [0, 255]
+bool cvb_quantize_sift(const float* src, size_t n, uint8_t* dst);
 
 // ransac_abs.cu: the seeded GP3P RANSAC of cvb_ransac_absolute_pose_seeded_batch on device inputs and outputs (one CTA per
 // problem on ctx->stream).  d_cam [n_prob][12] = camera offset (3) then rotation (9, row-major); d_inlier_mask nullable.

@@ -1678,9 +1678,13 @@ inline std::vector<NonCentralRelativePoseRansacResult> RansacCentralRelativePose
 // Resident-map descriptor database (cvb_db_*): the ORB descriptors of the map's keyframes live in HBM; the candidate
 // loop of PlaceRecognitionG::ComputeSE3 (placerec_gen_be.cpp:60-135) becomes one call per query keyframe.  The database
 // index of a keyframe is its insertion order; keep it next to the keyframe (e.g. std::map<idpair, int>).
+// A database constructed with the SiftDescriptors tag holds SIFT rows instead (feat.type SIFT, placerec_gen_be.cpp:86-87):
+// AddKeyframe / MatchAll then take CV_32F rows x 128, matched with the exact L2 2-NN of MatchCandidatesSIFT.
+struct SiftDescriptors {};
 class DescriptorDatabase {
  public:
   explicit DescriptorDatabase(Context& ctx) : ctx_(ctx) { ctx_.check(cvb_db_create(ctx_.get(), 32, &db_), "cvb_db_create"); }
+  DescriptorDatabase(Context& ctx, SiftDescriptors) : ctx_(ctx) { ctx_.check(cvb_db_create(ctx_.get(), 128, &db_), "cvb_db_create"); }
   ~DescriptorDatabase() { if (db_) cvb_db_destroy(ctx_.get(), db_); }
   DescriptorDatabase(const DescriptorDatabase&) = delete;
   DescriptorDatabase& operator=(const DescriptorDatabase&) = delete;
@@ -1688,6 +1692,12 @@ class DescriptorDatabase {
   int AddKeyframe(const uint8_t* descriptors, int rows) {
     const int32_t r = rows;
     ctx_.check(cvb_db_append(ctx_.get(), db_, descriptors, &r, 1), "cvb_db_append");
+    return n_kf_++;
+  }
+  // SIFT database: kf->descriptors_add_ as CV_32F, continuous, rows x 128, integer-valued in [0,255]
+  int AddKeyframe(const float* descriptors, int rows) {
+    const int32_t r = rows;
+    ctx_.check(cvb_db_append_sift(ctx_.get(), db_, descriptors, &r, 1), "cvb_db_append_sift");
     return n_kf_++;
   }
   int size() const { return n_kf_; }
@@ -1699,14 +1709,24 @@ class DescriptorDatabase {
   // knnMatch(k=2) + distance/ratio filter of the query keyframe against EVERY keyframe of the database:
   // result[db index] == the reference's img_matches for that candidate (accepted queries ascending, :102-114)
   std::vector<Matches> MatchAll(const uint8_t* query, int n_query, const OptParams& P) {
+    return match_all(cvb_db_match_hamming, "cvb_db_match_hamming", query, n_query, P);
+  }
+  // the same for a SIFT database: query = the query keyframe's CV_32F rows x 128
+  std::vector<Matches> MatchAll(const float* query, int n_query, const OptParams& P) {
+    return match_all(cvb_db_match_l2, "cvb_db_match_l2", query, n_query, P);
+  }
+
+ private:
+  template <class Fn, class Q>
+  std::vector<Matches> match_all(Fn fn, const char* name, const Q* query, int n_query, const OptParams& P) {
     std::vector<int32_t> nm(n_kf_ > 0 ? n_kf_ : 1);
     if (cap_ == 0) cap_ = 4096;
     for (;;) {
       m_kf_.resize(cap_); m_q_.resize(cap_); m_t_.resize(cap_); m_d_.resize(cap_);
       int32_t total = 0;
-      ctx_.check(cvb_db_match_hamming(ctx_.get(), db_, query, n_query, P.img_match_thres, P.ratio_thres, nm.data(), m_kf_.data(),
-                                      m_q_.data(), m_t_.data(), m_d_.data(), cap_, &total),
-                 "cvb_db_match_hamming");
+      ctx_.check(fn(ctx_.get(), db_, query, n_query, P.img_match_thres, P.ratio_thres, nm.data(), m_kf_.data(), m_q_.data(),
+                    m_t_.data(), m_d_.data(), cap_, &total),
+                 name);
       if (total <= cap_) {
         std::vector<Matches> out(n_kf_);
         for (int i = 0; i < total; i++) out[m_kf_[i]].push_back(Match{(size_t)m_q_[i], (size_t)m_t_[i], m_d_[i]});
@@ -1716,7 +1736,6 @@ class DescriptorDatabase {
     }
   }
 
- private:
   Context& ctx_;
   cvb_db* db_ = nullptr;
   int n_kf_ = 0, cap_ = 0;

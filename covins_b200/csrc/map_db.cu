@@ -1,10 +1,12 @@
-// map_db.cu — the merged map's ORB descriptors resident in HBM, queried per place-recognition request.
+// map_db.cu — the merged map's ORB or SIFT descriptors resident in HBM, queried per place-recognition request.
 //
 // Reference flow (covins_backend/src/covins_backend/placerec_gen_be.cpp:60-135): for every candidate keyframe the
 // query keyframe's descriptor matrix is matched (knnMatch k=2 → distance + ratio filter) and only the accepted
 // matches (img_matches, :102-114) and their count (:116-124) are consumed.  The descriptors of the map's keyframes
 // never change after a keyframe is added (keyframe_be.cpp:106-137 fills them once from the message), so they are
-// uploaded once (cvb_db_append) and stay in HBM; a query moves nq*32 B up and the accepted matches down.
+// uploaded once (cvb_db_append / cvb_db_append_sift) and stay in HBM; a query moves nq*32 B (ORB) or nq*128 B (SIFT, u8)
+// up and the accepted matches down.  Both row kinds share the code below; they differ in the row size, the tensor-core
+// tile image (cvb_tc::tile_bytes / expand_tiles by metric) and the host staging of SIFT rows (checked and quantised to u8).
 #include <string.h>
 
 #include <algorithm>
@@ -18,7 +20,7 @@ struct cvb_buf {
 };
 
 struct cvb_db {
-  int desc_bytes = 32;
+  int desc_bytes = 32;   // 32: ORB rows (Hamming); 128: SIFT rows as exact u8 (L2)
   uint8_t* d_rows = nullptr;
   size_t cap_rows = 0;
   std::vector<int32_t> seg_ptr{0};
@@ -33,6 +35,7 @@ struct cvb_db {
   int32_t* d_seg_tile = nullptr;
   // per-query scratch (grow-only)
   cvb_buf q, mt, md, nm, off, out_seg, out_q, out_t, out_d;
+  int metric() const { return desc_bytes == 32 ? 0 : 1; }   // cvb_tc metric of the rows
 };
 
 namespace {
@@ -73,7 +76,7 @@ int refresh_seg(cvb_ctx* ctx, cvb_db* db) {
 
 int reserve_tiles(cvb_ctx* ctx, cvb_db* db, size_t tiles, size_t used_tiles) {
   if (tiles <= db->cap_tiles) return CVB_OK;
-  const size_t want = std::max(tiles, db->cap_tiles * 3 / 2), tb = cvb_tc::tile_bytes();
+  const size_t want = std::max(tiles, db->cap_tiles * 3 / 2), tb = cvb_tc::tile_bytes(db->metric());
   uint8_t* p = nullptr;
   CVB_CUDA(ctx, cudaMalloc(&p, want * tb));
   const size_t used = used_tiles * tb;
@@ -152,6 +155,136 @@ __global__ void __launch_bounds__(256) db_compact_kernel(const int32_t* __restri
   }
 }
 
+// calls of one row kind on a database of the other are refused
+int require_kind(cvb_ctx* ctx, const cvb_db* db, bool sift, const char* fn) {
+  if ((db->desc_bytes == 128) != sift)
+    return cvb_fail(ctx, CVB_ERR_INVALID, "%s: the database holds %s descriptors", fn, db->desc_bytes == 128 ? "SIFT" : "ORB");
+  return CVB_OK;
+}
+
+int check_rows_per_kf(cvb_ctx* ctx, const cvb_db* db, const void* rows, const int32_t* rows_per_kf, int n_kf, const char* fn,
+                      int64_t* add) {
+  CVB_REQUIRE(ctx, n_kf >= 0 && (n_kf == 0 || rows_per_kf), "%s: bad arguments", fn);
+  *add = 0;
+  for (int i = 0; i < n_kf; ++i) {
+    CVB_REQUIRE(ctx, rows_per_kf[i] >= 0, "%s: negative row count", fn);
+    *add += rows_per_kf[i];
+  }
+  CVB_REQUIRE(ctx, db->seg_ptr.back() + *add < (int64_t)1 << 31, "%s: more than 2^31 rows", fn);
+  CVB_REQUIRE(ctx, *add == 0 || rows, "%s: null rows", fn);
+  return CVB_OK;
+}
+
+// appends checked keyframes whose rows are already in the database's u8 layout (host memory)
+int append_rows(cvb_ctx* ctx, cvb_db* db, const uint8_t* rows, const int32_t* rows_per_kf, int n_kf, int64_t add) {
+  const int64_t have = db->seg_ptr.back();
+  if ((size_t)(have + add) > db->cap_rows) {
+    const int rc = cvb_db_reserve(ctx, db, std::max<int64_t>(have + add, (int64_t)(db->cap_rows * 3 / 2)));
+    if (rc) return rc;
+  }
+  if (add) {
+    CVB_CUDA(ctx, cudaMemcpyAsync(db->d_rows + (size_t)have * db->desc_bytes, rows, (size_t)add * db->desc_bytes,
+                                  cudaMemcpyHostToDevice, ctx->stream));
+    CVB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));  // `rows` may be freed by the caller on return
+  }
+  const int seg_old = (int)db->seg_ptr.size() - 1, tile_old = db->seg_tile.back();
+  for (int i = 0; i < n_kf; ++i) {
+    db->seg_ptr.push_back(db->seg_ptr.back() + rows_per_kf[i]);
+    db->seg_tile.push_back(db->seg_tile.back() + (rows_per_kf[i] + 127) / 128);
+  }
+  db->seg_dirty = true;
+  // the new keyframes' operand tiles (HBM-bound, once per keyframe; every later query reads them through the TMA engine)
+  int rc = reserve_tiles(ctx, db, (size_t)db->seg_tile.back(), (size_t)tile_old);
+  if (rc) return rc;
+  if ((rc = refresh_seg(ctx, db))) return rc;
+  rc = cvb_tc::expand_tiles(ctx, db->metric(), db->d_rows, db->d_seg, db->d_seg_tile, seg_old, seg_old + n_kf, tile_old,
+                            db->seg_tile.back() - tile_old, db->d_xt, ctx->stream);
+  if (rc) return rc;
+  CVB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  return CVB_OK;
+}
+
+// the filtered 2-NN of the device query d_q (database layout) against every keyframe, dense device outputs; the keyframes
+// are matched from their resident operand tiles when the tensor-core kernel runs
+int match_dev(cvb_ctx* ctx, cvb_db* db, const uint8_t* d_q, int nq, float thr, float ratio, int32_t* d_mt, float* d_md, int32_t* d_nm,
+              void* stream) {
+  const int n_seg = (int)db->seg_ptr.size() - 1;
+  int rc = refresh_seg(ctx, db);
+  if (rc) return rc;
+  ctx->xt_for = db->d_rows; ctx->xt = db->d_xt; ctx->xt_seg_tile = db->d_seg_tile;
+  rc = db->desc_bytes == 32
+           ? cvb_match_hamming_batch_dev(ctx, d_q, nq, db->d_rows, db->d_seg, db->seg_ptr.data(), n_seg, thr, ratio, d_mt, d_md, d_nm, stream)
+           : cvb_match_l2_u8_dev(ctx, d_q, nq, db->d_rows, db->d_seg, db->seg_ptr.data(), n_seg, thr, ratio, d_mt, d_md, d_nm, stream);
+  ctx->xt_for = nullptr; ctx->xt = nullptr; ctx->xt_seg_tile = nullptr;
+  return rc;
+}
+
+// host request: q = ORB rows (u8) or SIFT rows (CV_32F, checked and quantised into the pinned staging buffer before any device
+// work); accepted matches compacted by (keyframe, queryIdx)
+int match_host(cvb_ctx* ctx, cvb_db* db, const void* q, int nq, float thr, float ratio, int32_t* n_matches, int32_t* m_kf,
+               int32_t* m_query, int32_t* m_train, float* m_dist, int cap, int32_t* n_total, const char* fn) {
+  const int n_seg = (int)db->seg_ptr.size() - 1;
+  CVB_REQUIRE(ctx, nq >= 0 && cap >= 0 && n_total && (nq == 0 || q), "%s: bad arguments", fn);
+  CVB_REQUIRE(ctx, cap == 0 || (m_kf && m_query && m_train && m_dist), "%s: null outputs", fn);
+  *n_total = 0;
+  const size_t qb = (size_t)nq * db->desc_bytes;
+  // pinned staging: [query | counts | offsets tail]
+  const size_t pin_q = (qb + 255) & ~(size_t)255;
+  uint8_t* pin = (uint8_t*)cvb_pinned(ctx, pin_q + (size_t)(n_seg + 1) * 4 + 64);
+  if (!pin) return CVB_ERR_CUDA;
+  if (db->desc_bytes == 32) memcpy(pin, q, qb);
+  else if (!cvb_quantize_sift((const float*)q, qb, pin))
+    return cvb_fail(ctx, CVB_ERR_UNSUPPORTED, "%s: SIFT descriptors must be integer-valued in [0,255] (cv::xfeatures2d::SIFT output)", fn);
+  if (n_seg == 0) return CVB_OK;
+  if (nq == 0) {
+    if (n_matches) std::fill(n_matches, n_matches + n_seg, 0);
+    return CVB_OK;
+  }
+  cudaStream_t st = ctx->stream;
+  int rc;
+  const size_t on = (size_t)n_seg * nq;
+  if ((rc = grow(ctx, db->q, qb))) return rc;
+  if ((rc = grow(ctx, db->mt, on * 4))) return rc;
+  if ((rc = grow(ctx, db->md, on * 4))) return rc;
+  if ((rc = grow(ctx, db->nm, (size_t)n_seg * 4))) return rc;
+  if ((rc = grow(ctx, db->off, (size_t)(n_seg + 1) * 4))) return rc;
+  if (cap) {
+    if ((rc = grow(ctx, db->out_seg, (size_t)cap * 4))) return rc;
+    if ((rc = grow(ctx, db->out_q, (size_t)cap * 4))) return rc;
+    if ((rc = grow(ctx, db->out_t, (size_t)cap * 4))) return rc;
+    if ((rc = grow(ctx, db->out_d, (size_t)cap * 4))) return rc;
+  }
+  CVB_CUDA(ctx, cudaMemcpyAsync(db->q.p, pin, qb, cudaMemcpyHostToDevice, st));
+  rc = match_dev(ctx, db, (const uint8_t*)db->q.p, nq, thr, ratio, (int32_t*)db->mt.p, (float*)db->md.p, (int32_t*)db->nm.p, nullptr);
+  if (rc) return rc;
+  db_offsets_kernel<<<1, 1024, 0, st>>>((const int32_t*)db->nm.p, n_seg, (int32_t*)db->off.p);
+  CVB_CHECK_LAUNCH(ctx);
+  if (cap) {
+    db_compact_kernel<<<(n_seg + 7) / 8, 256, 0, st>>>((const int32_t*)db->mt.p, (const float*)db->md.p, nq, n_seg,
+                                                       (const int32_t*)db->off.p, cap, (int32_t*)db->out_seg.p,
+                                                       (int32_t*)db->out_q.p, (int32_t*)db->out_t.p,
+                                                       (float*)db->out_d.p);
+    CVB_CHECK_LAUNCH(ctx);
+  }
+  int32_t* pin_cnt = (int32_t*)(pin + pin_q);
+  int32_t* pin_tot = pin_cnt + n_seg;
+  CVB_CUDA(ctx, cudaMemcpyAsync(pin_cnt, db->nm.p, (size_t)n_seg * 4, cudaMemcpyDeviceToHost, st));
+  CVB_CUDA(ctx, cudaMemcpyAsync(pin_tot, (int32_t*)db->off.p + n_seg, 4, cudaMemcpyDeviceToHost, st));
+  CVB_CUDA(ctx, cudaStreamSynchronize(st));
+  const int total = *pin_tot;
+  *n_total = total;
+  if (n_matches) memcpy(n_matches, pin_cnt, (size_t)n_seg * 4);
+  const int n_out = std::min(total, cap);
+  if (n_out) {
+    CVB_CUDA(ctx, cudaMemcpyAsync(m_kf, db->out_seg.p, (size_t)n_out * 4, cudaMemcpyDeviceToHost, st));
+    CVB_CUDA(ctx, cudaMemcpyAsync(m_query, db->out_q.p, (size_t)n_out * 4, cudaMemcpyDeviceToHost, st));
+    CVB_CUDA(ctx, cudaMemcpyAsync(m_train, db->out_t.p, (size_t)n_out * 4, cudaMemcpyDeviceToHost, st));
+    CVB_CUDA(ctx, cudaMemcpyAsync(m_dist, db->out_d.p, (size_t)n_out * 4, cudaMemcpyDeviceToHost, st));
+    CVB_CUDA(ctx, cudaStreamSynchronize(st));
+  }
+  return CVB_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -160,8 +293,8 @@ int cvb_db_create(cvb_ctx* ctx, int desc_bytes, cvb_db** out) {
   if (!ctx || !out) return CVB_ERR_INVALID;
   CVB_GUARD(ctx);
   *out = nullptr;
-  if (desc_bytes != 32)
-    return cvb_fail(ctx, CVB_ERR_UNSUPPORTED, "descriptor database: only 32-byte ORB descriptors, got %d", desc_bytes);
+  if (desc_bytes != 32 && desc_bytes != 128)
+    return cvb_fail(ctx, CVB_ERR_UNSUPPORTED, "descriptor database: 32-byte ORB or 128-byte SIFT descriptors, got %d", desc_bytes);
   cvb_db* db = new cvb_db();
   db->desc_bytes = desc_bytes;
   *out = db;
@@ -199,39 +332,25 @@ int cvb_db_reserve(cvb_ctx* ctx, cvb_db* db, int64_t rows) {
 int cvb_db_append(cvb_ctx* ctx, cvb_db* db, const uint8_t* rows, const int32_t* rows_per_kf, int n_kf) {
   if (!ctx || !db) return CVB_ERR_INVALID;
   CVB_GUARD(ctx);
-  CVB_REQUIRE(ctx, n_kf >= 0 && (n_kf == 0 || rows_per_kf), "cvb_db_append: bad arguments");
   int64_t add = 0;
-  for (int i = 0; i < n_kf; ++i) {
-    CVB_REQUIRE(ctx, rows_per_kf[i] >= 0, "cvb_db_append: negative row count");
-    add += rows_per_kf[i];
-  }
-  const int64_t have = db->seg_ptr.back();
-  CVB_REQUIRE(ctx, have + add < (int64_t)1 << 31, "cvb_db_append: more than 2^31 rows");
-  CVB_REQUIRE(ctx, add == 0 || rows, "cvb_db_append: null rows");
-  if ((size_t)(have + add) > db->cap_rows) {
-    const int rc = cvb_db_reserve(ctx, db, std::max<int64_t>(have + add, (int64_t)(db->cap_rows * 3 / 2)));
-    if (rc) return rc;
-  }
-  if (add) {
-    CVB_CUDA(ctx, cudaMemcpyAsync(db->d_rows + (size_t)have * db->desc_bytes, rows, (size_t)add * db->desc_bytes,
-                                  cudaMemcpyHostToDevice, ctx->stream));
-    CVB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));  // `rows` may be freed by the caller on return
-  }
-  const int seg_old = (int)db->seg_ptr.size() - 1, tile_old = db->seg_tile.back();
-  for (int i = 0; i < n_kf; ++i) {
-    db->seg_ptr.push_back(db->seg_ptr.back() + rows_per_kf[i]);
-    db->seg_tile.push_back(db->seg_tile.back() + (rows_per_kf[i] + 127) / 128);
-  }
-  db->seg_dirty = true;
-  // the new keyframes' operand tiles (HBM-bound, once per keyframe; every later query reads them through the TMA engine)
-  int rc = reserve_tiles(ctx, db, (size_t)db->seg_tile.back(), (size_t)tile_old);
-  if (rc) return rc;
-  if ((rc = refresh_seg(ctx, db))) return rc;
-  rc = cvb_tc::expand_tiles(ctx, db->d_rows, db->d_seg, db->d_seg_tile, seg_old, seg_old + n_kf, tile_old,
-                            db->seg_tile.back() - tile_old, db->d_xt, ctx->stream);
-  if (rc) return rc;
-  CVB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-  return CVB_OK;
+  int rc;
+  if ((rc = require_kind(ctx, db, false, "cvb_db_append")) || (rc = check_rows_per_kf(ctx, db, rows, rows_per_kf, n_kf, "cvb_db_append", &add)))
+    return rc;
+  return append_rows(ctx, db, rows, rows_per_kf, n_kf, add);
+}
+
+int cvb_db_append_sift(cvb_ctx* ctx, cvb_db* db, const float* rows, const int32_t* rows_per_kf, int n_kf) {
+  if (!ctx || !db) return CVB_ERR_INVALID;
+  CVB_GUARD(ctx);
+  int64_t add = 0;
+  int rc;
+  if ((rc = require_kind(ctx, db, true, "cvb_db_append_sift")) ||
+      (rc = check_rows_per_kf(ctx, db, rows, rows_per_kf, n_kf, "cvb_db_append_sift", &add)))
+    return rc;
+  std::vector<uint8_t> u8((size_t)add * 128);   // checked and quantised while staged: a refusal leaves the database unchanged
+  if (!cvb_quantize_sift(rows, u8.size(), u8.data()))
+    return cvb_fail(ctx, CVB_ERR_UNSUPPORTED, "cvb_db_append_sift: SIFT descriptors must be integer-valued in [0,255] (cv::xfeatures2d::SIFT output)");
+  return append_rows(ctx, db, u8.data(), rows_per_kf, n_kf, add);
 }
 
 int cvb_db_remove(cvb_ctx* ctx, cvb_db* db, int kf_index) {
@@ -251,7 +370,7 @@ int cvb_db_remove(cvb_ctx* ctx, cvb_db* db, int kf_index) {
     CVB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
   }
   {   // the same for the operand tiles
-    const size_t tb = cvb_tc::tile_bytes();
+    const size_t tb = cvb_tc::tile_bytes(db->metric());
     const int ta = db->seg_tile[kf_index], tbn = db->seg_tile[kf_index + 1], tend = db->seg_tile.back();
     const size_t ttail = (size_t)(tend - tbn) * tb;
     if (ttail && tbn > ta) {
@@ -283,16 +402,11 @@ int cvb_db_match_hamming_dev(cvb_ctx* ctx, cvb_db* db, const uint8_t* d_q, int n
                              int32_t* d_match_train, float* d_match_dist, int32_t* d_n_matches, void* stream) {
   if (!ctx || !db) return CVB_ERR_INVALID;
   CVB_GUARD(ctx);
+  if (const int rc = require_kind(ctx, db, false, "cvb_db_match_hamming_dev")) return rc;
   const int n_seg = (int)db->seg_ptr.size() - 1;
   CVB_REQUIRE(ctx, nq >= 0 && (nq == 0 || d_q) && (n_seg == 0 || d_n_matches), "cvb_db_match_hamming_dev: bad arguments");
   if (n_seg == 0) return CVB_OK;
-  int rc = refresh_seg(ctx, db);
-  if (rc) return rc;
-  ctx->xt_for = db->d_rows; ctx->xt = db->d_xt; ctx->xt_seg_tile = db->d_seg_tile;
-  rc = cvb_match_hamming_batch_dev(ctx, d_q, nq, db->d_rows, db->d_seg, db->seg_ptr.data(), n_seg, thr, ratio, d_match_train,
-                                   d_match_dist, d_n_matches, stream);
-  ctx->xt_for = nullptr; ctx->xt = nullptr; ctx->xt_seg_tile = nullptr;
-  return rc;
+  return match_dev(ctx, db, d_q, nq, thr, ratio, d_match_train, d_match_dist, d_n_matches, stream);
 }
 
 int cvb_db_match_hamming(cvb_ctx* ctx, cvb_db* db, const uint8_t* q, int nq, float thr, float ratio,
@@ -300,67 +414,28 @@ int cvb_db_match_hamming(cvb_ctx* ctx, cvb_db* db, const uint8_t* q, int nq, flo
                          int cap, int32_t* n_total) {
   if (!ctx || !db) return CVB_ERR_INVALID;
   CVB_GUARD(ctx);
+  if (const int rc = require_kind(ctx, db, false, "cvb_db_match_hamming")) return rc;
+  return match_host(ctx, db, q, nq, thr, ratio, n_matches, m_kf, m_query, m_train, m_dist, cap, n_total, "cvb_db_match_hamming");
+}
+
+int cvb_db_match_l2_dev(cvb_ctx* ctx, cvb_db* db, const uint8_t* d_q, int nq, float thr, float ratio,
+                        int32_t* d_match_train, float* d_match_dist, int32_t* d_n_matches, void* stream) {
+  if (!ctx || !db) return CVB_ERR_INVALID;
+  CVB_GUARD(ctx);
+  if (const int rc = require_kind(ctx, db, true, "cvb_db_match_l2_dev")) return rc;
   const int n_seg = (int)db->seg_ptr.size() - 1;
-  CVB_REQUIRE(ctx, nq >= 0 && cap >= 0 && n_total && (nq == 0 || q), "cvb_db_match_hamming: bad arguments");
-  CVB_REQUIRE(ctx, cap == 0 || (m_kf && m_query && m_train && m_dist), "cvb_db_match_hamming: null outputs");
-  *n_total = 0;
+  CVB_REQUIRE(ctx, nq >= 0 && (nq == 0 || d_q) && (n_seg == 0 || d_n_matches), "cvb_db_match_l2_dev: bad arguments");
   if (n_seg == 0) return CVB_OK;
-  if (nq == 0) {
-    if (n_matches) std::fill(n_matches, n_matches + n_seg, 0);
-    return CVB_OK;
-  }
-  cudaStream_t st = ctx->stream;
-  int rc;
-  if ((rc = refresh_seg(ctx, db))) return rc;
-  const size_t on = (size_t)n_seg * nq;
-  if ((rc = grow(ctx, db->q, (size_t)nq * 32))) return rc;
-  if ((rc = grow(ctx, db->mt, on * 4))) return rc;
-  if ((rc = grow(ctx, db->md, on * 4))) return rc;
-  if ((rc = grow(ctx, db->nm, (size_t)n_seg * 4))) return rc;
-  if ((rc = grow(ctx, db->off, (size_t)(n_seg + 1) * 4))) return rc;
-  if (cap) {
-    if ((rc = grow(ctx, db->out_seg, (size_t)cap * 4))) return rc;
-    if ((rc = grow(ctx, db->out_q, (size_t)cap * 4))) return rc;
-    if ((rc = grow(ctx, db->out_t, (size_t)cap * 4))) return rc;
-    if ((rc = grow(ctx, db->out_d, (size_t)cap * 4))) return rc;
-  }
-  // pinned staging: [query | counts | offsets tail]
-  const size_t pin_q = ((size_t)nq * 32 + 255) & ~(size_t)255;
-  uint8_t* pin = (uint8_t*)cvb_pinned(ctx, pin_q + (size_t)(n_seg + 1) * 4 + 64);
-  if (!pin) return CVB_ERR_CUDA;
-  memcpy(pin, q, (size_t)nq * 32);
-  CVB_CUDA(ctx, cudaMemcpyAsync(db->q.p, pin, (size_t)nq * 32, cudaMemcpyHostToDevice, st));
-  ctx->xt_for = db->d_rows; ctx->xt = db->d_xt; ctx->xt_seg_tile = db->d_seg_tile;   // resident operand tiles of these rows
-  rc = cvb_match_hamming_batch_dev(ctx, (const uint8_t*)db->q.p, nq, db->d_rows, db->d_seg, db->seg_ptr.data(), n_seg,
-                                   thr, ratio, (int32_t*)db->mt.p, (float*)db->md.p, (int32_t*)db->nm.p, nullptr);
-  ctx->xt_for = nullptr; ctx->xt = nullptr; ctx->xt_seg_tile = nullptr;
-  if (rc) return rc;
-  db_offsets_kernel<<<1, 1024, 0, st>>>((const int32_t*)db->nm.p, n_seg, (int32_t*)db->off.p);
-  CVB_CHECK_LAUNCH(ctx);
-  if (cap) {
-    db_compact_kernel<<<(n_seg + 7) / 8, 256, 0, st>>>((const int32_t*)db->mt.p, (const float*)db->md.p, nq, n_seg,
-                                                       (const int32_t*)db->off.p, cap, (int32_t*)db->out_seg.p,
-                                                       (int32_t*)db->out_q.p, (int32_t*)db->out_t.p,
-                                                       (float*)db->out_d.p);
-    CVB_CHECK_LAUNCH(ctx);
-  }
-  int32_t* pin_cnt = (int32_t*)(pin + pin_q);
-  int32_t* pin_tot = pin_cnt + n_seg;
-  CVB_CUDA(ctx, cudaMemcpyAsync(pin_cnt, db->nm.p, (size_t)n_seg * 4, cudaMemcpyDeviceToHost, st));
-  CVB_CUDA(ctx, cudaMemcpyAsync(pin_tot, (int32_t*)db->off.p + n_seg, 4, cudaMemcpyDeviceToHost, st));
-  CVB_CUDA(ctx, cudaStreamSynchronize(st));
-  const int total = *pin_tot;
-  *n_total = total;
-  if (n_matches) memcpy(n_matches, pin_cnt, (size_t)n_seg * 4);
-  const int n_out = std::min(total, cap);
-  if (n_out) {
-    CVB_CUDA(ctx, cudaMemcpyAsync(m_kf, db->out_seg.p, (size_t)n_out * 4, cudaMemcpyDeviceToHost, st));
-    CVB_CUDA(ctx, cudaMemcpyAsync(m_query, db->out_q.p, (size_t)n_out * 4, cudaMemcpyDeviceToHost, st));
-    CVB_CUDA(ctx, cudaMemcpyAsync(m_train, db->out_t.p, (size_t)n_out * 4, cudaMemcpyDeviceToHost, st));
-    CVB_CUDA(ctx, cudaMemcpyAsync(m_dist, db->out_d.p, (size_t)n_out * 4, cudaMemcpyDeviceToHost, st));
-    CVB_CUDA(ctx, cudaStreamSynchronize(st));
-  }
-  return CVB_OK;
+  return match_dev(ctx, db, d_q, nq, thr, ratio, d_match_train, d_match_dist, d_n_matches, stream);
+}
+
+int cvb_db_match_l2(cvb_ctx* ctx, cvb_db* db, const float* q, int nq, float thr, float ratio,
+                    int32_t* n_matches, int32_t* m_kf, int32_t* m_query, int32_t* m_train, float* m_dist,
+                    int cap, int32_t* n_total) {
+  if (!ctx || !db) return CVB_ERR_INVALID;
+  CVB_GUARD(ctx);
+  if (const int rc = require_kind(ctx, db, true, "cvb_db_match_l2")) return rc;
+  return match_host(ctx, db, q, nq, thr, ratio, n_matches, m_kf, m_query, m_train, m_dist, cap, n_total, "cvb_db_match_l2");
 }
 
 }  // extern "C"

@@ -1206,3 +1206,9 @@ int cvb_landmark_match_batch(cvb_ctx* ctx, const uint8_t* A, const uint8_t* skip
 }
 
 }  // extern "C"
+
+int cvb_match_l2_u8_dev(cvb_ctx* ctx, const uint8_t* d_q, int nq, const uint8_t* d_t, const int32_t* d_seg_ptr, const int32_t* h_seg_ptr,
+                        int n_seg, float thr, float ratio, int32_t* d_match_train, float* d_match_dist, int32_t* d_n_matches, void* stream) {
+  return knn_dev<L2Metric, 2>(ctx, d_q, nq, d_t, d_seg_ptr, h_seg_ptr, n_seg, 2, nullptr, nullptr, true, thr, ratio, d_match_train,
+                              d_match_dist, d_n_matches, cvb_stream(ctx, stream));
+}

@@ -1009,6 +1009,24 @@ extern "C" int cvb_noncentral_relative_pose_covariance_seeded_batch(cvb_ctx* ctx
 // verify_merge_kernel (5-point inliers -> 17-point problems), ransac_rel_kernel<Solver17>, rel_cov_solve_kernel / rel_cov_reduce_kernel
 // and verify_list_kernel (the correspondence list), all on the arrays of one device block (cvb_block).  The correspondence arrays are sized
 // by the host-known bound sum over pairings of rows(kf1); the problems are packed to the front in pairing (candidate) order.
+// SIFT rows (CV_32F) to the u8 layout of the L2 scan in one pass; false if a value is not an integer in [0, 255] (NaN and
+// +-inf included).  This is quantize_u8_kernel's test rintf(v) == v && 0 <= v <= 255 (checked equal on every float bit
+// pattern), written without branches or conversions so that the loop vectorises and runs at copy speed: c = v + 1.5 * 2^23
+// rounds v to an integer held in c's low mantissa bits (|v| < 2^22), and c - 1.5 * 2^23 == v holds exactly when v is one.
+// Needs IEEE arithmetic (no -ffast-math).
+bool cvb_quantize_sift(const float* src, size_t n, uint8_t* dst) {
+  int bad = 0;
+  for (size_t i = 0; i < n; i++) {
+    const float v = src[i];
+    const float c = v + 12582912.f;
+    int32_t bits;
+    memcpy(&bits, &c, 4);
+    bad |= (c - 12582912.f != v) | (v < 0.f) | (v > 255.f);
+    dst[i] = (uint8_t)(bits - 0x4B400000);   // the bits of 1.5 * 2^23
+  }
+  return bad == 0;
+}
+
 namespace {
 
 struct VerifyDev {
@@ -1087,23 +1105,6 @@ __global__ void __launch_bounds__(kGlueThreads) verify_list_kernel(VerifyDev V) 
   }
 }
 
-// SIFT rows (CV_32F) to the u8 layout of the L2 scan in one pass; false if a value is not an integer in [0, 255] (NaN and
-// +-inf included).  This is quantize_u8_kernel's test rintf(v) == v && 0 <= v <= 255 (checked equal on every float bit
-// pattern), written without branches or conversions so that the loop vectorises and runs at copy speed: c = v + 1.5 * 2^23
-// rounds v to an integer held in c's low mantissa bits (|v| < 2^22), and c - 1.5 * 2^23 == v holds exactly when v is one.
-// Needs IEEE arithmetic (no -ffast-math).
-bool quantize_sift(const float* src, size_t n, uint8_t* dst) {
-  int bad = 0;
-  for (size_t i = 0; i < n; i++) {
-    const float v = src[i];
-    const float c = v + 12582912.f;
-    int32_t bits;
-    memcpy(&bits, &c, 4);
-    bad |= (c - 12582912.f != v) | (v < 0.f) | (v > 255.f);
-    dst[i] = (uint8_t)(bits - 0x4B400000);   // the bits of 1.5 * 2^23
-  }
-  return bad == 0;
-}
 
 // cvb_verify_noncentral_relative_pose{,_sift}_seeded_batch: KF is cvb_verify_keyframes (ORB rows, staged as they are, matched by
 // the Hamming pair scan) or cvb_verify_keyframes_sift (SIFT rows, checked and quantised to u8 while staged, matched by the L2 one)
@@ -1161,7 +1162,7 @@ int verify_noncentral(cvb_ctx* ctx, const KF* kf, const cvb_verify_candidates* c
   std::vector<uint8_t> q8;   // the SIFT rows quantised; their check is an argument check, so it comes before the device block
   if constexpr (kSift) {
     q8.resize(R * 128);
-    if (!quantize_sift(kf->desc, R * 128, q8.data()))
+    if (!cvb_quantize_sift(kf->desc, R * 128, q8.data()))
       return cvb_fail(ctx, CVB_ERR_UNSUPPORTED, "%s: SIFT descriptors must be integer-valued in [0,255] (cv::xfeatures2d::SIFT output)", name);
   }
   const std::vector<double> rig1 = pack_cams(cd->cam_off1, cd->cam_rot1, NC1), rig2 = pack_cams(cd->cam_off2, cd->cam_rot2, NC2);

@@ -1,6 +1,6 @@
 // tc_match.cu — descriptor k-NN on the Hopper tensor cores (wgmma.mma_async, integer kinds, accumulators in registers).
 //
-// Same contract as scan_kernel in match_kernels.cu (K1 Hamming / K2 L2 / K3 DenseMatcher lists), different bound.
+// Same contract as scan_kernel in match_kernels.cu (K1 Hamming / K2 L2 lists), different bound.
 // The POPC formulation is bound by the integer pipe.  Here the pairwise term is a u8 x u8 -> s32 GEMM:
 //     Hamming(a,b) = popc(a) + popc(b) - 2 <bits(a), bits(b)>      (bits expanded to 0/1 bytes in shared memory)
 //     |a-b|^2      = |a|^2 + |b|^2 - 2 <a, b>                      (u8 SIFT, exact in s32)
@@ -10,7 +10,9 @@
 // keeps per-row k-lists with the sequential OpenCV / DenseMatcher rule, and the four threads of a quad merge their lists
 // by (key, index) at the end of a segment — so the result is bit-identical to the scalar kernel.
 //
-// Warp-specialised, persistent CTA (one per SM), 4-stage ring:
+// Both metrics run on operand tiles stored in the tensor core's own layout (namespace xt below).  tc_scan_kernel, the Hamming
+// kernel that expands the packed rows itself, stays behind COVINS_B200_TC_XT=0:
+// warp-specialised, persistent CTA (one per SM), 4-stage ring:
 //   warps 0-7   consumers  (two warpgroups, query rows [0, 64) and [64, 128)): wait full[s] → K/32 x wgmma → wait →
 //                          empty[s] → epilogue d = pt[j] - 2 acc (+ pq) → k-lists
 //   warps 8-15  producers  wait empty[s] → read packed rows from HBM (coalesced 16-B loads) → expand / copy into the
@@ -62,10 +64,20 @@ __device__ __forceinline__ void wg_mma_i8(uint32_t (&d)[64], uint64_t adesc, uin
         : CVB_D64 : "l"(adesc), "l"(bdesc), "r"(acc));
   }
 }
+#define CVB_D32 CVB_D8(0), CVB_D8(8), CVB_D8(16), CVB_D8(24)
+#define CVB_R32 "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}"
+// D[64 x 64] (+)= A[64 x 32] B[64 x 32]^T, u8 x u8 (the L2 tiles: half the accumulator registers of m64n128)
+__device__ __forceinline__ void wg_mma_u8_n64(uint32_t (&d)[32], uint64_t adesc, uint64_t bdesc, uint32_t acc) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %34, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n64k32.s32.u8.u8 " CVB_R32 ", %32, %33, p;\n}\n"
+      : CVB_D32 : "l"(adesc), "l"(bdesc), "r"(acc));
+}
 // the accumulator registers are written asynchronously: keep the compiler from moving their uses across the fence / wait
-__device__ __forceinline__ void wg_fence_operands(uint32_t (&d)[64]) {
+template <int N>
+__device__ __forceinline__ void wg_fence_operands(uint32_t (&d)[N]) {
 #pragma unroll
-  for (int i = 0; i < 64; i++) asm volatile("" : "+r"(d[i])::"memory");
+  for (int i = 0; i < N; i++) asm volatile("" : "+r"(d[i])::"memory");
 }
 __device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wg_commit_wait() {
@@ -80,6 +92,15 @@ __device__ __forceinline__ void wg_gemm(uint32_t (&d)[64], uint64_t adesc0, uint
   wg_fence();
 #pragma unroll
   for (int k = 0; k < NSLICE; k++) wg_mma_i8<B_SIGNED>(d, adesc0 + (uint64_t)(k * 16), bdesc0 + (uint64_t)(k * 16), k > 0 ? 1u : 0u);
+  wg_commit_wait();
+  wg_fence_operands(d);
+}
+template <int NSLICE>
+__device__ __forceinline__ void wg_gemm_u8_n64(uint32_t (&d)[32], uint64_t adesc0, uint64_t bdesc0) {
+  wg_fence_operands(d);
+  wg_fence();
+#pragma unroll
+  for (int k = 0; k < NSLICE; k++) wg_mma_u8_n64(d, adesc0 + (uint64_t)(k * 16), bdesc0 + (uint64_t)(k * 16), k > 0 ? 1u : 0u);
   wg_commit_wait();
   wg_fence_operands(d);
 }
@@ -113,7 +134,6 @@ struct TcHamming {
   static constexpr int kKBytes = 256;     // operand bytes (one byte per bit)
   static constexpr int kLoads = 1;        // uint4 per half row
   static constexpr int kPrefetch = 3;     // tiles in flight per producer thread
-  static constexpr bool kIsL2 = false;
   static __device__ __forceinline__ void load_half(const uint8_t* __restrict__ row, int half, uint4 (&v)[kLoads]) {
     v[0] = ldg_nc(row + 16 * half);
   }
@@ -153,12 +173,10 @@ struct TcHamming {
     for (int b = 0; b < 8; b++) r[b] = (w[i] >> b) & 0x01010101u;
   }
 };
+// u8 SIFT rows: the operand row is the row itself; the additive term is |row|^2 (the L2 operand tiles, namespace xt)
 struct TcL2 {
   static constexpr int kRowBytes = 128;
-  static constexpr int kKBytes = 128;
   static constexpr int kLoads = 4;
-  static constexpr int kPrefetch = 2;
-  static constexpr bool kIsL2 = true;
   static __device__ __forceinline__ void load_half(const uint8_t* __restrict__ row, int half, uint4 (&v)[kLoads]) {
 #pragma unroll
     for (int c = 0; c < 4; c++) v[c] = ldg_nc(row + 64 * half + 16 * c);
@@ -172,7 +190,6 @@ struct TcL2 {
     }
     return (int)n2;
   }
-  static constexpr int kQWords = 4;   // 128 operand bytes per row = 4 groups of 32
   static __device__ __forceinline__ int load_q(const uint8_t* __restrict__ row, uint32_t (&w)[32]) {
     unsigned n2 = 0;
 #pragma unroll
@@ -337,13 +354,13 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tc_scan_kernel(const TcParams 
   }
   if (tid < TM) {
     const int q = qb * TM + tid;
-    uint32_t w[M::kIsL2 ? 32 : 8];
+    uint32_t w[8];
     int nrm = 0;
     if (q < p.nq) {
       nrm = M::load_q(p.q + (size_t)q * M::kRowBytes, w);
     } else {
 #pragma unroll
-      for (int i = 0; i < (M::kIsL2 ? 32 : 8); i++) w[i] = 0;
+      for (int i = 0; i < 8; i++) w[i] = 0;
     }
     sQNorm[tid] = nrm;
     uint8_t* dst = sA + row_offset<KB>(tid);
@@ -413,10 +430,8 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tc_scan_kernel(const TcParams 
           for (int c = 0; c < KB / 32; c++) *reinterpret_cast<uint4*>(dst + (half * (KB / 32) + c) * 128) = make_uint4(0, 0, 0, 0);
         }
         part += __shfl_xor_sync(0xffffffffu, part, 8);   // the two halves of a row sit 8 lanes apart
-        if (M::kIsL2) {
-          if (half == 0) sNorm[(n % NORM_RING) * TN + prow] = rv ? part : kInf;
-        } else if (half == 0) {
-          // Hamming: 16-bit column term ((popc(row) + 256) << 5 | slot), slot = 2 (column / 8) + column % 2 — the position
+        if (half == 0) {
+          // 16-bit column term ((popc(row) + 256) << 5 | slot), slot = 2 (column / 8) + column % 2 — the position
           // of the column among the 32 columns one consumer thread holds; 0xFFFF = no row
           reinterpret_cast<uint16_t*>(sNorm)[(n % NORM_RING) * TN + prow] =
               rv ? (uint16_t)(((part + 256) << 5) | ((prow >> 3) << 1) | (prow & 1)) : (uint16_t)0xFFFFu;
@@ -438,16 +453,12 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tc_scan_kernel(const TcParams 
     const int qn0 = sQNorm[row0], qn1 = sQNorm[row0 + 8];
     const uint64_t a_desc = make_desc(cvb_smem_addr(sA + (size_t)h * 64 * KB), 128, KB * 8);
     const uint32_t b_addr0 = cvb_smem_addr(sB);
-    int wk0[K], wi0[K], wd0[K], wk1[K], wi1[K], wd1[K];   // key, index, raw integer distance (pre-test only) per row
+    int wk0[K], wk1[K];   // packed (distance, index) keys per row
     int n = 0;
     for (int seg = seg0; seg < seg1; seg++) {
       const int len = p.seg_ptr[seg + 1] - p.seg_ptr[seg];
 #pragma unroll
-      for (int c = 0; c < K; c++) {
-        wk0[c] = wk1[c] = M::kIsL2 ? kInfKey : INT_MAX;
-        wi0[c] = wi1[c] = -1;
-        wd0[c] = wd1[c] = kInf;
-      }
+      for (int c = 0; c < K; c++) wk0[c] = wk1[c] = INT_MAX;
       for (int r0 = 0; r0 < len; r0 += TN, n++) {
         const int s = n % STAGES;
         cvb_mbar_wait(&full[s], (n / STAGES) & 1);
@@ -455,7 +466,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tc_scan_kernel(const TcParams 
         wg_gemm<false, KB / 32>(acc, a_desc, make_desc(b_addr0 + (uint32_t)s * (TN * KB), 128, KB * 8));
         __syncwarp();
         if (lane == 0) mbar_arrive(&empty[s]);   // operands consumed: the producers may refill this stage
-        if (!M::kIsL2) {
+        {
           // Two columns per instruction: 16-bit keys ((popc(t) - 2 popc(q & t) + 256) << 5 | slot) packed pairwise
           // (even column low, odd column high), k-lists kept per half with packed 16-bit min/max, merged into the 32-bit
           // (distance, index) lists once per tile — and only if the tile holds a candidate that beats the current k-th
@@ -488,64 +499,30 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tc_scan_kernel(const TcParams 
                 }
             }
           }
-        } else {
-          const int* nrm = sNorm + (n % NORM_RING) * TN;
-#pragma unroll
-          for (int i = 0; i < 16; i++) {
-            const int2 nn = *reinterpret_cast<const int2*>(nrm + 8 * i + 2 * quad);
-#pragma unroll
-            for (int e = 0; e < 4; e++) {
-              const int j = 8 * i + 2 * quad + (e & 1);
-              const int tn = (e & 1) ? nn.y : nn.x;
-              int (&wk)[K] = e < 2 ? wk0 : wk1;
-              int (&wi)[K] = e < 2 ? wi0 : wi1;
-              int (&wd)[K] = e < 2 ? wd0 : wd1;
-              const int d = (e < 2 ? qn0 : qn1) + tn - 2 * (int)acc[4 * i + e];
-              if (d < wd[K - 1]) {
-                const int key = __float_as_int(__fsqrt_rn((float)d));
-                if (key < wk[K - 1]) {
-                  insert_key<K>(wk, wi, key, r0 + j);
-                  const float f = __int_as_float(wk[K - 1]);   // raw-distance bound of the worst entry (pre-test)
-                  wd[K - 1] = wk[K - 1] == kInfKey ? kInf : (int)ceilf(f * f * 1.000001f) + 1;
-                }
-              }
-            }
-          }
         }
       }
       // ---- segment finished: merge the quad's lists; lane quad 0 writes row0, quad 1 writes row0 + 8 ----
       const bool second = quad == 1;
       int wk[K], wi[K];
       float fd[K];
-      if (!M::kIsL2) {
-        quad_merge_packed<K>(wk0);
-        quad_merge_packed<K>(wk1);
-        const int qq = (second ? qn1 : qn0) << kIdxBits;
+      quad_merge_packed<K>(wk0);
+      quad_merge_packed<K>(wk1);
+      const int qq = (second ? qn1 : qn0) << kIdxBits;
 #pragma unroll
-        for (int c = 0; c < K; c++) {
-          const int x = second ? wk1[c] : wk0[c];
-          wi[c] = x == INT_MAX ? -1 : (x & ((1 << kIdxBits) - 1));
-          wk[c] = x == INT_MAX ? INT_MAX : ((x + qq) >> kIdxBits);
-          fd[c] = (float)wk[c];
-        }
-      } else {
-        quad_merge_lex<K>(wk0, wi0);
-        quad_merge_lex<K>(wk1, wi1);
-#pragma unroll
-        for (int c = 0; c < K; c++) {
-          wk[c] = second ? wk1[c] : wk0[c];
-          wi[c] = second ? wi1[c] : wi0[c];
-          fd[c] = __int_as_float(wk[c]);
-        }
+      for (int c = 0; c < K; c++) {
+        const int x = second ? wk1[c] : wk0[c];
+        wi[c] = x == INT_MAX ? -1 : (x & ((1 << kIdxBits) - 1));
+        wk[c] = x == INT_MAX ? INT_MAX : ((x + qq) >> kIdxBits);
+        fd[c] = (float)wk[c];
       }
-      write_list<K, M::kIsL2>(p, seg, qb * TM + row0 + (second ? 8 : 0), quad < 2 && (second ? valid1 : valid0), wk, wi, fd, lane);
+      write_list<K, false>(p, seg, qb * TM + row0 + (second ? 8 : 0), quad < 2 && (second ? valid1 : valid0), wk, wi, fd, lane);
     }
   }
 }
 
 
 // ===================================================================================================================
-// Hamming k-NN on PRE-EXPANDED operand tiles.
+// k-NN on PRE-EXPANDED operand tiles (Hamming as described here; L2 on tiles of u8 rows + |t|^2, see XtL2 below).
 //
 // The kernel above spends its issue slots on ALU work: producers turn every packed bit into a byte (>= 64 logic
 // operations per row and tile) and the epilogue rebuilds the distance from the accumulator and a per-column term read
@@ -568,20 +545,38 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tc_scan_kernel(const TcParams 
 //     their epilogue the other's keep the tensor cores busy.  A (query, keyframe) list lives in one quad's registers
 //     from the first tile to the output — no shared-memory lists, no CTA barrier per keyframe.
 namespace xt {
-constexpr int KX = 288;                       // operand bytes per row
-constexpr int NSLICE = KX / 32;               // 9 instructions of K = 32 per tile
-constexpr int TILE_BYTES = TN * KX;           // 36864
-constexpr int XSTAGES = 5;                    // shared-memory ring (180 KB) — more than NGRP (phase parity of full[])
+// The two tile images.  Hamming: 288 operand bytes per row as above.  L2 (u8 SIFT rows): the 128 bytes of each row, K-major
+// without swizzle (8-row groups of 1024 B), then the tile's 128 per-row terms |t|^2 as int32 (kInf for rows past a keyframe's
+// end; 132 bytes of HBM per row).  The epilogue rebuilds d = |q|^2 + |t|^2 - 2 <q, t>, exact in s32, and keeps OpenCV's lists
+// on the float key sqrtf(d).  The norm stays outside the GEMM (-2 <q, t> with u8 rows has no u8 / s8 factorisation), so an L2
+// stage is released after its epilogue, which reads the norms from it.
+struct XtHamming {
+  static constexpr int KX = 288;                        // operand bytes per row
+  static constexpr int NSLICE = KX / 32;                // 9 instructions of K = 32 per tile
+  static constexpr int TILE_BYTES = TN * KX;            // 36864
+  static constexpr int STAGES = 5;                      // shared-memory ring (180 KB) — more than NGRP (phase parity of full[])
+  static constexpr bool kIsL2 = false;
+};
+struct XtL2 {
+  static constexpr int KX = 128;
+  static constexpr int NSLICE = KX / 32;                // 4
+  static constexpr int TILE_BYTES = TN * KX + TN * 4;   // 16896: data, then |t|^2 per row
+  static constexpr int STAGES = 8;
+  static constexpr bool kIsL2 = true;
+};
 constexpr int NGRP = 2;                       // streams
 constexpr int CONS_WARPS = 4 * 2 * NGRP;      // warpgroups (h, g), h = query half
 constexpr int TMA_WARP = CONS_WARPS;
 constexpr int XTHREADS = (TMA_WARP + 1) * 32;
-constexpr int kKeyInvalid = 32896;            // keys >= this are "no row"
-constexpr size_t kSmemBytes = (size_t)(XSTAGES + 1) * TILE_BYTES + 1024;   // query block + ring + barriers
-
-__device__ __forceinline__ uint32_t xrow_off(int r) { return (uint32_t)(r >> 3) * (KX * 8) + (uint32_t)(r & 7) * 16; }
+constexpr int kKeyInvalid = 32896;            // Hamming keys >= this are "no row"
+// shared-memory stride of a tile (the query block and every stage start on a 1 KB boundary)
+template <class X>
+constexpr int smem_stride() { return (X::TILE_BYTES + 1023) / 1024 * 1024; }
+template <class X>
+constexpr size_t smem_bytes_xt() { return (size_t)(X::STAGES + 1) * smem_stride<X>() + 1024; }   // query block + ring + barriers
 
 // ---- one-time expansion (also the append path of the map database) ----
+template <class X>
 __global__ void __launch_bounds__(256) expand_tiles_kernel(const uint8_t* __restrict__ t, const int32_t* __restrict__ seg_ptr,
                                                            const int32_t* __restrict__ seg_tile, int seg_lo, int seg_hi,
                                                            int tile_lo, uint8_t* __restrict__ out) {
@@ -594,27 +589,41 @@ __global__ void __launch_bounds__(256) expand_tiles_kernel(const uint8_t* __rest
   const int s_begin = seg_ptr[lo], len = seg_ptr[lo + 1] - s_begin, r0 = (tile - seg_tile[lo]) * TN;
   const int pt = threadIdx.x, prow = (pt & 7) | ((pt >> 4) << 3), half = (pt >> 3) & 1;
   const bool rv = r0 + prow < len;
-  uint8_t* dst = out + (size_t)tile * TILE_BYTES + xrow_off(prow);
+  uint8_t* tile_base = out + (size_t)tile * X::TILE_BYTES;
+  uint8_t* dst = tile_base + row_offset<X::KX>(prow);
   int part = 0;
-  if (rv) {
-    uint4 v[1];
-    TcHamming::load_half(t + (size_t)(s_begin + r0 + prow) * 32, half, v);
-    part = TcHamming::store_half<7>(v, half, dst);
-  } else {
-#pragma unroll
-    for (int c = 0; c < 8; c++) *reinterpret_cast<uint4*>(dst + (8 * half + c) * 128) = make_uint4(0, 0, 0, 0);
-  }
-  part += __shfl_xor_sync(0xffffffffu, part, 8);
-  if (half == 0) {
-    uint4 key = make_uint4(0x7F7F7F7Fu, 0, 0, 0);
+  if constexpr (X::kIsL2) {
     if (rv) {
-      const int p1 = min(part, 127), p2 = min(part - p1, 127), p3 = part - p1 - p2;
-      key.x = (uint32_t)prow | ((uint32_t)p1 << 8) | ((uint32_t)p2 << 16) | ((uint32_t)p3 << 24);
-      key.y = 0x00404040u;
+      uint4 v[TcL2::kLoads];
+      TcL2::load_half(t + (size_t)(s_begin + r0 + prow) * TcL2::kRowBytes, half, v);
+      part = TcL2::store_half(v, half, dst);
+    } else {
+#pragma unroll
+      for (int c = 0; c < 4; c++) *reinterpret_cast<uint4*>(dst + (4 * half + c) * 128) = make_uint4(0, 0, 0, 0);
     }
-    *reinterpret_cast<uint4*>(dst + 16 * 128) = key;
+    part += __shfl_xor_sync(0xffffffffu, part, 8);
+    if (half == 0) reinterpret_cast<int*>(tile_base + TN * X::KX)[prow] = rv ? part : kInf;
   } else {
-    *reinterpret_cast<uint4*>(dst + 17 * 128) = make_uint4(0, 0, 0, 0);
+    if (rv) {
+      uint4 v[1];
+      TcHamming::load_half(t + (size_t)(s_begin + r0 + prow) * 32, half, v);
+      part = TcHamming::store_half<7>(v, half, dst);
+    } else {
+#pragma unroll
+      for (int c = 0; c < 8; c++) *reinterpret_cast<uint4*>(dst + (8 * half + c) * 128) = make_uint4(0, 0, 0, 0);
+    }
+    part += __shfl_xor_sync(0xffffffffu, part, 8);
+    if (half == 0) {
+      uint4 key = make_uint4(0x7F7F7F7Fu, 0, 0, 0);
+      if (rv) {
+        const int p1 = min(part, 127), p2 = min(part - p1, 127), p3 = part - p1 - p2;
+        key.x = (uint32_t)prow | ((uint32_t)p1 << 8) | ((uint32_t)p2 << 16) | ((uint32_t)p3 << 24);
+        key.y = 0x00404040u;
+      }
+      *reinterpret_cast<uint4*>(dst + 16 * 128) = key;
+    } else {
+      *reinterpret_cast<uint4*>(dst + 17 * 128) = make_uint4(0, 0, 0, 0);
+    }
   }
 }
 
@@ -650,49 +659,70 @@ struct Streams {
   }
 };
 
-template <int K>
+template <class X, int K>
 __global__ void __launch_bounds__(XTHREADS, 1) tc_xt_kernel(const TcParams p) {
   extern __shared__ __align__(1024) uint8_t smem[];
-  uint8_t* sA = smem;                                  // the query block, one tile image [TM][KX]
-  uint8_t* sB = smem + TILE_BYTES;                     // [XSTAGES] tiles
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + (size_t)(XSTAGES + 1) * TILE_BYTES);
-  uint64_t* full = bars;                  // [XSTAGES] TMA bytes landed (expect_tx)
-  uint64_t* empty = bars + XSTAGES;       // [XSTAGES] the stage's two warpgroups finished their MMAs (one arrival per warp)
+  constexpr int KX = X::KX, STAGES_X = X::STAGES, STRIDE = smem_stride<X>();
+  uint8_t* sA = smem;                                  // the query block, one tile image [TM][KX] (+ L2: |q|^2 [TM])
+  uint8_t* sB = smem + STRIDE;                         // [STAGES_X] tiles
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + (size_t)(STAGES_X + 1) * STRIDE);
+  uint64_t* full = bars;                  // [STAGES_X] TMA bytes landed (expect_tx)
+  uint64_t* empty = bars + STAGES_X;      // [STAGES_X] the stage's two warpgroups are done with it (one arrival per warp)
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int qb = blockIdx.x % p.nqb, part = blockIdx.x / p.nqb;
   const int seg0 = (int)((long)part * p.n_seg / p.parts), seg1 = (int)((long)(part + 1) * p.n_seg / p.parts);
 
   if (tid == 0) {
-    for (int s = 0; s < XSTAGES; s++) { cvb_mbar_init(&full[s], 1); cvb_mbar_init(&empty[s], 8); }
+    for (int s = 0; s < STAGES_X; s++) { cvb_mbar_init(&full[s], 1); cvb_mbar_init(&empty[s], 8); }
     cvb_fence_mbar_init();
   }
   if (tid < TM) {
-    // query block → shared memory (thread = row): data bytes 0/2, then the key slice
     const int q = qb * TM + tid;
-    uint32_t w[8];
-    int pq = 0;
-    if (q < p.nq) {
-      pq = TcHamming::load_q(p.q + (size_t)q * 32, w);
+    uint8_t* dst = sA + row_offset<KX>(tid);
+    if constexpr (X::kIsL2) {
+      // query block → shared memory (thread = row): the u8 row in the tile layout, |q|^2 after the block
+      uint32_t w[32];
+      int n2 = 0;
+      if (q < p.nq) {
+        n2 = TcL2::load_q(p.q + (size_t)q * TcL2::kRowBytes, w);
+      } else {
+#pragma unroll
+        for (int i = 0; i < 32; i++) w[i] = 0;
+      }
+#pragma unroll
+      for (int i = 0; i < KX / 32; i++) {
+        uint32_t r[8];
+        TcL2::expand_q(w, i, r);
+        *reinterpret_cast<uint4*>(dst + (2 * i) * 128) = make_uint4(r[0], r[1], r[2], r[3]);
+        *reinterpret_cast<uint4*>(dst + (2 * i + 1) * 128) = make_uint4(r[4], r[5], r[6], r[7]);
+      }
+      reinterpret_cast<int*>(sA + TM * KX)[tid] = n2;
     } else {
+      // query block → shared memory (thread = row): data bytes 0/2, then the key slice
+      uint32_t w[8];
+      int pq = 0;
+      if (q < p.nq) {
+        pq = TcHamming::load_q(p.q + (size_t)q * 32, w);
+      } else {
 #pragma unroll
-      for (int i = 0; i < 8; i++) w[i] = 0;
-    }
-    uint8_t* dst = sA + xrow_off(tid);
+        for (int i = 0; i < 8; i++) w[i] = 0;
+      }
 #pragma unroll
-    for (int i = 0; i < 8; i++) {
-      uint32_t r[8];
+      for (int i = 0; i < 8; i++) {
+        uint32_t r[8];
 #pragma unroll
-      for (int b = 0; b < 8; b++) r[b] = ((w[i] >> b) & 0x01010101u) * 2u;
-      *reinterpret_cast<uint4*>(dst + (2 * i) * 128) = make_uint4(r[0], r[1], r[2], r[3]);
-      *reinterpret_cast<uint4*>(dst + (2 * i + 1) * 128) = make_uint4(r[4], r[5], r[6], r[7]);
-    }
-    {
-      const int c4 = min(2 * pq, 255), c5 = min(2 * pq - c4, 255), c6 = 2 * pq - c4 - c5;
-      uint4 key = make_uint4(0, 0, 0, 0);
-      if (q < p.nq) { key.x = 0x80808001u; key.y = (uint32_t)c4 | ((uint32_t)c5 << 8) | ((uint32_t)c6 << 16); }
-      *reinterpret_cast<uint4*>(dst + 16 * 128) = key;
-      *reinterpret_cast<uint4*>(dst + 17 * 128) = make_uint4(0, 0, 0, 0);
+        for (int b = 0; b < 8; b++) r[b] = ((w[i] >> b) & 0x01010101u) * 2u;
+        *reinterpret_cast<uint4*>(dst + (2 * i) * 128) = make_uint4(r[0], r[1], r[2], r[3]);
+        *reinterpret_cast<uint4*>(dst + (2 * i + 1) * 128) = make_uint4(r[4], r[5], r[6], r[7]);
+      }
+      {
+        const int c4 = min(2 * pq, 255), c5 = min(2 * pq - c4, 255), c6 = 2 * pq - c4 - c5;
+        uint4 key = make_uint4(0, 0, 0, 0);
+        if (q < p.nq) { key.x = 0x80808001u; key.y = (uint32_t)c4 | ((uint32_t)c5 << 8) | ((uint32_t)c6 << 16); }
+        *reinterpret_cast<uint4*>(dst + 16 * 128) = key;
+        *reinterpret_cast<uint4*>(dst + 17 * 128) = make_uint4(0, 0, 0, 0);
+      }
     }
     fence_proxy_async();
   }
@@ -708,13 +738,13 @@ __global__ void __launch_bounds__(XTHREADS, 1) tc_xt_kernel(const TcParams p) {
 #pragma unroll
         for (int g = 0; g < NGRP; g++) {
           if (!S.active(g)) continue;
-          const int s = n % XSTAGES;
-          if (n >= XSTAGES) cvb_mbar_wait(&empty[s], ((n / XSTAGES) - 1) & 1);
-          cvb_mbar_expect_tx(&full[s], TILE_BYTES);
-          const uint8_t* src = p.xt + (size_t)(S.tile0[g] + S.t[g]) * TILE_BYTES;
-          uint8_t* dst = sB + (size_t)s * TILE_BYTES;
+          const int s = n % STAGES_X;
+          if (n >= STAGES_X) cvb_mbar_wait(&empty[s], ((n / STAGES_X) - 1) & 1);
+          cvb_mbar_expect_tx(&full[s], X::TILE_BYTES);
+          const uint8_t* src = p.xt + (size_t)(S.tile0[g] + S.t[g]) * X::TILE_BYTES;
+          uint8_t* dst = sB + (size_t)s * STRIDE;
 #pragma unroll
-          for (int c = 0; c < 4; c++) cvb_bulk_g2s(dst + c * (TILE_BYTES / 4), src + c * (TILE_BYTES / 4), TILE_BYTES / 4, &full[s]);
+          for (int c = 0; c < 4; c++) cvb_bulk_g2s(dst + c * (X::TILE_BYTES / 4), src + c * (X::TILE_BYTES / 4), X::TILE_BYTES / 4, &full[s]);
           S.advance(g);
           n++;
         }
@@ -735,11 +765,18 @@ __global__ void __launch_bounds__(XTHREADS, 1) tc_xt_kernel(const TcParams p) {
       float fd[K];
 #pragma unroll
       for (int c = 0; c < K; c++) { wk[c] = INT_MAX; wi[c] = -1; fd[c] = (float)INT_MAX; }
-      write_list<K, false>(p, seg, qb * TM + row0 + (quad == 1 ? 8 : 0), quad < 2, wk, wi, fd, lane);
+      write_list<K, X::kIsL2>(p, seg, qb * TM + row0 + (quad == 1 ? 8 : 0), quad < 2, wk, wi, fd, lane);
     }
     Streams S;
     S.init(seg0, seg1, p.seg_tile);
-    int wk0[K], wk1[K];   // (distance << kIdxBits) + row within the keyframe, ascending — rows row0 and row0 + 8
+    // Hamming: wk = (distance << kIdxBits) + row within the keyframe, ascending.  L2: wk = the sqrtf key, wi = row within the
+    // keyframe, wd = raw-distance bound of the worst entry (it skips the sqrt for rows that cannot enter).  Rows row0 and row0 + 8.
+    int wk0[K], wk1[K], wi0[K], wi1[K], wd0[K], wd1[K];
+    int qn0 = 0, qn1 = 0;
+    if constexpr (X::kIsL2) {
+      qn0 = reinterpret_cast<const int*>(sA + TM * KX)[row0];
+      qn1 = reinterpret_cast<const int*>(sA + TM * KX)[row0 + 8];
+    }
     int n = 0;
     while (S.any()) {
 #pragma unroll
@@ -749,55 +786,105 @@ __global__ void __launch_bounds__(XTHREADS, 1) tc_xt_kernel(const TcParams p) {
           const int t = S.t[g2];
           if (t == 0) {
 #pragma unroll
-            for (int c = 0; c < K; c++) wk0[c] = wk1[c] = INT_MAX;
-          }
-          const int s = n % XSTAGES;
-          cvb_mbar_wait(&full[s], (n / XSTAGES) & 1);
-          uint32_t acc[64];
-          wg_gemm<true, NSLICE>(acc, a_desc, make_desc(b_addr0 + (uint32_t)s * TILE_BYTES, 128, KX * 8));
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&empty[s]);   // operands consumed: the producer may refill this stage
-          unsigned pk0[K], pk1[K];
-#pragma unroll
-          for (int c = 0; c < K; c++) pk0[c] = pk1[c] = 0xFFFFFFFFu;
-#pragma unroll
-          for (int i = 0; i < 16; i++) {   // columns 8 i + 2 quad (low half) and + 1 (high half)
-            insert_packed16<K>(pk0, __byte_perm(acc[4 * i], acc[4 * i + 1], 0x5410));
-            insert_packed16<K>(pk1, __byte_perm(acc[4 * i + 2], acc[4 * i + 3], 0x5410));
-          }
-          // later tiles hold larger row indices: a candidate enters only with a strictly smaller distance than the k-th entry
-#pragma unroll
-          for (int rr = 0; rr < 2; rr++) {
-            unsigned (&pk)[K] = rr ? pk1 : pk0;
-            int (&wk)[K] = rr ? wk1 : wk0;
-            const unsigned best16 = min(pk[0] & 0xFFFFu, pk[0] >> 16);
-            const int worst_d = wk[K - 1] == INT_MAX ? 1024 : (wk[K - 1] >> kIdxBits);
-            if ((int)(best16 >> 7) < worst_d) {
-#pragma unroll
-              for (int c = 0; c < K; c++)
-#pragma unroll
-                for (int hh = 0; hh < 2; hh++) {
-                  const unsigned k16 = hh ? (pk[c] >> 16) : (pk[c] & 0xFFFFu);
-                  insert_packed<K>(wk, k16 >= (unsigned)kKeyInvalid ? INT_MAX
-                                                                   : (int)(((k16 >> 7) << kIdxBits) + (unsigned)(t * TN) + (k16 & 127u)));
-                }
+            for (int c = 0; c < K; c++) {
+              wk0[c] = wk1[c] = X::kIsL2 ? kInfKey : INT_MAX;
+              wi0[c] = wi1[c] = -1;
+              wd0[c] = wd1[c] = kInf;
             }
+          }
+          const int s = n % STAGES_X;
+          cvb_mbar_wait(&full[s], (n / STAGES_X) & 1);
+          if constexpr (!X::kIsL2) {
+            uint32_t acc[64];
+            wg_gemm<true, X::NSLICE>(acc, a_desc, make_desc(b_addr0 + (uint32_t)s * STRIDE, 128, KX * 8));
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&empty[s]);   // operands consumed: the producer may refill this stage
+            unsigned pk0[K], pk1[K];
+#pragma unroll
+            for (int c = 0; c < K; c++) pk0[c] = pk1[c] = 0xFFFFFFFFu;
+#pragma unroll
+            for (int i = 0; i < 16; i++) {   // columns 8 i + 2 quad (low half) and + 1 (high half)
+              insert_packed16<K>(pk0, __byte_perm(acc[4 * i], acc[4 * i + 1], 0x5410));
+              insert_packed16<K>(pk1, __byte_perm(acc[4 * i + 2], acc[4 * i + 3], 0x5410));
+            }
+            // later tiles hold larger row indices: a candidate enters only with a strictly smaller distance than the k-th entry
+#pragma unroll
+            for (int rr = 0; rr < 2; rr++) {
+              unsigned (&pk)[K] = rr ? pk1 : pk0;
+              int (&wk)[K] = rr ? wk1 : wk0;
+              const unsigned best16 = min(pk[0] & 0xFFFFu, pk[0] >> 16);
+              const int worst_d = wk[K - 1] == INT_MAX ? 1024 : (wk[K - 1] >> kIdxBits);
+              if ((int)(best16 >> 7) < worst_d) {
+#pragma unroll
+                for (int c = 0; c < K; c++)
+#pragma unroll
+                  for (int hh = 0; hh < 2; hh++) {
+                    const unsigned k16 = hh ? (pk[c] >> 16) : (pk[c] & 0xFFFFu);
+                    insert_packed<K>(wk, k16 >= (unsigned)kKeyInvalid ? INT_MAX
+                                                                     : (int)(((k16 >> 7) << kIdxBits) + (unsigned)(t * TN) + (k16 & 127u)));
+                  }
+              }
+            }
+          } else {
+            // d = |q|^2 + |t|^2 - 2 <q, t> (exact in s32); a row enters with OpenCV's rule on sqrtf(d).
+            // Two m64n64 GEMMs per tile, columns [0, 64) then [64, 128): 32 accumulator registers instead of 64 leave room for
+            // the (key, index, bound) lists within the 96 registers a thread of this 17-warp CTA gets.
+            const int* nrm = reinterpret_cast<const int*>(sB + (size_t)s * STRIDE + TN * KX);
+#pragma unroll 1
+            for (int hh = 0; hh < 2; hh++) {
+            uint32_t acc[32];
+            wg_gemm_u8_n64<X::NSLICE>(acc, a_desc, make_desc(b_addr0 + (uint32_t)s * STRIDE + (uint32_t)(hh * 64 * KX), 128, KX * 8));
+#pragma unroll
+            for (int i = 0; i < 8; i++) {
+              const int2 nn = *reinterpret_cast<const int2*>(nrm + 64 * hh + 8 * i + 2 * quad);
+#pragma unroll
+              for (int e = 0; e < 4; e++) {
+                const int j = 64 * hh + 8 * i + 2 * quad + (e & 1);
+                const int tn = (e & 1) ? nn.y : nn.x;
+                int (&wk)[K] = e < 2 ? wk0 : wk1;
+                int (&wi)[K] = e < 2 ? wi0 : wi1;
+                int (&wd)[K] = e < 2 ? wd0 : wd1;
+                const int d = (e < 2 ? qn0 : qn1) + tn - 2 * (int)acc[4 * i + e];
+                if (d < wd[K - 1]) {
+                  const int key = __float_as_int(__fsqrt_rn((float)d));
+                  if (key < wk[K - 1]) {
+                    insert_key<K>(wk, wi, key, t * TN + j);
+                    const float f = __int_as_float(wk[K - 1]);   // raw-distance bound of the worst entry (pre-test)
+                    wd[K - 1] = wk[K - 1] == kInfKey ? kInf : (int)ceilf(f * f * 1.000001f) + 1;
+                  }
+                }
+              }
+            }
+            }
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&empty[s]);   // operands and row norms consumed: the producer may refill this stage
           }
           if (t == S.nt[g2] - 1) {
             // ---- keyframe finished: merge the quad's lists; lane quad 0 writes row0, quad 1 writes row0 + 8 ----
-            quad_merge_packed<K>(wk0);
-            quad_merge_packed<K>(wk1);
             const bool second = quad == 1;
             int wk[K], wi[K];
             float fd[K];
+            if constexpr (X::kIsL2) {
+              quad_merge_lex<K>(wk0, wi0);
+              quad_merge_lex<K>(wk1, wi1);
 #pragma unroll
-            for (int c = 0; c < K; c++) {
-              const int x = second ? wk1[c] : wk0[c];
-              wi[c] = x == INT_MAX ? -1 : (x & ((1 << kIdxBits) - 1));
-              wk[c] = x == INT_MAX ? INT_MAX : (x >> kIdxBits);
-              fd[c] = (float)wk[c];
+              for (int c = 0; c < K; c++) {
+                wk[c] = second ? wk1[c] : wk0[c];
+                wi[c] = second ? wi1[c] : wi0[c];
+                fd[c] = __int_as_float(wk[c]);
+              }
+            } else {
+              quad_merge_packed<K>(wk0);
+              quad_merge_packed<K>(wk1);
+#pragma unroll
+              for (int c = 0; c < K; c++) {
+                const int x = second ? wk1[c] : wk0[c];
+                wi[c] = x == INT_MAX ? -1 : (x & ((1 << kIdxBits) - 1));
+                wk[c] = x == INT_MAX ? INT_MAX : (x >> kIdxBits);
+                fd[c] = (float)wk[c];
+              }
             }
-            write_list<K, false>(p, S.seg[g2], qb * TM + row0 + (second ? 8 : 0), quad < 2, wk, wi, fd, lane);
+            write_list<K, X::kIsL2>(p, S.seg[g2], qb * TM + row0 + (second ? 8 : 0), quad < 2, wk, wi, fd, lane);
           }
         }
         S.advance(g2);
@@ -807,16 +894,17 @@ __global__ void __launch_bounds__(XTHREADS, 1) tc_xt_kernel(const TcParams p) {
   }
 }
 
-template <int K>
+template <class X, int K>
 int launch_xt(cvb_ctx* ctx, const TcParams& p, cudaStream_t st) {
   static cvb_once_per_device once;
+  constexpr size_t smem = smem_bytes_xt<X>();
   {
     std::lock_guard<std::mutex> once_lk(once.mtx);
     if (once.first(ctx->device)) {
-      CVB_CUDA(ctx, cudaFuncSetAttribute(tc_xt_kernel<K>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes));
+      CVB_CUDA(ctx, cudaFuncSetAttribute(tc_xt_kernel<X, K>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     }
   }
-  tc_xt_kernel<K><<<p.nqb * p.parts, XTHREADS, kSmemBytes, st>>>(p);
+  tc_xt_kernel<X, K><<<p.nqb * p.parts, XTHREADS, smem, st>>>(p);
   CVB_CHECK_LAUNCH(ctx);
   return CVB_OK;
 }
@@ -831,12 +919,13 @@ int64_t tiles_of(const int32_t* h_seg, int n_seg, std::vector<int32_t>* seg_tile
   }
   return total;
 }
-size_t tile_bytes() { return xt::TILE_BYTES; }
+size_t tile_bytes(int metric) { return metric == 0 ? xt::XtHamming::TILE_BYTES : xt::XtL2::TILE_BYTES; }
 
-int expand_tiles(cvb_ctx* ctx, const uint8_t* d_rows, const int32_t* d_seg_ptr, const int32_t* d_seg_tile, int seg_lo, int seg_hi,
-                 int tile_lo, int n_tiles, uint8_t* d_xt, cudaStream_t st) {
+int expand_tiles(cvb_ctx* ctx, int metric, const uint8_t* d_rows, const int32_t* d_seg_ptr, const int32_t* d_seg_tile, int seg_lo,
+                 int seg_hi, int tile_lo, int n_tiles, uint8_t* d_xt, cudaStream_t st) {
   if (n_tiles <= 0) return CVB_OK;
-  xt::expand_tiles_kernel<<<n_tiles, 256, 0, st>>>(d_rows, d_seg_ptr, d_seg_tile, seg_lo, seg_hi, tile_lo, d_xt);
+  if (metric == 0) xt::expand_tiles_kernel<xt::XtHamming><<<n_tiles, 256, 0, st>>>(d_rows, d_seg_ptr, d_seg_tile, seg_lo, seg_hi, tile_lo, d_xt);
+  else xt::expand_tiles_kernel<xt::XtL2><<<n_tiles, 256, 0, st>>>(d_rows, d_seg_ptr, d_seg_tile, seg_lo, seg_hi, tile_lo, d_xt);
   CVB_CHECK_LAUNCH(ctx);
   return CVB_OK;
 }
@@ -872,36 +961,33 @@ int launch(cvb_ctx* ctx, TcParams p, int metric, int k, cudaStream_t st) {
   if (parts < 1) parts = 1;
   if (parts > p.n_seg) parts = p.n_seg;
   p.parts = parts;
-  if (metric == 0 && !(getenv("COVINS_B200_TC_XT") && !strcmp(getenv("COVINS_B200_TC_XT"), "0"))) {
+  if (metric == 1 || !(getenv("COVINS_B200_TC_XT") && !strcmp(getenv("COVINS_B200_TC_XT"), "0"))) {
     cvb_block B(ctx, st);
     if (!p.xt) {
       // no resident tile store for this train set (raw-pointer API): expand it into the call's block first (HBM-bound pre-pass)
-      CVB_REQUIRE(ctx, p.h_seg != nullptr, "tensor-core Hamming path needs the host copy of the segment table");
+      CVB_REQUIRE(ctx, p.h_seg != nullptr, "tensor-core path needs the host copy of the segment table");
       std::vector<int32_t> h_tile;
       const int64_t n_tiles = tiles_of(p.h_seg, p.n_seg, &h_tile);
       int32_t* d_tile;
       uint8_t* d_xt;
-      B.tmp(d_tile, (size_t)p.n_seg + 1); B.tmp(d_xt, (size_t)n_tiles * xt::TILE_BYTES);
+      B.tmp(d_tile, (size_t)p.n_seg + 1); B.tmp(d_xt, (size_t)n_tiles * tile_bytes(metric));
       if (const int rc = B.place()) return rc;
       CVB_CUDA(ctx, cudaMemcpyAsync(d_tile, h_tile.data(), sizeof(int32_t) * ((size_t)p.n_seg + 1), cudaMemcpyHostToDevice, st));
       CVB_CUDA(ctx, cudaStreamSynchronize(st));   // h_tile goes out of scope
-      const int rc = expand_tiles(ctx, p.t, p.seg_ptr, d_tile, 0, p.n_seg, 0, (int)n_tiles, d_xt, st);
+      const int rc = expand_tiles(ctx, metric, p.t, p.seg_ptr, d_tile, 0, p.n_seg, 0, (int)n_tiles, d_xt, st);
       if (rc) return rc;
       p.xt = d_xt;
       p.seg_tile = d_tile;
     }
-    switch (k) {
-      case 1: return xt::launch_xt<1>(ctx, p, st);
-      case 2: return xt::launch_xt<2>(ctx, p, st);
-      case 3: return xt::launch_xt<3>(ctx, p, st);
-      default: return xt::launch_xt<4>(ctx, p, st);
-    }
+#define XT_CASE(XX) \
+    switch (k) { case 1: return xt::launch_xt<XX, 1>(ctx, p, st); case 2: return xt::launch_xt<XX, 2>(ctx, p, st); \
+                 case 3: return xt::launch_xt<XX, 3>(ctx, p, st); default: return xt::launch_xt<XX, 4>(ctx, p, st); }
+    if (metric == 0) XT_CASE(xt::XtHamming)
+    XT_CASE(xt::XtL2)
+#undef XT_CASE
   }
 #define TC_CASE(MM, KK) return launch_tc<MM, KK>(ctx, p, st)
-  if (metric == 0) {
-    switch (k) { case 1: TC_CASE(TcHamming, 1); case 2: TC_CASE(TcHamming, 2); case 3: TC_CASE(TcHamming, 3); default: TC_CASE(TcHamming, 4); }
-  }
-  switch (k) { case 1: TC_CASE(TcL2, 1); case 2: TC_CASE(TcL2, 2); case 3: TC_CASE(TcL2, 3); default: TC_CASE(TcL2, 4); }
+  switch (k) { case 1: TC_CASE(TcHamming, 1); case 2: TC_CASE(TcHamming, 2); case 3: TC_CASE(TcHamming, 3); default: TC_CASE(TcHamming, 4); }
 #undef TC_CASE
 }
 

@@ -22,7 +22,7 @@ struct TcParams {
   int32_t* match_train;
   float* match_dist;
   int32_t* n_matches;
-  // Hamming only: the pre-expanded operand tiles of the train set (expand_tiles) and the first tile of every segment
+  // the operand tiles of the train set (expand_tiles, the metric's tile image) and the first tile of every segment
   // [n_seg + 1]; xt == nullptr → launch() expands into the call's device block (needs h_seg, the host copy of seg_ptr)
   const uint8_t* xt;
   const int32_t* seg_tile;
@@ -33,11 +33,12 @@ struct TcParams {
 // order dependent and stays on the scalar kernel)
 int launch(cvb_ctx* ctx, TcParams p, int metric, int k, cudaStream_t st);
 
-// pre-expanded operand store of the Hamming path: 128-row tiles per segment, tile_bytes() each
+// operand tile store of the tensor-core path: 128-row tiles per segment, tile_bytes(metric) each, in the shared-memory image the
+// metric's wgmma reads (Hamming: expanded bits + key slice; L2: u8 rows + |t|^2 per row)
 int64_t tiles_of(const int32_t* h_seg, int n_seg, std::vector<int32_t>* seg_tile);   // total tiles; optional prefix [n_seg + 1]
-size_t tile_bytes();
-int expand_tiles(cvb_ctx* ctx, const uint8_t* d_rows, const int32_t* d_seg_ptr, const int32_t* d_seg_tile, int seg_lo, int seg_hi,
-                 int tile_lo, int n_tiles, uint8_t* d_xt, cudaStream_t st);
+size_t tile_bytes(int metric);
+int expand_tiles(cvb_ctx* ctx, int metric, const uint8_t* d_rows, const int32_t* d_seg_ptr, const int32_t* d_seg_tile, int seg_lo,
+                 int seg_hi, int tile_lo, int n_tiles, uint8_t* d_xt, cudaStream_t st);
 
 // true when the tensor-core kernel fills the GPU for this shape (enough candidate segments per query block)
 bool profitable(const cvb_ctx* ctx, int nq, int n_seg, long total_rows, int max_seg_len);

@@ -95,25 +95,35 @@ def match_candidates_hamming(ctx: Context, q, t, seg_ptr=None, thr: float = 40.0
 
 
 class DescriptorDatabase:
-    """The merged map's ORB descriptors resident in HBM (cvb_db_*): keyframes are appended once, a place-recognition
-    request (placerec_gen_be.cpp:60-135) uploads only the query keyframe and downloads only the accepted matches."""
+    """The merged map's descriptors resident in HBM (cvb_db_*): keyframes are appended once, a place-recognition
+    request (placerec_gen_be.cpp:60-135) uploads only the query keyframe and downloads only the accepted matches.
+    kind="orb": 32-byte rows, match_hamming[_dev]; kind="sift": CV_32F rows x 128 kept as exact u8, match_l2[_dev]."""
 
-    def __init__(self, ctx: Context, reserve_rows: int = 0):
+    def __init__(self, ctx: Context, reserve_rows: int = 0, kind: str = "orb"):
         import ctypes as C
+        assert kind in ("orb", "sift"), kind
         self.ctx = ctx
+        self.kind = kind
+        self._dim = 32 if kind == "orb" else 128
         h = C.c_void_p()
-        ctx.check(lib().cvb_db_create(ctx.handle, 32, C.byref(h)))
+        ctx.check(lib().cvb_db_create(ctx.handle, self._dim, C.byref(h)))
         self.handle = h
         self._cap = 1 << 16
         if reserve_rows:
             ctx.check(lib().cvb_db_reserve(ctx.handle, self.handle, int(reserve_rows)))
 
     def append(self, rows, rows_per_kf):
-        """rows u8 [sum(rows_per_kf), 32] = the descriptor matrices of the new keyframes, concatenated."""
-        rows = _np(rows, np.uint8).reshape(-1, 32)
+        """rows = the descriptor matrices of the new keyframes, concatenated: u8 [sum(rows_per_kf), 32] (ORB) or float32
+        [sum(rows_per_kf), 128] (SIFT, integer-valued in [0,255])."""
         rpk = np.ascontiguousarray(np.asarray(rows_per_kf, np.int32).reshape(-1))
+        if self.kind == "orb":
+            rows = _np(rows, np.uint8).reshape(-1, 32)
+            fn = lib().cvb_db_append
+        else:
+            rows = _np(rows, np.float32).reshape(-1, 128)
+            fn = lib().cvb_db_append_sift
         assert int(rpk.sum()) == len(rows), "rows_per_kf does not add up to the number of rows"
-        self.ctx.check(lib().cvb_db_append(self.ctx.handle, self.handle, _ptr(rows), _ptr(rpk), len(rpk)))
+        self.ctx.check(fn(self.ctx.handle, self.handle, _ptr(rows), _ptr(rpk), len(rpk)))
 
     def remove(self, kf_index: int):
         """a keyframe leaves the map (culling / erase): later keyframes move down by one index"""
@@ -125,36 +135,49 @@ class DescriptorDatabase:
         self.ctx.check(lib().cvb_db_size(self.handle, C.byref(n_kf), C.byref(n_rows)))
         return n_kf.value, n_rows.value
 
-    def match_hamming(self, q, thr: float = 40.0, ratio: float = 0.8):
-        """→ (n_matches [n_kf] i32, m_kf, m_query, m_train (keyframe-local), m_dist): the accepted matches ordered by
-        (keyframe, queryIdx) — per keyframe the reference's img_matches vector."""
+    def _match(self, fn, q, thr, ratio):
         import ctypes as C
-        q = _np(q, np.uint8).reshape(-1, 32)
         n_kf, _ = self.size()
         nm = np.zeros(n_kf, np.int32)
         while True:
             cap = self._cap
             out = [np.empty(cap, np.int32), np.empty(cap, np.int32), np.empty(cap, np.int32), np.empty(cap, np.float32)]
             tot = C.c_int32()
-            self.ctx.check(lib().cvb_db_match_hamming(self.ctx.handle, self.handle, _ptr(q), len(q), thr, ratio,
-                                                      _ptr(nm), _ptr(out[0]), _ptr(out[1]), _ptr(out[2]), _ptr(out[3]),
-                                                      cap, C.byref(tot)))
+            self.ctx.check(fn(self.ctx.handle, self.handle, _ptr(q), len(q), thr, ratio, _ptr(nm), _ptr(out[0]), _ptr(out[1]),
+                              _ptr(out[2]), _ptr(out[3]), cap, C.byref(tot)))
             if tot.value <= cap:
                 return (nm,) + tuple(o[:tot.value] for o in out)
             self._cap = int(tot.value * 1.25) + 16
 
-    def match_hamming_dev(self, q, thr: float = 40.0, ratio: float = 0.8):
-        """device request: q = CUDA torch tensor u8 [nq, 32] → (match_train [n_kf, nq] i32, match_dist [n_kf, nq] f32,
-        n_matches [n_kf] i32) as CUDA tensors; no copies (cvb_db_match_hamming_dev)."""
+    def _match_dev(self, fn, q, thr, ratio):
         import torch
         n_kf, _ = self.size()
         nq = q.shape[0]
         mt = torch.empty((n_kf, nq), dtype=torch.int32, device=q.device)
         md = torch.empty((n_kf, nq), dtype=torch.float32, device=q.device)
         nm = torch.empty((n_kf,), dtype=torch.int32, device=q.device)
-        self.ctx.check(lib().cvb_db_match_hamming_dev(self.ctx.handle, self.handle, _ptr(q), nq, thr, ratio, _ptr(mt), _ptr(md), _ptr(nm),
-                                                      _torch_stream()))
+        self.ctx.check(fn(self.ctx.handle, self.handle, _ptr(q), nq, thr, ratio, _ptr(mt), _ptr(md), _ptr(nm), _torch_stream()))
         return mt, md, nm
+
+    def match_hamming(self, q, thr: float = 40.0, ratio: float = 0.8):
+        """→ (n_matches [n_kf] i32, m_kf, m_query, m_train (keyframe-local), m_dist): the accepted matches ordered by
+        (keyframe, queryIdx) — per keyframe the reference's img_matches vector."""
+        return self._match(lib().cvb_db_match_hamming, _np(q, np.uint8).reshape(-1, 32), thr, ratio)
+
+    def match_hamming_dev(self, q, thr: float = 40.0, ratio: float = 0.8):
+        """device request: q = CUDA torch tensor u8 [nq, 32] → (match_train [n_kf, nq] i32, match_dist [n_kf, nq] f32,
+        n_matches [n_kf] i32) as CUDA tensors; no copies (cvb_db_match_hamming_dev)."""
+        return self._match_dev(lib().cvb_db_match_hamming_dev, q, thr, ratio)
+
+    def match_l2(self, q, thr: float = 500.0, ratio: float = 0.8):
+        """SIFT database: q = float32 [nq, 128] (integer-valued in [0,255]) → the outputs of match_hamming, with the
+        semantics of match_candidates_l2 per keyframe (img_match_thres 500 for SIFT, config_backend.yaml:38)."""
+        return self._match(lib().cvb_db_match_l2, _np(q, np.float32).reshape(-1, 128), thr, ratio)
+
+    def match_l2_dev(self, q, thr: float = 500.0, ratio: float = 0.8):
+        """SIFT database, device request: q = CUDA torch tensor u8 [nq, 128] (see quantize_u8) → the outputs of
+        match_hamming_dev (cvb_db_match_l2_dev)."""
+        return self._match_dev(lib().cvb_db_match_l2_dev, q, thr, ratio)
 
     def close(self):
         if self.handle:

@@ -91,7 +91,7 @@ CVB_API int cvb_match_hamming_batch_dev(cvb_ctx* ctx, const uint8_t* d_q, int nq
                                         int32_t* d_n_matches, void* stream);
 
 /*
- * Resident descriptor database: the ORB descriptors of the merged map's keyframes stay in HBM.
+ * Resident descriptor database: the ORB or SIFT descriptors of the merged map's keyframes stay in HBM.
  * Replaces, for the place-recognition loop of placerec_gen_be.cpp:60-135 (one knnMatch + filter per
  * candidate keyframe, :82-114), the per-call upload of the train descriptors: a keyframe's descriptor
  * matrix is immutable once the keyframe exists (keyframe_be.cpp:106-137), so it is appended once
@@ -104,6 +104,10 @@ CVB_API int cvb_match_hamming_batch_dev(cvb_ctx* ctx, const uint8_t* d_q, int nq
  * reference's img_matches vector: m_kf / m_query / m_train (keyframe-local trainIdx) / m_dist.
  * *n_total = number of accepted matches over all keyframes; at most `cap` are written (call again with
  * a larger cap if *n_total > cap).
+ *
+ * cvb_db_create: desc_bytes 32 = ORB rows (cvb_db_append, cvb_db_match_hamming[_dev]); 128 = SIFT rows (cvb_db_append_sift,
+ * cvb_db_match_l2[_dev]); any other value → CVB_ERR_UNSUPPORTED.  A call of the other row kind → CVB_ERR_INVALID with a
+ * message.  cvb_db_reserve, cvb_db_remove and cvb_db_size serve both kinds.
  */
 typedef struct cvb_db cvb_db;
 CVB_API int cvb_db_create(cvb_ctx* ctx, int desc_bytes, cvb_db** out);
@@ -123,6 +127,27 @@ CVB_API int cvb_db_match_hamming(cvb_ctx* ctx, cvb_db* db, const uint8_t* q, int
  * keyframes are matched from their resident tensor-core operand tiles (written once by cvb_db_append). */
 CVB_API int cvb_db_match_hamming_dev(cvb_ctx* ctx, cvb_db* db, const uint8_t* d_q, int nq, float thr, float ratio,
                                      int32_t* d_match_train, float* d_match_dist, int32_t* d_n_matches, void* stream);
+/*
+ * The SIFT form of the database (desc_bytes == 128), for the SIFT branch of the same loop (placerec_gen_be.cpp:86-87,99-114).
+ * cvb_db_append_sift: rows = the new keyframes' descriptors_add_ (CV_32F, rows x 128 each, concatenated).  The values are
+ * checked and quantised to u8 on the host while staged, the rule of cvb_verify_noncentral_relative_pose_sift_seeded_batch: a
+ * value that is not an integer in [0,255] (NaN and +-inf included) → CVB_ERR_UNSUPPORTED before any device work, the database
+ * unchanged.  The rows are kept as exact u8 (as cvb_knn_l2_u8_batch_dev takes them) next to their tensor-core operand tiles
+ * (128-row tiles of the u8 rows and their |t|^2, written once here).
+ * cvb_db_match_l2: per keyframe the semantics of cvb_match_l2_batch with the caller's thresholds (SIFT config:
+ * img_match_thres about 500, ratio 0.8): exact brute-force 2-NN, dist = sqrtf(d2) in fp32, OpenCV's tie rule on the float
+ * distance (L2Metric::less: the lower trainIdx wins among equal floats), accepted iff d0 <= thr && d0 < ratio*d1.  q = the
+ * query keyframe's CV_32F rows [nq][128], checked like the appended rows (before any device work).  The outputs are exactly
+ * those of cvb_db_match_hamming: n_matches per keyframe, matches compacted by (keyframe, queryIdx), at most `cap`, *n_total.
+ * cvb_db_match_l2_dev: the device request, d_q = u8 [nq][128] in HBM (16-byte aligned), dense device outputs as
+ * cvb_db_match_hamming_dev.
+ */
+CVB_API int cvb_db_append_sift(cvb_ctx* ctx, cvb_db* db, const float* rows, const int32_t* rows_per_kf, int n_kf);
+CVB_API int cvb_db_match_l2(cvb_ctx* ctx, cvb_db* db, const float* q, int nq, float thr, float ratio,
+                            int32_t* n_matches, int32_t* m_kf, int32_t* m_query, int32_t* m_train,
+                            float* m_dist, int cap, int32_t* n_total);
+CVB_API int cvb_db_match_l2_dev(cvb_ctx* ctx, cvb_db* db, const uint8_t* d_q, int nq, float thr, float ratio,
+                                int32_t* d_match_train, float* d_match_dist, int32_t* d_n_matches, void* stream);
 
 /*
  * Replaces the SIFT branch, cv::FlannBasedMatcher()::knnMatch(query, train, out, 2)
