@@ -1,7 +1,7 @@
 // geom_common.cuh — helpers shared by the geometric-verification translation units (geom_kernels.cu, ransac_abs.cu,
 // ransac_rel.cu): the device arithmetic, including the cross product, the largest-cross-product
 // null vector of a rank-2 3x3 (P3P's eigenvectors, the 5-point solver's roots and baseline), the per-correspondence
-// absolute-pose score (score_abs_kernel, ransac_abs_kernel), the relative-pose score (score_rel_kernel, ransac_rel_kernel) and
+// absolute-pose score (score_abs_kernel, ransac_abs_kernel), SearchByProjection's camera projection, the relative-pose score (score_rel_kernel, ransac_rel_kernel) and
 // the 3x3 inverse of the RANSAC solvers.  Every device operation is an explicit round-to-nearest non-fused intrinsic, so
 // results are reproducible bit for bit against a plain IEEE evaluation compiled with -ffp-contract=off.  The RANSAC around the
 // solvers is in ransac_common.cuh.
@@ -118,6 +118,44 @@ __device__ __forceinline__ double rel_score(const double* __restrict__ M, const 
     e2 = r == 0 ? mul(d2, d2) : add(e2, mul(d2, d2));
   }
   return add(__ddiv_rn(mul(e1, 0.5), s1[i]), __ddiv_rn(mul(e2, 0.5), s2[i]));
+}
+
+// camera_->project3 of a camera-frame point pc: pixel (u, v) under intrinsics [fu, fv, cu, cv], the pinhole (0) or unified (1,
+// parameter xi) projection and the radtan (0), equidistant (1) or FOV (2) distortion; false = not projectable.  Every operation in
+// the oracle's order (geom_oracle.c project3).  The equidistant and FOV models call CUDA's atan / tan, which are not correctly
+// rounded: only those two models can differ from a host libm in the last bits.
+__device__ __forceinline__ bool project3_rn(const double* intr, const double* dist, int cam_model, int dist_model, double xi, const double* pc,
+                                            double* u, double* v) {
+  double den = pc[2];
+  if (cam_model == 1) den = add(pc[2], mul(xi, __dsqrt_rn(add(add(mul(pc[0], pc[0]), mul(pc[1], pc[1])), mul(pc[2], pc[2])))));
+  if (!(den > 1e-10)) return false;
+  const double x = __ddiv_rn(pc[0], den), y = __ddiv_rn(pc[1], den), r2 = add(mul(x, x), mul(y, y));
+  double xd, yd;
+  if (dist_model == 0) {
+    const double rad = add(add(1.0, mul(dist[0], r2)), mul(mul(dist[1], r2), r2));
+    xd = add(add(mul(x, rad), mul(mul(mul(2.0, dist[2]), x), y)), mul(dist[3], add(r2, mul(mul(2.0, x), x))));
+    yd = add(add(mul(y, rad), mul(dist[2], add(r2, mul(mul(2.0, y), y)))), mul(mul(mul(2.0, dist[3]), x), y));
+  } else {
+    double s = 1.0;
+    if (dist_model == 1) {
+      const double r = __dsqrt_rn(r2);
+      if (r >= 1e-8) {
+        const double th = atan(r), t2 = mul(th, th);
+        const double poly = add(add(add(add(1.0, mul(dist[0], t2)), mul(mul(dist[1], t2), t2)), mul(mul(mul(dist[2], t2), t2), t2)),
+                                mul(mul(mul(mul(dist[3], t2), t2), t2), t2));
+        s = __ddiv_rn(mul(th, poly), r);
+      }
+    } else {
+      const double w = dist[0];
+      if (mul(w, w) >= 1e-5) {
+        const double c = mul(2.0, tan(mul(0.5, w)));
+        s = r2 < 1e-5 ? __ddiv_rn(c, w) : __ddiv_rn(atan(mul(c, __dsqrt_rn(r2))), mul(w, __dsqrt_rn(r2)));
+      }
+    }
+    xd = mul(s, x); yd = mul(s, y);
+  }
+  *u = add(mul(intr[0], xd), intr[2]); *v = add(mul(intr[1], yd), intr[3]);
+  return true;
 }
 
 // inverse of a 3x3 matrix (row-major) by its adjugate

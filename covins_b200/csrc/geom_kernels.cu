@@ -51,20 +51,21 @@ __device__ __forceinline__ int ham256(const uint8_t* __restrict__ a, const uint8
 }
 __device__ __forceinline__ bool in_image(const double* img, double x, double y) { return x >= img[0] && x < img[1] && y >= img[2] && y < img[3]; }
 
-// LandmarkBase::PredictScale: ceil(log(ratio) / log(scale_factor)) clamped to [0, num_octaves - 1] = the smallest n >= 0
-// with scale_factor^n >= ratio (n capped): evaluated with exact repeated multiplication instead of two libm calls
-__device__ __forceinline__ int predict_scale(double maxdist, double dist3d, double sf, int num_octaves) {
+// LandmarkBase::PredictScale: ceil(log(ratio) / log(scale_factor)) clamped to [0, num_octaves - 1], as libm evaluates it.  That
+// level is monotone in ratio, so it is n = #{k : ratio > steps[k]} for the num_octaves - 1 ratios where it steps up (scale_table,
+// on the host).  Repeated multiplication by scale_factor is not the same: at scale_factor 1.2, ratio = 1.2 * 1.2 rounded gives
+// level 3 by the logarithms and 2 by the products.
+__device__ __forceinline__ int predict_scale(double maxdist, double dist3d, const double* steps, int num_octaves) {
   const double ratio = __ddiv_rn(maxdist, (double)(float)dist3d);   // `const float& currentDist`
   int n = 0;
-  double p = 1.0;
-  while (p < ratio && n < num_octaves - 1) { p = mul(p, sf); n++; }
+  while (n < num_octaves - 1 && ratio > steps[n]) n++;
   return n;
 }
 
 // best keypoint of `dst` for landmark i of `src` (float_best: direction 1→2 keeps the best distance as float — the same
 // integers — and both directions take the FIRST strict minimum in the grid's candidate order)
 __device__ int search_one(const DevKf& src, int i, const double* Tcw_src, const double* Tab, const double* Kdst, const DevKf& dst,
-                          const double* img, double th, double sf, int num_octaves, int* best_dist) {
+                          const double* img, double th, const double* steps, int num_octaves, int* best_dist) {
   double pw[3] = {src.lm_pos[3 * (size_t)i], src.lm_pos[3 * (size_t)i + 1], src.lm_pos[3 * (size_t)i + 2]};
   double pc_src[3], pc[3];
   rt_apply(Tcw_src, pw, pc_src);
@@ -74,7 +75,7 @@ __device__ int search_one(const DevKf& src, int i, const double* Tcw_src, const 
   const double u = __ddiv_rn(p0, p2), v = __ddiv_rn(p1, p2);
   if (!in_image(img, u, v)) return -1;
   const double dist3d = __dsqrt_rn(add(add(mul(pc[0], pc[0]), mul(pc[1], pc[1])), mul(pc[2], pc[2])));
-  const int level = predict_scale(src.lm_maxdist[i], dist3d, sf, num_octaves);
+  const int level = predict_scale(src.lm_maxdist[i], dist3d, steps, num_octaves);
   const double radius = mul(th, scalbn(1.0, level));
   const float tx = (float)u, ty = (float)v;
   int min_cx = (int)floor(mul(sub((double)tx, radius), dst.grid_w_inv)); if (min_cx < 0) min_cx = 0;
@@ -105,7 +106,7 @@ __device__ int search_one(const DevKf& src, int i, const double* Tcw_src, const 
   return best;
 }
 
-__global__ void __launch_bounds__(256) search_se3_kernel(DevKf k1, const DevPair* __restrict__ pairs, double th, int th_low, double sf,
+__global__ void __launch_bounds__(256) search_se3_kernel(DevKf k1, const DevPair* __restrict__ pairs, double th, int th_low, const double* __restrict__ steps,
                                                          int num_octaves) {
   const DevPair& P = pairs[blockIdx.x];
   const DevKf& k2 = P.k2;
@@ -116,7 +117,7 @@ __global__ void __launch_bounds__(256) search_se3_kernel(DevKf k1, const DevPair
     int m = -1;
     if (k1.lm_valid[i] && !P.already1[i]) {
       int bd;
-      const int b = search_one(k1, i, k1.Tcw, P.T21, k2.K, k2, k2.img, th, sf, num_octaves, &bd);
+      const int b = search_one(k1, i, k1.Tcw, P.T21, k2.K, k2, k2.img, th, steps, num_octaves, &bd);
       if (b >= 0 && bd <= th_low) m = b;              // bestDist <= desc_matching_th_low_ (:403)
     }
     P.match1[i] = m;
@@ -125,7 +126,7 @@ __global__ void __launch_bounds__(256) search_se3_kernel(DevKf k1, const DevPair
     int m = -1;
     if (k2.lm_valid[i] && !P.already2[i]) {
       int bd;
-      const int b = search_one(k2, i, k2.Tcw, P.T12, k1.K, k1, k2.img, th, sf, num_octaves, &bd);
+      const int b = search_one(k2, i, k2.Tcw, P.T12, k1.K, k1, k2.img, th, steps, num_octaves, &bd);
       if (b >= 0 && bd < th_low) m = b;               // bestDist < desc_matching_th_low_ (:479)
     }
     P.match2[i] = m;
@@ -163,7 +164,7 @@ struct ProjDev {
   int* action; int* best_idx; int* n_matches; int* overflow;
 };
 
-__global__ void __launch_bounds__(256, 1) search_proj_kernel(DevKf kf, ProjDev P, double th, int th_low, double sf, int num_octaves) {
+__global__ void __launch_bounds__(256, 1) search_proj_kernel(DevKf kf, ProjDev P, double th, int th_low, const double* __restrict__ scale, int num_octaves) {
   double Ow[3];
 #pragma unroll
   for (int r = 0; r < 3; r++) Ow[r] = -add(add(mul(P.Tcw[r], P.Tcw[3]), mul(P.Tcw[4 + r], P.Tcw[7])), mul(P.Tcw[8 + r], P.Tcw[11]));
@@ -175,19 +176,15 @@ __global__ void __launch_bounds__(256, 1) search_proj_kernel(DevKf kf, ProjDev P
       double pc[3];
       rt_apply(P.Tcw, pw, pc);
       if (pc[2] < 0.0) break;
-      const bam::CamModel cm{P.cam, P.dm, P.xi};
-      double x, y, xd, yd;
-      if (!bam::cam_normalise(cm, bam::V3{pc[0], pc[1], pc[2]}, &x, &y, nullptr, false)) break;
-      bam::cam_distort(cm, P.dist, x, y, &xd, &yd, nullptr, false);
-      const double u = P.intr[0] * xd + P.intr[2], v = P.intr[1] * yd + P.intr[3];
+      double u, v;
+      if (!project3_rn(P.intr, P.dist, P.cam, P.dm, P.xi, pc, &u, &v)) break;
       if (!in_image(kf.img, u, v)) break;
       const double PO[3] = {sub(pw[0], Ow[0]), sub(pw[1], Ow[1]), sub(pw[2], Ow[2])};
       const double d3 = __dsqrt_rn(add(add(mul(PO[0], PO[0]), mul(PO[1], PO[1])), mul(PO[2], PO[2])));
       if (d3 < P.min_dist[i] || d3 > P.max_dist[i]) break;
       if (add(add(mul(PO[0], P.normal[3 * (size_t)i]), mul(PO[1], P.normal[3 * (size_t)i + 1])), mul(PO[2], P.normal[3 * (size_t)i + 2])) < mul(0.5, d3)) break;
-      const int level = predict_scale(P.max_distance[i], d3, sf, num_octaves);
-      double radius = th;
-      for (int l = 0; l < level; l++) radius = mul(radius, sf);   // th * pow(scale_factor, level) for integer level
+      const int level = predict_scale(P.max_distance[i], d3, scale, num_octaves);
+      const double radius = mul(th, scale[num_octaves - 1 + level]);   // th * pow(scale_factor, level)
       const float tx = (float)u, ty = (float)v;
       int min_cx = (int)floor(mul(sub((double)tx, radius), kf.grid_w_inv)); if (min_cx < 0) min_cx = 0;
       if (min_cx >= GRID_COLS) break;
@@ -313,6 +310,32 @@ bool kf_ok(const cvb_kf_view* v) {
   return true;
 }
 
+// the host half of predict_scale and of SearchByProjection's radius th * pow(scale_factor, level), both by host libm as
+// LandmarkBase::PredictScale and the search evaluate them: [0, num_octaves - 1) the largest ratio of each level k below the
+// last (ratio > steps[k] <=> level > k; +inf if no finite ratio reaches level k + 1), then pow(scale_factor, l) for
+// l = 0 .. num_octaves - 1.  Requires scale_factor > 1.
+std::vector<double> scale_table(double sf, int num_octaves) {
+  auto level = [&](double r) {
+    const int n = (int)ceil(log(r) / log(sf));
+    return n < 0 ? 0 : (n >= num_octaves ? num_octaves - 1 : n);
+  };
+  auto bits = [](double d) { uint64_t u; memcpy(&u, &d, 8); return u; };
+  std::vector<double> t(2 * (size_t)num_octaves - 1);
+  for (int k = 0; k + 1 < num_octaves; k++) {
+    if (level(DBL_MAX) <= k) { t[k] = INFINITY; continue; }
+    uint64_t lo = bits(1.0), hi = bits(DBL_MAX);   // level(lo) <= k < level(hi); positive doubles order like their bits
+    while (hi - lo > 1) {
+      const uint64_t mid = lo + (hi - lo) / 2;
+      double r;
+      memcpy(&r, &mid, 8);
+      (level(r) <= k ? lo : hi) = mid;
+    }
+    memcpy(&t[k], &lo, 8);
+  }
+  for (int l = 0; l < num_octaves; l++) t[num_octaves - 1 + l] = pow(sf, (double)l);
+  return t;
+}
+
 }  // namespace
 
 extern "C" {
@@ -341,7 +364,9 @@ int cvb_search_by_se3_batch(cvb_ctx* ctx, const cvb_kf_view* kf1, const cvb_kf_v
   const uint8_t *d_a1, *d_a2;
   DevPair* d_pairs;
   int *d_m1, *d_m2, *d_m12, *d_nf;
-  B.in(d_a1, already1, (size_t)n_pairs * n1); B.in(d_a2, already2, n2_total); B.in(d_pairs, nullptr, n_pairs);
+  const std::vector<double> scale = scale_table(prm->scale_factor, prm->num_octaves);
+  const double* d_scale;
+  B.in(d_a1, already1, (size_t)n_pairs * n1); B.in(d_a2, already2, n2_total); B.in(d_pairs, nullptr, n_pairs); B.in(d_scale, scale.data(), scale.size());
   B.out(d_m1, match1, (size_t)n_pairs * n1); B.out(d_m2, match2, n2_total); B.out(d_m12, match12, (size_t)n_pairs * n1); B.out(d_nf, n_found, n_pairs);
   if (const int rc = B.place()) return rc;
   size_t a2 = 0;
@@ -354,7 +379,7 @@ int cvb_search_by_se3_batch(cvb_ctx* ctx, const cvb_kf_view* kf1, const cvb_kf_v
   }
   memcpy(B.host(d_pairs), hp.data(), hp.size() * sizeof(DevPair));
   if (const int rc = B.upload()) return rc;
-  search_se3_kernel<<<n_pairs, 256, 0, ctx->stream>>>(d1, d_pairs, prm->th, prm->desc_th_low, prm->scale_factor, prm->num_octaves);
+  search_se3_kernel<<<n_pairs, 256, 0, ctx->stream>>>(d1, d_pairs, prm->th, prm->desc_th_low, d_scale, prm->num_octaves);
   CVB_CHECK_LAUNCH(ctx);
   return B.download();
 }
@@ -417,6 +442,7 @@ int cvb_search_by_projection(cvb_ctx* ctx, const cvb_kf_view* kf, const int32_t*
   CVB_REQUIRE(ctx, kf->n >= 0 && kf->grid_ptr && (kf->n == 0 || (kf->kp && kf->octave && kf->desc && kf->lm_valid && kf_lm_cand && matched)),
               "search_by_projection: malformed keyframe view");
   CVB_REQUIRE(ctx, kf->grid_ptr[0] == 0 && kf->grid_ptr[GRID_COLS * GRID_ROWS] <= kf->n, "search_by_projection: malformed grid");
+  CVB_REQUIRE(ctx, prm->num_octaves >= 1 && prm->scale_factor > 1.0 && prm->th > 0.0, "search_by_projection: bad parameters");
   if (cam_model < 0 || cam_model > 1) return cvb_fail(ctx, CVB_ERR_UNSUPPORTED, "Unknown projection type.");
   if (dist_model < 0 || dist_model > 2) return cvb_fail(ctx, CVB_ERR_UNSUPPORTED, "Unknown distortion type.");
   const int n = kf->n, m = lms->m;
@@ -435,6 +461,9 @@ int cvb_search_by_projection(cvb_ctx* ctx, const cvb_kf_view* kf, const int32_t*
   B.in(P.valid, lms->valid, m); B.in(P.pos, lms->pos, (size_t)m * 3); B.in(P.normal, lms->normal, (size_t)m * 3); B.in(P.min_dist, lms->min_dist, m);
   B.in(P.max_dist, lms->max_dist, m); B.in(P.max_distance, lms->max_distance, m); B.in(P.desc, lms->desc, (size_t)m * 32);
   B.in(P.feat_idx, lms->feat_idx, m); B.in(P.feat, lms->feat_idx, m);
+  const std::vector<double> scale = scale_table(prm->scale_factor, prm->num_octaves);
+  const double* d_scale;
+  B.in(d_scale, scale.data(), scale.size());
   B.tmp(P.cand_idx, (size_t)m * kProjCap); B.tmp(P.cand_dist, (size_t)m * kProjCap); B.tmp(P.cand_n, m);
   B.out_host(P.action, m); B.out_host(P.best_idx, m); B.out_host(P.n_matches, 2);   // n_matches, then the overflow flag
   if (const int rc = B.place()) return rc;
@@ -447,7 +476,7 @@ int cvb_search_by_projection(cvb_ctx* ctx, const cvb_kf_view* kf, const int32_t*
   P.overflow = P.n_matches + 1;
   cudaStream_t st = ctx->stream;
   CVB_CUDA(ctx, cudaMemsetAsync(P.n_matches, 0, 8, st));
-  search_proj_kernel<<<1, 256, 0, st>>>(K, P, prm->th, prm->desc_th_low, prm->scale_factor, prm->num_octaves);
+  search_proj_kernel<<<1, 256, 0, st>>>(K, P, prm->th, prm->desc_th_low, d_scale, prm->num_octaves);
   CVB_CHECK_LAUNCH(ctx);
   if (const int rc = B.download()) return rc;
   const int* tail = B.host(P.n_matches);
@@ -718,6 +747,9 @@ int verify_landmark(cvb_ctx* ctx, const cvb_landmark_kf* q, const cvb_landmark_k
   B.in(d_skA, skipA.data(), nq); B.in(d_B, nullptr, NB * 32); B.in(d_skB, nullptr, NB);
   B.in(V.seg, seg.data(), (size_t)C + 1); B.in(d_seed, seed, C); B.in(d_cam, cam.data(), cam.size()); B.in(V.TcwB, TcwB.data(), TcwB.size());
   B.in(d_pairs, nullptr, C); B.in(d_recs, nullptr, C);
+  const std::vector<double> scale = scale_table(prm->search.scale_factor, prm->search.num_octaves);
+  const double* d_scale;
+  B.in(d_scale, scale.data(), scale.size());
   B.tmp(d_oA, NB); B.tmp(d_oB, NB); B.tmp(d_oD, NB); B.tmp(V.row, L); B.tmp(V.prob_ptr, (size_t)C + 1);
   B.tmp(V.pts, L * 3); B.tmp(V.f, L * 3); B.tmp(V.sg, L); B.tmp(V.srcA, L); B.tmp(d_mask, L);
   B.tmp(V.already1, L); B.tmp(d_a2, NB); B.tmp(d_mt1, L); B.tmp(d_mt2, NB); B.tmp(d_ms, L);
@@ -771,7 +803,7 @@ int verify_landmark(cvb_ctx* ctx, const cvb_landmark_kf* q, const cvb_landmark_k
   lmv_pose_kernel<<<C, kGlueThreads, 0, st>>>(V, d_pairs);
   CVB_CHECK_LAUNCH(ctx);
   // 4. SearchBySE3
-  search_se3_kernel<<<C, 256, 0, st>>>(d1, d_pairs, prm->search.th, prm->search.desc_th_low, prm->search.scale_factor, prm->search.num_octaves);
+  search_se3_kernel<<<C, 256, 0, st>>>(d1, d_pairs, prm->search.th, prm->search.desc_th_low, d_scale, prm->search.num_octaves);
   CVB_CHECK_LAUNCH(ctx);
   // 5. the residual pairs and the refinement
   lmv_residual_kernel<<<C, kGlueThreads, 0, st>>>(V, d_pairs, d_recs);

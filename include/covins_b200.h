@@ -252,7 +252,8 @@ typedef struct cvb_search_params {
   double th;                 /* search radius factor (matcher.search_radius_SE3 = 9.5) */
   int32_t desc_th_low;       /* matcher.desc_matching_th_low = 50 */
   int32_t num_octaves;       /* feat.num_octaves */
-  double scale_factor;       /* feat.scale_factor (PredictScale); the radius itself uses pow(2.0, level) (:366,:443) */
+  double scale_factor;       /* feat.scale_factor (> 1; PredictScale); SearchBySE3's radius uses pow(2.0, level) (:366,:443),
+                                SearchByProjection's pow(scale_factor, level) */
 } cvb_search_params;
 
 /*

@@ -1,5 +1,7 @@
 """Guided search (SearchBySE3) and RANSAC hypothesis scoring (SURVEY §8a M8 / V1): the C oracle against independent
 numpy restatements (CPU), the CUDA path against the oracle bit for bit (GPU, through the C-ABI)."""
+import math
+
 import numpy as np
 import pytest
 
@@ -230,38 +232,89 @@ def test_cuda_scoring_equals_oracle_bitwise(ctx):
 
 
 # ---------------------------------------------------------------------------------------------- SearchByProjection
-def _py_search_by_projection(view, kf_lm_cand, Tcw, cam, lms, matched, th=10.0, th_low=50):
-    """plain python restatement (pinhole + radtan, one octave), sequential like the reference"""
-    grid = _py_grid(view["kp"])
+def _py_rt(T, p):
+    """rows 0..2 of T (4x4, row-major flat) applied to p, each row summed left to right"""
+    return [(T[4 * r] * p[0] + T[4 * r + 1] * p[1] + T[4 * r + 2] * p[2]) + T[4 * r + 3] for r in range(3)]
+
+
+def py_project3(cam, pc):
+    """camera_->project3 in plain float64, the oracle's operation order: pinhole (0) / unified (1) x radtan (0) / equidistant
+    (1) / FOV (2); None = not projectable"""
+    intr, d = [float(v) for v in cam["intr"]], [float(v) for v in cam["dist"]]
+    dm = cam.get("dist_model", 0)
+    den = pc[2]
+    if cam.get("cam_model", 0) == 1:
+        den = pc[2] + float(cam["xi"]) * math.sqrt(pc[0] * pc[0] + pc[1] * pc[1] + pc[2] * pc[2])
+    if not den > 1e-10:
+        return None
+    x, y = pc[0] / den, pc[1] / den
+    r2 = x * x + y * y
+    if dm == 0:
+        rad = 1.0 + d[0] * r2 + d[1] * r2 * r2
+        xd = x * rad + 2.0 * d[2] * x * y + d[3] * (r2 + 2.0 * x * x)
+        yd = y * rad + d[2] * (r2 + 2.0 * y * y) + 2.0 * d[3] * x * y
+    else:
+        s = 1.0
+        if dm == 1:
+            r = math.sqrt(r2)
+            if r >= 1e-8:
+                th = math.atan(r); t2 = th * th
+                s = th * (1.0 + d[0] * t2 + d[1] * t2 * t2 + d[2] * t2 * t2 * t2 + d[3] * t2 * t2 * t2 * t2) / r
+        elif d[0] * d[0] >= 1e-5:
+            w = d[0]; c = 2.0 * math.tan(0.5 * w)
+            s = c / w if r2 < 1e-5 else math.atan(c * math.sqrt(r2)) / (w * math.sqrt(r2))
+        xd, yd = s * x, s * y
+    return intr[0] * xd + intr[2], intr[1] * yd + intr[3]
+
+
+def py_predict_scale(maxdist, d3, sf, num_octaves):
+    """LandmarkBase::PredictScale: ceil(log(maxdist / float(d3)) / log(sf)) clamped to [0, num_octaves - 1]"""
+    n = math.ceil(math.log(maxdist / float(np.float32(d3))) / math.log(sf))
+    return min(max(n, 0), num_octaves - 1)
+
+
+def _py_search_by_projection(view, kf_lm_cand, Tcw, cam, lms, matched, th=10.0, th_low=50, num_octaves=1, scale_factor=2.0):
+    """plain python restatement (every camera model, octaves), sequential like the reference; float64 / float32 scalars in the
+    oracle's operation order, so that it agrees at rounding boundaries too"""
+    grid = view["grid"] if "grid" in view else _py_grid(view["kp"])      # a scene may file keypoints in cells of its choice
     matched = matched.copy(); has_lm = view["lm_valid"].copy(); lm_cand = kf_lm_cand.copy(); feat = lms["feat_idx"].copy()
     bits = np.unpackbits(view["desc"], axis=1)
-    R, t = Tcw[:3, :3], Tcw[:3, 3]; Ow = -R.T @ t
-    d = np.asarray(cam["dist"]); intr = np.asarray(cam["intr"])
+    T = [float(v) for v in np.asarray(Tcw, np.float64).reshape(16)]
+    Ow = [-(T[r] * T[3] + T[4 + r] * T[7] + T[8 + r] * T[11]) for r in range(3)]
+    img = [float(v) for v in view["img_bounds"]]
+    w_inv, h_inv = 64 / 752.0, 48 / 480.0
+    kp = np.asarray(view["kp"], np.float32)
     m = len(lms["pos"]); action = np.zeros(m, np.int32); best_idx = np.full(m, -1, np.int32); nm = 0
     for i in range(m):
         if not lms["valid"][i]:
             continue
-        pw = lms["pos"][i]; pc = R @ pw + t
+        pw = [float(v) for v in lms["pos"][i]]
+        pc = _py_rt(T, pw)
         if pc[2] < 0:
             continue
-        x, y = pc[0] / pc[2], pc[1] / pc[2]; r2 = x * x + y * y; rad = 1 + d[0] * r2 + d[1] * r2 * r2
-        u = intr[0] * (x * rad + 2 * d[2] * x * y + d[3] * (r2 + 2 * x * x)) + intr[2]
-        v = intr[1] * (y * rad + d[2] * (r2 + 2 * y * y) + 2 * d[3] * x * y) + intr[3]
-        if not (0 <= u < 752 and 0 <= v < 480):
+        uv = py_project3(cam, pc)
+        if uv is None or not (img[0] <= uv[0] < img[1] and img[2] <= uv[1] < img[3]):
             continue
-        PO = pw - Ow; d3 = np.linalg.norm(PO)
-        if d3 < lms["min_dist"][i] or d3 > lms["max_dist"][i] or PO @ lms["normal"][i] < 0.5 * d3:
+        PO = [pw[r] - Ow[r] for r in range(3)]; n = [float(v) for v in lms["normal"][i]]
+        d3 = math.sqrt(PO[0] * PO[0] + PO[1] * PO[1] + PO[2] * PO[2])
+        if d3 < lms["min_dist"][i] or d3 > lms["max_dist"][i] or PO[0] * n[0] + PO[1] * n[1] + PO[2] * n[2] < 0.5 * d3:
             continue
-        tx, ty = np.float32(u), np.float32(v)
-        cx0 = max(0, int(np.floor((float(tx) - th) * 64 / 752))); cx1 = min(63, int(np.ceil((float(tx) + th) * 64 / 752)))
-        cy0 = max(0, int(np.floor((float(ty) - th) * 48 / 480))); cy1 = min(47, int(np.ceil((float(ty) + th) * 48 / 480)))
+        level = py_predict_scale(float(lms["max_distance"][i]), d3, scale_factor, num_octaves)
+        radius = th * math.pow(scale_factor, level)
+        tx, ty = np.float32(uv[0]), np.float32(uv[1])
+        cx0 = max(0, math.floor((float(tx) - radius) * w_inv)); cx1 = min(63, math.ceil((float(tx) + radius) * w_inv))
+        cy0 = max(0, math.floor((float(ty) - radius) * h_inv)); cy1 = min(47, math.ceil((float(ty) + radius) * h_inv))
+        if cx0 >= 64 or cx1 < 0 or cy0 >= 48 or cy1 < 0:
+            continue
         lb = np.unpackbits(lms["desc"][i]); ham = lambda k: int((bits[k] != lb).sum())
         bd, best = 256, -1
         for ix in range(cx0, cx1 + 1):
             for iy in range(cy0, cy1 + 1):
                 for idx in grid.get((ix, iy), []):
-                    dx = np.float32(view["kp"][idx, 0]) - tx; dy = np.float32(view["kp"][idx, 1]) - ty
-                    if float(np.sqrt(np.float32(dx * dx + dy * dy))) > th or matched[idx]:
+                    dx = kp[idx, 0] - tx; dy = kp[idx, 1] - ty
+                    if not float(np.sqrt(np.float32(dx * dx + dy * dy))) <= radius or matched[idx]:
+                        continue
+                    if not level - 1 <= int(view["octave"][idx]) <= level:
                         continue
                     dd = ham(idx)
                     if dd < bd:
