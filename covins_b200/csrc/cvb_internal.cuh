@@ -23,11 +23,6 @@ struct cvb_ctx {
   size_t h_pin_cap = 0;
   bool pin_busy = false;
   void* ba = nullptr;  // BA state (owned by ba_*.cu)
-  // resident operand tiles of a train set (set by the map database around its matching call, see tc_match.cu): when the
-  // matcher is handed the packed rows `xt_for`, their pre-expanded tiles are at `xt` / `xt_seg_tile`
-  const uint8_t* xt_for = nullptr;
-  const uint8_t* xt = nullptr;
-  const int32_t* xt_seg_tile = nullptr;
   // every extern "C" entry point holds this lock for its duration (cvb_device_guard): a ctx may be shared between host
   // threads — calls on one ctx are serialised, concurrency comes from one ctx per thread
   mutable std::recursive_mutex mtx;
@@ -114,10 +109,13 @@ int cvb_match_hamming_pairs_dev(cvb_ctx* ctx, const uint8_t* d_desc, const int32
                                 int32_t* d_match_train, float* d_match_dist, int32_t* d_n_matches);
 int cvb_match_l2_pairs_dev(cvb_ctx* ctx, const uint8_t* d_desc, const int32_t* d_pairs, int n_pairs, int max_nq, float thr, float ratio,
                            int32_t* d_match_train, float* d_match_dist, int32_t* d_n_matches);
-// cvb_match_l2_u8_dev: cvb_match_l2_batch on device u8 SIFT rows (the layout cvb_knn_l2_u8_batch_dev takes); outputs as
-// cvb_match_hamming_batch_dev.  The map database matches its SIFT keyframes through it.
-int cvb_match_l2_u8_dev(cvb_ctx* ctx, const uint8_t* d_q, int nq, const uint8_t* d_t, const int32_t* d_seg_ptr, const int32_t* h_seg_ptr,
-                        int n_seg, float thr, float ratio, int32_t* d_match_train, float* d_match_dist, int32_t* d_n_matches, void* stream);
+// cvb_match_dev: the fused 2-NN + ratio filter of cvb_match_{hamming,l2}_batch on device rows, metric 0 = Hamming (32-byte
+// rows), 1 = L2 (the u8 SIFT layout cvb_knn_l2_u8_batch_dev takes); outputs as cvb_match_hamming_batch_dev, on st.  d_xt /
+// d_seg_tile: the train rows' resident operand tiles (cvb_tc::expand_tiles), or nullptr when they have none.  The map
+// database matches its keyframes through it.
+int cvb_match_dev(cvb_ctx* ctx, int metric, const uint8_t* d_q, int nq, const uint8_t* d_t, const int32_t* d_seg_ptr,
+                  const int32_t* h_seg_ptr, int n_seg, const uint8_t* d_xt, const int32_t* d_seg_tile, float thr, float ratio,
+                  int32_t* d_match_train, float* d_match_dist, int32_t* d_n_matches, cudaStream_t st);
 
 // ransac_rel.cu: SIFT rows (CV_32F) to the u8 layout of the L2 kernels on the host; false if a value is not an integer in [0, 255]
 bool cvb_quantize_sift(const float* src, size_t n, uint8_t* dst);

@@ -211,12 +211,8 @@ int match_dev(cvb_ctx* ctx, cvb_db* db, const uint8_t* d_q, int nq, float thr, f
   const int n_seg = (int)db->seg_ptr.size() - 1;
   int rc = refresh_seg(ctx, db);
   if (rc) return rc;
-  ctx->xt_for = db->d_rows; ctx->xt = db->d_xt; ctx->xt_seg_tile = db->d_seg_tile;
-  rc = db->desc_bytes == 32
-           ? cvb_match_hamming_batch_dev(ctx, d_q, nq, db->d_rows, db->d_seg, db->seg_ptr.data(), n_seg, thr, ratio, d_mt, d_md, d_nm, stream)
-           : cvb_match_l2_u8_dev(ctx, d_q, nq, db->d_rows, db->d_seg, db->seg_ptr.data(), n_seg, thr, ratio, d_mt, d_md, d_nm, stream);
-  ctx->xt_for = nullptr; ctx->xt = nullptr; ctx->xt_seg_tile = nullptr;
-  return rc;
+  return cvb_match_dev(ctx, db->metric(), d_q, nq, db->d_rows, db->d_seg, db->seg_ptr.data(), n_seg, db->d_xt, db->d_seg_tile, thr,
+                       ratio, d_mt, d_md, d_nm, cvb_stream(ctx, stream));
 }
 
 // host request: q = ORB rows (u8) or SIFT rows (CV_32F, checked and quantised into the pinned staging buffer before any device

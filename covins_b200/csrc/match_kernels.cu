@@ -688,11 +688,13 @@ __global__ void shard_merge_kernel(const int32_t* __restrict__ idx_all, const in
     }
 }
 
-// Common implementation of knn / fused-match for both metrics (device pointers).
+// Common implementation of knn / fused-match for both metrics (device pointers).  d_xt / d_seg_tile: the train set's operand
+// tiles (cvb_tc::expand_tiles) when it has them resident, else nullptr (the tensor-core path then builds them per call).
 template <class M, int QPT_BIG>
 int knn_dev(cvb_ctx* ctx, const uint8_t* d_q, int nq, const uint8_t* d_t, const int32_t* d_seg_ptr,
-            const int32_t* h_seg_ptr, int n_seg, int k, int32_t* d_idx, void* d_dist, bool filter, float thr,
-            float ratio, int32_t* d_match_train, float* d_match_dist, int32_t* d_n_matches, cudaStream_t st) {
+            const int32_t* h_seg_ptr, int n_seg, const uint8_t* d_xt, const int32_t* d_seg_tile, int k, int32_t* d_idx,
+            void* d_dist, bool filter, float thr, float ratio, int32_t* d_match_train, float* d_match_dist,
+            int32_t* d_n_matches, cudaStream_t st) {
   CVB_REQUIRE(ctx, ctx != nullptr, "null ctx");
   CVB_REQUIRE(ctx, nq >= 0 && k >= 1 && k <= 4, "bad nq/k");
   int max_len = 0;
@@ -706,31 +708,21 @@ int knn_dev(cvb_ctx* ctx, const uint8_t* d_q, int nq, const uint8_t* d_t, const 
     CVB_CUDA(ctx, cudaMemsetAsync(d_n_matches, 0, sizeof(int32_t) * n_seg, st));
   }
   if (nq == 0) return CVB_OK;
-  if (cvb_tc::profitable(ctx, nq, n_seg, (long)total, max_len)) {   // tensor-core formulation (tc_match.cu), same results
-    cvb_tc::TcParams tp{};
-    tp.q = d_q; tp.nq = nq; tp.t = d_t; tp.seg_ptr = d_seg_ptr; tp.n_seg = n_seg;
-    tp.out_idx = d_idx; tp.out_dist = d_dist; tp.filter = filter ? 1 : 0; tp.thr = thr; tp.ratio = ratio;
-    tp.match_train = d_match_train; tp.match_dist = d_match_dist; tp.n_matches = d_n_matches;
-    tp.h_seg = h_seg_ptr;
-    if (ctx->xt_for == d_t && ctx->xt) { tp.xt = ctx->xt; tp.seg_tile = ctx->xt_seg_tile; }
-    return cvb_tc::launch(ctx, tp, M::kIsL2 ? 1 : 0, k, st);
-  }
-  {
-    // One very long segment (map-wide k-NN): too few segments to spread over the SMs as they are → cut it into uniform
-    // chunks, run the tensor-core kernel on the chunks and merge the chunk lists exactly (the same (distance, index)
-    // merge that combines GPU shards).
-    const char* e = getenv("COVINS_B200_MATCH_KERNEL");
-    const int nqb = (nq + 127) / 128;
-    const int parts = ctx->sm_count / nqb > 0 ? ctx->sm_count / nqb : 1;
-    if (!filter && n_seg == 1 && !(e && !strcmp(e, "popc")) && (long)nq * total >= (1L << 26) &&
-        total >= (int64_t)parts * 4 * 1024) {
-      int n_ps = parts * 4;
-      int64_t chunk = ((total + n_ps - 1) / n_ps + 127) / 128 * 128;
-      // the tensor-core kernel packs (distance, local index) keys: a chunk must stay below its index range (cvb_tc::profitable
-      // enforces the same bound on ordinary segments)
-      const int64_t max_chunk = ((int64_t)1 << cvb_tc::kIdxBits) - 128;
-      if (chunk > max_chunk) chunk = max_chunk;
-      n_ps = (int)((total + chunk - 1) / chunk);
+  const cvb_tc::Choice ch = cvb_tc::choose(ctx, nq, n_seg, total, max_len, filter);
+  switch (ch.kernel) {
+    case cvb_tc::Kernel::kTensor: {   // tensor-core formulation (tc_match.cu), same results
+      cvb_tc::TcParams tp{};
+      tp.q = d_q; tp.nq = nq; tp.t = d_t; tp.seg_ptr = d_seg_ptr; tp.n_seg = n_seg;
+      tp.out_idx = d_idx; tp.out_dist = d_dist; tp.filter = filter ? 1 : 0; tp.thr = thr; tp.ratio = ratio;
+      tp.match_train = d_match_train; tp.match_dist = d_match_dist; tp.n_matches = d_n_matches;
+      tp.xt = d_xt; tp.seg_tile = d_seg_tile; tp.h_seg = h_seg_ptr;
+      return cvb_tc::launch(ctx, tp, M::kIsL2 ? 1 : 0, k, st);
+    }
+    case cvb_tc::Kernel::kTensorChunks: {
+      // the tensor-core kernel on uniform chunks of the one segment, the chunk lists merged exactly (the same
+      // (distance, index) merge that combines GPU shards)
+      const int64_t chunk = ch.chunk;
+      const int n_ps = (int)((total + chunk - 1) / chunk);
       std::vector<int32_t> h_ps((size_t)n_ps + 1), h_off((size_t)n_ps);
       for (int c = 0; c <= n_ps; c++) h_ps[c] = (int32_t)std::min<int64_t>((int64_t)c * chunk, total);
       for (int c = 0; c < n_ps; c++) h_off[c] = (int32_t)((int64_t)c * chunk);
@@ -757,6 +749,8 @@ int knn_dev(cvb_ctx* ctx, const uint8_t* d_q, int nq, const uint8_t* d_t, const 
       CVB_CHECK_LAUNCH(ctx);
       return CVB_OK;
     }
+    case cvb_tc::Kernel::kScalar:
+      break;
   }
   const Plan pl = make_plan<M>(nq, n_seg, max_len, ctx->sm_count, QPT_BIG, true);
   ScanParams sp{};
@@ -939,8 +933,8 @@ int cvb_knn_hamming_batch_dev(cvb_ctx* ctx, const uint8_t* d_q, int nq, const ui
                               int32_t* d_idx, int32_t* d_dist, void* stream) {
   if (!ctx) return CVB_ERR_INVALID;
   CVB_GUARD(ctx);
-  return knn_dev<HammingMetric, 4>(ctx, d_q, nq, d_t, d_seg_ptr, h_seg_ptr, n_seg, k, d_idx, d_dist, false, 0.f,
-                                   0.f, nullptr, nullptr, nullptr, cvb_stream(ctx, stream));
+  return knn_dev<HammingMetric, 4>(ctx, d_q, nq, d_t, d_seg_ptr, h_seg_ptr, n_seg, nullptr, nullptr, k, d_idx, d_dist, false,
+                                   0.f, 0.f, nullptr, nullptr, nullptr, cvb_stream(ctx, stream));
 }
 
 int cvb_match_hamming_batch_dev(cvb_ctx* ctx, const uint8_t* d_q, int nq, const uint8_t* d_t,
@@ -949,8 +943,8 @@ int cvb_match_hamming_batch_dev(cvb_ctx* ctx, const uint8_t* d_q, int nq, const 
                                 void* stream) {
   if (!ctx) return CVB_ERR_INVALID;
   CVB_GUARD(ctx);
-  return knn_dev<HammingMetric, 4>(ctx, d_q, nq, d_t, d_seg_ptr, h_seg_ptr, n_seg, 2, nullptr, nullptr, true, thr,
-                                   ratio, d_match_train, d_match_dist, d_n_matches, cvb_stream(ctx, stream));
+  return knn_dev<HammingMetric, 4>(ctx, d_q, nq, d_t, d_seg_ptr, h_seg_ptr, n_seg, nullptr, nullptr, 2, nullptr, nullptr, true,
+                                   thr, ratio, d_match_train, d_match_dist, d_n_matches, cvb_stream(ctx, stream));
 }
 
 int cvb_knn_hamming_batch(cvb_ctx* ctx, const uint8_t* q, int nq, const uint8_t* t, const int32_t* seg_ptr,
@@ -1078,8 +1072,8 @@ int cvb_knn_l2_u8_batch_dev(cvb_ctx* ctx, const uint8_t* d_q, int nq, const uint
   if (!ctx) return CVB_ERR_INVALID;
   CVB_GUARD(ctx);
   if (dim != 128) return cvb_fail(ctx, CVB_ERR_UNSUPPORTED, "L2 k-NN is implemented for dim == 128 (SIFT), got %d", dim);
-  return knn_dev<L2Metric, 2>(ctx, d_q, nq, d_t, d_seg_ptr, h_seg_ptr, n_seg, k, d_idx, d_dist, false, 0.f, 0.f,
-                              nullptr, nullptr, nullptr, cvb_stream(ctx, stream));
+  return knn_dev<L2Metric, 2>(ctx, d_q, nq, d_t, d_seg_ptr, h_seg_ptr, n_seg, nullptr, nullptr, k, d_idx, d_dist, false, 0.f,
+                              0.f, nullptr, nullptr, nullptr, cvb_stream(ctx, stream));
 }
 
 // shared host path for cvb_knn_l2_batch / cvb_match_l2_batch
@@ -1113,8 +1107,8 @@ static int l2_host(cvb_ctx* ctx, const float* q, int nq, const float* t, const i
   if (bad[0] || bad[1])
     return cvb_fail(ctx, CVB_ERR_UNSUPPORTED,
                     "L2 descriptors must be integer-valued in [0,255] (cv::xfeatures2d::SIFT output)");
-  rc = knn_dev<L2Metric, 2>(ctx, d_q8, nq, d_t8, d_seg, seg_ptr, n_seg, k, d_i, d_d, filter, thr, ratio, d_i, d_d,
-                            d_nm, ctx->stream);
+  rc = knn_dev<L2Metric, 2>(ctx, d_q8, nq, d_t8, d_seg, seg_ptr, n_seg, nullptr, nullptr, k, d_i, d_d, filter, thr, ratio, d_i,
+                            d_d, d_nm, ctx->stream);
   if (rc) return rc;
   return B.download();
 }
@@ -1165,11 +1159,13 @@ int cvb_landmark_match_batch_dev(cvb_ctx* ctx, const uint8_t* d_A, const uint8_t
   rc = dispatch_scan<HammingMetric, 4, MODE_DM>(ctx, sp, pl, num_best, st);
   if (rc) return rc;
   if (smem <= 200 * 1024) {
-    static size_t attr = 0;
-    if (smem > attr) {
-      CVB_CUDA(ctx, cudaFuncSetAttribute(dm_assign_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         (int)(200 * 1024)));
-      attr = 200 * 1024;
+    static cvb_once_per_device once;
+    {
+      std::lock_guard<std::mutex> once_lk(once.mtx);
+      if (once.first(ctx->device)) {
+        CVB_CUDA(ctx, cudaFuncSetAttribute(dm_assign_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                           (int)(200 * 1024)));
+      }
     }
     dm_assign_kernel<true><<<n_seg, 256, smem, st>>>(li, ld, nA, num_best, d_seg_ptr, ithr, nullptr, nullptr, d_outA,
                                                      d_outB, d_outD, d_n_out);
@@ -1207,8 +1203,12 @@ int cvb_landmark_match_batch(cvb_ctx* ctx, const uint8_t* A, const uint8_t* skip
 
 }  // extern "C"
 
-int cvb_match_l2_u8_dev(cvb_ctx* ctx, const uint8_t* d_q, int nq, const uint8_t* d_t, const int32_t* d_seg_ptr, const int32_t* h_seg_ptr,
-                        int n_seg, float thr, float ratio, int32_t* d_match_train, float* d_match_dist, int32_t* d_n_matches, void* stream) {
-  return knn_dev<L2Metric, 2>(ctx, d_q, nq, d_t, d_seg_ptr, h_seg_ptr, n_seg, 2, nullptr, nullptr, true, thr, ratio, d_match_train,
-                              d_match_dist, d_n_matches, cvb_stream(ctx, stream));
+int cvb_match_dev(cvb_ctx* ctx, int metric, const uint8_t* d_q, int nq, const uint8_t* d_t, const int32_t* d_seg_ptr,
+                  const int32_t* h_seg_ptr, int n_seg, const uint8_t* d_xt, const int32_t* d_seg_tile, float thr, float ratio,
+                  int32_t* d_match_train, float* d_match_dist, int32_t* d_n_matches, cudaStream_t st) {
+  if (metric == 0)
+    return knn_dev<HammingMetric, 4>(ctx, d_q, nq, d_t, d_seg_ptr, h_seg_ptr, n_seg, d_xt, d_seg_tile, 2, nullptr, nullptr, true,
+                                     thr, ratio, d_match_train, d_match_dist, d_n_matches, st);
+  return knn_dev<L2Metric, 2>(ctx, d_q, nq, d_t, d_seg_ptr, h_seg_ptr, n_seg, d_xt, d_seg_tile, 2, nullptr, nullptr, true, thr,
+                              ratio, d_match_train, d_match_dist, d_n_matches, st);
 }

@@ -1,30 +1,28 @@
 // tc_match.cu — descriptor k-NN on the Hopper tensor cores (wgmma.mma_async, integer kinds, accumulators in registers).
 //
 // Same contract as scan_kernel in match_kernels.cu (K1 Hamming / K2 L2 lists), different bound.
-// The POPC formulation is bound by the integer pipe.  Here the pairwise term is a u8 x u8 -> s32 GEMM:
-//     Hamming(a,b) = popc(a) + popc(b) - 2 <bits(a), bits(b)>      (bits expanded to 0/1 bytes in shared memory)
-//     |a-b|^2      = |a|^2 + |b|^2 - 2 <a, b>                      (u8 SIFT, exact in s32)
-// issued as wgmma.mma_async.m64n128k32.s32.u8.u8 by a warpgroup (64 queries x 128 train rows, K = 32 bytes per
-// instruction) with both operands in shared memory.  A thread of the warpgroup holds two query rows x 32 columns of the
-// accumulator (rows 16 w + lane / 4 and + 8, columns 8 i + 2 (lane % 4) + {0, 1}); it sees its columns in ascending order,
-// keeps per-row k-lists with the sequential OpenCV / DenseMatcher rule, and the four threads of a quad merge their lists
-// by (key, index) at the end of a segment — so the result is bit-identical to the scalar kernel.
-//
-// Both metrics run on operand tiles stored in the tensor core's own layout (namespace xt below).  tc_scan_kernel, the Hamming
-// kernel that expands the packed rows itself, stays behind COVINS_B200_TC_XT=0:
-// warp-specialised, persistent CTA (one per SM), 4-stage ring:
-//   warps 0-7   consumers  (two warpgroups, query rows [0, 64) and [64, 128)): wait full[s] → K/32 x wgmma → wait →
-//                          empty[s] → epilogue d = pt[j] - 2 acc (+ pq) → k-lists
-//   warps 8-15  producers  wait empty[s] → read packed rows from HBM (coalesced 16-B loads) → expand / copy into the
-//                          canonical K-major no-swizzle layout → fence.proxy.async → full[s]
-// A CTA owns one block of 128 queries (expanded once into shared memory) and streams a contiguous range of candidate
-// segments.
+// The POPC formulation is bound by the integer pipe.  Here the pairwise term is an 8-bit GEMM, exact in s32:
+//     Hamming(a,b) = popc(a) + popc(b) - 2 <bits(a), bits(b)>      (bits expanded to bytes)
+//     |a-b|^2      = |a|^2 + |b|^2 - 2 <a, b>                      (u8 SIFT)
+// The train rows are read as operand tiles stored once in the tensor core's own shared-memory layout (expand_tiles: the map
+// database keeps them resident, the raw-pointer calls build them in the call's device memory first), so the matching kernel
+// (namespace xt) only copies tiles with the TMA engine and multiplies.  A CTA owns one block of 128 queries, written once into
+// shared memory, and a contiguous range of candidate segments:
+//   warp 16          producer: one lane issues cp.async.bulk copies of whole tiles into a ring of stages (mbarrier expect_tx)
+//   warps 0-15       consumers: four warpgroups (h, g) = query rows [64 h, 64 h + 64) x every second segment starting at g;
+//                    wgmma over the stage → epilogue into per-row k-lists; the stage is released once read (Hamming: after
+//                    the GEMM; L2: after the epilogue, which reads the tile's norms)
+// A thread of a warpgroup holds two query rows (16 (warp % 4) + lane / 4 and + 8) x the columns 8 i + 2 (lane % 4) + {0, 1} of the
+// accumulator; it sees its columns in ascending order, keeps per-row k-lists with the sequential OpenCV rule, and the four
+// threads of a quad merge their lists by (key, index) at the end of a segment — so the result is bit-identical to the scalar
+// kernel.
 #include <float.h>
 #include <limits.h>
 #include <stdio.h>
 #include <stdlib.h>
 #include <string.h>
 
+#include <algorithm>
 #include <vector>
 
 #include "cvb_internal.cuh"
@@ -34,8 +32,6 @@ namespace cvb_tc {
 
 constexpr int TM = 128;       // queries per CTA (two warpgroups of 64)
 constexpr int TN = 128;       // train rows per tile (wgmma N)
-constexpr int STAGES = 4;        // shared-memory ring of expanded train tiles
-constexpr int NORM_RING = 8;
 constexpr int kInf = 0x3FFFFFFF;   // list sentinel; rows that must never enter carry this as their norm term
 
 // ---- mbarrier / wgmma wrappers ---------------------------------------------------------------------------------
@@ -49,20 +45,12 @@ __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.
 #define CVB_R64                                                                                                         \
   "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31," \
   "%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}"
-// D[64 x 128] (+)= A[64 x 32] B[128 x 32]^T, both operands K-major in shared memory; B_SIGNED selects B = s8 (else u8)
-template <bool B_SIGNED>
-__device__ __forceinline__ void wg_mma_i8(uint32_t (&d)[64], uint64_t adesc, uint64_t bdesc, uint32_t acc) {
-  if constexpr (B_SIGNED) {
-    asm volatile(
-        "{\n.reg .pred p;\nsetp.ne.b32 p, %66, 0;\n"
-        "wgmma.mma_async.sync.aligned.m64n128k32.s32.u8.s8 " CVB_R64 ", %64, %65, p;\n}\n"
-        : CVB_D64 : "l"(adesc), "l"(bdesc), "r"(acc));
-  } else {
-    asm volatile(
-        "{\n.reg .pred p;\nsetp.ne.b32 p, %66, 0;\n"
-        "wgmma.mma_async.sync.aligned.m64n128k32.s32.u8.u8 " CVB_R64 ", %64, %65, p;\n}\n"
-        : CVB_D64 : "l"(adesc), "l"(bdesc), "r"(acc));
-  }
+// D[64 x 128] (+)= A[64 x 32] B[128 x 32]^T, A u8 and B s8 (the Hamming tiles), both operands K-major in shared memory
+__device__ __forceinline__ void wg_mma_u8s8(uint32_t (&d)[64], uint64_t adesc, uint64_t bdesc, uint32_t acc) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %66, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n128k32.s32.u8.s8 " CVB_R64 ", %64, %65, p;\n}\n"
+      : CVB_D64 : "l"(adesc), "l"(bdesc), "r"(acc));
 }
 #define CVB_D32 CVB_D8(0), CVB_D8(8), CVB_D8(16), CVB_D8(24)
 #define CVB_R32 "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}"
@@ -86,12 +74,12 @@ __device__ __forceinline__ void wg_commit_wait() {
 }
 // NSLICE instructions of K = 32 over operands whose K chunks of 16 B lie 128 B apart (+256 B = +16 in the address field
 // per instruction); the accumulator is overwritten by the first
-template <bool B_SIGNED, int NSLICE>
-__device__ __forceinline__ void wg_gemm(uint32_t (&d)[64], uint64_t adesc0, uint64_t bdesc0) {
+template <int NSLICE>
+__device__ __forceinline__ void wg_gemm_u8s8(uint32_t (&d)[64], uint64_t adesc0, uint64_t bdesc0) {
   wg_fence_operands(d);
   wg_fence();
 #pragma unroll
-  for (int k = 0; k < NSLICE; k++) wg_mma_i8<B_SIGNED>(d, adesc0 + (uint64_t)(k * 16), bdesc0 + (uint64_t)(k * 16), k > 0 ? 1u : 0u);
+  for (int k = 0; k < NSLICE; k++) wg_mma_u8s8(d, adesc0 + (uint64_t)(k * 16), bdesc0 + (uint64_t)(k * 16), k > 0 ? 1u : 0u);
   wg_commit_wait();
   wg_fence_operands(d);
 }
@@ -121,45 +109,34 @@ __device__ __forceinline__ uint4 ldg_nc(const void* p) {
   return r;
 }
 
-template <int S>
-__device__ __forceinline__ uint32_t shl(uint32_t w) {
-  if constexpr (S >= 0) return w << S; else return w >> (-S);
-}
-
-// ---- metrics: how a packed row becomes a K-major operand row, and its additive norm term ----------------------
-// A row is handled by TWO threads (half = 0/1), each loading kLoads 16-byte pieces of the packed row (so that the loads
-// of several tiles can be kept in flight in registers) and writing its share of the operand chunks.
+// ---- metrics: how a packed row becomes a K-major operand row of a tile, and its additive norm term ---------------
+// A train row is handled by TWO threads of expand_tiles_kernel (half = 0/1), each loading kLoads 16-byte pieces of the
+// packed row and writing its share of the operand chunks.
 struct TcHamming {
   static constexpr int kRowBytes = 32;    // packed bytes in HBM
-  static constexpr int kKBytes = 256;     // operand bytes (one byte per bit)
   static constexpr int kLoads = 1;        // uint4 per half row
-  static constexpr int kPrefetch = 3;     // tiles in flight per producer thread
   static __device__ __forceinline__ void load_half(const uint8_t* __restrict__ row, int half, uint4 (&v)[kLoads]) {
     v[0] = ldg_nc(row + 16 * half);
   }
   // writes operand chunks 8 half .. 8 half + 7 of the row and returns the partial popcount.  A set bit becomes the byte
-  // 1 << BIT: 0x40 (u8 64) in the train operand of tc_scan_kernel, 0x80 (s8 -128) in the resident tiles.
-  template <int BIT = 6>
+  // 0x80 (s8 -128).
   static __device__ __forceinline__ int store_half(const uint4 (&v)[kLoads], int half, uint8_t* dst_row0) {
     const uint32_t w[4] = {v[0].x, v[0].y, v[0].z, v[0].w};
-    constexpr uint32_t M = 0x01010101u << BIT;
+    constexpr uint32_t M = 0x80808080u;
     int pc = 0;
 #pragma unroll
     for (int i = 0; i < 4; i++) {
       pc += __popc(w[i]);
-      // byte j of output word k is 1 << BIT if bit (k + 8 j) of w[i] is set, else 0 (the same permutation on both operands)
+      // byte j of output word k is 0x80 if bit (k + 8 j) of w[i] is set, else 0 (the same permutation on both operands)
       uint4 lo, hi;
-      lo.x = shl<BIT>(w[i]) & M; lo.y = shl<BIT - 1>(w[i]) & M; lo.z = shl<BIT - 2>(w[i]) & M; lo.w = shl<BIT - 3>(w[i]) & M;
-      hi.x = shl<BIT - 4>(w[i]) & M; hi.y = shl<BIT - 5>(w[i]) & M; hi.z = shl<BIT - 6>(w[i]) & M; hi.w = shl<BIT - 7>(w[i]) & M;
+      lo.x = (w[i] << 7) & M; lo.y = (w[i] << 6) & M; lo.z = (w[i] << 5) & M; lo.w = (w[i] << 4) & M;
+      hi.x = (w[i] << 3) & M; hi.y = (w[i] << 2) & M; hi.z = (w[i] << 1) & M; hi.w = w[i] & M;
       *reinterpret_cast<uint4*>(dst_row0 + (8 * half + 2 * i) * 128) = lo;
       *reinterpret_cast<uint4*>(dst_row0 + (8 * half + 2 * i + 1) * 128) = hi;
     }
     return pc;
   }
-  // query side (one thread per row): the same K permutation with 0/1 bytes, so that accumulator = 64 popc(a & b) =
-  // (2 popc(a & b)) << 5, which is what the packed 16-bit keys of the epilogue subtract.  Packed word i of the row becomes
-  // operand bytes [32 i, 32 i + 32) = one K = 32 instruction.
-  static constexpr int kQWords = 8;
+  // query side (one thread per row): the packed row as 8 words and its popcount
   static __device__ __forceinline__ int load_q(const uint8_t* __restrict__ row, uint32_t (&w)[8]) {
     const uint4 a = ldg_nc(row), b = ldg_nc(row + 16);
     w[0] = a.x; w[1] = a.y; w[2] = a.z; w[3] = a.w; w[4] = b.x; w[5] = b.y; w[6] = b.z; w[7] = b.w;
@@ -167,10 +144,6 @@ struct TcHamming {
 #pragma unroll
     for (int i = 0; i < 8; i++) pc += __popc(w[i]);
     return pc;
-  }
-  static __device__ __forceinline__ void expand_q(const uint32_t (&w)[8], int i, uint32_t (&r)[8]) {
-#pragma unroll
-    for (int b = 0; b < 8; b++) r[b] = (w[i] >> b) & 0x01010101u;
   }
 };
 // u8 SIFT rows: the operand row is the row itself; the additive term is |row|^2 (the L2 operand tiles, namespace xt)
@@ -312,221 +285,18 @@ __device__ __forceinline__ void write_list(const TcParams& p, int seg, int q, bo
   }
 }
 
-constexpr int CONS_THREADS = 2 * 128;           // two consumer warpgroups
-constexpr int PROD_WARP0 = CONS_THREADS / 32;   // producer warps 8..15 (two threads per train row)
-constexpr int PROD_THREADS = 256;
-constexpr int NUM_THREADS = CONS_THREADS + PROD_THREADS;
-
-template <class M>
-constexpr size_t smem_bytes() {
-  return (size_t)(STAGES + 1) * TN * M::kKBytes + (size_t)NORM_RING * TN * sizeof(int) + 64 * sizeof(uint64_t);
-}
-
 // operand row r of a tile with KB operand bytes per row: byte offset of its chunk 0
 template <int KB>
 __device__ __forceinline__ uint32_t row_offset(int r) {
   return (uint32_t)(r >> 3) * (KB * 8) + (uint32_t)(r & 7) * 16;
 }
 
-template <class M, int K>
-__global__ void __launch_bounds__(NUM_THREADS, 1) tc_scan_kernel(const TcParams p) {
-  extern __shared__ __align__(1024) uint8_t smem[];
-  constexpr int KB = M::kKBytes;
-  uint8_t* sA = smem;                                        // the query block [TM][KB]
-  uint8_t* sB = sA + (size_t)TM * KB;                        // [STAGES][TN][KB]
-  int* sNorm = reinterpret_cast<int*>(sB + (size_t)STAGES * TN * KB);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sNorm + NORM_RING * TN);
-  uint64_t* full = bars;                 // [STAGES] producers → consumers (one arrival per producer warp)
-  uint64_t* empty = bars + STAGES;       // [STAGES] consumers' MMAs done → producers (one arrival per consumer warp)
-  __shared__ int sQNorm[TM];
-
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int qb = blockIdx.x % p.nqb, part = blockIdx.x / p.nqb;
-  const int seg0 = (int)((long)part * p.n_seg / p.parts), seg1 = (int)((long)(part + 1) * p.n_seg / p.parts);
-
-  // ---- one-time setup: barriers, the query operand ----
-  if (tid == 0) {
-    for (int s = 0; s < STAGES; s++) {
-      cvb_mbar_init(&full[s], PROD_THREADS / 32);
-      cvb_mbar_init(&empty[s], CONS_THREADS / 32);
-    }
-    cvb_fence_mbar_init();
-  }
-  if (tid < TM) {
-    const int q = qb * TM + tid;
-    uint32_t w[8];
-    int nrm = 0;
-    if (q < p.nq) {
-      nrm = M::load_q(p.q + (size_t)q * M::kRowBytes, w);
-    } else {
-#pragma unroll
-      for (int i = 0; i < 8; i++) w[i] = 0;
-    }
-    sQNorm[tid] = nrm;
-    uint8_t* dst = sA + row_offset<KB>(tid);
-#pragma unroll
-    for (int i = 0; i < KB / 32; i++) {
-      uint32_t r[8];
-      M::expand_q(w, i, r);
-      *reinterpret_cast<uint4*>(dst + (2 * i) * 128) = make_uint4(r[0], r[1], r[2], r[3]);
-      *reinterpret_cast<uint4*>(dst + (2 * i + 1) * 128) = make_uint4(r[4], r[5], r[6], r[7]);
-    }
-    fence_proxy_async();
-  }
-  __syncthreads();
-
-  if (warp >= PROD_WARP0) {
-    // =================================== producers ===================================
-    // Two threads per train row; the packed rows of the next kPrefetch tiles are held in registers so that the HBM
-    // latency (~1 us) of a tile overlaps the expansion of the previous ones.
-    const int pt = tid - PROD_WARP0 * 32;   // 0..255
-    const int prow = (pt & 7) | ((pt >> 4) << 3), half = (pt >> 3) & 1;
-    struct TileIt {
-      int seg, r0, s_begin, len, seg1;
-      const int32_t* sp;
-      bool done;
-      __device__ void next_seg() {
-        do {
-          seg++;
-          if (seg >= seg1) { done = true; return; }
-          s_begin = sp[seg];
-          len = sp[seg + 1] - s_begin;
-        } while (len == 0);
-        r0 = 0;
-      }
-      __device__ void advance() { r0 += TN; if (r0 >= len) next_seg(); }
-    };
-    TileIt it{seg0 - 1, 0, 0, 0, seg1, p.seg_ptr, false}, ld = it;
-    it.next_seg();
-    ld.next_seg();
-    constexpr int PF = M::kPrefetch;
-    uint4 pf[PF][M::kLoads];
-    auto issue_load = [&](uint4 (&v)[M::kLoads]) {
-      if (!ld.done) {
-        const int row = ld.r0 + prow;
-        if (row < ld.len) M::load_half(p.t + (size_t)(ld.s_begin + row) * M::kRowBytes, half, v);
-        ld.advance();
-      }
-    };
-#pragma unroll
-    for (int u = 0; u < PF; u++) issue_load(pf[u]);
-    int n = 0;
-    while (!it.done) {
-#pragma unroll
-      for (int u = 0; u < PF; u++) {
-        if (it.done) break;
-        uint4 cur[M::kLoads];
-#pragma unroll
-        for (int c = 0; c < M::kLoads; c++) cur[c] = pf[u][c];
-        issue_load(pf[u]);   // refill this register slot with the tile PF steps ahead
-        const int s = n % STAGES;
-        if (n >= STAGES) cvb_mbar_wait(&empty[s], ((n / STAGES) - 1) & 1);
-        uint8_t* dst = sB + (size_t)s * TN * KB + row_offset<KB>(prow);
-        const bool rv = it.r0 + prow < it.len;
-        int part = 0;
-        if (rv) {
-          part = M::store_half(cur, half, dst);
-        } else {
-          for (int c = 0; c < KB / 32; c++) *reinterpret_cast<uint4*>(dst + (half * (KB / 32) + c) * 128) = make_uint4(0, 0, 0, 0);
-        }
-        part += __shfl_xor_sync(0xffffffffu, part, 8);   // the two halves of a row sit 8 lanes apart
-        if (half == 0) {
-          // 16-bit column term ((popc(row) + 256) << 5 | slot), slot = 2 (column / 8) + column % 2 — the position
-          // of the column among the 32 columns one consumer thread holds; 0xFFFF = no row
-          reinterpret_cast<uint16_t*>(sNorm)[(n % NORM_RING) * TN + prow] =
-              rv ? (uint16_t)(((part + 256) << 5) | ((prow >> 3) << 1) | (prow & 1)) : (uint16_t)0xFFFFu;
-        }
-        // every lane makes its own stores visible to the async proxy; ONE arrival per warp
-        fence_proxy_async();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&full[s]);
-        it.advance();
-        n++;
-      }
-    }
-  } else {
-    // =================================== consumers: warpgroup h = query rows [64 h, 64 h + 64) ===================================
-    const int h = warp >> 2;
-    const int quad = lane & 3;
-    const int row0 = 64 * h + 16 * (warp & 3) + (lane >> 2);   // this thread's rows: row0 and row0 + 8
-    const bool valid0 = qb * TM + row0 < p.nq, valid1 = qb * TM + row0 + 8 < p.nq;
-    const int qn0 = sQNorm[row0], qn1 = sQNorm[row0 + 8];
-    const uint64_t a_desc = make_desc(cvb_smem_addr(sA + (size_t)h * 64 * KB), 128, KB * 8);
-    const uint32_t b_addr0 = cvb_smem_addr(sB);
-    int wk0[K], wk1[K];   // packed (distance, index) keys per row
-    int n = 0;
-    for (int seg = seg0; seg < seg1; seg++) {
-      const int len = p.seg_ptr[seg + 1] - p.seg_ptr[seg];
-#pragma unroll
-      for (int c = 0; c < K; c++) wk0[c] = wk1[c] = INT_MAX;
-      for (int r0 = 0; r0 < len; r0 += TN, n++) {
-        const int s = n % STAGES;
-        cvb_mbar_wait(&full[s], (n / STAGES) & 1);
-        uint32_t acc[64];
-        wg_gemm<false, KB / 32>(acc, a_desc, make_desc(b_addr0 + (uint32_t)s * (TN * KB), 128, KB * 8));
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&empty[s]);   // operands consumed: the producers may refill this stage
-        {
-          // Two columns per instruction: 16-bit keys ((popc(t) - 2 popc(q & t) + 256) << 5 | slot) packed pairwise
-          // (even column low, odd column high), k-lists kept per half with packed 16-bit min/max, merged into the 32-bit
-          // (distance, index) lists once per tile — and only if the tile holds a candidate that beats the current k-th
-          // entry (later tiles have larger indices, so "beats" is a strict distance comparison).
-          const uint32_t* nrm2 = reinterpret_cast<const uint32_t*>(reinterpret_cast<const uint16_t*>(sNorm) + (n % NORM_RING) * TN);
-          unsigned pk0[K], pk1[K];
-#pragma unroll
-          for (int c = 0; c < K; c++) pk0[c] = pk1[c] = 0xFFFFFFFFu;
-#pragma unroll
-          for (int i = 0; i < 16; i++) {
-            const unsigned nv = nrm2[4 * i + quad];   // columns 8 i + 2 quad (low half) and + 1 (high half)
-            insert_packed16<K>(pk0, nv - __byte_perm(acc[4 * i], acc[4 * i + 1], 0x5410));
-            insert_packed16<K>(pk1, nv - __byte_perm(acc[4 * i + 2], acc[4 * i + 3], 0x5410));
-          }
-#pragma unroll
-          for (int rr = 0; rr < 2; rr++) {
-            unsigned (&pk)[K] = rr ? pk1 : pk0;
-            int (&wk)[K] = rr ? wk1 : wk0;
-            const unsigned best16 = min(pk[0] & 0xFFFFu, pk[0] >> 16);
-            const int worst_v = wk[K - 1] == INT_MAX ? 1024 : (wk[K - 1] >> kIdxBits) + 256;   // arithmetic shift: t-domain value
-            if ((int)(best16 >> 5) < worst_v) {
-#pragma unroll
-              for (int c = 0; c < K; c++)
-#pragma unroll
-                for (int hh = 0; hh < 2; hh++) {
-                  const unsigned k16 = hh ? (pk[c] >> 16) : (pk[c] & 0xFFFFu);
-                  const int col = 8 * (int)((k16 & 31u) >> 1) + 2 * quad + (int)(k16 & 1u);
-                  insert_packed<K>(wk, k16 == 0xFFFFu ? INT_MAX
-                                                      : (int)((((unsigned)(k16 >> 5) - 256u) << kIdxBits) + (unsigned)(r0 + col)));
-                }
-            }
-          }
-        }
-      }
-      // ---- segment finished: merge the quad's lists; lane quad 0 writes row0, quad 1 writes row0 + 8 ----
-      const bool second = quad == 1;
-      int wk[K], wi[K];
-      float fd[K];
-      quad_merge_packed<K>(wk0);
-      quad_merge_packed<K>(wk1);
-      const int qq = (second ? qn1 : qn0) << kIdxBits;
-#pragma unroll
-      for (int c = 0; c < K; c++) {
-        const int x = second ? wk1[c] : wk0[c];
-        wi[c] = x == INT_MAX ? -1 : (x & ((1 << kIdxBits) - 1));
-        wk[c] = x == INT_MAX ? INT_MAX : ((x + qq) >> kIdxBits);
-        fd[c] = (float)wk[c];
-      }
-      write_list<K, false>(p, seg, qb * TM + row0 + (second ? 8 : 0), quad < 2 && (second ? valid1 : valid0), wk, wi, fd, lane);
-    }
-  }
-}
-
-
 // ===================================================================================================================
 // k-NN on PRE-EXPANDED operand tiles (Hamming as described here; L2 on tiles of u8 rows + |t|^2, see XtL2 below).
 //
-// The kernel above spends its issue slots on ALU work: producers turn every packed bit into a byte (>= 64 logic
-// operations per row and tile) and the epilogue rebuilds the distance from the accumulator and a per-column term read
-// from shared memory.  Both disappear when the operand the tensor core reads is stored once and reused by every query:
+// Turning every packed bit into a byte inside the matching kernel (>= 64 logic operations per row and tile) and rebuilding
+// the distance from the accumulator in the epilogue would spend the kernel's issue slots on ALU work.  Both disappear when
+// the operand the tensor core reads is stored once and reused by every query:
 //
 //   * cvb_tc::expand_tiles writes, per keyframe, ceil(rows / 128) tiles of 128 rows x 288 operand bytes in exactly the
 //     shared-memory image wgmma wants (K-major, no swizzle, 8-row groups of 2304 B): 256 data bytes (0x80 = -128
@@ -605,9 +375,9 @@ __global__ void __launch_bounds__(256) expand_tiles_kernel(const uint8_t* __rest
     if (half == 0) reinterpret_cast<int*>(tile_base + TN * X::KX)[prow] = rv ? part : kInf;
   } else {
     if (rv) {
-      uint4 v[1];
-      TcHamming::load_half(t + (size_t)(s_begin + r0 + prow) * 32, half, v);
-      part = TcHamming::store_half<7>(v, half, dst);
+      uint4 v[TcHamming::kLoads];
+      TcHamming::load_half(t + (size_t)(s_begin + r0 + prow) * TcHamming::kRowBytes, half, v);
+      part = TcHamming::store_half(v, half, dst);
     } else {
 #pragma unroll
       for (int c = 0; c < 8; c++) *reinterpret_cast<uint4*>(dst + (8 * half + c) * 128) = make_uint4(0, 0, 0, 0);
@@ -703,7 +473,7 @@ __global__ void __launch_bounds__(XTHREADS, 1) tc_xt_kernel(const TcParams p) {
       uint32_t w[8];
       int pq = 0;
       if (q < p.nq) {
-        pq = TcHamming::load_q(p.q + (size_t)q * 32, w);
+        pq = TcHamming::load_q(p.q + (size_t)q * TcHamming::kRowBytes, w);
       } else {
 #pragma unroll
         for (int i = 0; i < 8; i++) w[i] = 0;
@@ -796,7 +566,7 @@ __global__ void __launch_bounds__(XTHREADS, 1) tc_xt_kernel(const TcParams p) {
           cvb_mbar_wait(&full[s], (n / STAGES_X) & 1);
           if constexpr (!X::kIsL2) {
             uint32_t acc[64];
-            wg_gemm<true, X::NSLICE>(acc, a_desc, make_desc(b_addr0 + (uint32_t)s * STRIDE, 128, KX * 8));
+            wg_gemm_u8s8<X::NSLICE>(acc, a_desc, make_desc(b_addr0 + (uint32_t)s * STRIDE, 128, KX * 8));
             __syncwarp();
             if (lane == 0) mbar_arrive(&empty[s]);   // operands consumed: the producer may refill this stage
             unsigned pk0[K], pk1[K];
@@ -930,29 +700,20 @@ int expand_tiles(cvb_ctx* ctx, int metric, const uint8_t* d_rows, const int32_t*
   return CVB_OK;
 }
 
-template <class M, int K>
-int launch_tc(cvb_ctx* ctx, const TcParams& p, cudaStream_t st) {
-  static cvb_once_per_device once;
-  const size_t smem = smem_bytes<M>();
-  {
-    std::lock_guard<std::mutex> once_lk(once.mtx);
-    if (once.first(ctx->device)) {
-      CVB_CUDA(ctx, cudaFuncSetAttribute(tc_scan_kernel<M, K>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    }
-  }
-  tc_scan_kernel<M, K><<<p.nqb * p.parts, NUM_THREADS, smem, st>>>(p);
-  CVB_CHECK_LAUNCH(ctx);
-  return CVB_OK;
-}
-
-bool profitable(const cvb_ctx* ctx, int nq, int n_seg, long total_rows, int max_seg_len) {
-  if (max_seg_len >= (1 << kIdxBits)) return false;   // packed (distance, index) keys need < 4 Mi rows per segment
+Choice choose(const cvb_ctx* ctx, int nq, int n_seg, int64_t total, int max_len, bool filter) {
   const char* e = getenv("COVINS_B200_MATCH_KERNEL");
-  if (e && !strcmp(e, "popc")) return false;
-  if (e && !strcmp(e, "tc")) return n_seg >= 1 && nq >= 1;
+  const bool popc = e && !strcmp(e, "popc"), tc = e && !strcmp(e, "tc");
   const int nqb = (nq + TM - 1) / TM;
-  const int want_parts = ctx->sm_count / nqb > 0 ? ctx->sm_count / nqb : 1;
-  return n_seg >= want_parts && (long)nq * total_rows >= (1L << 26);
+  const int parts = std::max(1, ctx->sm_count / nqb);   // CTAs per query block that fill the SMs
+  const bool big = (int64_t)nq * total >= ((int64_t)1 << 26);
+  const int64_t max_rows = (int64_t)1 << kIdxBits;     // packed (distance, index) keys: a scanned segment stays below this
+  if (max_len < max_rows && (tc || (!popc && n_seg >= parts && big))) return {Kernel::kTensor, 0};
+  // one long segment (map-wide k-NN) is too few to spread over the SMs: about four whole-tile chunks per part
+  if (!filter && n_seg == 1 && !popc && big && total >= (int64_t)4 * parts * 1024) {
+    const int64_t chunk = ((total + 4 * parts - 1) / (4 * parts) + TN - 1) / TN * TN;
+    return {Kernel::kTensorChunks, std::min(chunk, max_rows - TN)};
+  }
+  return {Kernel::kScalar, 0};
 }
 
 int launch(cvb_ctx* ctx, TcParams p, int metric, int k, cudaStream_t st) {
@@ -961,34 +722,29 @@ int launch(cvb_ctx* ctx, TcParams p, int metric, int k, cudaStream_t st) {
   if (parts < 1) parts = 1;
   if (parts > p.n_seg) parts = p.n_seg;
   p.parts = parts;
-  if (metric == 1 || !(getenv("COVINS_B200_TC_XT") && !strcmp(getenv("COVINS_B200_TC_XT"), "0"))) {
-    cvb_block B(ctx, st);
-    if (!p.xt) {
-      // no resident tile store for this train set (raw-pointer API): expand it into the call's block first (HBM-bound pre-pass)
-      CVB_REQUIRE(ctx, p.h_seg != nullptr, "tensor-core path needs the host copy of the segment table");
-      std::vector<int32_t> h_tile;
-      const int64_t n_tiles = tiles_of(p.h_seg, p.n_seg, &h_tile);
-      int32_t* d_tile;
-      uint8_t* d_xt;
-      B.tmp(d_tile, (size_t)p.n_seg + 1); B.tmp(d_xt, (size_t)n_tiles * tile_bytes(metric));
-      if (const int rc = B.place()) return rc;
-      CVB_CUDA(ctx, cudaMemcpyAsync(d_tile, h_tile.data(), sizeof(int32_t) * ((size_t)p.n_seg + 1), cudaMemcpyHostToDevice, st));
-      CVB_CUDA(ctx, cudaStreamSynchronize(st));   // h_tile goes out of scope
-      const int rc = expand_tiles(ctx, metric, p.t, p.seg_ptr, d_tile, 0, p.n_seg, 0, (int)n_tiles, d_xt, st);
-      if (rc) return rc;
-      p.xt = d_xt;
-      p.seg_tile = d_tile;
-    }
-#define XT_CASE(XX) \
-    switch (k) { case 1: return xt::launch_xt<XX, 1>(ctx, p, st); case 2: return xt::launch_xt<XX, 2>(ctx, p, st); \
-                 case 3: return xt::launch_xt<XX, 3>(ctx, p, st); default: return xt::launch_xt<XX, 4>(ctx, p, st); }
-    if (metric == 0) XT_CASE(xt::XtHamming)
-    XT_CASE(xt::XtL2)
-#undef XT_CASE
+  cvb_block B(ctx, st);
+  if (!p.xt) {
+    // no resident tile store for this train set (raw-pointer API): expand it into the call's block first (HBM-bound pre-pass)
+    CVB_REQUIRE(ctx, p.h_seg != nullptr, "tensor-core path needs the host copy of the segment table");
+    std::vector<int32_t> h_tile;
+    const int64_t n_tiles = tiles_of(p.h_seg, p.n_seg, &h_tile);
+    int32_t* d_tile;
+    uint8_t* d_xt;
+    B.tmp(d_tile, (size_t)p.n_seg + 1); B.tmp(d_xt, (size_t)n_tiles * tile_bytes(metric));
+    if (const int rc = B.place()) return rc;
+    CVB_CUDA(ctx, cudaMemcpyAsync(d_tile, h_tile.data(), sizeof(int32_t) * ((size_t)p.n_seg + 1), cudaMemcpyHostToDevice, st));
+    CVB_CUDA(ctx, cudaStreamSynchronize(st));   // h_tile goes out of scope
+    const int rc = expand_tiles(ctx, metric, p.t, p.seg_ptr, d_tile, 0, p.n_seg, 0, (int)n_tiles, d_xt, st);
+    if (rc) return rc;
+    p.xt = d_xt;
+    p.seg_tile = d_tile;
   }
-#define TC_CASE(MM, KK) return launch_tc<MM, KK>(ctx, p, st)
-  switch (k) { case 1: TC_CASE(TcHamming, 1); case 2: TC_CASE(TcHamming, 2); case 3: TC_CASE(TcHamming, 3); default: TC_CASE(TcHamming, 4); }
-#undef TC_CASE
+#define XT_CASE(XX) \
+  switch (k) { case 1: return xt::launch_xt<XX, 1>(ctx, p, st); case 2: return xt::launch_xt<XX, 2>(ctx, p, st); \
+               case 3: return xt::launch_xt<XX, 3>(ctx, p, st); default: return xt::launch_xt<XX, 4>(ctx, p, st); }
+  if (metric == 0) XT_CASE(xt::XtHamming)
+  XT_CASE(xt::XtL2)
+#undef XT_CASE
 }
 
 }  // namespace cvb_tc

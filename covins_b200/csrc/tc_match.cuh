@@ -1,4 +1,4 @@
-// tc_match.cuh — interface of the wgmma (tensor-core) matching kernel, see tc_match.cu
+// tc_match.cuh — interface of the wgmma (tensor-core) matching kernel and of the matcher's kernel choice, see tc_match.cu
 #pragma once
 #include <vector>
 
@@ -40,7 +40,16 @@ size_t tile_bytes(int metric);
 int expand_tiles(cvb_ctx* ctx, int metric, const uint8_t* d_rows, const int32_t* d_seg_ptr, const int32_t* d_seg_tile, int seg_lo,
                  int seg_hi, int tile_lo, int n_tiles, uint8_t* d_xt, cudaStream_t st);
 
-// true when the tensor-core kernel fills the GPU for this shape (enough candidate segments per query block)
-bool profitable(const cvb_ctx* ctx, int nq, int n_seg, long total_rows, int max_seg_len);
+// The formulation that matches nq >= 1 queries against n_seg segments of `total` rows, the longest max_len rows (filter: the
+// fused ratio filter of k = 2).  kTensor: launch() on the segments, when there are enough of them per query block to fill
+// the SMs.  kTensorChunks: one long segment cut into `chunk`-row segments for launch(), whose lists the caller merges by
+// (distance, index).  kScalar: the POPC / DP4A scan of match_kernels.cu.  COVINS_B200_MATCH_KERNEL=popc forces the scalar
+// scan; =tc forces the tensor cores wherever the packed keys can index every segment.
+enum class Kernel { kScalar, kTensor, kTensorChunks };
+struct Choice {
+  Kernel kernel;
+  int64_t chunk;   // kTensorChunks: rows per chunk, a multiple of 128 below 2^kIdxBits
+};
+Choice choose(const cvb_ctx* ctx, int nq, int n_seg, int64_t total, int max_len, bool filter);
 
 }  // namespace cvb_tc

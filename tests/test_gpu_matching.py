@@ -150,6 +150,30 @@ def test_landmark_match_ties_and_displacement_chains(ctx):
     assert np.array_equal(a, ra) and np.array_equal(b, rb)
 
 
+def test_landmark_match_large_shared_memory_on_two_devices(ctx):
+    """The DenseMatcher's assignment kernel needs more than 48 KB of dynamic shared memory here ((2 nA num_best + 2 max_len)
+    int32), which each device has to allow separately: the same call on device 0, then on device 1."""
+    import torch
+    import covins_b200
+    if torch.cuda.device_count() < 2:
+        pytest.skip("needs two GPUs")
+    desc, lm = synth.orb_keyframes(seed=31, n_kf=3, n_feat=2000, n_lm=3000, window=3000)
+    A, skipA = desc[0], (lm[0] < 0).astype(np.uint8)
+    B, skipB = desc[1:].reshape(-1, 32), (lm[1:] < 0).reshape(-1).astype(np.uint8)
+    seg = synth.seg_ptr_uniform(2, 2000)
+    assert (2 * len(A) * 4 + 2 * 2000) * 4 > 48 * 1024
+    ref = [ora.landmark_match(A, skipA, B[seg[s]:seg[s + 1]], skipB[seg[s]:seg[s + 1]], 50.0, 4) for s in range(2)]
+    assert sum(len(r[0]) for r in ref) > 100
+    ctx1 = covins_b200.Context(1)
+    try:
+        for c in (ctx, ctx1):
+            out = M.landmark_match(c, A, skipA, B, skipB, seg, thr=50.0, num_best=4)
+            for s in range(2):
+                assert all(np.array_equal(x, r) for x, r in zip(out[s], ref[s])), (c.device, s)
+    finally:
+        ctx1.close()
+
+
 # ---------------------------------------------------------------------------------------------- device path
 def test_device_path_equals_host_path(ctx):
     import torch

@@ -69,13 +69,6 @@ def test_tc_ties_and_filter_vs_oracle(ctx, tc):
     assert np.array_equal(mt, rmt) and np.array_equal(nm, rc)
 
 
-def test_tc_expanding_hamming_kernel_ties_and_filter_vs_oracle(ctx, tc, monkeypatch):
-    """the same cases on the Hamming kernel that expands the packed rows itself (tc_scan_kernel) instead of reading
-    resident operand tiles"""
-    monkeypatch.setenv("COVINS_B200_TC_XT", "0")
-    test_tc_ties_and_filter_vs_oracle(ctx, None)
-
-
 def test_tc_l2_vs_oracle(ctx, tc):
     s, _ = synth.sift_keyframes(seed=3, n_kf=7, n_feat=300, n_lm=500, window=500)
     q = s[0][:211]
