@@ -52,8 +52,8 @@ using namespace bam;
 struct ObsLin {
   double r[2], Jp[12], Jl[6];
 };
-struct ObsWY {
-  double W[18], Y[18];
+struct __align__(16) ObsW {   // 16-byte aligned: gathered as nine 16-byte loads
+  double W[18];
 };
 
 // Column of (keyframe kf, local parameter c) in the reduced camera system: c < 6 pose, c >= 6 speed-bias.  The
@@ -142,7 +142,7 @@ struct Engine {
   DevArr<int> obs_kf, obs_lm, lm_ptr, kf_ptr, kf_obs;
   DevArr<double> obs_uv, obs_sigma;
   DevArr<ObsLin> lin;
-  DevArr<ObsWY> wy;
+  DevArr<ObsW> ow;
   DevArr<double> Hll, HllInv, bl;
   // imu
   DevArr<ImuPre> pre;
@@ -156,11 +156,18 @@ struct Engine {
   DevArr<int> fb_hi, fb_lo, fb_ptr, ft_type, ft_fac, ft_rhi, ft_rlo;   // factor blocks / terms
   int n_fb = 0;
   DevArr<int> sb_hi, sb_lo, sb_ptr, sp_a, sp_b;                         // schur blocks / pairs
-  int n_sb = 0;
+  DevArr<int> kf_sb;                                                    // first schur block of each hi keyframe
+  int n_sb = 0, row_stage = 0;                                          // row_stage: observations schur_row_kernel stages
   // vectors of size n_vec: [cam part n_c_pad | landmark part 3 L_in]
   DevArr<double> scale, colsq, diag, gvec, grad, sgrad, gn, step, xsol, yb, gs, tmp;
   DevArr<double> scale0;   // 0/1 activity mask of this rank's columns: engine_begin derives `scale` from it
   DevArr<double> S, linv;
+  // S's fill tiles (in L's structure, not in S's): zeroed on st_fill beside the block kernels, joined before the factor
+  DevArr<int> xt_fill;
+  int n_xt_fill = 0;
+  cudaStream_t st_fill = nullptr;
+  cudaEvent_t ev_fill_fork = nullptr, ev_fill_done = nullptr;
+  bool fill_pending = false;
   DevArr<int> flag;
   DevArr<double> partials, scalars, rankmax;
   double* h_scalars = nullptr;   // pinned
@@ -190,18 +197,21 @@ struct Engine {
       fprintf(stderr, "[destroy] %-26s %8.2f ms\n", what, std::chrono::duration<double, std::milli>(now - t_prev).count());
       t_prev = now;
     };
+    if (st_fill) { cudaStreamSynchronize(st_fill); cudaStreamDestroy(st_fill); }   // S may still be being cleared
+    if (ev_fill_fork) cudaEventDestroy(ev_fill_fork);
+    if (ev_fill_done) cudaEventDestroy(ev_fill_done);
     for (int i = 0; i < 2; i++) { pose[i].free_(); sb[i].free_(); lm[i].free_(); }
     pose0.free_(); sb0.free_(); lm0.free_();
     pose_const.free_(); off_pose.free_(); off_sb.free_(); xt_all.free_(); xt_own.free_(); col_owner.free_(); xbuf.free_(); flagd.free_(); plan.release(); extr_kf.free_(); intr_kf.free_(); dist_kf.free_(); xi_kf.free_(); model_kf.free_();
     obs_kf.free_(); obs_lm.free_(); lm_ptr.free_(); kf_ptr.free_(); kf_obs.free_(); obs_uv.free_(); obs_sigma.free_();
-    lin.free_(); wy.free_(); Hll.free_(); HllInv.free_(); bl.free_();
+    lin.free_(); ow.free_(); Hll.free_(); HllInv.free_(); bl.free_();
     pre.free_(); imu_i.free_(); imu_j.free_(); Jimu.free_(); rimu.free_();
     edge_i.free_(); edge_j.free_(); edge_q.free_(); edge_t.free_(); edge_S.free_(); Jedge.free_(); redge.free_();
     edge_robust.free_();
     fb_hi.free_(); fb_lo.free_(); fb_ptr.free_(); ft_type.free_(); ft_fac.free_(); ft_rhi.free_(); ft_rlo.free_();
-    sb_hi.free_(); sb_lo.free_(); sb_ptr.free_(); sp_a.free_(); sp_b.free_();
+    sb_hi.free_(); sb_lo.free_(); sb_ptr.free_(); sp_a.free_(); sp_b.free_(); kf_sb.free_();
     scale.free_(); scale0.free_(); colsq.free_(); diag.free_(); gvec.free_(); grad.free_(); sgrad.free_(); gn.free_(); step.free_();
-    xsol.free_(); yb.free_(); gs.free_(); tmp.free_();
+    xsol.free_(); yb.free_(); gs.free_(); tmp.free_(); xt_fill.free_();
     if (S_raw) { S.p = nullptr; linv.p = nullptr; }
     S.free_(); linv.free_(); flag.free_(); partials.free_();
     scalars.free_(); rankmax.free_();
@@ -280,7 +290,7 @@ __global__ void __launch_bounds__(256, 2) lin_obs_kernel(int n_obs, const int* _
                                                       const double* __restrict__ xi_kf, const double* __restrict__ scale,
                                                       const int* __restrict__ off_pose, int n_c_pad, double a2, int mode,
                                                       ObsLin* __restrict__ lin,
-                                                      ObsWY* __restrict__ wy, double* __restrict__ norms,
+                                                      ObsW* __restrict__ ow, double* __restrict__ norms,
                                                       double* __restrict__ partials, int slot) {
   double csum[1] = {0.0};
   for (int o = blockIdx.x * blockDim.x + threadIdx.x; o < n_obs; o += gridDim.x * blockDim.x) {
@@ -312,7 +322,7 @@ __global__ void __launch_bounds__(256, 2) lin_obs_kernel(int n_obs, const int* _
       rec.Jl[3 + c2] = Jl[3 + c2] * sc * sl[c2];
     }
     lin[o] = rec;
-    ObsWY* w = wy + o;   // W = Jp^T Jl (6x3)
+    ObsW* w = ow + o;   // W = Jp^T Jl (6x3)
 #pragma unroll
     for (int a = 0; a < 6; a++)
 #pragma unroll
@@ -375,72 +385,49 @@ __global__ void lm_damp_inv_kernel(int L, const double* __restrict__ Hll, const 
   o[5] = (a * d - b * b) * id;
 }
 
-// Y = W * Hll^-1 (6x3)
-__global__ void obs_Y_kernel(int n_obs, const int* __restrict__ obs_lm, const double* __restrict__ HllInv,
-                             ObsWY* __restrict__ wy) {
-  const int o = blockIdx.x * blockDim.x + threadIdx.x;
-  if (o >= n_obs) return;
-  const double* h = HllInv + 6 * (size_t)obs_lm[o];
+// Y = W * Hll^-1 (6x3) of one observation, h the packed symmetric inverse
+__device__ __forceinline__ void obs_y(const double* __restrict__ W, const double* __restrict__ h, double (&Y)[18]) {
   const double H[9] = {h[0], h[1], h[2], h[1], h[3], h[4], h[2], h[4], h[5]};
-  ObsWY* w = wy + o;
 #pragma unroll
   for (int a = 0; a < 6; a++)
 #pragma unroll
-    for (int b = 0; b < 3; b++) w->Y[3 * a + b] = w->W[3 * a] * H[b] + w->W[3 * a + 1] * H[3 + b] + w->W[3 * a + 2] * H[6 + b];
+    for (int b = 0; b < 3; b++) Y[3 * a + b] = W[3 * a] * H[b] + W[3 * a + 1] * H[3 + b] + W[3 * a + 2] * H[6 + b];
 }
 
-// per keyframe (one warp): Hpp = sum Jp^T Jp → lower part of the 6x6 diagonal block of S; g_c = sum Jp^T r;
-// yb = sum Y b_l
+// per keyframe (one warp): Hpp = sum Jp^T Jp → lower part of the 6x6 diagonal block of S; g_c = sum Jp^T r
 __global__ void __launch_bounds__(128) kf_visual_kernel(int K, const int* __restrict__ kf_ptr, const int* __restrict__ kf_obs,
-                                                        const int* __restrict__ obs_lm, const ObsLin* __restrict__ lin,
-                                                        const ObsWY* __restrict__ wy, const double* __restrict__ bl,
-                                                        const int* __restrict__ off_pose, SView S,
-                                                        double* __restrict__ g_c, double* __restrict__ yb, int what) {
+                                                        const ObsLin* __restrict__ lin, const int* __restrict__ off_pose,
+                                                        SView S, double* __restrict__ g_c) {
   const int k = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
   if (k >= K) return;
-  double h[21], b[6], y[6];
+  double h[21], b[6];
 #pragma unroll
   for (int i = 0; i < 21; i++) h[i] = 0.0;
 #pragma unroll
-  for (int i = 0; i < 6; i++) b[i] = y[i] = 0.0;
+  for (int i = 0; i < 6; i++) b[i] = 0.0;
   for (int e = kf_ptr[k] + lane; e < kf_ptr[k + 1]; e += 32) {
-    const int o = kf_obs[e];
-    if (what == 0) {
-      const ObsLin& L = lin[o];
-      int idx = 0;
+    const ObsLin& L = lin[kf_obs[e]];
+    int idx = 0;
 #pragma unroll
-      for (int r = 0; r < 6; r++)
+    for (int r = 0; r < 6; r++)
 #pragma unroll
-        for (int c = 0; c <= r; c++) h[idx++] += L.Jp[r] * L.Jp[c] + L.Jp[6 + r] * L.Jp[6 + c];
+      for (int c = 0; c <= r; c++) h[idx++] += L.Jp[r] * L.Jp[c] + L.Jp[6 + r] * L.Jp[6 + c];
 #pragma unroll
-      for (int r = 0; r < 6; r++) b[r] += L.Jp[r] * L.r[0] + L.Jp[6 + r] * L.r[1];
-    } else {
-      const double* bb = bl + 3 * (size_t)obs_lm[o];
-      const double* Y = wy[o].Y;
-#pragma unroll
-      for (int r = 0; r < 6; r++) y[r] += Y[3 * r] * bb[0] + Y[3 * r + 1] * bb[1] + Y[3 * r + 2] * bb[2];
-    }
+    for (int r = 0; r < 6; r++) b[r] += L.Jp[r] * L.r[0] + L.Jp[6 + r] * L.r[1];
   }
 #pragma unroll
   for (int off = 16; off > 0; off >>= 1) {
 #pragma unroll
     for (int i = 0; i < 21; i++) h[i] += __shfl_xor_sync(0xffffffffu, h[i], off);
 #pragma unroll
-    for (int i = 0; i < 6; i++) {
-      b[i] += __shfl_xor_sync(0xffffffffu, b[i], off);
-      y[i] += __shfl_xor_sync(0xffffffffu, y[i], off);
-    }
+    for (int i = 0; i < 6; i++) b[i] += __shfl_xor_sync(0xffffffffu, b[i], off);
   }
   if (lane == 0) {
     const int base = off_pose[k];
-    if (what == 0) {
-      int idx = 0;
-      for (int r = 0; r < 6; r++)
-        for (int c = 0; c <= r; c++) *s_at(S, base + r, base + c) = h[idx++];   // lower triangle only
-      for (int r = 0; r < 6; r++) g_c[base + r] = b[r];
-    } else {
-      for (int r = 0; r < 6; r++) yb[base + r] = y[r];
-    }
+    int idx = 0;
+    for (int r = 0; r < 6; r++)
+      for (int c = 0; c <= r; c++) *s_at(S, base + r, base + c) = h[idx++];   // lower triangle only
+    for (int r = 0; r < 6; r++) g_c[base + r] = b[r];
   }
 }
 
@@ -752,45 +739,140 @@ __global__ void cam_finish_kernel(int n_c_pad, const double* __restrict__ scale,
   }
 }
 
-// K7: S(hi,lo) -= sum over (a,b) pairs of Y_a W_b^T, one warp per block
-__global__ void __launch_bounds__(128) schur_kernel(int n_sb, const int* __restrict__ sb_hi, const int* __restrict__ sb_lo,
-                                                    const int* __restrict__ sb_ptr, const int* __restrict__ sp_a,
-                                                    const int* __restrict__ sp_b, const ObsWY* __restrict__ wy,
-                                                    const int* __restrict__ off_pose, SView S) {
-  const int b = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
-  if (b >= n_sb) return;
-  double acc[36];
+// K7: the Schur complement one hi keyframe k at a time (one CTA): S(k, lo) -= sum over (a, b) pairs of Y_a W_b^T for
+// every block of the row, and yb[k] = sum over k's observations of Y b_l.  All Y_a of a row belong to k's observations
+// (sp_a holds a's position in kf_obs[k]), so Y = W Hll^-1 is formed once per observation into shared memory and never
+// written to HBM; only W_b is gathered.  A row longer than `stage` observations recomputes Y of the rest where it is
+// used (same expression).  Summation orders: yb[k] by warp 0, lane-strided over kf_obs[k] then the xor tree; each
+// block as by one warp, lane L summing terms L, L+32, ... of the block's pair list, then the xor-16/8/4/2/1 tree.
+// A lane without a term holds +0.0 (never -0.0: 0.0 + t is +0.0 for t = -0.0), which adds nothing, so a tree level whose
+// partner lanes hold no term is skipped, and two blocks of at most 16 terms share a warp, one per half-warp (levels
+// 8/4/2/1 stay inside a half): the entries are bitwise those of the full 32-lane tree.  The lane holding a block's sum
+// parks its 36 entries in shared memory, and the warp's lanes then write one entry each.
+constexpr int ROW_THREADS = 128;
+constexpr int ROW_STAGE_MAX = 512;   // observations staged per row: 72 KB of shared memory, 3 CTAs per SM
+
+__device__ __forceinline__ void row_y(int i, int stage, const double2* __restrict__ ys, const int* __restrict__ kf_obs_k,
+                                      const int* __restrict__ obs_lm, const ObsW* __restrict__ ow,
+                                      const double* __restrict__ HllInv, double (&y)[18]) {
+  if (i < stage) {
+#pragma unroll
+    for (int j = 0; j < 9; j++) {
+      const double2 v = ys[9 * i + j];
+      y[2 * j] = v.x;
+      y[2 * j + 1] = v.y;
+    }
+  } else {
+    const int o = kf_obs_k[i];
+    obs_y(ow[o].W, HllInv + 6 * (size_t)obs_lm[o], y);
+  }
+}
+
+// acc += Y_a W_b^T over the pair terms p0, p0 + 32, ... < p1
+__device__ __forceinline__ void row_block_terms(int p0, int p1, int stage, const double2* __restrict__ ys,
+                                                const int* __restrict__ kf_obs_k, const int* __restrict__ obs_lm,
+                                                const ObsW* __restrict__ ow, const double* __restrict__ HllInv,
+                                                const int* __restrict__ sp_a, const int* __restrict__ sp_b, double (&acc)[36]) {
 #pragma unroll
   for (int i = 0; i < 36; i++) acc[i] = 0.0;
-  for (int p = sb_ptr[b] + lane; p < sb_ptr[b + 1]; p += 32) {
-    const double* Y = wy[sp_a[p]].Y;
-    const double* W = wy[sp_b[p]].W;
+  for (int p = p0; p < p1; p += 32) {
     double y[18], w[18];
+    row_y(sp_a[p], stage, ys, kf_obs_k, obs_lm, ow, HllInv, y);
+    const double2* W = reinterpret_cast<const double2*>(ow[sp_b[p]].W);
 #pragma unroll
-    for (int i = 0; i < 18; i++) { y[i] = Y[i]; w[i] = W[i]; }
+    for (int j = 0; j < 9; j++) {
+      const double2 v = W[j];
+      w[2 * j] = v.x;
+      w[2 * j + 1] = v.y;
+    }
 #pragma unroll
     for (int r = 0; r < 6; r++)
 #pragma unroll
       for (int c = 0; c < 6; c++) acc[6 * r + c] += y[3 * r] * w[3 * c] + y[3 * r + 1] * w[3 * c + 1] + y[3 * r + 2] * w[3 * c + 2];
   }
+}
+
+// the xor tree over the levels whose partner lanes can hold a term: n = the most terms of a block in the warp
+__device__ __forceinline__ void row_block_tree(int n, double (&acc)[36]) {
 #pragma unroll
   for (int off = 16; off > 0; off >>= 1)
+    if (n > off)
 #pragma unroll
-    for (int i = 0; i < 36; i++) acc[i] += __shfl_xor_sync(0xffffffffu, acc[i], off);
-  const int hi = sb_hi[b], lo = sb_lo[b];
-  // lanes 0..35 → not enough lanes; lane l writes entries l and l+32
-  for (int e = lane; e < 36; e += 32) {
-    const int r = e / 6, c = e % 6;
-    double v = 0.0;
+      for (int i = 0; i < 36; i++) acc[i] += __shfl_xor_sync(0xffffffffu, acc[i], off);
+}
+
+__global__ void __launch_bounds__(ROW_THREADS) schur_row_kernel(int stage, const int* __restrict__ kf_ptr,
+                                                                const int* __restrict__ kf_obs, const int* __restrict__ obs_lm,
+                                                                const double* __restrict__ HllInv, const double* __restrict__ bl,
+                                                                const ObsW* __restrict__ ow, const int* __restrict__ kf_sb,
+                                                                const int* __restrict__ sb_lo, const int* __restrict__ sb_ptr,
+                                                                const int* __restrict__ sp_a, const int* __restrict__ sp_b,
+                                                                const int* __restrict__ off_pose, SView S, double* __restrict__ yb) {
+  extern __shared__ double2 ys[];   // [min(n, stage)][9]: Y of the row's observations
+  const int k = blockIdx.x, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int* kf_obs_k = kf_obs + kf_ptr[k];
+  const int n = kf_ptr[k + 1] - kf_ptr[k];
+  for (int i = threadIdx.x; i < min(n, stage); i += ROW_THREADS) {
+    const int o = kf_obs_k[i];
+    double y[18];
+    obs_y(ow[o].W, HllInv + 6 * (size_t)obs_lm[o], y);
 #pragma unroll
-    for (int i = 0; i < 36; i++)
-      if (i == e) v = acc[i];
-    // the pose columns are laid out chain by chain, so a block of keyframes hi > lo may belong above the diagonal:
-    // store it transposed in the lower triangle then
-    const int br = off_pose[hi], bc = off_pose[lo];
-    if (hi == lo && c > r) continue;   // diagonal block: lower triangle only (the packed layout has no upper tiles)
-    if (br >= bc) *s_at(S, br + r, bc + c) -= v;
-    else *s_at(S, bc + c, br + r) -= v;
+    for (int j = 0; j < 9; j++) ys[9 * i + j] = make_double2(y[2 * j], y[2 * j + 1]);
+  }
+  __syncthreads();
+  const int br = off_pose[k];
+  if (warp == 0) {
+    double v[6];
+#pragma unroll
+    for (int r = 0; r < 6; r++) v[r] = 0.0;
+    for (int i = lane; i < n; i += 32) {
+      double y[18];
+      row_y(i, stage, ys, kf_obs_k, obs_lm, ow, HllInv, y);
+      const double* bb = bl + 3 * (size_t)obs_lm[kf_obs_k[i]];
+#pragma unroll
+      for (int r = 0; r < 6; r++) v[r] += y[3 * r] * bb[0] + y[3 * r + 1] * bb[1] + y[3 * r + 2] * bb[2];
+    }
+#pragma unroll
+    for (int off = 16; off > 0; off >>= 1)
+#pragma unroll
+      for (int r = 0; r < 6; r++) v[r] += __shfl_xor_sync(0xffffffffu, v[r], off);
+    if (lane == 0)
+      for (int r = 0; r < 6; r++) yb[br + r] = v[r];
+  }
+  // two blocks per warp visit: both in one pass (a half-warp each) when both have at most 16 terms, else one after the other
+  __shared__ double red_s[ROW_THREADS / 32][72];
+  double* red = red_s[warp];
+  for (int b = kf_sb[k] + 2 * warp; b < kf_sb[k + 1]; b += 2 * (ROW_THREADS / 32)) {
+    const int nb = min(2, kf_sb[k + 1] - b);
+    const int n0 = sb_ptr[b + 1] - sb_ptr[b], n1 = nb == 2 ? sb_ptr[b + 2] - sb_ptr[b + 1] : 0;
+    double acc[36];
+    if (nb == 2 && n0 <= 16 && n1 <= 16) {
+      const int h = lane >> 4;
+      row_block_terms(sb_ptr[b + h] + (lane & 15), sb_ptr[b + h + 1], stage, ys, kf_obs_k, obs_lm, ow, HllInv, sp_a, sp_b, acc);
+      row_block_tree(max(n0, n1), acc);
+      if ((lane & 15) == 0)
+#pragma unroll
+        for (int i = 0; i < 36; i++) red[36 * h + i] = acc[i];
+    } else {
+      for (int j = 0; j < nb; j++) {
+        row_block_terms(sb_ptr[b + j] + lane, sb_ptr[b + j + 1], stage, ys, kf_obs_k, obs_lm, ow, HllInv, sp_a, sp_b, acc);
+        row_block_tree(j ? n1 : n0, acc);
+        if (lane == 0)
+#pragma unroll
+          for (int i = 0; i < 36; i++) red[36 * j + i] = acc[i];
+      }
+    }
+    __syncwarp();
+    for (int e = lane; e < 36 * nb; e += 32) {
+      const int j = e >= 36, r = (e - 36 * j) / 6, c = (e - 36 * j) % 6, lo = sb_lo[b + j];
+      // the pose columns are laid out chain by chain, so a block of keyframes k > lo may belong above the diagonal:
+      // store it transposed in the lower triangle then
+      const int bc = off_pose[lo];
+      if (k == lo && c > r) continue;   // diagonal block: lower triangle only (the packed layout has no upper tiles)
+      if (br >= bc) *s_at(S, br + r, bc + c) -= red[e];
+      else *s_at(S, bc + c, br + r) -= red[e];
+    }
+    __syncwarp();
   }
 }
 
@@ -804,6 +886,12 @@ __global__ void __launch_bounds__(256) pack_tiles_kernel(double* __restrict__ St
     if (unpack) t[u] = b[u];
     else b[u] = t[u];
   }
+}
+
+// zero the listed tiles of S (one CTA per tile)
+__global__ void __launch_bounds__(256) zero_tiles_kernel(double* __restrict__ St, const int* __restrict__ tid) {
+  double2* t = reinterpret_cast<double2*>(St + ((size_t)tid[blockIdx.x] << 14));
+  for (int u = threadIdx.x; u < cvb_chol::T * cvb_chol::T / 2; u += blockDim.x) t[u] = make_double2(0.0, 0.0);
 }
 
 // Reduce-scatter by pull (peer access): the owner of a tile column adds the peers' partial tiles — read straight out of
@@ -827,13 +915,13 @@ __global__ void flag_to_double_kernel(const int* __restrict__ flag, double* __re
 
 // landmark back-substitution: x_l = Hll^-1 (b_l - sum W^T x_c)
 __global__ void backsub_kernel(int L, const int* __restrict__ lm_ptr, const int* __restrict__ obs_kf,
-                               const ObsWY* __restrict__ wy, const double* __restrict__ HllInv, const double* __restrict__ bl,
+                               const ObsW* __restrict__ ow, const double* __restrict__ HllInv, const double* __restrict__ bl,
                                const double* __restrict__ xc, const int* __restrict__ off_pose, double* __restrict__ xl) {
   const int l = blockIdx.x * blockDim.x + threadIdx.x;
   if (l >= L) return;
   double t[3] = {bl[3 * (size_t)l], bl[3 * (size_t)l + 1], bl[3 * (size_t)l + 2]};
   for (int o = lm_ptr[l]; o < lm_ptr[l + 1]; o++) {
-    const double* W = wy[o].W;
+    const double* W = ow[o].W;
     const double* x = xc + off_pose[obs_kf[o]];
 #pragma unroll
     for (int a = 0; a < 6; a++) {
@@ -1123,15 +1211,24 @@ __global__ void pair_heads_kernel(long long np, const unsigned long long* __rest
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i < np) head[i] = (i == 0 || keys[i] != keys[i - 1]) ? 1 : 0;
 }
+// position of every observation in its keyframe's kf_obs list
+__global__ void kf_pos_kernel(int n_obs, const int* __restrict__ kf_ptr, const int* __restrict__ kf_obs,
+                              const int* __restrict__ obs_kf, int* __restrict__ pos) {
+  const int e = blockIdx.x * blockDim.x + threadIdx.x;
+  if (e >= n_obs) return;
+  const int o = kf_obs[e];
+  pos[o] = e - kf_ptr[obs_kf[o]];
+}
+// sp_a: a's position in kf_obs[hi] (schur_row_kernel finds Y_a there); sp_b: the observation b
 __global__ void pair_scatter_kernel(long long np, const unsigned long long* __restrict__ keys,
                                     const unsigned long long* __restrict__ vals, const int* __restrict__ head,
-                                    const int* __restrict__ blk /*exclusive scan of head*/, int* __restrict__ sb_hi,
-                                    int* __restrict__ sb_lo, int* __restrict__ sb_ptr, int* __restrict__ sp_a,
-                                    int* __restrict__ sp_b) {
+                                    const int* __restrict__ blk /*exclusive scan of head*/, const int* __restrict__ kf_pos,
+                                    int* __restrict__ sb_hi, int* __restrict__ sb_lo, int* __restrict__ sb_ptr,
+                                    int* __restrict__ sp_a, int* __restrict__ sp_b) {
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= np) return;
   const unsigned long long v = vals[i];
-  sp_a[i] = (int)(v >> 32);
+  sp_a[i] = kf_pos[v >> 32];
   sp_b[i] = (int)(v & 0xffffffffu);
   if (head[i]) {
     const int bidx = blk[i];
@@ -1139,6 +1236,18 @@ __global__ void pair_scatter_kernel(long long np, const unsigned long long* __re
     sb_lo[bidx] = (int)(keys[i] & 0xffffffffu);
     sb_ptr[bidx] = (int)i;
   }
+}
+// kf_sb[k] = first block whose hi keyframe is >= k (blocks are sorted by hi), k = 0..K
+__global__ void kf_sb_kernel(int K, int n_sb, const int* __restrict__ sb_hi, int* __restrict__ kf_sb) {
+  const int k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k > K) return;
+  int lo = 0, hi = n_sb;
+  while (lo < hi) {
+    const int mid = (lo + hi) >> 1;
+    if (sb_hi[mid] < k) lo = mid + 1;
+    else hi = mid;
+  }
+  kf_sb[k] = lo;
 }
 
 int build_schur_lists(Engine& E, const std::vector<int>& h_lm_ptr, int K) {
@@ -1150,7 +1259,8 @@ int build_schur_lists(Engine& E, const std::vector<int>& h_lm_ptr, int K) {
   const long long np = h_pair_ptr[E.L_in];
   if (np >= (1LL << 31)) return cvb_fail(E.ctx, CVB_ERR_UNSUPPORTED, "more than 2^31 Schur observation pairs");
   int rc;
-  if ((rc = zalloc(E, E.sp_a, (size_t)np)) || (rc = zalloc(E, E.sp_b, (size_t)np))) return rc;
+  if ((rc = zalloc(E, E.sp_a, (size_t)np)) || (rc = zalloc(E, E.sp_b, (size_t)np)) || (rc = zalloc(E, E.kf_sb, (size_t)K + 1)))
+    return rc;
   E.n_sb = 0;
   if (np == 0) {
     if ((rc = zalloc(E, E.sb_hi, 0)) || (rc = zalloc(E, E.sb_lo, 0)) || (rc = zalloc(E, E.sb_ptr, 1))) return rc;
@@ -1158,12 +1268,14 @@ int build_schur_lists(Engine& E, const std::vector<int>& h_lm_ptr, int K) {
   }
   DevArr<long long> d_pair_ptr;
   DevArr<unsigned long long> k0, k1, v0, v1;
-  DevArr<int> head, blk;
+  DevArr<int> head, blk, kf_pos;
   DevArr<unsigned char> tmp;
   if ((rc = upload(E, d_pair_ptr, h_pair_ptr))) return rc;
   if (k0.alloc((size_t)np) || k1.alloc((size_t)np) || v0.alloc((size_t)np) || v1.alloc((size_t)np) || head.alloc((size_t)np + 1) ||
-      blk.alloc((size_t)np + 1))
+      blk.alloc((size_t)np + 1) || kf_pos.alloc((size_t)E.n_obs))
     return cvb_fail(E.ctx, CVB_ERR_CUDA, "cudaMalloc failed (Schur pair scratch, %lld pairs)", np);
+  kf_pos_kernel<<<grid1((size_t)E.n_obs), 256, 0, E.st>>>(E.n_obs, E.kf_ptr.p, E.kf_obs.p, E.obs_kf.p, kf_pos.p);
+  ENG_LAUNCH();
   gen_pairs_kernel<<<grid1((size_t)E.L_in), 256, 0, E.st>>>(E.L_in, E.lm_ptr.p, d_pair_ptr.p, E.obs_kf.p, k0.p, v0.p);
   ENG_LAUNCH();
   int bits = 1;
@@ -1186,13 +1298,15 @@ int build_schur_lists(Engine& E, const std::vector<int>& h_lm_ptr, int K) {
   E.n_sb = n_sb;
   if ((rc = zalloc(E, E.sb_hi, (size_t)n_sb)) || (rc = zalloc(E, E.sb_lo, (size_t)n_sb)) || (rc = zalloc(E, E.sb_ptr, (size_t)n_sb + 1)))
     return rc;
-  pair_scatter_kernel<<<grid1((size_t)np), 256, 0, E.st>>>(np, k0.p, v0.p, head.p, blk.p, E.sb_hi.p, E.sb_lo.p, E.sb_ptr.p, E.sp_a.p,
-                                                          E.sp_b.p);
+  pair_scatter_kernel<<<grid1((size_t)np), 256, 0, E.st>>>(np, k0.p, v0.p, head.p, blk.p, kf_pos.p, E.sb_hi.p, E.sb_lo.p,
+                                                          E.sb_ptr.p, E.sp_a.p, E.sp_b.p);
+  ENG_LAUNCH();
+  kf_sb_kernel<<<grid1((size_t)K + 1), 256, 0, E.st>>>(K, n_sb, E.sb_hi.p, E.kf_sb.p);
   ENG_LAUNCH();
   const int np_i = (int)np;
   ENG_CUDA(cudaMemcpyAsync(E.sb_ptr.p + n_sb, &np_i, sizeof(int), cudaMemcpyHostToDevice, E.st));
   ENG_CUDA(cudaStreamSynchronize(E.st));   // scratch arrays are freed on return
-  d_pair_ptr.free_(); k0.free_(); k1.free_(); v0.free_(); v1.free_(); head.free_(); blk.free_(); tmp.free_();
+  d_pair_ptr.free_(); k0.free_(); k1.free_(); v0.free_(); v1.free_(); head.free_(); blk.free_(); kf_pos.free_(); tmp.free_();
   return CVB_OK;
 }
 
@@ -1436,6 +1550,14 @@ int engine_setup(Engine& E, const cvb_ba_problem* p, const cvb_ba_options* o) {
       }
   E.n_xt_all = (int)h_xt_all.size();
   E.n_xt_own = (int)h_xt_own.size();
+  std::vector<int> h_xt_fill;
+  for (int j = 0; j < nt; j++)
+    for (int i = j; i < nt; i++)
+      if (!(pre_fill[(size_t)i * nt + j] || i == j) && E.plan.h_tile_of[(size_t)i * nt + j] >= 0)
+        h_xt_fill.push_back(E.plan.h_tile_of[(size_t)i * nt + j]);
+  E.n_xt_fill = (int)h_xt_fill.size();
+  if ((size_t)E.n_xt_all + E.n_xt_fill != E.n_tiles)
+    return cvb_fail(E.ctx, CVB_ERR_CUDA, "tile lists (%d + %d) do not cover S (%zu tiles)", E.n_xt_all, E.n_xt_fill, E.n_tiles);
   lap("tile structure + plan");
   // ---- by-keyframe CSR ----
   std::vector<int> h_kf_ptr(K + 1, 0), h_kf_obs(E.n_obs);
@@ -1444,6 +1566,14 @@ int engine_setup(Engine& E, const cvb_ba_problem* p, const cvb_ba_options* o) {
   {
     std::vector<int> fill(h_kf_ptr.begin(), h_kf_ptr.end() - 1);
     for (int ob = 0; ob < E.n_obs; ob++) h_kf_obs[fill[h_obs_kf[ob]]++] = ob;
+  }
+  E.row_stage = 0;
+  for (int k = 0; k < K; k++) E.row_stage = std::max(E.row_stage, std::min(h_kf_ptr[k + 1] - h_kf_ptr[k], ROW_STAGE_MAX));
+  {   // the attribute is shared by every engine on the device (ranks of a group among them): the largest stage any may use
+    static cvb_once_per_device once;
+    std::lock_guard<std::mutex> once_lk(once.mtx);
+    if (once.first(E.ctx->device))
+      ENG_CUDA(cudaFuncSetAttribute(schur_row_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, ROW_STAGE_MAX * 18 * (int)sizeof(double)));
   }
   lap("by-keyframe CSR");
   // ---- Schur (block → pair) lists: built on the device after the observation arrays are uploaded (build_schur_lists) ----
@@ -1531,7 +1661,7 @@ int engine_setup(Engine& E, const cvb_ba_problem* p, const cvb_ba_options* o) {
       (rc = upload(E, E.kf_ptr, h_kf_ptr)) || (rc = upload(E, E.kf_obs, h_kf_obs)) || (rc = upload(E, E.obs_uv, h_uv)) ||
       (rc = upload(E, E.obs_sigma, h_sigma)))
     return rc;
-  if ((rc = zalloc(E, E.lin, (size_t)E.n_obs)) || (rc = zalloc(E, E.wy, (size_t)E.n_obs))) return rc;
+  if ((rc = zalloc(E, E.lin, (size_t)E.n_obs)) || (rc = zalloc(E, E.ow, (size_t)E.n_obs))) return rc;
   if ((rc = zalloc(E, E.Hll, (size_t)6 * E.L_in)) || (rc = zalloc(E, E.HllInv, (size_t)6 * E.L_in)) ||
       (rc = zalloc(E, E.bl, (size_t)3 * E.L_in)))
     return rc;
@@ -1607,8 +1737,9 @@ int engine_setup(Engine& E, const cvb_ba_problem* p, const cvb_ba_options* o) {
   if ((rc = upload(E, E.scale0, h_scale)) || (rc = zalloc(E, E.scale, (size_t)E.n_vec))) return rc;
   if ((rc = upload(E, E.off_pose, E.h_off_pose)) || (rc = upload(E, E.off_sb, E.h_off_sb))) return rc;
   if ((rc = E.plan.upload(E.ctx, E.st))) return rc;
+  if ((rc = upload(E, E.xt_all, h_xt_all)) || (rc = upload(E, E.xt_fill, h_xt_fill))) return rc;
   if (E.world > 1) {
-    if ((rc = upload(E, E.xt_all, h_xt_all)) || (rc = upload(E, E.xt_own, h_xt_own)) || (rc = upload(E, E.col_owner, h_owner))) return rc;
+    if ((rc = upload(E, E.xt_own, h_xt_own)) || (rc = upload(E, E.col_owner, h_owner))) return rc;
     if ((rc = zalloc(E, E.flagd, 2))) return rc;
   }
   DevArr<double>* vecs[] = {&E.colsq, &E.diag, &E.gvec, &E.grad, &E.sgrad, &E.gn, &E.step, &E.xsol, &E.yb, &E.gs, &E.tmp};
@@ -1633,6 +1764,9 @@ int engine_setup(Engine& E, const cvb_ba_problem* p, const cvb_ba_options* o) {
     return rc;
   ENG_CUDA(cudaMallocHost(&E.h_scalars, RED_SLOTS * sizeof(double)));
   for (auto& e : E.ev) ENG_CUDA(cudaEventCreate(&e));
+  ENG_CUDA(cudaStreamCreateWithFlags(&E.st_fill, cudaStreamNonBlocking));
+  ENG_CUDA(cudaEventCreateWithFlags(&E.ev_fill_fork, cudaEventDisableTiming));
+  ENG_CUDA(cudaEventCreateWithFlags(&E.ev_fill_done, cudaEventDisableTiming));
   if ((rc = E.fs.create(E.ctx, E.plan.nt))) return rc;
   ENG_CUDA(cudaStreamSynchronize(E.st));
   lap("vectors, S, streams (sync)");
@@ -1644,7 +1778,7 @@ int evaluate(Engine& E, int b, int mode, double* cost_out) {
   const int rg = RED_BLOCKS;
   lin_obs_kernel<<<rg, 256, 0, E.st>>>(E.n_obs, E.obs_kf.p, E.obs_lm.p, E.obs_uv.p, E.obs_sigma.p, E.pose[b].p, E.lm[b].p,
                                        E.extr_kf.p, E.intr_kf.p, E.dist_kf.p, E.model_kf.p, E.xi_kf.p, E.scale.p, E.off_pose.p, E.n_c_pad, E.a2_reproj, mode,
-                                       E.lin.p, E.wy.p, nullptr, E.partials.p, 0);
+                                       E.lin.p, E.ow.p, nullptr, E.partials.p, 0);
   ENG_LAUNCH();
   lin_imu_kernel<<<rg, 256, 0, E.st>>>(E.n_imu, E.imu_i.p, E.imu_j.p, E.pre.p, E.pose[b].p, E.sb[b].p, E.scale.p, E.off_pose.p, E.off_sb.p, E.g,
                                        mode, E.Jimu.p, E.rimu.p, E.partials.p, 1);
@@ -1687,10 +1821,23 @@ int ar(Engine& E, double* p, size_t n) {
 int cam_blocks(Engine& E) {
   const size_t ld = (size_t)E.n_c_pad;
   const SView Sv{E.S.p, E.plan.d_tile_of, E.plan.nt};
-  ENG_CUDA(cudaMemsetAsync(E.S.p, 0, E.n_tiles * cvb_chol::T * cvb_chol::T * sizeof(double), E.st));
+  // S's own tiles (the ones the block kernels below add into) are cleared first on the engine stream; the fill tiles,
+  // which only the factorisation writes, on st_fill beside the block kernels (factor_rcs waits for them)
+  if (E.n_xt_fill > 0) {
+    ENG_CUDA(cudaEventRecord(E.ev_fill_fork, E.st));
+    ENG_CUDA(cudaStreamWaitEvent(E.st_fill, E.ev_fill_fork, 0));
+    zero_tiles_kernel<<<E.n_xt_fill, 256, 0, E.st_fill>>>(E.S.p, E.xt_fill.p);
+    ENG_LAUNCH();
+    ENG_CUDA(cudaEventRecord(E.ev_fill_done, E.st_fill));
+    E.fill_pending = true;
+  }
+  if (E.n_xt_all > 0) {
+    zero_tiles_kernel<<<E.n_xt_all, 256, 0, E.st>>>(E.S.p, E.xt_all.p);
+    ENG_LAUNCH();
+  }
   ENG_CUDA(cudaMemsetAsync(E.gvec.p, 0, ld * sizeof(double), E.st));
-  kf_visual_kernel<<<grid1((size_t)E.K * 32, 128), 128, 0, E.st>>>(E.K, E.kf_ptr.p, E.kf_obs.p, E.obs_lm.p, E.lin.p, E.wy.p,
-                                                                  E.bl.p, E.off_pose.p, Sv, E.gvec.p, E.yb.p, 0);
+  kf_visual_kernel<<<grid1((size_t)E.K * 32, 128), 128, 0, E.st>>>(E.K, E.kf_ptr.p, E.kf_obs.p, E.lin.p, E.off_pose.p, Sv,
+                                                                  E.gvec.p);
   ENG_LAUNCH();
   if (E.n_fb > 0) {
     factor_gather_kernel<<<E.n_fb, 256, 0, E.st>>>(E.n_fb, E.fb_hi.p, E.fb_lo.p, E.fb_ptr.p, E.ft_type.p, E.ft_fac.p,
@@ -1716,20 +1863,12 @@ int factor_rcs(Engine& E, double mu, bool* ok) {
   if (E.L_in > 0) {
     lm_damp_inv_kernel<<<grid1(E.L_in), 256, 0, E.st>>>(E.L_in, E.Hll.p, E.colsq.p + E.n_c_pad, mu, E.HllInv.p);
     ENG_LAUNCH();
-    if (E.n_obs > 0) {
-      obs_Y_kernel<<<grid1(E.n_obs), 256, 0, E.st>>>(E.n_obs, E.obs_lm.p, E.HllInv.p, E.wy.p);
-      ENG_LAUNCH();
-    }
   }
   ENG_CUDA(cudaMemsetAsync(E.yb.p, 0, ld * sizeof(double), E.st));
-  kf_visual_kernel<<<grid1((size_t)E.K * 32, 128), 128, 0, E.st>>>(E.K, E.kf_ptr.p, E.kf_obs.p, E.obs_lm.p, E.lin.p, E.wy.p,
-                                                                  E.bl.p, E.off_pose.p, Sv, E.gvec.p, E.yb.p, 1);
+  schur_row_kernel<<<E.K, ROW_THREADS, (size_t)E.row_stage * 18 * sizeof(double), E.st>>>(
+      E.row_stage, E.kf_ptr.p, E.kf_obs.p, E.obs_lm.p, E.HllInv.p, E.bl.p, E.ow.p, E.kf_sb.p, E.sb_lo.p, E.sb_ptr.p, E.sp_a.p,
+      E.sp_b.p, E.off_pose.p, Sv, E.yb.p);
   ENG_LAUNCH();
-  if (E.n_sb > 0) {
-    schur_kernel<<<grid1((size_t)E.n_sb * 32, 128), 128, 0, E.st>>>(E.n_sb, E.sb_hi.p, E.sb_lo.p, E.sb_ptr.p, E.sp_a.p,
-                                                                   E.sp_b.p, E.wy.p, E.off_pose.p, Sv);
-    ENG_LAUNCH();
-  }
   // the one exchange of the data path: sum the rank-partial reduced normal equations over NVLink
   int rc = CVB_OK;
   if (E.allreduce && E.world > 1 && !dist) {
@@ -1750,6 +1889,10 @@ int factor_rcs(Engine& E, double mu, bool* ok) {
   cam_finish_kernel<<<grid1(E.n_c_pad), 256, 0, E.st>>>(E.n_c_pad, E.scale.p, Sv, E.diag.p, E.gvec.p, E.yb.p, E.gs.p, mu,
                                                         dist ? E.col_owner.p : nullptr, E.rank);
   ENG_LAUNCH();
+  if (E.fill_pending) {
+    ENG_CUDA(cudaStreamWaitEvent(E.st, E.ev_fill_done, 0));
+    E.fill_pending = false;
+  }
   tick(E, 1);
   // first call: plain launches (sets kernel attributes); second call: stream-capture into a graph; then replay
   if (E.g_factor) {
@@ -1896,7 +2039,7 @@ int prepare_step(Engine& E, bool* solver_ok, bool* grad_converged) {
     }
     E.n_solve_calls++;
     if (E.L_in > 0) {
-      backsub_kernel<<<grid1(E.L_in), 256, 0, E.st>>>(E.L_in, E.lm_ptr.p, E.obs_kf.p, E.wy.p, E.HllInv.p, E.bl.p, E.xsol.p, E.off_pose.p,
+      backsub_kernel<<<grid1(E.L_in), 256, 0, E.st>>>(E.L_in, E.lm_ptr.p, E.obs_kf.p, E.ow.p, E.HllInv.p, E.bl.p, E.xsol.p, E.off_pose.p,
                                                       E.xsol.p + E.n_c_pad);
       ENG_LAUNCH();
     }
@@ -2052,7 +2195,7 @@ int engine_corrected_norms(Engine& E, double* h_norms_full, int n_obs_full) {
   if (d.alloc((size_t)E.n_obs)) return cvb_fail(E.ctx, CVB_ERR_CUDA, "cudaMalloc failed");
   lin_obs_kernel<<<RED_BLOCKS, 256, 0, E.st>>>(E.n_obs, E.obs_kf.p, E.obs_lm.p, E.obs_uv.p, E.obs_sigma.p, E.pose[E.cur].p,
                                                E.lm[E.cur].p, E.extr_kf.p, E.intr_kf.p, E.dist_kf.p, E.model_kf.p, E.xi_kf.p, E.scale.p, E.off_pose.p, E.n_c_pad,
-                                               E.a2_reproj, 2, E.lin.p, E.wy.p, d.p, E.partials.p, 0);
+                                               E.a2_reproj, 2, E.lin.p, E.ow.p, d.p, E.partials.p, 0);
   ENG_LAUNCH();
   std::vector<double> h(E.n_obs);
   ENG_CUDA(cudaMemcpyAsync(h.data(), d.p, sizeof(double) * E.n_obs, cudaMemcpyDeviceToHost, E.st));
