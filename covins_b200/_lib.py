@@ -108,6 +108,16 @@ SIGNATURES = {
     "cvb_group_allreduce_diag": (C.c_int, [c_vp, c_vp, C.c_size_t, c_vp]),
     "cvb_ba_solve_group": (C.c_int, [c_vp, c_vp, c_vp, C.c_int, c_vp]),
     "cvb_gba_group": (C.c_int, [c_vp, c_vp, c_vp, C.c_int, c_vp, c_vp]),
+    "cvb_db_group_create": (C.c_int, [c_vp, C.c_int, C.POINTER(c_vp)]),
+    "cvb_db_group_destroy": (C.c_int, [c_vp]),
+    "cvb_db_group_append": (C.c_int, [c_vp, c_vp, c_vp, C.c_int]),
+    "cvb_db_group_append_sift": (C.c_int, [c_vp, c_vp, c_vp, C.c_int]),
+    "cvb_db_group_remove": (C.c_int, [c_vp, C.c_int]),
+    "cvb_db_group_size": (C.c_int, [c_vp, C.POINTER(C.c_int32), C.POINTER(C.c_int64), c_vp]),
+    "cvb_db_group_match_hamming": (C.c_int, [c_vp, c_vp, C.c_int, C.c_float, C.c_float, c_vp, c_vp, c_vp, c_vp, c_vp, C.c_int,
+                                             C.POINTER(C.c_int32)]),
+    "cvb_db_group_match_l2": (C.c_int, [c_vp, c_vp, C.c_int, C.c_float, C.c_float, c_vp, c_vp, c_vp, c_vp, c_vp, C.c_int,
+                                        C.POINTER(C.c_int32)]),
     "cvb_covisibility": (C.c_int, [c_vp, C.c_int, C.c_int, c_vp, c_vp, c_vp, c_vp, C.c_int, c_vp, c_vp, c_vp, C.c_int64,
                                    C.POINTER(C.c_int64)]),
     "cvb_redundant_keyframes": (C.c_int, [c_vp, C.c_int, C.c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, C.c_double,

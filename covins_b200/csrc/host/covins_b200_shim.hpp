@@ -1680,53 +1680,75 @@ inline std::vector<NonCentralRelativePoseRansacResult> RansacCentralRelativePose
 // index of a keyframe is its insertion order; keep it next to the keyframe (e.g. std::map<idpair, int>).
 // A database constructed with the SiftDescriptors tag holds SIFT rows instead (feat.type SIFT, placerec_gen_be.cpp:86-87):
 // AddKeyframe / MatchAll then take CV_32F rows x 128, matched with the exact L2 2-NN of MatchCandidatesSIFT.
+// A database constructed over a ContextGroup spreads its keyframes over the group's GPUs (cvb_db_group_*): the same indices
+// and the same MatchAll results, each request scanning every GPU's share of the map on that GPU.  Give it a group of its
+// own (over the same devices if you like): its requests wait for any GlobalBundleAdjustment running on the same group.
 struct SiftDescriptors {};
 class DescriptorDatabase {
  public:
-  explicit DescriptorDatabase(Context& ctx) : ctx_(ctx) { ctx_.check(cvb_db_create(ctx_.get(), 32, &db_), "cvb_db_create"); }
-  DescriptorDatabase(Context& ctx, SiftDescriptors) : ctx_(ctx) { ctx_.check(cvb_db_create(ctx_.get(), 128, &db_), "cvb_db_create"); }
-  ~DescriptorDatabase() { if (db_) cvb_db_destroy(ctx_.get(), db_); }
+  explicit DescriptorDatabase(Context& ctx) : ctx_(&ctx) { ctx_->check(cvb_db_create(ctx_->get(), 32, &db_), "cvb_db_create"); }
+  DescriptorDatabase(Context& ctx, SiftDescriptors) : ctx_(&ctx) { ctx_->check(cvb_db_create(ctx_->get(), 128, &db_), "cvb_db_create"); }
+  explicit DescriptorDatabase(ContextGroup& group) : ctx_(&group.rank(0)) {
+    ctx_->check(cvb_db_group_create(group.get(), 32, &gdb_), "cvb_db_group_create");
+  }
+  DescriptorDatabase(ContextGroup& group, SiftDescriptors) : ctx_(&group.rank(0)) {
+    ctx_->check(cvb_db_group_create(group.get(), 128, &gdb_), "cvb_db_group_create");
+  }
+  ~DescriptorDatabase() {
+    if (db_) cvb_db_destroy(ctx_->get(), db_);
+    if (gdb_) cvb_db_group_destroy(gdb_);
+  }
   DescriptorDatabase(const DescriptorDatabase&) = delete;
   DescriptorDatabase& operator=(const DescriptorDatabase&) = delete;
   // descriptors: kf->descriptors_add_ (CV_8U, continuous, rows x 32; keyframe_be.cpp:103,137) → returns the database index
   int AddKeyframe(const uint8_t* descriptors, int rows) {
     const int32_t r = rows;
-    ctx_.check(cvb_db_append(ctx_.get(), db_, descriptors, &r, 1), "cvb_db_append");
+    if (gdb_) ctx_->check(cvb_db_group_append(gdb_, descriptors, &r, 1), "cvb_db_group_append");
+    else ctx_->check(cvb_db_append(ctx_->get(), db_, descriptors, &r, 1), "cvb_db_append");
     return n_kf_++;
   }
   // SIFT database: kf->descriptors_add_ as CV_32F, continuous, rows x 128, integer-valued in [0,255]
   int AddKeyframe(const float* descriptors, int rows) {
     const int32_t r = rows;
-    ctx_.check(cvb_db_append_sift(ctx_.get(), db_, descriptors, &r, 1), "cvb_db_append_sift");
+    if (gdb_) ctx_->check(cvb_db_group_append_sift(gdb_, descriptors, &r, 1), "cvb_db_group_append_sift");
+    else ctx_->check(cvb_db_append_sift(ctx_->get(), db_, descriptors, &r, 1), "cvb_db_append_sift");
     return n_kf_++;
   }
   int size() const { return n_kf_; }
   // the keyframe leaves the map (culling, keyframe_be.cpp:413-440 / Map::EraseKeyframe): later indices drop by one
   void RemoveKeyframe(int db_index) {
-    ctx_.check(cvb_db_remove(ctx_.get(), db_, db_index), "cvb_db_remove");
+    if (gdb_) ctx_->check(cvb_db_group_remove(gdb_, db_index), "cvb_db_group_remove");
+    else ctx_->check(cvb_db_remove(ctx_->get(), db_, db_index), "cvb_db_remove");
     n_kf_--;
   }
   // knnMatch(k=2) + distance/ratio filter of the query keyframe against EVERY keyframe of the database:
   // result[db index] == the reference's img_matches for that candidate (accepted queries ascending, :102-114)
   std::vector<Matches> MatchAll(const uint8_t* query, int n_query, const OptParams& P) {
-    return match_all(cvb_db_match_hamming, "cvb_db_match_hamming", query, n_query, P);
+    const float thr = P.img_match_thres, ratio = P.ratio_thres;
+    return match_all(gdb_ ? "cvb_db_group_match_hamming" : "cvb_db_match_hamming", [&](auto... out) {
+      return gdb_ ? cvb_db_group_match_hamming(gdb_, query, n_query, thr, ratio, out...)
+                  : cvb_db_match_hamming(ctx_->get(), db_, query, n_query, thr, ratio, out...);
+    });
   }
   // the same for a SIFT database: query = the query keyframe's CV_32F rows x 128
   std::vector<Matches> MatchAll(const float* query, int n_query, const OptParams& P) {
-    return match_all(cvb_db_match_l2, "cvb_db_match_l2", query, n_query, P);
+    const float thr = P.img_match_thres, ratio = P.ratio_thres;
+    return match_all(gdb_ ? "cvb_db_group_match_l2" : "cvb_db_match_l2", [&](auto... out) {
+      return gdb_ ? cvb_db_group_match_l2(gdb_, query, n_query, thr, ratio, out...)
+                  : cvb_db_match_l2(ctx_->get(), db_, query, n_query, thr, ratio, out...);
+    });
   }
 
  private:
-  template <class Fn, class Q>
-  std::vector<Matches> match_all(Fn fn, const char* name, const Q* query, int n_query, const OptParams& P) {
+  // fn(n_matches, m_kf, m_query, m_train, m_dist, cap, n_total): the request with the query bound
+  template <class Fn>
+  std::vector<Matches> match_all(const char* name, Fn fn) {
     std::vector<int32_t> nm(n_kf_ > 0 ? n_kf_ : 1);
     if (cap_ == 0) cap_ = 4096;
     for (;;) {
       m_kf_.resize(cap_); m_q_.resize(cap_); m_t_.resize(cap_); m_d_.resize(cap_);
       int32_t total = 0;
-      ctx_.check(fn(ctx_.get(), db_, query, n_query, P.img_match_thres, P.ratio_thres, nm.data(), m_kf_.data(), m_q_.data(),
-                    m_t_.data(), m_d_.data(), cap_, &total),
-                 name);
+      ctx_->check(fn(nm.data(), m_kf_.data(), m_q_.data(), m_t_.data(), m_d_.data(), cap_, &total), name);
       if (total <= cap_) {
         std::vector<Matches> out(n_kf_);
         for (int i = 0; i < total; i++) out[m_kf_[i]].push_back(Match{(size_t)m_q_[i], (size_t)m_t_[i], m_d_[i]});
@@ -1736,8 +1758,9 @@ class DescriptorDatabase {
     }
   }
 
-  Context& ctx_;
+  Context* ctx_;                  // the single database's context, or the group's rank 0 (its messages)
   cvb_db* db_ = nullptr;
+  cvb_db_group* gdb_ = nullptr;
   int n_kf_ = 0, cap_ = 0;
   std::vector<int32_t> m_kf_, m_q_, m_t_;
   std::vector<float> m_d_;

@@ -7,10 +7,16 @@
 // uploaded once (cvb_db_append / cvb_db_append_sift) and stay in HBM; a query moves nq*32 B (ORB) or nq*128 B (SIFT, u8)
 // up and the accepted matches down.  Both row kinds share the code below; they differ in the row size, the tensor-core
 // tile image (cvb_tc::tile_bytes / expand_tiles by metric) and the host staging of SIFT rows (checked and quantised to u8).
+//
+// cvb_db_group (end of file): the same database with its keyframes dealt over the ranks of a cvb_group, one ordinary cvb_db
+// per rank.  A request runs the per-rank 2-NN and compaction above on every rank's stream; a gather on rank 0 then reads
+// the ranks' counts and compacted lists (same device or peer access) and writes them in global keyframe order, so the
+// outputs are bit-identical to one cvb_db holding every keyframe.
 #include <string.h>
 
 #include <algorithm>
 
+#include "ba_group.cuh"
 #include "cvb_internal.cuh"
 #include "tc_match.cuh"
 
@@ -432,6 +438,376 @@ int cvb_db_match_l2(cvb_ctx* ctx, cvb_db* db, const float* q, int nq, float thr,
   CVB_GUARD(ctx);
   if (const int rc = require_kind(ctx, db, true, "cvb_db_match_l2")) return rc;
   return match_host(ctx, db, q, nq, thr, ratio, n_matches, m_kf, m_query, m_train, m_dist, cap, n_total, "cvb_db_match_l2");
+}
+
+}  // extern "C"
+
+// ---------------------------------------------------------------------------------------------------------------------
+// The database over a rank group
+// ---------------------------------------------------------------------------------------------------------------------
+struct cvb_db_group {
+  cvb_group* g = nullptr;
+  int desc_bytes = 32;
+  cvb_db* db[CVB_GROUP_MAX] = {};         // rank r's keyframes, in global order
+  int64_t rows[CVB_GROUP_MAX] = {};
+  std::vector<int2> loc;                  // global keyframe -> (rank, index in the rank's cvb_db)
+  bool loc_dirty = true;
+  cudaEvent_t done[CVB_GROUP_MAX] = {};   // rank r's part of a request is complete
+  // rank 0: the device copy of `loc` and the gather's buffers
+  cvb_buf d_loc, cnt, src, goff, o_kf, o_q, o_t, o_d;
+};
+
+namespace {
+
+// per rank: the request's per-keyframe counts, their exclusive offsets (db_offsets_kernel) and the compacted lists
+// (db_compact_kernel), in the rank's cvb_db scratch
+struct DbGatherSrc {
+  const int32_t* nm[CVB_GROUP_MAX];
+  const int32_t* off[CVB_GROUP_MAX];
+  const int32_t* q[CVB_GROUP_MAX];
+  const int32_t* t[CVB_GROUP_MAX];
+  const float* d[CVB_GROUP_MAX];
+};
+
+// The gather, part 1: every global keyframe's count and the start of its slice in its rank's list.  The counts are then
+// scanned in global keyframe order by db_offsets_kernel.  __grid_constant__: the pointer table is indexed in place in the
+// parameter bank (as group_sum_kernel's).
+__global__ void __launch_bounds__(256) db_group_counts_kernel(const __grid_constant__ DbGatherSrc s, const int2* __restrict__ loc,
+                                                               int n_kf, int32_t* __restrict__ cnt, int32_t* __restrict__ src) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n_kf) return;
+  const int2 rl = loc[i];
+  cnt[i] = s.nm[rl.x][rl.y];
+  src[i] = s.off[rl.x][rl.y];
+}
+
+// The gather, part 2: one warp per global keyframe copies its slice of its rank's list to its global position goff[kf],
+// m_kf rewritten to the global index.  As db_compact_kernel, a match is written iff its global position p < cap.  The ranks
+// compacted with the same cap, and nothing below cap is lost by that: a rank's earlier keyframes are a subset of the
+// globally earlier ones, in the same order, so a match's position in its rank's list is never larger than its global
+// position p (src[kf] + j <= goff[kf] + j < cap).
+__global__ void __launch_bounds__(256) db_group_gather_kernel(const __grid_constant__ DbGatherSrc s, const int2* __restrict__ loc,
+                                                               const int32_t* __restrict__ cnt, const int32_t* __restrict__ src,
+                                                               const int32_t* __restrict__ goff, int n_kf, int cap,
+                                                               int32_t* __restrict__ o_kf, int32_t* __restrict__ o_q,
+                                                               int32_t* __restrict__ o_t, float* __restrict__ o_d) {
+  const int kf = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  if (kf >= n_kf) return;
+  const int r = loc[kf].x, n = cnt[kf], p0 = goff[kf], s0 = src[kf];
+  for (int j = threadIdx.x & 31; j < n && p0 + j < cap; j += 32) {
+    const int p = p0 + j, ps = s0 + j;
+    o_kf[p] = kf;
+    o_q[p] = s.q[r][ps];
+    o_t[p] = s.t[r][ps];
+    o_d[p] = s.d[r][ps];
+  }
+}
+
+// a failure of rank r's work, reported on rank 0's context as the group drivers do
+int rank_fail(cvb_db_group* db, int r, int rc) {
+  const std::string m = db->g->ctx[r]->err;
+  return cvb_fail(db->g->ctx[0], rc, "rank %d: %s", r, m.c_str());
+}
+
+// no rank's stream still works on the request (the error path; the normal path ends in rank 0's synchronise, after the
+// gather that waited on every rank)
+void settle(cvb_db_group* db) {
+  for (int r = 0; r < db->g->n; r++) {
+    CVB_GUARD(db->g->ctx[r]);
+    cudaStreamSynchronize(db->g->ctx[r]->stream);
+  }
+}
+
+// Each keyframe to the rank holding the fewest rows at that moment (the lowest rank on a tie), one by one; rank r's
+// keyframes are appended to its cvb_db in their global order.  rows: u8, the database layout (host).
+int group_append(cvb_db_group* db, const uint8_t* rows, const int32_t* rows_per_kf, int n_kf) {
+  cvb_group* g = db->g;
+  const int n = g->n;
+  std::vector<int> dest((size_t)n_kf);
+  int64_t load[CVB_GROUP_MAX];
+  std::copy(db->rows, db->rows + n, load);
+  for (int i = 0; i < n_kf; i++) {
+    const int r = (int)(std::min_element(load, load + n) - load);
+    dest[i] = r;
+    load[r] += rows_per_kf[i];
+  }
+  std::vector<int64_t> first((size_t)n_kf + 1, 0);
+  for (int i = 0; i < n_kf; i++) first[i + 1] = first[i] + rows_per_kf[i];
+  int base[CVB_GROUP_MAX];
+  for (int r = 0; r < n; r++) {
+    base[r] = (int)db->db[r]->seg_ptr.size() - 1;
+    std::vector<uint8_t> buf;
+    std::vector<int32_t> cnt;
+    for (int i = 0; i < n_kf; i++)
+      if (dest[i] == r) {
+        buf.insert(buf.end(), rows + first[i] * db->desc_bytes, rows + first[i + 1] * db->desc_bytes);
+        cnt.push_back(rows_per_kf[i]);
+      }
+    if (cnt.empty()) continue;
+    CVB_GUARD(g->ctx[r]);
+    if (const int rc = append_rows(g->ctx[r], db->db[r], buf.data(), cnt.data(), (int)cnt.size(), (int64_t)buf.size() / db->desc_bytes))
+      return rank_fail(db, r, rc);
+    db->rows[r] = load[r];
+  }
+  for (int i = 0; i < n_kf; i++) db->loc.push_back(make_int2(dest[i], base[dest[i]]++));
+  db->loc_dirty = true;
+  return CVB_OK;
+}
+
+int group_append_checked(cvb_db_group* db, bool sift, const void* rows, const int32_t* rows_per_kf, int n_kf, const char* fn) {
+  cvb_ctx* c0 = db->g->ctx[0];
+  if (const int rc = require_kind(c0, db->db[0], sift, fn)) return rc;   // every rank's cvb_db holds the group's row kind
+  CVB_REQUIRE(c0, n_kf >= 0 && (n_kf == 0 || rows_per_kf), "%s: bad arguments", fn);
+  int64_t add = 0, have = 0;
+  for (int i = 0; i < n_kf; ++i) {
+    CVB_REQUIRE(c0, rows_per_kf[i] >= 0, "%s: negative row count", fn);
+    add += rows_per_kf[i];
+  }
+  for (int r = 0; r < db->g->n; r++) have += db->rows[r];
+  // the single database's limit, so that the group refuses what one cvb_db would refuse
+  CVB_REQUIRE(c0, have + add < (int64_t)1 << 31, "%s: more than 2^31 rows", fn);
+  CVB_REQUIRE(c0, add == 0 || rows, "%s: null rows", fn);
+  if (!sift) return group_append(db, (const uint8_t*)rows, rows_per_kf, n_kf);
+  std::vector<uint8_t> u8((size_t)add * 128);   // checked and quantised before any rank is touched
+  if (!cvb_quantize_sift((const float*)rows, u8.size(), u8.data()))
+    return cvb_fail(c0, CVB_ERR_UNSUPPORTED, "%s: SIFT descriptors must be integer-valued in [0,255] (cv::xfeatures2d::SIFT output)", fn);
+  return group_append(db, u8.data(), rows_per_kf, n_kf);
+}
+
+// rank r's part of a request, enqueued on its stream: the query from the pinned staging, the filtered 2-NN against its
+// keyframes, the scan of its counts and the compaction (at most cap), then its event
+int rank_request(cvb_ctx* ctx, cvb_db* d, const uint8_t* pin, size_t qb, int nq, float thr, float ratio, int cap, cudaEvent_t done) {
+  CVB_GUARD(ctx);
+  const int n_seg = (int)d->seg_ptr.size() - 1;
+  const size_t on = (size_t)n_seg * nq;
+  cudaStream_t st = ctx->stream;
+  int rc;
+  if ((rc = grow(ctx, d->q, qb)) || (rc = grow(ctx, d->mt, on * 4)) || (rc = grow(ctx, d->md, on * 4)) ||
+      (rc = grow(ctx, d->nm, (size_t)n_seg * 4)) || (rc = grow(ctx, d->off, (size_t)(n_seg + 1) * 4)))
+    return rc;
+  if (cap && ((rc = grow(ctx, d->out_seg, (size_t)cap * 4)) || (rc = grow(ctx, d->out_q, (size_t)cap * 4)) ||
+              (rc = grow(ctx, d->out_t, (size_t)cap * 4)) || (rc = grow(ctx, d->out_d, (size_t)cap * 4))))
+    return rc;
+  CVB_CUDA(ctx, cudaMemcpyAsync(d->q.p, pin, qb, cudaMemcpyHostToDevice, st));
+  if ((rc = match_dev(ctx, d, (const uint8_t*)d->q.p, nq, thr, ratio, (int32_t*)d->mt.p, (float*)d->md.p, (int32_t*)d->nm.p, nullptr)))
+    return rc;
+  db_offsets_kernel<<<1, 1024, 0, st>>>((const int32_t*)d->nm.p, n_seg, (int32_t*)d->off.p);
+  CVB_CHECK_LAUNCH(ctx);
+  if (cap) {
+    db_compact_kernel<<<(n_seg + 7) / 8, 256, 0, st>>>((const int32_t*)d->mt.p, (const float*)d->md.p, nq, n_seg, (const int32_t*)d->off.p,
+                                                       cap, (int32_t*)d->out_seg.p, (int32_t*)d->out_q.p, (int32_t*)d->out_t.p,
+                                                       (float*)d->out_d.p);
+    CVB_CHECK_LAUNCH(ctx);
+  }
+  CVB_CUDA(ctx, cudaEventRecord(done, st));
+  return CVB_OK;
+}
+
+// everything after the checks: *fail_rank = the rank whose work failed
+int group_request(cvb_db_group* db, const uint8_t* pin, size_t pin_q, int nq, float thr, float ratio, int32_t* n_matches,
+                  int32_t* m_kf, int32_t* m_query, int32_t* m_train, float* m_dist, int cap, int32_t* n_total, int* fail_rank) {
+  cvb_group* g = db->g;
+  cvb_ctx* c0 = g->ctx[0];
+  cudaStream_t st = c0->stream;
+  const int n_kf = (int)db->loc.size();
+  const size_t qb = (size_t)nq * db->desc_bytes;
+  int rc;
+  *fail_rank = 0;
+  // rank 0's buffers first: the table upload synchronises rank 0's stream, before any rank's work is enqueued
+  if ((rc = grow(c0, db->d_loc, (size_t)n_kf * sizeof(int2))) || (rc = grow(c0, db->cnt, (size_t)n_kf * 4)) ||
+      (rc = grow(c0, db->src, (size_t)n_kf * 4)) || (rc = grow(c0, db->goff, (size_t)(n_kf + 1) * 4)))
+    return rc;
+  if (cap && ((rc = grow(c0, db->o_kf, (size_t)cap * 4)) || (rc = grow(c0, db->o_q, (size_t)cap * 4)) ||
+              (rc = grow(c0, db->o_t, (size_t)cap * 4)) || (rc = grow(c0, db->o_d, (size_t)cap * 4))))
+    return rc;
+  if (db->loc_dirty) {
+    CVB_CUDA(c0, cudaMemcpyAsync(db->d_loc.p, db->loc.data(), (size_t)n_kf * sizeof(int2), cudaMemcpyHostToDevice, st));
+    CVB_CUDA(c0, cudaStreamSynchronize(st));
+    db->loc_dirty = false;
+  }
+  DbGatherSrc s{};
+  bool ran[CVB_GROUP_MAX] = {};
+  for (int r = 0; r < g->n; r++) {
+    cvb_db* d = db->db[r];
+    if (d->seg_ptr.size() == 1) continue;   // a rank without keyframes has no part in the request
+    if ((rc = rank_request(g->ctx[r], d, pin, qb, nq, thr, ratio, cap, db->done[r]))) {
+      *fail_rank = r;
+      return rc;
+    }
+    s.nm[r] = (const int32_t*)d->nm.p;
+    s.off[r] = (const int32_t*)d->off.p;
+    s.q[r] = (const int32_t*)d->out_q.p;
+    s.t[r] = (const int32_t*)d->out_t.p;
+    s.d[r] = (const float*)d->out_d.p;
+    ran[r] = true;
+  }
+  for (int r = 1; r < g->n; r++)
+    if (ran[r]) CVB_CUDA(c0, cudaStreamWaitEvent(st, db->done[r], 0));
+  const int2* loc = (const int2*)db->d_loc.p;
+  int32_t *cnt = (int32_t*)db->cnt.p, *src = (int32_t*)db->src.p, *goff = (int32_t*)db->goff.p;
+  db_group_counts_kernel<<<(n_kf + 255) / 256, 256, 0, st>>>(s, loc, n_kf, cnt, src);
+  CVB_CHECK_LAUNCH(c0);
+  db_offsets_kernel<<<1, 1024, 0, st>>>(cnt, n_kf, goff);
+  CVB_CHECK_LAUNCH(c0);
+  if (cap) {
+    db_group_gather_kernel<<<(n_kf + 7) / 8, 256, 0, st>>>(s, loc, cnt, src, goff, n_kf, cap, (int32_t*)db->o_kf.p,
+                                                           (int32_t*)db->o_q.p, (int32_t*)db->o_t.p, (float*)db->o_d.p);
+    CVB_CHECK_LAUNCH(c0);
+  }
+  int32_t* pin_cnt = (int32_t*)(pin + pin_q);
+  int32_t* pin_tot = pin_cnt + n_kf;
+  CVB_CUDA(c0, cudaMemcpyAsync(pin_cnt, cnt, (size_t)n_kf * 4, cudaMemcpyDeviceToHost, st));
+  CVB_CUDA(c0, cudaMemcpyAsync(pin_tot, goff + n_kf, 4, cudaMemcpyDeviceToHost, st));
+  CVB_CUDA(c0, cudaStreamSynchronize(st));
+  const int total = *pin_tot;
+  *n_total = total;
+  if (n_matches) memcpy(n_matches, pin_cnt, (size_t)n_kf * 4);
+  const int n_out = std::min(total, cap);
+  if (n_out) {
+    CVB_CUDA(c0, cudaMemcpyAsync(m_kf, db->o_kf.p, (size_t)n_out * 4, cudaMemcpyDeviceToHost, st));
+    CVB_CUDA(c0, cudaMemcpyAsync(m_query, db->o_q.p, (size_t)n_out * 4, cudaMemcpyDeviceToHost, st));
+    CVB_CUDA(c0, cudaMemcpyAsync(m_train, db->o_t.p, (size_t)n_out * 4, cudaMemcpyDeviceToHost, st));
+    CVB_CUDA(c0, cudaMemcpyAsync(m_dist, db->o_d.p, (size_t)n_out * 4, cudaMemcpyDeviceToHost, st));
+    CVB_CUDA(c0, cudaStreamSynchronize(st));
+  }
+  return CVB_OK;
+}
+
+int group_match(cvb_db_group* db, bool sift, const void* q, int nq, float thr, float ratio, int32_t* n_matches, int32_t* m_kf,
+                int32_t* m_query, int32_t* m_train, float* m_dist, int cap, int32_t* n_total, const char* fn) {
+  cvb_ctx* c0 = db->g->ctx[0];
+  if (const int rc = require_kind(c0, db->db[0], sift, fn)) return rc;
+  const int n_kf = (int)db->loc.size();
+  CVB_REQUIRE(c0, nq >= 0 && cap >= 0 && n_total && (nq == 0 || q), "%s: bad arguments", fn);
+  CVB_REQUIRE(c0, cap == 0 || (m_kf && m_query && m_train && m_dist), "%s: null outputs", fn);
+  *n_total = 0;
+  // pinned staging on rank 0's context: [query | counts | total]; every rank copies the query from it
+  const size_t qb = (size_t)nq * db->desc_bytes, pin_q = (qb + 255) & ~(size_t)255;
+  uint8_t* pin = (uint8_t*)cvb_pinned(c0, pin_q + (size_t)(n_kf + 1) * 4 + 64);
+  if (!pin) return CVB_ERR_CUDA;
+  if (!sift) memcpy(pin, q, qb);
+  else if (!cvb_quantize_sift((const float*)q, qb, pin))
+    return cvb_fail(c0, CVB_ERR_UNSUPPORTED, "%s: SIFT descriptors must be integer-valued in [0,255] (cv::xfeatures2d::SIFT output)", fn);
+  if (n_kf == 0) return CVB_OK;
+  if (nq == 0) {
+    if (n_matches) std::fill(n_matches, n_matches + n_kf, 0);
+    return CVB_OK;
+  }
+  int r = 0;
+  const int rc = group_request(db, pin, pin_q, nq, thr, ratio, n_matches, m_kf, m_query, m_train, m_dist, cap, n_total, &r);
+  if (!rc) return CVB_OK;
+  settle(db);
+  *n_total = 0;
+  return rank_fail(db, r, rc);
+}
+
+}  // namespace
+
+extern "C" {
+
+int cvb_db_group_create(cvb_group* g, int desc_bytes, cvb_db_group** out) {
+  if (!g || !out) return CVB_ERR_INVALID;
+  *out = nullptr;
+  std::lock_guard<std::recursive_mutex> lk(g->call_mtx);
+  cvb_ctx* c0 = g->ctx[0];
+  if (desc_bytes != 32 && desc_bytes != 128)
+    return cvb_fail(c0, CVB_ERR_UNSUPPORTED, "descriptor database: 32-byte ORB or 128-byte SIFT descriptors, got %d", desc_bytes);
+  cvb_db_group* db = new cvb_db_group();
+  db->g = g;
+  db->desc_bytes = desc_bytes;
+  int rc = CVB_OK;
+  for (int r = 0; r < g->n && !rc; r++) {
+    if ((rc = cvb_db_create(g->ctx[r], desc_bytes, &db->db[r]))) {
+      rc = rank_fail(db, r, rc);
+      break;
+    }
+    CVB_GUARD(g->ctx[r]);
+    const cudaError_t e = cudaEventCreateWithFlags(&db->done[r], cudaEventDisableTiming);
+    if (e != cudaSuccess) rc = cvb_fail(c0, CVB_ERR_CUDA, "cvb_db_group_create: rank %d: %s", r, cudaGetErrorString(e));
+  }
+  if (rc) {
+    cvb_db_group_destroy(db);
+    return rc;
+  }
+  *out = db;
+  return CVB_OK;
+}
+
+int cvb_db_group_destroy(cvb_db_group* db) {
+  if (!db) return CVB_OK;
+  cvb_group* g = db->g;
+  std::lock_guard<std::recursive_mutex> lk(g->call_mtx);
+  for (int r = 0; r < g->n; r++) {
+    CVB_GUARD(g->ctx[r]);
+    if (db->db[r]) cvb_db_destroy(g->ctx[r], db->db[r]);
+    if (db->done[r]) cudaEventDestroy(db->done[r]);
+  }
+  {
+    CVB_GUARD(g->ctx[0]);
+    for (cvb_buf* b : {&db->d_loc, &db->cnt, &db->src, &db->goff, &db->o_kf, &db->o_q, &db->o_t, &db->o_d})
+      if (b->p) cudaFree(b->p);
+  }
+  delete db;
+  return CVB_OK;
+}
+
+int cvb_db_group_append(cvb_db_group* db, const uint8_t* rows, const int32_t* rows_per_kf, int n_kf) {
+  if (!db) return CVB_ERR_INVALID;
+  std::lock_guard<std::recursive_mutex> lk(db->g->call_mtx);
+  return group_append_checked(db, false, rows, rows_per_kf, n_kf, "cvb_db_group_append");
+}
+
+int cvb_db_group_append_sift(cvb_db_group* db, const float* rows, const int32_t* rows_per_kf, int n_kf) {
+  if (!db) return CVB_ERR_INVALID;
+  std::lock_guard<std::recursive_mutex> lk(db->g->call_mtx);
+  return group_append_checked(db, true, rows, rows_per_kf, n_kf, "cvb_db_group_append_sift");
+}
+
+int cvb_db_group_remove(cvb_db_group* db, int kf_index) {
+  if (!db) return CVB_ERR_INVALID;
+  std::lock_guard<std::recursive_mutex> lk(db->g->call_mtx);
+  const int n_kf = (int)db->loc.size();
+  CVB_REQUIRE(db->g->ctx[0], kf_index >= 0 && kf_index < n_kf, "cvb_db_group_remove: keyframe index %d out of range (database holds %d)",
+              kf_index, n_kf);
+  const int r = db->loc[kf_index].x, l = db->loc[kf_index].y;
+  cvb_db* d = db->db[r];
+  const int64_t len = d->seg_ptr[l + 1] - d->seg_ptr[l];
+  if (const int rc = cvb_db_remove(db->g->ctx[r], d, l)) return rank_fail(db, r, rc);
+  db->rows[r] -= len;
+  db->loc.erase(db->loc.begin() + kf_index);
+  for (size_t i = (size_t)kf_index; i < db->loc.size(); i++)
+    if (db->loc[i].x == r) db->loc[i].y--;
+  db->loc_dirty = true;
+  return CVB_OK;
+}
+
+int cvb_db_group_size(const cvb_db_group* db, int32_t* n_kf, int64_t* n_rows, int64_t* rows_per_rank) {
+  if (!db) return CVB_ERR_INVALID;
+  std::lock_guard<std::recursive_mutex> lk(db->g->call_mtx);
+  int64_t all = 0;
+  for (int r = 0; r < db->g->n; r++) {
+    all += db->rows[r];
+    if (rows_per_rank) rows_per_rank[r] = db->rows[r];
+  }
+  if (n_kf) *n_kf = (int32_t)db->loc.size();
+  if (n_rows) *n_rows = all;
+  return CVB_OK;
+}
+
+int cvb_db_group_match_hamming(cvb_db_group* db, const uint8_t* q, int nq, float thr, float ratio, int32_t* n_matches,
+                               int32_t* m_kf, int32_t* m_query, int32_t* m_train, float* m_dist, int cap, int32_t* n_total) {
+  if (!db) return CVB_ERR_INVALID;
+  std::lock_guard<std::recursive_mutex> lk(db->g->call_mtx);
+  CVB_GUARD(db->g->ctx[0]);
+  return group_match(db, false, q, nq, thr, ratio, n_matches, m_kf, m_query, m_train, m_dist, cap, n_total, "cvb_db_group_match_hamming");
+}
+
+int cvb_db_group_match_l2(cvb_db_group* db, const float* q, int nq, float thr, float ratio, int32_t* n_matches, int32_t* m_kf,
+                          int32_t* m_query, int32_t* m_train, float* m_dist, int cap, int32_t* n_total) {
+  if (!db) return CVB_ERR_INVALID;
+  std::lock_guard<std::recursive_mutex> lk(db->g->call_mtx);
+  CVB_GUARD(db->g->ctx[0]);
+  return group_match(db, true, q, nq, thr, ratio, n_matches, m_kf, m_query, m_train, m_dist, cap, n_total, "cvb_db_group_match_l2");
 }
 
 }  // extern "C"

@@ -191,6 +191,83 @@ class DescriptorDatabase:
             pass
 
 
+class DescriptorDatabaseGroup:
+    """DescriptorDatabase with its keyframes spread over the ranks of an optimization.Group (cvb_db_group_*): each appended
+    keyframe goes to the rank holding the fewest rows (the lowest rank on a tie), and a request scans every rank's share
+    on that rank.  Indices, removals and the host requests' outputs are bit-identical to one DescriptorDatabase fed the same
+    appends and removes.  Give it a group of its own: its requests are serialised with every other call on the group.
+    The group must outlive the database."""
+
+    def __init__(self, group, kind: str = "orb"):
+        assert kind in ("orb", "sift"), kind
+        self.group = group
+        self.ctx = group.ctx          # rank 0's context carries the messages
+        self.kind = kind
+        h = C.c_void_p()
+        self.ctx.check(lib().cvb_db_group_create(group.h, 32 if kind == "orb" else 128, C.byref(h)))
+        self.handle = h
+        self._cap = 1 << 16
+
+    def append(self, rows, rows_per_kf):
+        """as DescriptorDatabase.append"""
+        rpk = np.ascontiguousarray(np.asarray(rows_per_kf, np.int32).reshape(-1))
+        if self.kind == "orb":
+            rows = _np(rows, np.uint8).reshape(-1, 32)
+            fn = lib().cvb_db_group_append
+        else:
+            rows = _np(rows, np.float32).reshape(-1, 128)
+            fn = lib().cvb_db_group_append_sift
+        assert int(rpk.sum()) == len(rows), "rows_per_kf does not add up to the number of rows"
+        self.ctx.check(fn(self.handle, _ptr(rows), _ptr(rpk), len(rpk)))
+
+    def remove(self, kf_index: int):
+        """a keyframe leaves the map: later keyframes move down by one global index"""
+        self.ctx.check(lib().cvb_db_group_remove(self.handle, int(kf_index)))
+
+    def size(self):
+        """→ (n_kf, n_rows)"""
+        return self.size_per_rank()[:2]
+
+    def size_per_rank(self):
+        """→ (n_kf, n_rows, rows_per_rank int64 [group size])"""
+        n_kf, n_rows = C.c_int32(), C.c_int64()
+        per = np.zeros(self.group.n, np.int64)
+        self.ctx.check(lib().cvb_db_group_size(self.handle, C.byref(n_kf), C.byref(n_rows), _ptr(per)))
+        return n_kf.value, n_rows.value, per
+
+    def _match(self, fn, q, thr, ratio):
+        n_kf, _ = self.size()
+        nm = np.zeros(n_kf, np.int32)
+        while True:
+            cap = self._cap
+            out = [np.empty(cap, np.int32), np.empty(cap, np.int32), np.empty(cap, np.int32), np.empty(cap, np.float32)]
+            tot = C.c_int32()
+            self.ctx.check(fn(self.handle, _ptr(q), len(q), thr, ratio, _ptr(nm), _ptr(out[0]), _ptr(out[1]), _ptr(out[2]),
+                              _ptr(out[3]), cap, C.byref(tot)))
+            if tot.value <= cap:
+                return (nm,) + tuple(o[:tot.value] for o in out)
+            self._cap = int(tot.value * 1.25) + 16
+
+    def match_hamming(self, q, thr: float = 40.0, ratio: float = 0.8):
+        """as DescriptorDatabase.match_hamming, m_kf = global keyframe index"""
+        return self._match(lib().cvb_db_group_match_hamming, _np(q, np.uint8).reshape(-1, 32), thr, ratio)
+
+    def match_l2(self, q, thr: float = 500.0, ratio: float = 0.8):
+        """as DescriptorDatabase.match_l2, m_kf = global keyframe index"""
+        return self._match(lib().cvb_db_group_match_l2, _np(q, np.float32).reshape(-1, 128), thr, ratio)
+
+    def close(self):
+        if self.handle:
+            lib().cvb_db_group_destroy(self.handle)
+            self.handle = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
 # ------------------------------------------------------------------------------------------------
 # L2 k-NN (SIFT)
 # ------------------------------------------------------------------------------------------------

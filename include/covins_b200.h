@@ -1003,6 +1003,43 @@ CVB_API int cvb_ba_solve_group(cvb_group* g, const cvb_ba_problem* p, const cvb_
 CVB_API int cvb_gba_group(cvb_group* g, const cvb_ba_problem* p, const cvb_gba_options* gba, int peer_path, cvb_ba_result* r,
                           uint8_t* obs_removed);
 
+/*
+ * The resident descriptor database (cvb_db_*) with its keyframes spread over the ranks of a group: every request scans each
+ * rank's share of the map on that rank, concurrently.  The operations are those of cvb_db with the same argument meaning;
+ * global keyframe indices, cvb_db_group_remove's index shift and every output (n_matches [n_kf], the matches compacted by
+ * (global keyframe, queryIdx), cap truncation, *n_total) are bit-identical to those of ONE cvb_db that received the same
+ * sequence of appends and removes.
+ *   Placement: each appended keyframe goes to the rank that holds the fewest rows at that moment, the lowest rank winning a
+ *   tie; the keyframes of one call are dealt one by one, in order.  Each rank keeps its keyframes in global order in an
+ *   ordinary cvb_db on its context; the host keeps the global -> (rank, local index) table and updates it on remove.
+ *   cvb_db_group_size: n_kf, n_rows as cvb_db_size; rows_per_rank [group size] (nullable) = the rows each rank holds.
+ *   A request: a SIFT query is checked and quantised once into rank 0's pinned staging before any device work and copied to
+ *   every rank; each rank holding keyframes runs the filtered 2-NN against them on its stream and compacts its accepted
+ *   matches (at most cap); rank 0's stream waits on the ranks' events and a gather on rank 0 reads every rank's counts and
+ *   compacted lists (same device, or over the peer access cvb_group_create enabled) into global keyframe order, so only
+ *   the accepted matches cross between devices; one copy of counts, total and min(total, cap) matches to the host.  The
+ *   calling thread enqueues everything; no host threads.
+ *   Refusals (before any rank is touched, every rank unchanged): a call of the other row kind -> CVB_ERR_INVALID; a SIFT
+ *   value that is not an integer in [0,255] -> CVB_ERR_UNSUPPORTED; a bad index, bad counts or bad arguments ->
+ *   CVB_ERR_INVALID.  Messages go to the group's ctxs[0]; a CUDA failure is reported there as "rank r: <message>" and leaves
+ *   the database undefined (destroy it).
+ *   Concurrency: the calls of a database are serialised on the group (cvb_group_create's call lock), with each other and
+ *   with the group's bundle-adjustment calls.  Give the database a group of its own (over the same devices if you like):
+ *   on a group that also runs cvb_gba_group, a place-recognition request waits for the whole GBA.  Destroy the database
+ *   before its group and the group's contexts.
+ */
+typedef struct cvb_db_group cvb_db_group;
+CVB_API int cvb_db_group_create(cvb_group* g, int desc_bytes, cvb_db_group** out);   /* 32 ORB, 128 SIFT, else CVB_ERR_UNSUPPORTED */
+CVB_API int cvb_db_group_destroy(cvb_db_group* db);
+CVB_API int cvb_db_group_append(cvb_db_group* db, const uint8_t* rows, const int32_t* rows_per_kf, int n_kf);
+CVB_API int cvb_db_group_append_sift(cvb_db_group* db, const float* rows, const int32_t* rows_per_kf, int n_kf);
+CVB_API int cvb_db_group_remove(cvb_db_group* db, int kf_index);
+CVB_API int cvb_db_group_size(const cvb_db_group* db, int32_t* n_kf, int64_t* n_rows, int64_t* rows_per_rank);
+CVB_API int cvb_db_group_match_hamming(cvb_db_group* db, const uint8_t* q, int nq, float thr, float ratio, int32_t* n_matches,
+                                       int32_t* m_kf, int32_t* m_query, int32_t* m_train, float* m_dist, int cap, int32_t* n_total);
+CVB_API int cvb_db_group_match_l2(cvb_db_group* db, const float* q, int nq, float thr, float ratio, int32_t* n_matches,
+                                  int32_t* m_kf, int32_t* m_query, int32_t* m_train, float* m_dist, int cap, int32_t* n_total);
+
 /* ------------------------------------------------------------------------------------------------
  * Map maintenance (SURVEY.md §8f rank 4)
  * ---------------------------------------------------------------------------------------------- */
