@@ -122,6 +122,8 @@ SIGNATURES = {
                                    C.POINTER(C.c_int64)]),
     "cvb_redundant_keyframes": (C.c_int, [c_vp, C.c_int, C.c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, C.c_double,
                                           C.c_double, C.c_int, C.c_int, c_vp, C.POINTER(C.c_int32)]),
+    "cvb_landmark_outliers": (C.c_int, [c_vp, c_vp, c_vp, C.c_double, C.c_double, C.c_int, c_vp, c_vp, c_vp, C.POINTER(C.c_int64),
+                                        C.POINTER(C.c_int32)]),
 }
 
 

@@ -332,6 +332,21 @@ __global__ void __launch_bounds__(256, 2) lin_obs_kernel(int n_obs, const int* _
   block_reduce_store<1>(csum, partials, slots);
 }
 
+// K4b: the loss-corrected residual norm of every observation (cvb_ba_reproj_norms) through bam::corrected_norm, the function
+// cvb_landmark_outliers calls too, so that the two report the same norms bit for bit
+__global__ void reproj_norms_kernel(int n_obs, const int* __restrict__ obs_kf, const int* __restrict__ obs_lm, const double* __restrict__ obs_uv,
+                                    const double* __restrict__ obs_sigma, const double* __restrict__ pose, const double* __restrict__ lm,
+                                    const double* __restrict__ extr_kf, const double* __restrict__ intr_kf, const double* __restrict__ dist_kf,
+                                    const int* __restrict__ model_kf, const double* __restrict__ xi_kf, double a2, double* __restrict__ norms) {
+  const int o = blockIdx.x * blockDim.x + threadIdx.x;
+  if (o >= n_obs) return;
+  const int k = obs_kf[o], mk = model_kf[k];
+  const CamModel cm{mk & 0xff, mk >> 8, xi_kf[k]};
+  bool projectable;
+  norms[o] = corrected_norm(pose + 7 * k, extr_kf + 7 * k, intr_kf + 4 * k, dist_kf + 4 * k, cm, lm + 3 * obs_lm[o], obs_uv[2 * o],
+                            obs_uv[2 * o + 1], obs_sigma[o], a2, &projectable);
+}
+
 // per landmark: Hll = sum Jl^T Jl (6 unique: 00 01 02 11 12 22), bl = sum Jl^T r, colsq of the 3 columns
 __global__ void lm_reduce_kernel(int L, const int* __restrict__ lm_ptr, const ObsLin* __restrict__ lin,
                                  double* __restrict__ Hll, double* __restrict__ bl, double* __restrict__ colsq_l,
@@ -1638,24 +1653,10 @@ int engine_setup(Engine& E, const cvb_ba_problem* p, const cvb_ba_options* o) {
   if ((rc = zalloc(E, E.lm[1], (size_t)3 * E.L_in))) return rc;
   if ((rc = upload(E, E.pose0, p->pose, (size_t)7 * K)) || (rc = upload(E, E.sb0, h_sb)) || (rc = upload(E, E.lm0, h_lm))) return rc;
   if ((rc = upload(E, E.pose_const, p->pose_const, (size_t)K))) return rc;
-  std::vector<double> ex((size_t)7 * K), in((size_t)4 * K), di((size_t)4 * K), xi(K, 0.0);
-  std::vector<int> mdl(K, 0);
-  for (int k = 0; k < K; k++) {
-    const int c = p->cam_of_kf ? p->cam_of_kf[k] : 0;
-    CVB_REQUIRE(ctx, c >= 0 && c < p->n_cam, "cam_of_kf out of range");
-    const int cam = p->cam_model ? p->cam_model[c] : 0, dm = p->dist_model ? p->dist_model[c] : 0;
-    // optimization_be.cpp:186-231: "Unknown projection type" / "Unknown distortion type" → exit(-1) in the reference
-    if (cam < 0 || cam > 1) return cvb_fail(ctx, CVB_ERR_UNSUPPORTED, "Unknown projection type (%d) for camera %d", cam, c);
-    if (dm < 0 || dm > 2) return cvb_fail(ctx, CVB_ERR_UNSUPPORTED, "Unknown distortion type (%d) for camera %d", dm, c);
-    CVB_REQUIRE(ctx, cam == 0 || p->cam_xi, "unified projection camera needs cam_xi");
-    mdl[k] = cam | (dm << 8);
-    xi[k] = (cam == 1) ? p->cam_xi[c] : 0.0;
-    std::memcpy(&ex[7 * (size_t)k], p->extr + 7 * (size_t)c, 7 * sizeof(double));
-    std::memcpy(&in[4 * (size_t)k], p->intr + 4 * (size_t)c, 4 * sizeof(double));
-    std::memcpy(&di[4 * (size_t)k], p->dist + 4 * (size_t)c, 4 * sizeof(double));
-  }
-  if ((rc = upload(E, E.extr_kf, ex)) || (rc = upload(E, E.intr_kf, in)) || (rc = upload(E, E.dist_kf, di)) ||
-      (rc = upload(E, E.model_kf, mdl)) || (rc = upload(E, E.xi_kf, xi)))
+  cvb_kf_cameras cams;
+  if ((rc = cvb_stage_kf_cameras(ctx, p, cams))) return rc;
+  if ((rc = upload(E, E.extr_kf, cams.extr)) || (rc = upload(E, E.intr_kf, cams.intr)) || (rc = upload(E, E.dist_kf, cams.dist)) ||
+      (rc = upload(E, E.model_kf, cams.model)) || (rc = upload(E, E.xi_kf, cams.xi)))
     return rc;
   if ((rc = upload(E, E.obs_kf, h_obs_kf)) || (rc = upload(E, E.obs_lm, h_obs_lm)) || (rc = upload(E, E.lm_ptr, h_lm_ptr)) ||
       (rc = upload(E, E.kf_ptr, h_kf_ptr)) || (rc = upload(E, E.kf_obs, h_kf_obs)) || (rc = upload(E, E.obs_uv, h_uv)) ||
@@ -2193,10 +2194,12 @@ int engine_iterate(Engine& E, bool* done) {
 int engine_corrected_norms(Engine& E, double* h_norms_full, int n_obs_full) {
   DevArr<double> d;
   if (d.alloc((size_t)E.n_obs)) return cvb_fail(E.ctx, CVB_ERR_CUDA, "cudaMalloc failed");
-  lin_obs_kernel<<<RED_BLOCKS, 256, 0, E.st>>>(E.n_obs, E.obs_kf.p, E.obs_lm.p, E.obs_uv.p, E.obs_sigma.p, E.pose[E.cur].p,
-                                               E.lm[E.cur].p, E.extr_kf.p, E.intr_kf.p, E.dist_kf.p, E.model_kf.p, E.xi_kf.p, E.scale.p, E.off_pose.p, E.n_c_pad,
-                                               E.a2_reproj, 2, E.lin.p, E.ow.p, d.p, E.partials.p, 0);
-  ENG_LAUNCH();
+  if (E.n_obs) {
+    reproj_norms_kernel<<<(E.n_obs + 255) / 256, 256, 0, E.st>>>(E.n_obs, E.obs_kf.p, E.obs_lm.p, E.obs_uv.p, E.obs_sigma.p, E.pose[E.cur].p,
+                                                                 E.lm[E.cur].p, E.extr_kf.p, E.intr_kf.p, E.dist_kf.p, E.model_kf.p, E.xi_kf.p,
+                                                                 E.a2_reproj, d.p);
+    ENG_LAUNCH();
+  }
   std::vector<double> h(E.n_obs);
   ENG_CUDA(cudaMemcpyAsync(h.data(), d.p, sizeof(double) * E.n_obs, cudaMemcpyDeviceToHost, E.st));
   ENG_CUDA(cudaStreamSynchronize(E.st));

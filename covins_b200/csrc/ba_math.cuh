@@ -277,6 +277,24 @@ __host__ __device__ inline bool reproj(const double* pose, const double* extr, c
   return true;
 }
 
+// ---- loss-corrected reprojection residual norm of one observation (cvb_ba_reproj_norms, optimization_be.cpp:270-290):
+// r from reproj, s = r.r, norm = sqrt(s) * the Cauchy scale (a2 <= 0: |r|); *projectable = reproj's result.  Never inlined:
+// ptxas may fuse a multiply and an add differently in different callers, so the kernels that must report the same norm
+// bit for bit (the bundle adjustment's reproj_norms_kernel, cvb_landmark_outliers) call this one separately compiled body.
+// Device code only: host translation units that include this header for its __host__ __device__ math do not see it.
+#ifdef __CUDACC__
+__device__ __noinline__ static double corrected_norm(const double* pose, const double* extr, const double* intr, const double* dist,
+                                                     const CamModel& cm, const double* lm, double u_obs, double v_obs, double sigma,
+                                                     double a2, bool* projectable) {
+  double r[2];
+  *projectable = reproj(pose, extr, intr, dist, cm, lm, u_obs, v_obs, sigma, r, nullptr, nullptr, false);
+  const double s = r[0] * r[0] + r[1] * r[1];
+  double sc, c;
+  cauchy(s, a2, &sc, &c);
+  return sqrt(s) * sc;
+}
+#endif
+
 // ---- between factor: e = S [2 vec(qm^-1 q1^-1 q2); R1^T (t2 - t1) - tm]   (6), J = [de/dx1 (6x6) | de/dx2 (6x6)]
 // stored row-major as 6 x 12.
 __host__ __device__ inline void between(const double* pose1, const double* pose2, const double* qm, const double* tm,

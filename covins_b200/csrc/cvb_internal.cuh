@@ -152,6 +152,15 @@ int cvb_covisibility_budgeted(cvb_ctx* ctx, int K, int L, const int32_t* lm_obs_
                               const uint8_t* lm_valid, int min_weight, int32_t* nbr_ptr, int32_t* nbr_kf, int32_t* nbr_w, int64_t cap,
                               int64_t* n_total, int64_t pair_budget);
 
+// Every keyframe's camera as the reprojection kernels read it (bam::reproj): the extr [K][7], intr [K][4] and
+// dist [K][4] of its calibration cam_of_kf[k], model = camera | distortion << 8, xi (0 for a pinhole camera).  The bundle
+// adjustment and cvb_landmark_outliers stage it here, so both project through the same numbers.  CVB_ERR_INVALID for a
+// calibration index out of range, CVB_ERR_UNSUPPORTED (the reference's messages) for an unknown camera or distortion model.
+struct cvb_kf_cameras {
+  std::vector<double> extr, intr, dist, xi;
+  std::vector<int> model;
+};
+
 #define CVB_CUDA(ctx, call)                                                                         \
   do {                                                                                              \
     cudaError_t e_ = (call);                                                                        \
@@ -246,6 +255,27 @@ inline int cvb_block::download() {
   CVB_CUDA(ctx, cudaStreamSynchronize(st));
   for (const Arr& a : arrs)
     if (a.kind == kOut && a.dst && a.bytes) memcpy(a.dst, h + in_hi + (a.off - out_lo), a.bytes);
+  return CVB_OK;
+}
+
+inline int cvb_stage_kf_cameras(cvb_ctx* ctx, const cvb_ba_problem* p, cvb_kf_cameras& out) {
+  const int K = p->K;
+  out.extr.assign((size_t)7 * K, 0.0); out.intr.assign((size_t)4 * K, 0.0); out.dist.assign((size_t)4 * K, 0.0);
+  out.xi.assign(K, 0.0); out.model.assign(K, 0);
+  for (int k = 0; k < K; k++) {
+    const int c = p->cam_of_kf ? p->cam_of_kf[k] : 0;
+    CVB_REQUIRE(ctx, c >= 0 && c < p->n_cam, "cam_of_kf out of range");
+    const int cam = p->cam_model ? p->cam_model[c] : 0, dm = p->dist_model ? p->dist_model[c] : 0;
+    // optimization_be.cpp:186-231: "Unknown projection type" / "Unknown distortion type" → exit(-1) in the reference
+    if (cam < 0 || cam > 1) return cvb_fail(ctx, CVB_ERR_UNSUPPORTED, "Unknown projection type (%d) for camera %d", cam, c);
+    if (dm < 0 || dm > 2) return cvb_fail(ctx, CVB_ERR_UNSUPPORTED, "Unknown distortion type (%d) for camera %d", dm, c);
+    CVB_REQUIRE(ctx, cam == 0 || p->cam_xi, "unified projection camera needs cam_xi");
+    out.model[k] = cam | (dm << 8);
+    out.xi[k] = (cam == 1) ? p->cam_xi[c] : 0.0;
+    memcpy(&out.extr[7 * (size_t)k], p->extr + 7 * (size_t)c, 7 * sizeof(double));
+    memcpy(&out.intr[4 * (size_t)k], p->intr + 4 * (size_t)c, 4 * sizeof(double));
+    memcpy(&out.dist[4 * (size_t)k], p->dist + 4 * (size_t)c, 4 * sizeof(double));
+  }
   return CVB_OK;
 }
 

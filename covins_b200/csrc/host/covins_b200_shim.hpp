@@ -291,6 +291,48 @@ inline void flatten_observations(const std::vector<LandmarkPtr>& landmarks, cons
   }
 }
 
+// The camera and observation part of a map's flat problem, shared by GlobalBundleAdjustment and RemoveLandmarkOutliers: every
+// keyframe of kfs (canonical order) with its state (UpdateCeresFromState, keyframe_base.cpp:486-521), its own calibration
+// (cam_of_kf[k] = k) and camera model, pose_const cleared; then the valid landmarks (flatten_observations) with their
+// positions and each observation's keypoint and sigma.  obs_ref[i] names observation i's keyframe, landmark and feature for
+// the write-back.
+template <class KeyframePtr>
+struct ObsRef {
+  KeyframePtr kf;
+  int lm;
+  int feat;
+};
+template <class KeyframePtr, class KF, class LandmarkPtr>
+inline void flatten_cameras_and_observations(const std::vector<KeyframePtr>& kfs, const std::map<const KF*, int>& kf_index,
+                                             const std::vector<LandmarkPtr>& landmarks, Flat& F, std::vector<LandmarkPtr>& lms,
+                                             std::vector<ObsRef<KeyframePtr>>& obs_ref) {
+  const int K = (int)kfs.size();
+  F.pose.resize(7 * (size_t)K); F.sb.resize(9 * (size_t)K); F.extr.resize(7 * (size_t)K); F.intr.resize(4 * (size_t)K);
+  F.dist.resize(4 * (size_t)K); F.pose_const.assign(K, 0); F.cam_of_kf.resize(K);
+  F.cam_model.assign(K, 0); F.dist_model.assign(K, 0); F.cam_xi.assign(K, 0.0);
+  for (int k = 0; k < K; k++) {
+    auto& kf = kfs[k];
+    kf->UpdateCeresFromState(&F.pose[7 * (size_t)k], &F.sb[9 * (size_t)k], &F.extr[7 * (size_t)k]);
+    F.cam_of_kf[k] = k;
+    if (!Adapter<KF>::camera(*kf, &F.intr[4 * (size_t)k], &F.dist[4 * (size_t)k])) {
+      std::printf("FATAL: Unknown projection type.\n");                                            // optimization_be.cpp:112-114
+      std::exit(-1);
+    }
+    Adapter<KF>::camera_model(*kf, &F.cam_model[k], &F.dist_model[k], &F.cam_xi[k]);                // :186-231
+  }
+  flatten_observations(landmarks, kf_index, lms, F.lm_obs_ptr, F.obs_kf, [&](int k, int feat, int l) {
+    auto& kfx = kfs[k];
+    const auto& kp = kfx->keypoints_distorted_[feat];
+    F.obs_uv.push_back((float)kp[0]); F.obs_uv.push_back((float)kp[1]);
+    F.obs_sigma.push_back((kfx->keypoints_aors_[feat][1] + 1) * 2.0);                              // :183-184, 477-478
+    obs_ref.push_back({kfx, l, feat});
+  });
+  for (auto& lm : lms) {
+    const auto pos = lm->GetWorldPos();
+    F.lm.push_back(pos[0]); F.lm.push_back(pos[1]); F.lm.push_back(pos[2]);
+  }
+}
+
 }  // namespace detail
 
 // parameters the reference reads from covins_params (config/config_backend.yaml; SURVEY.md §5)
@@ -330,26 +372,17 @@ void global_bundle_adjustment(MapPtr map, int interations_limit, bool visual_onl
   std::vector<KeyframePtr> kfs;               // valid keyframes, canonical order
   detail::canonical_keyframes(keyframes, kf_index, kfs);
   const int K = (int)kfs.size();
-  F.pose.resize(7 * (size_t)K); F.sb.resize(9 * (size_t)K); F.extr.resize(7 * (size_t)K); F.intr.resize(4 * (size_t)K);
-  F.dist.resize(4 * (size_t)K); F.pose_const.assign(K, 0); F.cam_of_kf.resize(K);
+  // keyframe states, cameras, landmarks + observations (detail::flatten_cameras_and_observations: the canonical landmark
+  // order and observation CSR)
+  using LandmarkPtr = typename std::decay<decltype(landmarks[0])>::type;
+  std::vector<LandmarkPtr> lms;
+  std::vector<detail::ObsRef<KeyframePtr>> obs_ref;
+  detail::flatten_cameras_and_observations(kfs, kf_index, landmarks, F, lms, obs_ref);
   F.imu_ptr.push_back(0);
   for (int k = 0; k < K; k++) {
     auto& kf = kfs[k];
-    // UpdateCeresFromState (keyframe_base.cpp:486-521) restated on the flat arrays
-    kf->UpdateCeresFromState(&F.pose[7 * (size_t)k], &F.sb[9 * (size_t)k], &F.extr[7 * (size_t)k]);
-    F.cam_of_kf[k] = k;
     if (kf->id_.first == 0 && kf->id_.second == map->id_map_) F.pose_const[k] = 1;                 // :88-89, 329-331
     if (kf->is_loaded_ && P.gba_fix_poses_loaded_maps) F.pose_const[k] = 1;                        // :338-341
-    if (!Adapter<KF>::camera(*kf, &F.intr[4 * (size_t)k], &F.dist[4 * (size_t)k])) {
-      std::printf("FATAL: Unknown projection type.\n");                                            // :112-114
-      std::exit(-1);
-    }
-    {
-      int cm = 0, dm = 0; double xi = 0.0;
-      Adapter<KF>::camera_model(*kf, &cm, &dm, &xi);                                               // :186-231
-      F.cam_model.resize(F.pose_const.size(), 0); F.dist_model.resize(F.pose_const.size(), 0); F.cam_xi.resize(F.pose_const.size(), 0.0);
-      F.cam_model[k] = cm; F.dist_model[k] = dm; F.cam_xi[k] = xi;
-    }
     if (!visual_only) {                                                                             // :117-144, 367-421
       auto pred = kf->GetPredecessor();
       if (!pred || pred->IsInvalid()) {
@@ -375,22 +408,6 @@ void global_bundle_adjustment(MapPtr map, int interations_limit, bool visual_onl
       F.imu_gyr0.insert(F.imu_gyr0.end(), g0, g0 + 3);
       F.imu_ptr.push_back((int32_t)F.imu_dt.size());
     }
-  }
-  // landmarks + observations (detail::flatten_observations: the canonical landmark order and observation CSR)
-  struct ObsRef { KeyframePtr kf; int lm; int feat; };
-  std::vector<ObsRef> obs_ref;
-  using LandmarkPtr = typename std::decay<decltype(landmarks[0])>::type;
-  std::vector<LandmarkPtr> lms;
-  detail::flatten_observations(landmarks, kf_index, lms, F.lm_obs_ptr, F.obs_kf, [&](int k, int feat, int l) {
-    auto& kfx = kfs[k];
-    const auto& kp = kfx->keypoints_distorted_[feat];
-    F.obs_uv.push_back((float)kp[0]); F.obs_uv.push_back((float)kp[1]);
-    F.obs_sigma.push_back((kfx->keypoints_aors_[feat][1] + 1) * 2.0);                              // :183-184, 477-478
-    obs_ref.push_back({kfx, l, feat});
-  });
-  for (auto& lm : lms) {
-    const auto pos = lm->GetWorldPos();
-    F.lm.push_back(pos[0]); F.lm.push_back(pos[1]); F.lm.push_back(pos[2]);
   }
   // loop edges (:236-254, 532-557): sqrt_info = diag(100 I3, 1e4 I3)
   if (P.gba_use_map_loop_constraints) {
@@ -560,6 +577,46 @@ void PruneRedundantKeyframes(Context& ctx, MapPtr map, double th_red, double max
             "cvb_redundant_keyframes");
   for (int k = 0; k < K; k++)
     if (culled[k]) kfs[k]->SetInvalid();
+  UpdateCovisibilityConnections(ctx, map);
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// The landmark outlier removal of Map::Clean (map_be.cpp:448-454, 698-743), found in one cvb_landmark_outliers call (the
+// rule is in include/covins_b200.h) on the flat map the GBA builds (detail::flatten_cameras_and_observations).  Write-back in
+// canonical order: each outlier observation through the calls of the GBA's round-1 purge (kf->EraseLandmark(feat),
+// lm->EraseObservation(kf), optimization_be.cpp:282-288), then each erased landmark through map->EraseLandmark(lm), then
+// the covisibility graph of what remains is rebuilt.  Map::Clean calls it in place of its own landmark pass
+// (INTEGRATION.md §3.7), so the map->Clean() that ends GlobalBundleAdjustment picks it up.
+// ---------------------------------------------------------------------------------------------------------------
+template <class MapPtr>
+void RemoveLandmarkOutliers(Context& ctx, MapPtr map, double th_outlier = 0.92, double cauchy = 1.0, int min_obs = 2) {
+  using KeyframePtr = typename std::decay<decltype(map->GetKeyframesVec()[0])>::type;
+  using KF = typename KeyframePtr::element_type;
+  auto landmarks = map->GetLandmarksVec();
+  using LandmarkPtr = typename std::decay<decltype(landmarks[0])>::type;
+  std::map<const KF*, int> kf_index;
+  std::vector<KeyframePtr> kfs;
+  detail::canonical_keyframes(map->GetKeyframesVec(), kf_index, kfs);
+  detail::Flat F;
+  std::vector<LandmarkPtr> lms;
+  std::vector<detail::ObsRef<KeyframePtr>> obs_ref;
+  detail::flatten_cameras_and_observations(kfs, kf_index, landmarks, F, lms, obs_ref);
+  const cvb_ba_problem prob = F.view();
+  std::vector<uint8_t> outlier(obs_ref.size() + 1, 0), erase(lms.size() + 1, 0);
+  int64_t n_outlier = 0;
+  int32_t n_erased = 0;
+  ctx.check(cvb_landmark_outliers(ctx.get(), &prob, nullptr, th_outlier, cauchy, min_obs, outlier.data(), erase.data(), nullptr, &n_outlier,
+                                  &n_erased),
+            "cvb_landmark_outliers");
+  for (size_t i = 0; i < obs_ref.size(); i++)
+    if (outlier[i]) {
+      obs_ref[i].kf->EraseLandmark(obs_ref[i].feat);
+      lms[obs_ref[i].lm]->EraseObservation(obs_ref[i].kf);
+    }
+  for (size_t l = 0; l < lms.size(); l++)
+    if (erase[l]) map->EraseLandmark(lms[l]);
+  std::printf("--> Landmark outliers: removed %lld of %zu observations, erased %d of %zu landmarks\n", (long long)n_outlier, obs_ref.size(),
+              n_erased, lms.size());
   UpdateCovisibilityConnections(ctx, map);
 }
 

@@ -25,7 +25,9 @@
 #include <cuda/std/functional>
 
 #include <algorithm>
+#include <cmath>
 
+#include "ba_math.cuh"
 #include "cvb_internal.cuh"
 
 namespace {
@@ -518,4 +520,154 @@ extern "C" int cvb_redundant_keyframes(cvb_ctx* ctx, int K, int L, const int32_t
   for (int k = 0; k < K; k++) culled[k] = state[k] == 2;
   if (n_rounds) *n_rounds = round;
   return CVB_OK;
+}
+
+// ======================================================================================================================
+// K15 cvb_landmark_outliers: the landmark outlier removal of Map::Clean (include/covins_b200.h states the rule), one thread
+// per observation and one per landmark:
+//   lo_obs_kernel  a CTA takes 256 consecutive observations and finds the landmarks of its first and last one by binary
+//                  search over lm_obs_ptr; each thread then searches only that range for its own.  So the work is cut by
+//                  observation wherever landmarks begin and end: a landmark seen by 2 000 keyframes spreads over 8 CTAs.
+//                  A participating observation's norm is bam::corrected_norm on the per-keyframe cameras the bundle adjustment
+//                  stages (cvb_stage_kf_cameras): the function lin_obs_kernel's mode 2 (cvb_ba_reproj_norms) calls;
+//                  its flag is 2 if the point is not projectable, 1 if norm > th_outlier, else 0 and an integer atomicAdd
+//                  to its landmark's count of good observations;
+//   lo_lm_kernel   a participating landmark is erased iff its count is below min_obs.
+// Both totals are integer atomicAdds of per-CTA counts.  Integer decisions on fixed-order FP64 arithmetic: the output is
+// bit-identical from run to run, and the launch count (2) does not depend on the map.
+// ======================================================================================================================
+namespace {
+
+constexpr int LO_THREADS = 256;
+
+// the landmark that holds observation o: the largest l in [lo, hi) with lm_ptr[l] <= o, given lm_ptr[lo] <= o < lm_ptr[hi]
+__device__ __forceinline__ int lo_landmark_of(const int32_t* __restrict__ lm_ptr, int o, int lo, int hi) {
+  while (hi - lo > 1) {
+    const int mid = (lo + hi) >> 1;
+    if (__ldg(lm_ptr + mid) <= o) lo = mid; else hi = mid;
+  }
+  return lo;
+}
+
+__global__ void __launch_bounds__(LO_THREADS) lo_obs_kernel(int n_obs, int L, const int32_t* __restrict__ lm_ptr, const int32_t* __restrict__ obs_kf,
+                                                            const float* __restrict__ obs_uv, const double* __restrict__ obs_sigma,
+                                                            const uint8_t* __restrict__ obs_skip, const uint8_t* __restrict__ lm_valid,
+                                                            const double* __restrict__ lm, const double* __restrict__ pose,
+                                                            const double* __restrict__ extr_kf, const double* __restrict__ intr_kf,
+                                                            const double* __restrict__ dist_kf, const int* __restrict__ model_kf,
+                                                            const double* __restrict__ xi_kf, double a2, double th_outlier,
+                                                            uint8_t* __restrict__ obs_outlier, double* __restrict__ norms, int32_t* good,
+                                                            unsigned long long* n_outlier) {
+  __shared__ int s_l[2];
+  const int o0 = blockIdx.x * LO_THREADS;
+  if (threadIdx.x < 2) s_l[threadIdx.x] = lo_landmark_of(lm_ptr, threadIdx.x == 0 ? o0 : min(o0 + LO_THREADS, n_obs) - 1, 0, L);
+  __syncthreads();
+  const int o = o0 + threadIdx.x;
+  int flag = 0;
+  if (o < n_obs) {
+    const int l = lo_landmark_of(lm_ptr, o, s_l[0], s_l[1] + 1);
+    double norm = -1.0;
+    if (!(obs_skip && obs_skip[o]) && !(lm_valid && !lm_valid[l])) {
+      const int k = obs_kf[o];
+      const int mk = model_kf[k];
+      const bam::CamModel cm{mk & 0xff, mk >> 8, xi_kf[k]};
+      bool projectable;
+      norm = bam::corrected_norm(pose + 7 * k, extr_kf + 7 * k, intr_kf + 4 * k, dist_kf + 4 * k, cm, lm + 3 * (size_t)l,
+                                 (double)obs_uv[2 * (size_t)o], (double)obs_uv[2 * (size_t)o + 1], obs_sigma[o], a2, &projectable);
+      flag = !projectable ? 2 : norm > th_outlier ? 1 : 0;
+      if (flag == 0) atomicAdd(&good[l], 1);
+    }
+    obs_outlier[o] = (uint8_t)flag;
+    if (norms) norms[o] = norm;
+  }
+  const int n = __syncthreads_count(flag != 0);
+  if (threadIdx.x == 0 && n) atomicAdd(n_outlier, (unsigned long long)n);
+}
+
+__global__ void __launch_bounds__(LO_THREADS) lo_lm_kernel(int L, const uint8_t* __restrict__ lm_valid, const int32_t* __restrict__ good, int min_obs,
+                                                           uint8_t* __restrict__ lm_erase, int32_t* n_erased) {
+  const int l = blockIdx.x * LO_THREADS + threadIdx.x;
+  int erase = 0;
+  if (l < L) {
+    erase = !(lm_valid && !lm_valid[l]) && good[l] < min_obs;
+    lm_erase[l] = (uint8_t)erase;
+  }
+  const int n = __syncthreads_count(erase);
+  if (threadIdx.x == 0 && n) atomicAdd(n_erased, n);
+}
+
+}  // namespace
+
+extern "C" int cvb_landmark_outliers(cvb_ctx* ctx, const cvb_ba_problem* p, const uint8_t* lm_valid, double th_outlier, double cauchy, int min_obs,
+                                     uint8_t* obs_outlier, uint8_t* lm_erase, double* norms, int64_t* n_obs_outlier, int32_t* n_lm_erased) {
+  if (!ctx) return CVB_ERR_INVALID;
+  CVB_GUARD(ctx);
+  CVB_REQUIRE(ctx, p && n_obs_outlier && n_lm_erased, "cvb_landmark_outliers: p, n_obs_outlier and n_lm_erased are required");
+  const int K = p->K, L = p->L, n_obs = p->n_obs;
+  CVB_REQUIRE(ctx, K >= 0 && L >= 0 && n_obs >= 0, "cvb_landmark_outliers: negative size (K %d, L %d, n_obs %d)", K, L, n_obs);
+  CVB_REQUIRE(ctx, th_outlier > 0.0, "cvb_landmark_outliers: th_outlier %g is not > 0", th_outlier);
+  CVB_REQUIRE(ctx, std::isfinite(cauchy), "cvb_landmark_outliers: cauchy %g is not finite", cauchy);
+  CVB_REQUIRE(ctx, min_obs >= 1, "cvb_landmark_outliers: min_obs %d < 1", min_obs);
+  CVB_REQUIRE(ctx, (obs_outlier || n_obs == 0) && (lm_erase || L == 0), "cvb_landmark_outliers: obs_outlier and lm_erase are required");
+  CVB_REQUIRE(ctx, p->lm_obs_ptr || (L == 0 && n_obs == 0), "cvb_landmark_outliers: lm_obs_ptr is null");
+  CVB_REQUIRE(ctx, !p->lm_obs_ptr || p->lm_obs_ptr[0] == 0, "cvb_landmark_outliers: lm_obs_ptr[0] = %d, not 0", p->lm_obs_ptr ? p->lm_obs_ptr[0] : 0);
+  for (int l = 0; l < L; l++)
+    CVB_REQUIRE(ctx, p->lm_obs_ptr[l + 1] >= p->lm_obs_ptr[l], "cvb_landmark_outliers: lm_obs_ptr decreases at landmark %d", l);
+  CVB_REQUIRE(ctx, !p->lm_obs_ptr || p->lm_obs_ptr[L] == n_obs, "cvb_landmark_outliers: lm_obs_ptr[L] = %d, not n_obs = %d",
+              p->lm_obs_ptr ? p->lm_obs_ptr[L] : 0, n_obs);
+  CVB_REQUIRE(ctx, n_obs == 0 || (p->obs_kf && p->obs_uv && p->obs_sigma && p->lm && p->pose),
+              "cvb_landmark_outliers: obs_kf, obs_uv, obs_sigma, lm and pose are required");
+  CVB_REQUIRE(ctx, K == 0 || (p->extr && p->intr && p->dist), "cvb_landmark_outliers: extr, intr and dist are required");
+  const int32_t* obs_kf = p->obs_kf;
+  const double* obs_sigma = p->obs_sigma;
+  for (int o = 0; o < n_obs; o++) {
+    CVB_REQUIRE(ctx, (unsigned)obs_kf[o] < (unsigned)K, "cvb_landmark_outliers: obs_kf[%d] = %d outside [0, %d)", o, obs_kf[o], K);
+    CVB_REQUIRE(ctx, obs_sigma[o] > 0.0 && obs_sigma[o] < INFINITY, "cvb_landmark_outliers: obs_sigma[%d] = %g is not positive and finite", o,
+                obs_sigma[o]);
+  }
+  cvb_kf_cameras cams;
+  if (const int rc = cvb_stage_kf_cameras(ctx, p, cams)) return rc;
+  *n_obs_outlier = 0;
+  *n_lm_erased = 0;
+  if (K == 0 || L == 0 || n_obs == 0) {   // nothing to judge: nothing is flagged
+    if (obs_outlier) std::fill(obs_outlier, obs_outlier + n_obs, 0);
+    if (lm_erase) std::fill(lm_erase, lm_erase + L, 0);
+    if (norms) std::fill(norms, norms + n_obs, -1.0);
+    return CVB_OK;
+  }
+
+  cudaStream_t st = ctx->stream;
+  cvb_block In(ctx, st, false);   // direct: the observation arrays are large
+  const int32_t *d_ptr, *d_kf, *d_model;
+  const float* d_uv;
+  const double *d_sigma, *d_lm, *d_pose, *d_extr, *d_intr, *d_dist, *d_xi;
+  const uint8_t *d_skip = nullptr, *d_valid = nullptr;
+  In.in(d_ptr, p->lm_obs_ptr, (size_t)L + 1); In.in(d_kf, obs_kf, n_obs); In.in(d_uv, p->obs_uv, 2 * (size_t)n_obs);
+  In.in(d_sigma, obs_sigma, n_obs); In.in(d_lm, p->lm, 3 * (size_t)L); In.in(d_pose, p->pose, 7 * (size_t)K);
+  In.in(d_extr, cams.extr.data(), cams.extr.size()); In.in(d_intr, cams.intr.data(), cams.intr.size());
+  In.in(d_dist, cams.dist.data(), cams.dist.size()); In.in(d_xi, cams.xi.data(), cams.xi.size()); In.in(d_model, cams.model.data(), K);
+  if (p->obs_skip) In.in(d_skip, p->obs_skip, n_obs);
+  if (lm_valid) In.in(d_valid, lm_valid, L);
+  if (const int rc = In.place()) return rc;
+  if (const int rc = In.upload()) return rc;
+  // the outputs in one range, downloaded by one copy: the two totals, the two masks, then the optional norms
+  cvb_block Out(ctx, st);
+  int32_t *good, *d_erased;
+  unsigned long long* d_n_outlier;
+  uint8_t *d_outlier, *d_erase;
+  double* d_norms = nullptr;
+  Out.tmp(good, L);
+  Out.out(d_n_outlier, n_obs_outlier, 1); Out.out(d_erased, n_lm_erased, 1);
+  Out.out(d_outlier, obs_outlier, n_obs); Out.out(d_erase, lm_erase, L);
+  if (norms) Out.out(d_norms, norms, n_obs);
+  if (const int rc = Out.place()) return rc;
+  // good and the two totals are adjacent: one memset zeroes the three
+  CVB_CUDA(ctx, cudaMemsetAsync(good, 0, (size_t)((char*)(d_erased + 1) - (char*)good), st));
+  lo_obs_kernel<<<(unsigned)((n_obs + LO_THREADS - 1) / LO_THREADS), LO_THREADS, 0, st>>>(
+      n_obs, L, d_ptr, d_kf, d_uv, d_sigma, d_skip, d_valid, d_lm, d_pose, d_extr, d_intr, d_dist, d_model, d_xi,
+      cauchy > 0.0 ? cauchy * cauchy : 0.0, th_outlier, d_outlier, d_norms, good, d_n_outlier);
+  CVB_CHECK_LAUNCH(ctx);
+  lo_lm_kernel<<<(unsigned)((L + LO_THREADS - 1) / LO_THREADS), LO_THREADS, 0, st>>>(L, d_valid, good, min_obs, d_erase, d_erased);
+  CVB_CHECK_LAUNCH(ctx);
+  return Out.download();
 }

@@ -5,6 +5,8 @@ call: the canonical, order-independent graph include/covins_b200.h defines for c
 observation CSR of the flat bundle-adjustment problem (`lm_obs_ptr`, `obs_kf`, `obs_skip`).
 `redundant_keyframes` is the redundancy pruning of Map::Clean (map_be.cpp:745-811): the reference's sequential culling
 pass on the same CSR, reproduced exactly by parallel rounds (cvb_redundant_keyframes).
+`landmark_outliers` is the landmark outlier removal of Map::Clean (map_be.cpp:448-454, 698-743): the outlier observations and
+the landmarks left with too few good observers, on the flat bundle-adjustment problem (cvb_landmark_outliers).
 """
 from __future__ import annotations
 
@@ -74,3 +76,24 @@ def redundant_keyframes(ctx: Context, lm_obs_ptr, obs_kf, obs_octave, kf_pred, k
                                             float(th_red), float(max_time_dist), int(th_obs), int(num_octaves), p(culled),
                                             C.byref(rounds)))
     return culled, rounds.value
+
+
+def landmark_outliers(ctx: Context, p: dict, lm_valid=None, th_outlier: float = 0.92, cauchy: float = 1.0, min_obs: int = 2,
+                      want_norms: bool = False):
+    """→ (obs_outlier [n_obs] u8, lm_erase [L] u8, norms [n_obs] f64 or None): the rule include/covins_b200.h defines for
+    cvb_landmark_outliers on the flat problem `p` (the dict optimization.py takes; p["obs_skip"], when present, marks the
+    observations that do not take part).  obs_outlier is 1 for norm > th_outlier, 2 for a point the camera cannot project;
+    lm_erase marks the participating landmarks left with fewer than min_obs good observations; norms (want_norms) is the
+    loss-corrected residual norm cvb_ba_reproj_norms reports, -1 for observations that do not take part."""
+    from .optimization import _Flat
+    flat = _Flat(p, obs_skip=p.get("obs_skip"), use_imu=False)
+    valid = _opt(lm_valid, flat.L, "lm_valid")
+    obs_outlier = np.zeros(flat.n_obs, np.uint8)
+    lm_erase = np.zeros(flat.L, np.uint8)
+    norms = np.zeros(flat.n_obs) if want_norms else None
+    n_out, n_erased = C.c_int64(0), C.c_int32(0)
+    p_ = lambda a: None if a is None else a.ctypes.data
+    ctx.check(lib().cvb_landmark_outliers(ctx.handle, C.byref(flat.s), p_(valid), float(th_outlier), float(cauchy), int(min_obs),
+                                          p_(obs_outlier), p_(lm_erase), p_(norms), C.byref(n_out), C.byref(n_erased)))
+    assert n_out.value == int(np.count_nonzero(obs_outlier)) and n_erased.value == int(lm_erase.sum())
+    return obs_outlier, lm_erase, norms

@@ -1096,6 +1096,41 @@ CVB_API int cvb_redundant_keyframes(cvb_ctx* ctx, int K, int L, const int32_t* l
                                     const uint8_t* kf_protect, double th_red, double max_time_dist, int th_obs,
                                     int num_octaves, uint8_t* culled /*[K]*/, int32_t* n_rounds /*nullable*/);
 
+/*
+ * Landmark outlier removal of Map::Clean (map_be.cpp:448-454, 698-743): which observations of a map are outliers and which
+ * landmarks lose too many observers, in one call.  ASSUMPTION (parity unpinned beyond the source): the reference does not
+ * record its rule; this call defines a canonical one from behaviour the library already pins (oracle/lm_outliers.py
+ * carries the same text).  It reads only the map part of p: K, L, n_obs, n_cam, pose, cam_of_kf, extr, intr, dist,
+ * cam_model, dist_model, cam_xi, lm, lm_obs_ptr, obs_kf, obs_uv, obs_sigma, obs_skip (no speed-biases, IMU data or edges).
+ * All pointers are host memory.
+ *   1. an observation takes part iff obs_skip is NULL or 0 for it, and its landmark iff lm_valid is NULL or non-zero for it
+ *      (rule 1 of cvb_covisibility);
+ *   2. norm of a participating observation = what cvb_ba_reproj_norms reports for it at the same state with
+ *      cvb_ba_options.cauchy_reproj = cauchy, bit for bit: r = the reprojection residual of cvb_ba_problem, s = r.r,
+ *      norm = sqrt(s) * sqrt(1 / (1 + s / cauchy^2)); cauchy <= 0 gives the plain |r|.  This is the test of
+ *      optimization_be.cpp:270-290;
+ *   3. obs_outlier [n_obs] = 2 if the point is not projectable in the keyframe's camera (behind the camera, or outside the
+ *      unified model's field of view: the residual the bundle adjustment defines as zero, so its own purge never removes
+ *      the observation; this clause follows the ORB-SLAM isDepthPositive lineage and is pure assumption), else 1 if
+ *      norm > th_outlier (th_gba_outlier_global, 0.92), else 0; 0 for every observation that does not take part;
+ *   4. lm_erase [L] = 1 iff the landmark takes part and fewer than min_obs of its participating observations have
+ *      obs_outlier == 0 (min_obs 2: the bundle adjustment's own inclusion rule, optimization_be.cpp:158-171, 438-453).  A
+ *      landmark that does not take part is never erased;
+ *   5. norms [n_obs] (nullable) = the norm of each participating observation (0 for a non-projectable one), -1 for the
+ *      others, as cvb_ba_reproj_norms reports an observation outside its problem.
+ * *n_obs_outlier = the number of non-zero obs_outlier, *n_lm_erased = the number of erased landmarks.  Integer decisions on
+ * fixed-order FP64 arithmetic, no floating-point atomics: the output is bit-identical from run to run.
+ * CVB_ERR_INVALID, before any launch: a NULL required pointer, a negative size, lm_obs_ptr[0] != 0, a decreasing
+ * lm_obs_ptr or lm_obs_ptr[L] != n_obs, obs_kf outside [0, K), cam_of_kf outside [0, n_cam), an obs_sigma that is not
+ * positive and finite, th_outlier NaN or not > 0, cauchy not finite, min_obs < 1.  An unknown camera or distortion model:
+ * CVB_ERR_UNSUPPORTED with cvb_ba_create's messages.  K == 0, L == 0 or n_obs == 0: nothing to judge, nothing flagged
+ * (norms -1).
+ */
+CVB_API int cvb_landmark_outliers(cvb_ctx* ctx, const cvb_ba_problem* p, const uint8_t* lm_valid /*nullable*/,
+                                  double th_outlier, double cauchy, int min_obs,
+                                  uint8_t* obs_outlier /*[n_obs]*/, uint8_t* lm_erase /*[L]*/, double* norms /*nullable*/,
+                                  int64_t* n_obs_outlier, int32_t* n_lm_erased);
+
 #ifdef __cplusplus
 }
 #endif
