@@ -58,6 +58,7 @@ SIGNATURES = {
     "cvb_db_match_l2": (C.c_int, [c_vp, c_vp, c_vp, C.c_int, C.c_float, C.c_float, c_vp, c_vp, c_vp, c_vp, c_vp,
                                   C.c_int, C.POINTER(C.c_int32)]),
     "cvb_db_match_l2_dev": (C.c_int, [c_vp, c_vp, c_vp, C.c_int, C.c_float, C.c_float, c_vp, c_vp, c_vp, c_vp]),
+    "cvb_db_merge": (C.c_int, [c_vp, c_vp, c_vp]),
     "cvb_knn_l2_batch": (C.c_int, [c_vp, c_vp, C.c_int, c_vp, c_vp, C.c_int, C.c_int, C.c_int, c_vp, c_vp]),
     "cvb_knn_l2_u8_batch_dev": (C.c_int, [c_vp, c_vp, C.c_int, c_vp, c_vp, c_vp, C.c_int, C.c_int, C.c_int, c_vp, c_vp, c_vp]),
     "cvb_match_l2_batch": (C.c_int, [c_vp, c_vp, C.c_int, c_vp, c_vp, C.c_int, C.c_int, C.c_float, C.c_float, c_vp, c_vp, c_vp]),
@@ -118,12 +119,14 @@ SIGNATURES = {
                                              C.POINTER(C.c_int32)]),
     "cvb_db_group_match_l2": (C.c_int, [c_vp, c_vp, C.c_int, C.c_float, C.c_float, c_vp, c_vp, c_vp, c_vp, c_vp, C.c_int,
                                         C.POINTER(C.c_int32)]),
+    "cvb_db_group_merge": (C.c_int, [c_vp, c_vp]),
     "cvb_covisibility": (C.c_int, [c_vp, C.c_int, C.c_int, c_vp, c_vp, c_vp, c_vp, C.c_int, c_vp, c_vp, c_vp, C.c_int64,
                                    C.POINTER(C.c_int64)]),
     "cvb_redundant_keyframes": (C.c_int, [c_vp, C.c_int, C.c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, C.c_double,
                                           C.c_double, C.c_int, C.c_int, c_vp, C.POINTER(C.c_int32)]),
     "cvb_landmark_outliers": (C.c_int, [c_vp, c_vp, c_vp, C.c_double, C.c_double, C.c_int, c_vp, c_vp, c_vp, C.POINTER(C.c_int64),
                                         C.POINTER(C.c_int32)]),
+    "cvb_map_rigid_transform": (C.c_int, [c_vp, c_vp, C.c_int, c_vp, c_vp, C.c_int, c_vp, c_vp, c_vp]),
 }
 
 

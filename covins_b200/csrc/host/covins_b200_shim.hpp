@@ -1778,6 +1778,13 @@ class DescriptorDatabase {
     else ctx_->check(cvb_db_remove(ctx_->get(), db_, db_index), "cvb_db_remove");
     n_kf_--;
   }
+  // two agents' maps are merged (MergeMaps): other's keyframes follow this database's, in other's order, copied in HBM
+  // (cvb_db_merge / cvb_db_group_merge); other is left unchanged.  Both of one kind, on one Context or one ContextGroup.
+  void Merge(const DescriptorDatabase& other) {
+    if (gdb_) ctx_->check(other.gdb_ ? cvb_db_group_merge(gdb_, other.gdb_) : CVB_ERR_INVALID, "cvb_db_group_merge");
+    else ctx_->check(other.db_ ? cvb_db_merge(ctx_->get(), db_, other.db_) : CVB_ERR_INVALID, "cvb_db_merge");
+    n_kf_ += other.n_kf_;
+  }
   // knnMatch(k=2) + distance/ratio filter of the query keyframe against EVERY keyframe of the database:
   // result[db index] == the reference's img_matches for that candidate (accepted queries ascending, :102-114)
   std::vector<Matches> MatchAll(const uint8_t* query, int n_query, const OptParams& P) {
@@ -1838,6 +1845,63 @@ inline std::vector<int> ComputeLandmarkDescriptors(Context& ctx, const std::vect
   std::vector<int32_t> best(n_lm > 0 ? n_lm : 1);
   ctx.check(cvb_landmark_descriptor_batch(ctx.get(), rows.data(), ptr.data(), n_lm, best.data(), out_desc), "cvb_landmark_descriptor_batch");
   return std::vector<int>(best.begin(), best.begin() + n_lm);
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// The merge constructor Map(map_target, map_tofuse, T_wtarget_wtofuse) (map_be.cpp:334-381), reached from
+// MapManager::PerformMerge (map_be.cpp:192-244): the fused map's valid keyframes (T_ws, velocity) and valid landmarks
+// (position) moved into the target's world frame by one cvb_map_rigid_transform call (the rule and its assumptions are in
+// include/covins_b200.h), written back keyframes first (SetPoseTws, SetStateVelocity), then landmarks (SetWorldPos), as the
+// constructor's loop does.  Then the union, on map_target, which becomes the merged map: every keyframe, landmark and loop
+// constraint of map_tofuse through map_target->AddKeyframe / AddLandmark / AddLoopConstraint (ids are kept: two agents'
+// ids do not collide).  With both databases given, db_tofuse's keyframes join db_target in HBM (their database indices
+// shift by db_target's size before the call; db_tofuse is left unchanged).  Last, the merged map's covisibility graph.
+// map_target's own keyframes and landmarks are not touched before the union.
+// ---------------------------------------------------------------------------------------------------------------
+template <class MapPtr, class Transform4>
+void MergeMaps(Context& ctx, MapPtr map_target, MapPtr map_tofuse, const Transform4& T_wtarget_wtofuse, DescriptorDatabase* db_target = nullptr,
+               DescriptorDatabase* db_tofuse = nullptr) {
+  using KeyframePtr = typename std::decay<decltype(map_tofuse->GetKeyframesVec()[0])>::type;
+  using KF = typename KeyframePtr::element_type;
+  const auto keyframes = map_tofuse->GetKeyframesVec();
+  const auto landmarks = map_tofuse->GetLandmarksVec();
+  using LandmarkPtr = typename std::decay<decltype(landmarks[0])>::type;
+  std::map<const KF*, int> kf_index;
+  std::vector<KeyframePtr> kfs;
+  detail::canonical_keyframes(keyframes, kf_index, kfs);
+  std::vector<LandmarkPtr> lms;
+  for (auto& lm : landmarks)
+    if (!lm->IsInvalid()) lms.push_back(lm);
+  const int K = (int)kfs.size(), L = (int)lms.size();
+  double T[16];
+  for (int r = 0; r < 4; r++)
+    for (int c = 0; c < 4; c++) T[4 * r + c] = T_wtarget_wtofuse(r, c);
+  std::vector<double> ws(16 * (size_t)K + 1), vel(3 * (size_t)K + 1), pos(3 * (size_t)L + 1);
+  for (int k = 0; k < K; k++) {
+    const auto Tws = kfs[k]->GetPoseTws();
+    for (int r = 0; r < 4; r++)
+      for (int c = 0; c < 4; c++) ws[16 * (size_t)k + 4 * r + c] = Tws(r, c);
+    const auto v = kfs[k]->GetStateVelocity();
+    for (int i = 0; i < 3; i++) vel[3 * (size_t)k + i] = v[i];
+  }
+  for (int l = 0; l < L; l++) {
+    const auto p = lms[l]->GetWorldPos();
+    for (int i = 0; i < 3; i++) pos[3 * (size_t)l + i] = p[i];
+  }
+  ctx.check(cvb_map_rigid_transform(ctx.get(), T, K, ws.data(), vel.data(), L, pos.data(), nullptr, nullptr), "cvb_map_rigid_transform");
+  for (int k = 0; k < K; k++) {
+    auto Tws = kfs[k]->GetPoseTws();
+    for (int r = 0; r < 4; r++)
+      for (int c = 0; c < 4; c++) Tws(r, c) = ws[16 * (size_t)k + 4 * r + c];
+    kfs[k]->SetPoseTws(Tws);
+    kfs[k]->SetStateVelocity({vel[3 * (size_t)k], vel[3 * (size_t)k + 1], vel[3 * (size_t)k + 2]});
+  }
+  for (int l = 0; l < L; l++) lms[l]->SetWorldPos({pos[3 * (size_t)l], pos[3 * (size_t)l + 1], pos[3 * (size_t)l + 2]});
+  for (auto& kf : keyframes) map_target->AddKeyframe(kf);
+  for (auto& lm : landmarks) map_target->AddLandmark(lm);
+  for (const auto& lc : map_tofuse->GetLoopConstraints()) map_target->AddLoopConstraint(lc);
+  if (db_target && db_tofuse) db_target->Merge(*db_tofuse);
+  UpdateCovisibilityConnections(ctx, map_target);
 }
 
 }  // namespace covins_b200

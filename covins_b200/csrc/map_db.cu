@@ -26,6 +26,7 @@ struct cvb_buf {
 };
 
 struct cvb_db {
+  const cvb_ctx* owner = nullptr;   // the ctx of cvb_db_create: the device the rows live on
   int desc_bytes = 32;   // 32: ORB rows (Hamming); 128: SIFT rows as exact u8 (L2)
   uint8_t* d_rows = nullptr;
   size_t cap_rows = 0;
@@ -298,6 +299,7 @@ int cvb_db_create(cvb_ctx* ctx, int desc_bytes, cvb_db** out) {
   if (desc_bytes != 32 && desc_bytes != 128)
     return cvb_fail(ctx, CVB_ERR_UNSUPPORTED, "descriptor database: 32-byte ORB or 128-byte SIFT descriptors, got %d", desc_bytes);
   cvb_db* db = new cvb_db();
+  db->owner = ctx;
   db->desc_bytes = desc_bytes;
   *out = db;
   return CVB_OK;
@@ -438,6 +440,40 @@ int cvb_db_match_l2(cvb_ctx* ctx, cvb_db* db, const float* q, int nq, float thr,
   CVB_GUARD(ctx);
   if (const int rc = require_kind(ctx, db, true, "cvb_db_match_l2")) return rc;
   return match_host(ctx, db, q, nq, thr, ratio, n_matches, m_kf, m_query, m_train, m_dist, cap, n_total, "cvb_db_match_l2");
+}
+
+// src's rows and operand tiles are copied behind dst's: an operand tile is a function of its keyframe's rows alone (the
+// key's column is the row within the tile, expand_tiles_kernel), so the copies equal what appending the rows would expand
+int cvb_db_merge(cvb_ctx* ctx, cvb_db* dst, const cvb_db* src) {
+  if (!ctx || !dst || !src) return CVB_ERR_INVALID;
+  CVB_GUARD(ctx);
+  CVB_REQUIRE(ctx, dst != src, "cvb_db_merge: dst and src are the same database");
+  CVB_REQUIRE(ctx, dst->desc_bytes == src->desc_bytes, "cvb_db_merge: dst holds %s descriptors, src %s", dst->desc_bytes == 128 ? "SIFT" : "ORB",
+              src->desc_bytes == 128 ? "SIFT" : "ORB");
+  if (dst->owner != ctx || src->owner != ctx)
+    return cvb_fail(ctx, CVB_ERR_UNSUPPORTED, "cvb_db_merge: the %s database was created on another context (device %d); merge databases of one "
+                    "context", dst->owner != ctx ? "dst" : "src", (dst->owner != ctx ? dst->owner : src->owner)->device);
+  const int64_t have = dst->seg_ptr.back(), add = src->seg_ptr.back();
+  CVB_REQUIRE(ctx, have + add < (int64_t)1 << 31, "cvb_db_merge: more than 2^31 rows");
+  if ((size_t)(have + add) > dst->cap_rows) {
+    const int rc = cvb_db_reserve(ctx, dst, std::max<int64_t>(have + add, (int64_t)(dst->cap_rows * 3 / 2)));
+    if (rc) return rc;
+  }
+  const int tile_old = dst->seg_tile.back(), tiles = src->seg_tile.back();
+  if (const int rc = reserve_tiles(ctx, dst, (size_t)tile_old + tiles, (size_t)tile_old)) return rc;
+  cudaStream_t st = ctx->stream;
+  if (add)
+    CVB_CUDA(ctx, cudaMemcpyAsync(dst->d_rows + (size_t)have * dst->desc_bytes, src->d_rows, (size_t)add * dst->desc_bytes,
+                                  cudaMemcpyDeviceToDevice, st));
+  const size_t tb = cvb_tc::tile_bytes(dst->metric());
+  if (tiles) CVB_CUDA(ctx, cudaMemcpyAsync(dst->d_xt + (size_t)tile_old * tb, src->d_xt, (size_t)tiles * tb, cudaMemcpyDeviceToDevice, st));
+  for (size_t i = 1; i < src->seg_ptr.size(); i++) {
+    dst->seg_ptr.push_back((int32_t)have + src->seg_ptr[i]);
+    dst->seg_tile.push_back(tile_old + src->seg_tile[i]);
+  }
+  dst->seg_dirty = true;
+  CVB_CUDA(ctx, cudaStreamSynchronize(st));
+  return CVB_OK;
 }
 
 }  // extern "C"
@@ -808,6 +844,31 @@ int cvb_db_group_match_l2(cvb_db_group* db, const float* q, int nq, float thr, f
   std::lock_guard<std::recursive_mutex> lk(db->g->call_mtx);
   CVB_GUARD(db->g->ctx[0]);
   return group_match(db, true, q, nq, thr, ratio, n_matches, m_kf, m_query, m_train, m_dist, cap, n_total, "cvb_db_group_match_l2");
+}
+
+// Rank r's share of src follows its share of dst, so every rank still holds its keyframes in global order
+int cvb_db_group_merge(cvb_db_group* dst, const cvb_db_group* src) {
+  if (!dst || !src) return CVB_ERR_INVALID;
+  std::lock_guard<std::recursive_mutex> lk(dst->g->call_mtx);
+  cvb_group* g = dst->g;
+  cvb_ctx* c0 = g->ctx[0];
+  CVB_REQUIRE(c0, dst != src, "cvb_db_group_merge: dst and src are the same database");
+  CVB_REQUIRE(c0, dst->desc_bytes == src->desc_bytes, "cvb_db_group_merge: dst holds %s descriptors, src %s",
+              dst->desc_bytes == 128 ? "SIFT" : "ORB", src->desc_bytes == 128 ? "SIFT" : "ORB");
+  if (src->g != g) return cvb_fail(c0, CVB_ERR_UNSUPPORTED, "cvb_db_group_merge: src is on another group; merge databases of one group");
+  int64_t all = 0;
+  for (int r = 0; r < g->n; r++) all += dst->rows[r] + src->rows[r];
+  CVB_REQUIRE(c0, all < (int64_t)1 << 31, "cvb_db_group_merge: more than 2^31 rows");
+  int base[CVB_GROUP_MAX];
+  for (int r = 0; r < g->n; r++) {
+    base[r] = (int)dst->db[r]->seg_ptr.size() - 1;
+    if (src->db[r]->seg_ptr.size() == 1) continue;
+    if (const int rc = cvb_db_merge(g->ctx[r], dst->db[r], src->db[r])) return rank_fail(dst, r, rc);
+    dst->rows[r] += src->rows[r];
+  }
+  for (const int2 rl : src->loc) dst->loc.push_back(make_int2(rl.x, base[rl.x] + rl.y));
+  dst->loc_dirty = true;
+  return CVB_OK;
 }
 
 }  // extern "C"

@@ -7,6 +7,8 @@ observation CSR of the flat bundle-adjustment problem (`lm_obs_ptr`, `obs_kf`, `
 pass on the same CSR, reproduced exactly by parallel rounds (cvb_redundant_keyframes).
 `landmark_outliers` is the landmark outlier removal of Map::Clean (map_be.cpp:448-454, 698-743): the outlier observations and
 the landmarks left with too few good observers, on the flat bundle-adjustment problem (cvb_landmark_outliers).
+`rigid_transform` is the transform loop of the merge constructor Map(map_target, map_tofuse, T) (map_be.cpp:365-380): the
+fused map's keyframe poses, velocities and landmark positions moved into the target's world frame (cvb_map_rigid_transform).
 """
 from __future__ import annotations
 
@@ -97,3 +99,37 @@ def landmark_outliers(ctx: Context, p: dict, lm_valid=None, th_outlier: float = 
                                           p_(obs_outlier), p_(lm_erase), p_(norms), C.byref(n_out), C.byref(n_erased)))
     assert n_out.value == int(np.count_nonzero(obs_outlier)) and n_erased.value == int(lm_erase.sum())
     return obs_outlier, lm_erase, norms
+
+
+def is_rigid(T) -> bool:
+    """cvb_map_rigid_transform's test of T: finite entries, last row exactly [0 0 0 1], every entry of R^T R within 1e-9 of
+    I and det R > 0"""
+    T = np.asarray(T, np.float64)
+    if T.shape != (4, 4) or not np.isfinite(T).all() or T[3].tolist() != [0.0, 0.0, 0.0, 1.0]:
+        return False
+    R = T[:3, :3].tolist()
+    for a in range(3):
+        for b in range(3):
+            if not abs((R[0][a] * R[0][b] + R[1][a] * R[1][b]) + R[2][a] * R[2][b] - (1.0 if a == b else 0.0)) <= 1e-9:
+                return False
+    return (R[0][0] * (R[1][1] * R[2][2] - R[1][2] * R[2][1]) - R[0][1] * (R[1][0] * R[2][2] - R[1][2] * R[2][0])) \
+        + R[0][2] * (R[1][0] * R[2][1] - R[1][1] * R[2][0]) > 0.0
+
+
+def rigid_transform(ctx: Context, T, T_ws, vel=None, lm_pos=None, kf_sel=None, lm_sel=None):
+    """→ (T_ws' [K,4,4], vel' [K,3] or None, lm_pos' [L,3]): the fused map's keyframe poses T_ws [K,4,4] (or [K,16],
+    row-major), velocities vel [K,3] (optional) and landmark positions lm_pos [L,3] moved by T = T_wtarget_wtofuse
+    [4,4]: T_ws <- T T_ws, v <- R v, p <- R p + t, for the entries kf_sel [K] / lm_sel [L] select (all when None), the
+    others returned unchanged.  The inputs are not modified.  A T that is not rigid raises ValueError before any device
+    work."""
+    T = np.ascontiguousarray(T, np.float64)
+    if not is_rigid(T):
+        raise ValueError("T is not rigid (finite entries, R^T R = I within 1e-9, det R > 0, last row [0 0 0 1])")
+    ws = np.array(T_ws, np.float64, order="C").reshape(-1, 16)
+    K = len(ws)
+    v = None if vel is None else np.array(vel, np.float64, order="C").reshape(K, 3)
+    p = np.array(lm_pos if lm_pos is not None else np.zeros((0, 3)), np.float64, order="C").reshape(-1, 3)
+    ks, ls = _opt(kf_sel, K, "kf_sel"), _opt(lm_sel, len(p), "lm_sel")
+    p_ = lambda a: None if a is None else a.ctypes.data
+    ctx.check(lib().cvb_map_rigid_transform(ctx.handle, T.ctypes.data, K, p_(ws), p_(v), len(p), p_(p), p_(ks), p_(ls)))
+    return ws.reshape(K, 4, 4), v, p

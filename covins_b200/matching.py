@@ -129,6 +129,12 @@ class DescriptorDatabase:
         """a keyframe leaves the map (culling / erase): later keyframes move down by one index"""
         self.ctx.check(lib().cvb_db_remove(self.ctx.handle, self.handle, int(kf_index)))
 
+    def merge(self, other: "DescriptorDatabase"):
+        """two agents' maps are merged: other's keyframes are appended after this database's, in other's order, copied
+        device to device (cvb_db_merge; no descriptor crosses PCIe).  other is left unchanged.  Both must be of one kind and
+        on one Context."""
+        self.ctx.check(lib().cvb_db_merge(self.ctx.handle, self.handle, other.handle))
+
     def size(self):
         import ctypes as C
         n_kf, n_rows = C.c_int32(), C.c_int64()
@@ -223,6 +229,11 @@ class DescriptorDatabaseGroup:
     def remove(self, kf_index: int):
         """a keyframe leaves the map: later keyframes move down by one global index"""
         self.ctx.check(lib().cvb_db_group_remove(self.handle, int(kf_index)))
+
+    def merge(self, other: "DescriptorDatabaseGroup"):
+        """as DescriptorDatabase.merge, rank by rank on the group's devices (cvb_db_group_merge): other's keyframes follow
+        this database's in global order, each staying on the rank that holds it.  Both must be on one Group."""
+        self.ctx.check(lib().cvb_db_group_merge(self.handle, other.handle))
 
     def size(self):
         """→ (n_kf, n_rows)"""

@@ -148,6 +148,19 @@ CVB_API int cvb_db_match_l2(cvb_ctx* ctx, cvb_db* db, const float* q, int nq, fl
                             float* m_dist, int cap, int32_t* n_total);
 CVB_API int cvb_db_match_l2_dev(cvb_ctx* ctx, cvb_db* db, const uint8_t* d_q, int nq, float thr, float ratio,
                                 int32_t* d_match_train, float* d_match_dist, int32_t* d_n_matches, void* stream);
+/*
+ * Two agents' maps are merged (MapManager::PerformMerge, map_be.cpp:192-244): the fused map's keyframes join the target's
+ * database without leaving HBM.  src's keyframes are appended after dst's, in src's order; src is left unchanged.  Every
+ * later request (cvb_db_match_hamming / _l2 and their _dev forms), cvb_db_size, cvb_db_remove and append on dst is
+ * bit-identical to that of a database that received dst's keyframes and then src's from the host.  A tile image depends
+ * only on the rows of its keyframe (the key's column is the row within the tile), so src's rows and operand tiles are
+ * copied device to device on ctx's stream and the segment tables rebased: no descriptor byte crosses PCIe and nothing is
+ * launched.  dst grows through the same reservation as an append.
+ * Refusals, before any device work and with dst unchanged: dst == src or databases of different row kinds ->
+ * CVB_ERR_INVALID; a database created on another ctx (so possibly another device) -> CVB_ERR_UNSUPPORTED; more than 2^31
+ * rows together -> CVB_ERR_INVALID.
+ */
+CVB_API int cvb_db_merge(cvb_ctx* ctx, cvb_db* dst, const cvb_db* src);
 
 /*
  * Replaces the SIFT branch, cv::FlannBasedMatcher()::knnMatch(query, train, out, 2)
@@ -1039,6 +1052,16 @@ CVB_API int cvb_db_group_match_hamming(cvb_db_group* db, const uint8_t* q, int n
                                        int32_t* m_kf, int32_t* m_query, int32_t* m_train, float* m_dist, int cap, int32_t* n_total);
 CVB_API int cvb_db_group_match_l2(cvb_db_group* db, const float* q, int nq, float thr, float ratio, int32_t* n_matches,
                                   int32_t* m_kf, int32_t* m_query, int32_t* m_train, float* m_dist, int cap, int32_t* n_total);
+/*
+ * cvb_db_merge for two databases of the same group: each rank merges src's share into dst's share on its own device
+ * (keyframes never move between devices), and the global -> (rank, local index) table takes src's entries after dst's.
+ * The outputs are placement-independent, so the merged database is bit-identical to one cvb_db that received dst's
+ * keyframes and then src's.  Later appends follow the fewest-rows rule from the merged state (each rank's rows are the
+ * sum of both shares).  Refusals before any rank is touched: dst == src or different row kinds -> CVB_ERR_INVALID; another
+ * group -> CVB_ERR_UNSUPPORTED; more than 2^31 rows together -> CVB_ERR_INVALID.  A CUDA failure is reported as
+ * "rank r: <message>" on ctxs[0] and leaves dst undefined.
+ */
+CVB_API int cvb_db_group_merge(cvb_db_group* dst, const cvb_db_group* src);
 
 /* ------------------------------------------------------------------------------------------------
  * Map maintenance (SURVEY.md §8f rank 4)
@@ -1130,6 +1153,32 @@ CVB_API int cvb_landmark_outliers(cvb_ctx* ctx, const cvb_ba_problem* p, const u
                                   double th_outlier, double cauchy, int min_obs,
                                   uint8_t* obs_outlier /*[n_obs]*/, uint8_t* lm_erase /*[L]*/, double* norms /*nullable*/,
                                   int64_t* n_obs_outlier, int32_t* n_lm_erased);
+
+/*
+ * The rigid transform of the merge constructor Map(map_target, map_tofuse, T) (map_be.cpp:334-381, the loop at :365-380),
+ * reached from MapManager::PerformMerge (map_be.cpp:192-244): the fused map's keyframes and landmarks moved into the
+ * target map's world frame in one call.  T = T_wtarget_wtofuse, row-major 4x4 [R t; 0 0 0 1].  All pointers are host memory.
+ *   keyframe k (selected iff kf_sel is NULL or kf_sel[k] != 0): T_ws[k] <- T * T_ws[k] (all 16 entries, row-major [K][16]),
+ *     vel[k] <- R * vel[k] (vel [K][3], nullable: then no velocity is touched);
+ *   landmark l (selected iff lm_sel is NULL or lm_sel[l] != 0): lm_pos[l] <- R * lm_pos[l] + t;
+ *   unselected entries are left bit for bit as they were.
+ * Every output entry is its products summed left to right without fused multiply-add: (T[r][0] X[0][c] + T[r][1] X[1][c])
+ * + T[r][2] X[2][c] + T[r][3] X[3][c] for a pose, ((R[r][0] v0 + R[r][1] v1) + R[r][2] v2) (+ t[r]) for a velocity and a
+ * position, so a float64 restatement in the same order (oracle/merge.py) gives the same bits.  Poses stay 4x4 matrices
+ * as the containers hold them: a quaternion round trip would add rounding the reference does not have.
+ * ASSUMPTIONS (the merge constructor is not in this tree; the rule is restated from SURVEY.md's citations, and
+ * oracle/merge.py carries the same text): the fused map's T_ws and velocity are transformed and its IMU biases are not;
+ * T_ws_vio_ is left unchanged (the pose graph reads it only as relative transforms between keyframes of one agent,
+ * opt.cpp:947-1021, which a common left factor does not change); landmark positions are transformed.  Loop constraints,
+ * ids and the union of the two maps are host container work (covins_b200::MergeMaps).
+ * One launch whatever the map's size, a grid-stride over K + L, with one upload and one download per array.
+ * CVB_ERR_INVALID, before any launch: T not rigid (an entry not finite, |R^T R - I| > 1e-9 in any entry, det R <= 0, or a
+ * last row other than [0 0 0 1]), a negative size, a NULL T, or a NULL T_ws / lm_pos with K / L > 0.  K + L == 0: nothing
+ * to do, no launch.
+ */
+CVB_API int cvb_map_rigid_transform(cvb_ctx* ctx, const double T[16], int K, double* T_ws /*[K][16] in/out*/,
+                                    double* vel /*[K][3] in/out, nullable*/, int L, double* lm_pos /*[L][3] in/out*/,
+                                    const uint8_t* kf_sel /*[K], nullable*/, const uint8_t* lm_sel /*[L], nullable*/);
 
 #ifdef __cplusplus
 }
