@@ -127,6 +127,7 @@ SIGNATURES = {
     "cvb_landmark_outliers": (C.c_int, [c_vp, c_vp, c_vp, C.c_double, C.c_double, C.c_int, c_vp, c_vp, c_vp, C.POINTER(C.c_int64),
                                         C.POINTER(C.c_int32)]),
     "cvb_map_rigid_transform": (C.c_int, [c_vp, c_vp, C.c_int, c_vp, c_vp, C.c_int, c_vp, c_vp, c_vp]),
+    "cvb_pgo": (C.c_int, [c_vp, c_vp, c_vp, c_vp]),
 }
 
 

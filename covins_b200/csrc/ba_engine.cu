@@ -1343,7 +1343,9 @@ int check_problem(cvb_ctx* ctx, const cvb_ba_problem* p, int visual_only) {
   return CVB_OK;
 }
 
-int engine_setup(Engine& E, const cvb_ba_problem* p, const cvb_ba_options* o) {
+// fill (cvb_ba_solve_dev_edges, single rank only): the start poses and edge measurements are written on the device by
+// fill(pose[0], pose0, edge_q, edge_t, edge_S) instead of uploaded from p->pose / edge_q / edge_t / edge_sqrt_info
+int engine_setup(Engine& E, const cvb_ba_problem* p, const cvb_ba_options* o, const cvb_dev_edges_fill* fill = nullptr) {
   cvb_ctx* ctx = E.ctx;
   const bool trace = getenv("COVINS_B200_SETUP_TRACE") != nullptr;   // development aid: host-side phase times to stderr
   auto t_prev = std::chrono::steady_clock::now();
@@ -1643,7 +1645,11 @@ int engine_setup(Engine& E, const cvb_ba_problem* p, const cvb_ba_options* o) {
   lap("factor lists");
   // ---- uploads ----
   E.h_const.assign(p->pose_const, p->pose_const + K);
-  if ((rc = upload(E, E.pose[0], p->pose, (size_t)7 * K))) return rc;
+  if (fill) {
+    if (E.pose[0].alloc((size_t)7 * K) || E.pose0.alloc((size_t)7 * K)) return cvb_fail(ctx, CVB_ERR_CUDA, "cudaMalloc failed (poses)");
+  } else if ((rc = upload(E, E.pose[0], p->pose, (size_t)7 * K))) {
+    return rc;
+  }
   if ((rc = zalloc(E, E.pose[1], (size_t)7 * K))) return rc;
   std::vector<double> h_sb((size_t)9 * K, 0.0);
   if (p->speedbias) std::memcpy(h_sb.data(), p->speedbias, sizeof(double) * 9 * K);
@@ -1651,7 +1657,7 @@ int engine_setup(Engine& E, const cvb_ba_problem* p, const cvb_ba_options* o) {
   if ((rc = zalloc(E, E.sb[1], (size_t)9 * K))) return rc;
   if ((rc = upload(E, E.lm[0], h_lm))) return rc;
   if ((rc = zalloc(E, E.lm[1], (size_t)3 * E.L_in))) return rc;
-  if ((rc = upload(E, E.pose0, p->pose, (size_t)7 * K)) || (rc = upload(E, E.sb0, h_sb)) || (rc = upload(E, E.lm0, h_lm))) return rc;
+  if ((!fill && (rc = upload(E, E.pose0, p->pose, (size_t)7 * K))) || (rc = upload(E, E.sb0, h_sb)) || (rc = upload(E, E.lm0, h_lm))) return rc;
   if ((rc = upload(E, E.pose_const, p->pose_const, (size_t)K))) return rc;
   cvb_kf_cameras cams;
   if ((rc = cvb_stage_kf_cameras(ctx, p, cams))) return rc;
@@ -1673,7 +1679,16 @@ int engine_setup(Engine& E, const cvb_ba_problem* p, const cvb_ba_options* o) {
       (rc = upload(E, E.ft_rlo, h_ft_rlo)))
     return rc;
   // edges
-  {
+  if (fill) {
+    CVB_REQUIRE(ctx, E.world == 1, "device-written edges need a single rank");
+    std::vector<uint8_t> rb(E.n_edge);
+    for (int e = 0; e < E.n_edge; e++) rb[e] = p->edge_robust ? p->edge_robust[e] : 0;
+    if ((rc = upload(E, E.edge_i, h_edge_i)) || (rc = upload(E, E.edge_j, h_edge_j)) || (rc = upload(E, E.edge_robust, rb))) return rc;
+    if (E.edge_q.alloc((size_t)4 * E.n_edge) || E.edge_t.alloc((size_t)3 * E.n_edge) || E.edge_S.alloc((size_t)36 * E.n_edge))
+      return cvb_fail(ctx, CVB_ERR_CUDA, "cudaMalloc failed (edges)");
+    if ((rc = (*fill)(E.pose[0].p, E.pose0.p, E.edge_q.p, E.edge_t.p, E.edge_S.p))) return rc;
+    if ((rc = zalloc(E, E.Jedge, (size_t)72 * E.n_edge)) || (rc = zalloc(E, E.redge, (size_t)6 * E.n_edge))) return rc;
+  } else {
     std::vector<double> q((size_t)4 * E.n_edge), t((size_t)3 * E.n_edge), S((size_t)36 * E.n_edge);
     std::vector<uint8_t> rb(E.n_edge);
     for (int e = 0; e < E.n_edge; e++) {
@@ -2508,6 +2523,25 @@ int cvb_ba_solve(cvb_ctx* ctx, const cvb_ba_problem* p, const cvb_ba_options* o,
 }
 
 }  // extern "C"
+
+int cvb_ba_solve_dev_edges(cvb_ctx* ctx, const cvb_ba_problem* p, const cvb_ba_options* o, cvb_ba_result* r, const cvb_dev_edges_fill& fill,
+                           const std::function<int(const double* d_pose)>& finish) {
+  cvb_ba* h = new cvb_ba();
+  h->E.ctx = ctx;
+  h->E.st = ctx->stream;
+  BaEnter enter(h);
+  h->prob_copy = *p;
+  Engine& E = h->E;
+  int rc = engine_setup(E, p, o, &fill);
+  if (!rc) rc = engine_begin(E);
+  bool done = false;
+  for (int n = 0; !rc && !done && n < o->max_iterations; n++) rc = engine_iterate(E, &done);
+  if (!rc) rc = finish(E.pose[E.cur].p);
+  if (!rc) rc = engine_download(E, p, r);
+  cudaStreamSynchronize(E.st);
+  delete h;
+  return rc;
+}
 
 namespace {
 

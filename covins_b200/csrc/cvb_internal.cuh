@@ -6,6 +6,7 @@
 #include <stdio.h>
 #include <string.h>
 #include <atomic>
+#include <functional>
 #include <mutex>
 #include <string>
 #include <vector>
@@ -151,6 +152,16 @@ int cvb_relpose_batch_dev(cvb_ctx* ctx, const cvb_relpose_dev* d_probs, int n_pr
 int cvb_covisibility_budgeted(cvb_ctx* ctx, int K, int L, const int32_t* lm_obs_ptr, const int32_t* obs_kf, const uint8_t* obs_skip,
                               const uint8_t* lm_valid, int min_weight, int32_t* nbr_ptr, int32_t* nbr_kf, int32_t* nbr_w, int64_t cap,
                               int64_t* n_total, int64_t pair_budget);
+
+// ba_engine.cu: cvb_ba_solve for cvb_pgo (pgo.cu), one rank, on a problem whose start poses and edge measurements are made
+// on the device.  p->pose, edge_q, edge_t and edge_sqrt_info are not read: fill(pose, pose0, edge_q, edge_t, edge_S) enqueues
+// on ctx->stream the work that writes the start poses [K][7] (into both of the engine's copies) and the measurements
+// [n_edge][4], [3], [36] straight into the engine's arrays; the topology (edge_i, edge_j, edge_robust) is read from p as
+// cvb_ba_solve reads it.  After the iterations finish(pose) enqueues work that reads the solved poses [K][7] on the device,
+// then r is filled as cvb_ba_result_get fills it.
+using cvb_dev_edges_fill = std::function<int(double* pose, double* pose0, double* edge_q, double* edge_t, double* edge_S)>;
+int cvb_ba_solve_dev_edges(cvb_ctx* ctx, const cvb_ba_problem* p, const cvb_ba_options* o, cvb_ba_result* r, const cvb_dev_edges_fill& fill,
+                           const std::function<int(const double* d_pose)>& finish);
 
 // Every keyframe's camera as the reprojection kernels read it (bam::reproj): the extr [K][7], intr [K][4] and
 // dist [K][4] of its calibration cam_of_kf[k], model = camera | distortion << 8, xi (0 for a pinhole camera).  The bundle

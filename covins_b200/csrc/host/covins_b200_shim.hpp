@@ -35,6 +35,7 @@
 #include <vector>
 
 #include "../../../include/covins_b200.h"
+#include "../../../include/covins_b200_pose.h"
 
 namespace covins_b200 {
 
@@ -120,111 +121,33 @@ struct Adapter {
 
 namespace detail {
 
-// rotation matrix (via operator()(r,c) of a 4x4 transform) → quaternion (x,y,z,w), the convention of
-// Eigen::Quaterniond(R) used at keyframe_base.cpp:490-499 (w >= 0 branch of Eigen's algorithm)
+// The pose conversions on the containers' 4x4 transforms (operator()(r,c)), through the one implementation the kernels use
+// too (include/covins_b200_pose.h): transform_to_pose7 is Eigen::Quaterniond(R) as keyframe_base.cpp:490-499 uses it,
+// pose7_to_transform is Utils::Ceres2Transform (utils_base.cpp:28-43).
 template <class T4>
-inline void transform_to_pose7(const T4& T, double* out) {
-  const double m00 = T(0, 0), m11 = T(1, 1), m22 = T(2, 2);
-  double q[4];  // x y z w
-  const double tr = m00 + m11 + m22;
-  if (tr > 0) {
-    double t = std::sqrt(tr + 1.0);
-    q[3] = 0.5 * t;
-    t = 0.5 / t;
-    q[0] = (T(2, 1) - T(1, 2)) * t;
-    q[1] = (T(0, 2) - T(2, 0)) * t;
-    q[2] = (T(1, 0) - T(0, 1)) * t;
-  } else {
-    int i = 0;
-    if (m11 > m00) i = 1;
-    if (m22 > T(i, i)) i = 2;
-    const int j = (i + 1) % 3, k = (j + 1) % 3;
-    double t = std::sqrt(T(i, i) - T(j, j) - T(k, k) + 1.0);
-    q[i] = 0.5 * t;
-    t = 0.5 / t;
-    q[3] = (T(k, j) - T(j, k)) * t;
-    q[j] = (T(j, i) + T(i, j)) * t;
-    q[k] = (T(k, i) + T(i, k)) * t;
-  }
-  out[0] = q[0]; out[1] = q[1]; out[2] = q[2]; out[3] = q[3];
-  out[4] = T(0, 3); out[5] = T(1, 3); out[6] = T(2, 3);
+inline void to_rowmajor(const T4& T, double* m) {
+  for (int r = 0; r < 4; r++)
+    for (int c = 0; c < 4; c++) m[4 * r + c] = T(r, c);
 }
-
-// Utils::Ceres2Transform (covins_comm/src/covins_base/utils_base.cpp:28-43): normalised quaternion → 4x4
 template <class T4>
-inline T4 pose7_to_transform(const double* p) {
-  double x = p[0], y = p[1], z = p[2], w = p[3];
-  const double n = 1.0 / std::sqrt(x * x + y * y + z * z + w * w);
-  x *= n; y *= n; z *= n; w *= n;
+inline T4 from_rowmajor(const double* m) {
   T4 T = T4::Identity();
-  T(0, 0) = 1 - 2 * (y * y + z * z); T(0, 1) = 2 * (x * y - z * w); T(0, 2) = 2 * (x * z + y * w);
-  T(1, 0) = 2 * (x * y + z * w); T(1, 1) = 1 - 2 * (x * x + z * z); T(1, 2) = 2 * (y * z - x * w);
-  T(2, 0) = 2 * (x * z - y * w); T(2, 1) = 2 * (y * z + x * w); T(2, 2) = 1 - 2 * (x * x + y * y);
-  T(0, 3) = p[4]; T(1, 3) = p[5]; T(2, 3) = p[6];
+  for (int r = 0; r < 3; r++)
+    for (int c = 0; c < 4; c++) T(r, c) = m[4 * r + c];
   return T;
 }
-
 template <class T4>
-inline T4 rel_transform(const T4& Ta, const T4& Tb) {  // Ta^-1 * Tb for rigid transforms
-  T4 R = T4::Identity();
-  for (int r = 0; r < 3; r++)
-    for (int c = 0; c < 3; c++) {
-      double s = 0;
-      for (int m = 0; m < 3; m++) s += Ta(m, r) * Tb(m, c);
-      R(r, c) = s;
-    }
-  for (int r = 0; r < 3; r++) {
-    double s = 0;
-    for (int m = 0; m < 3; m++) s += Ta(m, r) * (Tb(m, 3) - Ta(m, 3));
-    R(r, 3) = s;
-  }
-  return R;
+inline void transform_to_pose7(const T4& T, double* out) {
+  double m[16];
+  to_rowmajor(T, m);
+  cvb_pose::transform_to_pose7(m, out);
 }
-
-// lower Cholesky of a symmetric 6x6, transposed: LLT(cov^-1).matrixL().transpose() (optimization_be.cpp:922-923)
-inline bool sqrt_info_from_cov(const double* cov /*36 row-major*/, double* out /*36*/) {
-  // invert via Cholesky of cov, then Cholesky of the inverse
-  double L[36] = {0}, X[36] = {0}, P[36];
-  for (int c = 0; c < 6; c++)
-    for (int r = c; r < 6; r++) {
-      double s = cov[6 * r + c];
-      for (int m = 0; m < c; m++) s -= L[6 * r + m] * L[6 * c + m];
-      if (r == c) {
-        if (!(s > 0)) return false;
-        L[6 * c + c] = std::sqrt(s);
-      } else {
-        L[6 * r + c] = s / L[6 * c + c];
-      }
-    }
-  for (int c = 0; c < 6; c++)
-    for (int r = c; r < 6; r++) {
-      double s = (r == c) ? 1.0 : 0.0;
-      for (int m = c; m < r; m++) s -= L[6 * r + m] * X[6 * m + c];
-      X[6 * r + c] = s / L[6 * r + r];
-    }
-  for (int r = 0; r < 6; r++)
-    for (int c = 0; c < 6; c++) {
-      double s = 0;
-      for (int m = std::max(r, c); m < 6; m++) s += X[6 * m + r] * X[6 * m + c];
-      P[6 * r + c] = s;
-    }
-  double M[36] = {0};
-  for (int c = 0; c < 6; c++)
-    for (int r = c; r < 6; r++) {
-      double s = P[6 * r + c];
-      for (int m = 0; m < c; m++) s -= M[6 * r + m] * M[6 * c + m];
-      if (r == c) {
-        if (!(s > 0)) return false;
-        M[6 * c + c] = std::sqrt(s);
-      } else {
-        M[6 * r + c] = s / M[6 * c + c];
-      }
-    }
-  for (int r = 0; r < 6; r++)
-    for (int c = 0; c < 6; c++) out[6 * r + c] = M[6 * c + r];
-  return true;
+template <class T4>
+inline T4 pose7_to_transform(const double* p) {
+  double m[16];
+  cvb_pose::pose7_to_transform(p, m);
+  return from_rowmajor<T4>(m);
 }
-
 // Flattened problem with owning storage + the cvb_ba_problem view
 struct Flat {
   std::vector<double> pose, sb, extr, intr, dist, lm, obs_sigma, imu_dt, imu_acc, imu_gyr, imu_acc0, imu_gyr0, edge_q, edge_t,
@@ -622,161 +545,102 @@ void RemoveLandmarkOutliers(Context& ctx, MapPtr map, double th_outlier = 0.92, 
 
 // ---------------------------------------------------------------------------------------------------------------
 // Optimization::PoseGraphOptimization — optimization_be.hpp:46-47.  PoseMap = std::map<idpair, Transform>.
+// The chain is flattened in canonical keyframe order and handed to one cvb_pgo call (the edge rule, the solve and the
+// write-back are stated in include/covins_b200.h).  Write-back: keyframes in canonical order (SetPoseTws, SetStateVelocity,
+// SetPoseOptimized, :1033-1051), then the valid landmarks in map order: SetWorldPos + SetOptimized when re-anchored through
+// their reference keyframe, map->EraseLandmark when cvb_pgo flags them (:1054-1083).
 // ---------------------------------------------------------------------------------------------------------------
 template <class MapPtr, class PoseMap>
 void PoseGraphOptimization(Context& ctx, MapPtr map, PoseMap corrected_poses, const OptParams& P = OptParams()) {
   using KeyframePtr = typename std::decay<decltype(map->GetKeyframesVec()[0])>::type;
   using KF = typename KeyframePtr::element_type;
   using Transform = typename std::decay<decltype(map->GetKeyframesVec()[0]->GetPoseTws())>::type;
-  auto keyframes = map->GetKeyframesVec();
   auto landmarks = map->GetLandmarksVec();
-  detail::Flat F;
+  using LandmarkPtr = typename std::decay<decltype(landmarks[0])>::type;
   std::map<const KF*, int> kf_index;
   std::vector<KeyframePtr> kfs;
-  for (auto& kf : keyframes) {
-    if (kf->IsInvalid()) continue;
-    kf_index[kf.get()] = (int)kfs.size();
-    kfs.push_back(kf);
-  }
+  detail::canonical_keyframes(map->GetKeyframesVec(), kf_index, kfs);
   const int K = (int)kfs.size();
-  F.pose.resize(7 * (size_t)K); F.sb.assign(9 * (size_t)K, 0.0); F.extr.resize(7 * (size_t)K);
-  F.intr.assign(4 * (size_t)K, 1.0); F.dist.assign(4 * (size_t)K, 0.0); F.pose_const.assign(K, 0); F.cam_of_kf.resize(K);
-  F.lm_obs_ptr.push_back(0); F.imu_ptr.push_back(0);
-  for (int k = 0; k < K; k++) {
-    auto& kf = kfs[k];
-    double tmp_pose[7];
-    kf->UpdateCeresFromState(tmp_pose, &F.sb[9 * (size_t)k], &F.extr[7 * (size_t)k]);
-    auto mit = corrected_poses.find(kf->id_);                                                        // :854-868
-    const Transform T_ws_init = (mit != corrected_poses.end()) ? mit->second : kf->GetPoseTws();
-    detail::transform_to_pose7(T_ws_init, &F.pose[7 * (size_t)k]);
-    F.cam_of_kf[k] = k;
-    if (kf->id_.first == 0 && kf->id_.second == map->id_map_) F.pose_const[k] = 1;                  // :870-871
-    if (kf->is_gba_optimized_ && P.pgo_fix_kfs_after_gba) F.pose_const[k] = 1;                      // :875-877
-    else if (kf->is_loaded_ && P.pgo_fix_poses_loaded_maps) F.pose_const[k] = 1;                    // :878-881
-  }
-  double S1[36] = {0}, S23[36] = {0}, S45[36] = {0};
-  for (int d = 0; d < 6; d++) {
-    S1[7 * d] = (d < 3 ? P.wt_kf_r : P.wt_kf_t) * P.wt_kf_n1;                                        // :896-898
-    S23[7 * d] = S1[7 * d] / P.wt_kf_n23;
-    S45[7 * d] = S1[7 * d] / P.wt_kf_n45;
-  }
-  auto push_edge = [&](int i, int j, const Transform& T12, const double* S, bool robust) {
-    double p7[7];
-    detail::transform_to_pose7(T12, p7);
-    F.edge_i.push_back(i); F.edge_j.push_back(j);
-    F.edge_q.insert(F.edge_q.end(), p7, p7 + 4);
-    F.edge_t.insert(F.edge_t.end(), p7 + 4, p7 + 7);
-    F.edge_S.insert(F.edge_S.end(), S, S + 36);
-    F.edge_robust.push_back(robust ? 1 : 0);
+  const auto index_of = [&](const KeyframePtr& kf) -> int32_t {   // -1 none, -2 not among the valid keyframes
+    if (!kf) return -1;
+    auto it = kf_index.find(kf.get());
+    return it == kf_index.end() ? -2 : it->second;
   };
-  for (const auto& lc : map->GetLoopConstraints()) {                                                 // :910-943
-    double Sl[36];
-    if (P.placerec_type_covins) {
-      std::copy(S1, S1 + 36, Sl);
-    } else {
-      double cov[36];
-      for (int r = 0; r < 6; r++)
-        for (int c = 0; c < 6; c++) cov[6 * r + c] = lc.cov_mat(r, c);
-      if (!detail::sqrt_info_from_cov(cov, Sl)) {
-        std::printf("FATAL: loop covariance is not positive definite\n");
-        std::exit(-1);
-      }
-    }
-    push_edge(kf_index.at(lc.kf1.get()), kf_index.at(lc.kf2.get()), lc.T_s1_s2, Sl, P.use_robust_loss);
-  }
-  std::set<std::pair<const KF*, const KF*>> inserted_edges;                                          // :907
-  for (int k = 0; k < K; k++) {                                                                      // successor edges :947-972
-    auto& kf = kfs[k];
-    auto succ = kf->GetSuccessor();
-    if (!succ) continue;
-    auto key = std::make_pair((const KF*)kf.get(), (const KF*)succ.get());
-    if (inserted_edges.count(key)) {
-      std::printf("WARN: KF edge already added\n");
-      continue;
-    }
-    inserted_edges.insert(key);
-    push_edge(k, kf_index.at(succ.get()), detail::rel_transform(kf->GetPoseTws_vio(), succ->GetPoseTws_vio()), S1, false);
-  }
-  if (P.use_nbr_kfs) {                                                                               // :976-1021
-    for (int k = 0; k < K; k++) {
-      auto& kf = kfs[k];
-      std::vector<KeyframePtr> connections;
-      KeyframePtr temp_kf = kf;
-      for (int j = 1; j < 6; ++j)
-        if (int(kf->id_.first) - j > 0) {
-          temp_kf = temp_kf->GetPredecessor();
-          connections.push_back(temp_kf);
-        }
-      size_t n = 0;
-      for (auto& kfc : connections) {
-        n++;
-        const double* S = (n <= 1) ? S1 : (n <= 3 ? S23 : S45);
-        auto key = std::make_pair((const KF*)kf.get(), (const KF*)kfc.get());
-        if (inserted_edges.count(key)) continue;
-        inserted_edges.insert(key);
-        push_edge(k, kf_index.at(kfc.get()), detail::rel_transform(kf->GetPoseTws_vio(), kfc->GetPoseTws_vio()), S, false);
-      }
-    }
-  }
-  const cvb_ba_problem prob = F.view();
-  cvb_ba_options o{};
-  o.max_iterations = P.pgo_iteration_limit;
-  o.visual_only = 1;
-  o.cauchy_reproj = 0.0;
-  o.cauchy_edge = P.robust_loss_th;
-  o.world = 1;
-  std::vector<double> o_pose(7 * (size_t)K);
-  cvb_ba_result res{};
-  res.pose = o_pose.data();
-  ctx.check(cvb_ba_solve(ctx.get(), &prob, &o, &res), "cvb_ba_solve(PGO)");
-
-  // Recover the optimized data (:1033-1051)
-  std::map<typename std::decay<decltype(kfs[0]->id_)>::type, Transform> non_corrected_poses;
+  std::vector<double> T_ws(16 * (size_t)K), T_init(16 * (size_t)K), T_vio(16 * (size_t)K), vel(3 * (size_t)K);
+  std::vector<int32_t> pred(K), succ(K), kid(K);
+  std::vector<uint8_t> pose_const(K, 0);
   for (int k = 0; k < K; k++) {
     auto& kf = kfs[k];
-    const Transform T_ws_uncorrected = kf->GetPoseTws();
-    non_corrected_poses[kf->id_] = T_ws_uncorrected;
-    const Transform T_ws_corrected = detail::pose7_to_transform<Transform>(&o_pose[7 * (size_t)k]);
-    const auto vel = kf->GetStateVelocity();
-    kf->SetPoseTws(T_ws_corrected);
-    double v[3];   // R_corr * R_uncorr^T * v  (:1046-1047)
-    for (int r = 0; r < 3; r++) {
-      double s = 0;
-      for (int c = 0; c < 3; c++) {
-        double m = 0;
-        for (int x = 0; x < 3; x++) m += T_ws_corrected(r, x) * T_ws_uncorrected(c, x);
-        s += m * vel[c];
-      }
-      v[r] = s;
-    }
-    kf->SetStateVelocity({v[0], v[1], v[2]});
-    kf->SetPoseOptimized();
+    detail::to_rowmajor(kf->GetPoseTws(), &T_ws[16 * (size_t)k]);
+    auto mit = corrected_poses.find(kf->id_);                                                        // :854-868
+    if (mit != corrected_poses.end()) detail::to_rowmajor(mit->second, &T_init[16 * (size_t)k]);
+    else std::copy(&T_ws[16 * (size_t)k], &T_ws[16 * (size_t)k] + 16, &T_init[16 * (size_t)k]);
+    detail::to_rowmajor(kf->GetPoseTws_vio(), &T_vio[16 * (size_t)k]);
+    pred[k] = index_of(kf->GetPredecessor());
+    succ[k] = index_of(kf->GetSuccessor());
+    kid[k] = (int32_t)int(kf->id_.first);
+    if (kf->id_.first == 0 && kf->id_.second == map->id_map_) pose_const[k] = 1;                    // :870-871
+    if (kf->is_gba_optimized_ && P.pgo_fix_kfs_after_gba) pose_const[k] = 1;                        // :875-877
+    else if (kf->is_loaded_ && P.pgo_fix_poses_loaded_maps) pose_const[k] = 1;                      // :878-881
+    const auto v = kf->GetStateVelocity();
+    for (int c = 0; c < 3; c++) vel[3 * (size_t)k + c] = v[c];
   }
-  // Landmarks re-anchored through their reference keyframe (:1054-1083)
+  std::vector<int32_t> loop_i, loop_j;
+  std::vector<double> loop_q, loop_t, loop_cov;
+  for (const auto& lc : map->GetLoopConstraints()) {                                                 // :910-943
+    double p7[7];
+    detail::transform_to_pose7(lc.T_s1_s2, p7);
+    loop_i.push_back(index_of(lc.kf1));
+    loop_j.push_back(index_of(lc.kf2));
+    loop_q.insert(loop_q.end(), p7, p7 + 4);
+    loop_t.insert(loop_t.end(), p7 + 4, p7 + 7);
+    for (int r = 0; r < 6; r++)
+      for (int c = 0; c < 6; c++) loop_cov.push_back(lc.cov_mat(r, c));
+  }
+  std::vector<LandmarkPtr> lms;
+  std::vector<double> lm_pos;
+  std::vector<int32_t> lm_ref;
+  std::vector<uint8_t> lm_has_obs;
   for (auto& lm : landmarks) {
     if (lm->IsInvalid()) continue;
-    auto kf_ref = lm->GetReferenceKeyframe();
-    if (!kf_ref) {
-      if (!lm->GetObservations().empty()) map->EraseLandmark(lm);
-      continue;
-    }
-    auto mit = non_corrected_poses.find(kf_ref->id_);
-    if (mit == non_corrected_poses.end()) {
-      map->EraseLandmark(lm);
-      continue;
-    }
-    const Transform& Tu = mit->second;
     const auto pw = lm->GetWorldPos();
-    double ps[3], pc[3];
-    for (int r = 0; r < 3; r++) {
-      double s = 0;
-      for (int c = 0; c < 3; c++) s += Tu(c, r) * (pw[c] - Tu(c, 3));
-      ps[r] = s;
+    lm_pos.insert(lm_pos.end(), {pw[0], pw[1], pw[2]});
+    lm_ref.push_back(index_of(lm->GetReferenceKeyframe()));
+    lm_has_obs.push_back(lm->GetObservations().empty() ? 0 : 1);
+    lms.push_back(lm);
+  }
+  const int L = (int)lms.size();
+  cvb_pgo_problem pp{};
+  pp.K = K; pp.T_ws = T_ws.data(); pp.T_ws_init = T_init.data(); pp.T_ws_vio = T_vio.data();
+  pp.kf_pred = pred.data(); pp.kf_succ = succ.data(); pp.kf_id = kid.data(); pp.pose_const = pose_const.data(); pp.velocity = vel.data();
+  pp.n_loop = (int32_t)loop_i.size(); pp.loop_i = loop_i.data(); pp.loop_j = loop_j.data(); pp.loop_q = loop_q.data(); pp.loop_t = loop_t.data();
+  pp.loop_cov = P.placerec_type_covins ? nullptr : loop_cov.data();                                 // :929
+  pp.L = L; pp.lm_pos = lm_pos.data(); pp.lm_ref = lm_ref.data(); pp.lm_has_obs = lm_has_obs.data();
+  cvb_pgo_options po{P.wt_kf_r, P.wt_kf_t, P.wt_kf_n1, P.wt_kf_n23, P.wt_kf_n45, P.use_nbr_kfs ? 1 : 0, P.use_robust_loss ? 1 : 0,
+                     P.robust_loss_th, P.pgo_iteration_limit};
+  std::vector<double> T_out(16 * (size_t)K), vel_out(3 * (size_t)K), lm_out(3 * (size_t)L);
+  std::vector<uint8_t> lm_erase(L);
+  cvb_pgo_result res{};
+  res.T_ws_out = T_out.data(); res.velocity_out = vel_out.data(); res.lm_out = lm_out.data(); res.lm_erase = lm_erase.data();
+  const int rc = cvb_pgo(ctx.get(), &pp, &po, &res);
+  if (res.bad_loop >= 0) {
+    std::printf("FATAL: loop covariance is not positive definite\n");
+    std::exit(-1);
+  }
+  ctx.check(rc, "cvb_pgo");
+  for (int k = 0; k < K; k++) {                                                                      // :1033-1051
+    auto& kf = kfs[k];
+    kf->SetPoseTws(detail::from_rowmajor<Transform>(&T_out[16 * (size_t)k]));
+    kf->SetStateVelocity({vel_out[3 * (size_t)k], vel_out[3 * (size_t)k + 1], vel_out[3 * (size_t)k + 2]});
+    kf->SetPoseOptimized();
+  }
+  for (int l = 0; l < L; l++) {                                                                      // :1054-1083
+    if (lm_erase[l]) {
+      map->EraseLandmark(lms[l]);
+    } else if (lm_ref[l] >= 0) {
+      lms[l]->SetWorldPos({lm_out[3 * (size_t)l], lm_out[3 * (size_t)l + 1], lm_out[3 * (size_t)l + 2]});
+      lms[l]->SetOptimized();
     }
-    const Transform Tc = kf_ref->GetPoseTws();
-    for (int r = 0; r < 3; r++) pc[r] = Tc(r, 0) * ps[0] + Tc(r, 1) * ps[1] + Tc(r, 2) * ps[2] + Tc(r, 3);
-    lm->SetWorldPos({pc[0], pc[1], pc[2]});
-    lm->SetOptimized();
   }
   std::printf("--> PGO END \n");
 }

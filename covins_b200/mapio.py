@@ -408,4 +408,12 @@ def read_map(path: str) -> dict:
              descriptors=np.array(desc, np.uint8).reshape(-1, 32) if desc else np.zeros((0, 32), np.uint8),
              kf_descriptors=[k["descriptors"] for k in kfs], kf_descriptors_add=[k["descriptors_add"] for k in kfs],
              kf_keypoints_add=[k["keypoints_distorted_add"] for k in kfs], lm_ids=[l["id"] for l in lms])
+    # what the pose graph's write-back reads (covins_b200.optimization.pgo_map_problem): the stored 4x4 poses, the chain links and
+    # each landmark's reference keyframe, as keyframe indices (-1 none, -2 a keyframe that is not in the map)
+    link = lambda i: -1 if i == DEFPAIR else index.get(i, -2)
+    p.update(T_ws=np.array([k["T_w_s"] for k in kfs], np.float64).reshape(K, 4, 4),
+             T_ws_vio=np.array([k["T_w_s_vio"] for k in kfs], np.float64).reshape(K, 4, 4),
+             kf_pred=np.array([link(k["id_predecessor"]) for k in kfs], np.int32), kf_succ=np.array([link(k["id_successor"]) for k in kfs], np.int32),
+             lm_ref=np.array([link(l["id_reference"]) for l in lms], np.int32),
+             lm_has_obs=np.array([len(l["observations"]) > 0 for l in lms], np.uint8))
     return p

@@ -412,6 +412,106 @@ def pose_graph_optimization(ctx: Context, p: dict, edges: dict, iterations=10, r
     return res.as_dict()
 
 
+class PgoProblem(C.Structure):
+    _fields_ = [("K", C.c_int32)] + [(n, c_vp) for n in ("T_ws", "T_ws_init", "T_ws_vio", "kf_pred", "kf_succ", "kf_id", "pose_const",
+                                                          "velocity")] + \
+               [("n_loop", C.c_int32)] + [(n, c_vp) for n in ("loop_i", "loop_j", "loop_q", "loop_t", "loop_cov")] + \
+               [("L", C.c_int32)] + [(n, c_vp) for n in ("lm_pos", "lm_ref", "lm_has_obs")]
+
+
+class PgoOptions(C.Structure):
+    _fields_ = [("wt_kf_r", C.c_double), ("wt_kf_t", C.c_double), ("wt_kf_n1", C.c_double), ("wt_kf_n23", C.c_double),
+                ("wt_kf_n45", C.c_double), ("use_nbr_kfs", C.c_int32), ("use_robust_loss", C.c_int32), ("robust_loss_th", C.c_double),
+                ("iteration_limit", C.c_int32)]
+
+
+class PgoResult(C.Structure):
+    _fields_ = [("T_ws_out", c_vp), ("velocity_out", c_vp), ("lm_out", c_vp), ("lm_erase", c_vp), ("ba", BaResult),
+                ("n_edge", C.c_int32), ("bad_loop", C.c_int32)]
+
+
+def _chain_links(agent_of):
+    """predecessor / successor indices of keyframes listed agent by agent in id order (-1 at a chain's ends)"""
+    agent = np.asarray(agent_of)
+    K = len(agent)
+    same = agent[1:] == agent[:-1] if K > 1 else np.zeros(0, bool)
+    pred = np.full(K, -1, np.int32); succ = np.full(K, -1, np.int32)
+    idx = np.arange(K, dtype=np.int32)
+    pred[1:][same] = idx[:-1][same]
+    succ[:-1][same] = idx[1:][same]
+    return pred, succ
+
+
+def pgo_map_problem(p: dict, covins_mode=True, T_ws_init=None) -> dict:
+    """The map cvb_pgo takes (include/covins_b200.h), from a flat problem (covins_b200.synth_map or mapio.read_map):
+    T_ws from p["T_ws"] or else p["pose"]; T_ws_vio from p["T_ws_vio"] or else T_ws; kf_pred / kf_succ from p or else the
+    agents' chains; velocity from speedbias; lm_ref / lm_has_obs from p (mapio's id_reference) or else each landmark's first
+    observer, as the reference's landmarks are anchored; loop_cov only in COVINS_G mode (covins_mode False)."""
+    K = int(p["K"])
+    if p.get("T_ws") is not None:
+        T_ws = np.ascontiguousarray(p["T_ws"], np.float64).reshape(K, 4, 4)
+    else:
+        pose = np.asarray(p["pose"], np.float64)
+        T_ws = np.tile(np.eye(4), (K, 1, 1))
+        T_ws[:, :3, :3] = _quat_to_rot(pose[:, :4]); T_ws[:, :3, 3] = pose[:, 4:]
+    T_vio = p.get("T_ws_vio")
+    pred, succ = (p["kf_pred"], p["kf_succ"]) if p.get("kf_pred") is not None else _chain_links(p["agent_of"])
+    ptr = np.asarray(p.get("lm_obs_ptr", np.zeros(1)), np.int64)
+    n_obs = np.diff(ptr)
+    if p.get("lm_ref") is not None:
+        lm_ref, has = np.asarray(p["lm_ref"]), np.asarray(p["lm_has_obs"])
+    else:
+        obs_kf = np.asarray(p.get("obs_kf", np.zeros(0)), np.int32)
+        has = n_obs > 0
+        lm_ref = np.full(len(n_obs), -1, np.int32)
+        lm_ref[has] = obs_kf[ptr[:-1][has]]
+    sb = p.get("speedbias")
+    nl = len(p.get("loop_i", []))
+    return dict(T_ws=T_ws, T_ws_init=None if T_ws_init is None else np.asarray(T_ws_init, np.float64).reshape(K, 4, 4),
+                T_ws_vio=T_ws if T_vio is None else np.asarray(T_vio, np.float64).reshape(K, 4, 4),
+                kf_pred=np.asarray(pred, np.int32), kf_succ=np.asarray(succ, np.int32), kf_id=np.asarray(p["kf_id"], np.int32),
+                pose_const=np.asarray(p["pose_const"], np.uint8), velocity=None if sb is None else np.asarray(sb, np.float64)[:, :3],
+                loop_i=np.asarray(p.get("loop_i", np.zeros(0)), np.int32), loop_j=np.asarray(p.get("loop_j", np.zeros(0)), np.int32),
+                loop_q=np.asarray(p.get("loop_q", np.zeros((0, 4))), np.float64).reshape(nl, 4),
+                loop_t=np.asarray(p.get("loop_t", np.zeros((0, 3))), np.float64).reshape(nl, 3),
+                loop_cov=None if covins_mode else np.asarray(p["loop_cov"], np.float64).reshape(nl, 6, 6),
+                lm_pos=np.asarray(p.get("lm", np.zeros((0, 3))), np.float64).reshape(-1, 3),
+                lm_ref=np.asarray(lm_ref, np.int32), lm_has_obs=np.asarray(has, np.uint8))
+
+
+def pose_graph_optimization_map(ctx: Context, p: dict, wt=(10.0, 1.0, 10.0, 2.0, 3.0), covins_mode=True, use_robust=True,
+                                use_nbr=True, iterations=10, robust_th=0.5, T_ws_init=None, cap=64):
+    """Optimization::PoseGraphOptimization with its write-back (optimization_be.cpp:833-1086) in one cvb_pgo call: the edges of
+    the keyframe chain, the solve and what the server writes into its map afterwards.  `p` is a flat problem or a dict of
+    pgo_map_problem (it has T_ws).  Returns T_ws [K,4,4] (what SetPoseTws receives), pose [K,7] (the solved pose7),
+    velocity [K,3] (None without velocities), lm [L,3] (re-anchored; others keep their bits), lm_erase [L] bool, the
+    solver's cost history / steps / iterations / termination, and n_edge."""
+    pr = p if "lm_pos" in p else pgo_map_problem(p, covins_mode, T_ws_init)
+    K, L, nl = len(pr["kf_id"]), len(pr["lm_pos"]), len(pr["loop_i"])
+    a = {k: (None if v is None else np.ascontiguousarray(v)) for k, v in pr.items()}
+    s = PgoProblem()
+    s.K, s.n_loop, s.L = K, nl, L
+    for name, _ in PgoProblem._fields_:
+        if name not in ("K", "n_loop", "L"):
+            v = a.get(name)
+            setattr(s, name, v.ctypes.data if v is not None and v.size else None)
+    o = PgoOptions(*[float(w) for w in wt], int(use_nbr), int(use_robust), float(robust_th), int(iterations))
+    T_out = np.zeros((K, 4, 4)); vel = np.zeros((K, 3)); lm = np.zeros((max(L, 1), 3)); erase = np.zeros(max(L, 1), np.uint8)
+    res = _Res(K, 0, cap)
+    r = PgoResult()
+    r.T_ws_out, r.velocity_out, r.lm_out, r.lm_erase = T_out.ctypes.data, vel.ctypes.data, lm.ctypes.data, erase.ctypes.data
+    r.ba = res.r
+    r.ba.speedbias = r.ba.lm = r.ba.lm_owner = None
+    ctx.check(lib().cvb_pgo(ctx.handle, C.byref(s), C.byref(o), C.byref(r)))
+    res.r = r.ba
+    out = res.as_dict()
+    for k in ("speedbias", "lm", "lm_owner"):
+        out.pop(k)
+    out.update(T_ws=T_out, velocity=vel if pr.get("velocity") is not None else None, lm=lm[:L], lm_erase=erase[:L].astype(bool),
+               n_edge=int(r.n_edge))
+    return out
+
+
 def solve(ctx: Context, p: dict, max_iterations: int, visual_only=False, cauchy_reproj=1.0, cauchy_edge=1.0, edges=None,
           obs_skip=None):
     """one ceres::Solve on the flat problem (single GPU)."""

@@ -1180,6 +1180,81 @@ CVB_API int cvb_map_rigid_transform(cvb_ctx* ctx, const double T[16], int K, dou
                                     double* vel /*[K][3] in/out, nullable*/, int L, double* lm_pos /*[L][3] in/out*/,
                                     const uint8_t* kf_sel /*[K], nullable*/, const uint8_t* lm_sel /*[L], nullable*/);
 
+/*
+ * Optimization::PoseGraphOptimization (optimization_be.cpp:833-1086) on a flattened map in one call: the edges of the
+ * keyframe chain, the solve and the write-back of velocities and landmarks.  All arrays are host memory, keyframes in the
+ * canonical order (the valid keyframes of the map, id-sorted), poses row-major 4x4 as in cvb_map_rigid_transform.
+ * Keyframe indices: kf_pred / kf_succ / lm_ref hold an index in [0, K), -1 for none, -2 for a keyframe that exists but is not
+ * among the K (an invalid one).
+ * EDGES, in this order (the shim's rule before this call, :886-1021):
+ *   1. loop l = 0..n_loop-1 between loop_i[l] and loop_j[l], measurement (loop_q[l], loop_t[l]), sqrt_info chol(cov^-1)^T of
+ *      loop_cov[l] (COVINS_G, :922-923) or S1 when loop_cov is NULL (COVINS), Cauchy(robust_loss_th) iff use_robust_loss;
+ *   2. per keyframe k in order with kf_succ[k] >= 0: (k, kf_succ[k]) with S1 (:947-972);
+ *   3. when use_nbr_kfs, per keyframe k in order: the walk through kf_pred j = 1..5 steps while int(kf_id[k]) - j > 0, the
+ *      j-th keyframe reached with S1, S23, S23, S45, S45 (:976-1021).
+ *   An ordered pair already inserted by 2. or 3. is skipped; loops are not in that set.  Steps 2. and 3. measure
+ *   transform_to_pose7(rel_transform(T_ws_vio[i], T_ws_vio[j])).  S1 = diag(wt_kf_r x3, wt_kf_t x3) * wt_kf_n1, S23 = S1 /
+ *   wt_kf_n23, S45 = S1 / wt_kf_n45 (:896-903).  Only loops are robust.
+ * SOLVE: start poses transform_to_pose7(T_ws_init, or T_ws when NULL) (:854-868), pose_const as given, the bundle
+ *   adjustment engine with visual_only, no reprojection loss, cauchy_edge = robust_loss_th, iteration_limit iterations.
+ * WRITE-BACK, with Tu = T_ws[k] (the pose before the call) and Tc = pose7_to_transform(solved pose) (:1033-1083):
+ *   T_ws_out[k] = Tc (what the shim passes to SetPoseTws);
+ *   velocity_out[k][r] = sum_c (sum_x Tc(r,x) Tu(c,x)) velocity[k][c], each sum from 0 in that loop order (:1046-1047);
+ *   landmark l with lm_ref[l] = k >= 0: ps = Tu^T (p - t_u) (sums from 0), lm_out[l][r] = ((Tc(r,0) ps0 + Tc(r,1) ps1) +
+ *   Tc(r,2) ps2) + Tc(r,3), lm_erase[l] = 0; lm_ref -1: lm_erase = lm_has_obs[l]; lm_ref -2: lm_erase = 1; a landmark without
+ *   a reference keyframe keeps its input bits in lm_out.
+ *   Products and sums are rounded one by one in the order stated (include/covins_b200_pose.h), so oracle/pgo.py gives the
+ *   same bits.
+ * Device work: one launch for the start poses and the edge measurements (straight into the solver's arrays; the edge
+ * topology is built on the host), the solve, one launch for the write-back over K + L items, one download of all outputs.
+ * CVB_ERR_INVALID, before any launch: a NULL required pointer, K < 1, a negative n_loop / L, an index outside its range, a
+ * loop with loop_i == loop_j, a successor that is not among the K (-2), a neighbour walk that needs a predecessor that is
+ * absent (-1) or not among the K (-2), a non-finite entry in T_ws / T_ws_init / T_ws_vio, iteration_limit < 0.  A loop
+ * covariance that is not positive definite sets r->bad_loop to that loop (else -1) and is refused the same way, naming it.
+ */
+typedef struct cvb_pgo_problem {
+  int32_t K;
+  const double* T_ws;       /* [K][16] the pose before the call (the write-back's "uncorrected" pose) */
+  const double* T_ws_init;  /* [K][16] nullable: the start values of the solve (corrected_poses); NULL = T_ws */
+  const double* T_ws_vio;   /* [K][16] */
+  const int32_t* kf_pred;   /* [K] */
+  const int32_t* kf_succ;   /* [K] */
+  const int32_t* kf_id;     /* [K] id_.first */
+  const uint8_t* pose_const;/* [K] */
+  const double* velocity;   /* [K][3] nullable: then velocity_out is not written */
+  int32_t n_loop;
+  const int32_t* loop_i;    /* [n_loop] */
+  const int32_t* loop_j;
+  const double* loop_q;     /* [n_loop][4] x,y,z,w of T_s1_s2 */
+  const double* loop_t;     /* [n_loop][3] */
+  const double* loop_cov;   /* [n_loop][36] nullable: NULL = COVINS weights */
+  int32_t L;
+  const double* lm_pos;     /* [L][3] */
+  const int32_t* lm_ref;    /* [L] reference keyframe */
+  const uint8_t* lm_has_obs;/* [L] */
+} cvb_pgo_problem;
+
+typedef struct cvb_pgo_options {
+  double wt_kf_r, wt_kf_t, wt_kf_n1, wt_kf_n23, wt_kf_n45;   /* 10, 1, 10, 2, 3 */
+  int32_t use_nbr_kfs;       /* 1 */
+  int32_t use_robust_loss;   /* 1 */
+  double robust_loss_th;     /* 0.5 */
+  int32_t iteration_limit;   /* pgo_iteration_limit 10 */
+} cvb_pgo_options;
+
+typedef struct cvb_pgo_result {
+  double* T_ws_out;         /* [K][16] out */
+  double* velocity_out;     /* [K][3] out; required when problem velocity is given */
+  double* lm_out;           /* [L][3] out */
+  uint8_t* lm_erase;        /* [L] out */
+  cvb_ba_result ba;         /* the solve: ba.pose [K][7] (nullable), cost history, step status, iterations, termination;
+                               speedbias, lm and lm_owner are not written */
+  int32_t n_edge;           /* out: edges in the problem */
+  int32_t bad_loop;         /* out: the loop whose covariance is not positive definite, -1 for none */
+} cvb_pgo_result;
+
+CVB_API int cvb_pgo(cvb_ctx* ctx, const cvb_pgo_problem* p, const cvb_pgo_options* o, cvb_pgo_result* r);
+
 #ifdef __cplusplus
 }
 #endif
