@@ -80,6 +80,7 @@ SIGNATURES = {
     "cvb_ba_restart": (C.c_int, [c_vp]),
     "cvb_ba_enable_p2p": (C.c_int, [c_vp]),
     "cvb_db_remove": (C.c_int, [c_vp, c_vp, C.c_int]),
+    "cvb_db_remove_batch": (C.c_int, [c_vp, c_vp, c_vp, C.c_int]),
     "cvb_optimize_relative_pose": (C.c_int, [c_vp, c_vp, C.c_double, c_vp, c_vp, c_vp, c_vp]),
     "cvb_search_by_se3_batch": (C.c_int, [c_vp, c_vp, c_vp, C.c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
     "cvb_search_by_projection": (C.c_int, [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, C.c_int, C.c_int, C.c_double, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
@@ -114,6 +115,7 @@ SIGNATURES = {
     "cvb_db_group_append": (C.c_int, [c_vp, c_vp, c_vp, C.c_int]),
     "cvb_db_group_append_sift": (C.c_int, [c_vp, c_vp, c_vp, C.c_int]),
     "cvb_db_group_remove": (C.c_int, [c_vp, C.c_int]),
+    "cvb_db_group_remove_batch": (C.c_int, [c_vp, c_vp, C.c_int]),
     "cvb_db_group_size": (C.c_int, [c_vp, C.POINTER(C.c_int32), C.POINTER(C.c_int64), c_vp]),
     "cvb_db_group_match_hamming": (C.c_int, [c_vp, c_vp, C.c_int, C.c_float, C.c_float, c_vp, c_vp, c_vp, c_vp, c_vp, C.c_int,
                                              C.POINTER(C.c_int32)]),

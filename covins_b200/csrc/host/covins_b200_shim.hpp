@@ -1642,6 +1642,16 @@ class DescriptorDatabase {
     else ctx_->check(cvb_db_remove(ctx_->get(), db_, db_index), "cvb_db_remove");
     n_kf_--;
   }
+  // a batch of keyframes leaves the map in one call (cvb_db_remove_batch / cvb_db_group_remove_batch), e.g. the keyframes
+  // PruneRedundantKeyframes culled: db_indices as before the call, in any order; equal to RemoveKeyframe of each from the
+  // highest to the lowest.  A survivor's index drops by the number of removed indices below it.
+  void RemoveKeyframes(const std::vector<int>& db_indices) {
+    const std::vector<int32_t> idx(db_indices.begin(), db_indices.end());
+    const int n = (int)idx.size();
+    if (gdb_) ctx_->check(cvb_db_group_remove_batch(gdb_, idx.data(), n), "cvb_db_group_remove_batch");
+    else ctx_->check(cvb_db_remove_batch(ctx_->get(), db_, idx.data(), n), "cvb_db_remove_batch");
+    n_kf_ -= n;
+  }
   // two agents' maps are merged (MergeMaps): other's keyframes follow this database's, in other's order, copied in HBM
   // (cvb_db_merge / cvb_db_group_merge); other is left unchanged.  Both of one kind, on one Context or one ContextGroup.
   void Merge(const DescriptorDatabase& other) {

@@ -15,6 +15,7 @@
 #include <string.h>
 
 #include <algorithm>
+#include <memory>
 
 #include "ba_group.cuh"
 #include "cvb_internal.cuh"
@@ -160,6 +161,154 @@ __global__ void __launch_bounds__(256) db_compact_kernel(const int32_t* __restri
     }
     pos += __popc(m);
   }
+}
+
+// K18: the gather of a batch removal.  dst[v] = src[run_src[r] + (v - run_dst[r])] for every 16-byte vector v < n_vec of
+// the destination, r the kept run with run_dst[r] <= v < run_dst[r + 1] (offsets in vectors, run_dst strictly increasing,
+// run_dst[n_runs] = n_vec).  A CTA copies kGatherVecs * 256 consecutive vectors: its first thread finds the runs of its
+// first and last vector by binary search over the whole table, and every thread then searches only between those two
+// (one run for most CTAs).  Each thread issues its loads before its stores.
+constexpr int kGatherThreads = 256, kGatherVecs = 8;
+
+__device__ __forceinline__ int run_of(const int64_t* __restrict__ run_dst, int lo, int hi, int64_t v) {
+  while (lo < hi) {
+    const int mid = (lo + hi + 1) >> 1;
+    if (run_dst[mid] <= v) lo = mid;
+    else hi = mid - 1;
+  }
+  return lo;
+}
+
+__global__ void __launch_bounds__(kGatherThreads) db_remove_gather_kernel(const uint4* __restrict__ src, uint4* __restrict__ dst,
+                                                                          const int64_t* __restrict__ run_dst,
+                                                                          const int64_t* __restrict__ run_src, int n_runs, int64_t n_vec) {
+  __shared__ int lo_s, hi_s;
+  const int64_t v0 = (int64_t)blockIdx.x * (kGatherThreads * kGatherVecs);
+  const int64_t v_end = v0 + kGatherThreads * kGatherVecs, v_last = (v_end < n_vec ? v_end : n_vec) - 1;
+  if (threadIdx.x == 0) {
+    lo_s = run_of(run_dst, 0, n_runs - 1, v0);
+    hi_s = run_of(run_dst, lo_s, n_runs - 1, v_last);
+  }
+  __syncthreads();
+  const int lo = lo_s, hi = hi_s;
+  uint4 x[kGatherVecs];
+#pragma unroll
+  for (int j = 0; j < kGatherVecs; j++) {
+    const int64_t v = v0 + j * kGatherThreads + threadIdx.x;
+    if (v <= v_last) {
+      const int r = run_of(run_dst, lo, hi, v);
+      x[j] = src[run_src[r] + (v - run_dst[r])];
+    }
+  }
+#pragma unroll
+  for (int j = 0; j < kGatherVecs; j++) {
+    const int64_t v = v0 + j * kGatherThreads + threadIdx.x;
+    if (v <= v_last) dst[v] = x[j];
+  }
+}
+
+// The refusals of a batch removal from n_kf keyframes: gone[k] = 1 for every listed index k
+int check_removals(cvb_ctx* ctx, const int32_t* kf_index, int n, int n_kf, const char* fn, std::vector<char>& gone) {
+  CVB_REQUIRE(ctx, n >= 0, "%s: negative count n = %d", fn, n);
+  CVB_REQUIRE(ctx, n == 0 || kf_index, "%s: null index list with n = %d", fn, n);
+  gone.assign((size_t)n_kf, 0);
+  for (int i = 0; i < n; i++) {
+    const int k = kf_index[i];
+    CVB_REQUIRE(ctx, k >= 0 && k < n_kf, "%s: keyframe index %d out of range (database holds %d)", fn, k, n_kf);
+    CVB_REQUIRE(ctx, !gone[k], "%s: keyframe index %d given twice", fn, k);
+    gone[k] = 1;
+  }
+  return CVB_OK;
+}
+
+// The kept keyframes of [first, n_seg) of one array, keyframe s spanning units [off[s], off[s + 1]) of `unit` bytes, as runs
+// of 16-byte vectors relative to off[first]: run_src [n_runs] and run_dst [n_runs + 1] (the last entry: the vectors kept).
+// Kept keyframes that are adjacent in the source, removed empty ones between them included, form one run.
+void kept_runs(const std::vector<int32_t>& off, const std::vector<char>& gone, int first, size_t unit, std::vector<int64_t>& run_dst,
+               std::vector<int64_t>& run_src) {
+  const int64_t base = off[first];
+  int64_t total = 0, src_end = -1;
+  for (size_t s = (size_t)first; s + 1 < off.size(); s++) {
+    if (gone[s] || off[s + 1] == off[s]) continue;
+    const int64_t a = (off[s] - base) * (int64_t)unit / 16, b = (off[s + 1] - base) * (int64_t)unit / 16;
+    if (a != src_end) {
+      run_src.push_back(a);
+      run_dst.push_back(total);
+    }
+    total += b - a;
+    src_end = b;
+  }
+  run_dst.push_back(total);
+}
+
+// K18 on one array: the kept vectors from `base` on gathered into a scratch block of the pool, then copied back to `base`
+int gather_runs(cvb_ctx* ctx, uint8_t* base, const int64_t* d_run_dst, const int64_t* d_run_src, int n_runs, int64_t n_vec) {
+  if (n_vec == 0) return CVB_OK;
+  cudaStream_t st = ctx->stream;
+  cvb_block B(ctx, st, false);
+  uint4* tmp;
+  B.tmp(tmp, (size_t)n_vec);
+  if (const int rc = B.place()) return rc;
+  const int64_t per_cta = kGatherThreads * kGatherVecs;
+  db_remove_gather_kernel<<<(unsigned)((n_vec + per_cta - 1) / per_cta), kGatherThreads, 0, st>>>((const uint4*)base, tmp, d_run_dst,
+                                                                                                  d_run_src, n_runs, n_vec);
+  CVB_CHECK_LAUNCH(ctx);
+  CVB_CUDA(ctx, cudaMemcpyAsync(base, tmp, (size_t)n_vec * 16, cudaMemcpyDeviceToDevice, st));
+  return CVB_OK;
+}
+
+// Removes the checked keyframes gone[] from db: the device work enqueued on ctx->stream, the host tables rebuilt.  Only the
+// suffix from the first removed keyframe that holds rows moves (removing empty keyframes moves nothing).  `stage` receives
+// the block of the uploaded run tables when there is device work: it reads pinned memory, so the caller keeps it until it
+// has synchronised the stream.
+int compact(cvb_ctx* ctx, cvb_db* db, const std::vector<char>& gone, std::unique_ptr<cvb_block>& stage) {
+  const int n_seg = (int)db->seg_ptr.size() - 1;
+  int first = 0, moved = n_seg;
+  while (first < n_seg && !gone[first]) first++;
+  for (int s = first; s < n_seg && moved == n_seg; s++)
+    if (gone[s] && db->seg_ptr[s + 1] > db->seg_ptr[s]) moved = s;
+  if (moved < n_seg) {
+    const size_t tb = cvb_tc::tile_bytes(db->metric());
+    std::vector<int64_t> rd, rs, td, ts;
+    kept_runs(db->seg_ptr, gone, moved, (size_t)db->desc_bytes, rd, rs);
+    kept_runs(db->seg_tile, gone, moved, tb, td, ts);
+    if (rd.back()) {   // kept rows follow the first moved keyframe (and so kept tiles)
+      stage.reset(new cvb_block(ctx, ctx->stream));
+      int64_t *d_rd, *d_rs, *d_td, *d_ts;
+      stage->in(d_rd, rd.data(), rd.size());
+      stage->in(d_rs, rs.data(), rs.size());
+      stage->in(d_td, td.data(), td.size());
+      stage->in(d_ts, ts.data(), ts.size());
+      int rc;
+      if ((rc = stage->place()) || (rc = stage->upload())) return rc;
+      if ((rc = gather_runs(ctx, db->d_rows + (size_t)db->seg_ptr[moved] * db->desc_bytes, d_rd, d_rs, (int)rs.size(), rd.back())))
+        return rc;
+      if ((rc = gather_runs(ctx, db->d_xt + (size_t)db->seg_tile[moved] * tb, d_td, d_ts, (int)ts.size(), td.back()))) return rc;
+    }
+  }
+  std::vector<int32_t> p(db->seg_ptr.begin(), db->seg_ptr.begin() + first + 1), t(db->seg_tile.begin(), db->seg_tile.begin() + first + 1);
+  for (int s = first; s < n_seg; s++)
+    if (!gone[s]) {
+      p.push_back(p.back() + (db->seg_ptr[s + 1] - db->seg_ptr[s]));
+      t.push_back(t.back() + (db->seg_tile[s + 1] - db->seg_tile[s]));
+    }
+  db->seg_ptr.swap(p);
+  db->seg_tile.swap(t);
+  db->seg_dirty = true;
+  return CVB_OK;
+}
+
+int remove_batch(cvb_ctx* ctx, cvb_db* db, const int32_t* kf_index, int n, const char* fn) {
+  std::vector<char> gone;
+  int rc = check_removals(ctx, kf_index, n, (int)db->seg_ptr.size() - 1, fn, gone);
+  if (rc || n == 0) return rc;
+  std::unique_ptr<cvb_block> stage;
+  rc = compact(ctx, db, gone, stage);
+  if (stage) {
+    const cudaError_t e = cudaStreamSynchronize(ctx->stream);
+    if (!rc && e != cudaSuccess) rc = cvb_fail(ctx, CVB_ERR_CUDA, "%s: cudaStreamSynchronize failed: %s", fn, cudaGetErrorString(e));
+  }
+  return rc;
 }
 
 // calls of one row kind on a database of the other are refused
@@ -360,39 +509,14 @@ int cvb_db_append_sift(cvb_ctx* ctx, cvb_db* db, const float* rows, const int32_
 int cvb_db_remove(cvb_ctx* ctx, cvb_db* db, int kf_index) {
   if (!ctx || !db) return CVB_ERR_INVALID;
   CVB_GUARD(ctx);
-  const int n_seg = (int)db->seg_ptr.size() - 1;
-  CVB_REQUIRE(ctx, kf_index >= 0 && kf_index < n_seg, "cvb_db_remove: keyframe index %d out of range (database holds %d)", kf_index, n_seg);
-  const int64_t a = db->seg_ptr[kf_index], b = db->seg_ptr[kf_index + 1], end = db->seg_ptr.back();
-  const size_t tail = (size_t)(end - b) * db->desc_bytes, len = (size_t)(b - a);
-  if (tail && len) {   // move the tail down through a scratch buffer (source and destination overlap)
-    cvb_block B(ctx, ctx->stream);
-    uint8_t* tmp;
-    B.tmp(tmp, tail);
-    if (const int rc = B.place()) return rc;
-    CVB_CUDA(ctx, cudaMemcpyAsync(tmp, db->d_rows + (size_t)b * db->desc_bytes, tail, cudaMemcpyDeviceToDevice, ctx->stream));
-    CVB_CUDA(ctx, cudaMemcpyAsync(db->d_rows + (size_t)a * db->desc_bytes, tmp, tail, cudaMemcpyDeviceToDevice, ctx->stream));
-    CVB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-  }
-  {   // the same for the operand tiles
-    const size_t tb = cvb_tc::tile_bytes(db->metric());
-    const int ta = db->seg_tile[kf_index], tbn = db->seg_tile[kf_index + 1], tend = db->seg_tile.back();
-    const size_t ttail = (size_t)(tend - tbn) * tb;
-    if (ttail && tbn > ta) {
-      cvb_block B(ctx, ctx->stream);
-      uint8_t* tmp;
-      B.tmp(tmp, ttail);
-      if (const int rc = B.place()) return rc;
-      CVB_CUDA(ctx, cudaMemcpyAsync(tmp, db->d_xt + (size_t)tbn * tb, ttail, cudaMemcpyDeviceToDevice, ctx->stream));
-      CVB_CUDA(ctx, cudaMemcpyAsync(db->d_xt + (size_t)ta * tb, tmp, ttail, cudaMemcpyDeviceToDevice, ctx->stream));
-      CVB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    }
-    db->seg_tile.erase(db->seg_tile.begin() + kf_index + 1);
-    for (size_t i = (size_t)kf_index + 1; i < db->seg_tile.size(); i++) db->seg_tile[i] -= (int32_t)(tbn - ta);
-  }
-  db->seg_ptr.erase(db->seg_ptr.begin() + kf_index + 1);
-  for (size_t i = (size_t)kf_index + 1; i < db->seg_ptr.size(); i++) db->seg_ptr[i] -= (int32_t)len;
-  db->seg_dirty = true;
-  return CVB_OK;
+  const int32_t k = kf_index;
+  return remove_batch(ctx, db, &k, 1, "cvb_db_remove");
+}
+
+int cvb_db_remove_batch(cvb_ctx* ctx, cvb_db* db, const int32_t* kf_index, int n) {
+  if (!ctx || !db) return CVB_ERR_INVALID;
+  CVB_GUARD(ctx);
+  return remove_batch(ctx, db, kf_index, n, "cvb_db_remove_batch");
 }
 
 int cvb_db_size(const cvb_db* db, int32_t* n_kf, int64_t* n_rows) {
@@ -737,6 +861,52 @@ int group_match(cvb_db_group* db, bool sift, const void* q, int nq, float thr, f
   return rank_fail(db, r, rc);
 }
 
+// The removals dealt to the ranks holding them; every rank that loses keyframes compacts its share on its own stream (all
+// enqueued first, then each stream waited for), and the global table is rebuilt once.  A rank keeps its keyframes in global
+// order, so a survivor's new local index is its rank in that order.
+int group_remove(cvb_db_group* db, const int32_t* kf_index, int n, const char* fn) {
+  cvb_group* g = db->g;
+  std::vector<char> gone;
+  int rc = check_removals(g->ctx[0], kf_index, n, (int)db->loc.size(), fn, gone);
+  if (rc || n == 0) return rc;
+  std::vector<char> rgone[CVB_GROUP_MAX];
+  bool loses[CVB_GROUP_MAX] = {};
+  for (int r = 0; r < g->n; r++) rgone[r].assign(db->db[r]->seg_ptr.size() - 1, 0);
+  for (size_t i = 0; i < gone.size(); i++)
+    if (gone[i]) {
+      rgone[db->loc[i].x][db->loc[i].y] = 1;
+      loses[db->loc[i].x] = true;
+    }
+  std::unique_ptr<cvb_block> stage[CVB_GROUP_MAX];
+  int fail = 0;
+  for (int r = 0; r < g->n && !rc; r++) {
+    if (!loses[r]) continue;
+    CVB_GUARD(g->ctx[r]);
+    cvb_db* d = db->db[r];
+    const int64_t before = d->seg_ptr.back();
+    if ((rc = compact(g->ctx[r], d, rgone[r], stage[r]))) fail = r;
+    db->rows[r] -= before - d->seg_ptr.back();
+  }
+  for (int r = 0; r < g->n; r++) {
+    if (!stage[r]) continue;
+    CVB_GUARD(g->ctx[r]);
+    const cudaError_t e = cudaStreamSynchronize(g->ctx[r]->stream);
+    if (!rc && e != cudaSuccess) {
+      rc = cvb_fail(g->ctx[r], CVB_ERR_CUDA, "%s: cudaStreamSynchronize failed: %s", fn, cudaGetErrorString(e));
+      fail = r;
+    }
+    stage[r].reset();
+  }
+  if (rc) return rank_fail(db, fail, rc);
+  int next[CVB_GROUP_MAX] = {};
+  size_t w = 0;
+  for (size_t i = 0; i < gone.size(); i++)
+    if (!gone[i]) db->loc[w++] = make_int2(db->loc[i].x, next[db->loc[i].x]++);
+  db->loc.resize(w);
+  db->loc_dirty = true;
+  return CVB_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -802,19 +972,14 @@ int cvb_db_group_append_sift(cvb_db_group* db, const float* rows, const int32_t*
 int cvb_db_group_remove(cvb_db_group* db, int kf_index) {
   if (!db) return CVB_ERR_INVALID;
   std::lock_guard<std::recursive_mutex> lk(db->g->call_mtx);
-  const int n_kf = (int)db->loc.size();
-  CVB_REQUIRE(db->g->ctx[0], kf_index >= 0 && kf_index < n_kf, "cvb_db_group_remove: keyframe index %d out of range (database holds %d)",
-              kf_index, n_kf);
-  const int r = db->loc[kf_index].x, l = db->loc[kf_index].y;
-  cvb_db* d = db->db[r];
-  const int64_t len = d->seg_ptr[l + 1] - d->seg_ptr[l];
-  if (const int rc = cvb_db_remove(db->g->ctx[r], d, l)) return rank_fail(db, r, rc);
-  db->rows[r] -= len;
-  db->loc.erase(db->loc.begin() + kf_index);
-  for (size_t i = (size_t)kf_index; i < db->loc.size(); i++)
-    if (db->loc[i].x == r) db->loc[i].y--;
-  db->loc_dirty = true;
-  return CVB_OK;
+  const int32_t k = kf_index;
+  return group_remove(db, &k, 1, "cvb_db_group_remove");
+}
+
+int cvb_db_group_remove_batch(cvb_db_group* db, const int32_t* kf_index, int n) {
+  if (!db) return CVB_ERR_INVALID;
+  std::lock_guard<std::recursive_mutex> lk(db->g->call_mtx);
+  return group_remove(db, kf_index, n, "cvb_db_group_remove_batch");
 }
 
 int cvb_db_group_size(const cvb_db_group* db, int32_t* n_kf, int64_t* n_rows, int64_t* rows_per_rank) {

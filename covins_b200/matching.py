@@ -36,6 +36,21 @@ def _seg(seg_ptr, n_rows):
     return _np(seg_ptr, np.int32)
 
 
+def _kf_indices(indices):
+    """a batch of keyframe indices as the contiguous int32 array cvb_db_remove_batch takes; anything that is not a 1-D list
+    of integers, or an index outside int32 (which the conversion would wrap onto another keyframe), is refused here"""
+    a = np.asarray(indices)
+    if a.size == 0:
+        return np.zeros(0, np.int32)
+    if a.ndim != 1 or not np.issubdtype(a.dtype, np.integer):
+        raise TypeError(f"keyframe indices must be a 1-D list of integers, got dtype {a.dtype} and shape {a.shape}")
+    lo, hi = np.iinfo(np.int32).min, np.iinfo(np.int32).max
+    bad = a[(a < lo) | (a > hi)]
+    if bad.size:
+        raise ValueError(f"keyframe index {int(bad[0])} is outside int32")
+    return np.ascontiguousarray(a, np.int32)
+
+
 def _is_torch(x):
     return hasattr(x, "data_ptr")
 
@@ -128,6 +143,13 @@ class DescriptorDatabase:
     def remove(self, kf_index: int):
         """a keyframe leaves the map (culling / erase): later keyframes move down by one index"""
         self.ctx.check(lib().cvb_db_remove(self.ctx.handle, self.handle, int(kf_index)))
+
+    def remove_batch(self, indices):
+        """a batch of keyframes leaves the map in one call (cvb_db_remove_batch): indices as before the call, in any order;
+        the result equals remove() of each from the highest to the lowest.  A survivor's index drops by the number of
+        removed indices below it."""
+        idx = _kf_indices(indices)
+        self.ctx.check(lib().cvb_db_remove_batch(self.ctx.handle, self.handle, _ptr(idx), len(idx)))
 
     def merge(self, other: "DescriptorDatabase"):
         """two agents' maps are merged: other's keyframes are appended after this database's, in other's order, copied
@@ -229,6 +251,11 @@ class DescriptorDatabaseGroup:
     def remove(self, kf_index: int):
         """a keyframe leaves the map: later keyframes move down by one global index"""
         self.ctx.check(lib().cvb_db_group_remove(self.handle, int(kf_index)))
+
+    def remove_batch(self, indices):
+        """as DescriptorDatabase.remove_batch; each rank compacts its share on its own device (cvb_db_group_remove_batch)"""
+        idx = _kf_indices(indices)
+        self.ctx.check(lib().cvb_db_group_remove_batch(self.handle, _ptr(idx), len(idx)))
 
     def merge(self, other: "DescriptorDatabaseGroup"):
         """as DescriptorDatabase.merge, rank by rank on the group's devices (cvb_db_group_merge): other's keyframes follow

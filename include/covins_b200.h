@@ -107,7 +107,7 @@ CVB_API int cvb_match_hamming_batch_dev(cvb_ctx* ctx, const uint8_t* d_q, int nq
  *
  * cvb_db_create: desc_bytes 32 = ORB rows (cvb_db_append, cvb_db_match_hamming[_dev]); 128 = SIFT rows (cvb_db_append_sift,
  * cvb_db_match_l2[_dev]); any other value → CVB_ERR_UNSUPPORTED.  A call of the other row kind → CVB_ERR_INVALID with a
- * message.  cvb_db_reserve, cvb_db_remove and cvb_db_size serve both kinds.
+ * message.  cvb_db_reserve, cvb_db_remove, cvb_db_remove_batch and cvb_db_size serve both kinds.
  */
 typedef struct cvb_db cvb_db;
 CVB_API int cvb_db_create(cvb_ctx* ctx, int desc_bytes, cvb_db** out);
@@ -117,8 +117,24 @@ CVB_API int cvb_db_append(cvb_ctx* ctx, cvb_db* db, const uint8_t* rows, const i
 CVB_API int cvb_db_size(const cvb_db* db, int32_t* n_kf, int64_t* n_rows);
 /* A keyframe leaves the map (Keyframe::SetInvalid / culling, keyframe_be.cpp:413-440; Map::EraseKeyframe): its segment is
  * cut out of the resident descriptor array; the database indices of the keyframes appended after it drop by one (the
- * order of the remaining keyframes is kept, like erasing from a vector). */
+ * order of the remaining keyframes is kept, like erasing from a vector).  It is cvb_db_remove_batch of one index. */
 CVB_API int cvb_db_remove(cvb_ctx* ctx, cvb_db* db, int kf_index);
+/*
+ * A batch of keyframes leaves the map in one call (the keyframes Map::Clean culls, keyframe_be.cpp:413-440, or erases).
+ * kf_index [n]: database indices as they are BEFORE the call, in any order.  The result is that of calling cvb_db_remove
+ * for each index from the highest to the lowest: every later cvb_db_size, request (cvb_db_match_hamming / _l2 and their
+ * _dev forms), append, remove and merge is bit-identical to what it would be after that loop.  A surviving keyframe's new
+ * index is its old index minus the number of removed indices below it.  ORB and SIFT databases alike.
+ *   n == 0 does nothing and launches nothing.
+ *   Refusals, before any device work and with the database unchanged, each CVB_ERR_INVALID with a message naming the
+ *   index: n < 0, kf_index == NULL with n > 0, an index out of range, an index given twice.
+ *   Device work: only the suffix from the first removed keyframe moves.  Its kept keyframes' rows, and then their operand
+ *   tiles, are gathered into a scratch block of the stream-ordered pool by one launch per array and copied back by one
+ *   device-to-device copy per array (so a single removal moves exactly the bytes it always did, and the extra memory is at
+ *   most the moved suffix of one array).  Nothing is launched for an array when no kept byte follows the first removed
+ *   keyframe.  The host segment tables are rebuilt once; at most one host synchronisation, however many keyframes go.
+ */
+CVB_API int cvb_db_remove_batch(cvb_ctx* ctx, cvb_db* db, const int32_t* kf_index, int n);
 CVB_API int cvb_db_match_hamming(cvb_ctx* ctx, cvb_db* db, const uint8_t* q, int nq, float thr, float ratio,
                                  int32_t* n_matches, int32_t* m_kf, int32_t* m_query, int32_t* m_train,
                                  float* m_dist, int cap, int32_t* n_total);
@@ -1046,7 +1062,16 @@ CVB_API int cvb_db_group_create(cvb_group* g, int desc_bytes, cvb_db_group** out
 CVB_API int cvb_db_group_destroy(cvb_db_group* db);
 CVB_API int cvb_db_group_append(cvb_db_group* db, const uint8_t* rows, const int32_t* rows_per_kf, int n_kf);
 CVB_API int cvb_db_group_append_sift(cvb_db_group* db, const float* rows, const int32_t* rows_per_kf, int n_kf);
-CVB_API int cvb_db_group_remove(cvb_db_group* db, int kf_index);
+CVB_API int cvb_db_group_remove(cvb_db_group* db, int kf_index);   /* cvb_db_group_remove_batch of one index */
+/*
+ * cvb_db_remove_batch for the group: same index meaning, result and refusals (before any rank is touched).  The removals
+ * are dealt to the ranks that hold them through the global -> (rank, local index) table; each rank that loses keyframes
+ * compacts its share as cvb_db_remove_batch does, on its own stream (the calling thread enqueues every rank's work, then
+ * waits for each), and the table is rebuilt once.  Keyframes never move between ranks; rows_per_rank and the placement of
+ * later appends follow from the new state.  A CUDA failure is reported as "rank r: <message>" on ctxs[0] and leaves the
+ * database undefined.
+ */
+CVB_API int cvb_db_group_remove_batch(cvb_db_group* db, const int32_t* kf_index, int n);
 CVB_API int cvb_db_group_size(const cvb_db_group* db, int32_t* n_kf, int64_t* n_rows, int64_t* rows_per_rank);
 CVB_API int cvb_db_group_match_hamming(cvb_db_group* db, const uint8_t* q, int nq, float thr, float ratio, int32_t* n_matches,
                                        int32_t* m_kf, int32_t* m_query, int32_t* m_train, float* m_dist, int cap, int32_t* n_total);
