@@ -79,29 +79,9 @@ static_assert(cvb_chol::T == 128, "s_at assumes 128-wide tiles");
 constexpr int RED_BLOCKS = 512;   // fixed grid for reducing kernels → fixed summation order
 constexpr int RED_SLOTS = 8;
 
-// Device arrays come from the stream-ordered allocator on the engine's stream: the pool (release threshold raised in
-// cvb_ctx_create) keeps freed blocks, so building a second problem re-uses the first one's memory instead of paying
-// cudaMalloc/cudaFree (which cost ~100 ms of a 180 ms set-up at C3, the 7.4 GB S buffer alone several ms each way).
-// t_alloc_stream is (re)set by BaEnter at EVERY cvb_ba_* entry point (a handle may be driven from any host thread, and
-// several handles may exist); an array is freed on the stream it was allocated on.
-static thread_local cudaStream_t t_alloc_stream = nullptr;
-template <typename T>
-struct DevArr {
-  T* p = nullptr;
-  size_t n = 0;
-  cudaStream_t st = nullptr;
-  int alloc(size_t count) {
-    n = count;
-    if (count == 0) count = 1;
-    st = t_alloc_stream;
-    return cudaMallocAsync(&p, count * sizeof(T), st) == cudaSuccess ? 0 : 1;
-  }
-  void free_() {
-    if (p) cudaFreeAsync(p, st);
-    p = nullptr;
-  }
-};
-
+// The engine's device arrays come from the stream-ordered allocator on the engine's stream: the pool (release threshold
+// raised in cvb_ctx_create) keeps freed blocks, so building a second problem re-uses the first one's memory instead of
+// paying cudaMalloc/cudaFree (which cost ~100 ms of a 180 ms set-up at C3, the 7.4 GB S buffer alone several ms each way).
 struct Engine {
   cvb_ctx* ctx = nullptr;
   cudaStream_t st = nullptr;
@@ -115,61 +95,62 @@ struct Engine {
   std::vector<int> obs_of_compact;       // compact observation → original index
   std::vector<uint8_t> h_const;
   // device state (double buffered)
-  DevArr<double> pose[2], sb[2], lm[2];
-  DevArr<double> pose0, sb0, lm0;   // the state the problem was created with (cvb_ba_restart returns to it)
-  DevArr<uint8_t> pose_const;
-  DevArr<int> off_pose, off_sb;
+  cvb_dev_arr<double> pose[2], sb[2], lm[2];
+  cvb_dev_arr<double> pose0, sb0, lm0;   // the state the problem was created with (cvb_ba_restart returns to it)
+  cvb_dev_arr<uint8_t> pose_const;
+  cvb_dev_arr<int> off_pose, off_sb;
   // multi-GPU exchange of the reduced camera system: packed ids of the structurally non-zero (pre-fill) tiles — all of
   // them (all-reduce fallback, through xbuf) / those of the tile columns this rank owns (reduce-scatter by peer pull)
-  DevArr<int> xt_all, xt_own, col_owner;
-  DevArr<double> xbuf, flagd;
+  cvb_dev_arr<int> xt_all, xt_own, col_owner;
+  cvb_dev_arr<double> xbuf, flagd;
   int n_xt_all = 0, n_xt_own = 0;
   size_t n_tiles = 0;                           // tiles of L's structure = length of S in tiles
   // peer access: S, linv and the panel flags of every rank are mapped here (enable_p2p: through CUDA IPC, or handed over
   // by an in-process group, peer_ipc = false)
   bool p2p = false, peer_ipc = false;
-  double* S_raw = nullptr;                      // cudaMalloc'ed (IPC-exportable) when world > 1, else pool memory
-  double* linv_raw = nullptr;
-  int* pflag_raw = nullptr;
   cvb_chol::DistView dv;
-  double** d_peer_S = nullptr;
+  cvb_dev_arr<int> epoch;                       // dv.d_epoch
+  cvb_dev_arr<int*> peer_flag;                  // dv.d_peer_flag
+  cvb_dev_arr<double*> peer_S;                  // dv.peer_S on the device (reduce_pull_kernel)
   std::vector<uint8_t> h_prefill;               // tile mask of S before fill (the distributed plan is rebuilt from it)
   std::vector<int> h_owner;                     // tile column → owning rank
   std::vector<int> h_off_pose, h_off_sb;
   cvb_chol::TilePlan plan;
-  DevArr<double> extr_kf, intr_kf, dist_kf, xi_kf;
-  DevArr<int> model_kf;   // cam model | dist model << 8, per keyframe
-  DevArr<int> obs_kf, obs_lm, lm_ptr, kf_ptr, kf_obs;
-  DevArr<double> obs_uv, obs_sigma;
-  DevArr<ObsLin> lin;
-  DevArr<ObsW> ow;
-  DevArr<double> Hll, HllInv, bl;
+  cvb_dev_arr<double> extr_kf, intr_kf, dist_kf, xi_kf;
+  cvb_dev_arr<int> model_kf;   // cam model | dist model << 8, per keyframe
+  cvb_dev_arr<int> obs_kf, obs_lm, lm_ptr, kf_ptr, kf_obs;
+  cvb_dev_arr<double> obs_uv, obs_sigma;
+  cvb_dev_arr<ObsLin> lin;
+  cvb_dev_arr<ObsW> ow;
+  cvb_dev_arr<double> Hll, HllInv, bl;
   // imu
-  DevArr<ImuPre> pre;
-  DevArr<int> imu_i, imu_j;
-  DevArr<double> Jimu, rimu;
+  cvb_dev_arr<ImuPre> pre;
+  cvb_dev_arr<int> imu_i, imu_j;
+  cvb_dev_arr<double> Jimu, rimu;
   // edges
-  DevArr<int> edge_i, edge_j;
-  DevArr<double> edge_q, edge_t, edge_S, Jedge, redge;
-  DevArr<uint8_t> edge_robust;
+  cvb_dev_arr<int> edge_i, edge_j;
+  cvb_dev_arr<double> edge_q, edge_t, edge_S, Jedge, redge;
+  cvb_dev_arr<uint8_t> edge_robust;
   // gather structures
-  DevArr<int> fb_hi, fb_lo, fb_ptr, ft_type, ft_fac, ft_rhi, ft_rlo;   // factor blocks / terms
+  cvb_dev_arr<int> fb_hi, fb_lo, fb_ptr, ft_type, ft_fac, ft_rhi, ft_rlo;   // factor blocks / terms
   int n_fb = 0;
-  DevArr<int> sb_hi, sb_lo, sb_ptr, sp_a, sp_b;                         // schur blocks / pairs
-  DevArr<int> kf_sb;                                                    // first schur block of each hi keyframe
-  int n_sb = 0, row_stage = 0;                                          // row_stage: observations schur_row_kernel stages
+  cvb_dev_arr<int> sb_hi, sb_lo, sb_ptr, sp_a, sp_b;                        // schur blocks / pairs
+  cvb_dev_arr<int> kf_sb;                                                   // first schur block of each hi keyframe
+  int n_sb = 0, row_stage = 0;                                              // row_stage: observations schur_row_kernel stages
   // vectors of size n_vec: [cam part n_c_pad | landmark part 3 L_in]
-  DevArr<double> scale, colsq, diag, gvec, grad, sgrad, gn, step, xsol, yb, gs, tmp;
-  DevArr<double> scale0;   // 0/1 activity mask of this rank's columns: engine_begin derives `scale` from it
-  DevArr<double> S, linv;
+  cvb_dev_arr<double> scale, colsq, diag, gvec, grad, sgrad, gn, step, xsol, yb, gs, tmp;
+  cvb_dev_arr<double> scale0;   // 0/1 activity mask of this rank's columns: engine_begin derives `scale` from it
+  // S, the tile inverses and (world > 1) the panel flags; from cudaMalloc when world > 1, to be exported through CUDA IPC
+  cvb_dev_arr<double> S, linv;
+  cvb_dev_arr<int> pflag;
   // S's fill tiles (in L's structure, not in S's): zeroed on st_fill beside the block kernels, joined before the factor
-  DevArr<int> xt_fill;
+  cvb_dev_arr<int> xt_fill;
   int n_xt_fill = 0;
   cudaStream_t st_fill = nullptr;
   cudaEvent_t ev_fill_fork = nullptr, ev_fill_done = nullptr;
   bool fill_pending = false;
-  DevArr<int> flag;
-  DevArr<double> partials, scalars, rankmax;
+  cvb_dev_arr<int> flag;
+  cvb_dev_arr<double> partials, scalars, rankmax;
   double* h_scalars = nullptr;   // pinned
   int cur = 0;
   // trust-region state (Ceres DoglegStrategy / TrustRegionMinimizer)
@@ -189,53 +170,20 @@ struct Engine {
   double phase_ms[5] = {0, 0, 0, 0, 0};
   double chol_flops = 0.0;
   ~Engine() {
-    const bool trace = getenv("COVINS_B200_SETUP_TRACE") != nullptr;
-    auto t_prev = std::chrono::steady_clock::now();
-    auto lap = [&](const char* what) {
-      if (!trace) return;
-      const auto now = std::chrono::steady_clock::now();
-      fprintf(stderr, "[destroy] %-26s %8.2f ms\n", what, std::chrono::duration<double, std::milli>(now - t_prev).count());
-      t_prev = now;
-    };
     if (st_fill) { cudaStreamSynchronize(st_fill); cudaStreamDestroy(st_fill); }   // S may still be being cleared
     if (ev_fill_fork) cudaEventDestroy(ev_fill_fork);
     if (ev_fill_done) cudaEventDestroy(ev_fill_done);
-    for (int i = 0; i < 2; i++) { pose[i].free_(); sb[i].free_(); lm[i].free_(); }
-    pose0.free_(); sb0.free_(); lm0.free_();
-    pose_const.free_(); off_pose.free_(); off_sb.free_(); xt_all.free_(); xt_own.free_(); col_owner.free_(); xbuf.free_(); flagd.free_(); plan.release(); extr_kf.free_(); intr_kf.free_(); dist_kf.free_(); xi_kf.free_(); model_kf.free_();
-    obs_kf.free_(); obs_lm.free_(); lm_ptr.free_(); kf_ptr.free_(); kf_obs.free_(); obs_uv.free_(); obs_sigma.free_();
-    lin.free_(); ow.free_(); Hll.free_(); HllInv.free_(); bl.free_();
-    pre.free_(); imu_i.free_(); imu_j.free_(); Jimu.free_(); rimu.free_();
-    edge_i.free_(); edge_j.free_(); edge_q.free_(); edge_t.free_(); edge_S.free_(); Jedge.free_(); redge.free_();
-    edge_robust.free_();
-    fb_hi.free_(); fb_lo.free_(); fb_ptr.free_(); ft_type.free_(); ft_fac.free_(); ft_rhi.free_(); ft_rlo.free_();
-    sb_hi.free_(); sb_lo.free_(); sb_ptr.free_(); sp_a.free_(); sp_b.free_(); kf_sb.free_();
-    scale.free_(); scale0.free_(); colsq.free_(); diag.free_(); gvec.free_(); grad.free_(); sgrad.free_(); gn.free_(); step.free_();
-    xsol.free_(); yb.free_(); gs.free_(); tmp.free_(); xt_fill.free_();
-    if (S_raw) { S.p = nullptr; linv.p = nullptr; }
-    S.free_(); linv.free_(); flag.free_(); partials.free_();
-    scalars.free_(); rankmax.free_();
     for (int g = 0; g < dv.world && p2p && peer_ipc; g++) {
       if (g == dv.rank) continue;
       if (dv.peer_S[g]) cudaIpcCloseMemHandle(dv.peer_S[g]);
       if (dv.peer_linv[g]) cudaIpcCloseMemHandle(dv.peer_linv[g]);
       if (dv.peer_flag[g]) cudaIpcCloseMemHandle(dv.peer_flag[g]);
     }
-    if (S_raw) cudaFree(S_raw);
-    if (linv_raw) cudaFree(linv_raw);
-    if (pflag_raw) cudaFree(pflag_raw);
-    if (dv.d_epoch) cudaFree(dv.d_epoch);
-    if (dv.d_peer_flag) cudaFree(dv.d_peer_flag);
-    if (d_peer_S) cudaFree(d_peer_S);
-    lap("device arrays");
     if (h_scalars) cudaFreeHost(h_scalars);
-    lap("pinned scalars");
     for (auto& e : ev) if (e) cudaEventDestroy(e);
     fs.destroy();
-    lap("events, streams");
     if (g_factor) cudaGraphExecDestroy(g_factor);
     if (g_solve) cudaGraphExecDestroy(g_solve);
-    lap("graphs");
   }
 };
 
@@ -1172,31 +1120,37 @@ namespace {
 #define ENG_LAUNCH() CVB_CHECK_LAUNCH(E.ctx)
 
 template <typename T>
-int upload(Engine& E, DevArr<T>& d, const T* h, size_t n) {
-  if (d.alloc(n)) return cvb_fail(E.ctx, CVB_ERR_CUDA, "cudaMalloc failed (%zu bytes)", n * sizeof(T));
+int upload(Engine& E, cvb_dev_arr<T>& d, const T* h, size_t n) {
+  if (d.alloc(n, E.st)) return cvb_fail(E.ctx, CVB_ERR_CUDA, "cudaMalloc failed (%zu bytes)", n * sizeof(T));
   if (n) ENG_CUDA(cudaMemcpyAsync(d.p, h, n * sizeof(T), cudaMemcpyHostToDevice, E.st));
   return CVB_OK;
 }
 template <typename T>
-int upload(Engine& E, DevArr<T>& d, const std::vector<T>& h) {
+int upload(Engine& E, cvb_dev_arr<T>& d, const std::vector<T>& h) {
   return upload(E, d, h.data(), h.size());
 }
+// for_ipc: see cvb_dev_arr
 template <typename T>
-int zalloc(Engine& E, DevArr<T>& d, size_t n) {
-  if (d.alloc(n)) return cvb_fail(E.ctx, CVB_ERR_CUDA, "cudaMalloc failed (%zu bytes)", n * sizeof(T));
+int zalloc(Engine& E, cvb_dev_arr<T>& d, size_t n, bool for_ipc = false) {
+  if (d.alloc(n, E.st, for_ipc)) return cvb_fail(E.ctx, CVB_ERR_CUDA, "cudaMalloc failed (%zu bytes)", n * sizeof(T));
   ENG_CUDA(cudaMemsetAsync(d.p, 0, (n ? n : 1) * sizeof(T), E.st));
   return CVB_OK;
 }
 
 inline int grid1(size_t n, int b = 256) { return (int)((n + b - 1) / b); }
 
+int ar(Engine& E, double* p, size_t n) {
+  if (E.allreduce && E.world > 1) {
+    int rc = E.allreduce(p, n);
+    if (rc) return cvb_fail(E.ctx, CVB_ERR_CUDA, "allreduce callback failed (%d)", rc);
+  }
+  return CVB_OK;
+}
+
 int read_scalars(Engine& E, int nslots) {
   reduce_final<<<1, 256, 0, E.st>>>(E.partials.p, E.scalars.p, nslots, 0);
   ENG_LAUNCH();
-  if (E.allreduce && E.world > 1) {
-    int rc = E.allreduce(E.scalars.p, (size_t)nslots);
-    if (rc) return cvb_fail(E.ctx, CVB_ERR_CUDA, "allreduce callback failed (%d)", rc);
-  }
+  if (int rc = ar(E, E.scalars.p, (size_t)nslots)) return rc;
   ENG_CUDA(cudaMemcpyAsync(E.h_scalars, E.scalars.p, nslots * sizeof(double), cudaMemcpyDeviceToHost, E.st));
   ENG_CUDA(cudaStreamSynchronize(E.st));
   return CVB_OK;
@@ -1281,13 +1235,13 @@ int build_schur_lists(Engine& E, const std::vector<int>& h_lm_ptr, int K) {
     if ((rc = zalloc(E, E.sb_hi, 0)) || (rc = zalloc(E, E.sb_lo, 0)) || (rc = zalloc(E, E.sb_ptr, 1))) return rc;
     return CVB_OK;
   }
-  DevArr<long long> d_pair_ptr;
-  DevArr<unsigned long long> k0, k1, v0, v1;
-  DevArr<int> head, blk, kf_pos;
-  DevArr<unsigned char> tmp;
+  cvb_dev_arr<long long> d_pair_ptr;
+  cvb_dev_arr<unsigned long long> k0, k1, v0, v1;
+  cvb_dev_arr<int> head, blk, kf_pos;
+  cvb_dev_arr<unsigned char> tmp;
   if ((rc = upload(E, d_pair_ptr, h_pair_ptr))) return rc;
-  if (k0.alloc((size_t)np) || k1.alloc((size_t)np) || v0.alloc((size_t)np) || v1.alloc((size_t)np) || head.alloc((size_t)np + 1) ||
-      blk.alloc((size_t)np + 1) || kf_pos.alloc((size_t)E.n_obs))
+  if (k0.alloc((size_t)np, E.st) || k1.alloc((size_t)np, E.st) || v0.alloc((size_t)np, E.st) || v1.alloc((size_t)np, E.st) ||
+      head.alloc((size_t)np + 1, E.st) || blk.alloc((size_t)np + 1, E.st) || kf_pos.alloc((size_t)E.n_obs, E.st))
     return cvb_fail(E.ctx, CVB_ERR_CUDA, "cudaMalloc failed (Schur pair scratch, %lld pairs)", np);
   kf_pos_kernel<<<grid1((size_t)E.n_obs), 256, 0, E.st>>>(E.n_obs, E.kf_ptr.p, E.kf_obs.p, E.obs_kf.p, kf_pos.p);
   ENG_LAUNCH();
@@ -1300,7 +1254,7 @@ int build_schur_lists(Engine& E, const std::vector<int>& h_lm_ptr, int K) {
   cub::DeviceRadixSort::SortPairs(nullptr, t2, k1.p, k0.p, v1.p, v0.p, (int)np, 32, 32 + bits, E.st);
   cub::DeviceScan::ExclusiveSum(nullptr, t3, head.p, blk.p, (int)np + 1, E.st);
   size_t tb = std::max(t1, std::max(t2, t3));
-  if (tmp.alloc(tb ? tb : 1)) return cvb_fail(E.ctx, CVB_ERR_CUDA, "cudaMalloc failed (sort scratch)");
+  if (tmp.alloc(tb ? tb : 1, E.st)) return cvb_fail(E.ctx, CVB_ERR_CUDA, "cudaMalloc failed (sort scratch)");
   ENG_CUDA(cub::DeviceRadixSort::SortPairs(tmp.p, tb, k0.p, k1.p, v0.p, v1.p, (int)np, 0, bits, E.st));        // by lo keyframe
   ENG_CUDA(cub::DeviceRadixSort::SortPairs(tmp.p, tb, k1.p, k0.p, v1.p, v0.p, (int)np, 32, 32 + bits, E.st));  // by hi (stable)
   pair_heads_kernel<<<grid1((size_t)np), 256, 0, E.st>>>(np, k0.p, head.p);
@@ -1321,7 +1275,6 @@ int build_schur_lists(Engine& E, const std::vector<int>& h_lm_ptr, int K) {
   const int np_i = (int)np;
   ENG_CUDA(cudaMemcpyAsync(E.sb_ptr.p + n_sb, &np_i, sizeof(int), cudaMemcpyHostToDevice, E.st));
   ENG_CUDA(cudaStreamSynchronize(E.st));   // scratch arrays are freed on return
-  d_pair_ptr.free_(); k0.free_(); k1.free_(); v0.free_(); v1.free_(); head.free_(); blk.free_(); kf_pos.free_(); tmp.free_();
   return CVB_OK;
 }
 
@@ -1341,6 +1294,95 @@ int check_problem(cvb_ctx* ctx, const cvb_ba_problem* p, int visual_only) {
     for (int ob = p->lm_obs_ptr[l]; ob < p->lm_obs_ptr[l + 1]; ob++)
       CVB_REQUIRE(ctx, p->obs_kf[ob] >= 0 && p->obs_kf[ob] < K, "obs_kf out of range");
   return CVB_OK;
+}
+
+// The connected components of the keyframes 0..K-1 under links (pairs of keyframes) that have at least min_size
+// keyframes: each in ascending keyframe order, the components in order of their first keyframe.
+std::vector<std::vector<int>> kf_components(int K, const std::vector<std::pair<int, int>>& links, int min_size) {
+  std::vector<int> parent(K);
+  std::iota(parent.begin(), parent.end(), 0);
+  const auto find = [&](int x) { while (parent[x] != x) { parent[x] = parent[parent[x]]; x = parent[x]; } return x; };
+  for (const auto& l : links) {
+    const int a = find(l.first), b = find(l.second);
+    if (a != b) parent[std::max(a, b)] = std::min(a, b);   // the root of a component is its first keyframe
+  }
+  std::vector<std::vector<int>> of_root(K), comps;
+  for (int k = 0; k < K; k++) of_root[find(k)].push_back(k);
+  for (auto& c : of_root)
+    if ((int)c.size() >= min_size) comps.push_back(std::move(c));
+  return comps;
+}
+
+// Column layout of the reduced camera system (see cam_col()): the first column of every keyframe's pose block (off_pose)
+// and speed-bias block (off_sb), and the column group of every tile nd_layout() laid out; returns the number of columns.
+// The factorisation's schedule, and so the bits of the result, depend on this layout.
+int column_layout(const cvb_ba_problem* p, bool visual_only, bool pose_graph, std::vector<int>& off_pose, std::vector<int>& off_sb,
+                  std::vector<int>& group_of_tile) {
+  const int K = p->K, TT = cvb_chol::T;
+  const auto pad = [TT](int c) { return ((c + TT - 1) / TT) * TT; };
+  off_pose.resize(K); off_sb.assign(K, 0);
+  group_of_tile.clear();
+  std::vector<char> in_chain(K, 0);
+  if (!visual_only) {
+    // [speed-bias blocks (9 each) | pad to a tile | pose blocks (6 each)].  Every IMU chain (connected component of the
+    // IMU factor graph, i.e. one agent's trajectory) starts on a tile boundary, so that the tile-level elimination of one
+    // chain never touches another chain's tiles (a tile shared by two chains would carry the first chain's pose clique
+    // along the whole second chain).
+    std::vector<std::pair<int, int>> links;
+    for (int f = 0; f < p->n_imu; f++) links.push_back({p->imu_i[f], p->imu_j[f]});
+    const auto chains = kf_components(K, links, 2);
+    for (const auto& c : chains)
+      for (int k : c) in_chain[k] = 1;
+    int cursor = cvb_chol::nd_layout(chains, 9, off_sb, group_of_tile) * TT;
+    for (int k = 0; k < K; k++)                     // keyframes without an IMU factor: isolated speed-bias blocks
+      if (!in_chain[k]) { off_sb[k] = cursor; cursor += 9; }
+    // poses: chain by chain, each chain on its own tiles (so that the chains' eliminations touch disjoint tiles and
+    // can run concurrently), then the keyframes without IMU factors
+    for (const auto& c : chains) {
+      cursor = pad(cursor);
+      for (int k : c) { off_pose[k] = cursor; cursor += 6; }
+    }
+    cursor = pad(cursor);
+    for (int k = 0; k < K; k++)
+      if (!in_chain[k]) { off_pose[k] = cursor; cursor += 6; }
+    return cursor;
+  }
+  if (pose_graph) {
+    // Pose graph (PoseGraphOptimization: no landmarks, only between-factors): the keyframes of one agent form a banded chain
+    // (successor + 5 predecessor edges, optimization_be.cpp:947-1021) and the few loop edges couple distant keyframes.  In
+    // plain keyframe order the tile columns are one long dependent chain (94 columns x ~100 us at C3).  Nested dissection
+    // by hand: the endpoints of long-range edges go to a per-chain BORDER segment at the end; what remains are independent
+    // banded chains, each laid out on its own tiles → they are eliminated concurrently as column groups (like the IMU chains
+    // of the visual-inertial problem), then the small border is factored.  A chain's columns only ever touch its own tiles
+    // and its own border segment, so concurrent groups never update the same tile.
+    std::vector<char> border(K, 0);
+    std::vector<std::pair<int, int>> links;   // a chain = connected through short-range edges (border keyframes included)
+    for (int e = 0; e < p->n_edge; e++) {
+      if (std::abs(p->edge_i[e] - p->edge_j[e]) > 8) border[p->edge_i[e]] = border[p->edge_j[e]] = 1;
+      else links.push_back({p->edge_i[e], p->edge_j[e]});
+    }
+    const auto chains = kf_components(K, links, 64);
+    std::vector<std::vector<int>> members;    // interiors of the big chains: one column group each
+    for (const auto& c : chains) {
+      members.emplace_back();
+      for (int k : c) {
+        in_chain[k] = 1;
+        if (!border[k]) members.back().push_back(k);
+      }
+      if (members.back().empty()) members.pop_back();
+    }
+    int cursor = cvb_chol::nd_layout(members, 6, off_pose, group_of_tile) * TT;
+    for (int k = 0; k < K; k++)                   // small components: main sequence
+      if (!in_chain[k]) { off_pose[k] = cursor; cursor += 6; }
+    for (const auto& c : chains) {                // per-chain border segments
+      cursor = pad(cursor);
+      for (int k : c)
+        if (border[k]) { off_pose[k] = cursor; cursor += 6; }
+    }
+    return cursor;
+  }
+  for (int k = 0; k < K; k++) off_pose[k] = 6 * k;
+  return 6 * K;
 }
 
 // fill (cvb_ba_solve_dev_edges, single rank only): the start poses and edge measurements are written on the device by
@@ -1387,7 +1429,6 @@ int engine_setup(Engine& E, const cvb_ba_problem* p, const cvb_ba_options* o, co
       for (int ob = p->lm_obs_ptr[l]; ob < p->lm_obs_ptr[l + 1]; ob++) {
         if (p->obs_skip && p->obs_skip[ob]) continue;
         const int kf = p->obs_kf[ob];
-        CVB_REQUIRE(ctx, kf >= 0 && kf < K, "obs_kf out of range");
         CVB_REQUIRE(ctx, kf > prev, "observations of a landmark must be sorted by keyframe index and unique");
         prev = kf;
         h_obs_kf.push_back(kf);
@@ -1402,94 +1443,9 @@ int engine_setup(Engine& E, const cvb_ba_problem* p, const cvb_ba_options* o, co
   E.L_in = (int)E.lm_of_compact.size();
   E.n_obs = (int)h_obs_kf.size();
   E.n_c = K * E.per;
-  // column layout of the reduced camera system: [speed-bias blocks (9 each, keyframe order) | pad to a tile | pose
-  // blocks (6 each)] — see cam_col()
-  const int TT = cvb_chol::T;
-  // Speed-bias layout: every IMU chain (connected component of the IMU factor graph, i.e. one agent's trajectory)
-  // starts on a tile boundary, so that the tile-level elimination of one chain never touches another chain's tiles
-  // (a tile shared by two chains would carry the first chain's pose clique along the whole second chain).
-  E.h_off_pose.resize(K); E.h_off_sb.assign(K, 0);
-  int n_sb_pad = 0, n_total = 0;
   std::vector<int> group_of_tile;   // column group of every tile cvb_chol::nd_layout() laid out (tiles 0, 1, ...)
-  if (!E.visual_only) {
-    std::vector<int> parent(K);
-    std::iota(parent.begin(), parent.end(), 0);
-    std::function<int(int)> find = [&](int x) { while (parent[x] != x) { parent[x] = parent[parent[x]]; x = parent[x]; } return x; };
-    for (int f = 0; f < p->n_imu; f++) {
-      const int a = find(p->imu_i[f]), b = find(p->imu_j[f]);
-      if (a != b) parent[std::max(a, b)] = std::min(a, b);
-    }
-    std::vector<int> comp_size(K, 0);
-    for (int k = 0; k < K; k++) comp_size[find(k)]++;
-    std::vector<int> roots;
-    std::vector<std::vector<int>> members;
-    for (int root = 0; root < K; root++) {          // chains with >= 2 keyframes, in order of their first keyframe
-      if (find(root) != root || comp_size[root] < 2) continue;
-      roots.push_back(root);
-      members.emplace_back();
-      for (int k = root; k < K; k++)
-        if (find(k) == root) members.back().push_back(k);
-    }
-    int cursor = cvb_chol::nd_layout(members, 9, E.h_off_sb, group_of_tile) * TT;
-    for (int k = 0; k < K; k++)                     // keyframes without an IMU factor: isolated speed-bias blocks
-      if (comp_size[find(k)] < 2) { E.h_off_sb[k] = cursor; cursor += 9; }
-    n_sb_pad = ((cursor + TT - 1) / TT) * TT;
-    // poses: chain by chain, each chain on its own tiles (so that the chains' eliminations touch disjoint tiles and
-    // can run concurrently), then the keyframes without IMU factors
-    cursor = n_sb_pad;
-    for (int root : roots) {
-      cursor = ((cursor + TT - 1) / TT) * TT;
-      for (int k = root; k < K; k++)
-        if (find(k) == root) { E.h_off_pose[k] = cursor; cursor += 6; }
-    }
-    cursor = ((cursor + TT - 1) / TT) * TT;
-    for (int k = 0; k < K; k++)
-      if (comp_size[find(k)] < 2) { E.h_off_pose[k] = cursor; cursor += 6; }
-    n_total = cursor;
-  } else if (E.L_in == 0 && p->n_edge > 0) {
-    // Pose graph (PoseGraphOptimization: no landmarks, only between-factors): the keyframes of one agent form a banded chain
-    // (successor + 5 predecessor edges, optimization_be.cpp:947-1021) and the few loop edges couple distant keyframes.  In
-    // plain keyframe order the tile columns are one long dependent chain (94 columns x ~100 us at C3).  Nested dissection
-    // by hand: the endpoints of long-range edges go to a per-chain BORDER segment at the end; what remains are independent
-    // banded chains, each laid out on its own tiles → they are eliminated concurrently as column groups (like the IMU chains
-    // of the visual-inertial problem), then the small border is factored.  A chain's columns only ever touch its own tiles
-    // and its own border segment, so concurrent groups never update the same tile.
-    std::vector<char> border(K, 0);
-    for (int e = 0; e < p->n_edge; e++)
-      if (std::abs(p->edge_i[e] - p->edge_j[e]) > 8) border[p->edge_i[e]] = border[p->edge_j[e]] = 1;
-    std::vector<int> parent(K);
-    std::iota(parent.begin(), parent.end(), 0);
-    std::function<int(int)> find = [&](int x) { while (parent[x] != x) { parent[x] = parent[parent[x]]; x = parent[x]; } return x; };
-    for (int e = 0; e < p->n_edge; e++) {
-      if (std::abs(p->edge_i[e] - p->edge_j[e]) > 8) continue;       // a chain = connected through short-range edges (border keyframes included)
-      const int a = find(p->edge_i[e]), b = find(p->edge_j[e]);
-      if (a != b) parent[std::max(a, b)] = std::min(a, b);
-    }
-    std::vector<int> comp_size(K, 0);
-    for (int k = 0; k < K; k++) comp_size[find(k)]++;
-    std::vector<int> roots;
-    for (int r = 0; r < K; r++)
-      if (find(r) == r && comp_size[r] >= 64) roots.push_back(r);
-    std::vector<std::vector<int>> members;                            // interiors of the big chains: one column group each
-    for (int r : roots) {
-      members.emplace_back();
-      for (int k = r; k < K; k++)
-        if (find(k) == r && !border[k]) members.back().push_back(k);
-      if (members.back().empty()) members.pop_back();
-    }
-    int cursor = cvb_chol::nd_layout(members, 6, E.h_off_pose, group_of_tile) * TT;
-    for (int k = 0; k < K; k++)                                       // small components: main sequence
-      if (comp_size[find(k)] < 64) { E.h_off_pose[k] = cursor; cursor += 6; }
-    for (int r : roots) {                                             // per-chain border segments
-      cursor = ((cursor + TT - 1) / TT) * TT;
-      for (int k = r; k < K; k++)
-        if (find(k) == r && border[k]) { E.h_off_pose[k] = cursor; cursor += 6; }
-    }
-    n_total = cursor;
-  } else {
-    for (int k = 0; k < K; k++) E.h_off_pose[k] = 6 * k;
-    n_total = 6 * K;
-  }
+  const int n_total = column_layout(p, E.visual_only, E.L_in == 0 && p->n_edge > 0, E.h_off_pose, E.h_off_sb, group_of_tile);
+  const int TT = cvb_chol::T;
   E.n_c_pad = ((n_total + TT - 1) / TT) * TT;
   E.n_vec = E.n_c_pad + 3 * E.L_in;
   auto col_of = [&](int kf, int c) { return c < 6 ? E.h_off_pose[kf] + c : E.h_off_sb[kf] + (c - 6); };
@@ -1600,8 +1556,6 @@ int engine_setup(Engine& E, const cvb_ba_problem* p, const cvb_ba_options* o, co
   if (!E.visual_only)
     for (int f = 0; f < p->n_imu; f++) {
       if (f % E.world != E.rank) continue;
-      CVB_REQUIRE(ctx, p->imu_i[f] >= 0 && p->imu_i[f] < K && p->imu_j[f] >= 0 && p->imu_j[f] < K && p->imu_i[f] != p->imu_j[f],
-                  "bad IMU factor indices");
       CVB_REQUIRE(ctx, p->imu_ptr[f + 1] > p->imu_ptr[f], "IMU factor with 0 measurements (drop it: opt.cpp:382-385)");
       h_imu_i.push_back(p->imu_i[f]);
       h_imu_j.push_back(p->imu_j[f]);
@@ -1611,8 +1565,6 @@ int engine_setup(Engine& E, const cvb_ba_problem* p, const cvb_ba_options* o, co
   std::vector<int> h_edge_i, h_edge_j, sel_edge;
   for (int e = 0; e < p->n_edge; e++) {
     if (e % E.world != E.rank) continue;
-    CVB_REQUIRE(ctx, p->edge_i[e] >= 0 && p->edge_i[e] < K && p->edge_j[e] >= 0 && p->edge_j[e] < K && p->edge_i[e] != p->edge_j[e],
-                "bad edge indices");
     h_edge_i.push_back(p->edge_i[e]);
     h_edge_j.push_back(p->edge_j[e]);
     sel_edge.push_back(e);
@@ -1646,7 +1598,7 @@ int engine_setup(Engine& E, const cvb_ba_problem* p, const cvb_ba_options* o, co
   // ---- uploads ----
   E.h_const.assign(p->pose_const, p->pose_const + K);
   if (fill) {
-    if (E.pose[0].alloc((size_t)7 * K) || E.pose0.alloc((size_t)7 * K)) return cvb_fail(ctx, CVB_ERR_CUDA, "cudaMalloc failed (poses)");
+    if (E.pose[0].alloc((size_t)7 * K, E.st) || E.pose0.alloc((size_t)7 * K, E.st)) return cvb_fail(ctx, CVB_ERR_CUDA, "cudaMalloc failed (poses)");
   } else if ((rc = upload(E, E.pose[0], p->pose, (size_t)7 * K))) {
     return rc;
   }
@@ -1684,7 +1636,7 @@ int engine_setup(Engine& E, const cvb_ba_problem* p, const cvb_ba_options* o, co
     std::vector<uint8_t> rb(E.n_edge);
     for (int e = 0; e < E.n_edge; e++) rb[e] = p->edge_robust ? p->edge_robust[e] : 0;
     if ((rc = upload(E, E.edge_i, h_edge_i)) || (rc = upload(E, E.edge_j, h_edge_j)) || (rc = upload(E, E.edge_robust, rb))) return rc;
-    if (E.edge_q.alloc((size_t)4 * E.n_edge) || E.edge_t.alloc((size_t)3 * E.n_edge) || E.edge_S.alloc((size_t)36 * E.n_edge))
+    if (E.edge_q.alloc((size_t)4 * E.n_edge, E.st) || E.edge_t.alloc((size_t)3 * E.n_edge, E.st) || E.edge_S.alloc((size_t)36 * E.n_edge, E.st))
       return cvb_fail(ctx, CVB_ERR_CUDA, "cudaMalloc failed (edges)");
     if ((rc = (*fill)(E.pose[0].p, E.pose0.p, E.edge_q.p, E.edge_t.p, E.edge_S.p))) return rc;
     if ((rc = zalloc(E, E.Jedge, (size_t)72 * E.n_edge)) || (rc = zalloc(E, E.redge, (size_t)6 * E.n_edge))) return rc;
@@ -1722,7 +1674,7 @@ int engine_setup(Engine& E, const cvb_ba_problem* p, const cvb_ba_options* o, co
       for (int c = 0; c < 3; c++) { a0.push_back(p->imu_acc0[3 * (size_t)s + c]); g0.push_back(p->imu_gyr0[3 * (size_t)s + c]); }
       ptr.push_back((int)dt.size());
     }
-    DevArr<int> d_ptr; DevArr<double> d_dt, d_acc, d_gyr, d_a0, d_g0, d_noise;
+    cvb_dev_arr<int> d_ptr; cvb_dev_arr<double> d_dt, d_acc, d_gyr, d_a0, d_g0, d_noise;
     if ((rc = upload(E, d_ptr, ptr)) || (rc = upload(E, d_dt, dt)) || (rc = upload(E, d_acc, acc)) || (rc = upload(E, d_gyr, gyr)) ||
         (rc = upload(E, d_a0, a0)) || (rc = upload(E, d_g0, g0)) || (rc = upload(E, d_noise, p->imu_noise, 5)))
       return rc;
@@ -1732,7 +1684,6 @@ int engine_setup(Engine& E, const cvb_ba_problem* p, const cvb_ba_options* o, co
     int flag = 0;
     ENG_CUDA(cudaMemcpyAsync(&flag, E.flag.p, sizeof(int), cudaMemcpyDeviceToHost, E.st));
     ENG_CUDA(cudaStreamSynchronize(E.st));
-    d_ptr.free_(); d_dt.free_(); d_acc.free_(); d_gyr.free_(); d_a0.free_(); d_g0.free_(); d_noise.free_();
     // bit 2: a preintegrated covariance P that is not positive definite (e.g. a zero noise sigma in imu_noise); its
     // sqrt_info would be meaningless, and the reference's chol(P^-1) fails on the same input
     if (flag & 2)
@@ -1758,23 +1709,15 @@ int engine_setup(Engine& E, const cvb_ba_problem* p, const cvb_ba_options* o, co
     if ((rc = upload(E, E.xt_own, h_xt_own)) || (rc = upload(E, E.col_owner, h_owner))) return rc;
     if ((rc = zalloc(E, E.flagd, 2))) return rc;
   }
-  DevArr<double>* vecs[] = {&E.colsq, &E.diag, &E.gvec, &E.grad, &E.sgrad, &E.gn, &E.step, &E.xsol, &E.yb, &E.gs, &E.tmp};
+  cvb_dev_arr<double>* vecs[] = {&E.colsq, &E.diag, &E.gvec, &E.grad, &E.sgrad, &E.gn, &E.step, &E.xsol, &E.yb, &E.gs, &E.tmp};
   for (auto* v : vecs)
     if ((rc = zalloc(E, *v, (size_t)E.n_vec))) return rc;
   // S = the packed tiles of L's structure; cleared at the start of every linearisation (cam_blocks).  With several ranks
   // S, the tile inverses and the panel flags come from cudaMalloc so that they can be exported through CUDA IPC.
   const size_t s_doubles = E.n_tiles * cvb_chol::T * cvb_chol::T, linv_doubles = (size_t)E.n_c_pad * cvb_chol::T;
-  if (E.world > 1) {
-    if (cudaMalloc(&E.S_raw, s_doubles * 8) != cudaSuccess || cudaMalloc(&E.linv_raw, linv_doubles * 8) != cudaSuccess ||
-        cudaMalloc(&E.pflag_raw, sizeof(int) * 2 * (size_t)E.plan.nt) != cudaSuccess)
-      return cvb_fail(E.ctx, CVB_ERR_CUDA, "cudaMalloc failed (reduced camera system, %zu bytes)", s_doubles * 8);
-    ENG_CUDA(cudaMemsetAsync(E.linv_raw, 0, linv_doubles * 8, E.st));
-    ENG_CUDA(cudaMemsetAsync(E.pflag_raw, 0, sizeof(int) * 2 * (size_t)E.plan.nt, E.st));
-    E.S.p = E.S_raw; E.S.n = s_doubles; E.linv.p = E.linv_raw; E.linv.n = linv_doubles;
-  } else {
-    if (E.S.alloc(s_doubles)) return cvb_fail(E.ctx, CVB_ERR_CUDA, "cudaMalloc failed (reduced camera system, %zu bytes)", s_doubles * 8);
-    if ((rc = zalloc(E, E.linv, linv_doubles))) return rc;
-  }
+  const bool ipc = E.world > 1;
+  if (E.S.alloc(s_doubles, E.st, ipc)) return cvb_fail(E.ctx, CVB_ERR_CUDA, "cudaMalloc failed (reduced camera system, %zu bytes)", s_doubles * 8);
+  if ((rc = zalloc(E, E.linv, linv_doubles, ipc)) || (ipc && (rc = zalloc(E, E.pflag, 2 * (size_t)E.plan.nt, ipc)))) return rc;
   if ((rc = zalloc(E, E.partials, (size_t)RED_SLOTS * RED_BLOCKS)) || (rc = zalloc(E, E.scalars, RED_SLOTS)) ||
       (rc = zalloc(E, E.rankmax, (size_t)E.world)))
     return rc;
@@ -1825,18 +1768,10 @@ int lm_blocks(Engine& E) {
   return CVB_OK;
 }
 
-int ar(Engine& E, double* p, size_t n) {
-  if (E.allreduce && E.world > 1) {
-    int rc = E.allreduce(p, n);
-    if (rc) return cvb_fail(E.ctx, CVB_ERR_CUDA, "allreduce callback failed (%d)", rc);
-  }
-  return CVB_OK;
-}
-
 // camera blocks of J^T J (before Schur / damping) into S, camera gradient into gvec
 int cam_blocks(Engine& E) {
   const size_t ld = (size_t)E.n_c_pad;
-  const SView Sv{E.S.p, E.plan.d_tile_of, E.plan.nt};
+  const SView Sv{E.S.p, E.plan.d_tile_of.p, E.plan.nt};
   // S's own tiles (the ones the block kernels below add into) are cleared first on the engine stream; the fill tiles,
   // which only the factorisation writes, on st_fill beside the block kernels (factor_rcs waits for them)
   if (E.n_xt_fill > 0) {
@@ -1865,7 +1800,7 @@ int cam_blocks(Engine& E) {
 }
 
 int cam_colsq(Engine& E) {
-  cam_colsq_kernel<<<grid1(E.n_c_pad), 256, 0, E.st>>>(E.n_c_pad, E.scale.p, SView{E.S.p, E.plan.d_tile_of, E.plan.nt}, E.colsq.p);
+  cam_colsq_kernel<<<grid1(E.n_c_pad), 256, 0, E.st>>>(E.n_c_pad, E.scale.p, SView{E.S.p, E.plan.d_tile_of.p, E.plan.nt}, E.colsq.p);
   ENG_LAUNCH();
   return ar(E, E.colsq.p, (size_t)E.n_c_pad);
 }
@@ -1873,7 +1808,7 @@ int cam_colsq(Engine& E) {
 // damped Schur complement + Cholesky for the given mu; *ok = false if the factorisation broke down
 int factor_rcs(Engine& E, double mu, bool* ok) {
   const size_t ld = (size_t)E.n_c_pad;
-  const SView Sv{E.S.p, E.plan.d_tile_of, E.plan.nt};
+  const SView Sv{E.S.p, E.plan.d_tile_of.p, E.plan.nt};
   const bool dist = E.p2p && E.world > 1;
   tick(E, 0);
   if (E.L_in > 0) {
@@ -1899,7 +1834,7 @@ int factor_rcs(Engine& E, double mu, bool* ok) {
   // writing its partial S (stream order on each rank)
   if ((rc = ar(E, E.yb.p, ld))) return rc;
   if (dist && E.n_xt_own > 0) {
-    reduce_pull_kernel<<<E.n_xt_own, 256, 0, E.st>>>(E.S.p, E.d_peer_S, E.world, E.rank, E.xt_own.p);
+    reduce_pull_kernel<<<E.n_xt_own, 256, 0, E.st>>>(E.S.p, E.peer_S.p, E.world, E.rank, E.xt_own.p);
     ENG_LAUNCH();
   }
   cam_finish_kernel<<<grid1(E.n_c_pad), 256, 0, E.st>>>(E.n_c_pad, E.scale.p, Sv, E.diag.p, E.gvec.p, E.yb.p, E.gs.p, mu,
@@ -2207,8 +2142,8 @@ int engine_iterate(Engine& E, bool* done) {
 }
 
 int engine_corrected_norms(Engine& E, double* h_norms_full, int n_obs_full) {
-  DevArr<double> d;
-  if (d.alloc((size_t)E.n_obs)) return cvb_fail(E.ctx, CVB_ERR_CUDA, "cudaMalloc failed");
+  cvb_dev_arr<double> d;
+  if (d.alloc((size_t)E.n_obs, E.st)) return cvb_fail(E.ctx, CVB_ERR_CUDA, "cudaMalloc failed");
   if (E.n_obs) {
     reproj_norms_kernel<<<(E.n_obs + 255) / 256, 256, 0, E.st>>>(E.n_obs, E.obs_kf.p, E.obs_lm.p, E.obs_uv.p, E.obs_sigma.p, E.pose[E.cur].p,
                                                                  E.lm[E.cur].p, E.extr_kf.p, E.intr_kf.p, E.dist_kf.p, E.model_kf.p, E.xi_kf.p,
@@ -2218,7 +2153,6 @@ int engine_corrected_norms(Engine& E, double* h_norms_full, int n_obs_full) {
   std::vector<double> h(E.n_obs);
   ENG_CUDA(cudaMemcpyAsync(h.data(), d.p, sizeof(double) * E.n_obs, cudaMemcpyDeviceToHost, E.st));
   ENG_CUDA(cudaStreamSynchronize(E.st));
-  d.free_();
   for (int i = 0; i < n_obs_full; i++) h_norms_full[i] = -1.0;   // -1: observation not in this rank's problem
   for (int i = 0; i < E.n_obs; i++) h_norms_full[E.obs_of_compact[i]] = h[i];
   return CVB_OK;
@@ -2271,30 +2205,27 @@ int enable_p2p(Engine& E, bool ipc, const std::function<int(cvb_chol::DistView&,
   if (E.g_factor) return cvb_fail(E.ctx, CVB_ERR_INVALID, "cvb_ba_enable_p2p must precede the first iterations");
   cvb_chol::DistView dv;
   dv.rank = E.rank; dv.world = E.world;
-  dv.peer_S[E.rank] = E.S_raw; dv.peer_linv[E.rank] = E.linv_raw; dv.peer_flag[E.rank] = E.pflag_raw;
+  dv.peer_S[E.rank] = E.S.p; dv.peer_linv[E.rank] = E.linv.p; dv.peer_flag[E.rank] = E.pflag.p;
   bool opened = false;
   int rc;
   if ((rc = map_peers(dv, &opened))) return rc;
   // everybody must have mapped everybody: min over ranks via the sum of (1 - opened)
   {
-    DevArr<double> d_ok;
+    cvb_dev_arr<double> d_ok;
     std::vector<double> v(1, opened ? 0.0 : 1.0);
     if ((rc = upload(E, d_ok, v))) return rc;
     if ((rc = ar(E, d_ok.p, 1))) return rc;
     ENG_CUDA(cudaMemcpyAsync(v.data(), d_ok.p, sizeof(double), cudaMemcpyDeviceToHost, E.st));
     ENG_CUDA(cudaStreamSynchronize(E.st));
-    d_ok.free_();
     if (v[0] != 0.0) {
       unmap(dv);
       return cvb_fail(E.ctx, CVB_ERR_UNSUPPORTED, "peer mapping is not available between all ranks (all-reduce fallback stays in use)");
     }
   }
-  ENG_CUDA(cudaMalloc(&dv.d_epoch, sizeof(int)));
-  ENG_CUDA(cudaMemsetAsync(dv.d_epoch, 0, sizeof(int), E.st));
-  ENG_CUDA(cudaMalloc(&dv.d_peer_flag, sizeof(int*) * 16));
-  ENG_CUDA(cudaMemcpyAsync(dv.d_peer_flag, dv.peer_flag, sizeof(int*) * 16, cudaMemcpyHostToDevice, E.st));
-  ENG_CUDA(cudaMalloc(&E.d_peer_S, sizeof(double*) * 16));
-  ENG_CUDA(cudaMemcpyAsync(E.d_peer_S, dv.peer_S, sizeof(double*) * 16, cudaMemcpyHostToDevice, E.st));
+  if ((rc = zalloc(E, E.epoch, 1)) || (rc = upload(E, E.peer_flag, dv.peer_flag, 16)) || (rc = upload(E, E.peer_S, dv.peer_S, 16)))
+    return rc;
+  dv.d_epoch = E.epoch.p;
+  dv.d_peer_flag = E.peer_flag.p;
   ENG_CUDA(cudaStreamSynchronize(E.st));
   // distributed plan: same structure, pair lists restricted to the tile columns this rank owns
   E.plan.build(E.plan.nt, E.h_prefill, E.plan.h_col_group, &E.h_owner, E.rank);
@@ -2322,19 +2253,18 @@ int enable_p2p_ipc(Engine& E) {
     const int per_rank = 3 * HB + 1;                     // three handles + an "ok" byte
     std::vector<double> table((size_t)E.world * per_rank, 0.0);
     cudaIpcMemHandle_t hs[3];
-    bool ok = cudaIpcGetMemHandle(&hs[0], E.S_raw) == cudaSuccess && cudaIpcGetMemHandle(&hs[1], E.linv_raw) == cudaSuccess &&
-              cudaIpcGetMemHandle(&hs[2], E.pflag_raw) == cudaSuccess;
+    bool ok = cudaIpcGetMemHandle(&hs[0], E.S.p) == cudaSuccess && cudaIpcGetMemHandle(&hs[1], E.linv.p) == cudaSuccess &&
+              cudaIpcGetMemHandle(&hs[2], E.pflag.p) == cudaSuccess;
     cudaGetLastError();
     for (int q = 0; q < 3 && ok; q++)
       for (int b = 0; b < HB; b++) table[(size_t)E.rank * per_rank + q * HB + b] = (double)reinterpret_cast<unsigned char*>(&hs[q])[b];
     table[(size_t)E.rank * per_rank + 3 * HB] = ok ? 1.0 : 0.0;
-    DevArr<double> d_table;
+    cvb_dev_arr<double> d_table;
     int rc;
     if ((rc = upload(E, d_table, table))) return rc;
     if ((rc = ar(E, d_table.p, table.size()))) return rc;
     ENG_CUDA(cudaMemcpyAsync(table.data(), d_table.p, table.size() * sizeof(double), cudaMemcpyDeviceToHost, E.st));
     ENG_CUDA(cudaStreamSynchronize(E.st));
-    d_table.free_();
     for (int g = 0; g < E.world; g++) ok = ok && table[(size_t)g * per_rank + 3 * HB] == 1.0;
     *opened = ok;
     for (int g = 0; g < E.world && ok; g++) {
@@ -2355,7 +2285,7 @@ int enable_p2p_ipc(Engine& E) {
 // The peers' pointers from an in-process group (cvb_group_create enabled peer access between the ranks' devices).
 int enable_p2p_group(Engine& E, cvb_group* g, int rank) {
   const auto map_peers = [&E, g, rank](cvb_chol::DistView& dv, bool* opened) {
-    const void* mine[3] = {E.S_raw, E.linv_raw, E.pflag_raw};
+    const void* mine[3] = {E.S.p, E.linv.p, E.pflag.p};
     const void* all[3 * CVB_GROUP_MAX];
     int rc = cvb_grp::exchange(g, rank, mine, 3, all);
     if (rc) return cvb_fail(E.ctx, rc, "peer pointer exchange failed (group failed)");
@@ -2379,25 +2309,15 @@ struct cvb_ba {
   cvb_ba_problem prob_copy;
 };
 
-// every cvb_ba_* entry: make the ctx's device current and bind the stream-ordered allocator to the engine's stream
-struct BaEnter {
-  cvb_device_guard guard;
-  explicit BaEnter(cvb_ba* h) : guard(h ? h->E.ctx : nullptr) {
-    if (h) t_alloc_stream = h->E.st;
-  }
-};
-
 extern "C" {
-
-void cvb_ba_free(cvb_ctx*) {}
 
 int cvb_ba_create(cvb_ctx* ctx, const cvb_ba_problem* p, const cvb_ba_options* o, cvb_ba** out) {
   if (!ctx || !p || !o || !out) return CVB_ERR_INVALID;
+  CVB_GUARD(ctx);
   *out = nullptr;
   cvb_ba* h = new cvb_ba();
   h->E.ctx = ctx;
   h->E.st = ctx->stream;
-  BaEnter enter(h);
   h->prob_copy = *p;
   int rc = engine_setup(h->E, p, o);
   if (!rc) rc = engine_begin(h->E);
@@ -2421,7 +2341,7 @@ int cvb_ba_set_allreduce(cvb_ba* h, cvb_allreduce_fn fn, void* user) {
 
 int cvb_ba_enable_p2p(cvb_ba* h) {
   if (!h) return CVB_ERR_INVALID;
-  BaEnter enter(h);
+  CVB_GUARD(h->E.ctx);
   return enable_p2p_ipc(h->E);
 }
 
@@ -2429,7 +2349,7 @@ int cvb_ba_enable_p2p(cvb_ba* h) {
 // again: a restarted solve repeats the original one bit for bit.
 int cvb_ba_restart(cvb_ba* h) {
   if (!h) return CVB_ERR_INVALID;
-  BaEnter enter(h);
+  CVB_GUARD(h->E.ctx);
   Engine& E = h->E;
   E.cur = 0;
   ENG_CUDA(cudaMemcpyAsync(E.pose[0].p, E.pose0.p, sizeof(double) * 7 * E.K, cudaMemcpyDeviceToDevice, E.st));
@@ -2440,7 +2360,7 @@ int cvb_ba_restart(cvb_ba* h) {
 
 int cvb_ba_iterate(cvb_ba* h, int max_iterations, int* iterations_done) {
   if (!h) return CVB_ERR_INVALID;
-  BaEnter enter(h);
+  CVB_GUARD(h->E.ctx);
   Engine& E = h->E;
   int n = 0;
   bool done = E.termination != TERM_NO_CONVERGENCE;
@@ -2455,13 +2375,13 @@ int cvb_ba_iterate(cvb_ba* h, int max_iterations, int* iterations_done) {
 
 int cvb_ba_result_get(cvb_ba* h, const cvb_ba_problem* p, cvb_ba_result* r) {
   if (!h || !p || !r) return CVB_ERR_INVALID;
-  BaEnter enter(h);
+  CVB_GUARD(h->E.ctx);
   return engine_download(h->E, p, r);
 }
 
 int cvb_ba_reproj_norms(cvb_ba* h, double* norms, int n_obs) {
   if (!h || !norms) return CVB_ERR_INVALID;
-  BaEnter enter(h);
+  CVB_GUARD(h->E.ctx);
   return engine_corrected_norms(h->E, norms, n_obs);
 }
 
@@ -2469,9 +2389,9 @@ int cvb_ba_reproj_norms(cvb_ba* h, double* norms, int n_obs) {
 // which: 0 scale, 1 colsq, 2 diag, 3 gradient g, 4 grad/diag, 5 gn, 6 step, 7 x (linear solve), 8 reduced rhs
 int cvb_ba_debug_vector(cvb_ba* h, int which, double* out, int64_t cap, int64_t* n_cam, int64_t* n_total) {
   if (!h) return CVB_ERR_INVALID;
-  BaEnter enter(h);
+  CVB_GUARD(h->E.ctx);
   Engine& E = h->E;
-  const DevArr<double>* v[] = {&E.scale, &E.colsq, &E.diag, &E.gvec, &E.grad, &E.gn, &E.step, &E.xsol, &E.gs};
+  const cvb_dev_arr<double>* v[] = {&E.scale, &E.colsq, &E.diag, &E.gvec, &E.grad, &E.gn, &E.step, &E.xsol, &E.gs};
   if (which < 0 || which > 8) return CVB_ERR_INVALID;
   const int64_t nc = (int64_t)E.K * E.per, tot = nc + 3 * (int64_t)E.L_in;
   if (n_cam) *n_cam = nc;
@@ -2504,7 +2424,7 @@ int cvb_ba_timing(cvb_ba* h, double out[6], int reset) {
 
 int cvb_ba_destroy(cvb_ba* h) {
   if (h) {
-    BaEnter enter(h);
+    CVB_GUARD(h->E.ctx);
     cudaStreamSynchronize(h->E.st);
     delete h;
   }
@@ -2526,10 +2446,10 @@ int cvb_ba_solve(cvb_ctx* ctx, const cvb_ba_problem* p, const cvb_ba_options* o,
 
 int cvb_ba_solve_dev_edges(cvb_ctx* ctx, const cvb_ba_problem* p, const cvb_ba_options* o, cvb_ba_result* r, const cvb_dev_edges_fill& fill,
                            const std::function<int(const double* d_pose)>& finish) {
+  CVB_GUARD(ctx);
   cvb_ba* h = new cvb_ba();
   h->E.ctx = ctx;
   h->E.st = ctx->stream;
-  BaEnter enter(h);
   h->prob_copy = *p;
   Engine& E = h->E;
   int rc = engine_setup(E, p, o, &fill);
@@ -2591,7 +2511,7 @@ int group_solve(cvb_group* g, const cvb_ba_problem* p, const cvb_ba_options* o_i
     int rr = cvb_ba_create(g->ctx[r], p, &o, &h[r]);
     if (!rr) rr = cvb_ba_set_allreduce(h[r], cvb_grp::allreduce, &g->bind[r]);
     if (!rr && peer_path && n > 1) {
-      BaEnter enter(h[r]);
+      CVB_GUARD(h[r]->E.ctx);
       rr = enable_p2p_group(h[r]->E, g, r);
     }
     if (!rr) rr = cvb_ba_restart(h[r]);
@@ -2600,7 +2520,7 @@ int group_solve(cvb_group* g, const cvb_ba_problem* p, const cvb_ba_options* o_i
   });
   for (int r = 0; r < n; r++)
     if (h[r]) {
-      BaEnter enter(h[r]);
+      CVB_GUARD(h[r]->E.ctx);
       cudaStreamSynchronize(h[r]->E.st);
     }
   for (int r = 0; r < n && !rc; r++) {

@@ -1034,38 +1034,21 @@ int nd_layout(const std::vector<std::vector<int>>& members, int bw, std::vector<
 }
 
 int TilePlan::upload(cvb_ctx* ctx, cudaStream_t st) {
-  release();
-  auto up = [&](int** d, const std::vector<int>& h) -> int {
-    const size_t n = h.size() ? h.size() : 1;
-    CVB_CUDA(ctx, cudaMalloc(d, n * sizeof(int)));
-    if (h.size()) CVB_CUDA(ctx, cudaMemcpyAsync(*d, h.data(), h.size() * sizeof(int), cudaMemcpyHostToDevice, st));
+  auto up = [&](cvb_dev_arr<int>& d, const std::vector<int>& h) -> int {
+    CVB_CUDA(ctx, d.alloc(h.size(), st));
+    if (h.size()) CVB_CUDA(ctx, cudaMemcpyAsync(d.p, h.data(), h.size() * sizeof(int), cudaMemcpyHostToDevice, st));
     return CVB_OK;
   };
   int rc;
-  if ((rc = up(&d_row_idx, h_row_idx)) || (rc = up(&d_pair_i, h_pair_i)) || (rc = up(&d_pair_j, h_pair_j)) ||
-      (rc = up(&d_pair_mask, h_pair_mask)) || (rc = up(&d_rowc_idx, h_rowc_idx)) || (rc = up(&d_tile_of, h_tile_of)) ||
-      (rc = up(&d_lvl_pair_i, h_lvl_pair_i)) || (rc = up(&d_lvl_pair_j, h_lvl_pair_j)) ||
-      (rc = up(&d_lvl_pair_k0, h_lvl_pair_k0)) || (rc = up(&d_lvl_pair_mask, h_lvl_pair_mask)) ||
-      (rc = up(&d_lvl_trsm_tile, h_lvl_trsm_tile)) || (rc = up(&d_lvl_trsm_col, h_lvl_trsm_col)) ||
-      (rc = up(&d_col_ptr, h_col_ptr)) || (rc = up(&d_rowc_ptr, h_rowc_ptr)))
+  if ((rc = up(d_row_idx, h_row_idx)) || (rc = up(d_pair_i, h_pair_i)) || (rc = up(d_pair_j, h_pair_j)) ||
+      (rc = up(d_pair_mask, h_pair_mask)) || (rc = up(d_rowc_idx, h_rowc_idx)) || (rc = up(d_tile_of, h_tile_of)) ||
+      (rc = up(d_lvl_pair_i, h_lvl_pair_i)) || (rc = up(d_lvl_pair_j, h_lvl_pair_j)) ||
+      (rc = up(d_lvl_pair_k0, h_lvl_pair_k0)) || (rc = up(d_lvl_pair_mask, h_lvl_pair_mask)) ||
+      (rc = up(d_lvl_trsm_tile, h_lvl_trsm_tile)) || (rc = up(d_lvl_trsm_col, h_lvl_trsm_col)) ||
+      (rc = up(d_col_ptr, h_col_ptr)) || (rc = up(d_rowc_ptr, h_rowc_ptr)))
     return rc;
   CVB_CUDA(ctx, cudaStreamSynchronize(st));
   return CVB_OK;
-}
-
-void TilePlan::release() {
-  if (d_row_idx) cudaFree(d_row_idx);
-  if (d_pair_i) cudaFree(d_pair_i);
-  if (d_pair_j) cudaFree(d_pair_j);
-  if (d_pair_mask) cudaFree(d_pair_mask);
-  if (d_rowc_idx) cudaFree(d_rowc_idx);
-  if (d_tile_of) cudaFree(d_tile_of);
-  d_row_idx = d_pair_i = d_pair_j = d_pair_mask = d_rowc_idx = d_tile_of = nullptr;
-  for (int** d : {&d_lvl_pair_i, &d_lvl_pair_j, &d_lvl_pair_k0, &d_lvl_pair_mask, &d_lvl_trsm_tile, &d_lvl_trsm_col,
-                  &d_col_ptr, &d_rowc_ptr}) {
-    if (*d) cudaFree(*d);
-    *d = nullptr;
-  }
 }
 
 int FactorStreams::create(cvb_ctx* ctx, int nt) {
@@ -1164,7 +1147,7 @@ int factor(cvb_ctx* ctx, double* S, double* linv, int* d_flag, const TilePlan& p
   }
   const int nt = plan.nt;
   const bool dist = dv != nullptr && dv->world > 1 && !plan.h_owner.empty();
-  CVB_REQUIRE(ctx, plan.d_tile_of != nullptr && (int)plan.h_col_base.size() == nt, "tile plan not built / uploaded");
+  CVB_REQUIRE(ctx, plan.d_tile_of.p != nullptr && (int)plan.h_col_base.size() == nt, "tile plan not built / uploaded");
   CVB_REQUIRE(ctx, fs.ev.size() >= (size_t)5 * nt, "factor streams not created for this plan");
   CVB_CUDA(ctx, cudaMemsetAsync(d_flag, 0, sizeof(int), st));
   if (dist) {
@@ -1243,7 +1226,7 @@ int factor(cvb_ctx* ctx, double* S, double* linv, int* d_flag, const TilePlan& p
       if (tr) cudaEventRecord(tev[(size_t)c0 * 5 + e], st);
     };
     mark(0);
-    potrf_inv_level_kernel<<<nc, POTRF_THREADS, kPotrfSmem, st>>>(S, plan.d_tile_of, nt, c0, linv, d_flag);
+    potrf_inv_level_kernel<<<nc, POTRF_THREADS, kPotrfSmem, st>>>(S, plan.d_tile_of.p, nt, c0, linv, d_flag);
     CVB_CHECK_LAUNCH(ctx);
     mark(1);
     double* diag = S + (size_t)plan.h_col_base[kl] * TT;
@@ -1254,15 +1237,15 @@ int factor(cvb_ctx* ctx, double* S, double* linv, int* d_flag, const TilePlan& p
     }
     const int t0 = plan.h_lvl_trsm_ptr[l], ntr = plan.h_lvl_trsm_ptr[l + 1] - t0;
     if (ntr > 0) {
-      trsm_level_kernel<<<2 * ntr, TRSM_THREADS, kTrsmSmem, st>>>(S, linv, plan.d_lvl_trsm_tile + t0, plan.d_lvl_trsm_col + t0);
+      trsm_level_kernel<<<2 * ntr, TRSM_THREADS, kTrsmSmem, st>>>(S, linv, plan.d_lvl_trsm_tile.p + t0, plan.d_lvl_trsm_col.p + t0);
       CVB_CHECK_LAUNCH(ctx);
     }
     mark(2);
     const int p0 = plan.h_lvl_pair_ptr[l], np = plan.h_lvl_pair_ptr[l + 1] - p0;
     if (np > 0) {
-      tile_update_level_kernel<<<np, TILE_THREADS, kTileSmem, st>>>(S, plan.d_tile_of, nt, plan.d_lvl_pair_k0 + p0,
-                                                                    plan.d_lvl_pair_i + p0, plan.d_lvl_pair_j + p0,
-                                                                    plan.d_lvl_pair_mask + p0);
+      tile_update_level_kernel<<<np, TILE_THREADS, kTileSmem, st>>>(S, plan.d_tile_of.p, nt, plan.d_lvl_pair_k0.p + p0,
+                                                                    plan.d_lvl_pair_i.p + p0, plan.d_lvl_pair_j.p + p0,
+                                                                    plan.d_lvl_pair_mask.p + p0);
       CVB_CHECK_LAUNCH(ctx);
     }
     if (has_next) {
@@ -1361,8 +1344,8 @@ int factor(cvb_ctx* ctx, double* S, double* linv, int* d_flag, const TilePlan& p
     // lookahead rule
     if (lb >= 0) CVB_CUDA(ctx, cudaStreamWaitEvent(cs, ev[5 * lb + 1], 0));
     if (diag_pair) {
-      syrk_kernel<<<4, SYRK_THREADS, kSyrkSmem, cs>>>(S, plan.d_tile_of, nt, k0, plan.d_pair_i + p0, plan.d_pair_j + p0,
-                                                       plan.d_pair_mask + p0);
+      syrk_kernel<<<4, SYRK_THREADS, kSyrkSmem, cs>>>(S, plan.d_tile_of.p, nt, k0, plan.d_pair_i.p + p0, plan.d_pair_j.p + p0,
+                                                       plan.d_pair_mask.p + p0);
       CVB_CHECK_LAUNCH(ctx);
     }
     if (mine_n) {
@@ -1407,15 +1390,15 @@ int factor(cvb_ctx* ctx, double* S, double* linv, int* d_flag, const TilePlan& p
       if (lb >= 0) CVB_CUDA(ctx, cudaStreamWaitEvent(ws, ev[5 * lb + 1], 0));
       const int a0 = diag_pair ? 1 : 0;
       if (na - a0 > 0) {
-        tile_update_kernel<<<na - a0, TILE_THREADS, kTileSmem, ws>>>(S, plan.d_tile_of, nt, k0, plan.d_pair_i + p0 + a0,
-                                                                     plan.d_pair_j + p0 + a0, plan.d_pair_mask + p0 + a0);
+        tile_update_kernel<<<na - a0, TILE_THREADS, kTileSmem, ws>>>(S, plan.d_tile_of.p, nt, k0, plan.d_pair_i.p + p0 + a0,
+                                                                     plan.d_pair_j.p + p0 + a0, plan.d_pair_mask.p + p0 + a0);
         CVB_CHECK_LAUNCH(ctx);
       }
       if (tr) cudaEventRecord(tev[(size_t)k * 5 + 3], ws);
       if (np - na > 0) {
         CVB_CUDA(ctx, cudaStreamWaitEvent(st2, evPanel, 0));
-        tile_update_kernel<<<np - na, TILE_THREADS, kTileSmem, st2>>>(S, plan.d_tile_of, nt, k0, plan.d_pair_i + p0 + na,
-                                                                       plan.d_pair_j + p0 + na, plan.d_pair_mask + p0 + na);
+        tile_update_kernel<<<np - na, TILE_THREADS, kTileSmem, st2>>>(S, plan.d_tile_of.p, nt, k0, plan.d_pair_i.p + p0 + na,
+                                                                       plan.d_pair_j.p + p0 + na, plan.d_pair_mask.p + p0 + na);
         CVB_CHECK_LAUNCH(ctx);
         CVB_CUDA(ctx, cudaEventRecord(evBulk, st2));
         if (tr) cudaEventRecord(tev[(size_t)k * 5 + 4], st2);
@@ -1474,7 +1457,7 @@ int solve_grid(cvb_ctx* ctx, const double* L, const double* linv, const double* 
     }
   }
   const int nt = plan.nt;
-  CVB_REQUIRE(ctx, plan.d_rowc_ptr != nullptr && plan.d_col_ptr != nullptr, "tile plan not built / uploaded");
+  CVB_REQUIRE(ctx, plan.d_rowc_ptr.p != nullptr && plan.d_col_ptr.p != nullptr, "tile plan not built / uploaded");
   CVB_REQUIRE(ctx, fs.d_solve_sync != nullptr && fs.solve_nt >= nt, "factor streams not created for this plan");
   if (nt == 0) return CVB_OK;
   if (grid <= 0) {
@@ -1486,10 +1469,10 @@ int solve_grid(cvb_ctx* ctx, const double* L, const double* linv, const double* 
   grid = std::max(1, std::min(grid, nt));
   int* fsync = fs.d_solve_sync;   // forward: [0, nt], backward: [nt + 1, 2 nt + 1]
   CVB_CUDA(ctx, cudaMemsetAsync(fsync, 0, (size_t)2 * (nt + 1) * sizeof(int), st));
-  subst_kernel<true><<<grid, SOLVE_THREADS, kSolveSmem, st>>>(L, linv, plan.d_rowc_ptr, plan.d_rowc_idx, plan.d_tile_of,
+  subst_kernel<true><<<grid, SOLVE_THREADS, kSolveSmem, st>>>(L, linv, plan.d_rowc_ptr.p, plan.d_rowc_idx.p, plan.d_tile_of.p,
                                                               nt, b, tmp, fsync);
   CVB_CHECK_LAUNCH(ctx);
-  subst_kernel<false><<<grid, SOLVE_THREADS, kSolveSmem, st>>>(L, linv, plan.d_col_ptr, plan.d_row_idx, nullptr, nt, tmp,
+  subst_kernel<false><<<grid, SOLVE_THREADS, kSolveSmem, st>>>(L, linv, plan.d_col_ptr.p, plan.d_row_idx.p, nullptr, nt, tmp,
                                                                x, fsync + nt + 1);
   CVB_CHECK_LAUNCH(ctx);
   return CVB_OK;
@@ -1621,7 +1604,6 @@ extern "C" int cvb_dense_cholesky_solve(cvb_ctx* ctx, const double* A, int n, co
   cudaEventDestroy(e0);
   cudaEventDestroy(e1);
   if (factor_ms) *factor_ms = ms;
-  plan.release();
   if (*B.host(dflag)) return cvb_fail(ctx, CVB_ERR_NUMERIC, "matrix is not positive definite");
   memcpy(x, B.host(dx), (size_t)n * sizeof(double));
   return CVB_OK;

@@ -53,10 +53,8 @@ struct TilePlan {
   // single GPU).  With an owner map the pair lists hold only the pairs whose TARGET column this rank owns.
   std::vector<int> h_owner;
   int my_rank = 0;
-  int *d_row_idx = nullptr, *d_pair_i = nullptr, *d_pair_j = nullptr, *d_pair_mask = nullptr, *d_rowc_idx = nullptr,
-      *d_tile_of = nullptr;
-  int *d_lvl_pair_i = nullptr, *d_lvl_pair_j = nullptr, *d_lvl_pair_k0 = nullptr, *d_lvl_pair_mask = nullptr,
-      *d_lvl_trsm_tile = nullptr, *d_lvl_trsm_col = nullptr, *d_col_ptr = nullptr, *d_rowc_ptr = nullptr;
+  cvb_dev_arr<int> d_row_idx, d_pair_i, d_pair_j, d_pair_mask, d_rowc_idx, d_tile_of;
+  cvb_dev_arr<int> d_lvl_pair_i, d_lvl_pair_j, d_lvl_pair_k0, d_lvl_pair_mask, d_lvl_trsm_tile, d_lvl_trsm_col, d_col_ptr, d_rowc_ptr;
   long n_tiles_L = 0;
   double flops = 0.0;   // flops of one numeric factorisation with this plan
   // col_group (optional, nt entries): h_col_group.  owner (optional, nt entries) + rank: distributed plan.  flops = the
@@ -64,8 +62,9 @@ struct TilePlan {
   void build(int nt, std::vector<uint8_t> lower_mask, std::vector<int> col_group = {}, const std::vector<int>* owner = nullptr,
              int rank = 0);
   size_t tile_index(int i, int j) const { return (size_t)h_tile_of[(size_t)i * nt + j]; }
-  int upload(cvb_ctx* ctx, cudaStream_t st);
-  void release();
+  int upload(cvb_ctx* ctx, cudaStream_t st);   // the d_ lists, allocated on st (an earlier upload's are freed)
+  // empties the plan, its device lists freed, before it goes out of scope (which frees them otherwise)
+  void release() { *this = TilePlan(); }
 };
 
 // Tile layout of the column groups (IMU chains' speed-bias blocks; pose-graph chain interiors), starting at tile 0.

@@ -49,13 +49,10 @@ int cvb_ctx_create(int device, cvb_ctx** out) {
   return CVB_OK;
 }
 
-void cvb_ba_free(cvb_ctx* ctx);  // ba_api.cu
-
 int cvb_ctx_destroy(cvb_ctx* ctx) {
   if (!ctx) return CVB_OK;
   cudaSetDevice(ctx->device);
   cudaStreamSynchronize(ctx->stream);
-  cvb_ba_free(ctx);
   if (ctx->h_pin) cudaFreeHost(ctx->h_pin);
   cudaStreamDestroy(ctx->stream);
   delete ctx;

@@ -23,7 +23,6 @@ struct cvb_ctx {
   void* h_pin = nullptr;
   size_t h_pin_cap = 0;
   bool pin_busy = false;
-  void* ba = nullptr;  // BA state (owned by ba_*.cu)
   // every extern "C" entry point holds this lock for its duration (cvb_device_guard): a ctx may be shared between host
   // threads — calls on one ctx are serialised, concurrency comes from one ctx per thread
   mutable std::recursive_mutex mtx;
@@ -100,6 +99,48 @@ struct cvb_block {
   unsigned char* d = nullptr;   // device block
   unsigned char* h = nullptr;   // pinned: [0, in_hi) the inputs, then [out_lo, out_hi) of the outputs
   size_t in_hi = 0, out_lo = 0, out_hi = 0;
+};
+
+// A device array that owns its memory: n elements (room for at least one) from the device's stream-ordered pool,
+// allocated on stream st and freed there when the array is destroyed or allocated again, early returns included.
+// for_ipc: from cudaMalloc instead, so that the array can be exported through CUDA IPC; freed by cudaFree.
+template <typename T>
+struct cvb_dev_arr {
+  T* p = nullptr;
+  size_t n = 0;
+  cvb_dev_arr() = default;
+  cvb_dev_arr(cvb_dev_arr&& o) noexcept { *this = static_cast<cvb_dev_arr&&>(o); }
+  cvb_dev_arr& operator=(cvb_dev_arr&& o) noexcept {
+    if (this != &o) {
+      reset();
+      p = o.p; n = o.n; st = o.st; ipc = o.ipc;
+      o.p = nullptr; o.n = 0;
+    }
+    return *this;
+  }
+  ~cvb_dev_arr() { reset(); }
+  cudaError_t alloc(size_t count, cudaStream_t s, bool for_ipc = false) {
+    reset();
+    st = s;
+    ipc = for_ipc;
+    const size_t bytes = (count ? count : 1) * sizeof(T);
+    const cudaError_t e = ipc ? cudaMalloc((void**)&p, bytes) : cudaMallocAsync((void**)&p, bytes, st);
+    if (e != cudaSuccess) p = nullptr;
+    else n = count;
+    return e;
+  }
+
+ private:
+  void reset() {
+    if (p) {
+      if (ipc) cudaFree(p);
+      else cudaFreeAsync(p, st);
+    }
+    p = nullptr;
+    n = 0;
+  }
+  cudaStream_t st = nullptr;
+  bool ipc = false;
 };
 
 // match_kernels.cu: the fused 2-NN + ratio filter of cvb_match_hamming_batch for n_pairs pairs of keyframes of one device

@@ -14,8 +14,6 @@
 #include "../../covins_b200/csrc/ctx.cu"
 #include "../../covins_b200/csrc/map_graph.cu"
 
-extern "C" void cvb_ba_free(cvb_ctx*) {}   // ba_engine.cu is not part of this harness
-
 template <class V>
 static std::vector<V> load(const std::string& path, bool* found = nullptr) {
   std::vector<V> v;
